@@ -10,12 +10,12 @@ A "step" is one pass of the hot path (ray march -> hash/SH encode -> tiny MLPs -
              table and its cell image are meant to stay L2-resident, as in production)
   e2e        the same metric through the public API with HOST (pinned) ray buffers: H2D of the rays and D2H of rgb+alpha
              inside the timed region
-  roofline   dominant kernel (ngp_field_tc_kernel: hash gather + tcgen05 MLPs) timed live with CUDA events recorded inside the
+  roofline   dominant kernel (ngp_field_tc_kernel: hash gather + wgmma MLPs) timed live with CUDA events recorded inside the
              step; algorithmic bytes = 512 B gathered per sample (16 levels x 8 corners x 2 x fp16, SURVEY §8d) + 28 B coords in
              + 16 B raw out per sample
   cpu_baseline / --impl reference   the reference's own ngp_raymarch kernels compiled for CPU (oracle/_ref) for march and
              compositing + the C restatement of tcnn (oracle port) for the field, all host cores, on a bounded ray sample.
-  reference_gpu / nerf.reference_torch_gpu_mlp   BASELINE.md B4 / B3: the reference's own CUDA kernels (built unmodified for sm_100a, oracle/build_ref_cuda.py) and its
+  reference_gpu / nerf.reference_torch_gpu_mlp   BASELINE.md B4 / B3: the reference's own CUDA kernels (built unmodified for sm_90a, oracle/build_ref_cuda.py) and its
              NerfMLP arithmetic on cuBLAS, timed per op on this GPU next to ours (rank 0, N = 1)
 Steps are issued on `--pipeline` CUDA streams (default 8 batches in flight, each with its own workspace; stated in config.batches_in_flight): throughput, not latency.
 Multi-GPU (torchrun): rays shard over ranks with no data-path collective (weak scaling: 65 536 rays per rank per step); the training arm's optimiser exchange runs over
@@ -41,7 +41,7 @@ sys.path.insert(0, ROOT)
 
 N_RAYS = 65536
 BUDGET = 64          # max samples per ray the workspace is sized for (reference: 1024; measured mean is ~11-30)
-N_BATCHES = 96       # distinct ray batches cycled through: 96 x 1.5 MiB of rays = 151 MB > 126 MB L2 (inputs larger than L2)
+N_BATCHES = 96       # distinct ray batches cycled through: 96 x 1.5 MiB of rays = 151 MB > 50 MB L2 (inputs larger than L2)
 METRIC = 'rays/sec (inference render, Instant-NGP lego-shaped 800x800, 65536 rays/batch)'
 WORKLOAD = 'instant-ngp lego-like synthetic (configs[1]): 65536 rays/batch from 40 spiral 800x800 views, occupancy-grid march + hash(16x2,T=2^19) + SH4 + MLP(64;1+2 hidden) + composite, forward'
 BYTES_PER_SAMPLE = 512 + 28 + 16
@@ -53,7 +53,15 @@ def peaks():
             p = json.load(fh)
         return float(p['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+        return 3350.0, 'H100 SXM data sheet (3.35 TB/s HBM3)'
+
+
+def tensor_peak():
+    try:
+        with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as fh:
+            return float(json.load(fh)['bf16_tflops_sustained']), 'measured (MEASURED_PEAKS.json bf16_tflops_sustained; kernel timed inside a multi-kernel step)'
+    except Exception:
+        return 989.0, 'H100 SXM data sheet (989 TFLOP/s dense fp16 / bf16)'
 
 
 class ClockSampler:
@@ -253,7 +261,7 @@ def _torch_field_fp32(pts01, dirs01, hash_params, dens_params, color_params, chu
 
 
 def reference_gpu_leg(dev, bf, rays, field, ours_chain_ms, ours_field_ms):
-    """BASELINE.md B4: the reference's own `raymarch_cuda` kernels, built unmodified for sm_100a (oracle/build_ref_cuda.py), timed on this GPU on the same 65 536-ray batch,
+    """BASELINE.md B4: the reference's own `raymarch_cuda` kernels, built unmodified for sm_90a (oracle/build_ref_cuda.py), timed on this GPU on the same 65 536-ray batch,
     occupancy grid and weights, with the calls and allocations of the reference's Python wrappers (rays_sampler.py:20-27 zero-fills coords for n_rays x 1024 samples on every
     call; every *_api ends in cudaDeviceSynchronize). Field: fp32 torch restatement (tcnn is not in the image). Per-op times next to ours through the identical signatures."""
     import torch
@@ -316,9 +324,9 @@ def reference_gpu_leg(dev, bf, rays, field, ours_chain_ms, ours_field_ms):
     comp_err = float((rgb - rgb_ref).abs().max())
     naive_ms = t_ref_march_stock + t_field_torch + t_ref_comp
     return {'value': n / (naive_ms * 1e-3), 'unit': 'rays/s', 'ms_per_batch': naive_ms,
-            'what': 'naive GPU path on this B200, one 65 536-ray batch, sequential: reference rays_sampler (stock wrapper: coords zero-filled for n_rays x 1024 samples = 1.88 GB per call) '
+            'what': 'naive GPU path on this GPU, one 65 536-ray batch, sequential: reference rays_sampler (stock wrapper: coords zero-filled for n_rays x 1024 samples = 1.88 GB per call) '
                     '+ fp32 torch restatement of the tcnn field (tcnn absent from the image) + reference calc_rgb_inference; reference kernels = extensions/ngp_raymarch built '
-                    'unmodified for sm_100a (oracle/build_ref_cuda.py)',
+                    'unmodified for sm_90a (oracle/build_ref_cuda.py)',
             'per_op_ms': {'rays_sampler': {'reference_stock_wrapper': t_ref_march_stock, 'reference_kernel_same_capacity_as_ours': t_ref_march, 'ours': t_our_march},
                           'field': {'torch_fp32_restatement': t_field_torch, 'ours': ours_field_ms},
                           'calc_rgb_inference': {'reference': t_ref_comp, 'ours': t_our_comp}},
@@ -351,6 +359,14 @@ def psnr_obj(a, b, what):
 
 
 # ------------------------------------------------------------------------------------------- our arm
+def dump_outputs(path, arrays):
+    """What each timed path (chain_*, fused_*) returned for its last timed batch, one float32 .npy per array (n_samples: per-ray sample counts). The inputs
+    are seeded, so two builds run with the same arguments can be compared array by array."""
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(path, f'{name}.npy'), t.float().cpu().numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -421,6 +437,7 @@ def run_ours(args):
     join()
     e1.record(main)
     barrier()
+    last_chain = {'rgb': out[0].clone(), 'alpha': out[1].clone(), 'n_samples': out[2][:, 0].clone()}   # the renderer reuses its output buffers
     field_ms = [a.elapsed_time(b) for a, b in evf]
     samples = [int(c[1].item()) for c in counters_log]
     total_ms = float(e0.elapsed_time(e1))
@@ -477,7 +494,7 @@ def run_ours(args):
     except Exception as e:
         l2_roof = {'error': repr(e)[:200]}
 
-    # ---- single-launch arm: the same K steps through xrb_ngp_render_fused (march + encode + tcgen05 MLPs + composite in ONE kernel per batch)
+    # ---- single-launch arm: the same K steps through xrb_ngp_render_fused (march + encode + wgmma MLPs + composite in ONE kernel per batch)
     evk = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(K)]
     fork()
     for i in range(WU):
@@ -505,6 +522,7 @@ def run_ours(args):
     join()
     f1.record(main)
     barrier()
+    last_fused = {'rgb': outf[0].clone(), 'alpha': outf[1].clone(), 'n_samples': outf[2].clone()}
     if os.environ.get('XRB_BENCH_DEBUG') and kev:
         gaps = [evk[i][1].elapsed_time(evk[i + 1][0]) for i in range(K - 1)] if P == 1 else []
         kms = [a.elapsed_time(b) for a, b in evk]
@@ -518,6 +536,9 @@ def run_ours(args):
     fused_kernel_ms = float(np.mean([a.elapsed_time(b) for a, b in evk])) if kev else fused_total_ms / K
     fused_samples = float(np.mean([float(x.sum().item()) for x in ns_log]))
     use_fused = args.path == 'fused' or (args.path == 'auto' and fused_total_ms < total_ms_max)
+    if args.dump_outputs and rank == 0:   # both timed paths, whichever of them the headline reports
+        dump_outputs(args.dump_outputs, {**{'chain_' + k: v for k, v in last_chain.items()}, **{'fused_' + k: v for k, v in last_fused.items()}})
+    del last_chain, last_fused
 
     # ---- end-to-end arm: host (pinned) rays in, rgb+alpha out, every step, through the public API; P batches in flight
     slots = [dict(rgb_h=torch.empty((N_RAYS, 3), dtype=torch.float32).pin_memory(), alpha_h=torch.empty((N_RAYS, 1), dtype=torch.float32).pin_memory(),
@@ -620,7 +641,7 @@ def run_ours(args):
             ns_np = ns_g.cpu().numpy()
             parity_gpu[path] = (rgb_g.cpu().numpy().copy(), (ns_np[:, 0] if ns_np.ndim == 2 else ns_np).copy())
 
-    # ---- training arm (BASELINE configs[4] shape: 65 536 rays per rank per step; march + compaction + field fwd/bwd (tcgen05) + composite fwd/bwd + loss + gradient exchange +
+    # ---- training arm (BASELINE configs[4] shape: 65 536 rays per rank per step; march + compaction + field fwd/bwd (wgmma) + composite fwd/bwd + loss + gradient exchange +
     # fused Adam; device-resident batches, synthetic targets). T = 2^20 compacted samples so that NO ray of the batch is truncated away (the reference's 2^18 is sized for its
     # adaptive ~24 K-ray batches); `trained_rays_per_step` is counted on the device (rays whose every marched sample took part).
     train = None
@@ -652,8 +673,8 @@ def run_ours(args):
                 dist.all_reduce(tsum, op=dist.ReduceOp.SUM)
             train = {'value': float(tsum.item()) / (float(tm.item()) * 1e-3), 'unit': 'rays/s (trained rays only)', 'ms_per_step': float(tm.item()) / K,
                      'rays_per_step': world * N_RAYS, 'trained_rays_per_step': float(tsum.item()) / K, 'target_batch_size': T_TRAIN,
-                     'compacted_samples_per_step_rank0': int(tr.compacted_samples().item()), 'grad_comm': tr.grad_comm, 'host_issue_ms_per_step': host_issue_ms, 'field_backward': 'tcgen05' if tr.bwd_impl == 1 else 'cuda cores',
-                     'what': 'march + compaction (aux stream, one step ahead) | field fwd (tcgen05) + composite fwd + Huber x5 + composite bwd + field bwd (tcgen05 dX/dW) + gradient exchange '
+                     'compacted_samples_per_step_rank0': int(tr.compacted_samples().item()), 'grad_comm': tr.grad_comm, 'host_issue_ms_per_step': host_issue_ms, 'field_backward': 'wgmma' if tr.bwd_impl == 1 else 'cuda cores',
+                     'what': 'march + compaction (aux stream, one step ahead) | field fwd (wgmma) + composite fwd + Huber x5 + composite bwd + field bwd (wgmma dX/dW) + gradient exchange '
                              '+ Adam (world>1, grad_comm=peer: ONE optimiser kernel over NVLink peer memory - every rank sums all ranks\' bf16 gradients for its 1/N of the table, runs Adam on it and '
                              'stores the new fp16 values into every rank\'s working table, csrc/peer_adam.cu; grad_comm=sharded: NCCL bf16 reduce-scatter -> sharded Adam -> fp16 all-gather) + cell-image refresh'}
             if tr.px is not None:
@@ -701,7 +722,7 @@ def run_ours(args):
                 stream_bytes = (64 + 192 + 66) * 2 ** 20 + n_q * (2 * 16 + 4 + 4)
                 modes[name] = {'ms_per_update': ms, 'ms_per_training_step_amortised': ms / 16, 'candidate_cells': n_q, 'hbm_stream_bytes': stream_bytes,
                                'stream_gbs': stream_bytes / (ms * 1e-3) / 1e9}
-            grid_upd = dict(modes, what='NGPGridSampler.update_density_grid_func: generate_grid_samples x2, density-only field (tcgen05), splat (atomicMax), EMA, bitfield + cascade pooling + mean')
+            grid_upd = dict(modes, what='NGPGridSampler.update_density_grid_func: generate_grid_samples x2, density-only field (wgmma), splat (atomicMax), EMA, bitfield + cascade pooling + mean')
         except Exception as e:   # an auxiliary arm must never take the headline line down
             grid_upd = {'error': repr(e)[:300]}
 
@@ -734,7 +755,7 @@ def run_ours(args):
         except Exception as e:
             all_ones = {'error': repr(e)[:300]}
 
-    # ---- NeRF arm (BASELINE configs[2]: hierarchical 64 + 128, 800x800-shaped rays): fused tcgen05 NerfMLP path, device-resident rays
+    # ---- NeRF arm (BASELINE configs[2]: hierarchical 64 + 128, 800x800-shaped rays): fused wgmma NerfMLP path, device-resident rays
     nerf = None
     if not args.no_nerf:
         try:
@@ -761,11 +782,7 @@ def run_ours(args):
                 dist.all_reduce(nm, op=dist.ReduceOp.MAX)
             rps = world * n_nerf * KN / (float(nm.item()) * 1e-3)
             flop_per_ray = (64 + 192) * 593408 * 2
-            try:
-                with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as fh:
-                    tpeak = float(json.load(fh)['bf16_tflops_sustained'])
-            except Exception:
-                tpeak = 1400.0
+            tpeak, tsrc = tensor_peak()
             # CPU baseline leg of this arm (rank 0, N=1): BASELINE configs[0] shape - 1024 rays x 64 samples, coarse network only - through the numpy oracle
             # (embed -> 12-layer NerfMLP -> composite; multi-threaded BLAS on the box's host cores). Checker code, timed only.
             nerf_cpu = None
@@ -774,7 +791,7 @@ def run_ours(args):
                 try:
                     from oracle import nerf_oracle as NO
                     sd = {k: v.detach().cpu().numpy() for k, v in net.state_dict().items()}
-                    # parity of THIS arm on its own rays: 512 of the timed rays through the numpy restatement of the reference's hierarchical forward (fp32) vs the fused tcgen05 path (fp16 operands)
+                    # parity of THIS arm on its own rays: 512 of the timed rays through the numpy restatement of the reference's hierarchical forward (fp32) vs the fused wgmma path (fp16 operands)
                     po, pd, pv = (t[:512].contiguous() for t in nerf_rays[0])
                     got = nr.render(po, pd, pv)
                     o_p, d_p, v_p = po.cpu().numpy(), pd.cpu().numpy(), pv.cpu().numpy()
@@ -799,7 +816,7 @@ def run_ours(args):
                 except Exception as e:
                     nerf_cpu = {'error': repr(e)[:200]}
             # BASELINE.md B3 for the dominant op: the reference's NerfMLP.batchify_run_mlp arithmetic (nerf_mlp.py:70-94: 11 nn.Linear GEMMs + 2 cat per 32 768-row chunk, cuBLAS)
-            # on this GPU, fp32 with TF32 off and on, against the single tcgen05 kernel on the same 2 097 152 embedded rows and weights
+            # on this GPU, fp32 with TF32 off and on, against the single wgmma kernel on the same 2 097 152 embedded rows and weights
             torch_mlp = None
             if world == 1:
                 try:
@@ -827,22 +844,22 @@ def run_ours(args):
                         finally:
                             net.mlp.fused = True
                             torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old_flags
-                    torch_mlp = {'rows': rows, 'ms': {'torch_nn_linear_fp32': res_t['fp32'], 'torch_nn_linear_tf32': res_t['tf32'], 'ours_tcgen05_fp16': t_tc},
+                    torch_mlp = {'rows': rows, 'ms': {'torch_nn_linear_fp32': res_t['fp32'], 'torch_nn_linear_tf32': res_t['tf32'], 'ours_wgmma_fp16': t_tc},
                                  'speedup_vs_fp32': res_t['fp32'] / t_tc, 'speedup_vs_tf32': res_t['tf32'] / t_tc, 'max_abs_diff_vs_fp32': err_t,
                                  'what': 'NerfMLP.batchify_run_mlp on 2 097 152 embedded rows (= 32 768 rays x 64 samples): the reference module\'s own arithmetic (nn.Linear chain, cat at the skip, '
-                                         '32 768-row chunks, cuBLAS) vs the single tcgen05 kernel; same weights, CUDA events'}
+                                         '32 768-row chunks, cuBLAS) vs the single wgmma kernel; same weights, CUDA events'}
                     del xe
                 except Exception as e:   # noqa: BLE001
                     torch_mlp = {'error': repr(e)[:200]}
             nerf = {'value': rps, 'unit': 'rays/s', 'cpu_baseline': nerf_cpu, 'parity': nerf_parity, 'reference_torch_gpu_mlp': torch_mlp, 'rays': 'NeRF convention (GetRays on random pixels of Blender spiral poses, radius 4), near 2 / far 6', 'workload': 'vanilla NeRF hierarchical 64 coarse + 192 fine evaluations per ray (configs[2]), 32768-ray batches, inference',
                     'ms_per_batch': float(nm.item()) / KN, 'roofline': {'bound': 'tensor', 'achieved': rps * flop_per_ray / 1e12 / world, 'peak': tpeak, 'unit': 'TFLOP/s',
                                                                          'frac': rps * flop_per_ray / 1e12 / world / tpeak, 'flop_per_ray': flop_per_ray,
-                                                                         'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a multi-kernel step)'}}
+                                                                         'peak_source': tsrc}}
         except Exception as e:   # an auxiliary arm must never take the headline line down
             nerf = {'error': repr(e)[:300]}
 
     # ---- NeRF training step (configs[2], N_rand 4096 as configs/nerf/nerf_blender_base01.py): encoders / composite fwd+bwd / sample_pdf kernels + the 12 dense layers of both
-    # networks forward AND backward as UMMA kernels over fp16 tile images (csrc/nerf_train.cu), torch.optim.Adam on the fp32 nn.Linear parameters
+    # networks forward AND backward as wgmma kernels over fp16 tile images (csrc/nerf_train.cu), torch.optim.Adam on the fp32 nn.Linear parameters
     nerf_train = None
     if not args.no_nerf:
         try:
@@ -878,7 +895,7 @@ def run_ours(args):
                           'rows_per_step_per_gpu': n_t * (64 + 192), 'flop_per_step': 3 * n_t * (64 + 192) * 593408 * 2,
                           'tflops': 3 * n_t * (64 + 192) * 593408 * 2 / (float(qm.item()) / KT * 1e-3) / 1e12,
                           'what': 'NerfNetwork.train_step + Adam (per-rank, no gradient all-reduce in this arm): encoders / composite fwd+bwd / sample_pdf kernels; the dense layers of both '
-                                  'networks forward + backward on tcgen05 (tile-image GEMM kernels: forward, input gradient with fused ReLU mask, weight gradient accumulated in TMEM)'}
+                                  'networks forward + backward on wgmma (tile-image GEMM kernels: forward, input gradient with fused ReLU mask, weight gradient accumulated in registers)'}
             del tnet, topt, tdata
         except Exception as e:   # an auxiliary arm must never take the headline line down
             nerf_train = {'error': repr(e)[:300]}
@@ -919,13 +936,13 @@ def run_ours(args):
                 dist.all_reduce(wm, op=dist.ReduceOp.MAX)
             mip_train = {'value': world * n_mt * KMT / (float(wm.item()) * 1e-3), 'unit': 'rays/s', 'ms_per_step': float(wm.item()) / KMT, 'rays_per_step_per_gpu': n_mt,
                          'rows_per_step_per_gpu': n_mt * 256, 'tflops': 3 * n_mt * 256 * 610304 * 2 / (float(wm.item()) / KMT * 1e-3) / 1e12,
-                         'what': 'MipNerfNetwork.train_step + Adam: cast_rays + IPE + composite fwd/bwd + resample kernels; the MLP (both levels) forward + backward on tcgen05 tile-image GEMMs'}
+                         'what': 'MipNerfNetwork.train_step + Adam: cast_rays + IPE + composite fwd/bwd + resample kernels; the MLP (both levels) forward + backward on wgmma tile-image GEMMs'}
             del mtnet, mtopt, mdata
         except Exception as e:
             import traceback
             mip_train = {'error': repr(e)[:300], 'trace': traceback.format_exc()[-500:]}
 
-    # ---- Mip-NeRF arm (BASELINE configs[3]: 2 levels x 128 cone samples, IPE): the same tcgen05 NerfMLP on IPE tile images, device-resident rays
+    # ---- Mip-NeRF arm (BASELINE configs[3]: 2 levels x 128 cone samples, IPE): the same wgmma NerfMLP on IPE tile images, device-resident rays
     mip = None
     if not args.no_mip:
         try:
@@ -954,11 +971,7 @@ def run_ours(args):
                 dist.all_reduce(mm, op=dist.ReduceOp.MAX)
             mrps = world * n_mip * KM / (float(mm.item()) * 1e-3)
             mflop = 256 * 610304 * 2
-            try:
-                with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as fh:
-                    tpeak = float(json.load(fh)['bf16_tflops_sustained'])
-            except Exception:
-                tpeak = 1400.0
+            tpeak, tsrc = tensor_peak()
             mip_parity = None
             if world == 1:
                 try:
@@ -983,7 +996,7 @@ def run_ours(args):
             mip = {'value': mrps, 'unit': 'rays/s', 'parity': mip_parity, 'rays': 'NeRF convention with GetRays radii, near 2 / far 6', 'workload': 'Mip-NeRF 2 levels x 128 conical-frustum samples per ray, IPE 96 + 27 (configs[3]), 32768-ray batches, inference',
                    'ms_per_batch': float(mm.item()) / KM, 'roofline': {'bound': 'tensor', 'achieved': mrps * mflop / 1e12 / world, 'peak': tpeak, 'unit': 'TFLOP/s',
                                                                        'frac': mrps * mflop / 1e12 / world / tpeak, 'flop_per_ray': mflop,
-                                                                       'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a multi-kernel step)'}}
+                                                                       'peak_source': tsrc}}
         except Exception as e:   # an auxiliary arm must never take the headline line down
             mip = {'error': repr(e)[:300]}
 
@@ -1005,15 +1018,9 @@ def run_ours(args):
                 err = np.abs(rgb_g - rgb_cpu)
                 mse = float((err.astype(np.float64) ** 2).mean())
                 parity[path] = {'max_abs_rgb_err': float(err.max()), 'psnr_vs_ref_db': float(-10.0 * np.log10(max(mse, 1e-20))), 'sample_counts_bit_exact': bool(np.array_equal(ns_g, ns_cpu))}
-        # L2 -> SM sector traffic of ONE field launch at this workload, from the committed ncu --set full capture (profiles/r02_ngp_field_tc_ncu_final.md: lts__t_sectors_srcunit_tex_op_read.sum
-        # = 30.29 M sectors for 699 K samples = 43.3 sectors per sample): scaled to this run's sample count. DRAM traffic of the same capture: 47.15 MB read + 4.88 MB written.
-        SECTORS_PER_SAMPLE = 28552658 / 699287
-        l2_bytes = iso_samples * SECTORS_PER_SAMPLE * 32
-        l2_obj = None
-        if l2_roof and 'error' not in l2_roof:
-            l2_obj = {'bound': 'l2 sector rate (random 4-byte gather)', 'achieved': l2_bytes / (iso_field_ms * 1e-3) / 1e9, 'peak': l2_roof['sector_GBs_at_4B'], 'unit': 'GB/s of 32-byte sectors',
-                      'frac': l2_bytes / (iso_field_ms * 1e-3) / 1e9 / l2_roof['sector_GBs_at_4B'], 'sectors_per_sample': SECTORS_PER_SAMPLE,
-                      'sectors_source': 'quoted: ncu capture profiles/r02_ngp_field_tc_ncu_final.md (lts__t_sectors_srcunit_tex_op_read.sum / samples), scaled to this run', 'peak_measured_live': l2_roof}
+        # the roof the gather runs under, measured live (xrb_micro_gather): the field kernel's own sector count is not measured by this run
+        l2_obj = {'bound': 'l2 sector rate (random 4-byte gather)', 'peak': l2_roof['sector_GBs_at_4B'], 'unit': 'GB/s of 32-byte sectors', 'peak_measured_live': l2_roof} \
+            if l2_roof and 'error' not in l2_roof else l2_roof
         chain = {'value': world * N_RAYS * K / (total_ms_max * 1e-3), 'unit': 'rays/s', 'ms_per_step': total_ms_max / K, 'gpu_launches_per_step': 6,
                  'what': '6 launches per batch on one stream (memset, march count / scan / emit, field, composite), P batches in flight on P streams',
                  'roofline': {'kernel': 'xrb::ngp_field_tc_kernel<false>', 'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
@@ -1023,7 +1030,7 @@ def run_ours(args):
         f_bytes = fused_samples * 512 + N_RAYS * 44   # no coords[S,7] / raw[S,4] round trip: gather bytes + 44 B of ray I/O
         f_ach = f_bytes / (fused_kernel_ms * 1e-3) / 1e9
         fused = {'value': world * N_RAYS * K / (fused_total_ms * 1e-3), 'unit': 'rays/s', 'ms_per_step': fused_total_ms / K, 'gpu_launches_per_step': 1,
-                 'what': 'ONE launch per batch (xrb_ngp_render_fused: warp-specialised march + hash encode + tcgen05 MLPs + segmented-scan composite), P batches in flight on P streams',
+                 'what': 'ONE launch per batch (xrb_ngp_render_fused: warp-specialised march + hash encode + wgmma MLPs + segmented-scan composite), P batches in flight on P streams',
                  'roofline': {'kernel': 'xrb::ngp_render_fused_kernel', 'bound': 'hbm', 'achieved': f_ach, 'peak': peak, 'unit': 'GB/s', 'frac': f_ach / peak,
                               'kernel_ms': fused_kernel_ms, 'kernel_share_of_step': 1.0, 'kernel_ms_note': 'events around the launch while P-1 other launches share the SMs',
                               'algorithmic_bytes_per_launch': f_bytes}}
@@ -1038,7 +1045,7 @@ def run_ours(args):
             'metric': METRIC, 'value': head['value'], 'unit': 'rays/s', 'n_gpus': world, 'steps': K, 'warmup': W,
             'ms_per_step': head['ms_per_step'], 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f16', 'data': 'synthetic',
             'config': {'workload': WORKLOAD, 'rays_per_step_per_gpu': N_RAYS, 'samples_per_ray_mean': s_mean / N_RAYS, 'parallelism': f'ray-sharded x{world}, no data-path collective',
-                       'l2': f'inputs larger than L2: {N_BATCHES} distinct ray batches = {N_BATCHES * N_RAYS * 24 / 1e6:.0f} MB cycled (L2 126 MB), nothing flushed; the 24.4 MB fp16 hash table and its '
+                       'l2': f'inputs larger than L2: {N_BATCHES} distinct ray batches = {N_BATCHES * N_RAYS * 24 / 1e6:.0f} MB cycled (L2 50 MB), nothing flushed; the 24.4 MB fp16 hash table and its '
                              f'{field._cells.numel() / 1e6 if field._cells is not None else 0:.0f} MB cell image (levels 0..{field.n_packed - 1}) stay L2-resident as in production',
                        'timing': 'one CUDA-event pair around the K steps on the launching stream, max over ranks', 'batches_in_flight': P, 'untimed_warmup_steps_run': WU,
                        'path': 'fused single launch' if use_fused else 'chain of 6 launches', 'path_selection': args.path, 'cell_image_levels': field.n_packed},
@@ -1046,10 +1053,7 @@ def run_ours(args):
             'e2e': {'value': world * N_RAYS * K / (e2e_ms * 1e-3), 'unit': 'rays/s', 'h2d_bytes_per_step': N_RAYS * 24, 'd2h_bytes_per_step': N_RAYS * 16,
                     'ms_per_step': e2e_ms / K, 'host_wall_ms_per_step': e2e_wall_ms / K},
             'gpu_launches': head['gpu_launches_per_step'] * K,
-            # traffic: dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel at this workload, QUOTED from the committed ncu --set full capture of this
-            # round (profiles/r02_ngp_field_tc_ncu_final.md: 47.13 MB + 3.21 MB; fused kernel: profiles/r01b_ngp_render_fused_ncu.md 27.80 MB + 0.04 MB), not measured by this run
-            'roofline': dict(head['roofline'], traffic=(27.80e6 + 0.04e6) if use_fused else (47.13e6 + 3.21e6), traffic_source='quoted from the ncu --set full capture committed under profiles/ (bytes per launch); not measured by this run',
-                             peak_source=peak_src,
+            'roofline': dict(head['roofline'], peak_source=peak_src,
                              note='hash table (24.4 MB fp16) + cell image are L2-resident by design: DRAM traffic is far below the algorithmic bytes; the gather runs under the L2 sector rate '
                                   '(l2_gather_roofline: every 4-byte entry costs a 32-byte sector), not under the HBM copy peak this frac is quoted against'),
             'paths': {'chain': chain, 'fused': fused},
@@ -1081,10 +1085,12 @@ def main():
     ap.add_argument('--no-image', dest='no_image', action='store_true', help='skip the whole-image inference arm')
     ap.add_argument('--no-grid', dest='no_grid', action='store_true', help='skip the occupancy-grid update arm')
     ap.add_argument('--no-mip', dest='no_mip', action='store_true', help='skip the Mip-NeRF arm')
-    ap.add_argument('--no-ref-gpu', dest='no_ref_gpu', action='store_true', help='skip the GPU reference leg (reference raymarch_cuda kernels built for sm_100a, BASELINE.md B4)')
+    ap.add_argument('--no-ref-gpu', dest='no_ref_gpu', action='store_true', help='skip the GPU reference leg (reference raymarch_cuda kernels built for sm_90a, BASELINE.md B4)')
     ap.add_argument('--path', default='auto', choices=['auto', 'chain', 'fused'], help='inference path of the headline/e2e numbers: 5-launch chain, single-launch fused kernel, or the faster of the two (both are always measured)')
     ap.add_argument('--grad-comm', dest='grad_comm', default='auto', choices=['auto', 'peer', 'sharded', 'allreduce'], help='gradient exchange of the training arm at world > 1 (peer: one optimiser kernel over NVLink peer memory, csrc/peer_adam.cu; auto: peer where CUDA IPC works, else sharded NCCL)')
-    ap.add_argument('--pipeline', type=int, default=8, help='ray batches in flight (CUDA streams); 1 = strictly sequential steps. Measured on one B200: 2 -> 240, 4 -> 271, 6 -> 287, 8 -> 292 M rays/s')
+    ap.add_argument('--pipeline', type=int, default=8, help='ray batches in flight (CUDA streams); 1 = strictly sequential steps')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write rgb / alpha / n_samples of the last timed batch of the chain and the fused path as DIR/{chain,fused}_<name>.npy (float32)')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     if args.impl == 'reference':

@@ -1,5 +1,5 @@
 /*
- * xrnerf_b200 — C ABI of the B200-native volumetric-rendering hot path.
+ * xrnerf_b200 — C ABI of the H100-native (sm_90a) volumetric-rendering hot path.
  *
  * Drop-in boundary for the two native interfaces the reference's hot path binds:
  *   #1 `raymarch_cuda`  (pybind module; /root/reference/extensions/ngp_raymarch/include/pybind_api.h:3-95,
@@ -167,8 +167,8 @@ int xrb_tcnn_hashgrid_layout(const xrb_ngp_config *cfg, uint32_t *offsets_host /
 
 /* fp32 master -> fp16 working copy (what tcnn does on every forward; done once per optimiser step here) */
 int xrb_tcnn_cast_params(const float *src, void *dst_fp16, int64_t n, void *stream);
-/* packs the density+colour weights (fp32 master, tcnn layout W[out][in]) into the UMMA shared-memory image
- * (128-byte-swizzled K-major tiles) the tcgen05 kernels bulk-copy; image size = xrb_ngp_weight_image_bytes(). */
+/* packs the density+colour weights (fp32 master, tcnn layout W[out][in]) into the wgmma shared-memory image
+ * (128-byte-swizzled K-major tiles) the tensor-core kernels bulk-copy; image size = xrb_ngp_weight_image_bytes(). */
 size_t xrb_ngp_weight_image_bytes(const xrb_ngp_config *cfg);
 int xrb_ngp_pack_weights(const xrb_ngp_config *cfg, const float *density_params, const float *color_params, void *image, void *stream);
 
@@ -189,8 +189,7 @@ int xrb_tcnn_mlp_backward(const void *params_fp16, const void *x_fp16, const voi
 
 /* HashNerfMLP.run_mlp (hashnerf_mlp.py:55-79) fused: pts/dirs f32 rows (stride in floats, so `coords[:, :3]` /
  * `coords[:, 4:]` views of a [S,7] buffer work in place) -> raw f32[n,4] = (rgb3, density1).
- * impl: 0 = SIMT (CUDA cores), 1 (or 2) = tcgen05 tensor-core tiles (weights from `weight_image`); the kernel keeps a quarter of the register file free so that a
- * kernel of another stream - the march of the next batch - can run beside it.
+ * impl: 0 = SIMT (CUDA cores), 1 (or 2) = wgmma tensor-core tiles (weights from `weight_image`).
  * n_rows_dev (optional, device pointer): the effective row count is min(n, *n_rows_dev) — a sample count produced on the device by the
  * march / compaction never has to visit the host. */
 int xrb_ngp_mlp_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const void *color_fp16,
@@ -206,8 +205,8 @@ int xrb_ngp_mlp_backward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
                          const float *pts, int pts_stride, const float *dirs, int dirs_stride, const float *dl_draw, int n,
                          float *d_table, float *d_density, float *d_color, void *stream);
 
-/* The same backward on tcgen05 tensor-core tiles (csrc/ngp_backward_tc.cu): dX = dZ.W and dW += dZ^T.X per layer as UMMA instructions, the weight
- * gradients accumulated in TMEM over the whole launch; fp16 operands (dZ staged with a fixed 2^12 scale), fp32 accumulation. Built for
+/* The same backward on wgmma tensor-core tiles (csrc/ngp_backward_tc.cu): dX = dZ.W and dW += dZ^T.X per layer as tensor-core instructions, the weight
+ * gradients accumulated in registers over the whole launch; fp16 operands (dZ staged with a fixed 2^12 scale), fp32 accumulation. Built for
  * (density_hidden, color_hidden) = (1,1) and (1,2) — the reference config, configs/instant_ngp/nerf_blender_local01.py:113,123 — and returns
  * XRB_E_UNSUPPORTED otherwise. n_rows_dev (optional, device): the effective row count is min(n, *n_rows_dev) (the compacted sample count
  * stays on the device). Same accumulate-into-outputs contract as xrb_ngp_mlp_backward. */
@@ -254,7 +253,7 @@ int xrb_ngp_render(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const 
                    int dens_act, float *rgb_out, float *alpha_out, int32_t *numsteps, int32_t *counters, void *workspace,
                    void *ev_before_field, void *ev_after_field, void *stream);
 
-/* Single-launch variant: march + hash encode + MLPs (tcgen05) + composite in ONE persistent warp-specialised kernel; no per-sample
+/* Single-launch variant: march + hash encode + MLPs (wgmma) + composite in ONE persistent warp-specialised kernel; no per-sample
  * buffer exists, so there is no max_samples / overflow case. Same arithmetic as xrb_ngp_render (sample positions bit-identical; the
  * composite is a segmented warp scan: fp32 re-association only). `workspace`: xrb_ngp_render_fused_workspace() bytes, 256-byte
  * aligned, ZEROED ONCE by the caller at allocation (the kernel leaves its scheduler words zero on exit); one workspace per stream.
@@ -293,17 +292,17 @@ int xrb_nerf_sample_pdf(const float *z_vals, const float *weights, const float *
 int xrb_nerf_posenc(const float *pts, const float *viewdirs, int64_t n_pts, int samples_per_ray, int multires, int multires_dirs,
                     float *embedded, void *stream);
 
-/* NerfMLP.run_mlp (xrnerf/models/mlps/nerf_mlp.py:70-94; netdepth 8, netwidth 256, skips [4], use_viewdirs) as one persistent tcgen05
+/* NerfMLP.run_mlp (xrnerf/models/mlps/nerf_mlp.py:70-94; netdepth 8, netwidth 256, skips [4], use_viewdirs) as one persistent wgmma
  * kernel, inference forward. embedded f32[n, input_ch + input_ch_dirs] ((63,27) NeRF or (96,27) Mip-NeRF) -> raw f32[n,4] = (rgb3, alpha1).
  * weight_image / bias: produced by xrnerf_b200.nerf_mlp.pack_nerf_mlp (fp16 slabs, K-major, 128-byte swizzle, in streaming order). */
 int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* v2 of the same kernel: two epilogue warpgroups per tile, phased MMA issue, double-buffered TMEM accumulators, half-slab weight stream
- * (image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v2) */
+/* the same chain on an fp16 encoding tile image, weights as half slabs (image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v2); the bias is added in fp16 after
+ * rounding the accumulator and alpha is a dot product in the epilogue of pts_linears.7 */
 int xrb_nerf_mlp_forward_v2(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* v3 of the same chain — NerfMLP.run_mlp, /root/reference/xrnerf/models/mlps/nerf_mlp.py:70-94 — (csrc/nerf_mlp_tc3.cu): two 128-row tiles in flight per SM so the tensor core runs one tile's layer while the other tile's
- * accumulators are drained. weight_image / bias from the matching host packer (xrnerf_b200.nerf_mlp.pack_nerf_mlp_v3: bias = fp32 vector + fp16 copy). */
+/* v3: the same arithmetic as v2 with the 256-wide layers' weights as [256 x 32] K-half slabs (64-byte swizzle). weight_image / bias from the matching host packer
+ * (xrnerf_b200.nerf_mlp.pack_nerf_mlp_v3: bias = fp32 vector + fp16 copy). */
 int xrb_nerf_mlp_forward_v3(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* encoding tile image consumed by v2 (per 128-row tile: point-encoding block(s) then direction block, [128x64] fp16, UMMA K-major 128B swizzle):
+/* encoding tile image consumed by v2 / v3 (per 128-row tile: point-encoding block(s) then direction block, [128x64] fp16, K-major 128B swizzle):
  * size, conversion from an fp32 `embedded` matrix, and BaseEmbedder's positional encoding written directly in that form */
 size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch);
 int xrb_nerf_pack_embedded(const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, void *enc_image, void *stream);
@@ -346,7 +345,7 @@ int xrb_nerf_zvals(int64_t n_rays, int n_samples, float near_, float far_, int l
 
 /* ------------------------------------------------------------------------------------------------
  * NerfMLP training on tensor cores (csrc/nerf_train.cu): what torch.autograd + cuBLAS do for the reference's NerfMLP (xrnerf/models/mlps/nerf_mlp.py:70-94,
- * trained by networks/nerf.py:71-92 / networks/mipnerf.py:45-74) as UMMA kernels over TILE IMAGES (per 128-row tile, C/64 blocks of [128 x 64] fp16 in the
+ * trained by networks/nerf.py:71-92 / networks/mipnerf.py:45-74) as wgmma kernels over TILE IMAGES (per 128-row tile, C/64 blocks of [128 x 64] fp16 in the
  * K-major 128-byte-swizzle layout: the encoders' output format, xrb_nerf_enc_image_bytes). The host (xrnerf_b200/nerf_train.py) strings the layers together.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {

@@ -1,7 +1,7 @@
-"""TEST / BENCH INFRASTRUCTURE ONLY — builds the REFERENCE's own `raymarch_cuda` extension (extensions/ngp_raymarch, setup.py:4-34) for sm_100a, unmodified, from
-where its sources lie under /root/reference, into oracle/_ref/cuda/ (git-ignored, travels to the GPU box). Same sources, include dirs and nvcc flags as the reference's
-setup.py; only the arch is added (the reference ships no sm_100 path). Used by bench.py's `reference_gpu` leg (BASELINE.md B4: the reference's kernels timed on the same
-B200 next to ours) and by tests/test_gpu_vs_ref_cuda.py. Nothing in xrnerf_b200/ imports it.
+"""TEST / BENCH INFRASTRUCTURE ONLY — builds the REFERENCE's own `raymarch_cuda` extension (extensions/ngp_raymarch, setup.py:4-34) for sm_90a, unmodified, from
+the reference checkout named by XRB_REF_EXT, into oracle/_ref/cuda/ (git-ignored). Same sources, include dirs and nvcc flags as the reference's setup.py; only
+the arch is added. Used by bench.py's `reference_gpu` leg (BASELINE.md B4: the reference's kernels timed on the same GPU next to ours) and by
+tests/test_gpu_vs_ref_cuda.py. Nothing in xrnerf_b200/ imports it.
 
 python oracle/build_ref_cuda.py            # ~5 min on 8 cores, once; a no-op when the module is already there or the reference is absent"""
 import os
@@ -26,20 +26,20 @@ def build(verbose=False):
     if not os.path.isdir(os.path.join(REF, 'src')):
         return None
     os.makedirs(OUT, exist_ok=True)
-    os.environ['TORCH_CUDA_ARCH_LIST'] = '10.0a'
+    os.environ['TORCH_CUDA_ARCH_LIST'] = '9.0a'
     os.environ.setdefault('MAX_JOBS', str(os.cpu_count() or 4))
     from torch.utils.cpp_extension import load
     load(name=NAME, sources=[os.path.join(REF, 'src', s + '.cu') for s in SRCS],
          extra_include_paths=[os.path.join(REF, 'include'), os.path.join(REF, 'include', 'op_include', 'eigen'), os.path.join(REF, 'include', 'op_include', 'pcg32')],
          extra_cuda_cflags=['--extended-lambda', '--expt-relaxed-constexpr'], build_directory=OUT, verbose=verbose, is_python_module=False)
-    for f in os.listdir(OUT):   # keep the module only (objects and ninja files would travel with every gpurun snapshot)
+    for f in os.listdir(OUT):   # keep the module only
         if not f.endswith('.so'):
             os.remove(os.path.join(OUT, f))
     return module_path()
 
 
 def load_module():
-    """import the prebuilt module (GPU box: no compiler run, no /root/reference needed)"""
+    """import the prebuilt module (no compiler run, no reference checkout needed)"""
     p = module_path()
     if p is None:
         return None

@@ -1,4 +1,4 @@
-"""Developer probe: tensor-pipe throughput of the fused tcgen05 NerfMLP kernel vs the fp32 library-GEMM path (config-3 shape)."""
+"""Developer probe: tensor-pipe throughput of the fused wgmma NerfMLP kernel vs the fp32 library-GEMM path (config-3 shape)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -28,7 +28,7 @@ from xrnerf_b200.nerf_mlp import pack_nerf_mlp, pack_nerf_mlp_v2
 for v, packer in (((2, pack_nerf_mlp_v2),) if os.environ.get('XRB_NM_DBG') else ((1, pack_nerf_mlp), (2, pack_nerf_mlp_v2))):
     image, bias = packer(mlp)
     t = timeit(lambda: nerf_mlp_forward(image, bias, emb, 63, 27, version=v))
-    print(f'fused tcgen05 NerfMLP v{v}: {t:.3f} ms for {rows} rows -> {flop / t / 1e9:.1f} TFLOP/s ({rows / t / 1e3:.1f} Mrows/s)', flush=True)
+    print(f'fused wgmma NerfMLP v{v}: {t:.3f} ms for {rows} rows -> {flop / t / 1e9:.1f} TFLOP/s ({rows / t / 1e3:.1f} Mrows/s)', flush=True)
     if v == 2:
         from xrnerf_b200 import _C
         from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles

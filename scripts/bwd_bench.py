@@ -1,4 +1,4 @@
-"""Isolated timing of the NGP field backward (tcgen05) on the samples of one 65 536-ray batch.  python scripts/bwd_bench.py"""
+"""Isolated timing of the NGP field backward (wgmma) on the samples of one 65 536-ray batch.  python scripts/bwd_bench.py"""
 import os
 import sys
 import numpy as np

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,15 +30,6 @@ def pytest_collection_modifyitems(config, items):
 def port():
     from oracle.oracle import Port
     return Port()
-
-
-@pytest.fixture(scope='session')
-def ref():
-    from oracle.oracle import Ref, have_ref, build
-    build()
-    if not have_ref():
-        pytest.skip('oracle/_ref not built (needs /root/reference at build time)')
-    return Ref(serial=True)
 
 
 @pytest.fixture(scope='session')

@@ -115,9 +115,12 @@ def main():
     mse = met.img2mse(lx, ly)
     out.update({'loss.x': lx, 'loss.y': ly, 'loss.huber_sum': met.HuberLoss(lx, ly, 0.1, 'sum'), 'loss.huber_mean': met.HuberLoss(lx, ly, 0.1, 'mean'),
                 'loss.huber5_grad': lxg.grad, 'loss.mse': mse, 'loss.psnr': met.mse2psnr(mse)})
-    np.savez_compressed(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'nerf_golden.npz'),
-                        **{k: (v.detach().numpy() if torch.is_tensor(v) else np.asarray(v)) for k, v in out.items()})
-    print('wrote nerf_golden.npz with', len(out), 'arrays')
+    out = {k: (v.detach().numpy() if torch.is_tensor(v) else np.asarray(v)) for k, v in out.items()}
+    big = ('embedded', 'mip.embedded')   # in a file of their own: every stored file stays under 1 MB
+    here = os.path.dirname(os.path.abspath(__file__))
+    np.savez_compressed(os.path.join(here, 'nerf_golden.npz'), **{k: v for k, v in out.items() if k not in big})
+    np.savez_compressed(os.path.join(here, 'nerf_golden_embedded.npz'), **{k: out[k] for k in big})
+    print('wrote nerf_golden.npz and nerf_golden_embedded.npz with', len(out), 'arrays')
 
 
 if __name__ == '__main__':

@@ -1,5 +1,5 @@
 """The CPU reference arm of the bench contract (`bench.py --impl reference`) runs without a GPU and prints ONE JSON line with the keys the driver reads;
-under a multi-rank launch only rank 0 works. (The GPU arm is exercised on the B200 box.)"""
+under a multi-rank launch only rank 0 works. (The GPU arm needs a GPU.)"""
 import json
 import os
 import subprocess

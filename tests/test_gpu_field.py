@@ -1,4 +1,4 @@
-"""GPU parity of the tcnn-shaped boundary and of the fused HashNerfMLP field (CUDA-core impl 0 and tcgen05 impl 1) against
+"""GPU parity of the tcnn-shaped boundary and of the fused HashNerfMLP field (CUDA-core impl 0 and wgmma impl 1) against
 oracle/tcnn_oracle.c. Tolerances (stated, fp16 pipeline): encodings 1 fp16 ulp of the value range (2e-7 abs on 1e-4-scale
 table entries), MLP outputs 2e-3 abs / 1e-2 rel (fp16 activations; accumulation order differs on tensor cores)."""
 import numpy as np
@@ -149,7 +149,7 @@ def test_deeper_networks(port):
 @pytest.mark.parametrize('impl,n', [(0, 3000), (1, 3000), (1, 128), (1, 40001)])
 def test_field_backward_vs_oracle(port, field_and_weights, impl, n):
     """gradients of the three parameter vectors: fp32 oracle backward on the fp16-rounded forward. impl 0 (CUDA cores) stages only dY in fp16 (x4096);
-    impl 1 (tcgen05: dX and dW as UMMA instructions, dW accumulated in TMEM) rounds every layer's dZ to fp16 like tcnn does => 3e-3 relative to the
+    impl 1 (wgmma: dX and dW as tensor-core instructions, dW accumulated in registers) rounds every layer's dZ to fp16 like tcnn does => 3e-3 relative to the
     largest gradient of each vector for both."""
     f, table, dens, color = field_and_weights
     pts, dirs = _pts(n, seed=21)

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-G = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden.npz'))
+G = {**np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden.npz')), **np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden_embedded.npz'))}
 
 
 def dev(a):

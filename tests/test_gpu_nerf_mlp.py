@@ -1,4 +1,4 @@
-"""GPU parity of the fused tcgen05 NerfMLP kernel (xrb_nerf_mlp_forward) against the fp32 path of the same module (library GEMMs, the
+"""GPU parity of the fused wgmma NerfMLP kernel (xrb_nerf_mlp_forward) against the fp32 path of the same module (library GEMMs, the
 reference's arithmetic) and the numpy oracle. Tolerance for the fp16-operand / fp32-accumulate pipeline over 12 layers:
 |err| <= 2e-2 * max|raw| (measured ~3e-3); composited rgb <= 5e-3."""
 import numpy as np
@@ -150,7 +150,7 @@ def test_posenc_tile_images_match_fp32_posenc(monkeypatch):
 
 
 def test_fused_mip_renderer_matches_registry_network():
-    """MipNerfRenderer (IPE tile images -> tcgen05 MLP -> composite, 2 levels) vs MipNerfNetwork.forward(is_test=True) with the fp32 library-GEMM MLP.
+    """MipNerfRenderer (IPE tile images -> wgmma MLP -> composite, 2 levels) vs MipNerfNetwork.forward(is_test=True) with the fp32 library-GEMM MLP.
     Tolerance: fp16-operand MLP over 12 layers, then two composites and a resampling that moves with the coarse weights: rgb 1e-2."""
     from xrnerf_b200 import registry as R
     from xrnerf_b200.nerf import MipNerfRenderer
@@ -171,8 +171,8 @@ def test_fused_mip_renderer_matches_registry_network():
 
 @pytest.mark.parametrize('cfg,n_rows', [(NERF_MLP, 1), (NERF_MLP, 129), (NERF_MLP, 2 * 296 * 128 + 77), (MIP_MLP, 128), (MIP_MLP, 2 * 296 * 128 + 300)])
 def test_nerf_mlp_v3_two_tiles_in_flight_matches_v2_and_fp32(cfg, n_rows, monkeypatch):
-    """csrc/nerf_mlp_tc3.cu (two tile pipelines per SM, AUX block time-shared by point / direction encodings, several tiles per pipeline at the
-    larger sizes) against v2 (same fp16 arithmetic in the same K order: <= 1e-3 of max|raw|, normally bit-identical) and the fp32 library path (2e-2)."""
+    """the v3 entry of csrc/nerf_mlp_tc.cu (256-wide layers streamed as [256 x 32] K-half slabs with 64-byte swizzle, several tiles per CTA at the larger sizes)
+    against v2 (same fp16 arithmetic: <= 1e-3 of max|raw|, normally bit-identical) and the fp32 library path (2e-2)."""
     from xrnerf_b200 import registry as R
     from xrnerf_b200.nerf_mlp import nerf_mlp_forward
     torch.manual_seed(7)
@@ -189,26 +189,3 @@ def test_nerf_mlp_v3_two_tiles_in_flight_matches_v2_and_fp32(cfg, n_rows, monkey
     with torch.no_grad():
         ref = _ref_fp32(mlp, emb[:4096])
     assert (out['3'][:4096] - ref).abs().max().item() <= 2e-2 * ref.abs().max().item() + 1e-3
-
-
-@pytest.mark.parametrize('cfg,n_rows', [(NERF_MLP, 1), (NERF_MLP, 5 * 128 + 3), (NERF_MLP, 2 * 296 * 128 + 77), (MIP_MLP, 2 * 296 * 128 + 300)])
-def test_nerf_mlp_v3_cta_pair_multicast_matches_single_cta(cfg, n_rows, monkeypatch):
-    """XRB_N3_CLUSTER=1: clusters of two CTAs, rank 0 loads every weight slab once and the TMA multicasts it into both CTAs' rings (phantom tiles keep the
-    pair in lock step at the ragged end). Same arithmetic, same order: identical results."""
-    from xrnerf_b200 import registry as R
-    from xrnerf_b200.nerf_mlp import nerf_mlp_forward
-    torch.manual_seed(11)
-    mlp = R.build_mlp(cfg).cuda()
-    emb = torch.randn((n_rows, mlp.input_ch + mlp.input_ch_dirs), device='cuda').clamp_(-1, 1)
-    monkeypatch.setenv('XRB_NERF_MLP_V', '3')
-    image, bias = mlp._packed()
-    out = {}
-    monkeypatch.setenv('XRB_N3_SHARED_RING', '0')             # private 2-slot rings (MD 0) / CTA pairs (MD 1)
-    for cl in ('0', '1'):
-        monkeypatch.setenv('XRB_N3_CLUSTER', cl)
-        out[cl] = nerf_mlp_forward(image, bias, emb, mlp.input_ch, mlp.input_ch_dirs, version=3).clone()
-    monkeypatch.setenv('XRB_N3_CLUSTER', '0')
-    monkeypatch.setenv('XRB_N3_SHARED_RING', '1')             # one 4-slot ring consumed in the global order P0.layer, P1.layer, ... (csrc/nerf_mlp_tc3.cu, MD 2)
-    out['sr'] = nerf_mlp_forward(image, bias, emb, mlp.input_ch, mlp.input_ch_dirs, version=3).clone()
-    torch.cuda.synchronize()
-    assert torch.equal(out['0'], out['1']) and torch.equal(out['0'], out['sr'])

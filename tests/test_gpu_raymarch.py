@@ -73,9 +73,7 @@ def test_rays_sampler_dense_grid_1024_cap_and_empty(rm, port, scene):
 @pytest.mark.parametrize('aabb,cone', [((0.0, 1.0), 0.0), ((0.0, 1.0), 1.0 / 64), ((-0.5, 1.5), 1.0 / 256), ((-3.5, 4.5), 1.0 / 256), ((0.1, 0.8), 0.0)])
 def test_rays_sampler_any_aabb_cone(rm, port, scene, aabb, cone):
     """Which cell and cascade a tested position falls in depends on the position AND on the step at t (mip_from_dt): sparse random occupancy in EVERY cascade,
-    growing steps (cone > 0), boxes that are not the unit cube and axis-parallel rays (zero direction components), bit-exact vs the oracle. (Round 2 used this case to
-    validate three exact restructurings of the count pass - coarse culling, chain re-join, lane-split rays - none of which beat the plain kernel:
-    profiles/r02_march_experiments.md.)"""
+    growing steps (cone > 0), boxes that are not the unit cube and axis-parallel rays (zero direction components), bit-exact vs the oracle."""
     rng = np.random.default_rng(5)
     bf = np.zeros_like(scene['bitfield']).reshape(8, -1)
     for m in range(8):                       # a few isolated occupied cells per cascade, plus the scene's own cascade 0

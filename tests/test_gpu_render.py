@@ -1,4 +1,4 @@
-"""GPU parity of the fused NGP render (xrb_ngp_render: march -> tcgen05 field -> composite, no host sync) against the
+"""GPU parity of the fused NGP render (xrb_ngp_render: march -> wgmma field -> composite, no host sync) against the
 oracle chain (reference march kernels on CPU -> tcnn restatement -> reference compositing kernel on CPU).
 numsteps: bit-exact. rgb/alpha: 2e-3 abs (fp16 field, see test_gpu_field.py)."""
 import numpy as np
@@ -119,7 +119,7 @@ def test_strided_rays_render_the_same_image(scene, setup):
 
 
 def test_fused_single_launch_matches_oracle_and_unfused(port, scene, setup):
-    """xrb_ngp_render_fused (one launch: march + encode + tcgen05 MLPs + composite) vs the oracle chain and vs the 5-launch path.
+    """xrb_ngp_render_fused (one launch: march + encode + wgmma MLPs + composite) vs the oracle chain and vs the 5-launch path.
     samples per ray: bit-exact. rgb/alpha: 2e-3 vs the oracle (fp16 field), 2e-5 vs the unfused CUDA path (identical field arithmetic, the
     composite is a segmented scan instead of a sequential product)."""
     from xrnerf_b200.ngp import NgpRenderer
@@ -177,7 +177,7 @@ def test_fused_full_image_and_dense_grid(scene, setup):
 
 @pytest.mark.parametrize('T,bwd_impl', [(1 << 16, 1), (1 << 16, 0), (20000, 1)])
 def test_trainer_step_matches_autograd_path(scene, setup, T, bwd_impl):
-    """One fused training step (xrnerf_b200.train.NgpTrainer: march + compaction on the aux stream, device-side sample counts, tcgen05 field backward) against
+    """One fused training step (xrnerf_b200.train.NgpTrainer: march + compaction on the aux stream, device-side sample counts, wgmma field backward) against
     the registry/autograd path the reference's call sites use (rays_sampler_api -> compacted_coord_api -> NgpField autograd -> _CalcRgbBp -> HuberLoss x5):
     same loss, same parameter gradients (T = 2^16: nothing truncated; T = 20000: ray-order truncation, padding rows beyond the compacted count unread), and the
     trained-ray count the trainer reports is what the compaction kept."""
@@ -221,13 +221,13 @@ def test_trainer_step_matches_autograd_path(scene, setup, T, bwd_impl):
         scale = float(b.abs().max())
         err = (a - b).abs()
         assert scale > 0
-        # both sides run the same forward kernel; the backward differs only in the path compared (tcgen05 vs itself through autograd: identical; CUDA cores: fp16 dZ staging)
+        # both sides run the same forward kernel; the backward differs only in the path compared (wgmma vs itself through autograd: identical; CUDA cores: fp16 dZ staging)
         assert float(err.max()) <= (2e-2 if bwd_impl == 0 else 1e-5) * scale, (name, float(err.max()), scale)
         assert float(torch.sqrt((err.double() ** 2).sum() / (b.double() ** 2).sum())) <= 3e-3, name
 
 
 def test_trainer_reduces_loss_and_keeps_shadows_current(scene, setup):
-    """several fused steps with next-batch prefetch: the loss goes down and the fp16 table / cell image / UMMA weight image the optimiser refreshed are exactly
+    """several fused steps with next-batch prefetch: the loss goes down and the fp16 table / cell image / wgmma weight image the optimiser refreshed are exactly
     what a forced refresh() would build"""
     from xrnerf_b200.ngp import NgpField
     from xrnerf_b200.train import NgpTrainer

@@ -8,7 +8,7 @@ import pytest
 
 from oracle import nerf_oracle as O
 
-G = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden.npz'))
+G = {**np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden.npz')), **np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden_embedded.npz'))}
 
 
 def close(a, b, tol=1e-5):
@@ -19,7 +19,7 @@ def test_embed_and_mlp():
     e = O.embed(G['pts'], G['viewdirs'])
     assert e.shape == G['embedded'].shape == (24 * 64, 90)
     assert close(e, G['embedded'], 2e-5)
-    sd = {k[4:]: G[k] for k in G.files if k.startswith('mlp.')}
+    sd = {k[4:]: G[k] for k in G if k.startswith('mlp.')}
     raw = O.nerf_mlp(sd, G['embedded'], 63, 27).reshape(24, 64, 4)
     assert close(raw, G['raw'], 1e-4)
 

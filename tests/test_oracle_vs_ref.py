@@ -2,24 +2,186 @@
 
 CPU-only. The index path (march, compaction, grid sampling, bitfield) must agree bit for bit; compositing, whose
 only transcendental is expf on both sides here, must agree to the last ulp as well (we assert <= 1e-6 abs).
+The reference side is recorded in tests/golden/oracle_ref.npz (tests/golden/make_golden_oracle.py runs these same cases through oracle/_ref):
+SHA-256 digests of the arrays that must agree bit for bit, and a seeded sample of rows of the ones compared with a tolerance.
 """
+import hashlib
+import os
+
 import numpy as np
 import pytest
 
 from xrnerf_b200 import synth
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'oracle_ref.npz')
+N_ROWS_SAMPLED = 1024
 
 
 def _bits(a):
     return np.ascontiguousarray(a).view(np.uint32)
 
 
-@pytest.fixture(scope='module')
-def marched(port, ref, scene):
-    s = scene
+def digest(*arrays):
+    h = hashlib.sha256()
+    for a in arrays:
+        a = np.ascontiguousarray(a)
+        h.update(f'{a.dtype.str}{a.shape}'.encode()); h.update(a.tobytes())
+    return h.hexdigest()
+
+
+class Golden:
+    """compares the port's results with the recorded reference results"""
+
+    def __init__(self, path):
+        self.d = np.load(path)
+
+    def exact(self, key, *arrays):
+        assert digest(*arrays) == str(self.d[key]), key
+
+    def close(self, key, a, atol, relative=False):
+        a = np.asarray(a).reshape(a.shape[0], -1)
+        tol = atol * max(1.0, float(self.d[key + '/absmax'])) if relative else atol
+        assert np.abs(a[self.d[key + '/rows']] - self.d[key]).max() <= tol, key
+
+    def value(self, key):
+        return self.d[key]
+
+
+class Record:
+    """collects the reference's results (tests/golden/make_golden_oracle.py)"""
+
+    def __init__(self):
+        self.d = {}
+
+    def exact(self, key, *arrays):
+        self.d[key] = np.array(digest(*arrays))
+
+    def close(self, key, a, atol, relative=False):
+        a = np.asarray(a).reshape(a.shape[0], -1)
+        rows = np.sort(np.random.default_rng(len(self.d)).choice(a.shape[0], min(N_ROWS_SAMPLED, a.shape[0]), replace=False))
+        self.d[key + '/rows'], self.d[key], self.d[key + '/absmax'] = rows.astype(np.int32), a[rows], np.float64(np.abs(a).max())
+
+
+# ---- the cases: inputs always come from the port (as in a direct comparison), results from `impl` (the port here, the reference when recording)
+def march(impl, s):
     kw = dict(metadata=s['metadata'], img_ids=s['img_ids'], xforms=s['poses'])
-    p = port.rays_sampler(s['rays_o'], s['rays_d'], s['bitfield'], 4096 * 1024)
-    r = ref.rays_sampler(s['rays_o'], s['rays_d'], s['bitfield'], 4096 * 1024, **kw)
-    return p, r
+    return impl.rays_sampler(s['rays_o'], s['rays_d'], s['bitfield'], 4096 * 1024, **kw)
+
+
+def raw_for_march(marched):
+    _, _, _, cnt1 = marched
+    rng = np.random.default_rng(5)
+    raw = rng.normal(0, 1.5, (cnt1[1], 4)).astype(np.float32)
+    raw[:, 3] += 2.0
+    return raw
+
+
+def case_march(impl, s, chk, marched):
+    c1, ri1, ns1, cnt1 = marched
+    chk.exact('march', cnt1, ns1, ri1, _bits(c1))
+
+
+def case_second_call(impl, s, chk):
+    o, d = s['rays_o'][:512], s['rays_d'][:512]
+    a = impl.rays_sampler(o, d, s['bitfield'], 512 * 1024, n_prior_calls=3)
+    chk.exact('march_prior3', _bits(a[0]), a[2])
+    return a
+
+
+def case_edge_rays(impl, s, chk):
+    # axis-parallel dirs (division by zero inside the slab test), rays that miss, origin inside the box, and a tiny buffer
+    o = np.array([[0.5, 0.5, -1.0], [0.5, 0.5, 0.5], [2.0, 2.0, 2.0], [0.5, -1.0, 0.5], [0.1, 0.2, -0.5]], np.float32)
+    d = np.array([[0, 0, 1], [0.6, 0.0, 0.8], [1, 0, 0], [0, 1, 0], [0.3, 0.2, 0.9327379]], np.float32)
+    o = np.concatenate([o, s['rays_o'][:251]]); d = np.concatenate([d, s['rays_d'][:251]])
+    for cap in (256 * 1024, 700):
+        a = impl.rays_sampler(o, d, s['bitfield'], cap)
+        chk.exact(f'edge_{cap}', *[_bits(x) if x.dtype == np.float32 else x for x in a])
+
+
+def case_all_ones(impl, s, chk):
+    bf = np.full_like(s['bitfield'], 255)
+    a = impl.rays_sampler(s['rays_o'][:64], s['rays_d'][:64], bf, 64 * 1024)
+    chk.exact('all_ones', a[2], _bits(a[0]))
+    return a
+
+
+def case_compacted(impl, port, chk, marched, raw):
+    c1, _, ns1, cnt1 = marched
+    coords = c1[:cnt1[1]]
+    for cap in (1 << 18, 20000, 1):
+        a = impl.compacted_coord(raw, coords, ns1, cap)
+        chk.exact(f'compact_{cap}', a[1], a[2], a[3], _bits(a[0]))
+
+
+def case_calc_rgb(impl, port, chk, marched, raw_for, rgb_act, dens_act):
+    c1, _, ns1, cnt1 = marched
+    coords = c1[:cnt1[1]]
+    cc, nsc, _, _ = port.compacted_coord(raw_for, coords, ns1, 30000)  # truncation on: some rays lose their background term
+    raw = raw_for[:30000].copy()
+    if dens_act == 0:
+        raw[:, 3] = np.abs(raw[:, 3]) * 0.1
+    rng = np.random.default_rng(7)
+    bg = rng.random((ns1.shape[0], 3)).astype(np.float32)
+    f1 = port.calc_rgb_forward(raw, cc, ns1, nsc, bg, rgb_act, dens_act)
+    chk.close(f'fwd_{rgb_act}{dens_act}', impl.calc_rgb_forward(raw, cc, ns1, nsc, bg, rgb_act, dens_act), 1e-6)
+    g = rng.normal(0, 1, f1.shape).astype(np.float32)
+    for mean in (0.5, 0.001):
+        b = impl.calc_rgb_backward(raw, nsc, cc, g, f1, np.array([mean], np.float32), rgb_act, dens_act)
+        chk.close(f'bwd_{rgb_act}{dens_act}_{mean}', b, 1e-6, relative=True)
+    i = impl.calc_rgb_inference(raw_for, coords, ns1, np.array([0.2, 0.4, 0.9], np.float32), rgb_act, dens_act)
+    chk.close(f'inf_rgb_{rgb_act}{dens_act}', i[0], 1e-6)
+    chk.close(f'inf_alpha_{rgb_act}{dens_act}', i[1], 1e-6)
+
+
+def case_mark_untrained(impl, s, chk):
+    focal = np.full((s['poses'].shape[0], 2), synth.FOCAL, np.float32)
+    a = impl.mark_untrained(focal[:7], s['poses'][:7], 7, (800, 800))
+    chk.exact('mark_untrained', a)
+    return a
+
+
+def case_grid_samples(impl, s, chk):
+    grid = s['grid'].copy()
+    grid[128 ** 3:] = -1.0
+    for step, thresh, n, nprior in ((0, -0.01, 1 << 16, 0), (5, 0.01, 1 << 15, 4)):
+        a = impl.generate_grid_samples(grid, step, n, 0, thresh, n_prior_calls=nprior)
+        chk.exact(f'grid_samples_{step}', a[1], _bits(a[0]))
+    # multi-cascade scene (aabb_scale 4 -> max_cascade 2)
+    a = impl.generate_grid_samples(grid, 1, 1 << 14, 2, -0.01)
+    chk.exact('grid_samples_cascade', a[1], _bits(a[0]))
+
+
+def case_splat_ema_bitfield(impl, port, s, chk):
+    rng = np.random.default_rng(3)
+    n = 1 << 16
+    idx = rng.integers(0, 128 ** 3, n).astype(np.int32)
+    idx[:100] = idx[0]  # collisions
+    dens = rng.normal(-3, 2, (n, 1)).astype(np.float32)
+    tmp0 = np.zeros(8 * 128 ** 3, np.float32)
+    chk.exact('splat', _bits(impl.splat(dens, idx, tmp0)))
+    a = port.splat(dens, idx, tmp0)
+    grid = s['grid'].copy()
+    grid[rng.integers(0, grid.size, 5000)] = -1.0
+    chk.exact('ema', _bits(impl.ema(a, grid)))
+    e1 = port.ema(a, grid)
+    for k, g in enumerate((e1, s['grid'], np.zeros_like(grid))):
+        b, m = impl.update_bitfield(g)
+        chk.exact(f'bitfield_{k}', b, np.asarray(m[:1]))
+
+
+@pytest.fixture(scope='module')
+def golden():
+    return Golden(GOLDEN)
+
+
+@pytest.fixture(scope='module')
+def marched(port, scene):
+    return march(port, scene)
+
+
+@pytest.fixture(scope='module')
+def raw_for(marched):
+    return raw_for_march(marched)
 
 
 def test_pcg32_stream_matches_reference_header(port):
@@ -30,133 +192,48 @@ def test_pcg32_stream_matches_reference_header(port):
     assert len(set(v.tolist())) == 4
 
 
-def test_rays_sampler_bit_exact(marched):
-    (c1, ri1, ns1, cnt1), (c2, ri2, ns2, cnt2) = marched
-    assert np.array_equal(cnt1, cnt2)
-    assert np.array_equal(ns1, ns2)
-    assert np.array_equal(ri1, ri2)
-    assert np.array_equal(_bits(c1), _bits(c2))
-    assert cnt1[1] > 10000  # the scene is not degenerate
+def test_rays_sampler_bit_exact(port, scene, golden, marched):
+    case_march(port, scene, golden, marched)
+    assert marched[3][1] > 10000  # the scene is not degenerate
 
 
-def test_rays_sampler_second_call_uses_advanced_rng(port, ref, scene):
-    s = scene
-    o, d = s['rays_o'][:512], s['rays_d'][:512]
-    a = port.rays_sampler(o, d, s['bitfield'], 512 * 1024, n_prior_calls=3)
-    b = ref.rays_sampler(o, d, s['bitfield'], 512 * 1024, n_prior_calls=3)
-    a0 = port.rays_sampler(o, d, s['bitfield'], 512 * 1024, n_prior_calls=0)
-    assert np.array_equal(_bits(a[0]), _bits(b[0])) and np.array_equal(a[2], b[2])
+def test_rays_sampler_second_call_uses_advanced_rng(port, scene, golden):
+    a = case_second_call(port, scene, golden)
+    a0 = port.rays_sampler(scene['rays_o'][:512], scene['rays_d'][:512], scene['bitfield'], 512 * 1024, n_prior_calls=0)
     assert not np.array_equal(_bits(a[0]), _bits(a0[0]))
 
 
-def test_rays_sampler_overflow_and_edge_rays(port, ref, scene):
-    s = scene
-    # axis-parallel dirs (division by zero inside the slab test), rays that miss, origin inside the box, and a tiny buffer
-    o = np.array([[0.5, 0.5, -1.0], [0.5, 0.5, 0.5], [2.0, 2.0, 2.0], [0.5, -1.0, 0.5], [0.1, 0.2, -0.5]], np.float32)
-    d = np.array([[0, 0, 1], [0.6, 0.0, 0.8], [1, 0, 0], [0, 1, 0], [0.3, 0.2, 0.9327379]], np.float32)
-    o = np.concatenate([o, s['rays_o'][:251]]); d = np.concatenate([d, s['rays_d'][:251]])
-    for cap in (256 * 1024, 700):
-        a = port.rays_sampler(o, d, s['bitfield'], cap)
-        b = ref.rays_sampler(o, d, s['bitfield'], cap)
-        for x, y in zip(a, b):
-            assert np.array_equal(_bits(x) if x.dtype == np.float32 else x, _bits(y) if y.dtype == np.float32 else y)
+def test_rays_sampler_overflow_and_edge_rays(port, scene, golden):
+    case_edge_rays(port, scene, golden)
 
 
-def test_rays_sampler_all_ones_grid_hits_1024_cap(port, ref, scene):
-    bf = np.full_like(scene['bitfield'], 255)
-    o, d = scene['rays_o'][:64], scene['rays_d'][:64]
-    a = port.rays_sampler(o, d, bf, 64 * 1024)
-    b = ref.rays_sampler(o, d, bf, 64 * 1024)
-    assert np.array_equal(a[2], b[2]) and np.array_equal(_bits(a[0]), _bits(b[0]))
+def test_rays_sampler_all_ones_grid_hits_1024_cap(port, scene, golden):
+    a = case_all_ones(port, scene, golden)
     assert a[2][:, 0].max() > 300
 
 
-@pytest.fixture(scope='module')
-def raw_for(marched):
-    (c1, _, ns1, cnt1), _ = marched
-    rng = np.random.default_rng(5)
-    raw = rng.normal(0, 1.5, (cnt1[1], 4)).astype(np.float32)
-    raw[:, 3] += 2.0
-    return raw
-
-
-def test_compacted_coord(port, ref, marched, raw_for):
-    (c1, _, ns1, cnt1), _ = marched
-    coords = c1[:cnt1[1]]
-    for cap in (1 << 18, 20000, 1):
-        a = port.compacted_coord(raw_for, coords, ns1, cap)
-        b = ref.compacted_coord(raw_for, coords, ns1, cap)
-        assert np.array_equal(a[1], b[1]) and np.array_equal(a[2], b[2]) and np.array_equal(a[3], b[3])
-        assert np.array_equal(_bits(a[0]), _bits(b[0]))
+def test_compacted_coord(port, golden, marched, raw_for):
+    case_compacted(port, port, golden, marched, raw_for)
 
 
 @pytest.mark.parametrize('rgb_act,dens_act', [(2, 3), (3, 1), (0, 2), (1, 0)])
-def test_calc_rgb_forward_backward_inference(port, ref, marched, raw_for, rgb_act, dens_act):
-    (c1, _, ns1, cnt1), _ = marched
-    coords = c1[:cnt1[1]]
-    cc, nsc, _, _ = port.compacted_coord(raw_for, coords, ns1, 30000)  # truncation on: some rays lose their background term
-    raw = raw_for[:30000].copy()
-    if dens_act == 0:
-        raw[:, 3] = np.abs(raw[:, 3]) * 0.1
-    rng = np.random.default_rng(7)
-    bg = rng.random((ns1.shape[0], 3)).astype(np.float32)
-    f1 = port.calc_rgb_forward(raw, cc, ns1, nsc, bg, rgb_act, dens_act)
-    f2 = ref.calc_rgb_forward(raw, cc, ns1, nsc, bg, rgb_act, dens_act)
-    assert np.abs(f1 - f2).max() <= 1e-6
-    g = rng.normal(0, 1, f1.shape).astype(np.float32)
-    for mean in (0.5, 0.001):
-        b1 = port.calc_rgb_backward(raw, nsc, cc, g, f1, np.array([mean], np.float32), rgb_act, dens_act)
-        b2 = ref.calc_rgb_backward(raw, nsc, cc, g, f1, np.array([mean], np.float32), rgb_act, dens_act)
-        assert np.abs(b1 - b2).max() <= 1e-6 * max(1.0, np.abs(b2).max())
-    i1 = port.calc_rgb_inference(raw_for, coords, ns1, np.array([0.2, 0.4, 0.9], np.float32), rgb_act, dens_act)
-    i2 = ref.calc_rgb_inference(raw_for, coords, ns1, np.array([0.2, 0.4, 0.9], np.float32), rgb_act, dens_act)
-    assert np.abs(i1[0] - i2[0]).max() <= 1e-6 and np.abs(i1[1] - i2[1]).max() <= 1e-6
+def test_calc_rgb_forward_backward_inference(port, golden, marched, raw_for, rgb_act, dens_act):
+    case_calc_rgb(port, port, golden, marched, raw_for, rgb_act, dens_act)
 
 
-def test_mark_untrained(port, ref, scene):
-    focal = np.full((scene['poses'].shape[0], 2), synth.FOCAL, np.float32)
-    a = port.mark_untrained(focal[:7], scene['poses'][:7], 7, (800, 800))
-    b = ref.mark_untrained(focal[:7], scene['poses'][:7], 7, (800, 800))
-    assert np.array_equal(a, b)
+def test_mark_untrained(port, scene, golden):
+    a = case_mark_untrained(port, scene, golden)
     assert (a == 0).any() and (a == -1).any()
 
 
-def test_generate_grid_samples(port, ref, scene):
-    grid = scene['grid'].copy()
-    grid[128 ** 3:] = -1.0
-    for step, thresh, n, nprior in ((0, -0.01, 1 << 16, 0), (5, 0.01, 1 << 15, 4)):
-        a = port.generate_grid_samples(grid, step, n, 0, thresh, n_prior_calls=nprior)
-        b = ref.generate_grid_samples(grid, step, n, 0, thresh, n_prior_calls=nprior)
-        assert np.array_equal(a[1], b[1])
-        assert np.array_equal(_bits(a[0]), _bits(b[0]))
-    # multi-cascade scene (aabb_scale 4 -> max_cascade 2)
-    a = port.generate_grid_samples(grid, 1, 1 << 14, 2, -0.01)
-    b = ref.generate_grid_samples(grid, 1, 1 << 14, 2, -0.01)
-    assert np.array_equal(a[1], b[1]) and np.array_equal(_bits(a[0]), _bits(b[0]))
+def test_generate_grid_samples(port, scene, golden):
+    case_grid_samples(port, scene, golden)
 
 
-def test_splat_ema_bitfield(port, ref, scene):
-    rng = np.random.default_rng(3)
-    n = 1 << 16
-    idx = rng.integers(0, 128 ** 3, n).astype(np.int32)
-    idx[:100] = idx[0]  # collisions
-    dens = rng.normal(-3, 2, (n, 1)).astype(np.float32)
-    tmp0 = np.zeros(8 * 128 ** 3, np.float32)
-    a = port.splat(dens, idx, tmp0)
-    b = ref.splat(dens, idx, tmp0)
-    assert np.array_equal(_bits(a), _bits(b))
-    grid = scene['grid'].copy()
-    grid[rng.integers(0, grid.size, 5000)] = -1.0
-    e1 = port.ema(a, grid)
-    e2 = ref.ema(a, grid)
-    assert np.array_equal(_bits(e1), _bits(e2))
-    for g in (e1, scene['grid'], np.zeros_like(grid)):
-        b1, m1 = port.update_bitfield(g)
-        b2, m2 = ref.update_bitfield(g)
-        assert np.array_equal(b1, b2)
-        assert m1[0] == m2[0]
+def test_splat_ema_bitfield(port, scene, golden):
+    case_splat_ema_bitfield(port, port, scene, golden)
 
 
-def test_numpy_scene_builder_agrees_with_reference_bitfield(ref, scene):
-    b2, m2 = ref.update_bitfield(scene['grid'])
-    assert np.array_equal(b2, scene['bitfield']) and abs(m2[0] - scene['mean']) < 1e-9
+def test_numpy_scene_builder_agrees_with_reference_bitfield(scene, golden):
+    golden.exact('scene_bitfield', np.asarray(scene['bitfield'], np.uint8))
+    assert abs(float(golden.value('scene_mean')) - scene['mean']) < 1e-9

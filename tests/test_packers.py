@@ -1,5 +1,5 @@
-"""CPU checks of the host-side weight packers of the tcgen05 NerfMLP kernels (xrnerf_b200/nerf_mlp.py): the swizzled byte layouts the kernels'
-shared-memory descriptors assume, and the stream image sizes / bias vector layout of csrc/nerf_mlp_tc3.cu. No GPU needed."""
+"""CPU checks of the host-side weight packers of the wgmma NerfMLP kernels (xrnerf_b200/nerf_mlp.py): the swizzled byte layouts the kernels'
+shared-memory descriptors assume, and the stream image sizes / bias vector layout of the v3 entry of csrc/nerf_mlp_tc.cu. No GPU needed."""
 import numpy as np
 import torch
 

@@ -49,7 +49,7 @@ def test_reference_style_checkpoint_loads_into_modules_and_registry():
     mlp.field._ver = 'stale-marker'
     missing = mlp.load_state_dict(ckpt, strict=True)
     assert not missing.missing_keys and not missing.unexpected_keys
-    assert mlp.field._ver is None                                                           # load_state_dict marks the fp16 shadows / cell image / UMMA image dirty
+    assert mlp.field._ver is None                                                           # load_state_dict marks the fp16 shadows / cell image / wgmma weight image dirty
     for m, k in ((enc, 'embedder_pos.params'), (dnet, 'density_net.params'), (cnet, 'color_net.params')):
         m.import_params(ckpt[k])
         assert torch.equal(m.export_params(), mlp.state_dict()[k])

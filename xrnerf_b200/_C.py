@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libxrnerf_b200.so')
 
 if not os.path.exists(LIB_PATH):
-    raise ImportError(f'{LIB_PATH} is missing: run `python -m xrnerf_b200.build` (needs nvcc; cross-compiles for sm_100a without a GPU). '
+    raise ImportError(f'{LIB_PATH} is missing: run `python -m xrnerf_b200.build` (needs nvcc; cross-compiles for sm_90a without a GPU). '
                       'xrnerf_b200 has no CPU or PyTorch fallback for its kernels.')
 
 lib = C.CDLL(LIB_PATH)

@@ -1,8 +1,8 @@
-"""Builds xrnerf_b200/lib/libxrnerf_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds xrnerf_b200/lib/libxrnerf_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m xrnerf_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot. Sources: xrnerf_b200/csrc/*.cu.
+The .so is a build product (git-ignored). Sources: xrnerf_b200/csrc/*.cu.
 """
 import hashlib
 import os
@@ -15,7 +15,8 @@ CSRC = os.path.join(HERE, 'csrc')
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libxrnerf_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC'] + os.environ.get('XRB_NVCC_DEFINES', '').split()   # e.g. -DXRB_FUSED_TIMERS (developer builds)
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC'] + os.environ.get('XRB_NVCC_DEFINES', '').split()   # e.g. -DXRB_FUSED_TIMERS (developer builds)
 
 
 def _sources():
@@ -40,7 +41,7 @@ def build(force=False, verbose=False):
         return LIB
     if not os.path.exists(NVCC):
         if os.path.exists(LIB):
-            return LIB  # GPU box without a toolkit: use the prebuilt library that travelled with the snapshot
+            return LIB  # machine without a toolkit: use the library built earlier in this tree
         raise RuntimeError('nvcc not found and no prebuilt libxrnerf_b200.so')
     objs = []
 
@@ -53,7 +54,7 @@ def build(force=False, verbose=False):
         return obj
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    subprocess.check_call([NVCC, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs + ['-cudart', 'static'])
+    subprocess.check_call([NVCC, '-shared'] + ARCH + ['-o', LIB] + objs + ['-cudart', 'static'])
     for o in objs:
         os.remove(o)
     with open(stamp, 'w') as fh:

@@ -1,4 +1,4 @@
-// xrnerf_b200 — shared device helpers (sm_100a only).
+// xrnerf_b200 — shared device helpers (sm_90a only).
 //
 // Index-path arithmetic is written with explicit round-to-nearest intrinsics (__fmul_rn/__fadd_rn/__fdiv_rn):
 // nvcc never contracts those into FMAs, which makes the per-ray sample sets bit-reproducible against the
@@ -18,7 +18,7 @@ constexpr uint32_t NERF_CASCADES = 8u;      // :43
 constexpr uint32_t NERF_GRIDSIZE = 128u;    // :48
 constexpr uint32_t GRID_CELLS = 128u * 128u * 128u;
 constexpr float NERF_MIN_OPTICAL_THICKNESS = 0.01f;  // :56
-constexpr int NUM_SMS = 148;
+constexpr int NUM_SMS = 132;   // H100 SXM: the default of launches that query the device, and the cap of some grid-stride launches
 
 // constants folded exactly as the reference's constexpr chain folds them (fp32, left to right)
 __host__ __device__ constexpr float SQRT3() { return 1.73205080757f; }
@@ -89,7 +89,7 @@ __device__ __forceinline__ float div_(float a, float b) { return __fdiv_rn(a, b)
 __device__ __forceinline__ float clampf(float v, float lo, float hi) { return v < lo ? lo : (hi < v ? hi : v); }  // raymarch_shared.h:104-107
 __device__ __forceinline__ float calc_dt(float t, float cone) { return clampf(mul_(t, cone), MIN_CONE_STEPSIZE(), MAX_CONE_STEPSIZE()); }  // ray_sampler_header.h:24-25
 
-// floor() of |p| < 2^22 and its integer value on the FMA/ALU pipes (F2I / FRND / I2F are quarter-rate XU ops on sm_100):
+// floor() of |p| < 2^22 and its integer value on the FMA/ALU pipes (F2I / FRND / I2F run on the quarter-rate XU pipe):
 // t = p + 1.5*2^23 rounds p to the nearest integer into the low mantissa bits; one compare turns round-to-nearest into floor. Exact.
 __device__ __forceinline__ float floor_small(float p, int *ip) {
     float t = __fadd_rn(p, 12582912.0f);

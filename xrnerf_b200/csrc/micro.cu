@@ -16,9 +16,8 @@ __device__ __forceinline__ uint32_t ld_fold(const uint8_t *p);
 template <> __device__ __forceinline__ uint32_t ld_fold<4>(const uint8_t *p) { return __ldg(reinterpret_cast<const uint32_t *>(p)); }
 template <> __device__ __forceinline__ uint32_t ld_fold<8>(const uint8_t *p) { uint2 v = __ldg(reinterpret_cast<const uint2 *>(p)); return v.x ^ v.y; }
 template <> __device__ __forceinline__ uint32_t ld_fold<32>(const uint8_t *p) {
-    uint32_t r[8];
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
-    return r[0] ^ r[1] ^ r[2] ^ r[3] ^ r[4] ^ r[5] ^ r[6] ^ r[7];
+    const uint4 lo = __ldg(reinterpret_cast<const uint4 *>(p)), hi = __ldg(reinterpret_cast<const uint4 *>(p) + 1);   // one 32-byte sector, as ngp_field.cuh ldg_cell
+    return lo.x ^ lo.y ^ lo.z ^ lo.w ^ hi.x ^ hi.y ^ hi.z ^ hi.w;
 }
 
 // every thread: `rounds` rounds of 8 independent loads at pseudo-random record indices (one LCG stream per thread: no two lanes of a warp share a sector on purpose)

@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(256) mip_embed_kernel(int n_rays, int S, int m
     }
 }
 
-// The same cast_rays + IPE + view-direction encoding written straight into the fp16 UMMA tile images the tcgen05 NerfMLP kernel TMA-loads
+// The same cast_rays + IPE + view-direction encoding written straight into the fp16 tile images (wgmma operand layout) the NerfMLP kernel TMA-loads
 // (csrc/nerf_mlp_tc.cu: per 128-row tile, point blocks [128 x 64] x 2 (96 -> 128 columns, zero padded), then the direction block; K-major,
 // 128-byte swizzle): no fp32 `embedded` [N*S,123] round trip (63 GB per 800x800 image in the reference). One thread per (row, 16-byte chunk);
 // the frustum Gaussian is formed once per thread in registers. Values are the fp16 roundings of exactly what mip_embed_kernel produces.

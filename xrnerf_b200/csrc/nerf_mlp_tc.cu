@@ -1,19 +1,24 @@
 // xrnerf_b200 — NerfMLP.run_mlp (/root/reference/xrnerf/models/mlps/nerf_mlp.py:70-94: 8x256 ReLU MLP, skip-concat after layer 4,
-// alpha head, 256-wide feature layer, 128-wide view branch, rgb head) as ONE persistent tcgen05 kernel.
+// alpha head, 256-wide feature layer, 128-wide view branch, rgb head) as ONE persistent wgmma kernel.
 // The reference runs it as 11 cuBLAS fp32 GEMMs + 2 cat per 32 768-row chunk with every [chunk,256] activation round-tripping HBM.
 //
-// Per CTA (1 per SM, 192 threads), per 128-row tile:
-//   warps 0-3  compute warpgroup: thread r owns row r — converts its `embedded` row to fp16 into the A operand blocks, and after each
-//              layer reads its TMEM accumulator row (tcgen05.ld), adds the bias, applies ReLU, rounds to fp16 and rewrites the A blocks;
-//   warp 4     TMA producer: streams the pre-swizzled weight slabs ([N x 64] fp16, K-major SWIZZLE_128B) of all 12 layers from the
-//              L2-resident weight image through a 3-slot shared-memory ring (cp.async.bulk + mbarrier expect_tx);
-//   warp 5     MMA issuer: per slab 4 x tcgen05.mma (M=128, N=256|128|16, K=16), tcgen05.commit frees the slab slot; after the last
-//              slab of a layer a commit signals the epilogue.
+// Per CTA (1 per SM, 384 threads), per 128-row tile:
+//   warps 0-7  two consumer warpgroups: warpgroup h owns rows 64h..64h+63 of the tile. Per layer it issues wgmma.m64nNk16 (N = 256 | 128 | 16)
+//              over the weight slabs as they arrive, keeps the [64 x N] fp32 accumulator in registers (up to 128 per thread), then adds the bias,
+//              applies ReLU, rounds to fp16 and writes its rows of the next layer's A operand blocks straight from the accumulator fragment.
+//              The two warpgroups never wait for each other: a row's next-layer input depends on that row only.
+//   warp 8     TMA producer (its warpgroup gives its registers to the two consumer warpgroups: setmaxnreg 40 / 232): streams the pre-swizzled weight slabs of all 11 layers from the L2-resident weight image through a shared-memory
+//              ring (cp.async.bulk + mbarrier expect_tx; a slot is released when all 8 consumer warps have finished the MMAs that read it), and
+//              (v2 / v3) the tile's fp16 encoding blocks, re-armed once both warpgroups are past their last reader (views_linears.0).
 // A operand: [128 x 64]-blocks, K-major, 128-byte swizzle: blocks 0-3 hidden state h (256 wide), 4..4+AUX-1 the point encoding
-// (63 -> 64 for NeRF, 96 -> 128 for Mip-NeRF), last block the view-direction encoding (27 -> 64). Accumulators: TMEM columns 0-255
-// (main) and 256-271 (alpha head, issued next to the feature layer on the same A tile).
-// Numeric contract: fp16 operands (weights and activations), fp32 accumulate + fp32 bias; parity tolerance vs the fp32 reference
-// is stated in tests/test_gpu_nerf_mlp.py.
+// (63 -> 64 for NeRF, 96 -> 128 for Mip-NeRF), last block the view-direction encoding (27 -> 64).
+// The three entry points differ in how the host packed the weights (xrnerf_b200/nerf_mlp.py) and in one numeric detail:
+//   v1  [N x 64] slabs, one per K-block; fp32 embedded rows converted in the kernel; bias added in fp32 before rounding; alpha head as 16 extra
+//       rows of the feature layer's slabs (an N=16 MMA next to the N=256 one)
+//   v2  [N/2 x 64] half slabs; v3  [256 x 32] K-half slabs (64-byte swizzle) for the 256-wide layers, [N x 64] otherwise. Both take the fp16
+//       encoding tile image (xrb_nerf_pack_embedded / posenc / IPE kernels), add the bias in fp16 after rounding the accumulator, and form alpha
+//       as a register dot product with alpha_linear in the epilogue of pts_linears.7. Same arithmetic: v2 and v3 give the same result.
+// Numeric contract: fp16 operands (weights and activations), fp32 accumulate; parity tolerance vs the fp32 reference in tests/test_gpu_nerf_mlp.py.
 #include "tc.cuh"
 #include "common.cuh"
 #include <cuda_fp16.h>
@@ -21,381 +26,264 @@
 
 namespace xrb {
 
-constexpr int NM_W = 256;
-constexpr int NM_MAX_LAYERS = 12;
-constexpr int NM_SLOTS = 3;
-constexpr uint32_t NM_SLAB_BYTES = 272 * 128;   // largest slab: feature (256) + alpha (16) rows
-constexpr int NM_THREADS = 192;
-
-struct NmLayer {
-    int n_kblocks;        // K-blocks of 64
-    int kblock_src[6];    // which A block feeds each K-block
-    int N;                // main output width (256 / 128 / 16)
-    int n_alpha;          // 16 when the alpha head rides along (extra rows in every slab of this layer), else 0
-    int bias_off;         // offset into the bias vector (main), alpha bias follows at bias_off + N when n_alpha
-    int relu;
-    int out_blocks;       // how many 64-wide A blocks the epilogue writes (N/64; 0 for the last layer)
-};
-struct NmPlan {
-    int n_layers, aux_blocks, input_ch, input_ch_dirs;
-    NmLayer layer[NM_MAX_LAYERS];
-};
+constexpr int NM_THREADS = 384;
+constexpr int NM_LAYERS = 11;
+constexpr int NM_MAX_SLABS = 12;
+constexpr uint32_t NM_BLOCK = 16384;
 
 __device__ __forceinline__ uint32_t nm_pack_h2(float a, float b) { __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<uint32_t *>(&h); }
 __device__ __forceinline__ uint32_t nm_sw128(uint32_t row, uint32_t chunk16) { return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk16 ^ (row & 7u)) << 4); }
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory"); }
 
-__global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_tc_kernel(NmPlan plan, const uint8_t *__restrict__ weight_image, const float *__restrict__ bias, const float *__restrict__ embedded,
-                                                                     int64_t n_rows, float *__restrict__ raw) {
+// ---- compile-time layer schedule (the consumer's loops over layers and slabs are fully unrolled: accumulator offsets must be constants)
+struct NmSlab {
+    int a_blk;     // A block the slab contracts with
+    int kh;        // -1: all 64 columns of the block (128-byte swizzled [rows x 64] slab); 0 / 1: columns 32kh.. ([rows x 32], 64-byte swizzle)
+    int rows;      // output columns the slab covers (slab rows), starting at accumulator column col0
+    int col0;
+    int first;     // first slab of the layer that writes columns [col0, col0 + rows): overwrite instead of accumulate
+    int alpha;     // v1: 16 more rows (the alpha head) follow, into the separate N=16 accumulator
+};
+struct NmLayer {
+    int N, relu, bias_off, alpha_dot, n_slabs;
+    NmSlab s[NM_MAX_SLABS];
+};
+__host__ __device__ constexpr uint32_t nm_slab_bytes(const NmSlab &s) { return (uint32_t)(s.rows + (s.alpha ? 16 : 0)) * (s.kh >= 0 ? 64u : 128u); }
+
+template <int VER, bool MIP>
+__host__ __device__ constexpr NmLayer nm_layer(int l) {
+    const int aux = MIP ? 2 : 1, P0 = 4, P1 = 5, DIR = 4 + aux;
+    NmLayer L{};
+    L.N = l == 9 ? 128 : (l == 10 ? 16 : 256);
+    L.relu = (l == 8 || l == 10) ? 0 : 1;
+    L.alpha_dot = VER >= 2 && l == 7;
+    L.bias_off = VER == 1 ? (l <= 8 ? 256 * l : (l == 9 ? 2320 : 2448)) : (l <= 9 ? 256 * l : 2432);   // v1: the feature layer carries 16 alpha-head biases
+    int src[6] = {0, 1, 2, 3, 0, 0}, nk = 4;
+    if (l == 0) { src[0] = P0; src[1] = P1; nk = aux; }
+    else if (l == 5) {
+        if (VER == 1) { src[4] = P0; src[5] = P1; nk = 4 + aux; }
+        else if (VER == 2) { src[0] = P0; src[1] = P1; src[aux] = 0; src[aux + 1] = 1; src[aux + 2] = 2; src[aux + 3] = 3; nk = 4 + aux; }
+        else { src[0] = P0; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; src[5] = P1; nk = 4 + aux; }
+    } else if (l == 9) {
+        if (VER == 1) { src[4] = DIR; } else { src[0] = DIR; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; }
+        nk = 5;
+    } else if (l == 10) nk = 2;
+    int n = 0;
+    for (int k = 0; k < nk; ++k) {
+        if (VER == 1) {
+            L.s[n++] = NmSlab{src[k], -1, L.N, 0, k == 0, l == 8};
+        } else if (VER == 2) {
+            const int halves = L.N == 16 ? 1 : 2;
+            for (int h = 0; h < halves; ++h) L.s[n++] = NmSlab{src[k], -1, L.N / halves, h * (L.N / halves), k == 0, 0};
+        } else {
+            if (L.N == 256) { L.s[n++] = NmSlab{src[k], 0, 256, 0, k == 0, 0}; L.s[n++] = NmSlab{src[k], 1, 256, 0, 0, 0}; }
+            else L.s[n++] = NmSlab{src[k], -1, L.N, 0, k == 0, 0};
+        }
+    }
+    L.n_slabs = n;
+    return L;
+}
+
+struct NmParams {
+    const uint8_t *weight_image; const float *bias; const float *embedded; const uint8_t *enc_image;
+    int64_t n_rows; int input_ch, input_ch_dirs;
+    float *raw;
+    uint32_t slot_bytes; int n_slots;
+    uint32_t n_slabs[NM_LAYERS]; uint32_t slab_bytes[NM_LAYERS][NM_MAX_SLABS];   // the producer's stream (from nm_layer on the host)
+};
+
+struct NmCtx {
+    uint8_t *A, *ring; uint64_t *full, *empty;
+    uint32_t it, wg, t, r0, lane, n_slots, slot_bytes;
+};
+
+template <int N>
+__device__ __forceinline__ void nm_mma(float *acc, uint64_t ad, uint64_t bd, uint32_t sc) { tc::wgmma<N>(acc, ad, bd, sc); }
+
+// the MMAs of slabs [S, n_slabs) of layer L, one slab at a time through the ring
+template <int VER, bool MIP, int L, int S>
+__device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc, float *acc_a) {
+    constexpr NmLayer Ly = nm_layer<VER, MIP>(L);
+    if constexpr (S < Ly.n_slabs) {
+        constexpr NmSlab sl = Ly.s[S];
+        const uint32_t slot = x.it % x.n_slots, ph = (x.it / x.n_slots) & 1u;
+        tc::mbar_wait(x.full + slot, ph);
+        const uint32_t a0 = tc::smem_u32(x.A + (size_t)sl.a_blk * NM_BLOCK) + x.wg * 8192u + (sl.kh > 0 ? 64u : 0u);
+        const uint32_t b0 = tc::smem_u32(x.ring + (size_t)slot * x.slot_bytes);
+        tc::wg_fence();
+#pragma unroll
+        for (int k = 0; k < (sl.kh >= 0 ? 2 : 4); ++k) {
+            const uint32_t sc = (sl.first && k == 0) ? 0u : 1u;
+            const uint64_t ad = tc::desc_k128(a0 + k * 32), bd = sl.kh >= 0 ? tc::desc_k64(b0 + k * 32) : tc::desc_k128(b0 + k * 32);
+            nm_mma<sl.rows>(acc + sl.col0 / 2, ad, bd, sc);
+            if constexpr (sl.alpha) nm_mma<16>(acc_a, ad, tc::desc_k128(b0 + (uint32_t)sl.rows * 128u + k * 32), sc);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        __syncwarp();
+        if (x.lane == 0) tc::mbar_arrive(x.empty + slot);   // this warp's share of the MMAs reading the slot is complete
+        ++x.it;
+        nm_slabs<VER, MIP, L, S + 1>(x, acc, acc_a);
+    }
+}
+
+// layers [L, 11) of one tile for my 64 rows
+template <int VER, bool MIP, int L>
+__device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t tile, float *alpha) {
+    if constexpr (L < NM_LAYERS) {
+        constexpr NmLayer Ly = nm_layer<VER, MIP>(L);
+        float acc[Ly.N / 2], acc_a[8];
+        tc::fence_proxy_async_smem();        // my epilogue / staging writes -> visible to the tensor core
+        tc::named_bar_sync(1 + x.wg, 128);   // ... and every row of my warpgroup written
+        nm_slabs<VER, MIP, L, 0>(x, acc, acc_a);
+        tc::acc_fence<Ly.N / 2>(acc);
+        if constexpr (VER == 1 && L == 8) tc::acc_fence<8>(acc_a);
+        tc::named_bar_sync(1 + x.wg, 128);   // every warp's share of this layer's MMAs has completed before A blocks are rewritten
+        const float *b = P.bias + Ly.bias_off;
+        if constexpr (L == NM_LAYERS - 1) {
+            // rgb_linear: columns 0,1 sit in lane q = 0 of a quad, columns 2,3 in lane q = 1
+            const float c2a = __shfl_down_sync(0xffffffffu, acc[0], 1), c2b = __shfl_down_sync(0xffffffffu, acc[2], 1);
+            if ((x.t & 3u) == 0) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int64_t i = tile * 128 + x.r0 + 8 * e;
+                    if (i < P.n_rows) reinterpret_cast<float4 *>(P.raw)[i] = make_float4(acc[2 * e] + __ldg(b), acc[2 * e + 1] + __ldg(b + 1), (e ? c2b : c2a) + __ldg(b + 2), alpha[e]);
+                }
+            }
+        } else {
+            float adot[2] = {0.f, 0.f};
+            const float *wa = P.bias + 2448;   // v2 / v3: alpha_linear weights follow the per-layer biases, then its bias
+#pragma unroll
+            for (int j = 0; j < Ly.N / 8; ++j) {
+                const uint32_t col = tc::frag_col(x.t, j);
+                uint8_t *blk = x.A + (size_t)(col >> 6) * NM_BLOCK;
+                const float b0 = __ldg(b + col), b1 = __ldg(b + col + 1);
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    __half2 h;
+                    if (VER == 1) {
+                        float v0 = acc[4 * j + 2 * e] + b0, v1 = acc[4 * j + 2 * e + 1] + b1;
+                        if (Ly.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                        h = __floats2half2_rn(v0, v1);
+                    } else {
+                        h = __hadd2(__floats2half2_rn(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), __floats2half2_rn(b0, b1));
+                        if (Ly.relu) h = __hmax2(h, __float2half2_rn(0.f));
+                        if (Ly.alpha_dot) { const float2 f = __half22float2(h); adot[e] = fmaf(f.x, __ldg(wa + col), adot[e]); adot[e] = fmaf(f.y, __ldg(wa + col + 1), adot[e]); }
+                    }
+                    *reinterpret_cast<__half2 *>(blk + nm_sw128(x.r0 + 8u * (uint32_t)e, (col & 63u) >> 3) + (col & 7u) * 2u) = h;
+                }
+            }
+            if constexpr (Ly.alpha_dot) {   // the four lanes of a quad hold all 256 columns of its two rows
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    adot[e] += __shfl_xor_sync(0xffffffffu, adot[e], 1);
+                    adot[e] += __shfl_xor_sync(0xffffffffu, adot[e], 2);
+                    alpha[e] = adot[e] + __ldg(wa + 256);
+                }
+            }
+            if constexpr (VER == 1 && L == 8) { alpha[0] = acc_a[0] + __ldg(b + 256); alpha[1] = acc_a[2] + __ldg(b + 256); }   // column 0 of the alpha head
+        }
+        nm_layers<VER, MIP, L + 1>(x, P, tile, alpha);
+    }
+}
+
+template <int VER, bool MIP>
+__global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid_constant__ NmParams P) {
     extern __shared__ uint8_t dyn_smem[];
+    constexpr int AUX = MIP ? 2 : 1;
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    const int n_ablocks = 5 + plan.aux_blocks;
-    uint8_t *A = base;                                        // n_ablocks x 16 KB
-    uint8_t *slab = A + (size_t)n_ablocks * 16384;            // NM_SLOTS x NM_SLAB_BYTES (1024-aligned: 34816 = 34 x 1024)
-    uint64_t *bars = (uint64_t *)(slab + (size_t)NM_SLOTS * NM_SLAB_BYTES);
-    uint64_t *full = bars, *empty = bars + NM_SLOTS, *a_ready = bars + 2 * NM_SLOTS, *acc_full = bars + 2 * NM_SLOTS + 1;
-    uint32_t *tmem_slot = (uint32_t *)(bars + 2 * NM_SLOTS + 2);
+    uint8_t *A = base, *ring = A + (size_t)(5 + AUX) * NM_BLOCK;
+    uint64_t *bars = (uint64_t *)(ring + (size_t)P.n_slots * P.slot_bytes);
+    uint64_t *full = bars, *empty = bars + P.n_slots, *enc_full = bars + 2 * P.n_slots, *enc_free = enc_full + 1;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NM_SLOTS; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 1); }
-        tc::mbar_init(a_ready, 128);
-        tc::mbar_init(acc_full, 1);
+        for (int s = 0; s < P.n_slots; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 8); }
+        tc::mbar_init(enc_full, 1); tc::mbar_init(enc_free, 8);
         tc::fence_mbar_init();
     }
-    if (warp == 4) tc::tmem_alloc<512>(tmem_slot);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
-    const int64_t n_tiles = (n_rows + 127) / 128;
-    const int C = plan.input_ch + plan.input_ch_dirs;
+    const int64_t n_tiles = (P.n_rows + 127) / 128;
+    const uint32_t enc_bytes = (uint32_t)(AUX + 1) * NM_BLOCK;
 
-    if (warp == 4) {
-        // ===================================================== TMA producer
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    if (warp >= 8) {
+        // ===================================================== TMA producer (one lane)
+        tc::setmaxnreg_dec<40>();
+        if (warp == 8 && lane == 0) {
+            uint32_t it = 0, n = 0;
+            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
+                if (VER >= 2) {   // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block)
+                    if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
+                    tc::mbar_expect_tx(enc_full, enc_bytes);
+                    tc::tma_bulk_g2s(A + 4 * NM_BLOCK, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
+                }
                 size_t off = 0;
-                for (int l = 0; l < plan.n_layers; ++l) {
-                    const uint32_t bytes = (uint32_t)(plan.layer[l].N + plan.layer[l].n_alpha) * 128u;
-                    for (int kb = 0; kb < plan.layer[l].n_kblocks; ++kb, ++it) {
-                        const uint32_t slot = it % NM_SLOTS, round = it / NM_SLOTS;
+                for (int l = 0; l < NM_LAYERS; ++l)
+                    for (uint32_t s = 0; s < P.n_slabs[l]; ++s, ++it) {
+                        const uint32_t slot = it % P.n_slots, round = it / P.n_slots, bytes = P.slab_bytes[l][s];
                         if (round > 0) tc::mbar_wait(empty + slot, (round - 1) & 1);
                         tc::mbar_expect_tx(full + slot, bytes);
-                        tc::tma_bulk_g2s(slab + (size_t)slot * NM_SLAB_BYTES, weight_image + off, bytes, full + slot);
+                        tc::tma_bulk_g2s(ring + (size_t)slot * P.slot_bytes, P.weight_image + off, bytes, full + slot);
                         off += bytes;
                     }
-                }
             }
         }
-    } else if (warp == 5) {
-        // ===================================================== MMA issuer
-        if (lane == 0) {
-            uint32_t it = 0, a_phase = 0;
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                for (int l = 0; l < plan.n_layers; ++l) {
-                    const NmLayer &L = plan.layer[l];
-                    tc::mbar_wait(a_ready, a_phase); a_phase ^= 1;   // all 128 rows of this layer's input are in smem, previous accumulator drained
-                    tc::tc_fence_after_sync();
-                    const uint32_t idesc = tc::idesc_f16_m128((uint32_t)L.N), idesc_a = tc::idesc_f16_m128(16);
-                    for (int kb = 0; kb < L.n_kblocks; ++kb, ++it) {
-                        const uint32_t slot = it % NM_SLOTS, round = it / NM_SLOTS;
-                        tc::mbar_wait(full + slot, round & 1);
-                        tc::tc_fence_after_sync();
-                        const uint32_t a0 = tc::smem_u32(A + (size_t)L.kblock_src[kb] * 16384), b0 = tc::smem_u32(slab + (size_t)slot * NM_SLAB_BYTES);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint32_t acc = (kb | k) ? 1u : 0u;
-                            tc::mma_f16_ss(tmem, tc::smem_desc_sw128(a0 + k * 32), tc::smem_desc_sw128(b0 + k * 32), idesc, acc);
-                            if (L.n_alpha) tc::mma_f16_ss(tmem + 256, tc::smem_desc_sw128(a0 + k * 32), tc::smem_desc_sw128(b0 + (uint32_t)L.N * 128u + k * 32), idesc_a, acc);
-                        }
-                        tc::mma_commit(empty + slot);              // slab slot reusable once these MMAs have read it
-                    }
-                    tc::mma_commit(acc_full);                      // accumulator of layer l complete
-                }
-            }
-        }
-    } else {
-        // ===================================================== compute warpgroup (thread == row)
-        const uint32_t row = threadIdx.x;
-        const uint32_t taddr = tmem + ((warp * 32u) << 16);
-        uint32_t acc_phase = 0;
-        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int64_t i = tile * 128 + row;
-            const bool valid = i < n_rows;
-            // ---- stage the encodings: point encoding -> blocks 4.., direction encoding -> last block (zero padded)
-            {
-                const float *e = embedded + (size_t)(valid ? i : 0) * C;
-                for (int blk = 0; blk < plan.aux_blocks + 1; ++blk) {
-                    const bool is_dir = blk == plan.aux_blocks;
-                    const int width = is_dir ? plan.input_ch_dirs : plan.input_ch, c0 = is_dir ? plan.input_ch : blk * 64;
-                    const int local0 = is_dir ? 0 : blk * 64;
-                    uint8_t *dst = A + (size_t)(4 + blk) * 16384;
-                    for (int ch = 0; ch < 8; ++ch) {
-                        float v[8];
-#pragma unroll
-                        for (int q = 0; q < 8; ++q) { int k = local0 + ch * 8 + q; v[q] = (valid && k < width) ? __ldg(e + c0 + (is_dir ? ch * 8 + q : ch * 8 + q)) : 0.f; }
-                        *reinterpret_cast<uint4 *>(dst + nm_sw128(row, ch)) = make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
-                    }
-                }
-            }
-            tc::fence_proxy_async_smem();
-            mbar_arrive(a_ready);
-            float alpha_out = 0.f;
-            for (int l = 0; l < plan.n_layers; ++l) {
-                const NmLayer &L = plan.layer[l];
-                tc::mbar_wait(acc_full, acc_phase); acc_phase ^= 1;
-                tc::tc_fence_after_sync();
-                const float *b = bias + L.bias_off;
-                if (L.n_alpha) { float a16[16]; tc::tmem_ld16(taddr + 256, a16); alpha_out = a16[0] + __ldg(b + L.N); }
-                if (L.out_blocks > 0) {
-                    for (int blk = 0; blk < L.out_blocks; ++blk) {
-                        uint8_t *dst = A + (size_t)blk * 16384;
-#pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            uint32_t r[32];
-                            tc::tmem_ld32(taddr + blk * 64 + half * 32, r);
-                            const float *bb = b + blk * 64 + half * 32;
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                float v[8];
-#pragma unroll
-                                for (int e2 = 0; e2 < 8; ++e2) { float x = __uint_as_float(r[8 * q + e2]) + __ldg(bb + 8 * q + e2); v[e2] = L.relu ? fmaxf(x, 0.f) : x; }
-                                *reinterpret_cast<uint4 *>(dst + nm_sw128(row, half * 4 + q)) = make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
-                            }
-                        }
-                    }
-                    tc::fence_proxy_async_smem();
-                    tc::tc_fence_before_sync();
-                    mbar_arrive(a_ready);
-                } else {
-                    float o16[16];
-                    tc::tmem_ld16(taddr, o16);
-                    if (valid) reinterpret_cast<float4 *>(raw)[i] = make_float4(o16[0] + __ldg(b), o16[1] + __ldg(b + 1), o16[2] + __ldg(b + 2), alpha_out);
-                    tc::tc_fence_before_sync();
-                    // the next tile's staging writes only the encoding blocks, which the (completed) last layers no longer read
-                }
-            }
-        }
+        return;
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tc::tmem_dealloc<512>(tmem);
+    // ===================================================== consumer warpgroups
+    tc::setmaxnreg_inc<232>();
+    NmCtx x;
+    x.A = A; x.ring = ring; x.full = full; x.empty = empty; x.it = 0; x.n_slots = (uint32_t)P.n_slots; x.slot_bytes = P.slot_bytes;
+    x.wg = threadIdx.x >> 7; x.t = threadIdx.x & 127; x.lane = lane; x.r0 = 64u * x.wg + tc::frag_row(x.t);
+    uint32_t n = 0;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
+        if (VER == 1) {
+            // stage my 64 rows of the fp32 encodings as fp16: point encoding -> blocks 4.., direction encoding -> last block (zero padded)
+            const int C = P.input_ch + P.input_ch_dirs;
+            for (int item = (int)x.t; item < 64 * (AUX + 1) * 8; item += 128) {
+                const int rl = item / ((AUX + 1) * 8), rem = item % ((AUX + 1) * 8), blk = rem >> 3, ch = rem & 7;
+                const uint32_t row = 64u * x.wg + (uint32_t)rl;
+                const int64_t i = tile * 128 + row;
+                const bool is_dir = blk == AUX;
+                const int width = is_dir ? P.input_ch_dirs : P.input_ch, c0 = is_dir ? P.input_ch : 0, k0 = (is_dir ? 0 : blk * 64) + ch * 8;
+                float v[8];
+#pragma unroll
+                for (int q = 0; q < 8; ++q) v[q] = (i < P.n_rows && k0 + q < width) ? __ldg(P.embedded + (size_t)i * C + c0 + k0 + q) : 0.f;
+                *reinterpret_cast<uint4 *>(A + (size_t)(4 + blk) * NM_BLOCK + nm_sw128(row, ch)) = make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
+            }
+        } else {
+            tc::mbar_wait(enc_full, n & 1);
+        }
+        float alpha[2] = {0.f, 0.f};
+        nm_layers<VER, MIP, 0>(x, P, tile, alpha);
+        // (v2 / v3) views_linears.0 was the last reader of the encoding blocks: the producer may load the next tile's
+        if (VER >= 2) { __syncwarp(); if (lane == 0) tc::mbar_arrive(enc_free); }
+    }
 }
 
-
-// =====================================================================================================================
-// v2: the epilogue is the bottleneck of v1 (one warpgroup drains 256 accumulator columns per layer while the tensor core idles).
-//   * TWO compute warpgroups per tile: WG0 owns output columns [0,N/2), WG1 owns [N/2,N) of the same 128 rows;
-//   * every layer is issued as four MMA phases  S1=(half0; aux+lo K-blocks) S2=(half1; aux+lo) S3=(half0; hi) S4=(half1; hi)
-//     where "lo"/"hi" are the A blocks written by WG0/WG1 in the previous layer: half0's accumulator completes after S3, so WG0
-//     drains it while S4 runs, and the next layer's S1/S2 start as soon as WG0 is done (they only read lo blocks);
-//   * accumulators double-buffered in TMEM by layer parity (2 x 256 columns);
-//   * weights stream as HALF slabs ([N/2 x 64] fp16, <=16 KB) in exactly that issue order through a 6-slot ring;
-//   * biases live in shared memory (LDS.128 instead of 256 LDG per thread per layer); the 1-wide alpha head is a register dot
-//     product inside the epilogue of pts_linears.7 instead of an N=16 MMA.
-constexpr int N2_SLOTS = 6;        // two rings of 3 half-slab slots: ring h feeds the issuer of output half h
-constexpr uint32_t N2_SLAB_BYTES = 128 * 128;
-constexpr int N2_THREADS = 384;   // 8 compute warps + slab producer (8) + MMA issuer half 0 (9) + encoding producer (10) + MMA issuer half 1 (11)
-constexpr int N2_MAX_LAYERS = 11;
-
-struct N2Layer {
-    int n_first, n_second;      // K-blocks issued in S1/S2 (aux + lo) and in S3/S4 (hi)
-    int src[7];                 // A block per K-block, first-phase blocks then second-phase blocks
-    int N, n_halves, relu, writes_a, alpha_dot, bias_off;
-};
-struct N2Plan { int n_layers, aux_blocks, input_ch, input_ch_dirs, bias_total, dbg; N2Layer layer[N2_MAX_LAYERS]; };  // dbg bit0: skip TMA copies, bit1: skip MMAs, bit2: skip epilogue math (attribution experiments)
-
-__global__ void __launch_bounds__(N2_THREADS, 1) nerf_mlp_tc2_kernel(N2Plan plan, const uint8_t *__restrict__ weight_image, const float *__restrict__ bias_g, const uint8_t *__restrict__ enc_image,
-                                                                      int64_t n_rows, float *__restrict__ raw) {
-    extern __shared__ uint8_t dyn_smem[];
-    uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    const int n_ablocks = 5 + plan.aux_blocks;
-    uint8_t *A = base;
-    uint8_t *slab = A + (size_t)n_ablocks * 16384;
-    float *bias = (float *)(slab + (size_t)N2_SLOTS * N2_SLAB_BYTES);          // all biases, then Wa[256], ba
-    float *alpha_part = bias + ((plan.bias_total + 3) & ~3);                    // [128] partial alpha of WG1
-    __half *bias_h = (__half *)(alpha_part + 128);                              // fp16 copy of the biases for the packed-half2 epilogue
-    uint64_t *bars = (uint64_t *)(bias_h + ((plan.bias_total + 7) & ~7));
-    uint64_t *full = bars, *empty = bars + N2_SLOTS, *a_ready = bars + 2 * N2_SLOTS /*[2]*/, *acc_ready = bars + 2 * N2_SLOTS + 2 /*[2]*/;
-    uint64_t *enc_full = bars + 2 * N2_SLOTS + 4 /*[2]: pts, dir*/, *enc_free = bars + 2 * N2_SLOTS + 6 /*[2]*/;
-    uint32_t *tmem_slot = (uint32_t *)(bars + 2 * N2_SLOTS + 8);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < N2_SLOTS; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 1); }
-        tc::mbar_init(a_ready, 4); tc::mbar_init(a_ready + 1, 4);   // one elected arrival per warp (128 same-address arrives cost ~0.3 us per hop)
-        tc::mbar_init(acc_ready, 1); tc::mbar_init(acc_ready + 1, 1);
-        for (int q = 0; q < 2; ++q) { tc::mbar_init(enc_full + q, 1); tc::mbar_init(enc_free + q, 2); }   // both issuers release the encoding blocks
-        tc::fence_mbar_init();
+template <int VER>
+static int nm_launch(const void *weight_image, const float *bias, const float *embedded, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
+    NmParams P{};
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.embedded = embedded; P.enc_image = (const uint8_t *)enc_image;
+    P.n_rows = n_rows; P.input_ch = input_ch; P.input_ch_dirs = input_ch_dirs; P.raw = raw;
+    const bool mip = input_ch > 64;
+    uint32_t max_bytes = 0;
+    for (int l = 0; l < NM_LAYERS; ++l) {
+        const NmLayer L = mip ? nm_layer<VER, true>(l) : nm_layer<VER, false>(l);
+        P.n_slabs[l] = (uint32_t)L.n_slabs;
+        for (int k = 0; k < L.n_slabs; ++k) { P.slab_bytes[l][k] = nm_slab_bytes(L.s[k]); if (P.slab_bytes[l][k] > max_bytes) max_bytes = P.slab_bytes[l][k]; }
     }
-    for (int k = threadIdx.x; k < plan.bias_total; k += N2_THREADS) { float bv = bias_g[k]; bias[k] = bv; bias_h[k] = __float2half_rn(bv); }
-    if (warp == 8) tc::tmem_alloc<512>(tmem_slot);
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
+    P.slot_bytes = (max_bytes + 1023) & ~1023u;
+    P.n_slots = VER == 1 ? 3 : 4;
+    const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * NM_BLOCK + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
+    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int64_t n_tiles = (n_rows + 127) / 128;
-    const uint32_t enc_tile_bytes = (uint32_t)(plan.aux_blocks + 1) * 16384u;
-
-    if (warp == 10) {
-        // ===================================================== encoding producer: the tile's fp16, pre-swizzled encoding blocks land straight in
-        // the A operand blocks by TMA (no staging instructions, HBM latency off the critical path): the point blocks of tile t+1 are fetched as
-        // soon as pts_linears.5 of tile t has consumed them, the direction block as soon as views_linears.0 has.
-        if (lane == 0) {
-            uint32_t n = 0;
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
-                const uint8_t *src = enc_image + (size_t)tile * enc_tile_bytes;
-                if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
-                tc::mbar_expect_tx(enc_full, (uint32_t)plan.aux_blocks * 16384u);
-                tc::tma_bulk_g2s(A + (size_t)4 * 16384, src, (uint32_t)plan.aux_blocks * 16384u, enc_full);
-                if (n > 0) tc::mbar_wait(enc_free + 1, (n - 1) & 1);
-                tc::mbar_expect_tx(enc_full + 1, 16384u);
-                tc::tma_bulk_g2s(A + (size_t)(4 + plan.aux_blocks) * 16384, src + (size_t)plan.aux_blocks * 16384, 16384u, enc_full + 1);
-            }
-        }
-    } else if (warp == 8) {
-        // ===================================================== TMA producer: per K-block, half-slab 0 -> ring 0 (issuer 0), half-slab 1 -> ring 1
-        if (lane == 0) {
-            uint32_t it[2] = {0, 0};
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                size_t off = 0;
-                for (int l = 0; l < plan.n_layers; ++l) {
-                    const N2Layer &L = plan.layer[l];
-                    const uint32_t bytes = (uint32_t)(L.N / L.n_halves) * 128u;
-                    for (int kb = 0; kb < L.n_first + L.n_second; ++kb)
-                        for (int nh = 0; nh < L.n_halves; ++nh) {
-                            const uint32_t i = it[nh]++, slot = nh * 3 + i % 3, round = i / 3;
-                            if (round > 0) tc::mbar_wait(empty + slot, (round - 1) & 1);
-                            if (plan.dbg & 1) { mbar_arrive(full + slot); }
-                            else { tc::mbar_expect_tx(full + slot, bytes); tc::tma_bulk_g2s(slab + (size_t)slot * N2_SLAB_BYTES, weight_image + off, bytes, full + slot); }
-                            off += bytes;
-                        }
-                }
-            }
-        }
-    } else if (warp == 9 || warp == 11) {
-        // ===================================================== two MMA issuers, one per output half (a single issuing thread is the bottleneck:
-        // ~60-90 cycles per tcgen05.mma issue + ~200 per slab wait/commit, scripts/micro/lat.cu). Issuer h: S(h; aux+lo) after WG0's rows are in,
-        // S(h; hi) after WG1's; then commits accumulator half h.
-        if (lane == 0) {
-            const int nh = warp == 9 ? 0 : 1;
-            uint32_t it = 0, lo_phase = 0, hi_phase = 0, lcount = 0, tcount = 0;
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-                for (int l = 0; l < plan.n_layers; ++l, ++lcount) {
-                    const N2Layer &L = plan.layer[l];
-                    if (l == 0) { tc::mbar_wait(enc_full, tcount & 1); tc::tc_fence_after_sync(); }
-                    if (l == plan.n_layers - 2) { tc::mbar_wait(enc_full + 1, tcount & 1); tc::tc_fence_after_sync(); }
-                    const uint32_t nh_w = (uint32_t)(L.N / L.n_halves);
-                    const uint32_t idesc = tc::idesc_f16_m128(nh_w);
-                    const uint32_t dbase = tmem + (lcount & 1u) * 256u + nh * nh_w;
-                    const bool active = nh < L.n_halves;
-                    for (int second = 0; second < 2; ++second) {
-                        if (second == 0) { tc::mbar_wait(a_ready, lo_phase); lo_phase ^= 1; } else { tc::mbar_wait(a_ready + 1, hi_phase); hi_phase ^= 1; }
-                        tc::tc_fence_after_sync();
-                        if (!active) continue;
-                        const int kb0 = second ? L.n_first : 0, kb1 = second ? L.n_first + L.n_second : L.n_first;
-                        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                            const uint32_t slot = nh * 3 + it % 3, round = it / 3;
-                            tc::mbar_wait(full + slot, round & 1);
-                            tc::tc_fence_after_sync();
-                            const uint32_t a0 = tc::smem_u32(A + (size_t)L.src[kb] * 16384), b0 = tc::smem_u32(slab + (size_t)slot * N2_SLAB_BYTES);
-                            if (!(plan.dbg & 2)) {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) tc::mma_f16_ss(dbase, tc::smem_desc_sw128(a0 + k * 32), tc::smem_desc_sw128(b0 + k * 32), idesc, (kb | k) ? 1u : 0u);
-                            }
-                            tc::mma_commit(empty + slot);
-                        }
-                    }
-                    if (active) tc::mma_commit(acc_ready + nh);
-                    if (l == 5) tc::mma_commit(enc_free);                          // my MMAs of pts_linears.5 were the last readers of the point-encoding blocks
-                    if (l == plan.n_layers - 2) tc::mma_commit(enc_free + 1);      // ... of the direction block
-                }
-            }
-        }
-    } else {
-        // ===================================================== two compute warpgroups (thread == row, WG == column half)
-        const uint32_t wg = warp >> 2, row = threadIdx.x & 127;
-        const uint32_t lane_base = ((warp & 3) * 32u) << 16;
-        const uint32_t r7 = row & 7u, row_off = (row >> 3) * 1024u + r7 * 128u;   // my row inside a [128x64] swizzled block; chunk c lives at ((c ^ r7) << 4)
-        uint32_t acc_phase = 0, lcount = 0;
-        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int64_t i = tile * 128 + row;
-            const bool valid = i < n_rows;
-            // (encodings arrive by TMA; this arrival only tells the MMA issuer that my warp's reads of the previous tile's accumulators are done)
-            tc::fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(a_ready + wg);
-            float alpha_acc = 0.f;
-            for (int l = 0; l < plan.n_layers; ++l, ++lcount) {
-                const N2Layer &L = plan.layer[l];
-                const int nh_w = L.N / L.n_halves;
-                const bool last = l == plan.n_layers - 1;
-                if ((int)wg < L.n_halves) {
-                    if (lane == 0) tc::mbar_wait(acc_ready + wg, acc_phase);   // one poller per warp
-                    acc_phase ^= 1;
-                    __syncwarp();
-                    tc::tc_fence_after_sync();
-                    const uint32_t taddr = tmem + lane_base + (lcount & 1u) * 256u + wg * nh_w;
-                    const float *b = bias + L.bias_off + wg * nh_w;
-                    if (!last) {
-                        // lean epilogue: acc -> fp16 (F2FP), + bias and ReLU as packed half2 ops (HADD2/HMNMX2), one LDS.128 of fp16 biases and one
-                        // STS.128 per 8 columns, swizzled chunk offsets precomputed per thread (ncu/attribution: the epilogue was 1.6 of 4.3 ms)
-                        const __half2 zero2 = __float2half2_rn(0.f);
-                        const __half *bh = bias_h + L.bias_off + wg * nh_w;
-                        for (int c2 = 0; c2 < ((plan.dbg & 4) ? 0 : nh_w / 64); ++c2) {
-                            uint32_t r64[64];
-                            tc::tmem_ld64(taddr + c2 * 64, r64);          // one TMEM round trip per 64 columns
-                            const int colb = wg * nh_w + c2 * 64;         // first column of this 64-block inside the layer output (64-aligned)
-                            uint8_t *dst = A + (size_t)(colb >> 6) * 16384 + row_off;
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) {
-                                const uint4 bq = *reinterpret_cast<const uint4 *>(bh + c2 * 64 + 8 * q);
-                                const __half2 *b2 = reinterpret_cast<const __half2 *>(&bq);
-                                __half2 h[4];
-#pragma unroll
-                                for (int e2 = 0; e2 < 4; ++e2) {
-                                    h[e2] = __hadd2(__floats2half2_rn(__uint_as_float(r64[8 * q + 2 * e2]), __uint_as_float(r64[8 * q + 2 * e2 + 1])), b2[e2]);
-                                    if (L.relu) h[e2] = __hmax2(h[e2], zero2);
-                                }
-                                if (L.alpha_dot) {   // alpha_linear on the fp16 output of pts_linears.7: partial dot over my columns
-                                    const float *wa = bias + plan.bias_total - 257 + colb + 8 * q;
-#pragma unroll
-                                    for (int e2 = 0; e2 < 4; ++e2) { float2 f = __half22float2(h[e2]); alpha_acc = fmaf(f.x, wa[2 * e2], alpha_acc); alpha_acc = fmaf(f.y, wa[2 * e2 + 1], alpha_acc); }
-                                }
-                                *reinterpret_cast<uint4 *>(dst + (((uint32_t)q ^ r7) << 4)) = *reinterpret_cast<uint4 *>(h);
-                            }
-                        }
-                        if (L.alpha_dot && wg == 1) alpha_part[row] = alpha_acc;
-                    } else {
-                        float o16[16];
-                        tc::tmem_ld16(taddr, o16);
-                        tc::named_bar_sync(1, 256);   // WG1's partial alpha is in shared memory
-                        const float alpha = alpha_acc + alpha_part[row] + bias[plan.bias_total - 1];
-                        if (valid) reinterpret_cast<float4 *>(raw)[i] = make_float4(o16[0] + b[0], o16[1] + b[1], o16[2] + b[2], alpha);
-                    }
-                } else if (last) {
-                    tc::named_bar_sync(1, 256);
-                }
-                if (!last) {
-                    tc::fence_proxy_async_smem();
-                    tc::tc_fence_before_sync();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(a_ready + wg);
-                } else {
-                    tc::tc_fence_before_sync();
-                }
-            }
-        }
-    }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 8) tc::tmem_dealloc<512>(tmem);
+    const int grid = (int)(n_tiles < sms ? n_tiles : sms);
+    auto k = mip ? nerf_mlp_wg_kernel<VER, true> : nerf_mlp_wg_kernel<VER, false>;
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k<<<grid, NM_THREADS, smem, s>>>(P);
+    return XRB_OK;
 }
 
-
-// ---- encoding tile images for v2: per 128-row tile, (aux+1) blocks of [128 x 64] fp16 in the UMMA layout (K-major, 128-byte swizzle),
+// ---- encoding tile images for v2 / v3: per 128-row tile, (aux+1) blocks of [128 x 64] fp16 in the wgmma layout (K-major, 128-byte swizzle),
 // point-encoding block(s) first, direction block last, zero padded; written by fully coalesced 16-byte stores.
 __global__ void __launch_bounds__(256) pack_embedded_tiles_kernel(const float *__restrict__ embedded, int64_t n_rows, int ic, int icd, int aux, uint8_t *__restrict__ image) {
     const int chunks_per_row = (aux + 1) * 8;
@@ -468,31 +356,7 @@ int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const floa
     if (n_rows == 0) return XRB_OK;
     XRB_REQUIRE(weight_image && bias && embedded && raw, "nerf_mlp_forward: null pointer");
     XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0, "nerf_mlp_forward: weight image / raw must be 16-byte aligned");
-    NmPlan p{};
-    p.input_ch = input_ch; p.input_ch_dirs = input_ch_dirs; p.aux_blocks = (input_ch + 63) / 64;
-    const int aux = p.aux_blocks, dir_blk = 4 + aux;
-    int nl = 0, boff = 0;
-    auto add = [&](int nk, const int *src, int N, int n_alpha, int relu, int out_blocks) {
-        NmLayer &L = p.layer[nl++]; L.n_kblocks = nk; for (int k = 0; k < nk; ++k) L.kblock_src[k] = src[k];
-        L.N = N; L.n_alpha = n_alpha; L.bias_off = boff; L.relu = relu; L.out_blocks = out_blocks; boff += N + n_alpha;
-    };
-    const int h4[4] = {0, 1, 2, 3};
-    int pts_src[2] = {4, 5};
-    add(aux, pts_src, 256, 0, 1, 4);                                        // pts_linears.0
-    for (int l = 1; l <= 4; ++l) add(4, h4, 256, 0, 1, 4);                  // pts_linears.1-4
-    { int s[6] = {0, 1, 2, 3, 4, 5}; add(4 + aux, s, 256, 0, 1, 4); }       // pts_linears.5 on cat([pts, h]) (image columns permuted to [h | pts])
-    add(4, h4, 256, 0, 1, 4); add(4, h4, 256, 0, 1, 4);                     // pts_linears.6-7
-    add(4, h4, 256, 16, 0, 4);                                              // feature_linear (+ alpha_linear rows)
-    { int s[6] = {0, 1, 2, 3, dir_blk, 0}; add(5, s, 128, 0, 1, 2); }       // views_linears.0 on cat([feature, dirs])
-    { int s[6] = {0, 1, 0, 0, 0, 0}; add(2, s, 16, 0, 0, 0); }              // rgb_linear
-    p.n_layers = nl;
-    size_t smem = 1024 + (size_t)(5 + aux) * 16384 + (size_t)NM_SLOTS * NM_SLAB_BYTES + 8 * (2 * NM_SLOTS + 2) + 16;
-    cudaFuncSetAttribute(nerf_mlp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int64_t n_tiles = (n_rows + 127) / 128;
-    int grid = (int)(n_tiles < sms ? n_tiles : sms);
-    nerf_mlp_tc_kernel<<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(p, (const uint8_t *)weight_image, bias, embedded, n_rows, raw);
-    return check_launch("nerf_mlp_forward");
+    return nm_launch<1>(weight_image, bias, embedded, nullptr, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward");
 }
 
 // v2 entry (see the kernel comment); image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v2
@@ -505,33 +369,21 @@ int xrb_nerf_mlp_forward_v2(const void *weight_image, const float *bias, const v
     if (n_rows == 0) return XRB_OK;
     XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward_v2: null pointer");
     XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0, "nerf_mlp_forward_v2: images / raw must be 16-byte aligned");
-    N2Plan p{};
-    p.input_ch = input_ch; p.input_ch_dirs = input_ch_dirs; p.aux_blocks = (input_ch + 63) / 64;
-    const int aux = p.aux_blocks, dir_blk = 4 + aux;
-    int nl = 0, boff = 0;
-    auto add = [&](int n_first, int n_second, const int *src, int N, int n_halves, int relu, int writes_a, int alpha_dot) {
-        N2Layer &L = p.layer[nl++]; L.n_first = n_first; L.n_second = n_second; for (int k = 0; k < n_first + n_second; ++k) L.src[k] = src[k];
-        L.N = N; L.n_halves = n_halves; L.relu = relu; L.writes_a = writes_a; L.alpha_dot = alpha_dot; L.bias_off = boff; boff += N;
-    };
-    { int s[7] = {4, 5, 0, 0, 0, 0, 0}; add(aux, 0, s, 256, 2, 1, 1, 0); }                               // pts_linears.0 (point-encoding blocks only)
-    const int hh[7] = {0, 1, 2, 3, 0, 0, 0};
-    for (int l = 1; l <= 4; ++l) add(2, 2, hh, 256, 2, 1, 1, 0);                                         // pts_linears.1-4
-    { int s[7]; int n = 0; for (int a = 0; a < aux; ++a) s[n++] = 4 + a; s[n++] = 0; s[n++] = 1; s[n++] = 2; s[n++] = 3; add(aux + 2, 2, s, 256, 2, 1, 1, 0); }   // pts_linears.5 on cat([pts, h])
-    add(2, 2, hh, 256, 2, 1, 1, 0);                                                                       // pts_linears.6
-    add(2, 2, hh, 256, 2, 1, 1, 1);                                                                       // pts_linears.7 (+ alpha dot in its epilogue)
-    add(2, 2, hh, 256, 2, 0, 1, 0);                                                                       // feature_linear (no ReLU)
-    { int s[7] = {dir_blk, 0, 1, 2, 3, 0, 0}; add(3, 2, s, 128, 2, 1, 1, 0); }                            // views_linears.0 on cat([feature, dirs]) -> blocks 0 (WG0), 1 (WG1)
-    { int s[7] = {0, 1, 0, 0, 0, 0, 0}; add(1, 1, s, 16, 1, 0, 0, 0); }                                   // rgb_linear: K-block 0 (lo), 1 (hi)
-    p.n_layers = nl;
-    p.bias_total = boff + 257;                                                                            // + Wa[256] + ba
-    p.dbg = getenv("XRB_NM_DBG") ? atoi(getenv("XRB_NM_DBG")) : 0;
-    size_t smem = 1024 + (size_t)(5 + aux) * 16384 + (size_t)N2_SLOTS * N2_SLAB_BYTES + sizeof(float) * (((p.bias_total + 3) & ~3) + 128) + sizeof(__half) * ((p.bias_total + 7) & ~7) + 8 * (2 * N2_SLOTS + 8) + 16;
-    cudaFuncSetAttribute(nerf_mlp_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int64_t n_tiles = (n_rows + 127) / 128;
-    int grid = (int)(n_tiles < sms ? n_tiles : sms);
-    nerf_mlp_tc2_kernel<<<grid, N2_THREADS, smem, (cudaStream_t)stream>>>(p, (const uint8_t *)weight_image, bias, (const uint8_t *)enc_image, n_rows, raw);
-    return check_launch("nerf_mlp_forward_v2");
+    return nm_launch<2>(weight_image, bias, nullptr, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward_v2");
+}
+
+// v3 entry; image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v3
+int xrb_nerf_mlp_forward_v3(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream) {
+    XRB_REQUIRE(n_rows >= 0, "nerf_mlp_forward_v3: negative size");
+    if (!((input_ch == 63 && input_ch_dirs == 27) || (input_ch == 96 && input_ch_dirs == 27))) {
+        set_error("nerf_mlp_forward_v3: implemented for NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs) with (63,27) or (96,27) input channels");
+        return XRB_E_UNSUPPORTED;
+    }
+    if (n_rows == 0) return XRB_OK;
+    XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward_v3: null pointer");
+    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0 && ((uintptr_t)bias & 15) == 0,
+                "nerf_mlp_forward_v3: images / bias / raw must be 16-byte aligned");
+    return nm_launch<3>(weight_image, bias, nullptr, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward_v3");
 }
 
 size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch) { return (size_t)((n_rows + 127) / 128) * ((input_ch + 63) / 64 + 1) * 16384; }

@@ -1,19 +1,20 @@
-// xrnerf_b200 — NerfMLP training (forward with saved activations + backward) on tcgen05 tensor cores.
+// xrnerf_b200 — NerfMLP training (forward with saved activations + backward) on wgmma tensor cores.
 //
 // The reference trains NerfMLP (/root/reference/xrnerf/models/mlps/nerf_mlp.py:70-94: 8 x 256 ReLU trunk with the skip at layer 4, alpha / feature heads, a 128-wide view
 // branch) with torch.autograd over 11 nn.Linear modules: cuBLAS fp32 GEMMs forward, two more per layer backward, every [rows, 256] activation through HBM in fp32
-// (networks/nerf.py:71-92, networks/mipnerf.py:45-74). Here every dense contraction of the training step is a hand-written UMMA kernel over TILE IMAGES:
+// (networks/nerf.py:71-92, networks/mipnerf.py:45-74). Here every dense contraction of the training step is a hand-written wgmma kernel over TILE IMAGES:
 //
-//   tile image   an activation matrix [rows x C] stored per 128-row tile as C/64 blocks of [128 x 64] fp16 in the UMMA shared-memory layout (K-major, 128-byte swizzle,
+//   tile image   an activation matrix [rows x C] stored per 128-row tile as C/64 blocks of [128 x 64] fp16 in the wgmma shared-memory layout (K-major, 128-byte swizzle,
 //                16 KB per block) — the layout the encoders already write (xrb_nerf_posenc_tiles*, xrb_mip_ipe_tiles_rays). A block moves between HBM and shared memory
 //                with ONE 1-D bulk TMA copy and is an MMA operand as it lies; read K-major it contracts over its 64 columns, read MN-major over its 128 rows.
-//   tg_kernel    Y = epilogue( sum_p A_p . op(W_p) ) per 128-row tile, accumulator in TMEM (double-buffered: tile t+1's MMAs run while tile t's epilogue drains):
+//   tg_kernel    Y = epilogue( sum_p A_p . op(W_p) ) per 128-row tile, accumulators in registers (warpgroup h: rows 64h..64h+63, up to 256 columns):
 //                  forward   A = layer input blocks, W slabs [N x 64] K-major, epilogue +bias, ReLU, fp16 -> output blocks (saved: they are the backward's operands)
 //                  input grad dX = dZ . W : A = dZ blocks, the SAME weight slabs read MN-major (no transposed copy), epilogue * [activation > 0] -> dZ of the layer below
-//   tg_dw_kernel dW += dZ^T . X over all rows: both operands read MN-major (contraction over the 128 rows of a tile), M = 128 output features per CTA (two adjacent
-//                blocks through the leading-dimension offset), accumulators stay in TMEM across the CTA's whole tile range; the bias gradient is one more MMA against a
-//                block of ones. One flush per CTA (fp32 atomics).
-// Warp roles (320 threads): warps 0-7 two epilogue warpgroups (thread == row == TMEM lane), warp 8 TMA producer (one lane), warp 9 MMA issuer (one lane).
+//   tg_dw_kernel dW += dZ^T . X over all rows: both operands read MN-major (contraction over the 128 rows of a tile), M = 128 output features per CTA (one 64-row
+//                half per warpgroup), accumulators stay in registers across the CTA's whole tile range; the bias gradient (column sums of dZ) is summed on the
+//                CUDA cores from the same staged dZ block while the MMAs run. One flush per CTA (fp32 atomics).
+// Warp roles: warps 0-7 two consumer warpgroups (issue the MMAs of their rows, run the epilogue), warp 8 TMA producer (one lane); in tg_kernel the producer's
+// warpgroup (warps 8-11) hands its registers to the consumers (setmaxnreg 40 / 232).
 // dZ is staged in fp16 with a fixed scale (2^14, applied where dL/draw enters and removed at the dW flush): tcnn-style loss scaling for 1e-6-sized NeRF gradients.
 #include "tc.cuh"
 #include "common.cuh"
@@ -24,7 +25,7 @@
 namespace xrb {
 
 constexpr uint32_t TG_BLOCK = 16384;
-constexpr int TG_MAX_A = 6, TG_MAX_SLABS = 10, TG_THREADS = 320;   // 6 A blocks: Mip-NeRF's skip layer reads 2 IPE blocks + 4 hidden blocks
+constexpr int TG_MAX_A = 6, TG_MAX_SLABS = 10, TG_THREADS = 384, TG_DW_THREADS = 288;   // 6 A blocks: Mip-NeRF's skip layer reads 2 IPE blocks + 4 hidden blocks
 constexpr uint32_t TG_RING_SLOT = 32768;   // one [256 x 64] fp16 slab
 constexpr float TG_SCALE = 16384.f;
 
@@ -45,45 +46,43 @@ struct TgP {
     long long n_rows;
 };
 
-__device__ __forceinline__ void tg_bulk_s2g(void *gdst, const void *ssrc, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(tc::smem_u32(ssrc)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tg_bulk_commit_wait_read() {
-    asm volatile("cp.async.bulk.commit_group;\n\tcp.async.bulk.wait_group.read 0;" ::: "memory");
-}
-__device__ __forceinline__ void tg_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__host__ __device__ constexpr uint32_t tg_idesc(uint32_t m, uint32_t n, uint32_t a_mn, uint32_t b_mn) { return (1u << 4) | (a_mn << 15) | (b_mn << 16) | ((n >> 3) << 17) | ((m >> 4) << 24); }
-// MN-major SWIZZLE_128B operand: 64 MN elements per 128-byte row, 8-row K groups 1024 B apart (SBO), next 64-element MN atom `lbo` bytes away (LBO)
-__device__ __forceinline__ uint64_t tg_desc_mn(uint32_t addr, uint32_t lbo) {
-    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
+enum { TB_AFULL = 0, TB_AEMPTY = 1, TB_SFULL = 2, TB_SEMPTY = 4, TB_XFULL = 6, TB_YEMPTY = 7, TB_N = 8 };
 
-enum { TB_AFULL = 0, TB_AEMPTY = 1, TB_SFULL = 2, TB_SEMPTY = 4, TB_ACCFULL = 6, TB_ACCEMPTY = 8, TB_XFULL = 10, TB_YEMPTY = 11, TB_N = 12 };
+// acc[mma_n / 2 registers at column d_col] (+)= A . B for the run-time (mma_n, d_col) pairs the host produces: forward N = 16 | 128 | 256 at column 0,
+// input gradient N = 64 at column 0 | 64 | 128 | 192 (register arrays need compile-time offsets)
+template <int TB>
+__device__ __forceinline__ void tg_mma(float *acc, int mma_n, int d_col, uint64_t ad, uint64_t bd, uint32_t sc) {
+    if (mma_n == 256) tc::wgmma<256, 0, TB>(acc, ad, bd, sc);
+    else if (mma_n == 128) tc::wgmma<128, 0, TB>(acc, ad, bd, sc);
+    else if (mma_n == 16) tc::wgmma<16, 0, TB>(acc, ad, bd, sc);
+    else if (d_col == 0) tc::wgmma<64, 0, TB>(acc, ad, bd, sc);
+    else if (d_col == 64) tc::wgmma<64, 0, TB>(acc + 32, ad, bd, sc);
+    else if (d_col == 128) tc::wgmma<64, 0, TB>(acc + 64, ad, bd, sc);
+    else tc::wgmma<64, 0, TB>(acc + 96, ad, bd, sc);
+}
 
 __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant__ TgP P) {
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
     uint8_t *A = base, *RING = A + TG_MAX_A * TG_BLOCK, *Y = RING + 2 * TG_RING_SLOT;
     uint64_t *bars = (uint64_t *)(Y + 4 * TG_BLOCK);
-    uint32_t *tmem_slot = (uint32_t *)(bars + TB_N);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int k = 0; k < TB_N; ++k) tc::mbar_init(bars + k, 1);
+        tc::mbar_init(bars + TB_AEMPTY, 8); tc::mbar_init(bars + TB_SEMPTY, 8); tc::mbar_init(bars + TB_SEMPTY + 1, 8);   // one arrival per consumer warp
+        tc::mbar_init(bars + TB_YEMPTY, 2);                                                                             // one per consumer warpgroup
         tc::fence_mbar_init();
     }
-    if (warp == 8) tc::tmem_alloc<512>(tmem_slot);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
     const long long n_tiles = (P.n_rows + 127) / 128;
     int n_ablk = 0;
     for (int s = 0; s < P.n_a; ++s) n_ablk += P.a[s].n_blk;
     const int n_xblk = P.epi == 2 ? P.out_cols / 64 : 0;
 
-    if (warp == 8) {
+    if (warp >= 8) {
         // ===================================================== producer (one lane): A blocks of the tile, then its weight slabs through the 2-slot ring, then the mask blocks
-        if (lane == 0) {
+        tc::setmaxnreg_dec<40>();   // registers go to the consumer warpgroups
+        if (warp == 8 && lane == 0) {
             uint32_t it = 0, g = 0;
             for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
                 if (it > 0) tc::mbar_wait(bars + TB_AEMPTY, (it - 1) & 1);
@@ -106,109 +105,84 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
                 }
             }
         }
-    } else if (warp == 9) {
-        // ===================================================== MMA issuer (one lane)
-        if (lane == 0) {
-            uint32_t it = 0, g = 0;
-            const uint32_t idesc = tg_idesc(128, (uint32_t)P.mma_n, 0, (uint32_t)P.b_mn);
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                const uint32_t buf = it & 1u;
-                if (it >= 2) tc::mbar_wait(bars + TB_ACCEMPTY + buf, ((it >> 1) - 1) & 1);
-                tc::mbar_wait(bars + TB_AFULL, it & 1);
-                tc::tc_fence_after_sync();
-                const uint32_t d0 = tmem + buf * 256u;
-                for (int s = 0; s < P.n_slabs; ++s, ++g) {
-                    const uint32_t slot = g & 1u, round = g >> 1;
-                    tc::mbar_wait(bars + TB_SFULL + slot, round & 1);
-                    tc::tc_fence_after_sync();
-                    const TgSlab &S = P.slab[s];
-                    const uint32_t b_base = tc::smem_u32(RING + (size_t)slot * TG_RING_SLOT);
-                    for (int j = 0; j < S.n_sub; ++j) {
-                        const uint32_t a0 = tc::smem_u32(A + (size_t)(S.a_blk0 + j) * TG_BLOCK);
-                        for (int k = 0; k < S.n_k; ++k) {
-                            const uint64_t ad = tc::smem_desc_sw128(a0 + k * 32);
-                            const uint64_t bd = P.b_mn ? tg_desc_mn(b_base + j * 8192 + k * 2048, 1024) : tc::smem_desc_sw128(b_base + k * 32);
-                            tc::mma_f16_ss(d0 + (uint32_t)S.d_col, ad, bd, idesc, (S.first && j == 0 && k == 0) ? 0u : 1u);
-                        }
-                    }
-                    tc::mma_commit(bars + TB_SEMPTY + slot);
-                }
-                tc::mma_commit(bars + TB_AEMPTY);
-                tc::mma_commit(bars + TB_ACCFULL + buf);
-            }
-        }
     } else {
-        // ===================================================== epilogue warpgroups: thread == row == TMEM lane
-        const int wg = warp >> 2, row = threadIdx.x & 127;
-        const int cols_wg = P.out_cols >= 128 ? P.out_cols / 2 : (wg == 0 ? P.out_cols : 0), col0 = P.out_cols >= 128 ? wg * cols_wg : 0;
-        uint32_t it = 0;
+        // ===================================================== two consumer warpgroups: warpgroup h issues the MMAs of rows 64h..64h+63 and runs their epilogue
+        tc::setmaxnreg_inc<232>();
+        const int wg = warp >> 2, t = threadIdx.x & 127;
+        const uint32_t r0 = 64u * (uint32_t)wg + tc::frag_row((uint32_t)t);   // my fragment rows: r0, r0 + 8
+        uint32_t it = 0, g = 0;
+        float acc[128];
         for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-            const uint32_t buf = it & 1u;
-            const long long i = tile * 128 + row;
-            tc::mbar_wait(bars + TB_ACCFULL + buf, (it >> 1) & 1);
-            tc::tc_fence_after_sync();
-            if (P.epi == 2) tc::mbar_wait(bars + TB_XFULL, it & 1);
-            else tc::named_bar_sync(1, 256);                        // the previous tile's bulk store has finished reading Y (thread 0 waited before arriving here)
-            const uint32_t taddr = tmem + buf * 256u + (((uint32_t)(row >> 5) * 32u) << 16);
-            if (P.epi == 1) {
-                if (wg == 0) {
-                    float v[16];
-                    tc::tmem_ld16(taddr, v);
-                    if (i < P.n_rows)
-                        for (int k = 0; k < P.yf_n; ++k) P.yf[(size_t)i * P.yf_stride + P.yf_col + k] = (v[k] + (P.bias ? __ldg(P.bias + k) : 0.f)) * P.yf_scale;
-                }
-            } else {
-                for (int c = 0; c < cols_wg; c += 16) {
-                    const int col = col0 + c;
-                    float v[16];
-                    tc::tmem_ld16(taddr + col, v);
-                    uint8_t *yrow = Y + (size_t)(col >> 6) * TG_BLOCK;
-                    const uint32_t ch = (uint32_t)(col & 63) >> 3;
-                    uint4 o[2];
-                    if (P.epi == 0) {
-#pragma unroll
-                        for (int k = 0; k < 16; ++k) { v[k] += P.bias ? __ldg(P.bias + col + k) : 0.f; if (P.relu) v[k] = fmaxf(v[k], 0.f); }
+            tc::mbar_wait(bars + TB_AFULL, it & 1);
+            for (int s = 0; s < P.n_slabs; ++s, ++g) {
+                const uint32_t slot = g & 1u, round = g >> 1;
+                tc::mbar_wait(bars + TB_SFULL + slot, round & 1);
+                const TgSlab &S = P.slab[s];
+                const uint32_t b_base = tc::smem_u32(RING + (size_t)slot * TG_RING_SLOT);
+                tc::wg_fence();
+                for (int j = 0; j < S.n_sub; ++j) {
+                    const uint32_t a0 = tc::smem_u32(A + (size_t)(S.a_blk0 + j) * TG_BLOCK) + (uint32_t)wg * 8192u;
+                    for (int k = 0; k < S.n_k; ++k) {
+                        const uint64_t ad = tc::desc_k128(a0 + k * 32);
+                        const uint32_t sc = (S.first && j == 0 && k == 0) ? 0u : 1u;
+                        if (P.b_mn) tg_mma<1>(acc, P.mma_n, S.d_col, ad, tc::desc_mn128(b_base + j * 8192 + k * 2048, 1024), sc);
+                        else tg_mma<0>(acc, P.mma_n, S.d_col, ad, tc::desc_k128(b_base + k * 32), sc);
                     }
-                    uint32_t *ow = reinterpret_cast<uint32_t *>(o);
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) { __half2 h = __floats2half2_rn(v[2 * k], v[2 * k + 1]); ow[k] = *reinterpret_cast<uint32_t *>(&h); }
-                    if (P.epi == 2) {
-#pragma unroll
-                        for (int q = 0; q < 2; ++q) {
-                            const uint4 xa = *reinterpret_cast<const uint4 *>(yrow + sw128_offset(row, ch + q));
-                            const uint32_t *xw = reinterpret_cast<const uint32_t *>(&xa);
-                            uint32_t *oq = reinterpret_cast<uint32_t *>(&o[q]);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                const __half2 m = __hgt2(*reinterpret_cast<const __half2 *>(&xw[k]), __float2half2_rn(0.f));
-                                const __half2 r = __hmul2(*reinterpret_cast<const __half2 *>(&oq[k]), m);
-                                oq[k] = *reinterpret_cast<const uint32_t *>(&r);
-                            }
-                        }
-                    }
-                    *reinterpret_cast<uint4 *>(yrow + sw128_offset(row, ch)) = o[0];
-                    *reinterpret_cast<uint4 *>(yrow + sw128_offset(row, ch + 1)) = o[1];
                 }
+                tc::wg_commit();
+                tc::wg_wait<0>();
+                tc::acc_fence<128>(acc);
+                __syncwarp();
+                if (lane == 0) tc::mbar_arrive(bars + TB_SEMPTY + slot);   // this warp's share of the MMAs reading the slot is complete
             }
-            // accumulator drained; output rows are in Y
-            tc::tc_fence_before_sync();
-            tc::fence_proxy_async_smem();
-            tc::named_bar_sync(2, 256);
-            if (threadIdx.x == 0) {
-                tc::mbar_arrive(bars + TB_ACCEMPTY + buf);
-                if (P.epi != 1) {
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(bars + TB_AEMPTY);
+            // ---- epilogue straight from the accumulator fragments
+            if (P.epi == 2) tc::mbar_wait(bars + TB_XFULL, it & 1);
+            else tc::named_bar_sync(1 + wg, 128);                   // the previous tile's bulk store has finished reading my half of Y (its issuer waited)
+            if (P.epi == 1) {
+#pragma unroll
+                for (int j = 0; j < 2; ++j)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int col = (int)tc::frag_col((uint32_t)t, j) + (i & 1);
+                        const long long row = tile * 128 + r0 + 8 * (i >> 1);
+                        if (col < P.yf_n && row < P.n_rows) P.yf[(size_t)row * P.yf_stride + P.yf_col + col] = (acc[4 * j + i] + (P.bias ? __ldg(P.bias + col) : 0.f)) * P.yf_scale;
+                    }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const uint32_t col = tc::frag_col((uint32_t)t, j);
+                    if ((int)col >= P.out_cols) break;
+                    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+                    if (P.epi == 0) {
+                        const float b0 = P.bias ? __ldg(P.bias + col) : 0.f, b1 = P.bias ? __ldg(P.bias + col + 1) : 0.f;
+                        v[0] += b0; v[1] += b1; v[2] += b0; v[3] += b1;
+                        if (P.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); v[2] = fmaxf(v[2], 0.f); v[3] = fmaxf(v[3], 0.f); }
+                    }
+                    uint8_t *yb = Y + (size_t)(col >> 6) * TG_BLOCK;
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        uint32_t *w = reinterpret_cast<uint32_t *>(yb + sw128_offset(r0 + 8u * (uint32_t)e, (col & 63u) >> 3) + (col & 7u) * 2u);
+                        __half2 h = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
+                        if (P.epi == 2) h = __hmul2(h, __hgt2(*reinterpret_cast<const __half2 *>(w), __float2half2_rn(0.f)));   // * [x > 0]
+                        *w = *reinterpret_cast<uint32_t *>(&h);
+                    }
+                }
+                // my rows of Y are complete: one thread of the warpgroup stores them (rows 64h.. of every block are its second / first 8 KB)
+                tc::fence_proxy_async_smem();
+                tc::named_bar_sync(1 + wg, 128);
+                if (t == 0) {
                     const int n_out_blk = (P.out_cols + 63) / 64;
-                    for (int k = 0; k < n_out_blk; ++k) tg_bulk_s2g(P.y + (size_t)tile * P.y_tile_stride + P.y_blk_off + (size_t)k * TG_BLOCK, Y + (size_t)k * TG_BLOCK, TG_BLOCK);
-                    tg_bulk_commit_wait_read();
+                    for (int k = 0; k < n_out_blk; ++k)
+                        tc::tma_bulk_s2g(P.y + (size_t)tile * P.y_tile_stride + P.y_blk_off + (size_t)k * TG_BLOCK + (size_t)wg * 8192, Y + (size_t)k * TG_BLOCK + (size_t)wg * 8192, 8192);
+                    tc::tma_bulk_commit_wait_read();
                     if (P.epi == 2) tc::mbar_arrive(bars + TB_YEMPTY);
                 }
             }
         }
-        if (threadIdx.x == 0) tg_bulk_wait_all();
+        if (t == 0) tc::tma_bulk_wait_all();
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 8) tc::tmem_dealloc<512>(tmem);
 }
 
 // ---------------------------------------------------------------------------------------------------- weight gradient
@@ -223,28 +197,22 @@ struct TgDwP {
     long long n_rows;
 };
 
-__global__ void __launch_bounds__(192, 1) tg_dw_kernel(const __grid_constant__ TgDwP P) {
+// Warps 0-7: two consumer warpgroups, warpgroup h owns accumulator rows 64h..64h+63 of the CTA's 128-row chunk (registers, across the CTA's whole
+// tile range); warp 8: producer (one lane). One flush per CTA (fp32 atomics).
+__global__ void __launch_bounds__(TG_DW_THREADS, 1) tg_dw_kernel(const __grid_constant__ TgDwP P) {
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    // two stages of (dZ chunk: 2 blocks | X: 4 blocks), then one block of ones
+    // two stages of (dZ chunk: 2 blocks | X: 4 blocks)
     constexpr uint32_t STAGE = 6 * TG_BLOCK;
-    uint8_t *ONES = base + 2 * STAGE;
-    uint64_t *bars = (uint64_t *)(ONES + TG_BLOCK);      // full[2], empty[2], done
-    uint32_t *tmem_slot = (uint32_t *)(bars + 5);
+    uint64_t *bars = (uint64_t *)(base + 2 * STAGE);      // full[2], empty[2]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) { for (int k = 0; k < 5; ++k) tc::mbar_init(bars + k, 1); tc::fence_mbar_init(); }
-    for (uint32_t k = threadIdx.x; k < TG_BLOCK / 4; k += blockDim.x) reinterpret_cast<uint32_t *>(ONES)[k] = 0x3C003C00u;   // fp16 1.0 everywhere
-    if (warp == 4) tc::tmem_alloc<512>(tmem_slot);
-    tc::fence_proxy_async_smem();
-    tc::tc_fence_before_sync();
+    if (threadIdx.x == 0) { tc::mbar_init(bars, 1); tc::mbar_init(bars + 1, 1); tc::mbar_init(bars + 2, 8); tc::mbar_init(bars + 3, 8); tc::fence_mbar_init(); }
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem = *tmem_slot;
     const long long n_tiles = (P.n_rows + 127) / 128;
     const int chunk = blockIdx.x % P.n_chunks, cta = blockIdx.x / P.n_chunks, n_cta = gridDim.x / P.n_chunks;
     const int n_xblk = P.x.n_blk;
     const int z_blk = P.transposed ? 1 : 2;                                   // blocks of dZ per stage
-    if (warp == 4) {
+    if (warp == 8) {
         if (lane == 0) {
             uint32_t it = 0;
             for (long long tile = cta; tile < n_tiles; tile += n_cta, ++it) {
@@ -259,74 +227,71 @@ __global__ void __launch_bounds__(192, 1) tg_dw_kernel(const __grid_constant__ T
                     tc::tma_bulk_g2s(S + (size_t)(2 + k) * TG_BLOCK, P.x.base + (size_t)tile * P.x.tile_stride + P.x.blk_off + (size_t)k * TG_BLOCK, TG_BLOCK, bars + st);
             }
         }
-    } else if (warp == 5) {
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (long long tile = cta; tile < n_tiles; tile += n_cta, ++it) {
-                const uint32_t st = it & 1u;
-                tc::mbar_wait(bars + st, (it >> 1) & 1);
-                tc::tc_fence_after_sync();
-                const uint32_t S = tc::smem_u32(base + (size_t)st * STAGE), ones = tc::smem_u32(ONES);
-                if (!P.transposed) {
-                    // D[128 out x (64 * n_xblk) in] += dZchunk^T . X ; bias columns at column 64 * n_xblk
-                    for (int k = 0; k < 8; ++k) {
-                        const uint32_t acc = (it | (uint32_t)k) ? 1u : 0u;
-                        const uint64_t ad = tg_desc_mn(S + k * 2048, TG_BLOCK);                     // M = 128: two dZ blocks 16 KB apart
-                        for (int xb = 0; xb < n_xblk; ++xb)
-                            tc::mma_f16_ss(tmem + (uint32_t)xb * 64u, ad, tg_desc_mn(S + (2 + xb) * TG_BLOCK + k * 2048, 1024), tg_idesc(128, 64, 1, 1), acc);
-                        if (P.db) tc::mma_f16_ss(tmem + (uint32_t)n_xblk * 64u, ad, tg_desc_mn(ones + k * 2048, 1024), tg_idesc(128, 16, 1, 1), acc);
-                    }
-                } else {
-                    // D[128 in (blocks 2*chunk, 2*chunk+1 of X) x 16 out] += X^T . dZ
-                    for (int k = 0; k < 8; ++k) {
-                        const uint32_t acc = (it | (uint32_t)k) ? 1u : 0u;
-                        tc::mma_f16_ss(tmem, tg_desc_mn(S + (2 + 2 * chunk) * TG_BLOCK + k * 2048, TG_BLOCK), tg_desc_mn(S + k * 2048, 1024), tg_idesc(128, 16, 1, 1), acc);
-                        if (chunk == 0 && P.db) tc::mma_f16_ss(tmem + 16u, tg_desc_mn(ones + k * 2048, 1024), tg_desc_mn(S + k * 2048, 1024), tg_idesc(64, 16, 1, 1), acc);   // bias: ones^T . dZ
-                    }
-                }
-                tc::mma_commit(bars + 2 + st);
-            }
-            tc::mma_commit(bars + 4);
-        }
+        return;
     }
-    // ---- flush (warps 0-3: thread == accumulator row)
-    if (warp < 4 && cta < n_tiles) {
-        tc::mbar_wait(bars + 4, 0);
-        tc::tc_fence_after_sync();
-        const int row = threadIdx.x;
-        const uint32_t taddr = tmem + (((uint32_t)(row >> 5) * 32u) << 16);
-        const float inv = 1.f / TG_SCALE;
-        if (!P.transposed) {
-            const int out = chunk * 128 + row;
-            for (int b = 0; b < n_xblk; ++b) {
-                for (int c = 0; c < 64; c += 16) {
-                    float v[16];
-                    tc::tmem_ld16(taddr + (uint32_t)b * 64u + c, v);
-                    if (out < P.N)
-                        for (int k = 0; k < 16; ++k) { const int kc = b * 64 + c + k; if (kc < P.k_cols) atomicAdd(P.dW + (size_t)out * P.K + P.k_off + kc, v[k] * inv); }
-                }
-            }
-            if (P.db) {
-                float v[16];
-                tc::tmem_ld16(taddr + (uint32_t)n_xblk * 64u, v);     // every column of the ones block gives the same sum over rows of dZ
-                if (out < P.N) atomicAdd(P.db + out, v[0] * inv);
-            }
-        } else {
-            float v[16];
-            tc::tmem_ld16(taddr, v);
-            const int kin = chunk * 128 + row;
-            if (kin < P.k_cols)
-                for (int k = 0; k < P.N; ++k) atomicAdd(P.dW + (size_t)k * P.K + P.k_off + kin, v[k] * inv);
-            if (chunk == 0 && P.db) {
-                float b[16];
-                tc::tmem_ld16(taddr + 16u, b);                     // M = 64 atom: row 0 sits in lane 0 of warp 0
-                if (row == 0) for (int k = 0; k < P.N; ++k) atomicAdd(P.db + k, b[k] * inv);
+    if (cta >= n_tiles) return;
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const bool bias_here = P.db && (!P.transposed || (chunk == 0 && wg == 0));
+    // bias gradient = column sums of dZ, on the CUDA cores from the staged dZ block: transposed (<= 16 outputs): column t % 16, rows 16 (t / 16) ..;
+    // otherwise: column t % 64 of dZ block wg (output 64 wg + t % 64 of the chunk), rows 64 (t / 64) ..
+    const uint32_t b_col = P.transposed ? (uint32_t)t & 15u : (uint32_t)t & 63u, b_rows = P.transposed ? 16u : 64u, b_row0 = ((uint32_t)t / (P.transposed ? 16u : 64u)) * b_rows;
+    float acc[4][32], bsum = 0.f;
+    uint32_t it = 0;
+    for (long long tile = cta; tile < n_tiles; tile += n_cta, ++it) {
+        const uint32_t st = it & 1u;
+        tc::mbar_wait(bars + st, (it >> 1) & 1);
+        const uint32_t S = tc::smem_u32(base + (size_t)st * STAGE);
+        tc::wg_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {   // 16 sample rows (2 x 1024 bytes) per instruction
+            const uint32_t sc = (it | (uint32_t)k) ? 1u : 0u;
+            if (!P.transposed) {
+                // D[64 out (dZ block 2 chunk + h) x 64 in per X block] += dZ^T . X
+                const uint64_t ad = tc::desc_mn128(S + (uint32_t)wg * TG_BLOCK + k * 2048, 1024);
+#pragma unroll
+                for (int xb = 0; xb < 4; ++xb)
+                    if (xb < n_xblk) tc::wgmma<64, 1, 1>(acc[xb], ad, tc::desc_mn128(S + (2 + xb) * TG_BLOCK + k * 2048, 1024), sc);
+            } else {
+                // D[64 in (X block 2 chunk + h) x 16 out] += X^T . dZ
+                tc::wgmma<16, 1, 1>(acc[0], tc::desc_mn128(S + (2 + 2 * chunk + wg) * TG_BLOCK + k * 2048, 1024), tc::desc_mn128(S + k * 2048, 1024), sc);
             }
         }
+        tc::wg_commit();
+        if (bias_here) {
+            const uint8_t *zb = base + (size_t)st * STAGE + (P.transposed ? 0 : (size_t)wg * TG_BLOCK);
+            for (uint32_t r = b_row0; r < b_row0 + b_rows; ++r) bsum += __half2float(*reinterpret_cast<const __half *>(zb + sw128_offset(r, b_col >> 3) + (b_col & 7u) * 2u));
+        }
+        tc::wg_wait<0>();
+        tc::acc_fence<32>(acc[0]); tc::acc_fence<32>(acc[1]); tc::acc_fence<32>(acc[2]); tc::acc_fence<32>(acc[3]);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(bars + 2 + st);
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tc::tmem_dealloc<512>(tmem);
+    // ---- flush from the fragments: register 4j + i holds row m0 + 8 (i / 2), column 8j + 2 (t % 4) + i % 2
+    const float inv = 1.f / TG_SCALE;
+    const int m0 = 64 * wg + (int)tc::frag_row((uint32_t)t);
+    if (!P.transposed) {
+#pragma unroll
+        for (int xb = 0; xb < 4; ++xb) {
+            if (xb >= n_xblk) break;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int out = chunk * 128 + m0 + 8 * (i >> 1), kc = xb * 64 + (int)tc::frag_col((uint32_t)t, j) + (i & 1);
+                    if (out < P.N && kc < P.k_cols) atomicAdd(P.dW + (size_t)out * P.K + P.k_off + kc, acc[xb][4 * j + i] * inv);
+                }
+        }
+        if (bias_here) { const int out = chunk * 128 + 64 * wg + (int)b_col; if (out < P.N) atomicAdd(P.db + out, bsum * inv); }
+    } else {
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int kin = chunk * 128 + m0 + 8 * (i >> 1), n = (int)tc::frag_col((uint32_t)t, j) + (i & 1);
+                if (kin < P.k_cols && n < P.N) atomicAdd(P.dW + (size_t)n * P.K + P.k_off + kin, acc[0][4 * j + i] * inv);
+            }
+        if (bias_here && (int)b_col < P.N) atomicAdd(P.db + b_col, bsum * inv);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------- small helpers
@@ -359,7 +324,7 @@ __global__ void __launch_bounds__(128) tg_pack_draw_kernel(const float4 *__restr
 }
 
 static size_t tg_smem() { return 1024 + (size_t)TG_MAX_A * TG_BLOCK + 2 * TG_RING_SLOT + 4 * TG_BLOCK + 8 * TB_N + 64; }
-static size_t tg_dw_smem() { return 1024 + 2 * 6 * (size_t)TG_BLOCK + TG_BLOCK + 8 * 5 + 64; }
+static size_t tg_dw_smem() { return 1024 + 2 * 6 * (size_t)TG_BLOCK + 8 * 4 + 64; }
 
 }  // namespace xrb
 
@@ -374,7 +339,7 @@ int xrb_nerf_tg_layer(const xrb_tg_layer *L, void *stream) {
     if (L->n_rows == 0) return XRB_OK;
     XRB_REQUIRE(L->w && L->a_base[0], "tg_layer: null pointer");
     XRB_REQUIRE(L->epi >= 0 && L->epi <= 3 && L->out_cols >= 16 && L->out_cols <= 256 && (L->out_cols % 16) == 0, "tg_layer: bad epilogue");
-    XRB_REQUIRE(L->mma_n >= 16 && L->mma_n <= 256 && (L->mma_n % 16) == 0, "tg_layer: bad MMA N");
+    XRB_REQUIRE(L->mma_n == 16 || L->mma_n == 64 || L->mma_n == 128 || L->mma_n == 256, "tg_layer: MMA N must be 16, 64, 128 or 256");
     TgP P{};
     int n_ablk = 0;
     for (int s = 0; s < L->n_a; ++s) {
@@ -389,6 +354,8 @@ int xrb_nerf_tg_layer(const xrb_tg_layer *L, void *stream) {
         XRB_REQUIRE(L->slab_n_k[s] >= 1 && L->slab_n_k[s] <= 4 && L->slab_n_sub[s] >= 1, "tg_layer: slab K-steps");
         XRB_REQUIRE(L->slab_bytes[s] <= TG_RING_SLOT && (L->slab_bytes[s] % 1024) == 0 && (L->slab_w_off[s] % 128) == 0, "tg_layer: slab size/offset");
         XRB_REQUIRE(L->slab_a_blk0[s] + L->slab_n_sub[s] <= n_ablk && L->slab_d_col[s] + L->mma_n <= 256, "tg_layer: slab refers outside the tile");
+        XRB_REQUIRE(L->mma_n == 64 ? (L->slab_d_col[s] >= 0 && L->slab_d_col[s] % 64 == 0) : L->slab_d_col[s] == 0,
+                    "tg_layer: implemented MMA shapes are N = 16 / 128 / 256 at accumulator column 0 and N = 64 at columns 0 / 64 / 128 / 192");
     }
     P.b_mn = L->b_mn; P.mma_n = L->mma_n; P.out_cols = L->out_cols; P.epi = L->epi; P.relu = L->relu; P.bias = L->bias;
     P.x = TgOp{(const uint8_t *)L->x_base, L->x_tile_stride, L->x_blk_off, L->out_cols / 64};
@@ -421,7 +388,7 @@ int xrb_nerf_tg_dw(const xrb_tg_dw *L, void *stream) {
     int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long n_tiles = (L->n_rows + 127) / 128;
     int per = sms / P.n_chunks; if (per > n_tiles) per = (int)n_tiles; if (per < 1) per = 1;
-    tg_dw_kernel<<<per * P.n_chunks, 192, smem, (cudaStream_t)stream>>>(P);
+    tg_dw_kernel<<<per * P.n_chunks, TG_DW_THREADS, smem, (cudaStream_t)stream>>>(P);
     return check_launch("nerf_tg_dw");
 }
 

@@ -11,7 +11,7 @@
 //     3. scatter dL/d(encoding) into the fp32 hash-table gradient with vector atomics (red.global.add.v2.f32).
 // Numeric contract: fp32 backward math on the fp16-rounded forward activations (oracle/tcnn_oracle.c
 // oracle_ngp_mlp_backward); the dY staging uses fp16 with a fixed 2^12 scale (tcnn uses fp16 + loss scale 128).
-// v1 runs the GEMM-shaped parts on CUDA cores; moving dX/dW onto tcgen05 tiles is the next step (DESIGN.md §6).
+// v1 runs the GEMM-shaped parts on CUDA cores; the tensor-core version is ngp_backward_tc.cu.
 #include "ngp_field.cuh"
 #include <cuda_bf16.h>
 

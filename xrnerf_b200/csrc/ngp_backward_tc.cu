@@ -1,21 +1,22 @@
 // xrnerf_b200 — backward of the Instant-NGP field (HashNerfMLP.run_mlp, /root/reference/xrnerf/models/mlps/hashnerf_mlp.py:55-79: what tcnn's
-// backward computes behind it) on tcgen05 tensor-core tiles. Replaces the CUDA-core kernel of ngp_backward.cu on the training path (that kernel
+// backward computes behind it) on wgmma tensor-core tiles. Replaces the CUDA-core kernel of ngp_backward.cu on the training path (that kernel
 // stays as impl 0: reference-grade arithmetic for every (density_hidden, color_hidden) and the comparator of the tests).
 //
-// One persistent kernel, two warpgroups per CTA, each working on its own 128-sample tile (thread r == sample r == TMEM lane r == row r of every
+// One persistent kernel, two warpgroups per CTA, each working on its own 128-sample tile (thread r == sample r == row r of every
 // shared-memory tile). Per tile:
 //   forward recompute   hash gather -> ENC tile -> density net -> CIN tile (density features ++ SH ++ 1) -> colour hidden layers; every layer
-//                       INPUT stays in shared memory as a [128 x 64] fp16 tile (K-major, 128-byte swizzle: the UMMA operand layout);
-//   backward chain      per layer ONE round of tensor-core work issued by one thread:
-//                         dX  = dZ . W            M=128 (samples), N=in, K=out : A = dZ tile (K-major), B = the FORWARD weight image read MN-major
-//                                                 (W[out][in] rows are `in`-contiguous: no transposed weight copy exists)
+//                       INPUT stays in shared memory as a [128 x 64] fp16 tile (K-major, 128-byte swizzle: the wgmma operand layout);
+//   backward chain      per layer ONE round of tensor-core work issued by the warpgroup:
+//                         dX  = dZ . W            M=64 (samples, two halves), N=in, K=out : A = dZ tile (K-major), B = the FORWARD weight image read
+//                                                 MN-major (W[out][in] rows are `in`-contiguous: no transposed weight copy exists)
 //                         dW += dZ^T . X          M=64 (out features), N=in, K=128 samples : both operands are the sample tiles read MN-major
-//                                                 (contraction over ROWS); accumulators live in TMEM for the whole persistent loop
+//                                                 (contraction over ROWS); the accumulators stay in registers for the whole persistent loop
 //                       then the epilogue masks dX with ReLU'(activation) and writes the next dZ tile (fp16, fixed 2^12 scale like the CUDA-core
 //                       kernel; tcnn uses fp16 gradients with a loss scale);
-//   scatter             dL/d(encoding) -> fp32 hash-table gradient with vector atomics (red.global.add.v2.f32), as before.
-// At the end each warpgroup adds its dW accumulators (TMEM, M=64 atoms: row m sits in lane 32*(m/16) + m%16) to the fp32 gradient with atomics.
-// TMEM: 512 columns = 2 x (64 chain accumulator + <=160 dW).  Shared memory: weight image + 2 x (ENC, H.., CIN, C.., dZ) tiles.
+//   scatter             dL/d(encoding) -> fp32 hash-table gradient with vector atomics (red.global.add.v4.f32 / v2).
+// At the end each warpgroup adds its dW accumulators to the fp32 gradient with atomics.
+// Shared memory: weight image + 2 x (ENC, H.., CIN, C.., dZ) tiles. Row-wise reads of accumulators (density outputs, dL/dcin, dL/dencoding) are
+// staged through a tile that is dead at that point (fp32 [128 x 16|32]).
 #include "tc_field.cuh"
 #include <stdio.h>
 #include <stdlib.h>
@@ -25,122 +26,136 @@ namespace xrb {
 constexpr float BT_SCALE = 4096.f;        // dZ staging scale (fp16): |dL/draw| < 16 stays finite, 1e-8 stays normal
 constexpr uint32_t BT_TILE = 16384;
 
-// instruction descriptor: D=F32, A=B=F16; majors: 0 = K-major, 1 = MN-major
-__host__ __device__ constexpr uint32_t bt_idesc(uint32_t m, uint32_t n, uint32_t a_mn, uint32_t b_mn) {
-    return (1u << 4) | (a_mn << 15) | (b_mn << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-// MN-major, SWIZZLE_128B: 64 MN elements (128 bytes) contiguous per K row, 8-row groups 1024 bytes apart (SBO); LBO (next 64-element MN atom) unused: extent <= 64
-__device__ __forceinline__ uint64_t bt_desc_mn(uint32_t smem_addr_bytes) {
-    return (uint64_t)((smem_addr_bytes >> 4) & 0x3FFFu) | ((uint64_t)(1024u >> 4) << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
 struct BtWg {
     uint8_t *tiles;      // this warpgroup's tiles, BT_TILE bytes each
     const uint8_t *W;    // forward weight image (shared by both warpgroups)
-    uint64_t *mbar; uint32_t phase;
-    uint32_t tmem_chain; // 64 columns, M=128
-    uint32_t tmem_dw;    // dW accumulators, M=64 atoms
-    uint32_t wg, row;
+    uint32_t wg, row, bar;
     bool first;          // first tile of this warpgroup: dW accumulators are overwritten, not accumulated
 };
 
-// all 128 threads: make my smem writes visible to the tensor core, meet, ONE thread issues, everybody waits for completion
-template <class F>
-__device__ __forceinline__ void bt_round(BtWg &c, F issue) {
-    tc::fence_proxy_async_smem();
-    tc::tc_fence_before_sync();
-    tc::named_bar_sync(1 + c.wg, 128);
-    if (c.row == 0) {
-        tc::tc_fence_after_sync();
-        issue();
-        tc::mma_commit(c.mbar);
-    }
-    tc::mbar_wait(c.mbar, c.phase);
-    c.phase ^= 1u;
-    tc::tc_fence_after_sync();
-}
 __device__ __forceinline__ uint8_t *bt_tile(const BtWg &c, int t) { return c.tiles + (size_t)t * BT_TILE; }
 __device__ __forceinline__ void bt_store_chunk(const BtWg &c, int t, uint32_t chunk, uint4 v) { *reinterpret_cast<uint4 *>(bt_tile(c, t) + sw128_offset(c.row, chunk)) = v; }
-__device__ __forceinline__ uint4 bt_load_chunk(const BtWg &c, int t, uint32_t chunk) { return *reinterpret_cast<const uint4 *>(bt_tile(c, t) + sw128_offset(c.row, chunk)); }
+__device__ __forceinline__ void bt_bar(const BtWg &c) { tc::named_bar_sync(c.bar, 128); }
+// my smem writes -> visible to the tensor core; every row of the warpgroup written
+__device__ __forceinline__ void bt_sync(const BtWg &c) { tc::fence_proxy_async_smem(); bt_bar(c); }
 
-// forward layer: D[128 x N] = X[128 x K] . W[N x K]^T (both K-major), as tc_layer but with an explicit A tile
+// D[64 x N] of rows 64h.. = X[rows 64h.., K] . W[N x K]^T (both K-major)
 template <int K, int N>
-__device__ __forceinline__ void bt_fwd(BtWg &c, int x_tile, uint32_t w_off) {
-    bt_round(c, [&] {
-        const uint32_t a0 = tc::smem_u32(bt_tile(c, x_tile)), b0 = tc::smem_u32(c.W + w_off);
+__device__ __forceinline__ void bt_fwd_issue(const BtWg &c, int x_tile, uint32_t w_off, int h, float *acc) {
+    const uint32_t a0 = tc::smem_u32(bt_tile(c, x_tile)) + (uint32_t)h * 8192u, b0 = tc::smem_u32(c.W + w_off);
 #pragma unroll
-        for (int k = 0; k < K / 16; ++k) tc::mma_f16_ss(c.tmem_chain, tc::smem_desc_sw128(a0 + k * 32), tc::smem_desc_sw128(b0 + k * 32), bt_idesc(128, N, 0, 0), k > 0 ? 1u : 0u);
-    });
+    for (int k = 0; k < K / 16; ++k) tc::wgmma<N>(acc, tc::desc_k128(a0 + k * 32), tc::desc_k128(b0 + k * 32), k > 0 ? 1u : 0u);
 }
-// backward round of one layer with OUT outputs and IN inputs:
-//   dX[128 x IN] = dZ[128 x OUT] . W[OUT x IN]          (chain accumulator)
-//   dW accumulators (M=64 atoms at tmem_dw + dw_col):
-//     OUT == 64:  D[m = out][n = in]  += dZ^T X   (A = dZ tile, B = X tile, N = IN)
-//     OUT == 16:  D[m = in][n = out]  += X^T dZ   (A = X tile (IN == 64), B = dZ tile, N = 16)   -> stored transposed at the flush
-template <int IN, int OUT>
-__device__ __forceinline__ void bt_bwd(BtWg &c, int dz_tile, int x_tile, uint32_t w_off, uint32_t dw_col) {
-    bt_round(c, [&] {
-        const uint32_t z0 = tc::smem_u32(bt_tile(c, dz_tile)), x0 = tc::smem_u32(bt_tile(c, x_tile)), w0 = tc::smem_u32(c.W + w_off);
-        const uint32_t acc0 = c.first ? 0u : 1u;
-        // weight gradient: contraction over the 128 sample rows, 16 rows (2 x 1024 bytes) per instruction
-        if (OUT == 64) {
+// the fp16 pair at (row r, columns col, col+1) of tile t
+__device__ __forceinline__ uint32_t *bt_word(const BtWg &c, int t, uint32_t r, uint32_t col) {
+    return reinterpret_cast<uint32_t *>(bt_tile(c, t) + sw128_offset(r, col >> 3) + (col & 7u) * 2u);
+}
+// forward hidden layer: out_tile = ReLU(fp16(X W^T)), 64 wide
+template <int K>
+__device__ __forceinline__ void bt_fwd_hidden(const BtWg &c, int x_tile, uint32_t w_off, int out_tile) {
+    bt_sync(c);
 #pragma unroll
-            for (int k = 0; k < 8; ++k) tc::mma_f16_ss(c.tmem_dw + dw_col, bt_desc_mn(z0 + k * 2048), bt_desc_mn(x0 + k * 2048), bt_idesc(64, IN, 1, 1), k > 0 ? 1u : acc0);
-        } else {
+    for (int h = 0; h < 2; ++h) {
+        float acc[32];
+        tc::wg_fence();
+        bt_fwd_issue<K, 64>(c, x_tile, w_off, h, acc);
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::acc_fence<32>(acc);
+        const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
 #pragma unroll
-            for (int k = 0; k < 8; ++k) tc::mma_f16_ss(c.tmem_dw + dw_col, bt_desc_mn(x0 + k * 2048), bt_desc_mn(z0 + k * 2048), bt_idesc(64, OUT, 1, 1), k > 0 ? 1u : acc0);
+        for (int j = 0; j < 8; ++j) {
+            const uint32_t col = tc::frag_col(c.row, j);
+            *bt_word(c, out_tile, r, col) = pack_relu_h2f(acc[4 * j], acc[4 * j + 1]);
+            *bt_word(c, out_tile, r + 8, col) = pack_relu_h2f(acc[4 * j + 2], acc[4 * j + 3]);
         }
-        // input gradient: contraction over OUT; B = forward weight image W[OUT rows][IN cols] read MN-major (N = IN contiguous, K = OUT rows)
+    }
+}
+// accumulator fragments of both halves (N columns) -> fp32 [128 x N] staging in tile `st` (swizzled: word (r, c) at r*N + (c ^ 4 (r % (N/4))))
+// -> thread r reads row r. Barriers: before (other warps' MMAs of this round may still read the tile), between, after (the tile is rewritten next).
+template <int N>
+__device__ __forceinline__ void bt_stage_rows(const BtWg &c, int st, const float *acc0, const float *acc1, float *out) {
+    float *sp = reinterpret_cast<float *>(bt_tile(c, st));
+    constexpr uint32_t SW = N / 4 - 1;
+    bt_bar(c);
 #pragma unroll
-        for (int k = 0; k < OUT / 16; ++k) tc::mma_f16_ss(c.tmem_chain, tc::smem_desc_sw128(z0 + k * 32), bt_desc_mn(w0 + k * 2048), bt_idesc(128, IN, 0, 1), k > 0 ? 1u : 0u);
-    });
+    for (int h = 0; h < 2; ++h) {
+        const float *acc = h ? acc1 : acc0;
+        const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j) {
+            const uint32_t col = tc::frag_col(c.row, j);
+            *reinterpret_cast<float2 *>(sp + r * N + (col ^ ((r & SW) << 2))) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2 *>(sp + (r + 8) * N + (col ^ (((r + 8) & SW) << 2))) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+    }
+    bt_bar(c);
+#pragma unroll
+    for (int k = 0; k < N / 4; ++k) {
+        const float4 v = *reinterpret_cast<const float4 *>(sp + c.row * N + (((uint32_t)k ^ (c.row & SW)) << 2));
+        out[4 * k] = v.x; out[4 * k + 1] = v.y; out[4 * k + 2] = v.z; out[4 * k + 3] = v.w;
+    }
+    bt_bar(c);
+}
+// forward output layer (N = 16): thread r receives the 16 fp32 outputs of row r (staged through tile `st`)
+__device__ __forceinline__ void bt_fwd_out(const BtWg &c, int x_tile, uint32_t w_off, int st, float *out) {
+    bt_sync(c);
+    float acc[2][8];
+    tc::wg_fence();
+    bt_fwd_issue<64, 16>(c, x_tile, w_off, 0, acc[0]);
+    bt_fwd_issue<64, 16>(c, x_tile, w_off, 1, acc[1]);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::acc_fence<8>(acc[0]); tc::acc_fence<8>(acc[1]);
+    bt_stage_rows<16>(c, st, acc[0], acc[1], out);
 }
 
-// epilogues ------------------------------------------------------------------------------------------------------------------------
-// forward hidden layer: accumulator (64 cols of my lane) -> ReLU -> fp16 -> tile t
-__device__ __forceinline__ void bt_epi_relu(const BtWg &c, int t) {
-    const uint32_t taddr = c.tmem_chain + (((c.row >> 5) * 32u) << 16);
+// backward round of one layer with OUT outputs and IN inputs:
+//   dX[128 x IN] = dZ[128 x OUT] . W[OUT x IN]          (two M=64 halves)
+//   dW accumulators (registers, M = 64):
+//     OUT == 64:  D[m = out][n = in]  += dZ^T X   (A = dZ tile, B = X tile, N = IN)            IN/2 registers
+//     OUT == 16:  D[m = in][n = out]  += X^T dZ   (A = X tile (IN == 64), B = dZ tile, N = 16)   8 registers, stored transposed at the flush
+// EPI 0: dZ tile := fp16(dX) * [act > 0] (act_tile);  EPI 1: thread r receives dX row r in `out` (fp32, staged through tile `st`)
+template <int IN, int OUT, int EPI>
+__device__ __forceinline__ void bt_bwd(const BtWg &c, int dz_tile, int x_tile, uint32_t w_off, float *dw, int act_tile, int st, float *out) {
+    constexpr int DWN = OUT == 64 ? IN : 16;
+    bt_sync(c);
+    const uint32_t z0 = tc::smem_u32(bt_tile(c, dz_tile)), x0 = tc::smem_u32(bt_tile(c, x_tile)), w0 = tc::smem_u32(c.W + w_off);
+    float acc[2][IN / 2];
+    tc::wg_fence();
+    // weight gradient: contraction over the 128 sample rows, 16 rows (2 x 1024 bytes) per instruction
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-        uint32_t r[32];
-        tc::tmem_ld32(taddr + half * 32, r);
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-            bt_store_chunk(c, t, half * 4 + q, make_uint4(pack_relu_h2(r[8 * q], r[8 * q + 1]), pack_relu_h2(r[8 * q + 2], r[8 * q + 3]), pack_relu_h2(r[8 * q + 4], r[8 * q + 5]),
-                                                          pack_relu_h2(r[8 * q + 6], r[8 * q + 7])));
+    for (int k = 0; k < 8; ++k) {
+        const uint32_t sc = (k > 0 || !c.first) ? 1u : 0u;
+        if (OUT == 64) tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(z0 + k * 2048, 1024), tc::desc_mn128(x0 + k * 2048, 1024), sc);
+        else tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(x0 + k * 2048, 1024), tc::desc_mn128(z0 + k * 2048, 1024), sc);
     }
-}
-// backward hidden layer: dX (64 cols) * [activation > 0] -> fp16 -> dZ tile
-__device__ __forceinline__ uint32_t bt_mask_h2(uint32_t a_bits, uint32_t b_bits, uint32_t act2) {
-    const __half2 g = __floats2half2_rn(__uint_as_float(a_bits), __uint_as_float(b_bits));
-    const __half2 m = __hgt2(*reinterpret_cast<const __half2 *>(&act2), __float2half2_rn(0.f));   // 1.0 / 0.0 per half
-    const __half2 o = __hmul2(g, m);
-    return *reinterpret_cast<const uint32_t *>(&o);
-}
-__device__ __forceinline__ void bt_epi_mask(const BtWg &c, int act_tile, int dz_tile) {
-    const uint32_t taddr = c.tmem_chain + (((c.row >> 5) * 32u) << 16);
+    // input gradient: contraction over OUT; B = forward weight image W[OUT rows][IN cols] read MN-major (N = IN contiguous, K = OUT rows)
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-        uint32_t r[32];
-        tc::tmem_ld32(taddr + half * 32, r);
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const uint4 a = bt_load_chunk(c, act_tile, half * 4 + q);
-            bt_store_chunk(c, dz_tile, half * 4 + q, make_uint4(bt_mask_h2(r[8 * q], r[8 * q + 1], a.x), bt_mask_h2(r[8 * q + 2], r[8 * q + 3], a.y), bt_mask_h2(r[8 * q + 4], r[8 * q + 5], a.z),
-                                                                bt_mask_h2(r[8 * q + 6], r[8 * q + 7], a.w)));
+        for (int k = 0; k < OUT / 16; ++k) tc::wgmma<IN, 0, 1>(acc[h], tc::desc_k128(z0 + h * 8192 + k * 32), tc::desc_mn128(w0 + k * 2048, 1024), k > 0 ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::acc_fence<DWN / 2>(dw); tc::acc_fence<IN / 2>(acc[0]); tc::acc_fence<IN / 2>(acc[1]);
+    if (EPI == 1) { bt_stage_rows<IN>(c, st, acc[0], acc[1], out); return; }
+    bt_bar(c);   // every warp's share of the dW MMA (which reads all dZ rows) has completed before dZ is overwritten
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
+#pragma unroll
+        for (int j = 0; j < IN / 8; ++j) {
+            const uint32_t col = tc::frag_col(c.row, j);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const uint32_t rr = r + 8u * (uint32_t)e;
+                const __half2 g = __floats2half2_rn(acc[h][4 * j + 2 * e], acc[h][4 * j + 2 * e + 1]);
+                const __half2 a = *reinterpret_cast<const __half2 *>(bt_word(c, act_tile, rr, col));
+                const __half2 o = __hmul2(g, __hgt2(a, __float2half2_rn(0.f)));   // 1.0 / 0.0 per half
+                *bt_word(c, dz_tile, rr, col) = *reinterpret_cast<const uint32_t *>(&o);
+            }
         }
     }
-}
-__device__ __forceinline__ void bt_read32(const BtWg &c, float *v) {
-    const uint32_t taddr = c.tmem_chain + (((c.row >> 5) * 32u) << 16);
-    uint32_t r[32];
-    tc::tmem_ld32(taddr, r);
-#pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]);
-}
-__device__ __forceinline__ void bt_read16(const BtWg &c, float *v) {
-    const uint32_t taddr = c.tmem_chain + (((c.row >> 5) * 32u) << 16);
-    tc::tmem_ld16(taddr, v);
 }
 // 16 fp32 values -> chunks 0,1 of tile t (fp16)
 __device__ __forceinline__ void bt_store16(const BtWg &c, int t, const float *v) {
@@ -148,41 +163,31 @@ __device__ __forceinline__ void bt_store16(const BtWg &c, int t, const float *v)
     bt_store_chunk(c, t, 1, make_uint4(pack_h2(v[8], v[9]), pack_h2(v[10], v[11]), pack_h2(v[12], v[13]), pack_h2(v[14], v[15])));
 }
 
-struct BtLayout {   // tile indices and dW column offsets for (DH, CH)
+// flush one M=64 dW accumulator (fragment rows m = frag_row (+8), columns n) into the fp32 gradient
+// TRANSPOSED == false: D[m = out][n = in] -> dW[out][in] (row length in_w);  true: D[m = in][n = out] -> dW[out][in]
+template <int N, bool TRANSPOSED>
+__device__ __forceinline__ void bt_flush(const BtWg &c, const float *acc, float *__restrict__ dW, int in_w) {
+    const uint32_t m0 = tc::frag_row(c.row);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t m = m0 + 8u * (uint32_t)(i >> 1), n = tc::frag_col(c.row, j) + (uint32_t)(i & 1);
+            float *dst = TRANSPOSED ? dW + (size_t)n * in_w + m : dW + (size_t)m * in_w + n;
+            atomicAdd(dst, acc[4 * j + i] * (1.f / BT_SCALE));
+        }
+}
+
+struct BtLayout {   // tile indices for (DH, CH)
     int enc, h0, cin, c0, dz, n_tiles;
-    uint32_t dw_din, dw_dhid, dw_dout, dw_cin, dw_chid, dw_cout, dw_cols;
-};
+    };
 __host__ __device__ constexpr BtLayout bt_layout(int DH, int CH) {
     BtLayout L{};
     L.enc = 0; L.h0 = 1; L.cin = 1 + DH; L.c0 = 2 + DH; L.dz = 2 + DH + CH; L.n_tiles = 3 + DH + CH;
-    uint32_t o = 0;
-    L.dw_din = o; o += 32; L.dw_dhid = o; o += 64u * (DH - 1); L.dw_dout = o; o += 16; L.dw_cin = o; o += 32; L.dw_chid = o; o += 64u * (CH - 1); L.dw_cout = o; o += 16; L.dw_cols = o;
     return L;
 }
 template <int DH, int CH>
-__host__ __device__ constexpr size_t bt_smem_bytes(uint32_t image_bytes) { return 1024 + image_bytes + 2 * (size_t)bt_layout(DH, CH).n_tiles * BT_TILE + 64; }
-
-// flush one M=64 dW atom: row m of the accumulator lives in TMEM lane 32*(m/16) + m%16, i.e. the lower 16 lanes of warp m/16
-// TRANSPOSED == false: D[m = out][n = in] -> dW[out][in] (row length IN);  true: D[m = in][n = out] -> dW[out][in]
-template <int NCOLS, bool TRANSPOSED>
-__device__ __forceinline__ void bt_flush(const BtWg &c, uint32_t dw_col, float *__restrict__ dW, int in_w) {
-    const uint32_t warp = c.row >> 5, lane = c.row & 31;
-    const uint32_t taddr = c.tmem_dw + dw_col + ((warp * 32u) << 16);
-    const uint32_t m = warp * 16 + lane;
-#pragma unroll
-    for (int n0 = 0; n0 < NCOLS; n0 += 16) {
-        float v[16];
-        tc::tmem_ld16(taddr + n0, v);    // .sync.aligned: executed by the whole warp; only lanes < 16 hold accumulator rows
-        if (lane < 16) {
-#pragma unroll
-            for (int k = 0; k < 16; ++k) {
-                const int n = n0 + k;
-                float *dst = TRANSPOSED ? dW + (size_t)n * in_w + m : dW + (size_t)m * in_w + n;
-                atomicAdd(dst, v[k] * (1.f / BT_SCALE));
-            }
-        }
-    }
-}
+__host__ __device__ constexpr size_t bt_smem_bytes(uint32_t image_bytes) { return 1024 + image_bytes + 2 * (size_t)bt_layout(DH, CH).n_tiles * BT_TILE + 16; }
 
 template <int DH, int CH, int NP>
 __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
@@ -194,29 +199,23 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     constexpr BtLayout T = bt_layout(DH, CH);
-    static_assert(64 + T.dw_cols <= 256, "TMEM budget: 2 x (64 + dW columns) <= 512");
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
     uint8_t *W = base, *tiles0 = base + image_bytes;
-    uint64_t *bars = (uint64_t *)(tiles0 + 2 * (size_t)T.n_tiles * BT_TILE);
-    uint32_t *tmem_slot = (uint32_t *)(bars + 3);
-    const uint32_t warp = threadIdx.x >> 5;
+    uint64_t *wbar = (uint64_t *)(tiles0 + 2 * (size_t)T.n_tiles * BT_TILE);
     if (threadIdx.x == 0) {
-        for (int k = 0; k < 3; ++k) tc::mbar_init(bars + k, 1);
+        tc::mbar_init(wbar, 1);
         tc::fence_mbar_init();
-        tc::mbar_expect_tx(bars + 2, image_bytes);
-        tc::tma_bulk_g2s(W, weight_image, image_bytes, bars + 2);
+        tc::mbar_expect_tx(wbar, image_bytes);
+        tc::tma_bulk_g2s(W, weight_image, image_bytes, wbar);
     }
-    if (warp == 1) tc::tmem_alloc<512>(tmem_slot);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    tc::mbar_wait(bars + 2, 0);
+    tc::mbar_wait(wbar, 0);
     BtWg c;
-    c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127;
-    c.tiles = tiles0 + (size_t)c.wg * T.n_tiles * BT_TILE; c.W = W; c.mbar = bars + c.wg; c.phase = 0;
-    const uint32_t tmem_base = *tmem_slot;
-    c.tmem_chain = tmem_base + c.wg * 64; c.tmem_dw = tmem_base + 128 + c.wg * T.dw_cols; c.first = true;
+    c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127; c.bar = 1 + c.wg;
+    c.tiles = tiles0 + (size_t)c.wg * T.n_tiles * BT_TILE; c.W = W; c.first = true;
     const WeightImageLayout L = weight_image_layout(DH, CH);
+    // weight-gradient accumulators of this warpgroup, in registers for the whole persistent loop (M = 64 fragments)
+    float dw_din[16], dw_dhid[DH > 1 ? DH - 1 : 1][32], dw_dout[8], dw_cin[16], dw_chid[CH > 1 ? CH - 1 : 1][32], dw_cout[8];
 
     const int n_tiles = (n + 127) / 128;
     for (int tile = blockIdx.x * 2 + c.wg; tile < n_tiles; tile += gridDim.x * 2) {
@@ -245,14 +244,12 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
 #pragma unroll
             for (int k = 0; k < 32; ++k) genc[k] = gr.x * (float)k;
         } else {
-        bt_fwd<32, 64>(c, T.enc, L.d_in);
-        bt_epi_relu(c, T.h0);
+        bt_fwd_hidden<32>(c, T.enc, L.d_in, T.h0);
 #pragma unroll
-        for (int h = 1; h < DH; ++h) { bt_fwd<64, 64>(c, T.h0 + h - 1, L.d_hid[h - 1]); bt_epi_relu(c, T.h0 + h); }
-        bt_fwd<64, 16>(c, T.h0 + DH - 1, L.d_out);
+        for (int h = 1; h < DH; ++h) bt_fwd_hidden<64>(c, T.h0 + h - 1, L.d_hid[h - 1], T.h0 + h);
         {
             float dout[16], sh[16], cin[32];
-            bt_read16(c, dout);
+            bt_fwd_out(c, T.h0 + DH - 1, L.d_out, T.dz, dout);    // dZ is free until the colour backward
             sh4(dx, dy, dz, sh);
 #pragma unroll
             for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];        // fp16 rounding happens in the pack below (round(round(x)) == round(x))
@@ -263,10 +260,9 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
             for (int q = 0; q < 4; ++q)
                 bt_store_chunk(c, T.cin, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
         }
-        bt_fwd<32, 64>(c, T.cin, L.c_in);
-        bt_epi_relu(c, T.c0);
+        bt_fwd_hidden<32>(c, T.cin, L.c_in, T.c0);
 #pragma unroll
-        for (int h = 1; h < CH; ++h) { bt_fwd<64, 64>(c, T.c0 + h - 1, L.c_hid[h - 1]); bt_epi_relu(c, T.c0 + h); }
+        for (int h = 1; h < CH; ++h) bt_fwd_hidden<64>(c, T.c0 + h - 1, L.c_hid[h - 1], T.c0 + h);
         // (the colour output layer itself is not needed: dL/draw is given)
         // ------------------------------------------------ backward: colour net
         {
@@ -276,33 +272,25 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
             gy[0] = gr.x * BT_SCALE; gy[1] = gr.y * BT_SCALE; gy[2] = gr.z * BT_SCALE;
             bt_store16(c, T.dz, gy);
         }
-        bt_bwd<64, 16>(c, T.dz, T.c0 + CH - 1, L.c_out, T.dw_cout);
-        bt_epi_mask(c, T.c0 + CH - 1, T.dz);
+        bt_bwd<64, 16, 0>(c, T.dz, T.c0 + CH - 1, L.c_out, dw_cout, T.c0 + CH - 1, 0, nullptr);
 #pragma unroll
-        for (int k = CH - 1; k >= 1; --k) {      // hidden layer k: input C[k-1], output C[k]
-            bt_bwd<64, 64>(c, T.dz, T.c0 + k - 1, L.c_hid[k - 1], T.dw_chid + 64u * (k - 1));
-            bt_epi_mask(c, T.c0 + k - 1, T.dz);
-        }
-        bt_bwd<32, 64>(c, T.dz, T.cin, L.c_in, T.dw_cin);
+        for (int k = CH - 1; k >= 1; --k)       // hidden layer k: input C[k-1], output C[k]
+            bt_bwd<64, 64, 0>(c, T.dz, T.c0 + k - 1, L.c_hid[k - 1], dw_chid[k - 1], T.c0 + k - 1, 0, nullptr);
         {
             float gcin[32], gy[16];
-            bt_read32(c, gcin);                     // dL/dcin (scaled)
+            bt_bwd<32, 64, 1>(c, T.dz, T.cin, L.c_in, dw_cin, 0, T.cin, gcin);   // dL/dcin (scaled); CIN is dead after this round
             gy[0] = gr.w * BT_SCALE;                // dL/d density_out = (draw.w, dcin[0..14])   (hashnerf_mlp.py:69-78: raw[3] = density_out[0], colour input = density_out[1:])
 #pragma unroll
             for (int k = 0; k < 15; ++k) gy[k + 1] = gcin[k];
             bt_store16(c, T.dz, gy);
         }
         // ------------------------------------------------ backward: density net
-        bt_bwd<64, 16>(c, T.dz, T.h0 + DH - 1, L.d_out, T.dw_dout);
-        bt_epi_mask(c, T.h0 + DH - 1, T.dz);
+        bt_bwd<64, 16, 0>(c, T.dz, T.h0 + DH - 1, L.d_out, dw_dout, T.h0 + DH - 1, 0, nullptr);
 #pragma unroll
-        for (int k = DH - 1; k >= 1; --k) {
-            bt_bwd<64, 64>(c, T.dz, T.h0 + k - 1, L.d_hid[k - 1], T.dw_dhid + 64u * (k - 1));
-            bt_epi_mask(c, T.h0 + k - 1, T.dz);
-        }
-        bt_bwd<32, 64>(c, T.dz, T.enc, L.d_in, T.dw_din);
+        for (int k = DH - 1; k >= 1; --k)
+            bt_bwd<64, 64, 0>(c, T.dz, T.h0 + k - 1, L.d_hid[k - 1], dw_dhid[k - 1], T.h0 + k - 1, 0, nullptr);
+        bt_bwd<32, 64, 1>(c, T.dz, T.enc, L.d_in, dw_din, 0, T.enc, genc);      // dL/d encoding (scaled); ENC is dead after this round
         c.first = false;
-        bt_read32(c, genc);                         // dL/d encoding (scaled)
         }
         if ((dbg & 8) && valid) {
 #pragma unroll
@@ -350,20 +338,16 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
     }
     // ---------------------------------------------------- flush the weight-gradient accumulators (once per warpgroup)
     if (!c.first) {
-        tc::tc_fence_after_sync();
         float *dd = d_dens, *dc = d_color;
-        bt_flush<32, false>(c, T.dw_din, dd, 32);
+        bt_flush<32, false>(c, dw_din, dd, 32);
 #pragma unroll
-        for (int k = 1; k < DH; ++k) bt_flush<64, false>(c, T.dw_dhid + 64u * (k - 1), dd + 64 * 32 + (k - 1) * 64 * 64, 64);
-        bt_flush<16, true>(c, T.dw_dout, dd + 64 * 32 + (DH - 1) * 64 * 64, 64);
-        bt_flush<32, false>(c, T.dw_cin, dc, 32);
+        for (int k = 1; k < DH; ++k) bt_flush<64, false>(c, dw_dhid[k - 1], dd + 64 * 32 + (k - 1) * 64 * 64, 64);
+        bt_flush<16, true>(c, dw_dout, dd + 64 * 32 + (DH - 1) * 64 * 64, 64);
+        bt_flush<32, false>(c, dw_cin, dc, 32);
 #pragma unroll
-        for (int k = 1; k < CH; ++k) bt_flush<64, false>(c, T.dw_chid + 64u * (k - 1), dc + 64 * 32 + (k - 1) * 64 * 64, 64);
-        bt_flush<16, true>(c, T.dw_cout, dc + 64 * 32 + (CH - 1) * 64 * 64, 64);
+        for (int k = 1; k < CH; ++k) bt_flush<64, false>(c, dw_chid[k - 1], dc + 64 * 32 + (k - 1) * 64 * 64, 64);
+        bt_flush<16, true>(c, dw_cout, dc + 64 * 32 + (CH - 1) * 64 * 64, 64);
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<512>(tmem_base);
 }
 
 void launch_hashgrid_backward(const HashGridDev &g, const float *x, int x_stride, int n, const void *d_enc, float scale, float *d_table, cudaStream_t s);   // ngp_backward.cu

@@ -40,8 +40,8 @@ inline int64_t hashgrid_build(const xrb_ngp_config *cfg, HashGridDev *g) {
 }
 // Cell image: a gather-friendly COPY of the first `n_packed` levels of the fp16 table. Level l stores, for every grid cell
 // (gx,gy,gz) in [0,res)^3, its 8 corner feature pairs as ONE aligned 32-byte record (corner c = bit0 x, bit1 y, bit2 z; the entry
-// tcnn's grid_index() addresses for that corner), cells in x-fastest order. A sample then reads one 256-bit word per level (one L1
-// wavefront / one sector) instead of 8 scattered 4-byte entries (up to 8 wavefronts / sectors). The master parameters keep tcnn's
+// tcnn's grid_index() addresses for that corner), cells in x-fastest order. A sample then reads one 32-byte record per level (one
+// sector) instead of 8 scattered 4-byte entries (up to 8 wavefronts / sectors). The master parameters keep tcnn's
 // layout (state_dict compatibility); the image is rebuilt from the fp16 table whenever that changes. Returns the image size in bytes
 // and fills packed_mask / cell_off.
 inline size_t cell_image_layout(HashGridDev *g, int n_packed) {
@@ -52,7 +52,7 @@ inline size_t cell_image_layout(HashGridDev *g, int n_packed) {
     }
     return rec * 32;
 }
-constexpr int MAX_PACKED_LEVELS = 13;  // image sizes for the reference grid: ..6 = 73 MB, ..7 = 190 MB (about what the 126 MB L2 still helps with), ..9 = 1.3 GB, ..12 = 25 GB;
+constexpr int MAX_PACKED_LEVELS = 13;  // image sizes for the reference grid: ..6 = 73 MB, ..7 = 190 MB, ..9 = 1.3 GB, ..12 = 25 GB;
                                        // levels past the L2 are served by HBM at ONE 32-byte sector per sample and level, where the hashed table costs ~4.5 sectors of L2
                                        // traffic (4 (y,z) rows, the x neighbour shares the sector in 7 of 8 cases). Level 13 alone would be 39 GB.
 __host__ __device__ inline int64_t mlp_num_params(int in_w, int width, int n_hidden, int out_pad) { return (int64_t)width * in_w + (int64_t)(n_hidden - 1) * width * width + (int64_t)out_pad * width; }
@@ -67,7 +67,7 @@ inline int check_cfg(const xrb_ngp_config *cfg) {
     return XRB_OK;
 }
 
-// defined in ngp_mlp.cu: launches the field (impl 0 CUDA cores / 1 tcgen05) on n rows; if n_dev != NULL the effective row
+// defined in ngp_mlp.cu: launches the field (impl 0 CUDA cores / 1 wgmma) on n rows; if n_dev != NULL the effective row
 // count is min(n, *n_dev) read on the device. table_setup validates an xrb_ngp_table and describes it for the device.
 int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g, const char *who);
 struct HashGridDev;
@@ -81,7 +81,7 @@ __device__ __forceinline__ float round_h(float x) { return __half2float(__float2
 
 __device__ __forceinline__ uint32_t grid_index(uint32_t x, uint32_t y, uint32_t z, uint32_t hashmap_size, uint32_t res) {
     // tcnn grid.h grid_index(): dense strides while they fit, else the coherent prime hash; then `% hashmap_size`.
-    // The modulo is strength-reduced without changing its value (an integer division costs 3 XU-pipe ops on sm_100):
+    // The modulo is strength-reduced without changing its value (an integer division is a multi-instruction sequence):
     //   hashed levels have hashmap_size == 2^log2_hashmap_size (the cap)          -> mask (never the generic `%`: it costs ~130 issue slots);
     //   dense levels have index <= res^3 + res^2 + res < 2 * hashmap_size          -> one conditional subtract.
     if ((uint64_t)res * res * res > hashmap_size) {   // uniform per level
@@ -92,12 +92,12 @@ __device__ __forceinline__ uint32_t grid_index(uint32_t x, uint32_t y, uint32_t 
     return index >= hashmap_size ? index - hashmap_size : index;
 }
 
-// 256-bit / 64-bit read-only gathers (SASS: LDG.E.256.CONSTANT / LDG.E.64.CONSTANT)
+// one 32-byte cell record (one sector) as two 128-bit read-only loads (sm_90 has no 256-bit load)
 struct __align__(32) Cell32 { uint32_t v[8]; };
 __device__ __forceinline__ Cell32 ldg_cell(const void *p) {
     Cell32 r;
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7]) : "l"(p));
+    const uint4 lo = __ldg(reinterpret_cast<const uint4 *>(p)), hi = __ldg(reinterpret_cast<const uint4 *>(p) + 1);
+    r.v[0] = lo.x; r.v[1] = lo.y; r.v[2] = lo.z; r.v[3] = lo.w; r.v[4] = hi.x; r.v[5] = hi.y; r.v[6] = hi.z; r.v[7] = hi.w;
     return r;
 }
 __device__ __forceinline__ __half2 as_h2(uint32_t u) { return *reinterpret_cast<__half2 *>(&u); }
@@ -109,7 +109,7 @@ __device__ __forceinline__ __half2 as_h2(uint32_t u) { return *reinterpret_cast<
 // (the generic `%` compiled to ~130 predicated-off but ISSUED instructions per level: ncu r01d source view)
 // Three gather forms, all returning the same 8 entries (the L1 processes one 128-byte line per cycle per load instruction, and a warp's
 // 32 scattered 4-byte reads touch up to 32 lines: the number of load instructions x lines is what the field kernel is bound by):
-//   packed level   : ONE 256-bit load of the cell's record from the cell image (cells: see cell_image_layout)
+//   packed level   : the cell's 32-byte record from the cell image (cells: see cell_image_layout)
 //   hashed level   : the x-prime of the hash is 1, so entries (gx, y, z) and (gx^1, y, z) are the two halves of one aligned 8-byte word:
 //                    4 x 64-bit loads fetch both x-corners when gx is even and the gx corner when it is odd; odd lanes add 4 predicated
 //                    32-bit loads for gx+1 (6 instead of 8 lines per lane on average)
@@ -212,7 +212,7 @@ __device__ __forceinline__ void sh4(float dx01, float dy01, float dz01, float *o
     out[15] = 0.59004358992664352f * x * (-x2 + 3.0f * y2);
 }
 
-// ---------------------------------------------------------------------------- UMMA shared-memory image helpers
+// ---------------------------------------------------------------------------- wgmma shared-memory image helpers
 // K-major, 128-byte swizzle: row r (one sample / one output neuron) occupies 128 bytes = 64 halfs; 8-row atoms of 1024 B.
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) {  // byte offset of 16-byte chunk `chunk16` (0..7) of `row`
     return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk16 ^ (row & 7u)) << 4);

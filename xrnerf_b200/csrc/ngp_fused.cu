@@ -1,12 +1,12 @@
 // xrnerf_b200 — the Instant-NGP inference render of a ray batch in ONE kernel launch:
-//   occupancy-grid march -> multiresolution hash encoding -> density / colour MLPs (tcgen05 tiles) -> alpha compositing
+//   occupancy-grid march -> multiresolution hash encoding -> density / colour MLPs (wgmma tiles) -> alpha compositing
 // (replaces ngp_grid_sampler.py:205-228 + hashnerf_mlp.py:55-79 + hashnerf_render.py:42-46 + the 4096-ray chunk loop of
 // hashnerf.py:54-93; no sample ever touches HBM: no coords[S,7], no raw[S,4]).
 //
 // One persistent CTA per SM, warp-specialised (768 threads):
-//   warps 0..7   two "field" warpgroups: they own the tensor core. Thread r == row r of a 128-row tile == TMEM lane r. Per tile a
+//   warps 0..7   two "field" warpgroups: they own the tensor core. Thread r == row r of a 128-row tile. Per tile a
 //                warpgroup copies the encoded rows out of a tile slot into its swizzled A tile, runs the 5 (=1+1 / 1+2+1 hidden) layers
-//                with tcgen05.mma (weights resident in shared memory, accumulators in TMEM) and posts (rgb, sigma) of every row to the
+//                with wgmma (weights resident in shared memory, accumulators in registers) and posts (rgb, sigma) of every row to the
 //                mailbox of the producer warp that submitted it. Tiles alternate between the two warpgroups.
 //   warps 8..23  "producer" warps, each autonomous over groups of 32 rays taken from a global counter:
 //                  march   : lane i marches ray i (same arithmetic as xrb_rm_rays_sampler, bit-identical sample positions), in
@@ -52,16 +52,16 @@ template <int FR_N_WG, int N_PROD, int N_SLOTS>
 struct FusedCtl {
     uint64_t full[N_SLOTS];         // count 4: one arrival per chunk (producer lane 0, or the closing field thread for a skipped quarter)
     uint64_t mail[N_PROD][2];       // count 32: the 32 field threads holding a producer's rows; a producer's chunk k uses mailbox k & 1
-    uint64_t mma[FR_N_WG], wbar;
+    uint64_t wbar;
     uint32_t rounds_done[N_SLOTS];  // slot s may be written for round r once rounds_done[s] >= r (set when its rows have been copied out)
     uint32_t owner[N_SLOTS][4];     // (producer index << 1 | mailbox parity) of each quarter
     uint32_t issued_bcast[FR_N_WG];
-    uint32_t tmem_slot, ticket, closed, done, prod_done;
+    uint32_t ticket, closed, done, prod_done;
     uint32_t morton[128];           // expand_bits7 table for the occupancy test (common.cuh morton_lut_init)
 };
 template <int FR_N_WG, int N_PROD, int N_SLOTS>
 __host__ __device__ inline size_t fused_smem_bytes(uint32_t image_bytes) {
-    return 1024 + image_bytes + (size_t)FR_N_WG * 16384 + (size_t)N_SLOTS * FR_SLOT_BYTES + (size_t)N_PROD * 1024 + sizeof(FusedCtl<FR_N_WG, N_PROD, N_SLOTS>) + 64;
+    return 1024 + image_bytes + (size_t)FR_N_WG * (16384 + TC_STAGE_BYTES) + (size_t)N_SLOTS * FR_SLOT_BYTES + (size_t)N_PROD * 1024 + sizeof(FusedCtl<FR_N_WG, N_PROD, N_SLOTS>) + 64;
 }
 
 __device__ __forceinline__ void spin_until_ge(volatile uint32_t *p, uint32_t v) {
@@ -73,7 +73,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
     extern __shared__ uint8_t dyn_smem[];
     using Ctl = FusedCtl<FR_N_WG, N_PROD, N_SLOTS>;
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *W = base, *A = W + P.image_bytes, *slots = A + (size_t)FR_N_WG * 16384, *mailbox = slots + (size_t)N_SLOTS * FR_SLOT_BYTES;
+    uint8_t *W = base, *A = W + P.image_bytes, *stage = A + (size_t)FR_N_WG * 16384, *slots = stage + (size_t)FR_N_WG * TC_STAGE_BYTES, *mailbox = slots + (size_t)N_SLOTS * FR_SLOT_BYTES;
     Ctl *ctl = (Ctl *)(mailbox + (size_t)N_PROD * 1024);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if ((P.dbg & 8) && threadIdx.x == 0) {
@@ -85,25 +85,21 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
     if (threadIdx.x == 0) {
         for (int k = 0; k < N_SLOTS; ++k) { tc::mbar_init(ctl->full + k, 4); ctl->rounds_done[k] = 0; }
         for (int k = 0; k < N_PROD; ++k) { tc::mbar_init(&ctl->mail[k][0], 32); tc::mbar_init(&ctl->mail[k][1], 32); }
-        for (int k = 0; k < FR_N_WG; ++k) { tc::mbar_init(ctl->mma + k, 1); ctl->issued_bcast[k] = 0; }
+        for (int k = 0; k < FR_N_WG; ++k) ctl->issued_bcast[k] = 0;
         tc::mbar_init(&ctl->wbar, 1);
         ctl->ticket = 0; ctl->closed = 0; ctl->done = 0; ctl->prod_done = 0;
         tc::fence_mbar_init();
         tc::mbar_expect_tx(&ctl->wbar, P.image_bytes);
         tc::tma_bulk_g2s(W, P.weight_image, P.image_bytes, &ctl->wbar);
     }
-    if (warp == 1) tc::tmem_alloc<64 * FR_N_WG>(&ctl->tmem_slot);
     morton_lut_init(ctl->morton, threadIdx.x, blockDim.x);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = ctl->tmem_slot;
 
     if (warp < 4 * FR_N_WG) {
         // ===================================================================== field warpgroups
         TcWarpgroup c;
         c.wg = warp >> 2; c.row = threadIdx.x & 127;
-        c.A = A + (size_t)c.wg * 16384; c.W = W; c.mbar = ctl->mma + c.wg; c.tmem = tmem_base + c.wg * 64; c.phase = 0;
+        c.A = A + (size_t)c.wg * 16384; c.W = W; c.stage = (float *)(stage + (size_t)c.wg * TC_STAGE_BYTES); c.bar = 1 + c.wg;
         const WeightImageLayout L = weight_image_layout(P.density_hidden, P.color_hidden);
         const bool timed = (P.dbg & 8) && c.wg == 0;
         tc::mbar_wait(&ctl->wbar, 0);
@@ -376,9 +372,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
             if (atomicAdd(&ctl->prod_done, 1u) == N_PROD - 1) *(volatile uint32_t *)&ctl->done = 1u;
         }
     }
-    tc::tc_fence_before_sync();
     __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<64 * FR_N_WG>(tmem_base);
     if ((P.dbg & 8) && threadIdx.x == 0) { unsigned long long t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); P.dbg_out[16 * blockIdx.x + 1] = t1; }
     if (threadIdx.x == 0 && !P.field_only) {   // leave the scheduler words zero for the next launch
         __threadfence();

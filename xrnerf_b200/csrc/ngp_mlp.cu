@@ -1,6 +1,6 @@
 // xrnerf_b200 — tcnn-shaped boundary (#2): hash-grid / SH encodings, fully-fused MLP, and the fused HashNerfMLP field.
 // Two implementations of the field: impl 0 = CUDA cores (reference-grade, one thread per sample, weights broadcast from
-// shared memory), impl 1 = tcgen05 tensor-core tiles (tc_field.cuh). Both follow the numeric contract in
+// shared memory), impl 1 = wgmma tensor-core tiles (tc_field.cuh). Both follow the numeric contract in
 // oracle/tcnn_oracle.c (fp16 operands, fp32 accumulate, fp16 activations).
 #include "tc_field.cuh"
 #include <stdio.h>
@@ -158,8 +158,8 @@ __global__ void __launch_bounds__(128) mlp_forward_simt_kernel(const __half *__r
 }
 
 // ---------------------------------------------------------------------------- tensor-core field (impl 1)
-// NWG warpgroups (= concurrent 128-sample tiles) per CTA share ONE resident weight image; 64 fp32 accumulator columns of TMEM each.
-// The gather is latency-bound (ncu: 69 % of the stall samples are long-scoreboard, issue 32 %, L1 65 %, L2 45 %), so the shapes trade registers per
+// NWG warpgroups (= concurrent 128-sample tiles) per CTA share ONE resident weight image; accumulators live in registers (tc_field.cuh).
+// The gather is latency-bound, so the shapes trade registers per
 // thread for warps per SM:   <2,96> / <2,128>: two CTAs per SM (16 warps);  <6,80>: one CTA per SM, 24 warps;  <8,64>: one CTA per SM, 32 warps.
 // NP: static gather plan (ngp_field.cuh plan_mode): 0 = per-level form decided at run time, >0 = levels [0,NP) from the cell image, the rest hashed.
 // dbg (developer ablation, XRB_FIELD_DBG): 1 = no gather (encoding := position bits), 2 = no MLP layers, 4 = plain per-tile loop (gather, then MLP) instead of the gather-ahead pipeline.
@@ -170,9 +170,7 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
                     float *__restrict__ out, int dbg) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
-    constexpr uint32_t TMEM_COLS = NWG <= 2 ? 128 : (NWG <= 4 ? 256 : 512);
-    TcWarpgroup c = tc_cta_setup<NWG, TMEM_COLS>(dyn_smem, weight_image, image_bytes);
-    const uint32_t tmem_base = c.tmem - c.wg * 64;
+    TcWarpgroup c = tc_cta_setup<NWG>(dyn_smem, weight_image, image_bytes);
     const WeightImageLayout L = weight_image_layout(density_hidden, color_hidden);
     const int n_tiles = (n + 127) / 128;
     if (!(dbg & 7)) {
@@ -207,7 +205,6 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
                 dx = dxn; dy = dyn; dz = dzn;
             }
         }
-        tc_cta_teardown<TMEM_COLS>(tmem_base);
         return;
     }
     for (int tile = blockIdx.x * NWG + c.wg; tile < n_tiles; tile += gridDim.x * NWG) {
@@ -238,7 +235,6 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
             if (valid) reinterpret_cast<float4 *>(out)[i] = raw;
         }
     }
-    tc_cta_teardown<TMEM_COLS>(tmem_base);
 }
 
 static int persistent_grid(const void *kernel, int block, size_t smem, int work_ctas, int min_per_sm = 1) {
@@ -378,11 +374,11 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
                                                                  dirs, dirs_stride, n, n_dev, out);
     } else {
         uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-        // kernel shape (see ngp_field_tc_kernel): XRB_TC_SHAPE = 0 <2 WG, 96 regs> (default), 1 <2,128>, 2 <6,80>, 3 <8,64>. With the gather-ahead loop the two 2-warpgroup shapes
-        // are within 3 % of each other alone (151.6 vs 148.0 us per 699 K samples; before it 178 vs 154), and the 96-register one leaves 16 K registers per SM for a kernel
-        // of another stream - the march of the next batch - to run beside it: 276 vs 264-270 M rays/s with four batches in flight, 1.207 vs 1.27 ms per training step.
+        // kernel shape (see ngp_field_tc_kernel): XRB_TC_SHAPE = 0 <2 WG, 96 regs>, 1 <2,128> (default), 2 <6,80>, 3 <8,64>. Measured with bench.py on one H100 SXM
+        // (400 W power limit, 8 batches in flight): 139.8 M rays/s and 0.402 ms per 695 K samples for the field kernel alone with <2,128>, 135.7 M / 0.414 ms with <2,96>
+        // (the register accumulators of the wgmma layers spill at 96), 3.5 ms with <6,80> and <8,64>.
         static const int env_shape = getenv("XRB_TC_SHAPE") ? atoi(getenv("XRB_TC_SHAPE")) : -1;
-        const int shape = env_shape >= 0 ? env_shape : 0;   // (impl 2 is kept as a synonym of impl 1 for callers that asked for the co-residency shape explicitly)
+        const int shape = env_shape >= 0 ? env_shape : 1;   // (impl 2 is kept as a synonym of impl 1 for callers that asked for the co-residency shape explicitly)
         static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) : 0;
         // shape 4: the producer/consumer kernel (ngp_fused.cu in FIELD-ONLY mode): gather warps and tensor-core warpgroups are different warps
         if (shape == 4 && !density_only && (((uintptr_t)out) & 15) == 0) return launch_field_ps(cfg, g, tab, image, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, s);
@@ -404,7 +400,7 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
     } while (0)
 #define XRB_LAUNCH_TC_SHAPE(D)                                                                                                                      \
     do {                                                                                                                                            \
-        if (shape == 1) XRB_LAUNCH_TC_NP(D, 2, 128); else if (shape == 2) XRB_LAUNCH_TC_NP(D, 6, 80); else if (shape == 3) XRB_LAUNCH_TC_NP(D, 8, 64); else XRB_LAUNCH_TC_NP(D, 2, 96); \
+        if (shape == 0) XRB_LAUNCH_TC_NP(D, 2, 96); else if (shape == 2) XRB_LAUNCH_TC_NP(D, 6, 80); else if (shape == 3) XRB_LAUNCH_TC_NP(D, 8, 64); else XRB_LAUNCH_TC_NP(D, 2, 128); \
     } while (0)
         if (density_only) XRB_LAUNCH_TC_SHAPE(true); else XRB_LAUNCH_TC_SHAPE(false);
 #undef XRB_LAUNCH_TC_SHAPE

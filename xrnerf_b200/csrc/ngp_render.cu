@@ -1,5 +1,5 @@
 // xrnerf_b200 — render of a ray batch through the Instant-NGP path (inference):
-//   march (count -> scan -> emit)  ->  field (hash encode + MLPs on tcgen05 tiles)  ->  composite (warp per ray)
+//   march (count -> scan -> emit)  ->  field (hash encode + MLPs on wgmma tiles)  ->  composite (warp per ray)
 // replacing ngp_grid_sampler.py:205-228 + hashnerf_mlp.py:55-79 + hashnerf_render.py:42-46 of the reference with ZERO host
 // synchronisations: the sample count stays on the device (the field kernel reads it from `counters[1]`).
 // v1: the three stages are separate launches chained on one stream (5 launches per batch, CUDA-graph capturable);

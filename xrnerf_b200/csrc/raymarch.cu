@@ -1,11 +1,11 @@
-// xrnerf_b200 — sm_100a replacements for the 10 `raymarch_cuda` ops (C ABI: xrb_rm_*, include/xrnerf_b200.h).
+// xrnerf_b200 — sm_90a replacements for the 10 `raymarch_cuda` ops (C ABI: xrb_rm_*, include/xrnerf_b200.h).
 //
 // What differs from the reference kernels (all <<<n/128,128>>> thread-per-element, extensions/ngp_raymarch/src/*.cu):
 //   * ray march: count pass + 2-level exclusive scan + emit pass => deterministic ray-order layout, no global
 //     atomics, no device sync, start-t (the only RNG use) computed once and cached in the workspace;
 //   * compositing: one WARP per ray, lanes over samples (coalesced float4 reads of raw[S,4]), transmittance by a
 //     warp product-scan instead of a serial loop per thread;
-//   * grid kernels: 128-bit vector loads/stores, grid sized to a multiple of 148 SMs with grid-stride loops,
+//   * grid kernels: 128-bit vector loads/stores, grid sized to a multiple of the SM count with grid-stride loops,
 //     bitfield + 7 max-pool levels produced by ONE kernel launch sequence without atomics, fixed-order mean.
 // HBM roofline per op (algorithmic bytes) is listed in DESIGN.md §4.
 #include "common.cuh"
@@ -504,7 +504,7 @@ using namespace xrb;
 extern "C" {
 
 int xrb_abi_version(void) { return 2; }   // 2: xrb_ngp_table (cell image), explicit profile events in xrb_ngp_render
-int xrb_built_for_sm(void) { return 100; }
+int xrb_built_for_sm(void) { return 90; }
 const char *xrb_last_error(void) { return g_err; }
 
 size_t xrb_rm_rays_sampler_workspace(int n_rays) { return march_ws_bytes(n_rays) + 2048 * sizeof(float); }

@@ -1,5 +1,6 @@
-// xrnerf_b200 — thin inline-PTX wrappers for the Blackwell (sm_100a) tensor-core path: tcgen05.mma/ld/alloc/commit,
-// mbarrier, 1-D TMA bulk copy, proxy fences. No CUTLASS dependency; encodings follow cute/arch/mma_sm100_desc.hpp.
+// xrnerf_b200 — thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: wgmma (warpgroup MMA, shared-memory operands,
+// register accumulators), mbarrier, 1-D TMA bulk copy, proxy fences. No CUTLASS dependency; descriptor encodings follow the PTX ISA
+// ("Matrix Descriptor Format" of wgmma) and cute/arch/mma_sm90_desc.hpp.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,74 +27,109 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) { while (!mbar_try_wait(bar, parity)) {} }
 
-// ---- TMA: 1-D bulk copy global -> shared, completion on an mbarrier (SASS: UBLKCP)
+// ---- TMA: 1-D bulk copy global -> shared, completion on an mbarrier
 __device__ __forceinline__ void tma_bulk_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes),
                  "r"(smem_u32(bar)) : "memory");
 }
+// 1-D bulk copy shared -> global (bulk-group completion)
+__device__ __forceinline__ void tma_bulk_s2g(void *gdst, const void *ssrc, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_bulk_commit_wait_read() { asm volatile("cp.async.bulk.commit_group;\n\tcp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void tma_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- proxy / tcgen05 fences
+// ---- fences / barriers
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory"); }
 
-// ---- TMEM allocation (one full warp executes; result lands in shared memory)
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) { asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory"); }
+// ---- register re-balancing between warpgroups (all 128 threads of a warpgroup execute it): a producer warpgroup that only issues TMA copies hands its
+// registers to the MMA warpgroups, whose accumulators live in registers
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// ---- descriptors
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B, 8-row atoms 1024 B apart (SBO), version 1 (Blackwell)
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr_bytes) {
-    return (uint64_t)((smem_addr_bytes >> 4) & 0x3FFFu) | (1ull << 16) /*LBO (ignored for swizzled K-major)*/ | ((uint64_t)(1024u >> 4) << 32) /*SBO*/ | (1ull << 46) /*version*/ |
-           (2ull << 61) /*SWIZZLE_128B*/;
+// ---- wgmma shared-memory matrix descriptors (sm_90: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46), layout type [62,64): 1 = 128-byte swizzle, 2 = 64-byte)
+__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
+    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | ((uint64_t)layout << 62);
 }
-// instruction descriptor: D=F32, A=B=F16, both K-major, M=128, N given
-__host__ __device__ constexpr uint32_t idesc_f16_m128(uint32_t n) { return (1u << 4) | (0u << 7) | (0u << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24); }
+// K-major, SWIZZLE_128B: one row = 64 fp16 (128 bytes), 8-row atoms 1024 B apart (SBO); LBO unused. A K step of 16 advances the start by 32 bytes.
+__device__ __forceinline__ uint64_t desc_k128(uint32_t addr) { return smem_desc(addr, 16, 1024, 1); }
+// K-major, SWIZZLE_64B: one row = 32 fp16 (64 bytes), 8-row atoms 512 B apart
+__device__ __forceinline__ uint64_t desc_k64(uint32_t addr) { return smem_desc(addr, 16, 512, 2); }
+// MN-major, SWIZZLE_128B: 64 MN elements contiguous per K row (128 bytes), 8-row K groups 1024 B apart (SBO), next 64-element MN atom `lbo` bytes away.
+// A K step of 16 advances the start by 2048 bytes.
+__device__ __forceinline__ uint64_t desc_mn128(uint32_t addr, uint32_t lbo) { return smem_desc(addr, lbo, 1024, 1); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; single-thread issue
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all previously issued tcgen05 async ops of this thread arrive on the mbarrier when done (implies fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t *bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory"); }
+// ---- wgmma: D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands from shared memory, fp32 accumulators in registers; issued by all 128 threads of a
+// warpgroup. TA / TB: 0 = K-major, 1 = MN-major. scale_d == 0 overwrites D.
+// Accumulator fragment (PTX ISA, wgmma .m64nNk16 D fragment): thread t of the warpgroup, w = t / 32, l = t % 32, register i:
+//   row = 16 w + l / 4 + 8 ((i % 4) / 2),   col = 8 (i / 4) + 2 (l % 4) + (i % 2)
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+    template <int TA, int TB>
+    static __device__ __forceinline__ void mma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<32> {
+    template <int TA, int TB>
+    static __device__ __forceinline__ void mma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<64> {
+    template <int TA, int TB>
+    static __device__ __forceinline__ void mma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<128> {
+    template <int TA, int TB>
+    static __device__ __forceinline__ void mma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+};
+template <> struct Wgmma<256> {
+    template <int TA, int TB>
+    static __device__ __forceinline__ void mma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+    }
+};
 
-// ---- TMEM -> registers: lane = this thread's row, N consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float *v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
+template <int N, int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) { Wgmma<N>::template mma<TA, TB>(d, ad, bd, scale_d); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points
+template <int N>
+__device__ __forceinline__ void acc_fence(float *d) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// 32 columns; the wait is inside the same asm statement so the compiler cannot hoist uses of r[] above it
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-
-// 64 columns in one instruction (one wait for the whole batch)
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x64.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, [%64];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-        : "r"(taddr) : "memory");
-}
+// row (0..63) and first column of accumulator register pair j (registers 4j, 4j+1: row r; 4j+2, 4j+3: row r + 8)
+__device__ __forceinline__ uint32_t frag_row(uint32_t t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
+__device__ __forceinline__ uint32_t frag_col(uint32_t t, uint32_t j) { return 8u * j + 2u * (t & 3u); }
 
 }}  // namespace xrb::tc

@@ -1,8 +1,8 @@
 """Fused inference path of the hierarchical NeRF (NerfNetwork.forward with N_importance > 0,
 /root/reference/xrnerf/models/networks/nerf.py:39-48 + the val pipeline's GetZvals/GetPts, datasets/pipelines/create.py:486-597) for a batch of rays:
 
-  z_vals (linspace) -> [posenc straight into fp16 UMMA tile images, positions formed in registers] -> coarse NerfMLP (tcgen05) -> composite ->
-  sample_pdf (one kernel) -> posenc tiles -> fine NerfMLP (tcgen05) -> composite
+  z_vals (linspace) -> [posenc straight into fp16 tile images (wgmma operand layout), positions formed in registers] -> coarse NerfMLP (wgmma) -> composite ->
+  sample_pdf (one kernel) -> posenc tiles -> fine NerfMLP (wgmma) -> composite
 
 No [N,S,3] `pts`, no fp32 `embedded`, no per-chunk Python loop: 7 kernel launches per ray batch of any size.
 """
@@ -51,7 +51,7 @@ class NerfRenderer:
 
 class MipNerfRenderer:
     """Fused inference path of MipNerfNetwork.forward(is_test=True) (/root/reference/xrnerf/models/networks/mipnerf.py:25-43): per level
-    [cast_rays + IPE straight into fp16 UMMA tile images] -> the SAME NerfMLP (tcgen05) -> MipNerfRender composite, with resample_along_rays
+    [cast_rays + IPE straight into fp16 tile images (wgmma operand layout)] -> the SAME NerfMLP (wgmma) -> MipNerfRender composite, with resample_along_rays
     (one kernel) between the levels: 3 launches per level + 1, no [N,S,3] means/covs, no fp32 `embedded` [N*S,123]."""
 
     def __init__(self, network, near=2.0, far=6.0, n_samples=128):

@@ -1,4 +1,4 @@
-"""Host side of the fused tcgen05 NerfMLP (csrc/nerf_mlp_tc.cu): packs the nn.Linear weights of the reference-shaped NerfMLP
+"""Host side of the fused wgmma NerfMLP (csrc/nerf_mlp_tc.cu): packs the nn.Linear weights of the reference-shaped NerfMLP
 (/root/reference/xrnerf/models/mlps/nerf_mlp.py:29-49) into the kernel's weight image — a sequence of [N x 64] fp16 slabs, K-major,
 128-byte swizzled, in the exact order the kernel's TMA producer streams them — and the fp32 bias vector."""
 import numpy as np
@@ -136,7 +136,7 @@ def _slab64(w_rows_by_32):
 
 
 def pack_nerf_mlp_v3(mlp):
-    """Image for csrc/nerf_mlp_tc3.cu: 16 KB slabs in the kernel's stream order — per layer, per K-block (AUX block first where a layer reads it):
+    """Image for the v3 entry of csrc/nerf_mlp_tc.cu: 16 KB slabs in the kernel's stream order — per layer, per K-block (the point / direction block first where a layer reads it):
     the 256-wide layers as two K-halves [256 x 32] (SWIZZLE_64B), views_linears.0 / rgb_linear as one [N x 64] slab (SWIZZLE_128B). Bias vector: fp32 per-layer biases, Wa[256], ba, padded to 8 floats, then an fp16 copy of the per-layer biases."""
     assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256
     ic, icd = mlp.input_ch, mlp.input_ch_dirs

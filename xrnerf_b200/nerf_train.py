@@ -2,8 +2,8 @@
 
 The reference trains NerfMLP (/root/reference/xrnerf/models/mlps/nerf_mlp.py:70-94) through torch.autograd over its nn.Linear modules (cuBLAS fp32 GEMMs, every
 activation through HBM in fp32; networks/nerf.py:71-92, networks/mipnerf.py:45-74). Here `NerfMlpTrainFn` is ONE autograd node for run_mlp: its forward runs the 12 dense
-layers as UMMA kernels over fp16 tile images (xrb_nerf_tg_layer) and keeps every layer input as the backward's operand; its backward runs, per layer, the input gradient
-(the same weight slabs read MN-major, ReLU mask fused) and the weight / bias gradients (xrb_nerf_tg_dw: accumulators in TMEM across all rows). Parameters stay the
+layers as wgmma kernels over fp16 tile images (xrb_nerf_tg_layer) and keeps every layer input as the backward's operand; its backward runs, per layer, the input gradient
+(the same weight slabs read MN-major, ReLU mask fused) and the weight / bias gradients (xrb_nerf_tg_dw: accumulators in registers across all rows). Parameters stay the
 nn.Linear modules of the registry class (state_dict compatibility); their fp32 weights are re-packed into fp16 slabs at every forward (the optimiser changed them).
 
 Numeric contract: fp16 operands, fp32 accumulation, fp16 activations and activation gradients (loss-scaled by 2^14), fp32 parameter gradients; tests/test_gpu_nerf_train.py

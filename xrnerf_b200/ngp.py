@@ -16,7 +16,7 @@ class NgpField(nn.Module):
     """HashNerfMLP's arithmetic (hash grid + SH + density/colour FullyFusedMLPs) as ONE kernel.
 
     Parameters keep tcnn's flat layouts and the reference's state_dict keys are produced by the registry class
-    (xrnerf_b200.api.HashNerfMLP) that owns one of these. `impl`: 1 = tcgen05 tensor-core tiles, 0 = CUDA cores.
+    (xrnerf_b200.api.HashNerfMLP) that owns one of these. `impl`: 1 = wgmma tensor-core tiles, 0 = CUDA cores.
     """
 
     def __init__(self, n_levels=16, n_features=2, log2_hashmap_size=19, base_resolution=16, per_level_scale=PER_LEVEL_SCALE, width=64,
@@ -41,7 +41,7 @@ class NgpField(nn.Module):
         self._ver = None
         self._table16 = self._dens16 = self._color16 = self._image = self._cells = self.tab = None
 
-    # ---- fp16 working copies, cell image and packed UMMA weight image, refreshed when a master parameter changed
+    # ---- fp16 working copies, cell image and packed wgmma weight image, refreshed when a master parameter changed
     def mark_dirty(self):
         """Force the next refresh(). Parameter._version does not see writes through `.data` (mmcv's EMAHook swaps parameters with
         `value.data.copy_(ema)`), so every entry point that may run after such a write calls this (val_step/test_step, load_state_dict, _apply)."""
@@ -114,7 +114,7 @@ class NgpField(nn.Module):
 
     def backward_params(self, pts, dirs, grad_raw, out=None, impl=None):
         """dL/draw [S,4] -> (d_hash, d_density, d_color) fp32, accumulated into `out` if given (zero-initialised otherwise).
-        impl 1 = tcgen05 tensor-core tiles (xrb_ngp_mlp_backward_tc), 0 = CUDA cores; default: self.impl where the tensor-core kernel is built."""
+        impl 1 = wgmma tensor-core tiles (xrb_ngp_mlp_backward_tc), 0 = CUDA cores; default: self.impl where the tensor-core kernel is built."""
         _C.require_cuda(pts, dirs, grad_raw)
         self.refresh()
         if out is None:

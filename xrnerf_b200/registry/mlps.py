@@ -20,8 +20,8 @@ class NerfMLP(BaseMLP):
     """8x256 ReLU MLP with skip at layer 4 and a 128-wide view branch; parameters are nn.Linear modules with the reference's
     names (pts_linears.i, views_linears.0, feature_linear, alpha_linear, rgb_linear) so reference checkpoints load.
 
-    Inference (no_grad) runs the whole chain in ONE persistent tcgen05 kernel (csrc/nerf_mlp_tc3.cu; fp16 operands, fp32 accumulate).
-    With autograd enabled (training) run_mlp is ONE autograd node whose forward and backward are UMMA kernels over fp16 tile images
+    Inference (no_grad) runs the whole chain in ONE persistent wgmma kernel (csrc/nerf_mlp_tc.cu; fp16 operands, fp32 accumulate).
+    With autograd enabled (training) run_mlp is ONE autograd node whose forward and backward are wgmma kernels over fp16 tile images
     (xrnerf_b200/nerf_train.py, csrc/nerf_train.cu); `fused_train = False` (or an unsupported shape) falls back to nn.Linear under autograd."""
 
     def __init__(self, skips=[4], netdepth=8, netwidth=256, output_ch=4, use_viewdirs=True, netchunk=1024 * 32, embedder=None, fused=True, **kwarg):
@@ -46,7 +46,7 @@ class NerfMLP(BaseMLP):
         del data['unflatten_shape']
         return data
 
-    # the packed tcgen05 weight image is keyed on Parameter._version, which writes through `.data` (EMAHook swap, load_state_dict, .to()) do not bump
+    # the packed wgmma weight image is keyed on Parameter._version, which writes through `.data` (EMAHook swap, load_state_dict, .to()) do not bump
     def mark_dirty(self):
         self._pack_ver = None
 
@@ -73,13 +73,13 @@ class NerfMLP(BaseMLP):
         return self._pack
 
     def batchify_run_mlp(self, x):
-        if self._fused_ok(x):   # inference: the whole 12-GEMM chain in one tcgen05 kernel, no chunking needed (activations never leave the SM)
+        if self._fused_ok(x):   # inference: the whole 12-GEMM chain in one wgmma kernel, no chunking needed (activations never leave the SM)
             from ..nerf_mlp import nerf_mlp_forward
             image, bias = self._packed()
             return nerf_mlp_forward(image, bias, x, self.input_ch, self.input_ch_dirs, version=self.kernel_version)
         if self.fused and getattr(self, 'fused_train', True) and torch.is_grad_enabled() and x.is_cuda and any(p.requires_grad for p in self.parameters()):
             from .. import nerf_train
-            if nerf_train.supported(self):   # training: every dense layer forward + backward as UMMA kernels over fp16 tile images (csrc/nerf_train.cu), one autograd node
+            if nerf_train.supported(self):   # training: every dense layer forward + backward as wgmma kernels over fp16 tile images (csrc/nerf_train.cu), one autograd node
                 return nerf_train.run_mlp_train(self, x)
         if self.chunk is None:
             return self.run_mlp(x)
@@ -139,7 +139,7 @@ class HashNerfMLP(BaseMLP):
         self.density_net = _ParamHolder(f.density_params)
         self.color_net = _ParamHolder(f.color_params)
 
-    # the fused field caches fp16 shadows, the cell image and the UMMA weight image keyed on Parameter._version, which writes through `.data` (mmcv's EMAHook,
+    # the fused field caches fp16 shadows, the cell image and the wgmma weight image keyed on Parameter._version, which writes through `.data` (mmcv's EMAHook,
     # load_state_dict's copy_, .to()) do not bump: every such entry point marks the caches dirty (ADVICE r1, medium)
     def _apply(self, fn, *a, **kw):
         self.field.mark_dirty()

@@ -201,7 +201,7 @@ class HashNerfNetwork(NerfNetwork):
         if self.phase == 'test':
             return self.test_step(data, **kwargs)
         # validation may run right after mmcv's EMAHook swapped the parameters through `.data` (Parameter._version unchanged): rebuild the fp16 shadows, the cell
-        # image and the UMMA weight image once per call instead of trusting the version key
+        # image and the wgmma weight image once per call instead of trusting the version key
         self.mlp.mark_dirty()
         data = {k: unfold_batching(v) for k, v in data.items()}
         poses, images = data['poses'], data.get('images')

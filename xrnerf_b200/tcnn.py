@@ -4,12 +4,12 @@
     tcnn.Encoding(n_input_dims, encoding_config)   -> module with .n_output_dims, .params, __call__([S,3] f32) -> [S,D] f16
     tcnn.Network(n_input_dims, n_output_dims, network_config) -> module with .params, __call__([S,Din]) -> [S,Dout] f16
 
-so `import xrnerf_b200.tcnn as tcnn` lets the reference module run on the B200 kernels. Each module owns one flat fp32
+so `import xrnerf_b200.tcnn as tcnn` lets the reference module run on these kernels. Each module owns one flat fp32
 `params` nn.Parameter (tcnn's master-parameter layout: hash table levels back to back; MLP weight matrices W[out][in]
 row-major, first/hidden/last) and a cached fp16 working copy refreshed when `params` changes.
 Both modules are trainable like tcnn's: `params` receives gradients through torch.autograd (Encoding: table gradient by scatter; Network: input and
 parameter gradients), in the dtypes tcnn's bindings use (fp16 activations and activation gradients, fp32 parameter gradients), so the reference's
-`HashNerfMLP.run_mlp` (hashnerf_mlp.py:55-79) trains through them unchanged. The fused fast path (one kernel for encodings + both MLPs, tcgen05 forward and
+`HashNerfMLP.run_mlp` (hashnerf_mlp.py:55-79) trains through them unchanged. The fused fast path (one kernel for encodings + both MLPs, wgmma forward and
 backward) lives in xrnerf_b200.ngp.NgpField; these modules are the composable building blocks behind the same parameter layouts:
 `export_params()` / `import_params()` move a flat tcnn parameter vector in and out (checkpoint compatibility, SURVEY §8f-4).
 """

@@ -2,8 +2,8 @@
 ngp_grid_sampler.py:189-266 + the mmcv OptimizerHook/Adam it runs under) without host synchronisation:
 
   [aux stream, one step ahead]  march -> compaction            (needs only rays + occupancy bitfield, not the weights)
-  [main stream]  field forward (tcgen05) -> composite forward -> Huber x5 loss+grad (one kernel) -> composite backward ->
-                 field backward (tcgen05: dX and dW as UMMA instructions) -> gradient exchange -> fused Adam (+ fp16 / UMMA-image / cell-image refresh)
+  [main stream]  field forward (wgmma) -> composite forward -> Huber x5 loss+grad (one kernel) -> composite backward ->
+                 field backward (wgmma: dX and dW as tensor-core instructions) -> gradient exchange -> fused Adam (+ fp16 / weight-image / cell-image refresh)
 
 Every per-sample kernel reads the compacted sample count on the device (`n_rows_dev`), so the work follows the batch actually marched.
 
@@ -353,7 +353,7 @@ class NgpTrainer:
         self.gflat.zero_()
         if self.bwd_impl == 1:
             _C.check(_C.lib.xrb_ngp_mlp_backward_tc(f.cfg, f.tab, _C.ptr(f._image), pp, 7, dp, 7, _C.ptr(self.draw), self.T, n_rows_dev, _C.ptr(self.g_hash), _C.ptr(self.g_dens),
-                                                    _C.ptr(self.g_color), st), 'field bwd (tcgen05)')
+                                                    _C.ptr(self.g_color), st), 'field bwd (wgmma)')
         else:
             n_rows = int(s.cnt_c[1].item())           # the CUDA-core kernel has no device-side count: one sync (comparator path only)
             _C.check(_C.lib.xrb_ngp_mlp_backward(f.cfg, f.tab, _C.ptr(f._dens16), _C.ptr(f._color16), pp, 7, dp, 7, _C.ptr(self.draw), n_rows, _C.ptr(self.g_hash), _C.ptr(self.g_dens),
