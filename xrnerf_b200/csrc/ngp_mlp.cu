@@ -162,51 +162,20 @@ __global__ void __launch_bounds__(128) mlp_forward_simt_kernel(const __half *__r
 // The gather is latency-bound, so the shapes trade registers per
 // thread for warps per SM:   <2,96> / <2,128>: two CTAs per SM (16 warps);  <6,80>: one CTA per SM, 24 warps;  <8,64>: one CTA per SM, 32 warps.
 // NP: static gather plan (ngp_field.cuh plan_mode): 0 = per-level form decided at run time, >0 = levels [0,NP) from the cell image, the rest hashed.
-// dbg (developer ablation, XRB_FIELD_DBG): 1 = no gather (encoding := position bits), 2 = no MLP layers, 4 = plain per-tile loop (gather, then MLP) instead of the gather-ahead pipeline.
-template <bool DENSITY_ONLY, int NWG, int MAXREG, int NP>
+// Per tile a warpgroup gathers the 16 levels, then runs both nets; the two to four warpgroups of an SM overlap one's gather with another's tensor-core layers.
+// ABLATE: the developer ablation (XRB_FIELD_DBG, launched only at shape <2,128>; the production instantiations do not carry it): dbg bit 0 = 1 replaces the
+// gather by position bits, bit 1 = 2 skips the MLP layers.
+template <bool DENSITY_ONLY, int NWG, int MAXREG, int NP, bool ABLATE>
 __global__ void __launch_bounds__(128 * NWG, NWG == 2 ? 2 : 1) __maxnreg__(MAXREG)
 ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image, uint32_t image_bytes, int density_hidden,
                     int color_hidden, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride, int n, const int32_t *__restrict__ n_dev,
                     float *__restrict__ out, int dbg) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
+    if (!ABLATE) dbg = 0;
     TcWarpgroup c = tc_cta_setup<NWG>(dyn_smem, weight_image, image_bytes);
     const WeightImageLayout L = weight_image_layout(density_hidden, color_hidden);
     const int n_tiles = (n + 127) / 128;
-    if (!(dbg & 7)) {
-        // gather-ahead pipeline (dbg bit 2 = 4 selects the plain loop below): tile t+1's hash gather runs inside the waits of tile t's tensor-core layers
-        const int stride = gridDim.x * NWG;
-        int tile = blockIdx.x * NWG + c.wg;
-        if (tile < n_tiles) {
-            uint32_t e[16];
-            float dx = 0.5f, dy = 0.5f, dz = 0.5f;
-            {
-                const int i = tile * 128 + c.row;
-                float x = 0.5f, y = 0.5f, z = 0.5f;
-                if (i < n) {
-                    const float *p = pts + (size_t)i * pts_stride; x = p[0]; y = p[1]; z = p[2];
-                    if (!DENSITY_ONLY) { const float *d = dirs + (size_t)i * dirs_stride; dx = d[0]; dy = d[1]; dz = d[2]; }
-                }
-                tc_gather_levels<NP, 0, 16>(table, cells, g, x, y, z, e);
-            }
-            for (; tile < n_tiles; tile += stride) {
-                const int i = tile * 128 + c.row, in = i + stride * 128;
-                const bool has_next = tile + stride < n_tiles;
-                float xn = 0.5f, yn = 0.5f, zn = 0.5f, dxn = 0.5f, dyn = 0.5f, dzn = 0.5f;
-                if (has_next && in < n) {
-                    const float *p = pts + (size_t)in * pts_stride; xn = p[0]; yn = p[1]; zn = p[2];
-                    if (!DENSITY_ONLY) { const float *d = dirs + (size_t)in * dirs_stride; dxn = d[0]; dyn = d[1]; dzn = d[2]; }
-                }
-                uint32_t en[16];
-                const float4 raw = tc_field_gather_ahead<NP, DENSITY_ONLY>(c, L, density_hidden, color_hidden, table, cells, g, e, dx, dy, dz, has_next, xn, yn, zn, en);
-                if (i < n) { if (DENSITY_ONLY) out[i] = raw.x; else reinterpret_cast<float4 *>(out)[i] = raw; }
-#pragma unroll
-                for (int k = 0; k < 16; ++k) e[k] = en[k];
-                dx = dxn; dy = dyn; dz = dzn;
-            }
-        }
-        return;
-    }
     for (int tile = blockIdx.x * NWG + c.wg; tile < n_tiles; tile += gridDim.x * NWG) {
         const int i = tile * 128 + c.row;
         const bool valid = i < n;
@@ -216,22 +185,24 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
             if (!DENSITY_ONLY) { const float *d = dirs + (size_t)i * dirs_stride; dx = d[0]; dy = d[1]; dz = d[2]; }
         }
         float dout[16];
-        if (dbg & 1) {
+        if (dbg & 2) {   // gather only (or neither)
+            float acc = x;
+            if (!(dbg & 1)) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) a_store_chunk(c, q, make_uint4(pack_h2(x, y), pack_h2(z, x), pack_h2(y, z), pack_h2(x, z)));
-            if (dbg & 2) { for (int k = 0; k < 16; ++k) dout[k] = x; } else tc_density_from_a(c, L, density_hidden, dout);
-        } else if (dbg & 2) {
-            float acc = 0.f;
-#pragma unroll
-            for (int l = 0; l < 16; ++l) { float2 f = hash_level(table, cells, g, l, x, y, z, plan_mode<NP>(l)); acc += f.x + f.y; }
+                for (int l = 0; l < 16; ++l) { const float2 f = hash_level(table, cells, g, l, x, y, z, plan_mode<NP>(l)); acc += f.x + f.y; }
+            }
             for (int k = 0; k < 16; ++k) dout[k] = acc;
         } else {
-            tc_density<NP>(c, L, density_hidden, table, cells, g, x, y, z, dout);
+            uint32_t e[16];
+            if (dbg & 1) { for (int l = 0; l < 16; ++l) e[l] = pack_h2(x + l, y - l); } else tc_gather_levels<NP, 0, 16>(table, cells, g, x, y, z, e);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) a_store_chunk(c, q, make_uint4(e[4 * q], e[4 * q + 1], e[4 * q + 2], e[4 * q + 3]));
+            tc_density_from_a(c, L, density_hidden, dout);
         }
         if (DENSITY_ONLY) {
             if (valid) out[i] = dout[0];
         } else {
-            float4 raw = (dbg & 2) ? make_float4(dout[0], dout[1], dout[2], dout[3]) : tc_color_from_density(c, L, color_hidden, dout, dx, dy, dz);
+            const float4 raw = (dbg & 2) ? make_float4(dout[0], dout[1], dout[2], dout[3]) : tc_color_from_density(c, L, color_hidden, dout, dx, dy, dz);
             if (valid) reinterpret_cast<float4 *>(out)[i] = raw;
         }
     }
@@ -374,12 +345,12 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
                                                                  dirs, dirs_stride, n, n_dev, out);
     } else {
         uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-        // kernel shape (see ngp_field_tc_kernel): XRB_TC_SHAPE = 0 <2 WG, 96 regs>, 1 <2,128> (default), 2 <6,80>, 3 <8,64>. Measured with bench.py on one H100 SXM
-        // (400 W power limit, 8 batches in flight): 139.8 M rays/s and 0.402 ms per 695 K samples for the field kernel alone with <2,128>, 135.7 M / 0.414 ms with <2,96>
-        // (the register accumulators of the wgmma layers spill at 96), 3.5 ms with <6,80> and <8,64>.
+        // kernel shape (see ngp_field_tc_kernel): XRB_TC_SHAPE = 0 <2 WG, 96 regs>, 1 <2,128> (default), 2 <6,80>, 3 <8,64>, 4 the producer/consumer kernel. Measured
+        // with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us with <2,128>
+        // (ptxas: 128 registers, 0 spill bytes), 296 us with <2,96>, 343 us with <6,80>, 646 us with <8,64> (all three spill), 277 us with shape 4.
         static const int env_shape = getenv("XRB_TC_SHAPE") ? atoi(getenv("XRB_TC_SHAPE")) : -1;
-        const int shape = env_shape >= 0 ? env_shape : 1;   // (impl 2 is kept as a synonym of impl 1 for callers that asked for the co-residency shape explicitly)
-        static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) : 0;
+        static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) & 3 : 0;
+        const int shape = (env_shape >= 0 && !dbg) ? env_shape : 1;   // the ablation runs at <2,128> only (impl 2 is a synonym of impl 1)
         // shape 4: the producer/consumer kernel (ngp_fused.cu in FIELD-ONLY mode): gather warps and tensor-core warpgroups are different warps
         if (shape == 4 && !density_only && (((uintptr_t)out) & 15) == 0) return launch_field_ps(cfg, g, tab, image, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, s);
         // static gather plan: the kernel is specialised for "levels [0,NP) packed, all others hashed" (NP = 6, 7); anything else takes the run-time form
@@ -388,7 +359,7 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
         int n_tiles = (n + 127) / 128;
 #define XRB_LAUNCH_TC(D, NWG, R, NP)                                                                                                                \
     do {                                                                                                                                            \
-        auto k = ngp_field_tc_kernel<D, NWG, R, NP>;                                                                                                \
+        auto k = dbg ? ngp_field_tc_kernel<D, 2, 128, NP, true> : ngp_field_tc_kernel<D, NWG, R, NP, false>;                                        \
         const size_t smem = tc_cta_smem_bytes<NWG>(image_bytes);                                                                                    \
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                                                            \
         int grid = persistent_grid((const void *)k, 128 * NWG, smem, (n_tiles + NWG - 1) / NWG, NWG == 2 ? 2 : 1);                                  \

@@ -118,6 +118,33 @@ template <> struct Wgmma<256> {
 
 template <int N, int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma(float *d, uint64_t ad, uint64_t bd, uint32_t scale_d) { Wgmma<N>::template mma<TA, TB>(d, ad, bd, scale_d); }
+
+// ---- wgmma with A from registers: D[64 x N] (+)= A[64 x 16] * B[16 x N], B K-major from shared memory. A fragment (PTX ISA, wgmma .m64nNk16 A
+// fragment, f16): thread t, w = t / 32, l = t % 32, register j holds the fp16 pair (row, col), (row, col + 1) with
+//   row = 16 w + l / 4 + 8 (j % 2),   col = 2 (l % 4) + 8 (j / 2)
+// i.e. the registers 8s..8s+7 of an m64nN accumulator (columns 16s..16s+15), packed pairwise, are the A fragment of K step s: each warp's rows stay in that warp.
+// The A registers must not be written until the wgmma that reads them has been waited for.
+template <int N> struct WgmmaRA;
+template <> struct WgmmaRA<16> {
+    static __device__ __forceinline__ void mma(float *d, const uint32_t *a, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+    }
+};
+template <> struct WgmmaRA<64> {
+    static __device__ __forceinline__ void mma(float *d, const uint32_t *a, uint64_t bd, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bd), "r"(scale_d));
+    }
+};
+template <int N>
+__device__ __forceinline__ void wgmma_ra(float *d, const uint32_t *a, uint64_t bd, uint32_t scale_d) { WgmmaRA<N>::mma(d, a, bd, scale_d); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -3,14 +3,16 @@
 // HashNerfMLP.run_mlp) and ngp_fused.cu (fused render).
 //
 // Mapping (thread r of the warpgroup == sample r: it writes A row r and receives the field output of row r):
-//   A tile   : [128 x 64] fp16, K-major, SWIZZLE_128B, 16 KB per warpgroup, rewritten in place layer after layer
+//   A tile   : [128 x 64] fp16, K-major, SWIZZLE_128B, 16 KB per warpgroup: the input of each net's FIRST layer (the encoding for density_net,
+//              density outputs 1..15 ++ SH ++ 1 for color_net), one row per thread
 //   weights  : packed once per optimiser step into the same swizzled layout (xrb_ngp_pack_weights), bulk-copied (TMA,
 //              cp.async.bulk) into shared memory once per CTA and kept resident for the whole persistent kernel
-//   per layer: all threads write their A row (st.shared) -> fence.proxy.async -> warpgroup named barrier -> the warpgroup issues
-//              K/16 wgmma.m64nNk16 for rows 0-63, waits, writes ReLU(fp16) of that half straight from the accumulator fragment into
-//              the next A tile, then the same for rows 64-127. Halves run one after the other so that a layer holds 32 fp32 accumulator
-//              registers per thread (the fused render kernel runs 768 threads per SM, i.e. at most 80 registers each).
-//   outputs  : the two N=16 output layers go through an 8 KB per-warpgroup staging tile, from which thread r reads row r.
+//   per net  : the tile runs as two M=64 halves, one after the other. Per half the first layer (A from the shared-memory tile) is followed by a
+//              register chain: the fp32 accumulator fragment of an m64n64 layer, ReLU'd and packed to fp16 pairs, IS the A fragment of the next layer's
+//              K steps (tc.cuh wgmma_ra), so the hidden layers and the N=16 output layer need no st.shared, no proxy fence and no barrier, and each
+//              warp's rows stay in that warp. A half holds 32 fp32 accumulators and 16 A registers per thread (the fused render kernel runs 768
+//              threads per SM, i.e. at most 80 registers each).
+//   outputs  : the N=16 output layer of each net goes through an 8 KB per-warpgroup staging tile, from which thread r reads row r.
 #pragma once
 #include "ngp_field.cuh"
 #include "tc.cuh"
@@ -41,115 +43,93 @@ __device__ __forceinline__ uint32_t pack_relu_h2f(float a, float b) {
     h = __hmax2(h, __float2half2_rn(0.f));
     return *reinterpret_cast<uint32_t *>(&h);
 }
+// m64n64 accumulator -> ReLU(fp16) A fragment of the next layer: K step s = accumulator registers 8s..8s+7 (tc.cuh wgmma_ra)
+__device__ __forceinline__ void acc_relu_to_a(const float *acc, uint32_t *a) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) a[i] = pack_relu_h2f(acc[2 * i], acc[2 * i + 1]);
+}
 
-// D[64 x N] = A[rows 64h.., K] * W[N x K]^T, issued (not waited for)
-template <int K, int N>
-__device__ __forceinline__ void tc_half_issue(const TcWarpgroup &c, uint32_t w_off, int h, float *acc) {
+// first layer of a net on half h of the tile: D[64 x 64] = A[rows 64h.., K] * W[64 x K]^T, issued (not waited for)
+template <int K>
+__device__ __forceinline__ void tc_first_issue(const TcWarpgroup &c, uint32_t w_off, int h, float *acc) {
     const uint32_t a0 = tc::smem_u32(c.A) + (uint32_t)h * 8192u, b0 = tc::smem_u32(c.W + w_off);
     tc::wg_fence();
 #pragma unroll
-    for (int k = 0; k < K / 16; ++k) tc::wgmma<N>(acc, tc::desc_k128(a0 + k * 32), tc::desc_k128(b0 + k * 32), k > 0 ? 1u : 0u);
+    for (int k = 0; k < K / 16; ++k) tc::wgmma<64>(acc, tc::desc_k128(a0 + k * 32), tc::desc_k128(b0 + k * 32), k > 0 ? 1u : 0u);
+    tc::wg_commit();
+}
+// chained layer: D[64 x N] = a[64 x 64] * W[N x 64]^T with a in registers, issued (not waited for)
+template <int N>
+__device__ __forceinline__ void tc_chain_issue(const TcWarpgroup &c, uint32_t w_off, const uint32_t *a, float *acc) {
+    const uint32_t b0 = tc::smem_u32(c.W + w_off);
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tc::wgmma_ra<N>(acc, a + 4 * k, tc::desc_k128(b0 + k * 32), k > 0 ? 1u : 0u);
     tc::wg_commit();
 }
 template <int N>
-__device__ __forceinline__ void tc_half_wait(float *acc) {
+__device__ __forceinline__ void tc_wait_all(float *acc) {
     tc::wg_wait<0>();
-    tc::acc_fence<N / 2>(acc);
+    tc::acc_fence<N>(acc);
 }
 // my st.shared of the A rows -> visible to the tensor core (async proxy), and every row of the warpgroup written
 __device__ __forceinline__ void tc_sync_a(const TcWarpgroup &c) {
     tc::fence_proxy_async_smem();
     tc_bar(c);
 }
-// half h of a 64-wide accumulator -> ReLU(fp16) -> A rows 64h.. (the rows this thread's fragment holds)
-__device__ __forceinline__ void tc_epilogue_relu_half(const TcWarpgroup &c, int h, const float *acc) {
-    const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row), q4 = (c.row & 3u) * 4u;
+
+// output fragment of half h of an N=16 layer -> staging tile (its own rows: no barrier needed before the stores)
+__device__ __forceinline__ void tc_stage_half(const TcWarpgroup &c, int h, const float *acc) {
+    // staging word of (row, col): row * 16 + (col ^ 4 (row & 3)) — conflict-free float2 stores, float4 loads of a row
+    const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        *reinterpret_cast<uint32_t *>(c.A + sw128_offset(r, j) + q4) = pack_relu_h2f(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<uint32_t *>(c.A + sw128_offset(r + 8, j) + q4) = pack_relu_h2f(acc[4 * j + 2], acc[4 * j + 3]);
+    for (int j = 0; j < 2; ++j) {
+        const uint32_t col = tc::frag_col(c.row, j);
+        *reinterpret_cast<float2 *>(c.stage + r * 16 + (col ^ ((r & 3u) << 2))) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2 *>(c.stage + (r + 8) * 16 + (col ^ (((r + 8) & 3u) << 2))) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
 }
-// hidden layer: A (K wide) -> ReLU(A W^T) (64 wide) in place, split in two so that a caller can put independent work (the next tile's hash gather)
-// between the issue of the first half and its wait:  float acc[32]; tc_hidden_begin<K>(c, w, acc); ...; tc_hidden_end<K>(c, w, acc);
-template <int K>
-__device__ __forceinline__ void tc_hidden_begin(const TcWarpgroup &c, uint32_t w_off, float *acc) {
-    tc_sync_a(c);
-    tc_half_issue<K, 64>(c, w_off, 0, acc);
-}
-template <int K>
-__device__ __forceinline__ void tc_hidden_end(const TcWarpgroup &c, uint32_t w_off, float *acc) {
-    tc_half_wait<64>(acc);
-    tc_bar(c);   // every warp's share of this half's MMA has completed before A rows are overwritten
-    tc_epilogue_relu_half(c, 0, acc);
-    tc_half_issue<K, 64>(c, w_off, 1, acc);   // reads rows 64-127, which the epilogue above did not touch
-    tc_half_wait<64>(acc);
-    tc_bar(c);
-    tc_epilogue_relu_half(c, 1, acc);
-}
-template <int K>
-__device__ __forceinline__ void tc_hidden_layer(const TcWarpgroup &c, uint32_t w_off) {
-    float acc[32];
-    tc_hidden_begin<K>(c, w_off, acc);
-    tc_hidden_end<K>(c, w_off, acc);
-}
-// output layer (N = 16): thread r receives the 16 fp32 outputs of row r;  float acc[16]; tc_output_begin(c, w, acc); ...; tc_output_end(c, acc, out);
-__device__ __forceinline__ void tc_output_begin(const TcWarpgroup &c, uint32_t w_off, float *acc) {
-    tc_sync_a(c);
-    tc_half_issue<64, 16>(c, w_off, 0, acc);
-    tc_half_issue<64, 16>(c, w_off, 1, acc + 8);
-}
-__device__ __forceinline__ void tc_output_end(const TcWarpgroup &c, float *acc, float *out) {
-    tc::wg_wait<0>();
-    tc::acc_fence<16>(acc);
-    // staging word of (row, col): row * 16 + (col ^ 4 (row & 3)) — conflict-free float2 stores, float4 loads of a row
+// One net (first layer from the A tile, n_hidden - 1 chained hidden layers, chained N=16 output layer) on the whole tile; thread r receives the 16 fp32
+// outputs of row r. Hidden layer l's weights follow the first layer's at w_in + 8192 (l + 1) (weight_image_layout; computed, so that no layout array is
+// indexed at run time, which would put it in local memory). The A tile must have been published (tc_sync_a). Half 1's first layer is issued while half 0's
+// output layer is still in flight.
+template <int K_IN>
+__device__ __forceinline__ void tc_net(const TcWarpgroup &c, uint32_t w_in, int n_hidden, uint32_t w_out, float *out) {
+    float acc[32], acc16[8];
+    uint32_t a[16];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const uint32_t col = tc::frag_col(c.row, j);
-            *reinterpret_cast<float2 *>(c.stage + r * 16 + (col ^ ((r & 3u) << 2))) = make_float2(acc[8 * h + 4 * j], acc[8 * h + 4 * j + 1]);
-            *reinterpret_cast<float2 *>(c.stage + (r + 8) * 16 + (col ^ (((r + 8) & 3u) << 2))) = make_float2(acc[8 * h + 4 * j + 2], acc[8 * h + 4 * j + 3]);
+        tc_first_issue<K_IN>(c, w_in, h, acc);
+        tc_wait_all<32>(acc);   // (h = 1: also half 0's output layer, the last reader of a)
+        if (h == 1) { tc::acc_fence<8>(acc16); tc_stage_half(c, 0, acc16); }
+        acc_relu_to_a(acc, a);
+        for (int l = 0; l < n_hidden - 1; ++l) {
+            tc_chain_issue<64>(c, w_in + 8192u * (uint32_t)(l + 1), a, acc);
+            tc_wait_all<32>(acc);
+            acc_relu_to_a(acc, a);
         }
+        tc_chain_issue<16>(c, w_out, a, acc16);
     }
-    tc_bar(c);
+    tc_wait_all<8>(acc16);
+    tc_stage_half(c, 1, acc16);
+    tc_bar(c);   // every row staged; also every warp's wgmma of the net has completed, so the A tile may be rewritten after this
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const float4 v = *reinterpret_cast<const float4 *>(c.stage + c.row * 16 + (((uint32_t)k ^ (c.row & 3u)) << 2));
         out[4 * k] = v.x; out[4 * k + 1] = v.y; out[4 * k + 2] = v.z; out[4 * k + 3] = v.w;
     }
-    // the staging tile is rewritten only after the next layer's tc_sync_a barrier: every row has been read by then
+    // the staging tile is rewritten only after the next net's tc_sync_a barrier: every row has been read by then
 }
-__device__ __forceinline__ void tc_output_layer(const TcWarpgroup &c, uint32_t w_off, float *out) {
-    float acc[16];
-    tc_output_begin(c, w_off, acc);
-    tc_output_end(c, acc, out);
-}
-
-// Density half of the field, the 32 encoded features already sitting in chunks 0..3 of my A row: density_net's 16 fp16-rounded outputs.
-__device__ __forceinline__ void tc_density_from_a(TcWarpgroup &c, const WeightImageLayout &L, int density_hidden, float *dout) {
-    tc_hidden_layer<32>(c, L.d_in);
-    for (int h = 0; h < density_hidden - 1; ++h) tc_hidden_layer<64>(c, L.d_hid[h]);
-    tc_output_layer(c, L.d_out, dout);
+// density_net on the tile, the 32 encoded features already sitting in chunks 0..3 of my A row: its 16 fp16-rounded outputs for my row
+__device__ __forceinline__ void tc_density_from_a(const TcWarpgroup &c, const WeightImageLayout &L, int density_hidden, float *dout) {
+    tc_sync_a(c);
+    tc_net<32>(c, L.d_in, density_hidden, L.d_out, dout);
 #pragma unroll
     for (int k = 0; k < 16; ++k) dout[k] = round_h(dout[k]);
 }
-template <int NP>
-__device__ __forceinline__ void tc_density(TcWarpgroup &c, const WeightImageLayout &L, int density_hidden, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells,
-                                           const HashGridDev &g, float x, float y, float z, float *dout) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        uint32_t e[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { float2 f = hash_level(table, cells, g, 4 * q + k, x, y, z, plan_mode<NP>(4 * q + k)); e[k] = pack_h2(f.x, f.y); }
-        a_store_chunk(c, q, make_uint4(e[0], e[1], e[2], e[3]));
-    }
-    tc_density_from_a(c, L, density_hidden, dout);
-}
 
 // colour-net input row of my sample: density_out[1:16] (15) ++ SH (16) ++ 1.0 pad (tcnn.Network pads 31 -> 32 with ones)
-__device__ __forceinline__ void tc_store_color_input(TcWarpgroup &c, const float *dout, float dx, float dy, float dz) {
+__device__ __forceinline__ void tc_store_color_input(const TcWarpgroup &c, const float *dout, float dx, float dy, float dz) {
     float sh[16];
     sh4(dx, dy, dz, sh);
     float cin[32];
@@ -163,21 +143,12 @@ __device__ __forceinline__ void tc_store_color_input(TcWarpgroup &c, const float
         a_store_chunk(c, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
 }
 // Colour half (HashNerfMLP.run_mlp, hashnerf_mlp.py:66-79) given density_net's outputs: raw = (rgb[3], density[1]) for my sample
-__device__ __forceinline__ float4 tc_color_from_density(TcWarpgroup &c, const WeightImageLayout &L, int color_hidden, const float *dout, float dx, float dy, float dz) {
+__device__ __forceinline__ float4 tc_color_from_density(const TcWarpgroup &c, const WeightImageLayout &L, int color_hidden, const float *dout, float dx, float dy, float dz) {
     tc_store_color_input(c, dout, dx, dy, dz);
-    tc_hidden_layer<32>(c, L.c_in);
-    for (int h = 0; h < color_hidden - 1; ++h) tc_hidden_layer<64>(c, L.c_hid[h]);
+    tc_sync_a(c);
     float cout[16];
-    tc_output_layer(c, L.c_out, cout);
+    tc_net<32>(c, L.c_in, color_hidden, L.c_out, cout);
     return make_float4(round_h(cout[0]), round_h(cout[1]), round_h(cout[2]), dout[0]);
-}
-// Whole field: hash encode + both nets
-template <int NP>
-__device__ __forceinline__ float4 tc_field(TcWarpgroup &c, const WeightImageLayout &L, int density_hidden, int color_hidden, const __half2 *__restrict__ table,
-                                           const uint8_t *__restrict__ cells, const HashGridDev &g, float x, float y, float z, float dx, float dy, float dz) {
-    float dout[16];
-    tc_density<NP>(c, L, density_hidden, table, cells, g, x, y, z, dout);
-    return tc_color_from_density(c, L, color_hidden, dout, dx, dy, dz);
 }
 
 // levels [L0, L1) of the hash encoding of one sample as packed half2 words
@@ -186,49 +157,6 @@ __device__ __forceinline__ void tc_gather_levels(const __half2 *__restrict__ tab
 #pragma unroll
     for (int l = L0; l < L1; ++l) { const float2 f = hash_level(table, cells, g, l, x, y, z, plan_mode<NP>(l)); e[l] = pack_h2(f.x, f.y); }
 }
-// One tile of the field with the NEXT tile's gather folded into the waits of this tile's tensor-core layers (the layers of a tile are a chain of
-// issue -> wait round trips during which this warpgroup would otherwise load nothing).
-//   e  : encoding of THIS tile's sample (16 packed half2), already gathered
-//   en : receives the encoding of the next tile's sample at (xn, yn, zn) when has_next
-// Same arithmetic, same order per sample: bit-identical to tc_density / tc_color_from_density.
-template <int NP, bool DENSITY_ONLY>
-__device__ __forceinline__ float4 tc_field_gather_ahead(TcWarpgroup &c, const WeightImageLayout &L, int density_hidden, int color_hidden, const __half2 *__restrict__ table,
-                                                        const uint8_t *__restrict__ cells, const HashGridDev &g, const uint32_t *e, float dx, float dy, float dz, bool has_next, float xn, float yn,
-                                                        float zn, uint32_t *en) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) a_store_chunk(c, q, make_uint4(e[4 * q], e[4 * q + 1], e[4 * q + 2], e[4 * q + 3]));
-    float acc[32], acc16[16];
-    tc_hidden_begin<32>(c, L.d_in, acc);
-    if (has_next) tc_gather_levels<NP, 0, 3>(table, cells, g, xn, yn, zn, en);
-    tc_hidden_end<32>(c, L.d_in, acc);
-    for (int h = 0; h < density_hidden - 1; ++h) tc_hidden_layer<64>(c, L.d_hid[h]);
-    float dout[16];
-    tc_output_begin(c, L.d_out, acc16);
-    if (has_next) tc_gather_levels<NP, 3, 6>(table, cells, g, xn, yn, zn, en);
-    tc_output_end(c, acc16, dout);
-#pragma unroll
-    for (int k = 0; k < 16; ++k) dout[k] = round_h(dout[k]);
-    if (DENSITY_ONLY) {
-        if (has_next) tc_gather_levels<NP, 6, 16>(table, cells, g, xn, yn, zn, en);
-        return make_float4(dout[0], 0.f, 0.f, 0.f);
-    }
-    tc_store_color_input(c, dout, dx, dy, dz);
-    tc_hidden_begin<32>(c, L.c_in, acc);
-    if (has_next) tc_gather_levels<NP, 6, 9>(table, cells, g, xn, yn, zn, en);
-    tc_hidden_end<32>(c, L.c_in, acc);
-    for (int h = 0; h < color_hidden - 1; ++h) {
-        tc_hidden_begin<64>(c, L.c_hid[h], acc);
-        if (h == 0 && has_next) tc_gather_levels<NP, 9, 12>(table, cells, g, xn, yn, zn, en);
-        tc_hidden_end<64>(c, L.c_hid[h], acc);
-    }
-    if (color_hidden < 2 && has_next) tc_gather_levels<NP, 9, 12>(table, cells, g, xn, yn, zn, en);
-    float cout[16];
-    tc_output_begin(c, L.c_out, acc16);
-    if (has_next) tc_gather_levels<NP, 12, 16>(table, cells, g, xn, yn, zn, en);
-    tc_output_end(c, acc16, cout);
-    return make_float4(round_h(cout[0]), round_h(cout[1]), round_h(cout[2]), dout[0]);
-}
-
 // ---- CTA-level setup shared by the kernels that use the warpgroup evaluator
 // dynamic shared memory layout: [weights image][A tile x WG][staging tile x WG][mbarrier]
 template <int WG>
