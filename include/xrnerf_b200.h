@@ -293,16 +293,12 @@ int xrb_nerf_posenc(const float *pts, const float *viewdirs, int64_t n_pts, int 
                     float *embedded, void *stream);
 
 /* NerfMLP.run_mlp (xrnerf/models/mlps/nerf_mlp.py:70-94; netdepth 8, netwidth 256, skips [4], use_viewdirs) as one persistent wgmma
- * kernel, inference forward. embedded f32[n, input_ch + input_ch_dirs] ((63,27) NeRF or (96,27) Mip-NeRF) -> raw f32[n,4] = (rgb3, alpha1).
- * weight_image / bias: produced by xrnerf_b200.nerf_mlp.pack_nerf_mlp (fp16 slabs, K-major, 128-byte swizzle, in streaming order). */
-int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* the same chain on an fp16 encoding tile image, weights as half slabs (image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v2); the bias is added in fp16 after
- * rounding the accumulator and alpha is a dot product in the epilogue of pts_linears.7 */
-int xrb_nerf_mlp_forward_v2(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* v3: the same arithmetic as v2 with the 256-wide layers' weights as [256 x 32] K-half slabs (64-byte swizzle). weight_image / bias from the matching host packer
- * (xrnerf_b200.nerf_mlp.pack_nerf_mlp_v3: bias = fp32 vector + fp16 copy). */
-int xrb_nerf_mlp_forward_v3(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
-/* encoding tile image consumed by v2 / v3 (per 128-row tile: point-encoding block(s) then direction block, [128x64] fp16, K-major 128B swizzle):
+ * kernel, inference forward. enc_image: the fp16 encoding tile image of n rows with (input_ch, input_ch_dirs) = (63,27) NeRF or (96,27) Mip-NeRF
+ * -> raw f32[n,4] = (rgb3, alpha1). weight_image / bias: produced by xrnerf_b200.nerf_mlp.pack_nerf_mlp (fp16 slabs in streaming order; bias = fp32
+ * vector + fp16 copy). Each layer's fp32 accumulator is rounded to fp16 before the bias is added in fp16; alpha is a dot product in the epilogue of
+ * pts_linears.7. All pointers 16-byte aligned. */
+int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream);
+/* encoding tile image consumed by xrb_nerf_mlp_forward (per 128-row tile: point-encoding block(s) then direction block, [128x64] fp16, K-major 128B swizzle):
  * size, conversion from an fp32 `embedded` matrix, and BaseEmbedder's positional encoding written directly in that form */
 size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch);
 int xrb_nerf_pack_embedded(const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, void *enc_image, void *stream);
@@ -318,7 +314,7 @@ int xrb_mip_embed(const float *z_vals, const float *rays_o, const float *rays_d,
                   int max_deg_point, int min_deg_view, int max_deg_view, float *embedded, float *means_out, float *covs_out, void *stream);
 
 /* The same cast_rays + IPE + view-direction encoding (networks/utils/mip.py:66-129, embedders/mipnerf_embedder.py:43-99) written straight into the fp16 tile image
- * xrb_nerf_mlp_forward_v2 / _v3 consume
+ * xrb_nerf_mlp_forward consumes
  * (xrb_nerf_enc_image_bytes(N*S, 6*(max_deg_point-min_deg_point)) bytes): no fp32 `embedded` round trip. Values are the fp16 roundings of xrb_mip_embed's. */
 int xrb_mip_ipe_tiles_rays(const float *z_vals, const float *rays_o, const float *rays_d, const float *radii, const float *viewdirs, int64_t n_rays, int n_samples, int min_deg_point,
                            int max_deg_point, int min_deg_view, int max_deg_view, void *enc_image, void *stream);

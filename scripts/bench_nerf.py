@@ -24,27 +24,16 @@ mlp = R.build_mlp(MLP).cuda()
 rows = 32768 * 64            # 32 768 rays x 64 samples
 emb = torch.randn((rows, 90), device='cuda')
 flop = rows * 593408 * 2
-from xrnerf_b200.nerf_mlp import pack_nerf_mlp, pack_nerf_mlp_v2
-for v, packer in (((2, pack_nerf_mlp_v2),) if os.environ.get('XRB_NM_DBG') else ((1, pack_nerf_mlp), (2, pack_nerf_mlp_v2))):
-    image, bias = packer(mlp)
-    t = timeit(lambda: nerf_mlp_forward(image, bias, emb, 63, 27, version=v))
-    print(f'fused wgmma NerfMLP v{v}: {t:.3f} ms for {rows} rows -> {flop / t / 1e9:.1f} TFLOP/s ({rows / t / 1e3:.1f} Mrows/s)', flush=True)
-    if v == 2:
-        from xrnerf_b200 import _C
-        from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles
-        enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(rows, 63), dtype=torch.uint8, device='cuda')
-        _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb), rows, 63, 27, _C.ptr(enc), _C.stream()))
-        raw = torch.empty((rows, 4), device='cuda')
-        t = timeit(lambda: nerf_mlp_forward_tiles(image, bias, enc, rows, 63, 27, raw))
-        print(f'   v2 MLP kernel alone (pre-packed encodings): {t:.3f} ms -> {flop / t / 1e9:.1f} TFLOP/s', flush=True)
 from xrnerf_b200 import _C
-from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles, pack_nerf_mlp_v3
+from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles, pack_nerf_mlp
+image, bias = pack_nerf_mlp(mlp)
+t = timeit(lambda: nerf_mlp_forward(image, bias, emb, 63, 27))
+print(f'fused wgmma NerfMLP (fp32 rows, packing included): {t:.3f} ms for {rows} rows -> {flop / t / 1e9:.1f} TFLOP/s ({rows / t / 1e3:.1f} Mrows/s)', flush=True)
 enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(rows, 63), dtype=torch.uint8, device='cuda')
 _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb), rows, 63, 27, _C.ptr(enc), _C.stream()))
-raw3 = torch.empty((rows, 4), device='cuda')
-image3, bias3 = pack_nerf_mlp_v3(mlp)
-t = timeit(lambda: nerf_mlp_forward_tiles(image3, bias3, enc, rows, 63, 27, raw3, version=3))
-print(f'   v3 MLP kernel alone (two tiles in flight per SM): {t:.3f} ms -> {flop / t / 1e9:.1f} TFLOP/s', flush=True)
+raw = torch.empty((rows, 4), device='cuda')
+t = timeit(lambda: nerf_mlp_forward_tiles(image, bias, enc, rows, 63, 27, raw))
+print(f'   MLP kernel alone (pre-packed encodings): {t:.3f} ms -> {flop / t / 1e9:.1f} TFLOP/s', flush=True)
 z = torch.linspace(2, 6, 64, device='cuda').expand(32768, 64).contiguous(); o = torch.rand((32768, 3), device='cuda'); d = torch.nn.functional.normalize(torch.randn((32768, 3), device='cuda'), dim=-1)
 t = timeit(lambda: _C.check(_C.lib.xrb_nerf_posenc_tiles_rays(_C.ptr(o), _C.ptr(d), _C.ptr(z), _C.ptr(d), 32768, 64, 10, 4, _C.ptr(enc), _C.stream())))
 print(f'   posenc tile images (ray mode, 32768 x 64): {t:.3f} ms', flush=True)
@@ -52,7 +41,7 @@ z2 = torch.linspace(2, 6, 129, device='cuda').expand(32768, 129).contiguous(); r
 enc2 = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(32768 * 128, 96), dtype=torch.uint8, device='cuda')
 t = timeit(lambda: _C.check(_C.lib.xrb_mip_ipe_tiles_rays(_C.ptr(z2), _C.ptr(o), _C.ptr(d), _C.ptr(rad), _C.ptr(d), 32768, 128, 0, 16, 0, 4, _C.ptr(enc2), _C.stream())))
 print(f'   IPE tile images (32768 x 128): {t:.3f} ms', flush=True)
-if os.environ.get('XRB_NM_DBG') or os.environ.get('XRB_SKIP_LIB'):
+if os.environ.get('XRB_SKIP_LIB'):
     sys.exit(0)
 with torch.enable_grad():
     x = emb[:32768 * 8].clone().requires_grad_(True)

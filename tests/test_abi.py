@@ -22,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert len(names) >= 40
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, missing
-    assert lib.xrb_abi_version() == 2 and lib.xrb_built_for_sm() == 90
+    assert lib.xrb_abi_version() == 3 and lib.xrb_built_for_sm() == 90
 
 
 def test_python_binding_covers_header():
@@ -43,17 +43,17 @@ def test_argument_validation_without_gpu():
     assert lib.xrb_tcnn_hashgrid_num_params(cfg) == 12196240
     bad = _C.NgpConfig(16, 4, 19, 16, 1.38191288, 64, 1, 2)   # n_features 4 is not implemented: loud, not silent
     assert lib.xrb_tcnn_hashgrid_num_params(bad) == -1 and b'unsupported' in lib.xrb_last_error()
-    assert lib.xrb_nerf_mlp_forward(None, None, None, 10, 50, 27, None, None) == -2
     assert lib.xrb_nerf_sample_pdf(None, None, None, None, None, 4, 300, 128, None, None, None) == -2
-    # entry points added in round 1, session 2: sizes / supported shapes / null pointers / alignment, all checked before any CUDA call
-    assert lib.xrb_nerf_mlp_forward_v3(None, None, None, -1, 63, 27, None, None) == -1
-    assert lib.xrb_nerf_mlp_forward_v3(None, None, None, 10, 60, 27, None, None) == -2 and b'(63,27) or (96,27)' in lib.xrb_last_error()
-    assert lib.xrb_nerf_mlp_forward_v3(None, None, None, 0, 63, 27, None, None) == 0                       # empty input is not an error
-    assert lib.xrb_nerf_mlp_forward_v3(None, None, None, 10, 63, 27, None, None) == -1 and b'null' in lib.xrb_last_error()
+    # NerfMLP: sizes / supported shapes / null pointers / alignment, all checked before any CUDA call
+    assert lib.xrb_nerf_mlp_forward(None, None, None, -1, 63, 27, None, None) == -1
+    assert lib.xrb_nerf_mlp_forward(None, None, None, 10, 50, 27, None, None) == -2
+    assert lib.xrb_nerf_mlp_forward(None, None, None, 10, 60, 27, None, None) == -2 and b'(63,27) or (96,27)' in lib.xrb_last_error()
+    assert lib.xrb_nerf_mlp_forward(None, None, None, 0, 63, 27, None, None) == 0                          # empty input is not an error
+    assert lib.xrb_nerf_mlp_forward(None, None, None, 10, 63, 27, None, None) == -1 and b'null' in lib.xrb_last_error()
     buf = (C.c_char * 64)()
     a = C.addressof(buf)
     odd = C.c_void_p(a + 4)                                                                                  # not 16-byte aligned
-    assert lib.xrb_nerf_mlp_forward_v3(odd, odd, odd, 10, 63, 27, odd, None) == -1 and b'aligned' in lib.xrb_last_error()
+    assert lib.xrb_nerf_mlp_forward(odd, odd, odd, 10, 63, 27, odd, None) == -1 and b'aligned' in lib.xrb_last_error()
     assert lib.xrb_mip_ipe_tiles_rays(None, None, None, None, None, 4, 8, 0, 30, 0, 4, None, None) == -1 and b'wider' in lib.xrb_last_error()   # 180 IPE columns do not fit two blocks
     assert lib.xrb_mip_ipe_tiles_rays(None, None, None, None, None, 0, 8, 0, 16, 0, 4, None, None) == 0
     assert lib.xrb_mip_ipe_tiles_rays(None, None, None, None, None, 4, 8, 0, 16, 0, 4, None, None) == -1

@@ -58,7 +58,7 @@ def test_reference_nerf_mlp_checkpoints_load_into_registry_modules():
     """SURVEY 8f-4 (checkpoint compatibility): the state_dict of the REFERENCE's own NerfMLP (NeRF and Mip-NeRF embedders) has exactly our keys and shapes and loads
     with strict=True; the packed wgmma weight image is rebuilt from the loaded weights."""
     from xrnerf_b200 import registry as R
-    from xrnerf_b200.nerf_mlp import pack_nerf_mlp_v3
+    from xrnerf_b200.nerf_mlp import pack_nerf_mlp
     G = np.load(GOLDEN)
     for c, cfg in enumerate(NERF_MLP_CFGS):
         keys, shapes = [str(k) for k in G[f'ckpt{c}/keys']], [tuple(int(x) for x in s if x) for s in G[f'ckpt{c}/shapes']]
@@ -70,5 +70,5 @@ def test_reference_nerf_mlp_checkpoints_load_into_registry_modules():
         assert list(sd_ref) == list(sd_ours) and all(sd_ref[k].shape == sd_ours[k].shape for k in sd_ref)
         assert (ours.input_ch, ours.input_ch_dirs) == tuple(int(x) for x in G[f'ckpt{c}/input_ch'])
         ours.load_state_dict(sd_ref, strict=True)
-        image, bias = pack_nerf_mlp_v3(ours)
+        image, bias = pack_nerf_mlp(ours)
         assert torch.equal(bias[:256], sd_ref['pts_linears.0.bias']) and image.numel() > 1_000_000

@@ -1,5 +1,5 @@
 """CPU checks of the host-side weight packers of the wgmma NerfMLP kernels (xrnerf_b200/nerf_mlp.py): the swizzled byte layouts the kernels'
-shared-memory descriptors assume, and the stream image sizes / bias vector layout of the v3 entry of csrc/nerf_mlp_tc.cu. No GPU needed."""
+shared-memory descriptors assume, and the stream image sizes / bias vector layout of csrc/nerf_mlp_tc.cu. No GPU needed."""
 import numpy as np
 import torch
 
@@ -34,11 +34,11 @@ def test_swizzle_64b_slab_layout():
     assert len(np.unique(off)) == off.size
 
 
-def test_v3_stream_image_and_bias_vector():
+def test_stream_image_and_bias_vector():
     torch.manual_seed(0)
     for cfg, n_kb in ((NERF_MLP, [1, 4, 4, 4, 4, 5, 4, 4, 4]), (MIP_MLP, [2, 4, 4, 4, 4, 6, 4, 4, 4])):
         mlp = R.build_mlp(cfg)
-        image, bias = nm.pack_nerf_mlp_v3(mlp)
+        image, bias = nm.pack_nerf_mlp(mlp)
         # 256-wide layers: 2 slabs of 16 KB per K-block; views_linears.0: 5 slabs [128 x 64]; rgb_linear: 2 slabs [16 x 64]
         assert image.numel() == sum(n_kb) * 2 * 16384 + 5 * 16384 + 2 * 2048
         n_layer_bias = 9 * 256 + 128 + 16

@@ -100,8 +100,6 @@ _SIGS = {
     'xrb_nerf_sample_pdf': (_i, [P, P, P, P, P, _i, _i, _i, P, P, P]),
     'xrb_nerf_posenc': (_i, [P, P, _i64, _i, _i, _i, P, P]),
     'xrb_nerf_mlp_forward': (_i, [P, P, P, _i64, _i, _i, P, P]),
-    'xrb_nerf_mlp_forward_v2': (_i, [P, P, P, _i64, _i, _i, P, P]),
-    'xrb_nerf_mlp_forward_v3': (_i, [P, P, P, _i64, _i, _i, P, P]),
     'xrb_nerf_enc_image_bytes': (_sz, [_i64, _i]),
     'xrb_nerf_pack_embedded': (_i, [P, _i64, _i, _i, P, P]),
     'xrb_nerf_posenc_tiles': (_i, [P, P, _i64, _i, _i, _i, P, P]),

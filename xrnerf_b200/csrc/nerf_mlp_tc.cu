@@ -9,16 +9,15 @@
 //              The two warpgroups never wait for each other: a row's next-layer input depends on that row only.
 //   warp 8     TMA producer (its warpgroup gives its registers to the two consumer warpgroups: setmaxnreg 40 / 232): streams the pre-swizzled weight slabs of all 11 layers from the L2-resident weight image through a shared-memory
 //              ring (cp.async.bulk + mbarrier expect_tx; a slot is released when all 8 consumer warps have finished the MMAs that read it), and
-//              (v2 / v3) the tile's fp16 encoding blocks, re-armed once both warpgroups are past their last reader (views_linears.0).
+//              the tile's fp16 encoding blocks, re-armed once both warpgroups are past their last reader (views_linears.0).
 // A operand: [128 x 64]-blocks, K-major, 128-byte swizzle: blocks 0-3 hidden state h (256 wide), 4..4+AUX-1 the point encoding
-// (63 -> 64 for NeRF, 96 -> 128 for Mip-NeRF), last block the view-direction encoding (27 -> 64).
-// The three entry points differ in how the host packed the weights (xrnerf_b200/nerf_mlp.py) and in one numeric detail:
-//   v1  [N x 64] slabs, one per K-block; fp32 embedded rows converted in the kernel; bias added in fp32 before rounding; alpha head as 16 extra
-//       rows of the feature layer's slabs (an N=16 MMA next to the N=256 one)
-//   v2  [N/2 x 64] half slabs; v3  [256 x 32] K-half slabs (64-byte swizzle) for the 256-wide layers, [N x 64] otherwise. Both take the fp16
-//       encoding tile image (xrb_nerf_pack_embedded / posenc / IPE kernels), add the bias in fp16 after rounding the accumulator, and form alpha
-//       as a register dot product with alpha_linear in the epilogue of pts_linears.7. Same arithmetic: v2 and v3 give the same result.
-// Numeric contract: fp16 operands (weights and activations), fp32 accumulate; parity tolerance vs the fp32 reference in tests/test_gpu_nerf_mlp.py.
+// (63 -> 64 for NeRF, 96 -> 128 for Mip-NeRF), last block the view-direction encoding (27 -> 64). The encoding blocks come from the fp16
+// encoding tile image (xrb_nerf_pack_embedded / posenc / IPE kernels).
+// Weights (packed by xrnerf_b200/nerf_mlp.py pack_nerf_mlp): [256 x 32] K-half slabs (64-byte swizzle) for the 256-wide layers, [N x 64] slabs
+// (128-byte swizzle) otherwise.
+// Numeric contract: fp16 operands (weights and activations), fp32 accumulate; each layer's accumulator is rounded to fp16, then the bias is added in
+// fp16; alpha is an fp32 register dot product of the fp16 pts_linears.7 output with alpha_linear, formed in that layer's epilogue.
+// Parity tolerance vs the fp32 reference in tests/test_gpu_nerf_mlp.py.
 #include "tc.cuh"
 #include "common.cuh"
 #include <cuda_fp16.h>
@@ -38,53 +37,39 @@ __device__ __forceinline__ uint32_t nm_sw128(uint32_t row, uint32_t chunk16) { r
 struct NmSlab {
     int a_blk;     // A block the slab contracts with
     int kh;        // -1: all 64 columns of the block (128-byte swizzled [rows x 64] slab); 0 / 1: columns 32kh.. ([rows x 32], 64-byte swizzle)
-    int rows;      // output columns the slab covers (slab rows), starting at accumulator column col0
-    int col0;
-    int first;     // first slab of the layer that writes columns [col0, col0 + rows): overwrite instead of accumulate
-    int alpha;     // v1: 16 more rows (the alpha head) follow, into the separate N=16 accumulator
+    int rows;      // output columns the slab covers (slab rows)
+    int first;     // first slab of the layer: overwrite the accumulator instead of accumulating
 };
 struct NmLayer {
     int N, relu, bias_off, alpha_dot, n_slabs;
     NmSlab s[NM_MAX_SLABS];
 };
-__host__ __device__ constexpr uint32_t nm_slab_bytes(const NmSlab &s) { return (uint32_t)(s.rows + (s.alpha ? 16 : 0)) * (s.kh >= 0 ? 64u : 128u); }
+__host__ __device__ constexpr uint32_t nm_slab_bytes(const NmSlab &s) { return (uint32_t)s.rows * (s.kh >= 0 ? 64u : 128u); }
 
-template <int VER, bool MIP>
+template <bool MIP>
 __host__ __device__ constexpr NmLayer nm_layer(int l) {
     const int aux = MIP ? 2 : 1, P0 = 4, P1 = 5, DIR = 4 + aux;
     NmLayer L{};
     L.N = l == 9 ? 128 : (l == 10 ? 16 : 256);
     L.relu = (l == 8 || l == 10) ? 0 : 1;
-    L.alpha_dot = VER >= 2 && l == 7;
-    L.bias_off = VER == 1 ? (l <= 8 ? 256 * l : (l == 9 ? 2320 : 2448)) : (l <= 9 ? 256 * l : 2432);   // v1: the feature layer carries 16 alpha-head biases
+    L.alpha_dot = l == 7;
+    L.bias_off = l <= 9 ? 256 * l : 2432;
     int src[6] = {0, 1, 2, 3, 0, 0}, nk = 4;
     if (l == 0) { src[0] = P0; src[1] = P1; nk = aux; }
-    else if (l == 5) {
-        if (VER == 1) { src[4] = P0; src[5] = P1; nk = 4 + aux; }
-        else if (VER == 2) { src[0] = P0; src[1] = P1; src[aux] = 0; src[aux + 1] = 1; src[aux + 2] = 2; src[aux + 3] = 3; nk = 4 + aux; }
-        else { src[0] = P0; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; src[5] = P1; nk = 4 + aux; }
-    } else if (l == 9) {
-        if (VER == 1) { src[4] = DIR; } else { src[0] = DIR; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; }
-        nk = 5;
-    } else if (l == 10) nk = 2;
+    else if (l == 5) { src[0] = P0; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; src[5] = P1; nk = 4 + aux; }
+    else if (l == 9) { src[0] = DIR; src[1] = 0; src[2] = 1; src[3] = 2; src[4] = 3; nk = 5; }
+    else if (l == 10) nk = 2;
     int n = 0;
     for (int k = 0; k < nk; ++k) {
-        if (VER == 1) {
-            L.s[n++] = NmSlab{src[k], -1, L.N, 0, k == 0, l == 8};
-        } else if (VER == 2) {
-            const int halves = L.N == 16 ? 1 : 2;
-            for (int h = 0; h < halves; ++h) L.s[n++] = NmSlab{src[k], -1, L.N / halves, h * (L.N / halves), k == 0, 0};
-        } else {
-            if (L.N == 256) { L.s[n++] = NmSlab{src[k], 0, 256, 0, k == 0, 0}; L.s[n++] = NmSlab{src[k], 1, 256, 0, 0, 0}; }
-            else L.s[n++] = NmSlab{src[k], -1, L.N, 0, k == 0, 0};
-        }
+        if (L.N == 256) { L.s[n++] = NmSlab{src[k], 0, 256, k == 0}; L.s[n++] = NmSlab{src[k], 1, 256, 0}; }
+        else L.s[n++] = NmSlab{src[k], -1, L.N, k == 0};
     }
     L.n_slabs = n;
     return L;
 }
 
 struct NmParams {
-    const uint8_t *weight_image; const float *bias; const float *embedded; const uint8_t *enc_image;
+    const uint8_t *weight_image; const float *bias; const uint8_t *enc_image;
     int64_t n_rows; int input_ch, input_ch_dirs;
     float *raw;
     uint32_t slot_bytes; int n_slots;
@@ -100,9 +85,9 @@ template <int N>
 __device__ __forceinline__ void nm_mma(float *acc, uint64_t ad, uint64_t bd, uint32_t sc) { tc::wgmma<N>(acc, ad, bd, sc); }
 
 // the MMAs of slabs [S, n_slabs) of layer L, one slab at a time through the ring
-template <int VER, bool MIP, int L, int S>
-__device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc, float *acc_a) {
-    constexpr NmLayer Ly = nm_layer<VER, MIP>(L);
+template <bool MIP, int L, int S>
+__device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc) {
+    constexpr NmLayer Ly = nm_layer<MIP>(L);
     if constexpr (S < Ly.n_slabs) {
         constexpr NmSlab sl = Ly.s[S];
         const uint32_t slot = x.it % x.n_slots, ph = (x.it / x.n_slots) & 1u;
@@ -114,29 +99,27 @@ __device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc, float *acc_a) {
         for (int k = 0; k < (sl.kh >= 0 ? 2 : 4); ++k) {
             const uint32_t sc = (sl.first && k == 0) ? 0u : 1u;
             const uint64_t ad = tc::desc_k128(a0 + k * 32), bd = sl.kh >= 0 ? tc::desc_k64(b0 + k * 32) : tc::desc_k128(b0 + k * 32);
-            nm_mma<sl.rows>(acc + sl.col0 / 2, ad, bd, sc);
-            if constexpr (sl.alpha) nm_mma<16>(acc_a, ad, tc::desc_k128(b0 + (uint32_t)sl.rows * 128u + k * 32), sc);
+            nm_mma<sl.rows>(acc, ad, bd, sc);
         }
         tc::wg_commit();
         tc::wg_wait<0>();
         __syncwarp();
         if (x.lane == 0) tc::mbar_arrive(x.empty + slot);   // this warp's share of the MMAs reading the slot is complete
         ++x.it;
-        nm_slabs<VER, MIP, L, S + 1>(x, acc, acc_a);
+        nm_slabs<MIP, L, S + 1>(x, acc);
     }
 }
 
 // layers [L, 11) of one tile for my 64 rows
-template <int VER, bool MIP, int L>
+template <bool MIP, int L>
 __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t tile, float *alpha) {
     if constexpr (L < NM_LAYERS) {
-        constexpr NmLayer Ly = nm_layer<VER, MIP>(L);
-        float acc[Ly.N / 2], acc_a[8];
-        tc::fence_proxy_async_smem();        // my epilogue / staging writes -> visible to the tensor core
+        constexpr NmLayer Ly = nm_layer<MIP>(L);
+        float acc[Ly.N / 2];
+        tc::fence_proxy_async_smem();        // my epilogue writes -> visible to the tensor core
         tc::named_bar_sync(1 + x.wg, 128);   // ... and every row of my warpgroup written
-        nm_slabs<VER, MIP, L, 0>(x, acc, acc_a);
+        nm_slabs<MIP, L, 0>(x, acc);
         tc::acc_fence<Ly.N / 2>(acc);
-        if constexpr (VER == 1 && L == 8) tc::acc_fence<8>(acc_a);
         tc::named_bar_sync(1 + x.wg, 128);   // every warp's share of this layer's MMAs has completed before A blocks are rewritten
         const float *b = P.bias + Ly.bias_off;
         if constexpr (L == NM_LAYERS - 1) {
@@ -151,7 +134,7 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
             }
         } else {
             float adot[2] = {0.f, 0.f};
-            const float *wa = P.bias + 2448;   // v2 / v3: alpha_linear weights follow the per-layer biases, then its bias
+            const float *wa = P.bias + 2448;   // alpha_linear weights follow the per-layer biases, then its bias
 #pragma unroll
             for (int j = 0; j < Ly.N / 8; ++j) {
                 const uint32_t col = tc::frag_col(x.t, j);
@@ -159,16 +142,9 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
                 const float b0 = __ldg(b + col), b1 = __ldg(b + col + 1);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    __half2 h;
-                    if (VER == 1) {
-                        float v0 = acc[4 * j + 2 * e] + b0, v1 = acc[4 * j + 2 * e + 1] + b1;
-                        if (Ly.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                        h = __floats2half2_rn(v0, v1);
-                    } else {
-                        h = __hadd2(__floats2half2_rn(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), __floats2half2_rn(b0, b1));
-                        if (Ly.relu) h = __hmax2(h, __float2half2_rn(0.f));
-                        if (Ly.alpha_dot) { const float2 f = __half22float2(h); adot[e] = fmaf(f.x, __ldg(wa + col), adot[e]); adot[e] = fmaf(f.y, __ldg(wa + col + 1), adot[e]); }
-                    }
+                    __half2 h = __hadd2(__floats2half2_rn(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), __floats2half2_rn(b0, b1));
+                    if (Ly.relu) h = __hmax2(h, __float2half2_rn(0.f));
+                    if (Ly.alpha_dot) { const float2 f = __half22float2(h); adot[e] = fmaf(f.x, __ldg(wa + col), adot[e]); adot[e] = fmaf(f.y, __ldg(wa + col + 1), adot[e]); }
                     *reinterpret_cast<__half2 *>(blk + nm_sw128(x.r0 + 8u * (uint32_t)e, (col & 63u) >> 3) + (col & 7u) * 2u) = h;
                 }
             }
@@ -180,13 +156,12 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
                     alpha[e] = adot[e] + __ldg(wa + 256);
                 }
             }
-            if constexpr (VER == 1 && L == 8) { alpha[0] = acc_a[0] + __ldg(b + 256); alpha[1] = acc_a[2] + __ldg(b + 256); }   // column 0 of the alpha head
         }
-        nm_layers<VER, MIP, L + 1>(x, P, tile, alpha);
+        nm_layers<MIP, L + 1>(x, P, tile, alpha);
     }
 }
 
-template <int VER, bool MIP>
+template <bool MIP>
 __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid_constant__ NmParams P) {
     extern __shared__ uint8_t dyn_smem[];
     constexpr int AUX = MIP ? 2 : 1;
@@ -210,11 +185,10 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
         if (warp == 8 && lane == 0) {
             uint32_t it = 0, n = 0;
             for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
-                if (VER >= 2) {   // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block)
-                    if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
-                    tc::mbar_expect_tx(enc_full, enc_bytes);
-                    tc::tma_bulk_g2s(A + 4 * NM_BLOCK, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
-                }
+                // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block)
+                if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
+                tc::mbar_expect_tx(enc_full, enc_bytes);
+                tc::tma_bulk_g2s(A + 4 * NM_BLOCK, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
                 size_t off = 0;
                 for (int l = 0; l < NM_LAYERS; ++l)
                     for (uint32_t s = 0; s < P.n_slabs[l]; ++s, ++it) {
@@ -235,55 +209,39 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     x.wg = threadIdx.x >> 7; x.t = threadIdx.x & 127; x.lane = lane; x.r0 = 64u * x.wg + tc::frag_row(x.t);
     uint32_t n = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
-        if (VER == 1) {
-            // stage my 64 rows of the fp32 encodings as fp16: point encoding -> blocks 4.., direction encoding -> last block (zero padded)
-            const int C = P.input_ch + P.input_ch_dirs;
-            for (int item = (int)x.t; item < 64 * (AUX + 1) * 8; item += 128) {
-                const int rl = item / ((AUX + 1) * 8), rem = item % ((AUX + 1) * 8), blk = rem >> 3, ch = rem & 7;
-                const uint32_t row = 64u * x.wg + (uint32_t)rl;
-                const int64_t i = tile * 128 + row;
-                const bool is_dir = blk == AUX;
-                const int width = is_dir ? P.input_ch_dirs : P.input_ch, c0 = is_dir ? P.input_ch : 0, k0 = (is_dir ? 0 : blk * 64) + ch * 8;
-                float v[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) v[q] = (i < P.n_rows && k0 + q < width) ? __ldg(P.embedded + (size_t)i * C + c0 + k0 + q) : 0.f;
-                *reinterpret_cast<uint4 *>(A + (size_t)(4 + blk) * NM_BLOCK + nm_sw128(row, ch)) = make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
-            }
-        } else {
-            tc::mbar_wait(enc_full, n & 1);
-        }
+        tc::mbar_wait(enc_full, n & 1);
         float alpha[2] = {0.f, 0.f};
-        nm_layers<VER, MIP, 0>(x, P, tile, alpha);
-        // (v2 / v3) views_linears.0 was the last reader of the encoding blocks: the producer may load the next tile's
-        if (VER >= 2) { __syncwarp(); if (lane == 0) tc::mbar_arrive(enc_free); }
+        nm_layers<MIP, 0>(x, P, tile, alpha);
+        // views_linears.0 was the last reader of the encoding blocks: the producer may load the next tile's
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(enc_free);
     }
 }
 
-template <int VER>
-static int nm_launch(const void *weight_image, const float *bias, const float *embedded, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
+static int nm_launch(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
     NmParams P{};
-    P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.embedded = embedded; P.enc_image = (const uint8_t *)enc_image;
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.enc_image = (const uint8_t *)enc_image;
     P.n_rows = n_rows; P.input_ch = input_ch; P.input_ch_dirs = input_ch_dirs; P.raw = raw;
     const bool mip = input_ch > 64;
     uint32_t max_bytes = 0;
     for (int l = 0; l < NM_LAYERS; ++l) {
-        const NmLayer L = mip ? nm_layer<VER, true>(l) : nm_layer<VER, false>(l);
+        const NmLayer L = mip ? nm_layer<true>(l) : nm_layer<false>(l);
         P.n_slabs[l] = (uint32_t)L.n_slabs;
         for (int k = 0; k < L.n_slabs; ++k) { P.slab_bytes[l][k] = nm_slab_bytes(L.s[k]); if (P.slab_bytes[l][k] > max_bytes) max_bytes = P.slab_bytes[l][k]; }
     }
     P.slot_bytes = (max_bytes + 1023) & ~1023u;
-    P.n_slots = VER == 1 ? 3 : 4;
+    P.n_slots = 4;
     const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * NM_BLOCK + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
     int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int64_t n_tiles = (n_rows + 127) / 128;
     const int grid = (int)(n_tiles < sms ? n_tiles : sms);
-    auto k = mip ? nerf_mlp_wg_kernel<VER, true> : nerf_mlp_wg_kernel<VER, false>;
+    auto k = mip ? nerf_mlp_wg_kernel<true> : nerf_mlp_wg_kernel<false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);
     return XRB_OK;
 }
 
-// ---- encoding tile images for v2 / v3: per 128-row tile, (aux+1) blocks of [128 x 64] fp16 in the wgmma layout (K-major, 128-byte swizzle),
+// ---- encoding tile images: per 128-row tile, (aux+1) blocks of [128 x 64] fp16 in the wgmma layout (K-major, 128-byte swizzle),
 // point-encoding block(s) first, direction block last, zero padded; written by fully coalesced 16-byte stores.
 __global__ void __launch_bounds__(256) pack_embedded_tiles_kernel(const float *__restrict__ embedded, int64_t n_rows, int ic, int icd, int aux, uint8_t *__restrict__ image) {
     const int chunks_per_row = (aux + 1) * 8;
@@ -346,44 +304,18 @@ extern "C" int xrb_internal_posenc_tiles_fast(const float *pts, const float *vie
 
 extern "C" {
 
-// weight image / bias layout are produced by the host (xrnerf_b200/nerf_mlp.py: pack_nerf_mlp) following the same NmPlan.
-int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream) {
+// image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp (in the order nm_layer streams the slabs); enc_image: the fp16 encoding tile image
+int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream) {
     XRB_REQUIRE(n_rows >= 0, "nerf_mlp_forward: negative size");
     if (!((input_ch == 63 && input_ch_dirs == 27) || (input_ch == 96 && input_ch_dirs == 27))) {
         set_error("nerf_mlp_forward: implemented for NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs) with (63,27) or (96,27) input channels");
         return XRB_E_UNSUPPORTED;
     }
     if (n_rows == 0) return XRB_OK;
-    XRB_REQUIRE(weight_image && bias && embedded && raw, "nerf_mlp_forward: null pointer");
-    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0, "nerf_mlp_forward: weight image / raw must be 16-byte aligned");
-    return nm_launch<1>(weight_image, bias, embedded, nullptr, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward");
-}
-
-// v2 entry (see the kernel comment); image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v2
-int xrb_nerf_mlp_forward_v2(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream) {
-    XRB_REQUIRE(n_rows >= 0, "nerf_mlp_forward_v2: negative size");
-    if (!((input_ch == 63 && input_ch_dirs == 27) || (input_ch == 96 && input_ch_dirs == 27))) {
-        set_error("nerf_mlp_forward_v2: implemented for NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs) with (63,27) or (96,27) input channels");
-        return XRB_E_UNSUPPORTED;
-    }
-    if (n_rows == 0) return XRB_OK;
-    XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward_v2: null pointer");
-    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0, "nerf_mlp_forward_v2: images / raw must be 16-byte aligned");
-    return nm_launch<2>(weight_image, bias, nullptr, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward_v2");
-}
-
-// v3 entry; image/bias from xrnerf_b200.nerf_mlp.pack_nerf_mlp_v3
-int xrb_nerf_mlp_forward_v3(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, void *stream) {
-    XRB_REQUIRE(n_rows >= 0, "nerf_mlp_forward_v3: negative size");
-    if (!((input_ch == 63 && input_ch_dirs == 27) || (input_ch == 96 && input_ch_dirs == 27))) {
-        set_error("nerf_mlp_forward_v3: implemented for NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs) with (63,27) or (96,27) input channels");
-        return XRB_E_UNSUPPORTED;
-    }
-    if (n_rows == 0) return XRB_OK;
-    XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward_v3: null pointer");
+    XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward: null pointer");
     XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0 && ((uintptr_t)bias & 15) == 0,
-                "nerf_mlp_forward_v3: images / bias / raw must be 16-byte aligned");
-    return nm_launch<3>(weight_image, bias, nullptr, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward_v3");
+                "nerf_mlp_forward: images / bias / raw must be 16-byte aligned");
+    return nm_launch(weight_image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward");
 }
 
 size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch) { return (size_t)((n_rows + 127) / 128) * ((input_ch + 63) / 64 + 1) * 16384; }

@@ -70,9 +70,6 @@ inline int check_cfg(const xrb_ngp_config *cfg) {
 // defined in ngp_mlp.cu: launches the field (impl 0 CUDA cores / 1 wgmma) on n rows; if n_dev != NULL the effective row
 // count is min(n, *n_dev) read on the device. table_setup validates an xrb_ngp_table and describes it for the device.
 int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g, const char *who);
-struct HashGridDev;
-int launch_field_ps(const xrb_ngp_config *cfg, const HashGridDev &g, const xrb_ngp_table *tab, const void *image, const float *pts, int pts_stride, const float *dirs, int dirs_stride, int n,
-                    const int32_t *n_dev, float *raw, cudaStream_t s);   // ngp_fused.cu: the producer/consumer shape of the field kernel
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
                  int dirs_stride, int n, const int32_t *n_dev, float *out, int impl, bool density_only, cudaStream_t s);
 

@@ -31,7 +31,9 @@ namespace xrb {
 constexpr uint32_t FR_ROW_BYTES = 80;                    // tile-slot row: 64 B = 32 fp16 features, 16 B = warped direction (3 floats) + pad
 constexpr uint32_t FR_SLOT_BYTES = 128 * FR_ROW_BYTES;   // 80-byte row stride is bank-conflict-free for 16-byte accesses
 constexpr uint32_t FR_TCAP = 64;                         // samples per ray per march round
-constexpr int FR_MAX_WG = 2;                             // field warpgroups per CTA: 2 (one 768-thread CTA per SM) or 1 (two 384-thread CTAs per SM)
+constexpr int FR_N_WG = 2;                               // field warpgroups per CTA
+constexpr int FR_N_PROD = 16;                            // producer warps per CTA (one 768-thread CTA per SM)
+constexpr int FR_N_SLOTS = 5;                            // tile slots
 
 struct FusedParams {
     HashGridDev g;
@@ -40,41 +42,35 @@ struct FusedParams {
     float lo, hi, near_distance, cone; Pcg32 rng;
     float bg[3]; int rgb_act, dens_act;
     float *rgb_out; float *alpha_out; int32_t *n_samples_out;
-    float *tscratch;     // [gridDim.x * N_PROD][32][FR_TCAP]
+    float *tscratch;     // [gridDim.x * FR_N_PROD][32][FR_TCAP]
     uint32_t *sched;     // [0] next ray group, [1] CTAs finished (both zero between launches)
     unsigned long long *dbg_out;   // [gridDim.x][16]: start ns, end ns, smid, tiles, 5 field-phase (warpgroup 0) and 7 producer-phase cycle sums (only written when dbg & 8)
     int dbg;             // developer ablation bits (XRB_FUSED_DBG): 1 skip the hash gather, 2 skip the MLP layers, 4 fake march (11 samples/ray)
-    // FIELD-ONLY mode (xrb_ngp_mlp_forward, shape 4): the producers read sample rows instead of marching and write raw instead of compositing
-    int field_only; const float *pts; int pts_stride; const float *dirs; int dirs_stride; int n_samples; const int32_t *n_dev; float4 *raw_out;
 };
 
-template <int FR_N_WG, int N_PROD, int N_SLOTS>
 struct FusedCtl {
-    uint64_t full[N_SLOTS];         // count 4: one arrival per chunk (producer lane 0, or the closing field thread for a skipped quarter)
-    uint64_t mail[N_PROD][2];       // count 32: the 32 field threads holding a producer's rows; a producer's chunk k uses mailbox k & 1
+    uint64_t full[FR_N_SLOTS];            // count 4: one arrival per chunk (producer lane 0, or the closing field thread for a skipped quarter)
+    uint64_t mail[FR_N_PROD][2];          // count 32: the 32 field threads holding a producer's rows; a producer's chunk k uses mailbox k & 1
     uint64_t wbar;
-    uint32_t rounds_done[N_SLOTS];  // slot s may be written for round r once rounds_done[s] >= r (set when its rows have been copied out)
-    uint32_t owner[N_SLOTS][4];     // (producer index << 1 | mailbox parity) of each quarter
+    uint32_t rounds_done[FR_N_SLOTS];     // slot s may be written for round r once rounds_done[s] >= r (set when its rows have been copied out)
+    uint32_t owner[FR_N_SLOTS][4];        // (producer index << 1 | mailbox parity) of each quarter
     uint32_t issued_bcast[FR_N_WG];
     uint32_t ticket, closed, done, prod_done;
-    uint32_t morton[128];           // expand_bits7 table for the occupancy test (common.cuh morton_lut_init)
+    uint32_t morton[128];                 // expand_bits7 table for the occupancy test (common.cuh morton_lut_init)
 };
-template <int FR_N_WG, int N_PROD, int N_SLOTS>
 __host__ __device__ inline size_t fused_smem_bytes(uint32_t image_bytes) {
-    return 1024 + image_bytes + (size_t)FR_N_WG * (16384 + TC_STAGE_BYTES) + (size_t)N_SLOTS * FR_SLOT_BYTES + (size_t)N_PROD * 1024 + sizeof(FusedCtl<FR_N_WG, N_PROD, N_SLOTS>) + 64;
+    return 1024 + image_bytes + (size_t)FR_N_WG * (16384 + TC_STAGE_BYTES) + (size_t)FR_N_SLOTS * FR_SLOT_BYTES + (size_t)FR_N_PROD * 1024 + sizeof(FusedCtl) + 64;
 }
 
 __device__ __forceinline__ void spin_until_ge(volatile uint32_t *p, uint32_t v) {
     while (*p < v) __nanosleep(20);
 }
 
-template <int FR_N_WG, int N_PROD, int N_SLOTS>
-__global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_render_fused_kernel(const __grid_constant__ FusedParams P) {
+__global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_fused_kernel(const __grid_constant__ FusedParams P) {
     extern __shared__ uint8_t dyn_smem[];
-    using Ctl = FusedCtl<FR_N_WG, N_PROD, N_SLOTS>;
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *W = base, *A = W + P.image_bytes, *stage = A + (size_t)FR_N_WG * 16384, *slots = stage + (size_t)FR_N_WG * TC_STAGE_BYTES, *mailbox = slots + (size_t)N_SLOTS * FR_SLOT_BYTES;
-    Ctl *ctl = (Ctl *)(mailbox + (size_t)N_PROD * 1024);
+    uint8_t *W = base, *A = W + P.image_bytes, *stage = A + (size_t)FR_N_WG * 16384, *slots = stage + (size_t)FR_N_WG * TC_STAGE_BYTES, *mailbox = slots + (size_t)FR_N_SLOTS * FR_SLOT_BYTES;
+    FusedCtl *ctl = (FusedCtl *)(mailbox + (size_t)FR_N_PROD * 1024);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if ((P.dbg & 8) && threadIdx.x == 0) {
         unsigned long long t0; uint32_t smid;
@@ -83,8 +79,8 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
     }
 
     if (threadIdx.x == 0) {
-        for (int k = 0; k < N_SLOTS; ++k) { tc::mbar_init(ctl->full + k, 4); ctl->rounds_done[k] = 0; }
-        for (int k = 0; k < N_PROD; ++k) { tc::mbar_init(&ctl->mail[k][0], 32); tc::mbar_init(&ctl->mail[k][1], 32); }
+        for (int k = 0; k < FR_N_SLOTS; ++k) { tc::mbar_init(ctl->full + k, 4); ctl->rounds_done[k] = 0; }
+        for (int k = 0; k < FR_N_PROD; ++k) { tc::mbar_init(&ctl->mail[k][0], 32); tc::mbar_init(&ctl->mail[k][1], 32); }
         for (int k = 0; k < FR_N_WG; ++k) ctl->issued_bcast[k] = 0;
         tc::mbar_init(&ctl->wbar, 1);
         ctl->ticket = 0; ctl->closed = 0; ctl->done = 0; ctl->prod_done = 0;
@@ -110,7 +106,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
 #define FTICK(k) do { } while (0)
 #endif
         for (uint32_t X = c.wg;; X += FR_N_WG) {
-            const uint32_t s = X % N_SLOTS, r = X / N_SLOTS;
+            const uint32_t s = X % FR_N_SLOTS, r = X / FR_N_SLOTS;
             FTICK(4);
             if (c.row == 0) {
                 volatile uint32_t *tk = &ctl->ticket; volatile uint32_t *dn = &ctl->done; volatile uint32_t *cl = &ctl->closed;
@@ -164,7 +160,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
     } else {
         // ===================================================================== producer warps
         const uint32_t pw = warp - 4 * FR_N_WG;
-        float *tb = P.tscratch + ((size_t)blockIdx.x * N_PROD + pw) * 32 * FR_TCAP;
+        float *tb = P.tscratch + ((size_t)blockIdx.x * FR_N_PROD + pw) * 32 * FR_TCAP;
         const float diag = sub_(P.hi, P.lo);
         uint32_t n_submitted = 0;   // chunks this warp has submitted so far (chunk k: mailbox k & 1, phase (k >> 1) & 1)
         long long pc[7] = {0, 0, 0, 0, 0, 0, 0}, ck = 0; (void)ck;
@@ -178,7 +174,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
             uint32_t tk = 0;
             if (lane == 0) tk = atomicAdd(&ctl->ticket, 1u);
             tk = __shfl_sync(0xffffffffu, tk, 0);
-            const uint32_t X = tk >> 2, sub = tk & 3, s = X % N_SLOTS, r = X / N_SLOTS;
+            const uint32_t X = tk >> 2, sub = tk & 3, s = X % FR_N_SLOTS, r = X / FR_N_SLOTS;
             if (lane == 0) { spin_until_ge(&ctl->rounds_done[s], r); __threadfence_block(); ctl->owner[s][sub] = (pw << 1) | (n_submitted & 1); }
             __syncwarp();
             PTICK(5);
@@ -208,38 +204,6 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(ctl->full + s);
         };
-        if (P.field_only) {
-            // ---- FIELD-ONLY producers: 32-sample chunks from a global counter; lane = sample. The results of chunk k come back through the mailbox while
-            // chunk k+1 is being gathered, exactly as in the render mode.
-            int n = P.n_samples;
-            if (P.n_dev) n = min(n, max(*P.n_dev, 0));
-            bool pending = false, prev_valid = false; int prev_q = 0;
-            // chunks are dealt out statically (warp w of the grid takes chunks w, w + W, ...): uniform work, no scheduler word, no workspace
-            const uint32_t n_pw = gridDim.x * N_PROD;
-            for (uint32_t chunk = blockIdx.x * N_PROD + pw;; chunk += n_pw) {
-                const bool have_chunk = (uint64_t)chunk * 32 < (uint64_t)n;
-                int q = 0; bool valid = false;
-                if (have_chunk) {
-                    q = (int)(chunk * 32u + lane); valid = q < n;
-                    float x = 0.5f, y = 0.5f, z = 0.5f, wd0 = 0.5f, wd1 = 0.5f, wd2 = 0.5f;
-                    if (valid) {
-                        const float *c = P.pts + (size_t)q * P.pts_stride, *d = P.dirs + (size_t)q * P.dirs_stride;
-                        x = __ldg(c); y = __ldg(c + 1); z = __ldg(c + 2); wd0 = __ldg(d); wd1 = __ldg(d + 1); wd2 = __ldg(d + 2);
-                    }
-                    submit_chunk(x, y, z, wd0, wd1, wd2);
-                }
-                if (pending) {
-                    const uint32_t kprev = n_submitted - 1;
-                    if (lane == 0) tc::mbar_wait(&ctl->mail[pw][kprev & 1], (kprev >> 1) & 1);
-                    __syncwarp();
-                    const float4 raw = *reinterpret_cast<const float4 *>(mailbox + (size_t)((pw << 1) | (kprev & 1)) * 512 + lane * 16);
-                    if (prev_valid) P.raw_out[prev_q] = raw;
-                    pending = false;
-                }
-                if (!have_chunk) break;
-                ++n_submitted; pending = true; prev_q = q; prev_valid = valid;
-            }
-        } else
         for (;;) {
             PTICK(6);
             uint32_t grp = 0;
@@ -369,42 +333,18 @@ __global__ void __launch_bounds__((4 * FR_N_WG + N_PROD) * 32, 3 - FR_N_WG) ngp_
         if ((P.dbg & 8) && lane == 0) { for (int k = 0; k < 7; ++k) atomicAdd(P.dbg_out + 16 * blockIdx.x + 9 + k, (unsigned long long)pc[k]); }
         if (lane == 0) {
             __threadfence_block();
-            if (atomicAdd(&ctl->prod_done, 1u) == N_PROD - 1) *(volatile uint32_t *)&ctl->done = 1u;
+            if (atomicAdd(&ctl->prod_done, 1u) == FR_N_PROD - 1) *(volatile uint32_t *)&ctl->done = 1u;
         }
     }
     __syncthreads();
     if ((P.dbg & 8) && threadIdx.x == 0) { unsigned long long t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); P.dbg_out[16 * blockIdx.x + 1] = t1; }
-    if (threadIdx.x == 0 && !P.field_only) {   // leave the scheduler words zero for the next launch
+    if (threadIdx.x == 0) {   // leave the scheduler words zero for the next launch
         __threadfence();
         if (atomicAdd(P.sched + 1, 1u) == gridDim.x - 1) { P.sched[0] = 0; P.sched[1] = 0; __threadfence(); }
     }
 }
 
 constexpr int FUSED_MAX_PROD_PER_SM = 24;
-// variant 0: one CTA per SM = 2 field warpgroups + 16 producers, 5 tile slots; variant 1: two CTAs per SM, each 1 field warpgroup + 8 producers,
-// 3 tile slots (batches on different streams then share every SM: the tail of one render overlaps the head of the next)
-static int fused_variant() { static int v = -1; if (v < 0) { const char *e = getenv("XRB_FUSED_VARIANT"); v = e ? atoi(e) : 0; if (v != 0 && v != 1) v = 0; } return v; }
-
-// FIELD-ONLY launch of the same kernel (HashNerfMLP.run_mlp): 16 producer warps per SM gather while the two field warpgroups run the MLPs on the tensor core, so the memory
-// phase and the tensor phase of different tiles overlap (in ngp_field_tc_kernel every warpgroup alternates between them and the ablation shows the sum: 130 + 52 us)
-int launch_field_ps(const xrb_ngp_config *cfg, const HashGridDev &g, const xrb_ngp_table *tab, const void *image, const float *pts, int pts_stride, const float *dirs, int dirs_stride, int n,
-                    const int32_t *n_dev, float *raw, cudaStream_t s) {
-    FusedParams P{};
-    P.g = g;
-    P.table = (const __half2 *)tab->table_fp16; P.cells = (const uint8_t *)tab->cell_image; P.np = plan_valid(P.g, tab->n_packed_levels) ? tab->n_packed_levels : 0;
-    P.weight_image = image; P.image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-    P.density_hidden = cfg->density_hidden; P.color_hidden = cfg->color_hidden;
-    P.field_only = 1; P.pts = pts; P.pts_stride = pts_stride; P.dirs = dirs; P.dirs_stride = dirs_stride; P.n_samples = n; P.n_dev = n_dev; P.raw_out = (float4 *)raw;
-    { static const int dbg = getenv("XRB_FUSED_DBG") ? atoi(getenv("XRB_FUSED_DBG")) : 0; P.dbg = dbg & 3; }
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    auto k = ngp_render_fused_kernel<2, 16, 5>;
-    const size_t smem = fused_smem_bytes<2, 16, 5>(P.image_bytes);
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    const int64_t n_chunks = ((int64_t)n + 31) / 32;
-    int grid = sms; if (n_chunks < (int64_t)grid * 16) grid = (int)((n_chunks + 15) / 16); if (grid < 1) grid = 1;
-    k<<<grid, (4 * 2 + 16) * 32, smem, s>>>(P);
-    return check_launch("ngp_mlp_forward (producer/consumer)");
-}
 
 }  // namespace xrb
 
@@ -439,17 +379,10 @@ int xrb_ngp_render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
     P.sched = (uint32_t *)workspace; P.tscratch = (float *)((uint8_t *)workspace + 256);
     P.dbg_out = (unsigned long long *)((uint8_t *)workspace + 256 + (size_t)sms * FUSED_MAX_PROD_PER_SM * 32 * FR_TCAP * sizeof(float));
     const int64_t n_groups = ((int64_t)n_rays + 31) / 32;
-    P.field_only = 0; P.pts = nullptr; P.dirs = nullptr; P.pts_stride = P.dirs_stride = 0; P.n_samples = 0; P.n_dev = nullptr; P.raw_out = nullptr;
-#define XRB_LAUNCH_FUSED(NWG, NP, NS)                                                                                                                  \
-    do {                                                                                                                                               \
-        auto k = ngp_render_fused_kernel<NWG, NP, NS>;                                                                                                 \
-        const size_t smem = fused_smem_bytes<NWG, NP, NS>(P.image_bytes);                                                                              \
-        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   /* per call: the attribute is per device and per image size */ \
-        int grid = sms * (3 - NWG); if (n_groups < grid) grid = (int)n_groups;                                                                         \
-        k<<<grid, (4 * NWG + NP) * 32, smem, (cudaStream_t)stream>>>(P);                                                                               \
-    } while (0)
-    if (fused_variant() == 1) XRB_LAUNCH_FUSED(1, 8, 3); else XRB_LAUNCH_FUSED(2, 16, 5);
-#undef XRB_LAUNCH_FUSED
+    const size_t smem = fused_smem_bytes(P.image_bytes);
+    cudaFuncSetAttribute(ngp_render_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // per call: the attribute is per device and per image size
+    int grid = sms; if (n_groups < grid) grid = (int)n_groups;
+    ngp_render_fused_kernel<<<grid, (4 * FR_N_WG + FR_N_PROD) * 32, smem, (cudaStream_t)stream>>>(P);
     return check_launch("ngp_render_fused");
 }
 

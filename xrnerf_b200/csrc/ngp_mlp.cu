@@ -158,25 +158,26 @@ __global__ void __launch_bounds__(128) mlp_forward_simt_kernel(const __half *__r
 }
 
 // ---------------------------------------------------------------------------- tensor-core field (impl 1)
-// NWG warpgroups (= concurrent 128-sample tiles) per CTA share ONE resident weight image; accumulators live in registers (tc_field.cuh).
-// The gather is latency-bound, so the shapes trade registers per
-// thread for warps per SM:   <2,96> / <2,128>: two CTAs per SM (16 warps);  <6,80>: one CTA per SM, 24 warps;  <8,64>: one CTA per SM, 32 warps.
+// FIELD_NWG warpgroups (= concurrent 128-sample tiles) per CTA share ONE resident weight image; accumulators live in registers (tc_field.cuh).
+// The gather is latency-bound; two CTAs per SM (16 warps), which caps a thread at 128 registers, is the fastest shape measured and the only one
+// without spills (DESIGN §4.1 has the sweep).
 // NP: static gather plan (ngp_field.cuh plan_mode): 0 = per-level form decided at run time, >0 = levels [0,NP) from the cell image, the rest hashed.
-// Per tile a warpgroup gathers the 16 levels, then runs both nets; the two to four warpgroups of an SM overlap one's gather with another's tensor-core layers.
-// ABLATE: the developer ablation (XRB_FIELD_DBG, launched only at shape <2,128>; the production instantiations do not carry it): dbg bit 0 = 1 replaces the
+// Per tile a warpgroup gathers the 16 levels, then runs both nets; the four warpgroups of an SM overlap one's gather with another's tensor-core layers.
+// ABLATE: the developer ablation (XRB_FIELD_DBG; the production instantiations do not carry it): dbg bit 0 = 1 replaces the
 // gather by position bits, bit 1 = 2 skips the MLP layers.
-template <bool DENSITY_ONLY, int NWG, int MAXREG, int NP, bool ABLATE>
-__global__ void __launch_bounds__(128 * NWG, NWG == 2 ? 2 : 1) __maxnreg__(MAXREG)
+constexpr int FIELD_NWG = 2;
+template <bool DENSITY_ONLY, int NP, bool ABLATE>
+__global__ void __launch_bounds__(128 * FIELD_NWG, 2)
 ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image, uint32_t image_bytes, int density_hidden,
                     int color_hidden, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride, int n, const int32_t *__restrict__ n_dev,
                     float *__restrict__ out, int dbg) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     if (!ABLATE) dbg = 0;
-    TcWarpgroup c = tc_cta_setup<NWG>(dyn_smem, weight_image, image_bytes);
+    TcWarpgroup c = tc_cta_setup<FIELD_NWG>(dyn_smem, weight_image, image_bytes);
     const WeightImageLayout L = weight_image_layout(density_hidden, color_hidden);
     const int n_tiles = (n + 127) / 128;
-    for (int tile = blockIdx.x * NWG + c.wg; tile < n_tiles; tile += gridDim.x * NWG) {
+    for (int tile = blockIdx.x * FIELD_NWG + c.wg; tile < n_tiles; tile += gridDim.x * FIELD_NWG) {
         const int i = tile * 128 + c.row;
         const bool valid = i < n;
         float x = 0.5f, y = 0.5f, z = 0.5f, dx = 0.5f, dy = 0.5f, dz = 0.5f;
@@ -345,36 +346,26 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
                                                                  dirs, dirs_stride, n, n_dev, out);
     } else {
         uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-        // kernel shape (see ngp_field_tc_kernel): XRB_TC_SHAPE = 0 <2 WG, 96 regs>, 1 <2,128> (default), 2 <6,80>, 3 <8,64>, 4 the producer/consumer kernel. Measured
-        // with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us with <2,128>
-        // (ptxas: 128 registers, 0 spill bytes), 296 us with <2,96>, 343 us with <6,80>, 646 us with <8,64> (all three spill), 277 us with shape 4.
-        static const int env_shape = getenv("XRB_TC_SHAPE") ? atoi(getenv("XRB_TC_SHAPE")) : -1;
-        static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) & 3 : 0;
-        const int shape = (env_shape >= 0 && !dbg) ? env_shape : 1;   // the ablation runs at <2,128> only (impl 2 is a synonym of impl 1)
-        // shape 4: the producer/consumer kernel (ngp_fused.cu in FIELD-ONLY mode): gather warps and tensor-core warpgroups are different warps
-        if (shape == 4 && !density_only && (((uintptr_t)out) & 15) == 0) return launch_field_ps(cfg, g, tab, image, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, s);
+        // Measured with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us
+        // (ptxas: 128 registers, 0 spill bytes).
+        static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) & 3 : 0;   // developer ablation (impl 2 is a synonym of impl 1)
         // static gather plan: the kernel is specialised for "levels [0,NP) packed, all others hashed" (NP = 6, 7); anything else takes the run-time form
         const int npl = tab->n_packed_levels;
         const int np = (plan_valid(g, npl) && (npl == 6 || npl == 7)) ? npl : 0;
-        int n_tiles = (n + 127) / 128;
-#define XRB_LAUNCH_TC(D, NWG, R, NP)                                                                                                                \
+        const int n_tiles = (n + 127) / 128;
+        const size_t smem = tc_cta_smem_bytes<FIELD_NWG>(image_bytes);
+#define XRB_LAUNCH_TC(D, NP)                                                                                                                        \
     do {                                                                                                                                            \
-        auto k = dbg ? ngp_field_tc_kernel<D, 2, 128, NP, true> : ngp_field_tc_kernel<D, NWG, R, NP, false>;                                        \
-        const size_t smem = tc_cta_smem_bytes<NWG>(image_bytes);                                                                                    \
+        auto k = dbg ? ngp_field_tc_kernel<D, NP, true> : ngp_field_tc_kernel<D, NP, false>;                                                        \
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                                                            \
-        int grid = persistent_grid((const void *)k, 128 * NWG, smem, (n_tiles + NWG - 1) / NWG, NWG == 2 ? 2 : 1);                                  \
-        k<<<grid, 128 * NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, dbg); \
+        int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);                               \
+        k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, dbg); \
     } while (0)
-#define XRB_LAUNCH_TC_NP(D, NWG, R)                                                                                                                 \
+#define XRB_LAUNCH_TC_NP(D)                                                                                                                         \
     do {                                                                                                                                            \
-        if (np == 6) XRB_LAUNCH_TC(D, NWG, R, 6); else if (np == 7) XRB_LAUNCH_TC(D, NWG, R, 7); else XRB_LAUNCH_TC(D, NWG, R, 0);                   \
+        if (np == 6) XRB_LAUNCH_TC(D, 6); else if (np == 7) XRB_LAUNCH_TC(D, 7); else XRB_LAUNCH_TC(D, 0);                                         \
     } while (0)
-#define XRB_LAUNCH_TC_SHAPE(D)                                                                                                                      \
-    do {                                                                                                                                            \
-        if (shape == 0) XRB_LAUNCH_TC_NP(D, 2, 96); else if (shape == 2) XRB_LAUNCH_TC_NP(D, 6, 80); else if (shape == 3) XRB_LAUNCH_TC_NP(D, 8, 64); else XRB_LAUNCH_TC_NP(D, 2, 128); \
-    } while (0)
-        if (density_only) XRB_LAUNCH_TC_SHAPE(true); else XRB_LAUNCH_TC_SHAPE(false);
-#undef XRB_LAUNCH_TC_SHAPE
+        if (density_only) XRB_LAUNCH_TC_NP(true); else XRB_LAUNCH_TC_NP(false);
 #undef XRB_LAUNCH_TC_NP
 #undef XRB_LAUNCH_TC
     }

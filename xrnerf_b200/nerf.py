@@ -26,8 +26,7 @@ class NerfRenderer:
         _C.check(_C.lib.xrb_nerf_posenc_tiles_rays(_C.ptr(rays_o), _C.ptr(rays_d), _C.ptr(z), _C.ptr(viewdirs), n, s, self.multires, self.multires_dirs, _C.ptr(enc), _C.stream()),
                  'posenc_tiles_rays')
         image, bias = mlp._packed()
-        assert mlp.kernel_version in (2, 3)
-        return nerf_mlp_forward_tiles(image, bias, enc, rows, mlp.input_ch, mlp.input_ch_dirs, version=mlp.kernel_version).view(n, s, 4)
+        return nerf_mlp_forward_tiles(image, bias, enc, rows, mlp.input_ch, mlp.input_ch_dirs).view(n, s, 4)
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, viewdirs):
@@ -66,8 +65,7 @@ class MipNerfRenderer:
         enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(rows, mlp.input_ch), dtype=torch.uint8, device=z.device)
         _C.check(_C.lib.xrb_mip_ipe_tiles_rays(_C.ptr(z), _C.ptr(rays_o), _C.ptr(rays_d), _C.ptr(radii), _C.ptr(viewdirs), n, s, *self.degs, _C.ptr(enc), _C.stream()), 'mip_ipe_tiles_rays')
         image, bias = mlp._packed()
-        assert mlp.kernel_version in (2, 3)
-        return nerf_mlp_forward_tiles(image, bias, enc, rows, mlp.input_ch, mlp.input_ch_dirs, version=mlp.kernel_version).view(n, s, 4)
+        return nerf_mlp_forward_tiles(image, bias, enc, rows, mlp.input_ch, mlp.input_ch_dirs).view(n, s, 4)
 
     @torch.no_grad()
     def render(self, rays_o, rays_d, viewdirs, radii):

@@ -1,6 +1,6 @@
 """Host side of the fused wgmma NerfMLP (csrc/nerf_mlp_tc.cu): packs the nn.Linear weights of the reference-shaped NerfMLP
-(/root/reference/xrnerf/models/mlps/nerf_mlp.py:29-49) into the kernel's weight image — a sequence of [N x 64] fp16 slabs, K-major,
-128-byte swizzled, in the exact order the kernel's TMA producer streams them — and the fp32 bias vector."""
+(/root/reference/xrnerf/models/mlps/nerf_mlp.py:29-49) into the kernel's weight image — fp16 slabs, K-major, in the exact order the kernel's
+TMA producer streams them — and its bias vector, and runs the kernel on the fp16 encoding tile image of the rows."""
 import numpy as np
 import torch
 
@@ -29,99 +29,6 @@ def _pad_cols(w, k0, k1):
     return blk
 
 
-def pack_nerf_mlp(mlp):
-    """mlp: registry NerfMLP (netdepth 8, netwidth 256, skips [4], use_viewdirs). Returns (image u8 cuda, bias f32 cuda)."""
-    assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256, \
-        'fused NerfMLP kernel: netdepth=8, netwidth=256, skips=[4], use_viewdirs=True'
-    ic, icd = mlp.input_ch, mlp.input_ch_dirs
-    aux = (ic + 63) // 64
-    g = lambda lin: (lin.weight.detach().float().cpu().numpy(), lin.bias.detach().float().cpu().numpy())
-    slabs, biases = [], []
-    W, b = g(mlp.pts_linears[0])
-    for kb in range(aux):
-        slabs.append(_slab(_pad_cols(W, kb * 64, (kb + 1) * 64)))
-    biases.append(b)
-    for l in range(1, 8):
-        W, b = g(mlp.pts_linears[l])
-        if l == 5:   # input = cat([input_pts(ic), h(256)]) -> image K order [h | pts]
-            for kb in range(4):
-                slabs.append(_slab(_pad_cols(W, ic + kb * 64, ic + (kb + 1) * 64)))
-            for kb in range(aux):
-                slabs.append(_slab(_pad_cols(W[:, :ic], kb * 64, (kb + 1) * 64)))
-        else:
-            for kb in range(4):
-                slabs.append(_slab(_pad_cols(W, kb * 64, (kb + 1) * 64)))
-        biases.append(b)
-    Wf, bf = g(mlp.feature_linear)
-    Wa, ba = g(mlp.alpha_linear)
-    Wfa = np.zeros((272, 256), np.float32); Wfa[:256] = Wf; Wfa[256] = Wa[0]
-    for kb in range(4):
-        slabs.append(_slab(_pad_cols(Wfa, kb * 64, (kb + 1) * 64)))
-    biases += [bf, np.concatenate([ba, np.zeros(15, np.float32)])]
-    Wv, bv = g(mlp.views_linears[0])                     # [128, 256 + icd] on cat([feature, input_views])
-    for kb in range(4):
-        slabs.append(_slab(_pad_cols(Wv, kb * 64, (kb + 1) * 64)))
-    slabs.append(_slab(_pad_cols(Wv[:, 256:], 0, 64)))
-    biases.append(bv)
-    Wr, br = g(mlp.rgb_linear)
-    Wr16 = np.zeros((16, 128), np.float32); Wr16[:3] = Wr
-    for kb in range(2):
-        slabs.append(_slab(_pad_cols(Wr16, kb * 64, (kb + 1) * 64)))
-    biases.append(np.concatenate([br, np.zeros(13, np.float32)]))
-    dev = mlp.pts_linears[0].weight.device
-    image = torch.from_numpy(np.concatenate(slabs)).to(dev)
-    bias = torch.from_numpy(np.concatenate(biases).astype(np.float32)).to(dev)
-    return image, bias
-
-
-def pack_nerf_mlp_v2(mlp):
-    """Image for csrc/nerf_mlp_tc.cu v2: HALF slabs ([N/2 x 64]) in the kernel's MMA issue order
-    S1=(half0; aux+lo blocks) S2=(half1; aux+lo) S3=(half0; hi blocks) S4=(half1; hi); bias vector = per-layer biases, then Wa[256], ba."""
-    assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256
-    ic, icd = mlp.input_ch, mlp.input_ch_dirs
-    aux = (ic + 63) // 64
-    g = lambda lin: (lin.weight.detach().float().cpu().numpy(), lin.bias.detach().float().cpu().numpy())
-    PTS, DIR = 'pts', 'dir'
-
-    def cols(W, kind, j, h_off=0, pts_w=None):
-        """64 weight columns feeding A block (kind, j): hidden block j -> W[:, h_off+64j ..]; pts block j -> pts part; dir -> W[:, 256:]"""
-        if kind == 'h':
-            return _pad_cols(W, h_off + 64 * j, h_off + 64 * (j + 1))
-        if kind == PTS:
-            return _pad_cols(pts_w, 64 * j, 64 * (j + 1))
-        return _pad_cols(W[:, 256:], 0, 64)
-
-    layers = []   # (W_padded_rows [N, ...], first blocks, second blocks, N, n_halves, bias)
-    W, b = g(mlp.pts_linears[0])
-    layers.append((W, [(PTS, j, dict(pts_w=W)) for j in range(aux)], [], 256, 2, b))
-    for l in range(1, 8):
-        W, b = g(mlp.pts_linears[l])
-        if l == 5:
-            first = [(PTS, j, dict(pts_w=W[:, :ic])) for j in range(aux)] + [('h', 0, dict(h_off=ic)), ('h', 1, dict(h_off=ic))]
-            second = [('h', 2, dict(h_off=ic)), ('h', 3, dict(h_off=ic))]
-        else:
-            first, second = [('h', 0, {}), ('h', 1, {})], [('h', 2, {}), ('h', 3, {})]
-        layers.append((W, first, second, 256, 2, b))
-    W, b = g(mlp.feature_linear)
-    layers.append((W, [('h', 0, {}), ('h', 1, {})], [('h', 2, {}), ('h', 3, {})], 256, 2, b))
-    W, b = g(mlp.views_linears[0])
-    layers.append((W, [(DIR, 0, {}), ('h', 0, {}), ('h', 1, {})], [('h', 2, {}), ('h', 3, {})], 128, 2, b))
-    Wr, br = g(mlp.rgb_linear)
-    W16 = np.zeros((16, 128), np.float32); W16[:3] = Wr
-    layers.append((W16, [('h', 0, {})], [('h', 1, {})], 16, 1, np.concatenate([br, np.zeros(13, np.float32)])))
-    slabs, biases = [], []
-    for (W, first, second, N, nh, b) in layers:
-        hw = N // nh
-        for (kind, j, kw) in first + second:        # stream order: per K-block, output half 0 then half 1 (one ring per issuer)
-            for half in range(nh):
-                slabs.append(_slab(cols(W, kind, j, **kw)[half * hw:(half + 1) * hw]))
-        biases.append(b.astype(np.float32))
-    Wa, ba = g(mlp.alpha_linear)
-    biases += [Wa[0].astype(np.float32), ba.astype(np.float32)]
-    dev = mlp.pts_linears[0].weight.device
-    return torch.from_numpy(np.concatenate(slabs)).to(dev), torch.from_numpy(np.concatenate(biases)).to(dev)
-
-
 def _slab64(w_rows_by_32):
     """[N,32] float32 -> K-major SWIZZLE_64B bytes (N*64): element (n,k) -> (n>>3)*512 + (n&7)*64 + (((k>>3) ^ ((n>>1)&3))<<4) + (k&7)*2"""
     n = w_rows_by_32.shape[0]
@@ -135,10 +42,12 @@ def _slab64(w_rows_by_32):
     return out.reshape(-1).view(np.uint8)
 
 
-def pack_nerf_mlp_v3(mlp):
-    """Image for the v3 entry of csrc/nerf_mlp_tc.cu: 16 KB slabs in the kernel's stream order — per layer, per K-block (the point / direction block first where a layer reads it):
+def pack_nerf_mlp(mlp):
+    """mlp: registry NerfMLP (netdepth 8, netwidth 256, skips [4], use_viewdirs). Returns (image u8, bias f32) on the module's device.
+    Image: 16 KB slabs in the kernel's stream order — per layer, per K-block (the point / direction block first where a layer reads it):
     the 256-wide layers as two K-halves [256 x 32] (SWIZZLE_64B), views_linears.0 / rgb_linear as one [N x 64] slab (SWIZZLE_128B). Bias vector: fp32 per-layer biases, Wa[256], ba, padded to 8 floats, then an fp16 copy of the per-layer biases."""
-    assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256
+    assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256, \
+        'fused NerfMLP kernel: netdepth=8, netwidth=256, skips=[4], use_viewdirs=True'
     ic, icd = mlp.input_ch, mlp.input_ch_dirs
     aux = (ic + 63) // 64
     assert aux in (1, 2)
@@ -183,27 +92,22 @@ def pack_nerf_mlp_v3(mlp):
     return torch.from_numpy(np.concatenate(slabs)).to(dev), torch.from_numpy(np.concatenate([f32, h16.view(np.float32)])).to(dev)
 
 
-def nerf_mlp_forward(image, bias, embedded, input_ch, input_ch_dirs, version=1):
+def nerf_mlp_forward(image, bias, embedded, input_ch, input_ch_dirs):
+    """fp32 embedded rows [n, input_ch + input_ch_dirs] -> raw [n, 4]: packs the fp16 encoding tile image (one streaming kernel), then runs the MLP kernel,
+    which TMA-loads it. image/bias come from pack_nerf_mlp."""
     _C.require_cuda(image, bias, embedded)
     embedded = embedded.contiguous().float()
     n = embedded.shape[0]
     raw = torch.empty((n, 4), dtype=torch.float32, device=embedded.device)
-    if version >= 2:   # fp32 embedded -> fp16 tile image (one streaming kernel) -> MLP kernel that TMA-loads it
-        enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(n, int(input_ch)), dtype=torch.uint8, device=embedded.device)
-        _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(embedded), n, int(input_ch), int(input_ch_dirs), _C.ptr(enc), _C.stream()), 'nerf_pack_embedded')
-        return nerf_mlp_forward_tiles(image, bias, enc, n, input_ch, input_ch_dirs, raw, version=version)
-    fn = _C.lib.xrb_nerf_mlp_forward
-    _C.check(fn(_C.ptr(image), _C.ptr(bias), _C.ptr(embedded), n, int(input_ch), int(input_ch_dirs), _C.ptr(raw), _C.stream()), 'nerf_mlp_forward')
-    return raw
+    enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(n, int(input_ch)), dtype=torch.uint8, device=embedded.device)
+    _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(embedded), n, int(input_ch), int(input_ch_dirs), _C.ptr(enc), _C.stream()), 'nerf_pack_embedded')
+    return nerf_mlp_forward_tiles(image, bias, enc, n, input_ch, input_ch_dirs, raw)
 
 
-def nerf_mlp_forward_tiles(image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw=None, version=2):
-    """v2 / v3 kernel on an already packed encoding tile image (xrb_nerf_pack_embedded / xrb_nerf_posenc_tiles / xrb_mip_ipe_tiles_rays);
-    image/bias must come from the matching packer (pack_nerf_mlp_v2 / pack_nerf_mlp_v3)."""
+def nerf_mlp_forward_tiles(image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw=None):
+    """The MLP kernel on an already packed encoding tile image (xrb_nerf_pack_embedded / xrb_nerf_posenc_tiles / xrb_mip_ipe_tiles_rays);
+    image/bias come from pack_nerf_mlp."""
     if raw is None:
         raw = torch.empty((n_rows, 4), dtype=torch.float32, device=enc_image.device)
-    if version == 3:
-        _C.check(_C.lib.xrb_nerf_mlp_forward_v3(_C.ptr(image), _C.ptr(bias), _C.ptr(enc_image), n_rows, int(input_ch), int(input_ch_dirs), _C.ptr(raw), _C.stream()), 'nerf_mlp_forward_v3')
-        return raw
-    _C.check(_C.lib.xrb_nerf_mlp_forward_v2(_C.ptr(image), _C.ptr(bias), _C.ptr(enc_image), n_rows, int(input_ch), int(input_ch_dirs), _C.ptr(raw), _C.stream()), 'nerf_mlp_forward_v2')
+    _C.check(_C.lib.xrb_nerf_mlp_forward(_C.ptr(image), _C.ptr(bias), _C.ptr(enc_image), n_rows, int(input_ch), int(input_ch_dirs), _C.ptr(raw), _C.stream()), 'nerf_mlp_forward')
     return raw

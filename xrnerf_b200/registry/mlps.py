@@ -63,12 +63,10 @@ class NerfMLP(BaseMLP):
                 and self.pts_linears[0].out_features == 256 and (self.input_ch, self.input_ch_dirs) in ((63, 27), (96, 27)))
 
     def _packed(self):
-        import os
-        self.kernel_version = int(os.environ.get('XRB_NERF_MLP_V', '3'))
-        ver = tuple(p._version for p in self.parameters()) + (self.pts_linears[0].weight.device, self.kernel_version)
+        ver = tuple(p._version for p in self.parameters()) + (self.pts_linears[0].weight.device,)
         if getattr(self, '_pack_ver', None) != ver:
-            from ..nerf_mlp import pack_nerf_mlp, pack_nerf_mlp_v2, pack_nerf_mlp_v3
-            self._pack = {1: pack_nerf_mlp, 2: pack_nerf_mlp_v2, 3: pack_nerf_mlp_v3}[self.kernel_version](self)
+            from ..nerf_mlp import pack_nerf_mlp
+            self._pack = pack_nerf_mlp(self)
             self._pack_ver = ver
         return self._pack
 
@@ -76,7 +74,7 @@ class NerfMLP(BaseMLP):
         if self._fused_ok(x):   # inference: the whole 12-GEMM chain in one wgmma kernel, no chunking needed (activations never leave the SM)
             from ..nerf_mlp import nerf_mlp_forward
             image, bias = self._packed()
-            return nerf_mlp_forward(image, bias, x, self.input_ch, self.input_ch_dirs, version=self.kernel_version)
+            return nerf_mlp_forward(image, bias, x, self.input_ch, self.input_ch_dirs)
         if self.fused and getattr(self, 'fused_train', True) and torch.is_grad_enabled() and x.is_cuda and any(p.requires_grad for p in self.parameters()):
             from .. import nerf_train
             if nerf_train.supported(self):   # training: every dense layer forward + backward as wgmma kernels over fp16 tile images (csrc/nerf_train.cu), one autograd node
