@@ -242,9 +242,14 @@ int xrb_ngp_huber5_grad(const float *rgb, const float *target, int64_t n_element
  *   hashnerf_render.py:42-46) without materialising coords[S,7] or raw[S,4] in HBM.
  * rays_o/rays_d f32[N,3]; rgb f32[N,3]; alpha f32[N]; numsteps i32[N,2] (count, base) is also produced;
  * counters i32[2] as in xrb_rm_rays_sampler (counters[1] = total samples marched).
- * workspace: xrb_ngp_render_workspace(N, max_samples) bytes.
- * ev_before_field / ev_after_field: optional cudaEvent_t handles (NULL = none) recorded on `stream` right before / after the field
- * kernel, so a caller can time the dominant kernel live inside its own timed region (no library-global state).
+ * Up to 2^21 samples, the field evaluates the marched samples bucketed by position (a counting sort on a 64^3 Morton grid, on the
+ * device), not in ray order; every output row is bit-identical to a ray-order evaluation. Larger sample counts are evaluated in ray order.
+ * workspace: xrb_ngp_render_workspace(N, max_samples) bytes, 256-byte aligned. It starts with the march workspace, rounded up to
+ * 256 bytes, followed by coords f32[max_samples,7], raw f32[max_samples,4] and the field's evaluation order u32[max_samples]
+ * (when n = min(counters[1], max_samples) <= 2^21, order[0, n) is a permutation of the rows [0, n)).
+ * ev_before_field / ev_after_field: optional cudaEvent_t handles (NULL = none) recorded on `stream` right before the sample-ordering
+ * kernels and right after the field kernel, so a caller can time the ordering plus the dominant kernel live inside its own timed
+ * region (no library-global state).
  * ---------------------------------------------------------------------------------------------- */
 size_t xrb_ngp_render_workspace(int n_rays, int max_samples);
 int xrb_ngp_render(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield,

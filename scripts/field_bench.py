@@ -1,5 +1,7 @@
 """Isolated timings of the NGP chain's kernels on one 65 536-ray batch (CUDA events, L2 flushed between repetitions):
-march (count+scan+emit), field (per gather plan), composite, and the single-launch kernel.  python scripts/field_bench.py [n_packed ...]"""
+march (count+scan+emit), field (per gather plan), composite, and the single-launch kernel; then, per kernel (torch.profiler), the cost of
+ordering the samples by position against the field on the same samples in ray order and in bucket order.
+python scripts/field_bench.py [n_packed ...]"""
 import os
 import sys
 import numpy as np
@@ -66,4 +68,41 @@ for npk in plans:
     med, mn = timed(lambda i: r.render_fused(*batches[i % 8], bf))
     print('   fused single launch: median %.1f us min %.1f us' % (med, mn))
     med, mn = timed(lambda i: r.render(*batches[i % 8], bf))
-    print('   chain (5 launches, sequential): median %.1f us min %.1f us' % (med, mn))
+    print('   chain (sequential launches): median %.1f us min %.1f us' % (med, mn))
+    if npk != plans[-1]:
+        continue
+    # the same samples (same RNG call index) through the field in ray order (run_mlp on the march's rows) and inside the chain (bucket order)
+    def per_kernel(fn, reps=10):
+        from torch.profiler import profile, ProfilerActivity
+        for i in range(2):
+            fn(i)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for i in range(reps):
+                flush.zero_()
+                fn(i)
+            torch.cuda.synchronize()
+        return {e.key: e.device_time_total / reps for e in prof.key_averages() if e.device_time_total > 0}
+
+    def ray_order(i):
+        rm.reset_rng(ray_sampler=i)
+        march(i)
+        flush.zero_()
+        n = min(int(cnt[1].item()), cap)
+        f.run_mlp(coords[:n, :3], coords[:n, 4:])
+
+    def bucket_order(i):
+        r.calls = i
+        r.render(*batches[i % 8], bf)
+
+    name = lambda k, sub: [v for key, v in k.items() if sub in key]
+    ka, kb = per_kernel(ray_order), per_kernel(bucket_order)
+    print('   per kernel, us per batch (torch.profiler, L2 flushed before each batch):')
+    for label, sub in (('memset (bucket counts, counters)', 'Memset'), ('order_key_kernel', 'order_key_kernel'), ('order_chunk_sum_kernel', 'order_chunk_sum_kernel'),
+                       ('order_scan_kernel', 'order_scan_kernel'), ('order_scatter_kernel', 'order_scatter_kernel')):
+        print('      %-34s %7.1f' % (label, sum(name(kb, sub))))
+    order_us = sum(sum(name(kb, sub)) for sub in ('order_key_kernel', 'order_chunk_sum_kernel', 'order_scan_kernel', 'order_scatter_kernel'))
+    fa, fb = sum(name(ka, 'ngp_field_tc_kernel')), sum(name(kb, 'ngp_field_tc_kernel'))
+    print('      ordering kernels total              %7.1f' % order_us)
+    print('      field, ray order                    %7.1f' % fa)
+    print('      field, bucket order                 %7.1f  (ordering + field %.1f, %.2fx the ray-order field)' % (fb, order_us + fb, fa / (order_us + fb)))

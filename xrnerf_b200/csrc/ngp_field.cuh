@@ -67,11 +67,18 @@ inline int check_cfg(const xrb_ngp_config *cfg) {
     return XRB_OK;
 }
 
+// Sample order of the chain render (ngp_render.cu): the field evaluates the rows bucketed by position only while there are at most this many.
+// Beyond that the 28-byte sample rows no longer fit in L2, and reading and writing them in permuted order through HBM costs more than the
+// coherent hash gather saves (measured: 0.7 M- and 1.8 M-sample batches faster, 6.5 M-sample whole 800x800 images slower; DESIGN.md §4.1).
+constexpr uint32_t SAMPLE_ORDER_MAX_ROWS = 1u << 21;
+
 // defined in ngp_mlp.cu: launches the field (impl 0 CUDA cores / 1 wgmma) on n rows; if n_dev != NULL the effective row
-// count is min(n, *n_dev) read on the device. table_setup validates an xrb_ngp_table and describes it for the device.
+// count is min(n, *n_dev) read on the device. order (impl 1, full field only; NULL = row order): a permutation of the effective rows, evaluated
+// in that order (tile slot j reads and writes row order[j]); ignored when there are more than SAMPLE_ORDER_MAX_ROWS effective rows.
+// table_setup validates an xrb_ngp_table and describes it for the device.
 int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g, const char *who);
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
-                 int dirs_stride, int n, const int32_t *n_dev, float *out, int impl, bool density_only, cudaStream_t s);
+                 int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s);
 
 #ifdef __CUDACC__
 __device__ __forceinline__ float round_h(float x) { return __half2float(__float2half_rn(x)); }

@@ -170,16 +170,18 @@ template <bool DENSITY_ONLY, int NP, bool ABLATE>
 __global__ void __launch_bounds__(128 * FIELD_NWG, 2)
 ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image, uint32_t image_bytes, int density_hidden,
                     int color_hidden, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride, int n, const int32_t *__restrict__ n_dev,
-                    float *__restrict__ out, int dbg) {
+                    const uint32_t *__restrict__ order, float *__restrict__ out, int dbg) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
+    if (n > (int)SAMPLE_ORDER_MAX_ROWS) order = nullptr;
     if (!ABLATE) dbg = 0;
     TcWarpgroup c = tc_cta_setup<FIELD_NWG>(dyn_smem, weight_image, image_bytes);
     const WeightImageLayout L = weight_image_layout(density_hidden, color_hidden);
     const int n_tiles = (n + 127) / 128;
     for (int tile = blockIdx.x * FIELD_NWG + c.wg; tile < n_tiles; tile += gridDim.x * FIELD_NWG) {
-        const int i = tile * 128 + c.row;
-        const bool valid = i < n;
+        const int j = tile * 128 + c.row;
+        const bool valid = j < n;
+        const int i = !DENSITY_ONLY && valid && order ? (int)__ldg(order + j) : j;   // the row this tile slot evaluates: the rows of a tile are independent
         float x = 0.5f, y = 0.5f, z = 0.5f, dx = 0.5f, dy = 0.5f, dz = 0.5f;
         if (valid) {
             const float *p = pts + (size_t)i * pts_stride; x = p[0]; y = p[1]; z = p[2];
@@ -330,9 +332,10 @@ int xrb_tcnn_mlp_forward(const void *params_fp16, const void *x_fp16, int n, int
 }  // extern "C"
 namespace xrb {
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
-                 int dirs_stride, int n, const int32_t *n_dev, float *out, int impl, bool density_only, cudaStream_t s) {
+                 int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s) {
     HashGridDev g; int e = table_setup(cfg, tab, &g, "field"); if (e) return e;
     const void *table = tab->table_fp16; const uint8_t *cells = (const uint8_t *)tab->cell_image;
+    XRB_REQUIRE(impl != 0 || order == nullptr, "field: an evaluation order needs the tensor-core field");
     if (impl == 0) {
         size_t smem = (mlp_num_params(32, 64, cfg->density_hidden, 16) + (density_only ? 0 : mlp_num_params(32, 64, cfg->color_hidden, 16))) * sizeof(__half);
         const void *k = density_only ? (const void *)ngp_field_simt_kernel<true> : (const void *)ngp_field_simt_kernel<false>;
@@ -359,7 +362,7 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
         auto k = dbg ? ngp_field_tc_kernel<D, NP, true> : ngp_field_tc_kernel<D, NP, false>;                                                        \
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                                                            \
         int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);                               \
-        k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, out, dbg); \
+        k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, order, out, dbg); \
     } while (0)
 #define XRB_LAUNCH_TC_NP(D)                                                                                                                         \
     do {                                                                                                                                            \
@@ -382,7 +385,7 @@ int xrb_ngp_mlp_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, c
     XRB_REQUIRE(table && pts && dirs && raw, "ngp_mlp_forward: null pointer");
     XRB_REQUIRE(((uintptr_t)raw & 15) == 0, "ngp_mlp_forward: raw must be 16-byte aligned");
     XRB_REQUIRE(impl == 0 ? (density_fp16 && color_fp16) : (weight_image != nullptr), "ngp_mlp_forward: missing weights for the requested impl");
-    return launch_field(cfg, table, density_fp16, color_fp16, weight_image, pts, pts_stride, dirs, dirs_stride, n, n_rows_dev, raw, impl, false, (cudaStream_t)stream);
+    return launch_field(cfg, table, density_fp16, color_fp16, weight_image, pts, pts_stride, dirs, dirs_stride, n, n_rows_dev, nullptr, raw, impl, false, (cudaStream_t)stream);
 }
 
 int xrb_ngp_density_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const void *weight_image, const float *pts, int pts_stride, int n, float *density,
@@ -392,7 +395,7 @@ int xrb_ngp_density_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *tabl
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(table && pts && density, "ngp_density_forward: null pointer");
     XRB_REQUIRE(impl == 0 ? (density_fp16 != nullptr) : (weight_image != nullptr), "ngp_density_forward: missing weights for the requested impl");
-    return launch_field(cfg, table, density_fp16, nullptr, weight_image, pts, pts_stride, nullptr, 3, n, nullptr, density, impl, true, (cudaStream_t)stream);
+    return launch_field(cfg, table, density_fp16, nullptr, weight_image, pts, pts_stride, nullptr, 3, n, nullptr, nullptr, density, impl, true, (cudaStream_t)stream);
 }
 
 }  // extern "C"
