@@ -1,4 +1,4 @@
-"""Isolated timing of the NGP field backward (wgmma) on the samples of one 65 536-ray batch.  python scripts/bwd_bench.py"""
+"""Isolated timing of the NGP field backward (wgmma) on the samples of one 65 536-ray batch.  python scripts/bwd_bench.py [n_packed]"""
 import os
 import sys
 import numpy as np
@@ -17,7 +17,7 @@ coords = torch.zeros((cap, 7), device=dev); ridx = torch.zeros((N, 1), dtype=tor
 rm.rays_sampler_api(o, d, bf, None, None, None, 0.0, 1.0, 0.05, 1.0 / 256, coords, ridx, ns, cnt)
 S = int(cnt[1].item())
 c = coords[:S]
-f = NgpField(n_packed_levels=int(os.environ.get('XRB_PACKED_LEVELS', '6'))).to(dev)
+f = NgpField(n_packed_levels=int(sys.argv[1]) if len(sys.argv) > 1 else 6).to(dev)
 f.refresh()
 draw = torch.randn((S, 4), device=dev) * 1e-3
 out = (torch.zeros_like(f.hash_params), torch.zeros_like(f.density_params), torch.zeros_like(f.color_params))
@@ -29,4 +29,4 @@ for i in range(8):
     e0.record(); f.backward_params(c[:, :3], c[:, 4:], draw, out=out, impl=int(os.environ.get('BWD_IMPL', '1'))); e1.record(); torch.cuda.synchronize()
     if i >= 2:
         ts.append(e0.elapsed_time(e1) * 1e3)
-print('field backward impl=%s dbg=%s: %d samples, median %.1f us min %.1f us' % (os.environ.get('BWD_IMPL', '1'), os.environ.get('XRB_BWD_DBG', '0'), S, np.median(ts), min(ts)), flush=True)
+print('field backward impl=%s: %d samples, median %.1f us min %.1f us' % (os.environ.get('BWD_IMPL', '1'), S, np.median(ts), min(ts)), flush=True)

@@ -59,7 +59,7 @@ for npk in plans:
     print('n_packed=%d: cell image %.2f GB' % (npk, (f._cells.numel() if f._cells is not None else 0) / 1e9), flush=True)
     c = coords[:S]
     med, mn = timed(lambda i: f.run_mlp(c[:, :3], c[:, 4:]))
-    print('field n_packed=%d dbg=%s: median %.1f us min %.1f us -> %.0f GB/s algorithmic (556 B/sample)' % (npk, os.environ.get('XRB_FIELD_DBG', '0'), med, mn, S * 556 / med / 1e3), flush=True)
+    print('field n_packed=%d: median %.1f us min %.1f us -> %.0f GB/s algorithmic (556 B/sample)' % (npk, med, mn, S * 556 / med / 1e3), flush=True)
     if os.environ.get('XRB_FIELD_ONLY'):
         continue
     med, mn = timed(lambda i: f.rebuild_cells())

@@ -1,4 +1,4 @@
-"""A few fused NGP training steps (for ncu launch lists / quick timing).  python scripts/train_probe.py [steps]"""
+"""A few fused NGP training steps (for ncu launch lists / quick timing).  python scripts/train_probe.py [steps] [n_packed]"""
 import os
 import sys
 import torch
@@ -13,7 +13,7 @@ K = int(sys.argv[1]) if len(sys.argv) > 1 else 6
 bf = torch.from_numpy(synth.bitfield_from_grid_numpy(synth.lego_like_density_grid(0))[0]).to(dev)
 NB = int(os.environ.get('NB', '4'))
 batches = [tuple(torch.from_numpy(x).to(dev) for x in synth.ray_batch(N, seed=b)[:2]) for b in range(NB)]
-f = NgpField(n_packed_levels=int(os.environ.get('XRB_PACKED_LEVELS', '6'))).to(dev)
+f = NgpField(n_packed_levels=int(sys.argv[2]) if len(sys.argv) > 2 else 6).to(dev)
 PRE = int(os.environ.get('PRE', '0'))
 if PRE:
     from xrnerf_b200.ngp import NgpRenderer

@@ -126,8 +126,9 @@ def _mip_rays(n, seed):
     return o, d, torch.nn.functional.normalize(d, dim=-1), torch.full((n, 1), 1.2e-3, device='cuda')
 
 
-def test_mip_ipe_tile_image_is_the_fp16_rounding_of_mip_embed(monkeypatch):
-    """xrb_mip_ipe_tiles_rays == xrb_nerf_pack_embedded(xrb_mip_embed(...)) byte for byte (same fp32 expressions, one fp16 rounding); ragged last tile."""
+def test_mip_ipe_tile_images_are_the_fp16_rounding_of_mip_embed():
+    """xrb_mip_ipe_tiles_rays == xrb_nerf_pack_embedded(xrb_mip_embed(...)) byte for byte (same fp32 expressions, one fp16 rounding); ragged last tile.
+    Degrees (0, 16, 0, 4) take the specialised kernel, (0, 16, 0, 3) the generic one."""
     from xrnerf_b200 import _C
     n, s = 37, 19                         # 703 rows: 5 full tiles + a ragged one
     o, d, vd, radii = _mip_rays(n, 4)
@@ -140,15 +141,18 @@ def test_mip_ipe_tile_image_is_the_fp16_rounding_of_mip_embed(monkeypatch):
     _C.check(_C.lib.xrb_mip_ipe_tiles_rays(_C.ptr(z), _C.ptr(o), _C.ptr(d), _C.ptr(radii.reshape(-1)), _C.ptr(vd), n, s, 0, 16, 0, 4, _C.ptr(b), _C.stream()))
     assert nbytes == 6 * 3 * 16384
     assert torch.equal(a.view(torch.float16), b.view(torch.float16))      # as fp16 VALUES: where exp(-y_var/2) < 2^-25 the specialised kernel writes +0 without evaluating sin (may be -0 above)
-    monkeypatch.setenv('XRB_GENERIC_ENCODERS', '1')                        # the generic-degree kernel: byte for byte
+    emb3 = torch.empty((n * s, 117), device='cuda')                        # the generic-degree kernel: byte for byte
+    _C.check(_C.lib.xrb_mip_embed(_C.ptr(z), _C.ptr(o), _C.ptr(d), _C.ptr(radii.reshape(-1)), _C.ptr(vd), n, s, 0, 16, 0, 3, _C.ptr(emb3), None, None, _C.stream()))
+    a3 = torch.zeros(nbytes, dtype=torch.uint8, device='cuda')
+    _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb3), n * s, 96, 21, _C.ptr(a3), _C.stream()))
     c = torch.full((nbytes,), 0x5A, dtype=torch.uint8, device='cuda')
-    _C.check(_C.lib.xrb_mip_ipe_tiles_rays(_C.ptr(z), _C.ptr(o), _C.ptr(d), _C.ptr(radii.reshape(-1)), _C.ptr(vd), n, s, 0, 16, 0, 4, _C.ptr(c), _C.stream()))
-    assert torch.equal(a, c)
+    _C.check(_C.lib.xrb_mip_ipe_tiles_rays(_C.ptr(z), _C.ptr(o), _C.ptr(d), _C.ptr(radii.reshape(-1)), _C.ptr(vd), n, s, 0, 16, 0, 3, _C.ptr(c), _C.stream()))
+    assert torch.equal(a3, c)
 
 
-def test_posenc_tile_images_match_fp32_posenc(monkeypatch):
-    """xrb_nerf_posenc_tiles / _rays (specialised multires 10/4 kernel and the generic one) == fp16 rounding of xrb_nerf_posenc on pts = o + d*z formed
-    by torch (GetPts). The specialised kernel uses sincosf where the fp32 kernel uses sinf / cosf: allow 1 fp16 ulp on < 0.1 % of the entries."""
+def test_posenc_tile_images_match_fp32_posenc():
+    """xrb_nerf_posenc_tiles / _rays (specialised multires 10/4 kernel, and the generic one at 10/3) == fp16 rounding of xrb_nerf_posenc on pts = o + d*z
+    formed by torch (GetPts). The specialised kernel uses sincosf where the fp32 kernel uses sinf / cosf: allow 1 fp16 ulp on < 0.1 % of the entries."""
     from xrnerf_b200 import _C
     n, s = 29, 21
     g = torch.Generator(device='cuda').manual_seed(9)
@@ -156,21 +160,21 @@ def test_posenc_tile_images_match_fp32_posenc(monkeypatch):
     vd = torch.nn.functional.normalize(d, dim=-1)
     z = (2.0 + 4.0 * torch.rand((n, s), device='cuda', generator=g)).sort(dim=-1).values.contiguous()
     pts = (o[:, None, :] + d[:, None, :] * z[:, :, None]).contiguous()
-    emb = torch.empty((n * s, 90), device='cuda')
-    _C.check(_C.lib.xrb_nerf_posenc(_C.ptr(pts), _C.ptr(vd), n * s, s, 10, 4, _C.ptr(emb), _C.stream()))
     nbytes = _C.lib.xrb_nerf_enc_image_bytes(n * s, 63)
-    ref = torch.zeros(nbytes, dtype=torch.uint8, device='cuda')
-    _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb), n * s, 63, 27, _C.ptr(ref), _C.stream()))
-    ref16 = ref.view(torch.float16).float()
     for generic in (False, True):
-        if generic:
-            monkeypatch.setenv('XRB_GENERIC_ENCODERS', '1')
+        multires_dirs = 3 if generic else 4                                 # 10/4 takes the specialised kernel, 10/3 the generic one
+        input_ch_dirs = 3 + 6 * multires_dirs
+        emb = torch.empty((n * s, 63 + input_ch_dirs), device='cuda')
+        _C.check(_C.lib.xrb_nerf_posenc(_C.ptr(pts), _C.ptr(vd), n * s, s, 10, multires_dirs, _C.ptr(emb), _C.stream()))
+        ref = torch.zeros(nbytes, dtype=torch.uint8, device='cuda')
+        _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb), n * s, 63, input_ch_dirs, _C.ptr(ref), _C.stream()))
+        ref16 = ref.view(torch.float16).float()
         for ray_mode in (False, True):
             img = torch.full((nbytes,), 0xA5, dtype=torch.uint8, device='cuda')
             if ray_mode:
-                _C.check(_C.lib.xrb_nerf_posenc_tiles_rays(_C.ptr(o), _C.ptr(d), _C.ptr(z), _C.ptr(vd), n, s, 10, 4, _C.ptr(img), _C.stream()))
+                _C.check(_C.lib.xrb_nerf_posenc_tiles_rays(_C.ptr(o), _C.ptr(d), _C.ptr(z), _C.ptr(vd), n, s, 10, multires_dirs, _C.ptr(img), _C.stream()))
             else:
-                _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.ptr(pts), _C.ptr(vd), n * s, s, 10, 4, _C.ptr(img), _C.stream()))
+                _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.ptr(pts), _C.ptr(vd), n * s, s, 10, multires_dirs, _C.ptr(img), _C.stream()))
             got = img.view(torch.float16).float()
             diff = (got - ref16).abs()
             assert diff.max().item() <= 1e-3, (generic, ray_mode)             # one fp16 ulp below 1.0 is 4.9e-4

@@ -2,7 +2,6 @@
 // render call, a full sort + expanded gathers per sample_pdf call; SURVEY §3a): one launch each, one WARP per ray,
 // lanes over samples with shuffle scans. References relative to /root/reference/xrnerf/models/.
 #include "common.cuh"
-#include <stdlib.h>
 
 namespace xrb {
 
@@ -638,8 +637,8 @@ int xrb_mip_ipe_tiles_rays(const float *z_vals, const float *rays_o, const float
     XRB_REQUIRE(z_vals && rays_o && rays_d && radii && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "mip_ipe_tiles_rays: null/misaligned pointer");
     const int aux = (6 * (max_deg_point - min_deg_point) + 63) / 64;
     int64_t total = ((n_rays * n_samples + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    if (max_deg_point - min_deg_point == 16 && max_deg_view - min_deg_view == 4 && min_deg_point >= -100 && max_deg_point <= 100 && min_deg_view >= -100 && max_deg_view <= 100 &&
-        !getenv("XRB_GENERIC_ENCODERS")) {                     // the reference configuration (configs/mipnerf/*.py): specialised kernel
+    if (max_deg_point - min_deg_point == 16 && max_deg_view - min_deg_view == 4 && min_deg_point >= -100 && max_deg_point <= 100 && min_deg_view >= -100 && max_deg_view <= 100) {
+        // the reference configuration (configs/mipnerf/*.py): specialised kernel
         int64_t items = ((n_rays * n_samples + 127) / 128) * 256, fb = (items + 255) / 256; if (fb > NUM_SMS * 16) fb = NUM_SMS * 16;
         mip_ipe_tiles_fast_kernel<16, 4><<<(int)fb, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, min_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
         return check_launch("mip_ipe_tiles_rays");

@@ -21,7 +21,6 @@
 #include "tc.cuh"
 #include "common.cuh"
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 namespace xrb {
 
@@ -334,7 +333,7 @@ int xrb_nerf_posenc_tiles(const float *pts, const float *viewdirs, int64_t n_pts
     XRB_REQUIRE(n_pts >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles: bad size");
     if (n_pts == 0) return XRB_OK;
     XRB_REQUIRE(pts && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles: null/misaligned pointer");
-    if (multires == 10 && multires_dirs == 4 && !getenv("XRB_GENERIC_ENCODERS")) return xrb_internal_posenc_tiles_fast(pts, viewdirs, n_pts, samples_per_ray, enc_image, nullptr, nullptr, stream);
+    if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(pts, viewdirs, n_pts, samples_per_ray, enc_image, nullptr, nullptr, stream);
     const int aux = (3 + 6 * multires + 63) / 64;
     int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
     posenc_tiles_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, nullptr, nullptr);
@@ -346,7 +345,7 @@ int xrb_nerf_posenc_tiles_rays(const float *rays_o, const float *rays_d, const f
     XRB_REQUIRE(n_rays >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles_rays: bad size");
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(rays_o && rays_d && z_vals && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles_rays: null/misaligned pointer");
-    if (multires == 10 && multires_dirs == 4 && !getenv("XRB_GENERIC_ENCODERS")) return xrb_internal_posenc_tiles_fast(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, enc_image, rays_o, rays_d, stream);
+    if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, enc_image, rays_o, rays_d, stream);
     const int aux = (3 + 6 * multires + 63) / 64;
     const int64_t n_pts = n_rays * samples_per_ray;
     int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;

@@ -18,8 +18,6 @@
 // Shared memory: weight image + 2 x (ENC, H.., CIN, C.., dZ) tiles. Row-wise reads of accumulators (density outputs, dL/dcin, dL/dencoding) are
 // staged through a tile that is dead at that point (fp32 [128 x 16|32]).
 #include "tc_field.cuh"
-#include <stdio.h>
-#include <stdlib.h>
 
 namespace xrb {
 
@@ -193,9 +191,7 @@ template <int DH, int CH, int NP>
 __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
                                                                   uint32_t image_bytes, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride,
                                                                   const float4 *__restrict__ dl_draw, int n, const int32_t *__restrict__ n_dev, float *__restrict__ d_table,
-                                                                  float *__restrict__ d_dens, float *__restrict__ d_color, int dbg, __half2 *__restrict__ genc_out) {
-    // dbg (developer ablation, XRB_BWD_DBG): 1 = no hash-gradient scatter, 2 = no gather (encoding := position bits), 4 = no tensor-core rounds,
-    // 8 = dL/d encoding written to genc_out (fp16 [n,32]) for a separate scatter kernel instead of the in-kernel atomics
+                                                                  float *__restrict__ d_dens, float *__restrict__ d_color) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     constexpr BtLayout T = bt_layout(DH, CH);
@@ -234,16 +230,12 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
             uint32_t e[4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                float2 f = (dbg & 2) ? make_float2(px, py) : hash_level(table, cells, g, 4 * q + k, px, py, pz, plan_mode<NP>(4 * q + k));
+                float2 f = hash_level(table, cells, g, 4 * q + k, px, py, pz, plan_mode<NP>(4 * q + k));
                 e[k] = pack_h2(f.x, f.y);
             }
             bt_store_chunk(c, T.enc, q, make_uint4(e[0], e[1], e[2], e[3]));
         }
         float genc[32];
-        if (dbg & 4) {
-#pragma unroll
-            for (int k = 0; k < 32; ++k) genc[k] = gr.x * (float)k;
-        } else {
         bt_fwd_hidden<32>(c, T.enc, L.d_in, T.h0);
 #pragma unroll
         for (int h = 1; h < DH; ++h) bt_fwd_hidden<64>(c, T.h0 + h - 1, L.d_hid[h - 1], T.h0 + h);
@@ -291,13 +283,8 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
             bt_bwd<64, 64, 0>(c, T.dz, T.h0 + k - 1, L.d_hid[k - 1], dw_dhid[k - 1], T.h0 + k - 1, 0, nullptr);
         bt_bwd<32, 64, 1>(c, T.dz, T.enc, L.d_in, dw_din, 0, T.enc, genc);      // dL/d encoding (scaled); ENC is dead after this round
         c.first = false;
-        }
-        if ((dbg & 8) && valid) {
-#pragma unroll
-            for (int q = 0; q < 16; ++q) genc_out[(size_t)i * 16 + q] = __floats2half2_rn(genc[2 * q], genc[2 * q + 1]);
-        }
         // ------------------------------------------------ hash-table gradient scatter
-        if (valid && !(dbg & 9)) {
+        if (valid) {
             // The scatter is bound by the LSU's reduction issue rate (~1.3 cycles per lane and RED, measured: 450 of 880 us per 700 K samples with 128 two-float
             // REDs per sample), so x-adjacent corners that are also adjacent in memory go out as ONE 16-byte red.global.add.v4.f32:
             //   hashed level: entries of (gx, y, z) and (gx^1, y, z) are the two halves of an aligned 16-byte pair -> even gx: 4 v4 instead of 8 v2
@@ -350,8 +337,6 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
     }
 }
 
-void launch_hashgrid_backward(const HashGridDev &g, const float *x, int x_stride, int n, const void *d_enc, float scale, float *d_table, cudaStream_t s);   // ngp_backward.cu
-
 template <int DH, int CH, int NP>
 static int launch_bwd_tc(const HashGridDev &g, const xrb_ngp_table *tab, const void *image, uint32_t image_bytes, const float *pts, int pts_stride, const float *dirs, int dirs_stride,
                          const float *dl_draw, int n, const int32_t *n_dev, float *d_table, float *d_dens, float *d_color, cudaStream_t s) {
@@ -360,12 +345,8 @@ static int launch_bwd_tc(const HashGridDev &g, const xrb_ngp_table *tab, const v
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int n_tiles = (n + 127) / 128, grid = sms; if (grid > (n_tiles + 1) / 2) grid = (n_tiles + 1) / 2; if (grid < 1) grid = 1;
-    static const int dbg = getenv("XRB_BWD_DBG") ? atoi(getenv("XRB_BWD_DBG")) : 0;
-    static __half2 *genc_dbg = nullptr;
-    if ((dbg & 8) && !genc_dbg) cudaMalloc(&genc_dbg, (size_t)(1 << 20) * 64);
     k<<<grid, 256, smem, s>>>(g, (const __half2 *)tab->table_fp16, (const uint8_t *)tab->cell_image, image, image_bytes, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev,
-                              d_table, d_dens, d_color, dbg, genc_dbg);
-    if (dbg & 8) launch_hashgrid_backward(g, pts, pts_stride, n, genc_dbg, 1.f / BT_SCALE, d_table, s);
+                              d_table, d_dens, d_color);
     return check_launch("ngp_mlp_backward_tc");
 }
 

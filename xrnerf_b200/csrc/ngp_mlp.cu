@@ -3,8 +3,6 @@
 // shared memory), impl 1 = wgmma tensor-core tiles (tc_field.cuh). Both follow the numeric contract in
 // oracle/tcnn_oracle.c (fp16 operands, fp32 accumulate, fp16 activations).
 #include "tc_field.cuh"
-#include <stdio.h>
-#include <stdlib.h>
 
 namespace xrb {
 
@@ -163,18 +161,15 @@ __global__ void __launch_bounds__(128) mlp_forward_simt_kernel(const __half *__r
 // without spills (DESIGN §4.1 has the sweep).
 // NP: static gather plan (ngp_field.cuh plan_mode): 0 = per-level form decided at run time, >0 = levels [0,NP) from the cell image, the rest hashed.
 // Per tile a warpgroup gathers the 16 levels, then runs both nets; the four warpgroups of an SM overlap one's gather with another's tensor-core layers.
-// ABLATE: the developer ablation (XRB_FIELD_DBG; the production instantiations do not carry it): dbg bit 0 = 1 replaces the
-// gather by position bits, bit 1 = 2 skips the MLP layers.
 constexpr int FIELD_NWG = 2;
-template <bool DENSITY_ONLY, int NP, bool ABLATE>
+template <bool DENSITY_ONLY, int NP>
 __global__ void __launch_bounds__(128 * FIELD_NWG, 2)
 ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image, uint32_t image_bytes, int density_hidden,
                     int color_hidden, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride, int n, const int32_t *__restrict__ n_dev,
-                    const uint32_t *__restrict__ order, float *__restrict__ out, int dbg) {
+                    const uint32_t *__restrict__ order, float *__restrict__ out) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     if (n > (int)SAMPLE_ORDER_MAX_ROWS) order = nullptr;
-    if (!ABLATE) dbg = 0;
     TcWarpgroup c = tc_cta_setup<FIELD_NWG>(dyn_smem, weight_image, image_bytes);
     const WeightImageLayout L = weight_image_layout(density_hidden, color_hidden);
     const int n_tiles = (n + 127) / 128;
@@ -187,25 +182,16 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
             const float *p = pts + (size_t)i * pts_stride; x = p[0]; y = p[1]; z = p[2];
             if (!DENSITY_ONLY) { const float *d = dirs + (size_t)i * dirs_stride; dx = d[0]; dy = d[1]; dz = d[2]; }
         }
+        uint32_t e[16];
+        tc_gather_levels<NP, 0, 16>(table, cells, g, x, y, z, e);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) a_store_chunk(c, q, make_uint4(e[4 * q], e[4 * q + 1], e[4 * q + 2], e[4 * q + 3]));
         float dout[16];
-        if (dbg & 2) {   // gather only (or neither)
-            float acc = x;
-            if (!(dbg & 1)) {
-#pragma unroll
-                for (int l = 0; l < 16; ++l) { const float2 f = hash_level(table, cells, g, l, x, y, z, plan_mode<NP>(l)); acc += f.x + f.y; }
-            }
-            for (int k = 0; k < 16; ++k) dout[k] = acc;
-        } else {
-            uint32_t e[16];
-            if (dbg & 1) { for (int l = 0; l < 16; ++l) e[l] = pack_h2(x + l, y - l); } else tc_gather_levels<NP, 0, 16>(table, cells, g, x, y, z, e);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) a_store_chunk(c, q, make_uint4(e[4 * q], e[4 * q + 1], e[4 * q + 2], e[4 * q + 3]));
-            tc_density_from_a(c, L, density_hidden, dout);
-        }
+        tc_density_from_a(c, L, density_hidden, dout);
         if (DENSITY_ONLY) {
             if (valid) out[i] = dout[0];
         } else {
-            const float4 raw = (dbg & 2) ? make_float4(dout[0], dout[1], dout[2], dout[3]) : tc_color_from_density(c, L, color_hidden, dout, dx, dy, dz);
+            const float4 raw = tc_color_from_density(c, L, color_hidden, dout, dx, dy, dz);
             if (valid) reinterpret_cast<float4 *>(out)[i] = raw;
         }
     }
@@ -213,9 +199,7 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
 
 static int persistent_grid(const void *kernel, int block, size_t smem, int work_ctas, int min_per_sm = 1) {
     int per_sm = 1;
-    cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem);
-    if (getenv("XRB_DEBUG")) fprintf(stderr, "[xrb] occupancy query: err=%d per_sm=%d block=%d smem=%zu\n", (int)oe, per_sm, block, smem);
-    if (oe != cudaSuccess) cudaGetLastError();
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem) != cudaSuccess) cudaGetLastError();
     if (per_sm < min_per_sm) per_sm = min_per_sm;  // the calculator has been seen to under-report; extra CTAs simply queue
     int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int g = sms * per_sm;
@@ -331,6 +315,18 @@ int xrb_tcnn_mlp_forward(const void *params_fp16, const void *x_fp16, int n, int
 
 }  // extern "C"
 namespace xrb {
+template <bool DENSITY_ONLY, int NP>
+static void launch_field_tc(const xrb_ngp_config *cfg, const HashGridDev &g, const void *table, const uint8_t *cells, const void *image, uint32_t image_bytes, const float *pts,
+                            int pts_stride, const float *dirs, int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, cudaStream_t s) {
+    auto k = ngp_field_tc_kernel<DENSITY_ONLY, NP>;
+    const size_t smem = tc_cta_smem_bytes<FIELD_NWG>(image_bytes);
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int n_tiles = (n + 127) / 128;
+    const int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);
+    k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, order,
+                                          out);
+}
+
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
                  int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s) {
     HashGridDev g; int e = table_setup(cfg, tab, &g, "field"); if (e) return e;
@@ -350,27 +346,13 @@ int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void
     } else {
         uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
         // Measured with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us
-        // (ptxas: 128 registers, 0 spill bytes).
-        static const int dbg = getenv("XRB_FIELD_DBG") ? atoi(getenv("XRB_FIELD_DBG")) & 3 : 0;   // developer ablation (impl 2 is a synonym of impl 1)
+        // (ptxas: 128 registers, 0 spill bytes). impl 2 is a synonym of impl 1.
         // static gather plan: the kernel is specialised for "levels [0,NP) packed, all others hashed" (NP = 6, 7); anything else takes the run-time form
         const int npl = tab->n_packed_levels;
         const int np = (plan_valid(g, npl) && (npl == 6 || npl == 7)) ? npl : 0;
-        const int n_tiles = (n + 127) / 128;
-        const size_t smem = tc_cta_smem_bytes<FIELD_NWG>(image_bytes);
-#define XRB_LAUNCH_TC(D, NP)                                                                                                                        \
-    do {                                                                                                                                            \
-        auto k = dbg ? ngp_field_tc_kernel<D, NP, true> : ngp_field_tc_kernel<D, NP, false>;                                                        \
-        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                                                            \
-        int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);                               \
-        k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, order, out, dbg); \
-    } while (0)
-#define XRB_LAUNCH_TC_NP(D)                                                                                                                         \
-    do {                                                                                                                                            \
-        if (np == 6) XRB_LAUNCH_TC(D, 6); else if (np == 7) XRB_LAUNCH_TC(D, 7); else XRB_LAUNCH_TC(D, 0);                                         \
-    } while (0)
-        if (density_only) XRB_LAUNCH_TC_NP(true); else XRB_LAUNCH_TC_NP(false);
-#undef XRB_LAUNCH_TC_NP
-#undef XRB_LAUNCH_TC
+        auto launch = density_only ? (np == 6 ? launch_field_tc<true, 6> : np == 7 ? launch_field_tc<true, 7> : launch_field_tc<true, 0>)
+                                   : (np == 6 ? launch_field_tc<false, 6> : np == 7 ? launch_field_tc<false, 7> : launch_field_tc<false, 0>);
+        launch(cfg, g, table, cells, image, image_bytes, pts, pts_stride, dirs, dirs_stride, n, n_dev, order, out, s);
     }
     return check_launch(density_only ? "ngp_density_forward" : "ngp_mlp_forward");
 }

@@ -11,7 +11,6 @@
 #include "common.cuh"
 #include <stdio.h>
 #include <string.h>
-#include <stdlib.h>
 
 namespace xrb {
 
@@ -73,12 +72,6 @@ __device__ __forceinline__ uint32_t march_ray(const float o[3], const float d[3]
 constexpr int MARCH_BLOCK = 128;
 // grid for warp-per-ray kernels with persistent (ray-strided) warps
 static inline int warp_grid(int n_rays) { size_t b = ((size_t)n_rays * 32 + 255) / 256, cap = (size_t)NUM_SMS * 8; return (int)(b < cap ? (b ? b : 1) : cap); }
-// The march is a long, divergent, latency-bound chain per ray (ncu r01: kernel time == the slowest warp's serialised union of 32
-// rays' paths). Only every LANE_STRIDE-th lane owns a ray: 4x more warps (the SMs have the slots: 14 -> 55 warps/SM at 65 536 rays),
-// each serialising 8 rays instead of 32.
-constexpr int MAX_LANE_STRIDE = 4;
-constexpr int MARCH_RAYS_PER_BLOCK_MIN = MARCH_BLOCK / MAX_LANE_STRIDE;
-static int lane_stride() { static int v = -1; if (v < 0) { const char *e = getenv("XRB_MARCH_LANE_STRIDE"); v = e ? atoi(e) : 1; if (v != 1 && v != 2 && v != 4) v = 1; } return v; }
 
 struct MarchWs {  // device workspace layout for N rays
     uint32_t *local_excl;  // [N]
@@ -90,14 +83,13 @@ struct MarchWs {  // device workspace layout for N rays
     float *ovf;            // [n_chunks][OVF_CAP]
     uint32_t n_chunks;
 };
+__host__ __device__ inline size_t march_n_blocks(int n) { return ((size_t)n + MARCH_BLOCK - 1) / MARCH_BLOCK; }   // count-pass blocks = block sums in the workspace
 __host__ __device__ inline uint32_t march_n_chunks(int n) { uint32_t c = (uint32_t)n / 8u; return c < 64u ? 64u : c; }   // every 8th ray may be longer than TCAP samples
 __host__ __device__ inline size_t march_ws_bytes(int n) {
-    size_t nb = (size_t)(n + MARCH_RAYS_PER_BLOCK_MIN - 1) / MARCH_RAYS_PER_BLOCK_MIN;
-    return sizeof(uint32_t) * ((size_t)n * 3 + nb + 16 + (size_t)n * TCAP + (size_t)march_n_chunks(n) * OVF_CAP);
+    return sizeof(uint32_t) * ((size_t)n * 3 + march_n_blocks(n) + 16 + (size_t)n * TCAP + (size_t)march_n_chunks(n) * OVF_CAP);
 }
 inline MarchWs march_ws(void *ws, int n) {
-    size_t nb = (size_t)(n + MARCH_RAYS_PER_BLOCK_MIN - 1) / MARCH_RAYS_PER_BLOCK_MIN;
-    MarchWs w; w.local_excl = (uint32_t *)ws; w.startt = (float *)(w.local_excl + n); w.block_sum = (uint32_t *)(w.startt + n); w.misc = w.block_sum + nb; w.tbuf = (float *)(w.misc + 16);
+    MarchWs w; w.local_excl = (uint32_t *)ws; w.startt = (float *)(w.local_excl + n); w.block_sum = (uint32_t *)(w.startt + n); w.misc = w.block_sum + march_n_blocks(n); w.tbuf = (float *)(w.misc + 16);
     w.chunk_of = (int32_t *)(w.tbuf + (size_t)n * TCAP); w.ovf = (float *)(w.chunk_of + n); w.n_chunks = march_n_chunks(n);
     return w;
 }
@@ -116,19 +108,17 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *total)
     return off + incl - v;
 }
 
-template <int LANE_STRIDE>
+// Count pass: thread i marches ray i, caching its sample t values, and the block scans the per-ray sample counts.
 __global__ void __launch_bounds__(MARCH_BLOCK) march_count_kernel(int n_rays, const float *__restrict__ rays_o, const float *__restrict__ rays_d,
                                                                   const uint8_t *__restrict__ bitfield, float lo, float hi, float near_distance, float cone,
                                                                   Pcg32 rng, uint32_t *__restrict__ local_excl, float *__restrict__ startt_out,
                                                                   uint32_t *__restrict__ block_sum, int32_t *__restrict__ numsteps, float *__restrict__ tbuf, OvfPool pool) {
-    constexpr int MARCH_RAYS_PER_BLOCK = MARCH_BLOCK / LANE_STRIDE;
     __shared__ uint32_t lut[128];
     morton_lut_init(lut, threadIdx.x, MARCH_BLOCK);
     __syncthreads();
-    const bool owner = (threadIdx.x % LANE_STRIDE) == 0;
-    uint32_t i = blockIdx.x * MARCH_RAYS_PER_BLOCK + threadIdx.x / LANE_STRIDE;
+    uint32_t i = blockIdx.x * MARCH_BLOCK + threadIdx.x;
     uint32_t n = 0;
-    if (owner && i < (uint32_t)n_rays) {
+    if (i < (uint32_t)n_rays) {
         float o[3] = {rays_o[3 * (size_t)i], rays_o[3 * (size_t)i + 1], rays_o[3 * (size_t)i + 2]};
         float d[3] = {rays_d[3 * (size_t)i], rays_d[3 * (size_t)i + 1], rays_d[3 * (size_t)i + 2]};
         float st = ray_start_t(rng, i, lo, hi, o, d, near_distance, cone);
@@ -138,7 +128,7 @@ __global__ void __launch_bounds__(MARCH_BLOCK) march_count_kernel(int n_rays, co
     }
     uint32_t tot;
     uint32_t ex = block_excl_scan(n, &tot);
-    if (owner && i < (uint32_t)n_rays) local_excl[i] = ex;
+    if (i < (uint32_t)n_rays) local_excl[i] = ex;
     if (threadIdx.x == 0) block_sum[blockIdx.x] = tot;
 }
 
@@ -177,13 +167,13 @@ __global__ void __launch_bounds__(256) march_emit_kernel(int n_rays, const float
                                                          float hi, float cone, uint32_t max_samples, const uint32_t *__restrict__ local_excl, const float *__restrict__ startt,
                                                          const uint32_t *__restrict__ block_off, const uint32_t *__restrict__ misc, const float *__restrict__ tbuf,
                                                          const int32_t *__restrict__ chunk_of, const float *__restrict__ ovf, float *__restrict__ coords_out, int32_t *__restrict__ rays_index, int32_t *__restrict__ numsteps,
-                                                         int32_t *__restrict__ counters, int rays_per_scan_block) {
+                                                         int32_t *__restrict__ counters) {
     const int lane = threadIdx.x & 31;
     const uint32_t n_warps = (gridDim.x * 256) >> 5;
     uint32_t ok_count = 0;
     for (uint32_t i = (blockIdx.x * 256 + threadIdx.x) >> 5; i < (uint32_t)n_rays; i += n_warps) {   // persistent warps: 8192 tiny blocks cost more to schedule than to run
         uint32_t n = (uint32_t)numsteps[2 * (size_t)i];
-        uint32_t base = misc[0] + block_off[i / rays_per_scan_block] + local_excl[i];
+        uint32_t base = misc[0] + block_off[i / MARCH_BLOCK] + local_excl[i];
         __syncwarp();
         if (base + n > max_samples) {  // ray_sampler.cu:76-82
             if (lane == 0) { numsteps[2 * (size_t)i] = 0; numsteps[2 * (size_t)i + 1] = (int32_t)base; }
@@ -521,23 +511,19 @@ int xrb_rm_rays_sampler(const float *rays_o, const float *rays_d, const uint8_t 
     XRB_REQUIRE(rays_o && rays_d && bitfield && coords_out && rays_index && numsteps && counters && workspace, "rays_sampler: null pointer");
     cudaStream_t s = (cudaStream_t)stream;
     MarchWs w = march_ws(workspace, n_rays);
-    const int ls = lane_stride(), rpb = MARCH_BLOCK / ls;
-    int nb = (n_rays + rpb - 1) / rpb;
+    const int nb = (int)march_n_blocks(n_rays);
     Pcg32 rng = host_rng(seed, n_prior_calls);
     cudaMemsetAsync(w.misc + 3, 0, sizeof(uint32_t), s);   // overflow-chunk counter
     OvfPool pool{w.misc + 3, w.ovf, w.n_chunks, w.chunk_of};
-    if (ls == 1) march_count_kernel<1><<<nb, MARCH_BLOCK, 0, s>>>(n_rays, rays_o, rays_d, bitfield, aabb0, aabb1, near_distance, cone_angle, rng, w.local_excl, w.startt, w.block_sum, numsteps, w.tbuf, pool);
-    else if (ls == 2) march_count_kernel<2><<<nb, MARCH_BLOCK, 0, s>>>(n_rays, rays_o, rays_d, bitfield, aabb0, aabb1, near_distance, cone_angle, rng, w.local_excl, w.startt, w.block_sum, numsteps, w.tbuf, pool);
-    else march_count_kernel<4><<<nb, MARCH_BLOCK, 0, s>>>(n_rays, rays_o, rays_d, bitfield, aabb0, aabb1, near_distance, cone_angle, rng, w.local_excl, w.startt, w.block_sum, numsteps, w.tbuf, pool);
+    march_count_kernel<<<nb, MARCH_BLOCK, 0, s>>>(n_rays, rays_o, rays_d, bitfield, aabb0, aabb1, near_distance, cone_angle, rng, w.local_excl, w.startt, w.block_sum, numsteps, w.tbuf, pool);
     march_scan_kernel<<<1, 1024, 0, s>>>(nb, w.block_sum, w.misc, counters);
     march_emit_kernel<<<warp_grid(n_rays), 256, 0, s>>>(n_rays, rays_o, rays_d, bitfield, aabb0, aabb1, cone_angle, (uint32_t)max_samples, w.local_excl, w.startt,
-                                                                             w.block_sum, w.misc, w.tbuf, w.chunk_of, w.ovf, coords_out, rays_index, numsteps, counters, rpb);
+                                                                             w.block_sum, w.misc, w.tbuf, w.chunk_of, w.ovf, coords_out, rays_index, numsteps, counters);
     return check_launch("rays_sampler");
 }
 
 size_t xrb_rm_compacted_coord_workspace(int n_rays) {   // the compaction uses only the scan part of the march workspace layout (local_excl, startt, block_sum, misc)
-    size_t nb = (size_t)(n_rays + MARCH_RAYS_PER_BLOCK_MIN - 1) / MARCH_RAYS_PER_BLOCK_MIN;
-    return sizeof(uint32_t) * ((size_t)n_rays * 2 + nb + 16);
+    return sizeof(uint32_t) * ((size_t)n_rays * 2 + march_n_blocks(n_rays) + 16);
 }
 
 int xrb_rm_compacted_coord(const float *network_output, const float *coords_in, const int32_t *numsteps, int n_rays, int max_compacted, float *coords_out,
@@ -548,7 +534,7 @@ int xrb_rm_compacted_coord(const float *network_output, const float *coords_in, 
     XRB_REQUIRE(coords_in && numsteps && coords_out && numsteps_compacted && ray_counter && step_counter && workspace, "compacted_coord: null pointer");
     cudaStream_t s = (cudaStream_t)stream;
     MarchWs w = march_ws(workspace, n_rays);
-    int nb = (n_rays + MARCH_BLOCK - 1) / MARCH_BLOCK;
+    const int nb = (int)march_n_blocks(n_rays);
     compact_count_kernel<<<nb, MARCH_BLOCK, 0, s>>>(n_rays, numsteps, w.local_excl, w.block_sum);
     // reuse the scan kernel: "counters" = {ray_counter, step_counter} must be adjacent for it; they are separate tensors in the
     // reference API, so run it on a 2-int staging area in the workspace instead.

@@ -2,7 +2,6 @@
 tensor-core weight image, and thin wrappers over the C ABI (include/xrnerf_b200.h: xrb_ngp_*).
 """
 import math
-import os
 
 import torch
 from torch import nn
@@ -25,7 +24,7 @@ class NgpField(nn.Module):
         # levels [0, n_packed_levels) are gathered from the cell image (xrb_ngp_table, include/xrnerf_b200.h): 7 = the five dense levels + the first two hashed
         # ones, 72.5 MB. With the 24.4 MB table that exceeds H100's 50 MB L2 (only 5 levels, 10.6 MB, or 6, 27.6 MB, fit beside it), yet on H100
         # 5, 6 and 7 levels show no measurable difference in speed (DESIGN.md §4.1). The trainer drops to 6 (the image is rebuilt after every optimiser step); 0 disables it.
-        self.n_packed = int(os.environ.get('XRB_PACKED_LEVELS', '7')) if n_packed_levels is None else int(n_packed_levels)
+        self.n_packed = 7 if n_packed_levels is None else int(n_packed_levels)
         self.cfg = _C.NgpConfig(n_levels, n_features, log2_hashmap_size, base_resolution, per_level_scale, width, density_hidden, color_hidden)
         n_hash = _C.lib.xrb_tcnn_hashgrid_num_params(self.cfg)
         if n_hash < 0:
