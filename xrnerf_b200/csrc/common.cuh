@@ -33,6 +33,27 @@ int check_launch(const char *what);
         if (!(cond)) { xrb::set_error(msg); return XRB_E_BADARG; } \
     } while (0)
 
+// ---------------------------------------------------------------- persistent launches (host)
+// SM count of the current device; a failed query clears the sticky error and falls back to NUM_SMS
+inline int sm_count() {
+    int dev = 0, sms = NUM_SMS;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) { cudaGetLastError(); sms = NUM_SMS; }
+    return sms;
+}
+// grid of a persistent kernel that keeps per_sm CTAs resident on every SM: never more CTAs than there is work, never fewer than one
+inline int persistent_grid(int per_sm, int64_t work_ctas) {
+    const int64_t g = (int64_t)sm_count() * per_sm;
+    return (int)(work_ctas < g ? (work_ctas > 0 ? work_ctas : 1) : g);
+}
+// the same with per_sm taken from the occupancy calculator, but at least min_per_sm
+inline int persistent_grid(const void *kernel, int block, size_t smem, int64_t work_ctas, int min_per_sm = 1) {
+    int per_sm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem) != cudaSuccess) cudaGetLastError();
+    if (per_sm < min_per_sm) per_sm = min_per_sm;  // the calculator has been seen to under-report; extra CTAs simply queue
+    return persistent_grid(per_sm, work_ctas);
+}
+
 // ---------------------------------------------------------------- pcg32 (include/op_include/pcg32/pcg32.h:41-165)
 struct Pcg32 {
     uint64_t state, inc;

@@ -49,8 +49,7 @@ int xrb_micro_gather(const void *table, int64_t n_records, int record_bytes, int
     XRB_REQUIRE(table && sink && n_records > 0 && n_records < (1ll << 28) && rounds > 0, "micro_gather: bad arguments");
     XRB_REQUIRE(record_bytes == 4 || record_bytes == 8 || record_bytes == 32, "micro_gather: record_bytes must be 4, 8 or 32");
     XRB_REQUIRE(((uintptr_t)table & 31) == 0, "micro_gather: table must be 32-byte aligned");
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int grid = sms * 8;
+    const int grid = sm_count() * 8;
     cudaStream_t s = (cudaStream_t)stream;
     if (record_bytes == 4) micro_gather_kernel<4><<<grid, 256, 0, s>>>((const uint8_t *)table, (uint32_t)n_records, rounds, (uint32_t *)sink);
     else if (record_bytes == 8) micro_gather_kernel<8><<<grid, 256, 0, s>>>((const uint8_t *)table, (uint32_t)n_records, rounds, (uint32_t *)sink);

@@ -231,9 +231,7 @@ static int nm_launch(const void *weight_image, const float *bias, const void *en
     P.slot_bytes = (max_bytes + 1023) & ~1023u;
     P.n_slots = 4;
     const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * NM_BLOCK + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int64_t n_tiles = (n_rows + 127) / 128;
-    const int grid = (int)(n_tiles < sms ? n_tiles : sms);
+    const int grid = persistent_grid(1, (n_rows + 127) / 128);
     auto k = mip ? nerf_mlp_wg_kernel<true> : nerf_mlp_wg_kernel<false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);

@@ -365,8 +365,7 @@ int xrb_nerf_tg_layer(const xrb_tg_layer *L, void *stream) {
     XRB_REQUIRE(L->epi != 2 || L->x_base != nullptr, "tg_layer: mask image missing");
     const size_t smem = tg_smem();
     cudaFuncSetAttribute(tg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    long long n_tiles = (L->n_rows + 127) / 128; int grid = n_tiles < sms ? (int)n_tiles : sms;
+    const int grid = persistent_grid(1, (L->n_rows + 127) / 128);
     tg_kernel<<<grid, TG_THREADS, smem, (cudaStream_t)stream>>>(P);
     return check_launch("nerf_tg_layer");
 }
@@ -385,9 +384,8 @@ int xrb_nerf_tg_dw(const xrb_tg_dw *L, void *stream) {
     else { XRB_REQUIRE(L->N == 128 || L->N == 256, "tg_dw: N must be 128 or 256 (or <= 16)"); P.n_chunks = L->N / 128; }
     const size_t smem = tg_dw_smem();
     cudaFuncSetAttribute(tg_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long n_tiles = (L->n_rows + 127) / 128;
-    int per = sms / P.n_chunks; if (per > n_tiles) per = (int)n_tiles; if (per < 1) per = 1;
+    int per = sm_count() / P.n_chunks; if (per > n_tiles) per = (int)n_tiles; if (per < 1) per = 1;
     tg_dw_kernel<<<per * P.n_chunks, TG_DW_THREADS, smem, (cudaStream_t)stream>>>(P);
     return check_launch("nerf_tg_dw");
 }

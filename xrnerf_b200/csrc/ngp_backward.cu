@@ -20,29 +20,10 @@ namespace xrb {
 constexpr int BW_THREADS = 128;
 constexpr float DY_SCALE = 4096.f;
 
-struct BwSmem {
-    __half *W;      // fp16 weights: density net then colour net (tcnn layout)
-    __half *ENC;    // [128][32]
-    __half *H[4];   // density hidden activations [128][64] each (up to 4)
-    __half *CIN;    // [128][32]
-    __half *C[4];   // colour hidden activations
-    __half *DY;     // [128][64] staged, scaled dY of the layer being processed
-};
-
-// y[o] = sum_k W[o][k] x[k]  (x from shared fp16 row, fp32 accumulate), optional relu, fp16 rounding — forward semantics
-template <int IN, int OUT, bool RELU>
-__device__ __forceinline__ void fwd_layer_smem(const __half *__restrict__ W, const __half *__restrict__ xrow, float *y) {
-    float x[IN];
+// loads / stores my row of a shared-memory tile (fp16) as fp32 registers
+__device__ __forceinline__ void load_row_h(const __half *row, float *v, int n) {
 #pragma unroll
-    for (int k = 0; k < IN / 2; ++k) { float2 v = __half22float2(reinterpret_cast<const __half2 *>(xrow)[k]); x[2 * k] = v.x; x[2 * k + 1] = v.y; }
-#pragma unroll 4
-    for (int o = 0; o < OUT; ++o) {
-        float s = 0.f;
-        const __half2 *w2 = reinterpret_cast<const __half2 *>(W + (size_t)o * IN);
-#pragma unroll
-        for (int k = 0; k < IN / 2; ++k) { float2 w = __half22float2(w2[k]); s = fmaf(w.x, x[2 * k], s); s = fmaf(w.y, x[2 * k + 1], s); }
-        y[o] = round_h(RELU ? fmaxf(s, 0.f) : s);
-    }
+    for (int k = 0; k < n; k += 2) { float2 f = __half22float2(reinterpret_cast<const __half2 *>(row)[k >> 1]); v[k] = f.x; v[k + 1] = f.y; }
 }
 __device__ __forceinline__ void store_row_h(__half *row, const float *v, int n) {
     for (int k = 0; k < n; k += 2) reinterpret_cast<__half2 *>(row)[k >> 1] = __floats2half2_rn(v[k], v[k + 1]);
@@ -90,7 +71,78 @@ __device__ __forceinline__ void stage_dy(__half *DY, const float *g, int n) {  /
     for (int k = 0; k < n; k += 2) reinterpret_cast<__half2 *>(row)[k >> 1] = __floats2half2_rn(g[k] * DY_SCALE, g[k + 1] * DY_SCALE);
 }
 
-// DH/CH fixed by template so that the register accumulators have static shapes
+// ---------------------------------------------------------------------------- backward of one tcnn-shaped net (32 -> 64 x NH -> 16) on a 128-sample tile
+// NH is a template parameter so that the register accumulators have static shapes. Parameters in tcnn's order: W_in [64][32], NH - 1 x W_hid [64][64], W_out [16][64].
+constexpr int NET_IN = 64 * 32, NET_HID = 64 * 64;   // elements of the input matrix / of one hidden matrix
+__host__ __device__ constexpr int net_params(int nh) { return (int)mlp_num_params(32, 64, nh, 16); }
+__host__ __device__ constexpr int net_tile_halfs(int nh) { return 128 * 32 + nh * 128 * 64; }
+// the net's layer inputs of the tile, fp16 in shared memory: needed both for the ReLU masks and as the X operand of the weight gradients
+template <int NH> struct NetTiles {
+    __half *X;       // [128][32] input rows
+    __half *H[NH];   // [128][64] output of hidden layer k
+    __device__ __forceinline__ explicit NetTiles(__half *&p) { X = p; p += 128 * 32; for (int k = 0; k < NH; ++k) { H[k] = p; p += 128 * 64; } }
+};
+// the net's weight-gradient accumulators (scaled by DY_SCALE): this thread's tile of each matrix (dw_accumulate), in registers for the whole persistent loop
+template <int NH> struct NetGrad { float in[16] = {}, hid[NH > 1 ? (NH - 1) * 32 : 1] = {}, out[8] = {}; };
+
+// forward recompute of my row from t.X (already written), parking every hidden layer's output in t.H; out16 != NULL: also the output layer
+template <int NH>
+__device__ __forceinline__ void net_forward_park(const __half *__restrict__ W, const NetTiles<NH> &t, float *out16) {
+    float x[64], h[64];
+    load_row_h(t.X + (size_t)threadIdx.x * 32, x, 32);
+    simt_layer<32, 64, true, 4>(W, x, h);
+    store_row_h(t.H[0] + (size_t)threadIdx.x * 64, h, 64);
+#pragma unroll
+    for (int k = 1; k < NH; ++k) {
+        load_row_h(t.H[k - 1] + (size_t)threadIdx.x * 64, x, 64);
+        simt_layer<64, 64, true, 4>(W + NET_IN + (k - 1) * NET_HID, x, h);
+        store_row_h(t.H[k] + (size_t)threadIdx.x * 64, h, 64);
+    }
+    if (out16) { load_row_h(t.H[NH - 1] + (size_t)threadIdx.x * 64, x, 64); simt_layer<64, 16, false, 4>(W + NET_IN + (NH - 1) * NET_HID, x, out16); }
+}
+// one layer step: gy (my row of dL/d layer output, staged for the block) -> dW += gy^T X over the tile's n_valid rows, gx = W^T gy. Two barriers: the
+// staged rows are complete before the GEMM reads them, and read before the next step overwrites them.
+template <int IN, int OUT, int TO, int TI>
+__device__ __forceinline__ void net_layer_backward(const __half *__restrict__ W, const __half *X, __half *DY, const float *gy, float *gx, float *acc, int n_valid) {
+    stage_dy(DY, gy, OUT);
+    __syncthreads();
+    dw_accumulate<IN, OUT, TO, TI>(DY, X, acc, n_valid);
+    bwd_layer_dx<IN, OUT>(W, gy, gx);
+    __syncthreads();
+}
+// gx = gx masked by ReLU'(my row of the activation tile) -> gy
+__device__ __forceinline__ void relu_mask(const __half *act_tile, const float *gx, float *gy) {
+    const __half *act = act_tile + (size_t)threadIdx.x * 64;
+#pragma unroll
+    for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
+}
+// backward of the net on the tile: gy[0..15] = dL/d(my output row) on entry; gx[0..31] = dL/d(my input row) on return (both are 64-wide work arrays)
+template <int NH>
+__device__ __forceinline__ void net_backward(const __half *__restrict__ W, const NetTiles<NH> &t, __half *DY, float *gy, float *gx, NetGrad<NH> &acc, int n_valid) {
+    net_layer_backward<64, 16, 2, 4>(W + NET_IN + (NH - 1) * NET_HID, t.H[NH - 1], DY, gy, gx, acc.out, n_valid);
+#pragma unroll
+    for (int k = NH - 1; k >= 1; --k) {  // hidden layer k: input H[k-1], output H[k]
+        relu_mask(t.H[k], gx, gy);
+        net_layer_backward<64, 64, 4, 8>(W + NET_IN + (k - 1) * NET_HID, t.H[k - 1], DY, gy, gx, acc.hid + (k - 1) * 32, n_valid);
+    }
+    relu_mask(t.H[0], gx, gy);
+    net_layer_backward<32, 64, 4, 4>(W, t.X, DY, gy, gx, acc.in, n_valid);
+}
+// adds the accumulators to the fp32 parameter gradient (once per CTA)
+template <int NH>
+__device__ __forceinline__ void net_flush(const NetGrad<NH> &acc, float *__restrict__ dW) {
+    dw_flush<32, 64, 4, 4>(acc.in, dW);
+#pragma unroll
+    for (int k = 1; k < NH; ++k) dw_flush<64, 64, 4, 8>(acc.hid + (k - 1) * 32, dW + NET_IN + (k - 1) * NET_HID);
+    dw_flush<64, 16, 2, 4>(acc.out, dW + NET_IN + (NH - 1) * NET_HID);
+}
+// opts a backward kernel in to `smem` bytes of dynamic shared memory and returns its persistent grid for n samples (one CTA works on 128-sample tiles)
+template <typename K>
+static int bwd_grid(K kernel, size_t smem, int n) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    return persistent_grid((const void *)kernel, BW_THREADS, smem, (n + 127) / 128);
+}
+
 template <int DH, int CH>
 __global__ void __launch_bounds__(BW_THREADS) ngp_field_bwd_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const __half *__restrict__ dens_p, const __half *__restrict__ color_p,
                                                                    const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride,
@@ -98,19 +150,17 @@ __global__ void __launch_bounds__(BW_THREADS) ngp_field_bwd_kernel(HashGridDev g
                                                                    float *__restrict__ d_dens, float *__restrict__ d_color) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     if (n_dev) n = min(n, max(*n_dev, 0));
-    constexpr int ND = 64 * 32 + (DH - 1) * 64 * 64 + 16 * 64, NC = 64 * 32 + (CH - 1) * 64 * 64 + 16 * 64;
+    constexpr int ND = net_params(DH), NC = net_params(CH);
     __half *p = reinterpret_cast<__half *>(smem_raw);
-    __half *W = p; p += ND + NC;
-    __half *ENC = p; p += 128 * 32;
-    __half *H[DH]; for (int k = 0; k < DH; ++k) { H[k] = p; p += 128 * 64; }
-    __half *CIN = p; p += 128 * 32;
-    __half *C[CH]; for (int k = 0; k < CH; ++k) { C[k] = p; p += 128 * 64; }
-    __half *DY = p; p += 128 * 64;
+    __half *W = p; p += ND + NC;      // fp16 weights: density net then colour net (tcnn layout)
+    const NetTiles<DH> D(p);          // X = the encoding
+    const NetTiles<CH> C(p);          // X = the colour-net input row
+    __half *DY = p;                   // [128][64] staged, scaled dY of the layer being processed
     for (int k = threadIdx.x; k < ND; k += BW_THREADS) W[k] = dens_p[k];
     for (int k = threadIdx.x; k < NC; k += BW_THREADS) W[ND + k] = color_p[k];
     const __half *Wd = W, *Wc = W + ND;
-    // register accumulators of the weight gradients (scaled by DY_SCALE)
-    float a_d0[16] = {0}, a_dh[DH > 1 ? (DH - 1) * 32 : 1] = {0}, a_do[8] = {0}, a_c0[16] = {0}, a_ch[CH > 1 ? (CH - 1) * 32 : 1] = {0}, a_co[8] = {0};
+    NetGrad<DH> a_d;
+    NetGrad<CH> a_c;
     __syncthreads();
 
     const int n_tiles = (n + 127) / 128;
@@ -130,139 +180,43 @@ __global__ void __launch_bounds__(BW_THREADS) ngp_field_bwd_kernel(HashGridDev g
             float enc[32];
 #pragma unroll
             for (int l = 0; l < 16; ++l) { float2 f = hash_level(table, cells, g, l, px, py, pz); enc[2 * l] = f.x; enc[2 * l + 1] = f.y; }
-            store_row_h(ENC + (size_t)threadIdx.x * 32, enc, 32);
+            store_row_h(D.X + (size_t)threadIdx.x * 32, enc, 32);
         }
         float dout[16];
+        net_forward_park<DH>(Wd, D, dout);
         {
-            float h[64];
-            fwd_layer_smem<32, 64, true>(Wd, ENC + (size_t)threadIdx.x * 32, h);
-            store_row_h(H[0] + (size_t)threadIdx.x * 64, h, 64);
-#pragma unroll
-            for (int k = 1; k < DH; ++k) { fwd_layer_smem<64, 64, true>(Wd + 64 * 32 + (k - 1) * 64 * 64, H[k - 1] + (size_t)threadIdx.x * 64, h); store_row_h(H[k] + (size_t)threadIdx.x * 64, h, 64); }
-            fwd_layer_smem<64, 16, false>(Wd + 64 * 32 + (DH - 1) * 64 * 64, H[DH - 1] + (size_t)threadIdx.x * 64, dout);
+            float cin[32];
+            color_input_row(dout, dx, dy, dz, cin);
+            store_row_h(C.X + (size_t)threadIdx.x * 32, cin, 32);
         }
-        {
-            float cin[32], sh[16];
-            sh4(dx, dy, dz, sh);
-#pragma unroll
-            for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) cin[15 + k] = sh[k];
-            cin[31] = 1.0f;
-            store_row_h(CIN + (size_t)threadIdx.x * 32, cin, 32);
-            float h[64];
-            fwd_layer_smem<32, 64, true>(Wc, CIN + (size_t)threadIdx.x * 32, h);
-            store_row_h(C[0] + (size_t)threadIdx.x * 64, h, 64);
-#pragma unroll
-            for (int k = 1; k < CH; ++k) { fwd_layer_smem<64, 64, true>(Wc + 64 * 32 + (k - 1) * 64 * 64, C[k - 1] + (size_t)threadIdx.x * 64, h); store_row_h(C[k] + (size_t)threadIdx.x * 64, h, 64); }
-        }
-        // ------------------------------------------------ backward: colour net
+        net_forward_park<CH>(Wc, C, nullptr);   // (the colour output layer itself is not needed: dL/draw is given)
+        // ------------------------------------------------ backward: colour net, then density net with dL/ddout = (draw.w, dcin[0..14])
         float gy[64], gx[64];
 #pragma unroll
         for (int k = 0; k < 16; ++k) gy[k] = 0.f;
         gy[0] = gr.x; gy[1] = gr.y; gy[2] = gr.z;
-        // output layer  [16 x 64]
-        stage_dy(DY, gy, 16);
-        __syncthreads();
-        dw_accumulate<64, 16, 2, 4>(DY, C[CH - 1], a_co, n_valid);
-        bwd_layer_dx<64, 16>(Wc + 64 * 32 + (CH - 1) * 64 * 64, gy, gx);
-        __syncthreads();
-#pragma unroll
-        for (int k = CH - 1; k >= 1; --k) {  // hidden layer k: input C[k-1], output C[k]
-            const __half *act = C[k] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<64, 64, 4, 8>(DY, C[k - 1], a_ch + (k - 1) * 32, n_valid);
-            bwd_layer_dx<64, 64>(Wc + 64 * 32 + (k - 1) * 64 * 64, gy, gx);
-            __syncthreads();
-        }
-        {
-            const __half *act = C[0] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<32, 64, 4, 4>(DY, CIN, a_c0, n_valid);
-            bwd_layer_dx<32, 64>(Wc, gy, gx);   // gx[0..31] = dL/dcin
-            __syncthreads();
-        }
-        // ------------------------------------------------ backward: density net; dL/ddout = (draw.w, dcin[0..14])
+        net_backward<CH>(Wc, C, DY, gy, gx, a_c, n_valid);   // gx[0..31] = dL/dcin
         gy[0] = gr.w;
 #pragma unroll
         for (int k = 0; k < 15; ++k) gy[k + 1] = gx[k];
-        stage_dy(DY, gy, 16);
-        __syncthreads();
-        dw_accumulate<64, 16, 2, 4>(DY, H[DH - 1], a_do, n_valid);
-        bwd_layer_dx<64, 16>(Wd + 64 * 32 + (DH - 1) * 64 * 64, gy, gx);
-        __syncthreads();
-#pragma unroll
-        for (int k = DH - 1; k >= 1; --k) {
-            const __half *act = H[k] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<64, 64, 4, 8>(DY, H[k - 1], a_dh + (k - 1) * 32, n_valid);
-            bwd_layer_dx<64, 64>(Wd + 64 * 32 + (k - 1) * 64 * 64, gy, gx);
-            __syncthreads();
-        }
-        {
-            const __half *act = H[0] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<32, 64, 4, 4>(DY, ENC, a_d0, n_valid);
-            bwd_layer_dx<32, 64>(Wd, gy, gx);   // gx[0..31] = dL/denc
-            __syncthreads();
-        }
+        net_backward<DH>(Wd, D, DY, gy, gx, a_d, n_valid);   // gx[0..31] = dL/denc
         // ------------------------------------------------ hash-table gradient scatter
         if (valid) {
 #pragma unroll 1
-            for (int l = 0; l < 16; ++l) {
-                const uint32_t hs = g.offset[l + 1] - g.offset[l], res = g.res[l];
-                float2 *tl = reinterpret_cast<float2 *>(d_table) + g.offset[l];
-                const float sc = g.scale[l];
-                float qx = __fmaf_rn(sc, px, 0.5f), qy = __fmaf_rn(sc, py, 0.5f), qz = __fmaf_rn(sc, pz, 0.5f);
-                int ixs, iys, izs;
-                float fx = floor_small(qx, &ixs), fy = floor_small(qy, &iys), fz = floor_small(qz, &izs);
-                const uint32_t ix = (uint32_t)ixs, iy = (uint32_t)iys, iz = (uint32_t)izs;
-                fx = qx - fx; fy = qy - fy; fz = qz - fz;
-                const float g0 = gx[2 * l], g1 = gx[2 * l + 1];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    float w = ((c & 1) ? fx : 1.f - fx) * ((c & 2) ? fy : 1.f - fy) * ((c & 4) ? fz : 1.f - fz);
-                    uint32_t idx = grid_index(ix + (c & 1), iy + ((c >> 1) & 1), iz + ((c >> 2) & 1), hs, res);
-                    atomicAdd(tl + idx, make_float2(w * g0, w * g1));
-                }
-            }
+            for (int l = 0; l < 16; ++l) scatter_level(d_table, grid_cell(g, l, px, py, pz), gx[2 * l], gx[2 * l + 1]);
         }
     }
-    // ---------------------------------------------------- flush weight-gradient accumulators (once per CTA)
-    dw_flush<32, 64, 4, 4>(a_d0, d_dens);
-#pragma unroll
-    for (int k = 1; k < DH; ++k) dw_flush<64, 64, 4, 8>(a_dh + (k - 1) * 32, d_dens + 64 * 32 + (k - 1) * 64 * 64);
-    dw_flush<64, 16, 2, 4>(a_do, d_dens + 64 * 32 + (DH - 1) * 64 * 64);
-    dw_flush<32, 64, 4, 4>(a_c0, d_color);
-#pragma unroll
-    for (int k = 1; k < CH; ++k) dw_flush<64, 64, 4, 8>(a_ch + (k - 1) * 32, d_color + 64 * 32 + (k - 1) * 64 * 64);
-    dw_flush<64, 16, 2, 4>(a_co, d_color + 64 * 32 + (CH - 1) * 64 * 64);
+    net_flush<DH>(a_d, d_dens);
+    net_flush<CH>(a_c, d_color);
 }
 
 template <int DH, int CH>
 static int launch_bwd(const HashGridDev &g, const void *table, const void *cells, const void *dens, const void *color, const float *pts, int pts_stride, const float *dirs, int dirs_stride,
                       const float *dl_draw, int n, const int32_t *n_dev, float *d_table, float *d_dens, float *d_color, cudaStream_t s) {
-    constexpr int ND = 64 * 32 + (DH - 1) * 64 * 64 + 16 * 64, NC = 64 * 32 + (CH - 1) * 64 * 64 + 16 * 64;
-    size_t smem = sizeof(__half) * ((size_t)ND + NC + 128 * 32 * 2 + (size_t)(DH + CH) * 128 * 64 + 128 * 64);
+    const size_t smem = sizeof(__half) * ((size_t)net_params(DH) + net_params(CH) + net_tile_halfs(DH) + net_tile_halfs(CH) + 128 * 64);
     auto k = ngp_field_bwd_kernel<DH, CH>;
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int per_sm = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, BW_THREADS, smem); if (per_sm < 1) per_sm = 1;
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int n_tiles = (n + 127) / 128, grid = sms * per_sm; if (grid > n_tiles) grid = n_tiles; if (grid < 1) grid = 1;
-    k<<<grid, BW_THREADS, smem, s>>>(g, (const __half2 *)table, (const uint8_t *)cells, (const __half *)dens, (const __half *)color, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev, d_table,
-                                     d_dens, d_color);
+    k<<<bwd_grid(k, smem, n), BW_THREADS, smem, s>>>(g, (const __half2 *)table, (const uint8_t *)cells, (const __half *)dens, (const __half *)color, pts, pts_stride, dirs, dirs_stride,
+                                                     (const float4 *)dl_draw, n, n_dev, d_table, d_dens, d_color);
     return check_launch("ngp_mlp_backward");
 }
 
@@ -299,41 +253,21 @@ __global__ void __launch_bounds__(256) hashgrid_backward_kernel(HashGridDev g, c
     const float2 gy = __half22float2(d_enc[(size_t)i * 16 + l]);
     const float g0 = gy.x * scale, g1 = gy.y * scale;
     if (g0 == 0.f && g1 == 0.f) return;
-    const uint32_t hs = g.offset[l + 1] - g.offset[l], res = g.res[l];
-    float2 *tl = reinterpret_cast<float2 *>(d_table) + g.offset[l];
-    const float sc = g.scale[l];
-    float qx = __fmaf_rn(sc, p[0], 0.5f), qy = __fmaf_rn(sc, p[1], 0.5f), qz = __fmaf_rn(sc, p[2], 0.5f);
-    int ixs, iys, izs;
-    float fx = floor_small(qx, &ixs), fy = floor_small(qy, &iys), fz = floor_small(qz, &izs);
-    const uint32_t ix = (uint32_t)ixs, iy = (uint32_t)iys, iz = (uint32_t)izs;
-    fx = qx - fx; fy = qy - fy; fz = qz - fz;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        float w = ((c & 1) ? fx : 1.f - fx) * ((c & 2) ? fy : 1.f - fy) * ((c & 4) ? fz : 1.f - fz);
-        uint32_t idx = grid_index(ix + (c & 1), iy + ((c >> 1) & 1), iz + ((c >> 2) & 1), hs, res);
-        atomicAdd(tl + idx, make_float2(w * g0, w * g1));
-    }
+    scatter_level(d_table, grid_cell(g, l, p[0], p[1], p[2]), g0, g1);
 }
 
-void launch_hashgrid_backward(const HashGridDev &g, const float *x, int x_stride, int n, const void *d_enc, float scale, float *d_table, cudaStream_t s) {
-    int64_t threads = (int64_t)n * 16;
-    hashgrid_backward_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(g, x, x_stride, n, (const __half2 *)d_enc, scale, d_table);
-}
-
-// tcnn.Network(FullyFusedMLP).backward: x fp16[n,32], dy fp16[n,16] -> dx fp16[n,32] (optional), fp32 parameter gradient (+=). Same structure as the density half of
-// ngp_field_bwd_kernel: forward recompute with the layer inputs parked in shared memory, per-thread dX, block GEMM dW with register accumulators.
+// tcnn.Network(FullyFusedMLP).backward: x fp16[n,32], dy fp16[n,16] -> dx fp16[n,32] (optional), fp32 parameter gradient (+=): the net backward above on its own.
 template <int NH>
 __global__ void __launch_bounds__(BW_THREADS) tcnn_mlp_bwd_kernel(const __half *__restrict__ params, const __half *__restrict__ x, const __half *__restrict__ dy, int n,
                                                                   __half *__restrict__ dx, float *__restrict__ d_params) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    constexpr int NPAR = 64 * 32 + (NH - 1) * 64 * 64 + 16 * 64;
+    constexpr int NPAR = net_params(NH);
     __half *p = reinterpret_cast<__half *>(smem_raw);
     __half *W = p; p += NPAR;
-    __half *X = p; p += 128 * 32;
-    __half *H[NH]; for (int k = 0; k < NH; ++k) { H[k] = p; p += 128 * 64; }
-    __half *DY = p; p += 128 * 64;
+    const NetTiles<NH> T(p);
+    __half *DY = p;
     for (int k = threadIdx.x; k < NPAR; k += BW_THREADS) W[k] = params[k];
-    float a_in[16] = {0}, a_hid[NH > 1 ? (NH - 1) * 32 : 1] = {0}, a_out[8] = {0};
+    NetGrad<NH> acc;
     __syncthreads();
     const int n_tiles = (n + 127) / 128;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -341,63 +275,26 @@ __global__ void __launch_bounds__(BW_THREADS) tcnn_mlp_bwd_kernel(const __half *
         const bool valid = i < n;
         const int n_valid = min(128, n - tile * 128);
         {
-            uint4 *dst = reinterpret_cast<uint4 *>(X + (size_t)threadIdx.x * 32);
+            uint4 *dst = reinterpret_cast<uint4 *>(T.X + (size_t)threadIdx.x * 32);
             const uint4 *src = reinterpret_cast<const uint4 *>(x + (size_t)i * 32);
 #pragma unroll
             for (int q = 0; q < 4; ++q) dst[q] = valid ? src[q] : make_uint4(0, 0, 0, 0);
         }
-        float h[64];
-        fwd_layer_smem<32, 64, true>(W, X + (size_t)threadIdx.x * 32, h);
-        store_row_h(H[0] + (size_t)threadIdx.x * 64, h, 64);
-#pragma unroll
-        for (int k = 1; k < NH; ++k) { fwd_layer_smem<64, 64, true>(W + 64 * 32 + (k - 1) * 64 * 64, H[k - 1] + (size_t)threadIdx.x * 64, h); store_row_h(H[k] + (size_t)threadIdx.x * 64, h, 64); }
+        net_forward_park<NH>(W, T, nullptr);
         float gy[64], gx[64];
 #pragma unroll
         for (int k = 0; k < 16; ++k) gy[k] = valid ? __half2float(dy[(size_t)i * 16 + k]) : 0.f;
-        stage_dy(DY, gy, 16);
-        __syncthreads();
-        dw_accumulate<64, 16, 2, 4>(DY, H[NH - 1], a_out, n_valid);
-        bwd_layer_dx<64, 16>(W + 64 * 32 + (NH - 1) * 64 * 64, gy, gx);
-        __syncthreads();
-#pragma unroll
-        for (int k = NH - 1; k >= 1; --k) {
-            const __half *act = H[k] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<64, 64, 4, 8>(DY, H[k - 1], a_hid + (k - 1) * 32, n_valid);
-            bwd_layer_dx<64, 64>(W + 64 * 32 + (k - 1) * 64 * 64, gy, gx);
-            __syncthreads();
-        }
-        {
-            const __half *act = H[0] + (size_t)threadIdx.x * 64;
-#pragma unroll
-            for (int q = 0; q < 64; ++q) gy[q] = __half2float(act[q]) > 0.f ? gx[q] : 0.f;
-            stage_dy(DY, gy, 64);
-            __syncthreads();
-            dw_accumulate<32, 64, 4, 4>(DY, X, a_in, n_valid);
-            bwd_layer_dx<32, 64>(W, gy, gx);
-            __syncthreads();
-        }
+        net_backward<NH>(W, T, DY, gy, gx, acc, n_valid);
         if (dx && valid) store_row_h(dx + (size_t)i * 32, gx, 32);
     }
-    dw_flush<32, 64, 4, 4>(a_in, d_params);
-#pragma unroll
-    for (int k = 1; k < NH; ++k) dw_flush<64, 64, 4, 8>(a_hid + (k - 1) * 32, d_params + 64 * 32 + (k - 1) * 64 * 64);
-    dw_flush<64, 16, 2, 4>(a_out, d_params + 64 * 32 + (NH - 1) * 64 * 64);
+    net_flush<NH>(acc, d_params);
 }
 
 template <int NH>
 static int launch_tcnn_mlp_bwd(const void *params, const void *x, const void *dy, int n, void *dx, float *d_params, cudaStream_t s) {
-    constexpr int NPAR = 64 * 32 + (NH - 1) * 64 * 64 + 16 * 64;
-    size_t smem = sizeof(__half) * ((size_t)NPAR + 128 * 32 + (size_t)NH * 128 * 64 + 128 * 64);
+    const size_t smem = sizeof(__half) * ((size_t)net_params(NH) + net_tile_halfs(NH) + 128 * 64);
     auto k = tcnn_mlp_bwd_kernel<NH>;
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int per_sm = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, BW_THREADS, smem); if (per_sm < 1) per_sm = 1;
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int n_tiles = (n + 127) / 128, grid = sms * per_sm; if (grid > n_tiles) grid = n_tiles; if (grid < 1) grid = 1;
-    k<<<grid, BW_THREADS, smem, s>>>((const __half *)params, (const __half *)x, (const __half *)dy, n, (__half *)dx, d_params);
+    k<<<bwd_grid(k, smem, n), BW_THREADS, smem, s>>>((const __half *)params, (const __half *)x, (const __half *)dy, n, (__half *)dx, d_params);
     return check_launch("tcnn_mlp_backward");
 }
 
@@ -489,7 +386,7 @@ int xrb_ngp_mlp_backward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(table && density_fp16 && color_fp16 && pts && dirs && dl_draw && d_table && d_density && d_color, "ngp_mlp_backward: null pointer");
     XRB_REQUIRE(((uintptr_t)dl_draw & 15) == 0 && ((uintptr_t)d_table & 7) == 0, "ngp_mlp_backward: dl_draw must be 16-byte, d_table 8-byte aligned");
-    HashGridDev g; e = table_setup(cfg, table, &g, "ngp_mlp_backward"); if (e) return e;
+    HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
     cudaStream_t s = (cudaStream_t)stream;
 #define XRB_BW(DH, CH) if (cfg->density_hidden == DH && cfg->color_hidden == CH) return launch_bwd<DH, CH>(g, table->table_fp16, table->cell_image, density_fp16, color_fp16, pts, pts_stride, dirs, dirs_stride, dl_draw, n, nullptr, d_table, d_density, d_color, s);
     XRB_BW(1, 1) XRB_BW(1, 2) XRB_BW(2, 2) XRB_BW(1, 3) XRB_BW(2, 3)

@@ -195,17 +195,8 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     constexpr BtLayout T = bt_layout(DH, CH);
-    uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *W = base, *tiles0 = base + image_bytes;
-    uint64_t *wbar = (uint64_t *)(tiles0 + 2 * (size_t)T.n_tiles * BT_TILE);
-    if (threadIdx.x == 0) {
-        tc::mbar_init(wbar, 1);
-        tc::fence_mbar_init();
-        tc::mbar_expect_tx(wbar, image_bytes);
-        tc::tma_bulk_g2s(W, weight_image, image_bytes, wbar);
-    }
-    __syncthreads();
-    tc::mbar_wait(wbar, 0);
+    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, 2 * (size_t)T.n_tiles * BT_TILE);
+    uint8_t *tiles0 = W + image_bytes;
     BtWg c;
     c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127; c.bar = 1 + c.wg;
     c.tiles = tiles0 + (size_t)c.wg * T.n_tiles * BT_TILE; c.W = W; c.first = true;
@@ -240,14 +231,9 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
 #pragma unroll
         for (int h = 1; h < DH; ++h) bt_fwd_hidden<64>(c, T.h0 + h - 1, L.d_hid[h - 1], T.h0 + h);
         {
-            float dout[16], sh[16], cin[32];
+            float dout[16], cin[32];
             bt_fwd_out(c, T.h0 + DH - 1, L.d_out, T.dz, dout);    // dZ is free until the colour backward
-            sh4(dx, dy, dz, sh);
-#pragma unroll
-            for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];        // fp16 rounding happens in the pack below (round(round(x)) == round(x))
-#pragma unroll
-            for (int k = 0; k < 16; ++k) cin[15 + k] = sh[k];
-            cin[31] = 1.0f;
+            color_input_row(dout, dx, dy, dz, cin);                   // fp16 rounding happens in the pack below (round(round(x)) == round(x))
 #pragma unroll
             for (int q = 0; q < 4; ++q)
                 bt_store_chunk(c, T.cin, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
@@ -285,41 +271,12 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
         c.first = false;
         // ------------------------------------------------ hash-table gradient scatter
         if (valid) {
-            // The scatter is bound by the LSU's reduction issue rate (~1.3 cycles per lane and RED, measured: 450 of 880 us per 700 K samples with 128 two-float
-            // REDs per sample), so x-adjacent corners that are also adjacent in memory go out as ONE 16-byte red.global.add.v4.f32:
-            //   hashed level: entries of (gx, y, z) and (gx^1, y, z) are the two halves of an aligned 16-byte pair -> even gx: 4 v4 instead of 8 v2
-            //   dense level : idx and idx + 1 -> one v4 when idx is even (and the pair does not wrap at the table end)
 #pragma unroll 1
             for (int l = 0; l < 16; ++l) {
-                const uint32_t hs = g.offset[l + 1] - g.offset[l], res = g.res[l];
-                float2 *tl = reinterpret_cast<float2 *>(d_table) + g.offset[l];
-                const float sc = g.scale[l];
-                float qx = __fmaf_rn(sc, px, 0.5f), qy = __fmaf_rn(sc, py, 0.5f), qz = __fmaf_rn(sc, pz, 0.5f);
-                int ixs, iys, izs;
-                float fx = floor_small(qx, &ixs), fy = floor_small(qy, &iys), fz = floor_small(qz, &izs);
-                const uint32_t ix = (uint32_t)ixs, iy = (uint32_t)iys, iz = (uint32_t)izs;
-                fx = qx - fx; fy = qy - fy; fz = qz - fz;
                 float g0 = 0.f, g1 = 0.f;
 #pragma unroll
                 for (int q = 0; q < 16; ++q) if (q == l) { g0 = genc[2 * q]; g1 = genc[2 * q + 1]; }   // register array indexed by the rolled loop counter: select, never spill
-                g0 *= (1.f / BT_SCALE); g1 *= (1.f / BT_SCALE);
-                const bool hashed = (g.hashed_mask >> l) & 1u;
-#pragma unroll
-                for (int yz = 0; yz < 4; ++yz) {
-                    const float wyz = ((yz & 1) ? fy : 1.f - fy) * ((yz & 2) ? fz : 1.f - fz);
-                    const float w0 = (1.f - fx) * wyz, w1 = fx * wyz;
-                    const uint32_t i0 = grid_index(ix, iy + (yz & 1), iz + (yz >> 1), hs, res), i1 = grid_index(ix + 1u, iy + (yz & 1), iz + (yz >> 1), hs, res);
-                    const bool pair = hashed ? ((ix & 1u) == 0u) : (((i0 & 1u) == 0u) && i1 == i0 + 1u);   // hashed, even gx: i1 == i0 ^ 1; both cases: i0 even, i1 = i0 + 1... or i0 odd (hashed)
-                    if (pair) {
-                        const uint32_t lo = i0 & ~1u;                      // hashed level with an odd i0: the pair is (i1, i0) in memory order
-                        const bool swap = (i0 & 1u) != 0u;
-                        const float a0 = swap ? w1 : w0, a1 = swap ? w0 : w1;
-                        atomicAdd(reinterpret_cast<float4 *>(tl + lo), make_float4(a0 * g0, a0 * g1, a1 * g0, a1 * g1));
-                    } else {
-                        atomicAdd(tl + i0, make_float2(w0 * g0, w0 * g1));
-                        atomicAdd(tl + i1, make_float2(w1 * g0, w1 * g1));
-                    }
-                }
+                scatter_level_paired(d_table, grid_cell(g, l, px, py, pz), (g.hashed_mask >> l) & 1u, g0 * (1.f / BT_SCALE), g1 * (1.f / BT_SCALE));
             }
         }
     }
@@ -343,8 +300,7 @@ static int launch_bwd_tc(const HashGridDev &g, const xrb_ngp_table *tab, const v
     auto k = ngp_field_bwd_tc_kernel<DH, CH, NP>;
     const size_t smem = bt_smem_bytes<DH, CH>(image_bytes);
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int n_tiles = (n + 127) / 128, grid = sms; if (grid > (n_tiles + 1) / 2) grid = (n_tiles + 1) / 2; if (grid < 1) grid = 1;
+    const int n_tiles = (n + 127) / 128, grid = persistent_grid(1, (n_tiles + 1) / 2);   // one CTA per SM, two tiles (warpgroups) per CTA
     k<<<grid, 256, smem, s>>>(g, (const __half2 *)tab->table_fp16, (const uint8_t *)tab->cell_image, image, image_bytes, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev,
                               d_table, d_dens, d_color);
     return check_launch("ngp_mlp_backward_tc");
@@ -367,7 +323,7 @@ int xrb_ngp_mlp_backward_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tabl
         set_error("ngp_mlp_backward_tc: tensor-core backward is built for (density_hidden, color_hidden) = (1,1) or (1,2); use xrb_ngp_mlp_backward");
         return XRB_E_UNSUPPORTED;
     }
-    HashGridDev g; e = table_setup(cfg, table, &g, "ngp_mlp_backward_tc"); if (e) return e;
+    HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
     const uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
     cudaStream_t s = (cudaStream_t)stream;
     const bool plan6 = plan_valid(g, table->n_packed_levels) && table->n_packed_levels == 6;

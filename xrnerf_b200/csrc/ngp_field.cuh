@@ -1,5 +1,5 @@
 // xrnerf_b200 — device building blocks of the Instant-NGP field (hash-grid encoding, SH, tiny MLP) shared by the
-// stand-alone tcnn-shaped kernels (ngp_mlp.cu) and the fused render kernel (ngp_render.cu).
+// stand-alone tcnn-shaped kernels (ngp_mlp.cu), the backward kernels (ngp_backward.cu, ngp_backward_tc.cu) and the fused render kernel (ngp_fused.cu).
 //
 // Semantics restated from tiny-cuda-nn (see oracle/tcnn_oracle.c header: the reference delegates this arithmetic to an
 // unpinned third-party package; call sites /root/reference/xrnerf/models/mlps/hashnerf_mlp.py:36-45,:55-79).
@@ -55,7 +55,7 @@ inline size_t cell_image_layout(HashGridDev *g, int n_packed) {
 constexpr int MAX_PACKED_LEVELS = 13;  // image sizes for the reference grid: ..6 = 73 MB, ..7 = 190 MB, ..9 = 1.3 GB, ..12 = 25 GB;
                                        // levels past the L2 are served by HBM at ONE 32-byte sector per sample and level, where the hashed table costs ~4.5 sectors of L2
                                        // traffic (4 (y,z) rows, the x neighbour shares the sector in 7 of 8 cases). Level 13 alone would be 39 GB.
-__host__ __device__ inline int64_t mlp_num_params(int in_w, int width, int n_hidden, int out_pad) { return (int64_t)width * in_w + (int64_t)(n_hidden - 1) * width * width + (int64_t)out_pad * width; }
+__host__ __device__ constexpr int64_t mlp_num_params(int in_w, int width, int n_hidden, int out_pad) { return (int64_t)width * in_w + (int64_t)(n_hidden - 1) * width * width + (int64_t)out_pad * width; }
 
 inline int check_cfg(const xrb_ngp_config *cfg) {
     if (!cfg) { set_error("ngp config is null"); return XRB_E_BADARG; }
@@ -76,7 +76,7 @@ constexpr uint32_t SAMPLE_ORDER_MAX_ROWS = 1u << 21;
 // count is min(n, *n_dev) read on the device. order (impl 1, full field only; NULL = row order): a permutation of the effective rows, evaluated
 // in that order (tile slot j reads and writes row order[j]); ignored when there are more than SAMPLE_ORDER_MAX_ROWS effective rows.
 // table_setup validates an xrb_ngp_table and describes it for the device.
-int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g, const char *who);
+int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g);
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
                  int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s);
 
@@ -106,6 +106,22 @@ __device__ __forceinline__ Cell32 ldg_cell(const void *p) {
 }
 __device__ __forceinline__ __half2 as_h2(uint32_t u) { return *reinterpret_cast<__half2 *>(&u); }
 
+// The grid cell of a sample on level l: the level's slice of the table (first entry `off`, `hs` entries), its resolution, the integer cell and the
+// position inside it. The ONLY place this arithmetic is written: the gather (hash_level) and every gradient scatter must agree on it bit for bit,
+// or a sample on a cell boundary scatters into a different cell than it gathered from.
+struct GridCell { uint32_t off, hs, res, gx, gy, gz; float fx, fy, fz; };
+__device__ __forceinline__ GridCell grid_cell(const HashGridDev &g, int l, float x, float y, float z) {
+    GridCell c;
+    c.off = g.offset[l]; c.hs = g.offset[l + 1] - c.off; c.res = g.res[l];
+    const float sc = g.scale[l];
+    const float px = __fmaf_rn(sc, x, 0.5f), py = __fmaf_rn(sc, y, 0.5f), pz = __fmaf_rn(sc, z, 0.5f);
+    int ix, iy, iz;
+    const float flx = floor_small(px, &ix), fly = floor_small(py, &iy), flz = floor_small(pz, &iz);
+    c.gx = (uint32_t)ix; c.gy = (uint32_t)iy; c.gz = (uint32_t)iz;
+    c.fx = px - flx; c.fy = py - fly; c.fz = pz - flz;
+    return c;
+}
+
 // one level of the multiresolution hash encoding: returns the two interpolated features (fp32, NOT yet rounded).
 // Index arithmetic is tcnn's grid_index() strength-reduced without changing any value:
 //   hashed level (res^3 > table size == 2^log2_hashmap_size): (x ^ y*P1 ^ z*P2) & (size-1); the two products are shared by the 8 corners
@@ -133,13 +149,9 @@ inline bool plan_valid(const HashGridDev &g, int np) {
 // (MODE is an ordinary argument of a force-inlined function: after unrolling it is a constant and the dead forms disappear)
 __device__ __forceinline__ float2 hash_level(const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const HashGridDev &g, int l, float x, float y, float z,
                                              const int MODE = GATHER_RUNTIME) {
-    const uint32_t off = g.offset[l], hs = g.offset[l + 1] - off, res = g.res[l];
-    const float sc = g.scale[l];
-    float px = __fmaf_rn(sc, x, 0.5f), py = __fmaf_rn(sc, y, 0.5f), pz = __fmaf_rn(sc, z, 0.5f);
-    int ix_, iy_, iz_;
-    float fx = floor_small(px, &ix_), fy = floor_small(py, &iy_), fz = floor_small(pz, &iz_);
-    const uint32_t gx = (uint32_t)ix_, gy = (uint32_t)iy_, gz = (uint32_t)iz_;
-    fx = px - fx; fy = py - fy; fz = pz - fz;
+    const GridCell c = grid_cell(g, l, x, y, z);
+    const uint32_t off = c.off, hs = c.hs, res = c.res, gx = c.gx, gy = c.gy, gz = c.gz;
+    const float fx = c.fx, fy = c.fy, fz = c.fz;
     __half2 v[8];
     const bool is_packed = MODE == GATHER_PACKED || (MODE == GATHER_RUNTIME && ((g.packed_mask >> l) & 1u));
     const bool is_hashed = MODE == GATHER_HASHED || (MODE == GATHER_RUNTIME && ((g.hashed_mask >> l) & 1u));
@@ -214,6 +226,65 @@ __device__ __forceinline__ void sh4(float dx01, float dy01, float dz01, float *o
     out[13] = 0.45704579946446572f * x * (1.0f - 5.0f * z2);
     out[14] = 1.4453057213202769f * z * (x2 - y2);
     out[15] = 0.59004358992664352f * x * (-x2 + 3.0f * y2);
+}
+
+// Backward of hash_level: adds the trilinear shares of (g0, g1) = dL/d(the level's two features) to the 8 corner entries of the fp32 table gradient.
+// The plain form: one red.global.add.v2.f32 per corner. The CUDA-core backward kernels use it; they are what the tests compare the paired form against.
+__device__ __forceinline__ void scatter_level(float *__restrict__ d_table, const GridCell &c, float g0, float g1) {
+    float2 *tl = reinterpret_cast<float2 *>(d_table) + c.off;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        float w = ((k & 1) ? c.fx : 1.f - c.fx) * ((k & 2) ? c.fy : 1.f - c.fy) * ((k & 4) ? c.fz : 1.f - c.fz);
+        uint32_t idx = grid_index(c.gx + (k & 1), c.gy + ((k >> 1) & 1), c.gz + ((k >> 2) & 1), c.hs, c.res);
+        atomicAdd(tl + idx, make_float2(w * g0, w * g1));
+    }
+}
+// The paired form of the tensor-core backward (d_table 16-byte aligned). Its scatter is bound by the LSU's reduction issue rate (~1.3 cycles per lane
+// and RED, measured: 450 of 880 us per 700 K samples with 128 two-float REDs per sample), so x-adjacent corners that are also adjacent in memory go out
+// as ONE 16-byte red.global.add.v4.f32:
+//   hashed level: entries of (gx, y, z) and (gx^1, y, z) are the two halves of an aligned 16-byte pair -> even gx: 4 v4 instead of 8 v2
+//   dense level : idx and idx + 1 -> one v4 when idx is even (and the pair does not wrap at the table end)
+__device__ __forceinline__ void scatter_level_paired(float *__restrict__ d_table, const GridCell &c, bool hashed, float g0, float g1) {
+    float2 *tl = reinterpret_cast<float2 *>(d_table) + c.off;
+#pragma unroll
+    for (int yz = 0; yz < 4; ++yz) {
+        const float wyz = ((yz & 1) ? c.fy : 1.f - c.fy) * ((yz & 2) ? c.fz : 1.f - c.fz);
+        const float w0 = (1.f - c.fx) * wyz, w1 = c.fx * wyz;
+        const uint32_t i0 = grid_index(c.gx, c.gy + (yz & 1), c.gz + (yz >> 1), c.hs, c.res), i1 = grid_index(c.gx + 1u, c.gy + (yz & 1), c.gz + (yz >> 1), c.hs, c.res);
+        const bool pair = hashed ? ((c.gx & 1u) == 0u) : (((i0 & 1u) == 0u) && i1 == i0 + 1u);   // hashed, even gx: i1 == i0 ^ 1; both cases: i0 even, i1 = i0 + 1... or i0 odd (hashed)
+        if (pair) {
+            const uint32_t lo = i0 & ~1u;                      // hashed level with an odd i0: the pair is (i1, i0) in memory order
+            const bool swap = (i0 & 1u) != 0u;
+            const float a0 = swap ? w1 : w0, a1 = swap ? w0 : w1;
+            atomicAdd(reinterpret_cast<float4 *>(tl + lo), make_float4(a0 * g0, a0 * g1, a1 * g0, a1 * g1));
+        } else {
+            atomicAdd(tl + i0, make_float2(w0 * g0, w0 * g1));
+            atomicAdd(tl + i1, make_float2(w1 * g0, w1 * g1));
+        }
+    }
+}
+
+// colour-net input row of a sample: density_out[1:16] (15) ++ SH of the direction (16) ++ 1.0 pad (tcnn.Network pads 31 -> 32 with ones).
+// fp32 values; the caller rounds to fp16
+__device__ __forceinline__ void color_input_row(const float *dout, float dx, float dy, float dz, float *cin) {
+#pragma unroll
+    for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];
+    sh4(dx, dy, dz, cin + 15);
+    cin[31] = 1.0f;
+}
+
+// One layer on CUDA cores: y[o] = act(sum_k W[o][k] x[k]), W fp16 in shared memory (all lanes read the same address: broadcast), x/y fp32 registers.
+// UNROLL: how many outputs are unrolled (all by default; the backward kernels, which are short of registers, take 4)
+template <int IN, int OUT, bool RELU, int UNROLL = OUT>
+__device__ __forceinline__ void simt_layer(const __half *__restrict__ W, const float *x, float *y) {
+#pragma unroll UNROLL
+    for (int o = 0; o < OUT; ++o) {
+        float s = 0.f;
+        const __half2 *w2 = reinterpret_cast<const __half2 *>(W + (size_t)o * IN);
+#pragma unroll
+        for (int k = 0; k < IN / 2; ++k) { float2 w = __half22float2(w2[k]); s = fmaf(w.x, x[2 * k], s); s = fmaf(w.y, x[2 * k + 1], s); }
+        y[o] = round_h(RELU ? fmaxf(s, 0.f) : s);
+    }
 }
 
 // ---------------------------------------------------------------------------- wgmma shared-memory image helpers

@@ -353,7 +353,7 @@ using namespace xrb;
 extern "C" {
 
 size_t xrb_ngp_render_fused_workspace(void) {
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) { cudaGetLastError(); sms = NUM_SMS; }
+    const int sms = sm_count();
     return 256 + (size_t)sms * FUSED_MAX_PROD_PER_SM * 32 * FR_TCAP * sizeof(float) + (size_t)sms * 2 * 128;
 }
 
@@ -366,7 +366,7 @@ int xrb_ngp_render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
     XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && workspace, "ngp_render_fused: null pointer");
     XRB_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)weight_image & 15) == 0, "ngp_render_fused: workspace must be 256-byte aligned, weight image 16-byte aligned");
     FusedParams P;
-    e = table_setup(cfg, table, &P.g, "ngp_render_fused"); if (e) return e;
+    e = table_setup(cfg, table, &P.g); if (e) return e;
     P.table = (const __half2 *)table->table_fp16; P.cells = (const uint8_t *)table->cell_image; P.np = plan_valid(P.g, table->n_packed_levels) ? table->n_packed_levels : 0;
     P.weight_image = weight_image; P.image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
     P.density_hidden = cfg->density_hidden; P.color_hidden = cfg->color_hidden;
@@ -375,7 +375,7 @@ int xrb_ngp_render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
     P.bg[0] = bg3_host[0]; P.bg[1] = bg3_host[1]; P.bg[2] = bg3_host[2]; P.rgb_act = rgb_act; P.dens_act = dens_act;
     P.rgb_out = rgb_out; P.alpha_out = alpha_out; P.n_samples_out = n_samples_out;
     { static const int dbg = getenv("XRB_FUSED_DBG") ? atoi(getenv("XRB_FUSED_DBG")) : 0; P.dbg = dbg; }
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
     P.sched = (uint32_t *)workspace; P.tscratch = (float *)((uint8_t *)workspace + 256);
     P.dbg_out = (unsigned long long *)((uint8_t *)workspace + 256 + (size_t)sms * FUSED_MAX_PROD_PER_SM * 32 * FR_TCAP * sizeof(float));
     const int64_t n_groups = ((int64_t)n_rays + 31) / 32;

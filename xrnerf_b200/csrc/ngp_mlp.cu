@@ -83,18 +83,6 @@ __global__ void __launch_bounds__(256) sh4_forward_kernel(const float *__restric
 }
 
 // ---------------------------------------------------------------------------- CUDA-core MLP (impl 0)
-// y[o] = act(sum_k W[o][k] x[k]), W fp16 in shared memory (all lanes read the same address: broadcast), x/y fp32 registers
-template <int IN, int OUT, bool RELU>
-__device__ __forceinline__ void simt_layer(const __half *__restrict__ W, const float *x, float *y) {
-#pragma unroll
-    for (int o = 0; o < OUT; ++o) {
-        float s = 0.f;
-        const __half2 *w2 = reinterpret_cast<const __half2 *>(W + (size_t)o * IN);
-#pragma unroll
-        for (int k = 0; k < IN / 2; ++k) { float2 w = __half22float2(w2[k]); s = fmaf(w.x, x[2 * k], s); s = fmaf(w.y, x[2 * k + 1], s); }
-        y[o] = round_h(RELU ? fmaxf(s, 0.f) : s);
-    }
-}
 // generic net: in_w (32) -> [64]*n_hidden -> 16; params = contiguous fp16 in shared memory
 __device__ __forceinline__ void simt_net(const __half *__restrict__ P, int n_hidden, const float *x32, float *out16) {
     float a[64], b[64];
@@ -126,13 +114,10 @@ __global__ void __launch_bounds__(128) ngp_field_simt_kernel(HashGridDev g, cons
         simt_net(s_w, density_hidden, enc, dout);
         if (DENSITY_ONLY) { out[i] = dout[0]; continue; }
         const float *d = dirs + (size_t)i * dirs_stride;
-        float cin[32], sh[16];
-        sh4(d[0], d[1], d[2], sh);
+        float cin[32];
+        color_input_row(dout, d[0], d[1], d[2], cin);
 #pragma unroll
-        for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];
-#pragma unroll
-        for (int k = 0; k < 16; ++k) cin[15 + k] = round_h(sh[k]);
-        cin[31] = 1.0f;
+        for (int k = 15; k < 31; ++k) cin[k] = round_h(cin[k]);   // the SH values; dout and 1.0 are fp16 values already
         float cout[16];
         simt_net(s_w + nd, color_hidden, cin, cout);
         reinterpret_cast<float4 *>(out)[i] = make_float4(cout[0], cout[1], cout[2], dout[0]);
@@ -197,13 +182,60 @@ ngp_field_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint
     }
 }
 
-static int persistent_grid(const void *kernel, int block, size_t smem, int work_ctas, int min_per_sm = 1) {
-    int per_sm = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem) != cudaSuccess) cudaGetLastError();
-    if (per_sm < min_per_sm) per_sm = min_per_sm;  // the calculator has been seen to under-report; extra CTAs simply queue
-    int dev = 0, sms = NUM_SMS; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int g = sms * per_sm;
-    return work_ctas < g ? (work_ctas > 0 ? work_ctas : 1) : g;
+// ---------------------------------------------------------------------------- host side: table description and the field launchers
+// validates an xrb_ngp_table and fills the device-side grid description (incl. the cell-image layout)
+int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g) {
+    if (!t || !t->table_fp16) { set_error("null hash table"); return XRB_E_BADARG; }
+    if (((uintptr_t)t->table_fp16 & 15) != 0) { set_error("hash table must be 16-byte aligned"); return XRB_E_BADARG; }
+    hashgrid_build(cfg, g);
+    if (t->n_packed_levels < 0 || t->n_packed_levels > MAX_PACKED_LEVELS) { set_error("n_packed_levels must be 0..13"); return XRB_E_BADARG; }
+    if (t->n_packed_levels > 0) {
+        if (!t->cell_image || ((uintptr_t)t->cell_image & 31) != 0) { set_error("cell image missing or not 32-byte aligned"); return XRB_E_BADARG; }
+        cell_image_layout(g, t->n_packed_levels);
+    }
+    return XRB_OK;
+}
+
+template <bool DENSITY_ONLY, int NP>
+static void launch_field_tc(const xrb_ngp_config *cfg, const HashGridDev &g, const void *table, const uint8_t *cells, const void *image, uint32_t image_bytes, const float *pts,
+                            int pts_stride, const float *dirs, int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, cudaStream_t s) {
+    auto k = ngp_field_tc_kernel<DENSITY_ONLY, NP>;
+    const size_t smem = tc_cta_smem_bytes<FIELD_NWG>(image_bytes);
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int n_tiles = (n + 127) / 128;
+    const int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);
+    k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, order,
+                                          out);
+}
+
+int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
+                 int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s) {
+    HashGridDev g; int e = table_setup(cfg, tab, &g); if (e) return e;
+    const void *table = tab->table_fp16; const uint8_t *cells = (const uint8_t *)tab->cell_image;
+    XRB_REQUIRE(impl != 0 || order == nullptr, "field: an evaluation order needs the tensor-core field");
+    if (impl == 0) {
+        size_t smem = (mlp_num_params(32, 64, cfg->density_hidden, 16) + (density_only ? 0 : mlp_num_params(32, 64, cfg->color_hidden, 16))) * sizeof(__half);
+        const void *k = density_only ? (const void *)ngp_field_simt_kernel<true> : (const void *)ngp_field_simt_kernel<false>;
+        if (smem > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        int grid = persistent_grid(k, 128, smem, (n + 127) / 128);
+        if (density_only)
+            ngp_field_simt_kernel<true><<<grid, 128, smem, s>>>(g, (const __half2 *)table, cells, (const __half *)dens, (const __half *)color, cfg->density_hidden, cfg->color_hidden, pts, pts_stride,
+                                                                dirs, dirs_stride, n, n_dev, out);
+        else
+            ngp_field_simt_kernel<false><<<grid, 128, smem, s>>>(g, (const __half2 *)table, cells, (const __half *)dens, (const __half *)color, cfg->density_hidden, cfg->color_hidden, pts, pts_stride,
+                                                                 dirs, dirs_stride, n, n_dev, out);
+    } else {
+        uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
+        // Measured with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us
+        // (ptxas: 128 registers, 0 spill bytes).
+        // static gather plan: the kernel is specialised for "levels [0,NP) packed, all others hashed" (NP = 6, 7); anything else takes the run-time form
+        const int npl = tab->n_packed_levels;
+        const int np = (plan_valid(g, npl) && (npl == 6 || npl == 7)) ? npl : 0;
+        auto launch = density_only ? (np == 6 ? launch_field_tc<true, 6> : np == 7 ? launch_field_tc<true, 7> : launch_field_tc<true, 0>)
+                                   : (np == 6 ? launch_field_tc<false, 6> : np == 7 ? launch_field_tc<false, 7> : launch_field_tc<false, 0>);
+        launch(cfg, g, table, cells, image, image_bytes, pts, pts_stride, dirs, dirs_stride, n, n_dev, order, out, s);
+    }
+    return check_launch(density_only ? "ngp_density_forward" : "ngp_mlp_forward");
 }
 
 }  // namespace xrb
@@ -263,30 +295,12 @@ int xrb_ngp_build_cell_image(const xrb_ngp_config *cfg, const void *table_fp16, 
     return check_launch("build_cell_image");
 }
 
-}  // extern "C"
-namespace xrb {
-// validates an xrb_ngp_table and fills the device-side grid description (incl. the cell-image layout)
-int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g, const char *who) {
-    if (!t || !t->table_fp16) { set_error("null hash table"); return XRB_E_BADARG; }
-    if (((uintptr_t)t->table_fp16 & 15) != 0) { set_error("hash table must be 16-byte aligned"); return XRB_E_BADARG; }
-    hashgrid_build(cfg, g);
-    if (t->n_packed_levels < 0 || t->n_packed_levels > MAX_PACKED_LEVELS) { set_error("n_packed_levels must be 0..13"); return XRB_E_BADARG; }
-    if (t->n_packed_levels > 0) {
-        if (!t->cell_image || ((uintptr_t)t->cell_image & 31) != 0) { set_error("cell image missing or not 32-byte aligned"); return XRB_E_BADARG; }
-        cell_image_layout(g, t->n_packed_levels);
-    }
-    (void)who;
-    return XRB_OK;
-}
-}  // namespace xrb
-extern "C" {
-
 int xrb_tcnn_hashgrid_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const float *x, int x_stride, int n, void *enc_fp16, void *stream) {
     int e = check_cfg(cfg); if (e) return e;
     XRB_REQUIRE(n >= 0 && x_stride >= 3, "hashgrid_forward: bad size");
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(table && x && enc_fp16, "hashgrid_forward: null pointer");
-    HashGridDev g; e = table_setup(cfg, table, &g, "hashgrid_forward"); if (e) return e;
+    HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
     int64_t threads = (int64_t)n * 16;
     hashgrid_forward_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(g, (const __half2 *)table->table_fp16, (const uint8_t *)table->cell_image, x, x_stride, n,
                                                                                                  (__half2 *)enc_fp16);
@@ -312,52 +326,6 @@ int xrb_tcnn_mlp_forward(const void *params_fp16, const void *x_fp16, int n, int
     mlp_forward_simt_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>((const __half *)params_fp16, (const __half *)x_fp16, n, n_hidden, (__half *)y_fp16);
     return check_launch("mlp_forward");
 }
-
-}  // extern "C"
-namespace xrb {
-template <bool DENSITY_ONLY, int NP>
-static void launch_field_tc(const xrb_ngp_config *cfg, const HashGridDev &g, const void *table, const uint8_t *cells, const void *image, uint32_t image_bytes, const float *pts,
-                            int pts_stride, const float *dirs, int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, cudaStream_t s) {
-    auto k = ngp_field_tc_kernel<DENSITY_ONLY, NP>;
-    const size_t smem = tc_cta_smem_bytes<FIELD_NWG>(image_bytes);
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    const int n_tiles = (n + 127) / 128;
-    const int grid = persistent_grid((const void *)k, 128 * FIELD_NWG, smem, (n_tiles + FIELD_NWG - 1) / FIELD_NWG, 2);
-    k<<<grid, 128 * FIELD_NWG, smem, s>>>(g, (const __half2 *)table, cells, image, image_bytes, cfg->density_hidden, cfg->color_hidden, pts, pts_stride, dirs, dirs_stride, n, n_dev, order,
-                                          out);
-}
-
-int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
-                 int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s) {
-    HashGridDev g; int e = table_setup(cfg, tab, &g, "field"); if (e) return e;
-    const void *table = tab->table_fp16; const uint8_t *cells = (const uint8_t *)tab->cell_image;
-    XRB_REQUIRE(impl != 0 || order == nullptr, "field: an evaluation order needs the tensor-core field");
-    if (impl == 0) {
-        size_t smem = (mlp_num_params(32, 64, cfg->density_hidden, 16) + (density_only ? 0 : mlp_num_params(32, 64, cfg->color_hidden, 16))) * sizeof(__half);
-        const void *k = density_only ? (const void *)ngp_field_simt_kernel<true> : (const void *)ngp_field_simt_kernel<false>;
-        if (smem > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        int grid = persistent_grid(k, 128, smem, (n + 127) / 128);
-        if (density_only)
-            ngp_field_simt_kernel<true><<<grid, 128, smem, s>>>(g, (const __half2 *)table, cells, (const __half *)dens, (const __half *)color, cfg->density_hidden, cfg->color_hidden, pts, pts_stride,
-                                                                dirs, dirs_stride, n, n_dev, out);
-        else
-            ngp_field_simt_kernel<false><<<grid, 128, smem, s>>>(g, (const __half2 *)table, cells, (const __half *)dens, (const __half *)color, cfg->density_hidden, cfg->color_hidden, pts, pts_stride,
-                                                                 dirs, dirs_stride, n, n_dev, out);
-    } else {
-        uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-        // Measured with scripts/field_bench.py on one H100 80GB HBM3 (700 W power limit, 1980 MHz max SM clock), 699 K samples, 7-level cell image: 248 us
-        // (ptxas: 128 registers, 0 spill bytes). impl 2 is a synonym of impl 1.
-        // static gather plan: the kernel is specialised for "levels [0,NP) packed, all others hashed" (NP = 6, 7); anything else takes the run-time form
-        const int npl = tab->n_packed_levels;
-        const int np = (plan_valid(g, npl) && (npl == 6 || npl == 7)) ? npl : 0;
-        auto launch = density_only ? (np == 6 ? launch_field_tc<true, 6> : np == 7 ? launch_field_tc<true, 7> : launch_field_tc<true, 0>)
-                                   : (np == 6 ? launch_field_tc<false, 6> : np == 7 ? launch_field_tc<false, 7> : launch_field_tc<false, 0>);
-        launch(cfg, g, table, cells, image, image_bytes, pts, pts_stride, dirs, dirs_stride, n, n_dev, order, out, s);
-    }
-    return check_launch(density_only ? "ngp_density_forward" : "ngp_mlp_forward");
-}
-}  // namespace xrb
-extern "C" {
 
 int xrb_ngp_mlp_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const void *color_fp16, const void *weight_image, const float *pts, int pts_stride,
                         const float *dirs, int dirs_stride, int n, const int32_t *n_rows_dev, float *raw, int impl, void *stream) {

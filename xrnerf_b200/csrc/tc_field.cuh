@@ -128,16 +128,10 @@ __device__ __forceinline__ void tc_density_from_a(const TcWarpgroup &c, const We
     for (int k = 0; k < 16; ++k) dout[k] = round_h(dout[k]);
 }
 
-// colour-net input row of my sample: density_out[1:16] (15) ++ SH (16) ++ 1.0 pad (tcnn.Network pads 31 -> 32 with ones)
+// colour-net input row of my sample (color_input_row) -> my A row
 __device__ __forceinline__ void tc_store_color_input(const TcWarpgroup &c, const float *dout, float dx, float dy, float dz) {
-    float sh[16];
-    sh4(dx, dy, dz, sh);
     float cin[32];
-#pragma unroll
-    for (int k = 0; k < 15; ++k) cin[k] = dout[k + 1];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) cin[15 + k] = sh[k];
-    cin[31] = 1.0f;
+    color_input_row(dout, dx, dy, dz, cin);
 #pragma unroll
     for (int q = 0; q < 4; ++q)
         a_store_chunk(c, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
@@ -162,12 +156,11 @@ __device__ __forceinline__ void tc_gather_levels(const __half2 *__restrict__ tab
 template <int WG>
 __host__ __device__ inline size_t tc_cta_smem_bytes(uint32_t image_bytes) { return 1024 /*align slack*/ + image_bytes + (size_t)WG * (16384 + TC_STAGE_BYTES) + 16; }
 
-template <int WG>
-__device__ __forceinline__ TcWarpgroup tc_cta_setup(uint8_t *dyn_smem, const void *weight_image, uint32_t image_bytes) {
-    uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *W = base, *A0 = base + image_bytes;  // image_bytes is a multiple of 1024
-    float *stage0 = (float *)(A0 + (size_t)WG * 16384);
-    uint64_t *wbar = (uint64_t *)((uint8_t *)stage0 + (size_t)WG * TC_STAGE_BYTES);
+// Called by every thread of the CTA: bulk-copies (TMA) the weight image to the first 1024-byte aligned address of the dynamic shared memory, waits for it
+// and returns that address. tiles_bytes: what the kernel keeps between the image (a multiple of 1024 bytes) and the copy's mbarrier.
+__device__ __forceinline__ uint8_t *tc_load_weight_image(uint8_t *dyn_smem, const void *weight_image, uint32_t image_bytes, size_t tiles_bytes) {
+    uint8_t *W = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
+    uint64_t *wbar = (uint64_t *)(W + image_bytes + tiles_bytes);
     if (threadIdx.x == 0) {
         tc::mbar_init(wbar, 1);
         tc::fence_mbar_init();
@@ -176,6 +169,14 @@ __device__ __forceinline__ TcWarpgroup tc_cta_setup(uint8_t *dyn_smem, const voi
     }
     __syncthreads();
     tc::mbar_wait(wbar, 0);  // weights have landed
+    return W;
+}
+
+template <int WG>
+__device__ __forceinline__ TcWarpgroup tc_cta_setup(uint8_t *dyn_smem, const void *weight_image, uint32_t image_bytes) {
+    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, (size_t)WG * (16384 + TC_STAGE_BYTES));
+    uint8_t *A0 = W + image_bytes;
+    float *stage0 = (float *)(A0 + (size_t)WG * 16384);
     TcWarpgroup c;
     c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127; c.bar = 1 + c.wg;
     c.A = A0 + (size_t)c.wg * 16384; c.W = W; c.stage = stage0 + (size_t)c.wg * (TC_STAGE_BYTES / 4);
