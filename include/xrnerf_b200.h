@@ -269,6 +269,25 @@ int xrb_ngp_render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
                          float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act, int dens_act,
                          float *rgb_out, float *alpha_out, int32_t *n_samples_out, void *workspace, void *stream);
 
+/* Depth of the two render paths above: the same call with one more output, depth_out f32[n_rays] (non-NULL), right after alpha_out.
+ *   depth = sum_k T_k * alpha_k * t_k
+ * over the ray's samples k (T_k: transmittance in front of sample k, alpha_k: its opacity, t_k: its ray parameter), so depth is in the
+ * units of t (for unit-norm rays: distance in the frame of [aabb0, aabb1]^3). It is NOT divided by alpha (as NerfRender's depth_map);
+ * a ray without samples has depth 0. rgb, alpha and the sample counts are bit-identical to the depth-free call's.
+ * xrb_ngp_render_depth rebuilds t_k from the sample row, t_k = ((aabb0 + x_k * (aabb1 - aabb0)) - o) . d / (d . d) with x_k the warped
+ * position; xrb_ngp_render_fused_depth uses the marched t_k itself. Both agree to fp32 rounding.
+ * Disparity (xrnerf_b200.ngp.disparity) = 1 / max(1e-10, depth / alpha) where alpha > 0 and 0 where alpha == 0: unlike NeRF's disp_map,
+ * which is NaN there, so that an image of rays that miss the scene normalises without NaNs. */
+int xrb_ngp_render_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield,
+                         const float *rays_o, const float *rays_d, int n_rays, int max_samples, float aabb0, float aabb1,
+                         float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                         int dens_act, float *rgb_out, float *alpha_out, float *depth_out, int32_t *numsteps, int32_t *counters, void *workspace,
+                         void *ev_before_field, void *ev_after_field, void *stream);
+int xrb_ngp_render_fused_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield,
+                               const float *rays_o, const float *rays_d, int n_rays, float aabb0, float aabb1, float near_distance,
+                               float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act, int dens_act,
+                               float *rgb_out, float *alpha_out, float *depth_out, int32_t *n_samples_out, void *workspace, void *stream);
+
 
 /* ------------------------------------------------------------------------------------------------
  * NeRF / Mip-NeRF composite + sampling kernels (pure-PyTorch in the reference)

@@ -117,6 +117,8 @@ _SIGS = {
     'xrb_micro_gather': (_i, [P, _i64, _i, _i, C.POINTER(C.c_int64), P, P]),
     'xrb_nerf_zvals': (_i, [_i64, _i, _f, _f, _i, P, P, P]),
     'xrb_ngp_render': (_i, [_cfg, _tab, P, P, P, P, _i, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P, P, P]),
+    'xrb_ngp_render_depth': (_i, [_cfg, _tab, P, P, P, P, _i, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P, P, P, P]),
+    'xrb_ngp_render_fused_depth': (_i, [_cfg, _tab, P, P, P, P, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P]),
 }
 
 EXPORTS = sorted(_SIGS)  # every symbol the header declares and the library currently implements

@@ -79,6 +79,9 @@ constexpr uint32_t SAMPLE_ORDER_MAX_ROWS = 1u << 21;
 int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g);
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
                  int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s);
+// defined in raymarch.cu: xrb_rm_calc_rgb_inference that also writes depth f32[n_rays] (t of each sample rebuilt from its coords row and the ray)
+int launch_composite_depth(const float *raw, const float *coords, const int32_t *numsteps, const float *bg3_host, int n_rays, int rgb_act, int dens_act, const float *rays_o,
+                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s);
 
 #ifdef __CUDACC__
 __device__ __forceinline__ float round_h(float x) { return __half2float(__float2half_rn(x)); }

@@ -16,7 +16,8 @@
 //                            flight per lane per level) straight into the slot row as fp16 pairs
 //                  fold    : (rgb, sigma) of the PREVIOUS chunk come back through the mailbox (its MLP ran during this gather); a
 //                            segmented warp scan composites them and lane i accumulates ray i's transmittance / colour in registers
-//                finally lane i writes rgb/alpha of ray i.
+//                            (DEPTH: alpha * t as a fourth scanned channel, so lane i also accumulates ray i's depth)
+//                finally lane i writes rgb/alpha (and depth) of ray i.
 // Tiles are ELASTIC: when a field warpgroup is idle it closes the current tile with however many 32-row chunks (1..4) have
 // been ticketed (the missing quarters are skipped), so a chunk never waits for other producers. A producer never waits for a
 // result while it owes an arrival, and arrivals never wait for results: nothing can deadlock.
@@ -46,6 +47,7 @@ struct FusedParams {
     uint32_t *sched;     // [0] next ray group, [1] CTAs finished (both zero between launches)
     unsigned long long *dbg_out;   // [gridDim.x][16]: start ns, end ns, smid, tiles, 5 field-phase (warpgroup 0) and 7 producer-phase cycle sums (only written when dbg & 8)
     int dbg;             // developer ablation bits (XRB_FUSED_DBG): 1 skip the hash gather, 2 skip the MLP layers, 4 fake march (11 samples/ray)
+    float *depth_out;    // [n_rays], written by the DEPTH instantiation only (last member: the depth-free kernel reads every other one at its old offset)
 };
 
 struct FusedCtl {
@@ -66,6 +68,8 @@ __device__ __forceinline__ void spin_until_ge(volatile uint32_t *p, uint32_t v) 
     while (*p < v) __nanosleep(20);
 }
 
+// DEPTH = false is the kernel without depth (no register or instruction of the depth channel exists in it).
+template <bool DEPTH>
 __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_fused_kernel(const __grid_constant__ FusedParams P) {
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
@@ -218,7 +222,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                 const float d[3] = {__ldg(P.rays_d + 3 * (size_t)ray), __ldg(P.rays_d + 3 * (size_t)ray + 1), __ldg(P.rays_d + 3 * (size_t)ray + 2)};
                 t = ray_start_t(P.rng, ray, P.lo, P.hi, o, d, P.near_distance, P.cone);
             }
-            float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f;
+            float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f, ad = 0.f;
             bool any_alive;
             do {
                 // ---- march round: up to FR_TCAP samples of my ray (ray_sampler.cu:58-72; pausing keeps the t sequence unchanged)
@@ -252,10 +256,10 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                 const uint32_t incl = warp_incl_scan_u32(m, lane);
                 const uint32_t rbase = incl - m, total = __shfl_sync(0xffffffffu, incl, 31);
 
-                bool pending = false; uint32_t pend_key = 0; float pend_dt = 0.f;   // pend_key: ray-in-group of my sample of the previous chunk (>= 32: none)
+                bool pending = false; uint32_t pend_key = 0; float pend_dt = 0.f, pend_t = 0.f;   // pend_key: ray-in-group of my sample of the previous chunk (>= 32: none)
                 for (uint32_t q0 = 0; q0 < total || pending; q0 += 32) {
                     const bool have_chunk = q0 < total;
-                    float dtc = 0.f; uint32_t key = 32u + lane;
+                    float dtc = 0.f, tc = 0.f; uint32_t key = 32u + lane;
                     PTICK(6);
                     if (have_chunk) {
                         // ---- lane = sample q of the round's ray-ordered stream: which ray, which t
@@ -278,6 +282,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                             x = div_(sub_(add_(oj0, mul_(tt, dj0)), P.lo), diag); y = div_(sub_(add_(oj1, mul_(tt, dj1)), P.lo), diag); z = div_(sub_(add_(oj2, mul_(tt, dj2)), P.lo), diag);
                             wd0 = mul_(add_(dj0, 1.0f), 0.5f); wd1 = mul_(add_(dj1, 1.0f), 0.5f); wd2 = mul_(add_(dj2, 1.0f), 0.5f);
                             dtc = unwarp_dt(warp_dt(calc_dt(tt, P.cone)));   // the value the unfused composite reads back from coords[:,3]
+                            if (DEPTH) tc = tt;
                             key = j;
                         }
 #ifdef XRB_FUSED_TIMERS
@@ -294,11 +299,12 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                         __syncwarp();                                                               // iterations run the scan below diverged (shfl slow path)
                         PTICK(3);
                         const float4 raw = *reinterpret_cast<const float4 *>(mailbox + (size_t)((pw << 1) | (kprev & 1)) * 512 + lane * 16);
-                        float alpha = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
+                        float alpha = 0.f, sx = 0.f, sy = 0.f, sz = 0.f, sd = 0.f;
                         if (pend_key < 32) {
                             const float density = net_to_density(raw.w, P.dens_act);
                             alpha = 1.f - __expf(-density * pend_dt);
                             sx = alpha * net_to_rgb(raw.x, P.rgb_act); sy = alpha * net_to_rgb(raw.y, P.rgb_act); sz = alpha * net_to_rgb(raw.z, P.rgb_act);
+                            if (DEPTH) sd = alpha * pend_t;
                         }
                         float pr = 1.f - alpha;
                         // segmented inclusive scan over the 32 samples; a segment = consecutive samples of one ray
@@ -309,7 +315,8 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                         for (int off = 1; off < 32; off <<= 1) {
                             const float np = __shfl_up_sync(0xffffffffu, pr, off), nx = __shfl_up_sync(0xffffffffu, sx, off), ny = __shfl_up_sync(0xffffffffu, sy, off),
                                         nz = __shfl_up_sync(0xffffffffu, sz, off);
-                            if ((int)lane - off >= seg_start) { sx = nx + np * sx; sy = ny + np * sy; sz = nz + np * sz; pr = np * pr; }
+                            const float nd = DEPTH ? __shfl_up_sync(0xffffffffu, sd, off) : 0.f;
+                            if ((int)lane - off >= seg_start) { sx = nx + np * sx; sy = ny + np * sy; sz = nz + np * sz; if (DEPTH) sd = nd + np * sd; pr = np * pr; }
                         }
                         // lane i == ray i: take the aggregate of my segment (at its last sample inside the previous chunk [q0-32, q0))
                         const uint32_t pq0 = q0 - 32;
@@ -317,16 +324,18 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                         const uint32_t tail = (hi_q - 1 - pq0) & 31;
                         const float gp = __shfl_sync(0xffffffffu, pr, tail), gx = __shfl_sync(0xffffffffu, sx, tail), gy = __shfl_sync(0xffffffffu, sy, tail),
                                     gz = __shfl_sync(0xffffffffu, sz, tail);
-                        if (hi_q > lo_q) { ax += T * gx; ay += T * gy; az += T * gz; T *= gp; }
+                        const float gd = DEPTH ? __shfl_sync(0xffffffffu, sd, tail) : 0.f;
+                        if (hi_q > lo_q) { ax += T * gx; ay += T * gy; az += T * gz; if (DEPTH) ad += T * gd; T *= gp; }
                         pending = false;
                         PTICK(4);
                     }
-                    if (have_chunk) { ++n_submitted; pending = true; pend_key = key; pend_dt = dtc; }
+                    if (have_chunk) { ++n_submitted; pending = true; pend_key = key; pend_dt = dtc; if (DEPTH) pend_t = tc; }
                 }
             } while (any_alive);
             if (ray < (uint32_t)P.n_rays) {
                 P.rgb_out[3 * (size_t)ray] = ax + T * P.bg[0]; P.rgb_out[3 * (size_t)ray + 1] = ay + T * P.bg[1]; P.rgb_out[3 * (size_t)ray + 2] = az + T * P.bg[2];
                 P.alpha_out[ray] = 1.f - T;
+                if (DEPTH) P.depth_out[ray] = ad;
                 if (P.n_samples_out) P.n_samples_out[ray] = (int32_t)nsteps;
             }
         }
@@ -346,6 +355,37 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
 
 constexpr int FUSED_MAX_PROD_PER_SM = 24;
 
+// xrb_ngp_render_fused (DEPTH = false, depth_out unused) and xrb_ngp_render_fused_depth
+template <bool DEPTH>
+static int render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
+                        float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act, int dens_act,
+                        float *rgb_out, float *alpha_out, float *depth_out, int32_t *n_samples_out, void *workspace, void *stream) {
+    int e = check_cfg(cfg); if (e) return e;
+    XRB_REQUIRE(n_rays >= 0, "ngp_render_fused: bad size");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && (depth_out || !DEPTH) && workspace, "ngp_render_fused: null pointer");
+    XRB_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)weight_image & 15) == 0, "ngp_render_fused: workspace must be 256-byte aligned, weight image 16-byte aligned");
+    FusedParams P;
+    e = table_setup(cfg, table, &P.g); if (e) return e;
+    P.table = (const __half2 *)table->table_fp16; P.cells = (const uint8_t *)table->cell_image; P.np = plan_valid(P.g, table->n_packed_levels) ? table->n_packed_levels : 0;
+    P.weight_image = weight_image; P.image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
+    P.density_hidden = cfg->density_hidden; P.color_hidden = cfg->color_hidden;
+    P.bitfield = bitfield; P.rays_o = rays_o; P.rays_d = rays_d; P.n_rays = n_rays;
+    P.lo = aabb0; P.hi = aabb1; P.near_distance = near_distance; P.cone = cone_angle; P.rng = host_rng(seed, n_prior_calls);
+    P.bg[0] = bg3_host[0]; P.bg[1] = bg3_host[1]; P.bg[2] = bg3_host[2]; P.rgb_act = rgb_act; P.dens_act = dens_act;
+    P.rgb_out = rgb_out; P.alpha_out = alpha_out; P.depth_out = depth_out; P.n_samples_out = n_samples_out;
+    { static const int dbg = getenv("XRB_FUSED_DBG") ? atoi(getenv("XRB_FUSED_DBG")) : 0; P.dbg = dbg; }
+    const int sms = sm_count();
+    P.sched = (uint32_t *)workspace; P.tscratch = (float *)((uint8_t *)workspace + 256);
+    P.dbg_out = (unsigned long long *)((uint8_t *)workspace + 256 + (size_t)sms * FUSED_MAX_PROD_PER_SM * 32 * FR_TCAP * sizeof(float));
+    const int64_t n_groups = ((int64_t)n_rays + 31) / 32;
+    const size_t smem = fused_smem_bytes(P.image_bytes);
+    cudaFuncSetAttribute(ngp_render_fused_kernel<DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // per call: the attribute is per device and per image size
+    int grid = sms; if (n_groups < grid) grid = (int)n_groups;
+    ngp_render_fused_kernel<DEPTH><<<grid, (4 * FR_N_WG + FR_N_PROD) * 32, smem, (cudaStream_t)stream>>>(P);
+    return check_launch("ngp_render_fused");
+}
+
 }  // namespace xrb
 
 using namespace xrb;
@@ -360,30 +400,15 @@ size_t xrb_ngp_render_fused_workspace(void) {
 int xrb_ngp_render_fused(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
                          float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act, int dens_act,
                          float *rgb_out, float *alpha_out, int32_t *n_samples_out, void *workspace, void *stream) {
-    int e = check_cfg(cfg); if (e) return e;
-    XRB_REQUIRE(n_rays >= 0, "ngp_render_fused: bad size");
-    if (n_rays == 0) return XRB_OK;
-    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && workspace, "ngp_render_fused: null pointer");
-    XRB_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)weight_image & 15) == 0, "ngp_render_fused: workspace must be 256-byte aligned, weight image 16-byte aligned");
-    FusedParams P;
-    e = table_setup(cfg, table, &P.g); if (e) return e;
-    P.table = (const __half2 *)table->table_fp16; P.cells = (const uint8_t *)table->cell_image; P.np = plan_valid(P.g, table->n_packed_levels) ? table->n_packed_levels : 0;
-    P.weight_image = weight_image; P.image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
-    P.density_hidden = cfg->density_hidden; P.color_hidden = cfg->color_hidden;
-    P.bitfield = bitfield; P.rays_o = rays_o; P.rays_d = rays_d; P.n_rays = n_rays;
-    P.lo = aabb0; P.hi = aabb1; P.near_distance = near_distance; P.cone = cone_angle; P.rng = host_rng(seed, n_prior_calls);
-    P.bg[0] = bg3_host[0]; P.bg[1] = bg3_host[1]; P.bg[2] = bg3_host[2]; P.rgb_act = rgb_act; P.dens_act = dens_act;
-    P.rgb_out = rgb_out; P.alpha_out = alpha_out; P.n_samples_out = n_samples_out;
-    { static const int dbg = getenv("XRB_FUSED_DBG") ? atoi(getenv("XRB_FUSED_DBG")) : 0; P.dbg = dbg; }
-    const int sms = sm_count();
-    P.sched = (uint32_t *)workspace; P.tscratch = (float *)((uint8_t *)workspace + 256);
-    P.dbg_out = (unsigned long long *)((uint8_t *)workspace + 256 + (size_t)sms * FUSED_MAX_PROD_PER_SM * 32 * FR_TCAP * sizeof(float));
-    const int64_t n_groups = ((int64_t)n_rays + 31) / 32;
-    const size_t smem = fused_smem_bytes(P.image_bytes);
-    cudaFuncSetAttribute(ngp_render_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // per call: the attribute is per device and per image size
-    int grid = sms; if (n_groups < grid) grid = (int)n_groups;
-    ngp_render_fused_kernel<<<grid, (4 * FR_N_WG + FR_N_PROD) * 32, smem, (cudaStream_t)stream>>>(P);
-    return check_launch("ngp_render_fused");
+    return render_fused<false>(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act, dens_act,
+                               rgb_out, alpha_out, nullptr, n_samples_out, workspace, stream);
+}
+
+int xrb_ngp_render_fused_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d,
+                               int n_rays, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                               int dens_act, float *rgb_out, float *alpha_out, float *depth_out, int32_t *n_samples_out, void *workspace, void *stream) {
+    return render_fused<true>(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act, dens_act,
+                              rgb_out, alpha_out, depth_out, n_samples_out, workspace, stream);
 }
 
 }  // extern "C"

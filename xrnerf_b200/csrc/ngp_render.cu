@@ -127,6 +127,34 @@ static void launch_sample_order(const float *coords, int max_samples, const int3
     order_scatter_kernel<<<grid, ORDER_THREADS, 0, s>>>(key, (uint32_t)max_samples, n_dev, count, order);
 }
 
+// xrb_ngp_render (depth == false, depth_out unused) and xrb_ngp_render_depth
+static int render_chain(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
+                        int max_samples, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                        int dens_act, float *rgb_out, float *alpha_out, bool depth, float *depth_out, int32_t *numsteps, int32_t *counters, void *workspace, void *ev_before_field,
+                        void *ev_after_field, void *stream) {
+    int e = check_cfg(cfg); if (e) return e;
+    XRB_REQUIRE(n_rays >= 0 && max_samples > 0, "ngp_render: bad size");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && (depth_out || !depth) && numsteps && counters && workspace,
+                "ngp_render: null pointer");
+    cudaStream_t s = (cudaStream_t)stream;
+    const RenderWs w = render_ws(workspace, n_rays, max_samples, nullptr);
+    cudaMemsetAsync(counters, 0, 2 * sizeof(int32_t), s);
+    e = xrb_rm_rays_sampler(rays_o, rays_d, bitfield, nullptr, nullptr, nullptr, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, w.coords, w.rays_index,
+                            numsteps, counters, w.march, stream);
+    if (e) return e;
+    // counters[1] counts overflowed rays too; rows beyond max_samples do not exist, the ordering kernels and launch_field clamp to max_samples
+    // measurement hook: events recorded right before the sample order / after the field kernel let a caller time them inside its own timed region
+    if (ev_before_field) cudaEventRecord((cudaEvent_t)ev_before_field, s);
+    // the keys live in `raw` until the field kernel overwrites it with its outputs
+    launch_sample_order(w.coords, max_samples, counters + 1, (uint32_t *)w.raw, w.count, w.chunk_sum, w.order, s);
+    e = launch_field(cfg, table, nullptr, nullptr, weight_image, w.coords, 7, w.coords + 4, 7, max_samples, counters + 1, w.order, w.raw, 1, false, s);
+    if (ev_after_field) cudaEventRecord((cudaEvent_t)ev_after_field, s);
+    if (e) return e;
+    if (depth) return launch_composite_depth(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rays_o, rays_d, aabb0, aabb1, rgb_out, alpha_out, depth_out, s);
+    return xrb_rm_calc_rgb_inference(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rgb_out, alpha_out, stream);
+}
+
 }  // namespace xrb
 
 extern "C" {
@@ -140,25 +168,16 @@ size_t xrb_ngp_render_workspace(int n_rays, int max_samples) {
 int xrb_ngp_render(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
                    int max_samples, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
                    int dens_act, float *rgb_out, float *alpha_out, int32_t *numsteps, int32_t *counters, void *workspace, void *ev_before_field, void *ev_after_field, void *stream) {
-    int e = xrb::check_cfg(cfg); if (e) return e;
-    XRB_REQUIRE(n_rays >= 0 && max_samples > 0, "ngp_render: bad size");
-    if (n_rays == 0) return XRB_OK;
-    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && numsteps && counters && workspace, "ngp_render: null pointer");
-    cudaStream_t s = (cudaStream_t)stream;
-    const xrb::RenderWs w = xrb::render_ws(workspace, n_rays, max_samples, nullptr);
-    cudaMemsetAsync(counters, 0, 2 * sizeof(int32_t), s);
-    e = xrb_rm_rays_sampler(rays_o, rays_d, bitfield, nullptr, nullptr, nullptr, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, w.coords, w.rays_index,
-                            numsteps, counters, w.march, stream);
-    if (e) return e;
-    // counters[1] counts overflowed rays too; rows beyond max_samples do not exist, the ordering kernels and launch_field clamp to max_samples
-    // measurement hook: events recorded right before the sample order / after the field kernel let a caller time them inside its own timed region
-    if (ev_before_field) cudaEventRecord((cudaEvent_t)ev_before_field, s);
-    // the keys live in `raw` until the field kernel overwrites it with its outputs
-    xrb::launch_sample_order(w.coords, max_samples, counters + 1, (uint32_t *)w.raw, w.count, w.chunk_sum, w.order, s);
-    e = xrb::launch_field(cfg, table, nullptr, nullptr, weight_image, w.coords, 7, w.coords + 4, 7, max_samples, counters + 1, w.order, w.raw, 1, false, s);
-    if (ev_after_field) cudaEventRecord((cudaEvent_t)ev_after_field, s);
-    if (e) return e;
-    return xrb_rm_calc_rgb_inference(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rgb_out, alpha_out, stream);
+    return xrb::render_chain(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act,
+                             dens_act, rgb_out, alpha_out, false, nullptr, numsteps, counters, workspace, ev_before_field, ev_after_field, stream);
+}
+
+int xrb_ngp_render_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
+                         int max_samples, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                         int dens_act, float *rgb_out, float *alpha_out, float *depth_out, int32_t *numsteps, int32_t *counters, void *workspace, void *ev_before_field,
+                         void *ev_after_field, void *stream) {
+    return xrb::render_chain(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act,
+                             dens_act, rgb_out, alpha_out, true, depth_out, numsteps, counters, workspace, ev_before_field, ev_after_field, stream);
 }
 
 }  // extern "C"

@@ -261,12 +261,18 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// what the depth composite (MODE 2) needs to rebuild each sample's t from its warped position
+struct CompositeDepth {
+    const float *rays_o, *rays_d; float lo, diag; float *depth_out;
+};
+
 // MODE 0: training forward (per-ray bg, background only if not truncated; calc_rgb.cu:5-67)
 // MODE 1: inference (global bg, alpha out; calc_rgb.cu:143-206)
+// MODE 2: inference as MODE 1, plus depth = sum of w * t (include/xrnerf_b200.h, xrb_ngp_render_depth)
 template <int MODE>
 __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const float4 *__restrict__ raw, const float *__restrict__ coords, const int32_t *__restrict__ numsteps,
                                                             const int32_t *__restrict__ numsteps_c, const float *__restrict__ bg, float3 bg_global, int rgb_act, int dens_act,
-                                                            float *__restrict__ rgb_out, float *__restrict__ alpha_out) {
+                                                            float *__restrict__ rgb_out, float *__restrict__ alpha_out, CompositeDepth dp) {
     int lane = threadIdx.x & 31;
     const uint32_t n_warps = (gridDim.x * 256) >> 5;
     for (uint32_t ray = (blockIdx.x * 256 + threadIdx.x) >> 5; ray < (uint32_t)n_rays; ray += n_warps) {
@@ -274,33 +280,60 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const fl
     uint32_t n = (uint32_t)ns[2 * (size_t)ray], base = (uint32_t)ns[2 * (size_t)ray + 1];
     float3 b = MODE == 0 ? make_float3(bg[3 * (size_t)ray], bg[3 * (size_t)ray + 1], bg[3 * (size_t)ray + 2]) : bg_global;
     if (n == 0) {
-        if (lane == 0) { rgb_out[3 * (size_t)ray] = b.x; rgb_out[3 * (size_t)ray + 1] = b.y; rgb_out[3 * (size_t)ray + 2] = b.z; if (MODE == 1) alpha_out[ray] = 0.f; }
+        if (lane == 0) {
+            rgb_out[3 * (size_t)ray] = b.x; rgb_out[3 * (size_t)ray + 1] = b.y; rgb_out[3 * (size_t)ray + 2] = b.z;
+            if (MODE >= 1) alpha_out[ray] = 0.f;
+            if (MODE == 2) dp.depth_out[ray] = 0.f;
+        }
         continue;
     }
-    float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f;
+    float o0 = 0.f, o1 = 0.f, o2 = 0.f, d0 = 0.f, d1 = 0.f, d2 = 0.f, inv_dd = 1.f;   // one division per ray, not per sample
+    if (MODE == 2) {
+        o0 = __ldg(dp.rays_o + 3 * (size_t)ray); o1 = __ldg(dp.rays_o + 3 * (size_t)ray + 1); o2 = __ldg(dp.rays_o + 3 * (size_t)ray + 2);
+        d0 = __ldg(dp.rays_d + 3 * (size_t)ray); d1 = __ldg(dp.rays_d + 3 * (size_t)ray + 1); d2 = __ldg(dp.rays_d + 3 * (size_t)ray + 2);
+        inv_dd = 1.f / (d0 * d0 + d1 * d1 + d2 * d2);
+    }
+    float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f, ad = 0.f;
     for (uint32_t k0 = 0; k0 < n; k0 += 32) {
         uint32_t k = k0 + lane; bool valid = k < n;
-        float alpha = 0.f, cx = 0.f, cy = 0.f, cz = 0.f;
+        float alpha = 0.f, cx = 0.f, cy = 0.f, cz = 0.f, t = 0.f;
         if (valid) {
             float4 r = __ldg(raw + base + k);
             float dt = unwarp_dt(__ldg(coords + 7 * (size_t)(base + k) + 3));
             float density = net_to_density(r.w, dens_act);
             alpha = 1.f - __expf(-density * dt);
             cx = net_to_rgb(r.x, rgb_act); cy = net_to_rgb(r.y, rgb_act); cz = net_to_rgb(r.z, rgb_act);
+            if (MODE == 2) {
+                const float *c = coords + 7 * (size_t)(base + k);
+                const float p0 = dp.lo + __ldg(c) * dp.diag - o0, p1 = dp.lo + __ldg(c + 1) * dp.diag - o1, p2 = dp.lo + __ldg(c + 2) * dp.diag - o2;
+                t = (p0 * d0 + p1 * d1 + p2 * d2) * inv_dd;
+            }
         }
         float incl, ex = warp_excl_prod(1.f - alpha, lane, &incl);
         float w = alpha * (T * ex);
         ax += w * cx; ay += w * cy; az += w * cz;
+        if (MODE == 2) ad += w * t;
         T *= __shfl_sync(0xffffffffu, incl, 31);
     }
     ax = warp_sum(ax); ay = warp_sum(ay); az = warp_sum(az);
+    if (MODE == 2) ad = warp_sum(ad);
     if (lane == 0) {
-        bool add_bg = MODE == 1 ? true : (n == (uint32_t)numsteps[2 * (size_t)ray]);  // :61-64 / :199-202
+        bool add_bg = MODE >= 1 ? true : (n == (uint32_t)numsteps[2 * (size_t)ray]);  // :61-64 / :199-202
         if (add_bg) { ax += T * b.x; ay += T * b.y; az += T * b.z; }
         rgb_out[3 * (size_t)ray] = ax; rgb_out[3 * (size_t)ray + 1] = ay; rgb_out[3 * (size_t)ray + 2] = az;
-        if (MODE == 1) alpha_out[ray] = 1.f - T;
+        if (MODE >= 1) alpha_out[ray] = 1.f - T;
+        if (MODE == 2) dp.depth_out[ray] = ad;
     }
     }
+}
+
+// the chain render's composite with depth (xrb_ngp_render_depth; arguments validated there)
+int launch_composite_depth(const float *raw, const float *coords, const int32_t *numsteps, const float *bg3_host, int n_rays, int rgb_act, int dens_act, const float *rays_o,
+                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s) {
+    const CompositeDepth dp{rays_o, rays_d, aabb0, aabb1 - aabb0, depth_out};
+    composite_fwd_kernel<2><<<warp_grid(n_rays), 256, 0, s>>>(n_rays, (const float4 *)raw, coords, numsteps, nullptr, nullptr, make_float3(bg3_host[0], bg3_host[1], bg3_host[2]),
+                                                              rgb_act, dens_act, rgb_out, alpha_out, dp);
+    return check_launch("ngp_render_depth composite");
 }
 
 // compute_rgbs_grad (calc_rgb.cu:70-140)
@@ -565,7 +598,7 @@ int xrb_rm_calc_rgb_forward(const float *raw, const float *coords, const int32_t
     XRB_REQUIRE(((uintptr_t)raw & 15) == 0, "calc_rgb_forward: raw must be 16-byte aligned");
     int blocks = warp_grid(n_rays);
     composite_fwd_kernel<0><<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps, numsteps_compacted, bg, make_float3(0, 0, 0), rgb_act, dens_act,
-                                                                      rgb_out, nullptr);
+                                                                      rgb_out, nullptr, CompositeDepth{});
     return check_launch("calc_rgb_forward");
 }
 
@@ -589,7 +622,8 @@ int xrb_rm_calc_rgb_inference(const float *raw, const float *coords, const int32
     XRB_REQUIRE(((uintptr_t)raw & 15) == 0, "calc_rgb_inference: raw must be 16-byte aligned");
     int blocks = warp_grid(n_rays);
     composite_fwd_kernel<1><<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps, nullptr, nullptr,
-                                                                      make_float3(bg3_host[0], bg3_host[1], bg3_host[2]), rgb_act, dens_act, rgb_out, alpha_out);
+                                                                      make_float3(bg3_host[0], bg3_host[1], bg3_host[2]), rgb_act, dens_act, rgb_out, alpha_out,
+                                                                      CompositeDepth{});
     return check_launch("calc_rgb_inference");
 }
 

@@ -170,6 +170,23 @@ def _rays(t):
     return t.contiguous()
 
 
+def _depth_ptr(depth, n, device):
+    """pointer of a caller-owned depth output: a dense float32 tensor of n elements on the rays' device"""
+    if not torch.is_tensor(depth) or depth.dtype != torch.float32 or depth.numel() != n or depth.device != device:
+        what = f'{depth.dtype} {tuple(depth.shape)} on {depth.device}' if torch.is_tensor(depth) else type(depth).__name__
+        raise _C.XrbError(f'XRB_E_BADARG: depth must be a float32 tensor of {n} elements on {device}, got {what}')
+    return _C.f32(depth)
+
+
+def disparity(depth, alpha):
+    """1 / max(1e-10, depth / alpha) where alpha > 0, and 0 where alpha == 0.
+
+    NeRF's disp_map (nerf_render.py:32-36) is NaN where no weight was accumulated; an NGP image has many rays that miss the scene, and one NaN
+    breaks the `x / max(x)` normalisation of a disparity video, so those rays get 0 here."""
+    hit = alpha > 0
+    return torch.where(hit, 1.0 / torch.clamp(depth / torch.where(hit, alpha, torch.ones_like(alpha)), min=1e-10), torch.zeros_like(alpha))
+
+
 class NgpRenderer:
     """Fused inference render of a ray batch (xrb_ngp_render / xrb_ngp_render_fused): march -> field -> composite, no host sync, persistent workspace.
 
@@ -192,13 +209,16 @@ class NgpRenderer:
         """0-dim bool tensor (device): did the last chain render drop rays because the batch marched more samples than the budget holds?"""
         return counters[1] > self._max_samples
 
-    def render(self, rays_o, rays_d, bitfield, out=None, profile_events=None):
-        """profile_events: optional (torch.cuda.Event, torch.cuda.Event) recorded right before / after the field kernel (bench roofline)."""
+    def render(self, rays_o, rays_d, bitfield, out=None, profile_events=None, depth=None):
+        """profile_events: optional (torch.cuda.Event, torch.cuda.Event) recorded right before / after the field kernel (bench roofline).
+        depth: optional caller-owned float32 tensor of n elements on the rays' device, filled with each ray's depth (xrb_ngp_render_depth,
+        include/xrnerf_b200.h); the returned tuple is the same either way."""
         _C.require_cuda(rays_o, rays_d, bitfield)
         rays_o, rays_d = _rays(rays_o), _rays(rays_d)
+        n = rays_o.shape[0]
+        depth_p = None if depth is None else _depth_ptr(depth, n, rays_o.device)
         f = self.field
         f.refresh()
-        n = rays_o.shape[0]
         max_samples = n * self.budget
         self._max_samples = max_samples
         need = _C.lib.xrb_ngp_render_workspace(n, max_samples)
@@ -214,20 +234,26 @@ class NgpRenderer:
         ev0 = ev1 = None
         if profile_events is not None:
             ev0, ev1 = (_C.C.c_void_p(e.cuda_event) for e in profile_events)
-        _C.check(_C.lib.xrb_ngp_render(f.cfg, f.tab, _C.ptr(f._image), _C.u8(bitfield), _C.ptr(rays_o), _C.ptr(rays_d), n, max_samples, self.aabb[0],
-                                       self.aabb[1], self.near, self.cone, 9121, self.calls, _C.float3(self.bg), self.rgb_act, self.dens_act, _C.f32(rgb), _C.f32(alpha),
-                                       _C.i32(numsteps), _C.i32(counters), _C.ptr(self._ws), ev0, ev1, _C.stream()), 'ngp_render')
+        head = (f.cfg, f.tab, _C.ptr(f._image), _C.u8(bitfield), _C.ptr(rays_o), _C.ptr(rays_d), n, max_samples, self.aabb[0], self.aabb[1], self.near, self.cone, 9121,
+                self.calls, _C.float3(self.bg), self.rgb_act, self.dens_act, _C.f32(rgb), _C.f32(alpha))
+        tail = (_C.i32(numsteps), _C.i32(counters), _C.ptr(self._ws), ev0, ev1, _C.stream())
+        if depth_p is None:
+            _C.check(_C.lib.xrb_ngp_render(*head, *tail), 'ngp_render')
+        else:
+            _C.check(_C.lib.xrb_ngp_render_depth(*head, depth_p, *tail), 'ngp_render_depth')
         self.calls += 1
         return rgb, alpha, numsteps, counters
 
-    def render_fused(self, rays_o, rays_d, bitfield, out=None, ws=None):
+    def render_fused(self, rays_o, rays_d, bitfield, out=None, ws=None, depth=None):
         """Single-launch render (xrb_ngp_render_fused). Returns (rgb [n,3], alpha [n,1], n_samples i32[n]). `ws`: a zero-initialised workspace
-        owned by the caller (one per stream when several batches are in flight); default: one per renderer."""
+        owned by the caller (one per stream when several batches are in flight); default: one per renderer. depth: as in render()
+        (xrb_ngp_render_fused_depth)."""
         _C.require_cuda(rays_o, rays_d, bitfield)
         rays_o, rays_d = _rays(rays_o), _rays(rays_d)
+        n = rays_o.shape[0]
+        depth_p = None if depth is None else _depth_ptr(depth, n, rays_o.device)
         f = self.field
         f.refresh()
-        n = rays_o.shape[0]
         if ws is None:
             if getattr(self, '_ws_fused', None) is None or self._ws_fused.device != rays_o.device:
                 self._ws_fused = torch.zeros(_C.lib.xrb_ngp_render_fused_workspace(), dtype=torch.uint8, device=rays_o.device)
@@ -239,8 +265,12 @@ class NgpRenderer:
                                   torch.empty(n, dtype=torch.int32, device=rays_o.device))
             out = self._out[key]
         rgb, alpha, ns = out
-        _C.check(_C.lib.xrb_ngp_render_fused(f.cfg, f.tab, _C.ptr(f._image), _C.u8(bitfield), _C.ptr(rays_o), _C.ptr(rays_d), n, self.aabb[0], self.aabb[1],
-                                             self.near, self.cone, 9121, self.calls, _C.float3(self.bg), self.rgb_act, self.dens_act, _C.f32(rgb), _C.f32(alpha), _C.i32(ns),
-                                             _C.ptr(ws), _C.stream()), 'ngp_render_fused')
+        head = (f.cfg, f.tab, _C.ptr(f._image), _C.u8(bitfield), _C.ptr(rays_o), _C.ptr(rays_d), n, self.aabb[0], self.aabb[1], self.near, self.cone, 9121, self.calls,
+                _C.float3(self.bg), self.rgb_act, self.dens_act, _C.f32(rgb), _C.f32(alpha))
+        tail = (_C.i32(ns), _C.ptr(ws), _C.stream())
+        if depth_p is None:
+            _C.check(_C.lib.xrb_ngp_render_fused(*head, *tail), 'ngp_render_fused')
+        else:
+            _C.check(_C.lib.xrb_ngp_render_fused_depth(*head, depth_p, *tail), 'ngp_render_fused_depth')
         self.calls += 1
         return rgb, alpha, ns

@@ -179,11 +179,13 @@ class HashNerfNetwork(NerfNetwork):
     def batchify_forward(self, data, is_test=False):
         """Inference over a whole ray set (hashnerf.py:69-71 via nerf.py:50-69: 4096-ray chunks, each = sample (host sync) -> 3 tcnn launches -> composite).
         Here the test path is ONE fused launch per call for any number of rays (xrb_ngp_render_fused; no chunk loop, no host sync, no [S,7]/[S,4] buffers);
-        `fused_inference = False` or training falls back to the reference-shaped chunk loop over forward()."""
+        `fused_inference = False` or training falls back to the reference-shaped chunk loop over forward().
+        The fused path also returns each ray's `depth` [n,1] (sum of w * t, not divided by alpha) and `disp` [n,1] (xrnerf_b200.ngp.disparity: 0 where
+        alpha == 0); the reference-shaped path returns the reference's keys only."""
         smp = self.sampler
         if not (is_test and getattr(self, 'fused_inference', True) and data['rays_o'].is_cuda and hasattr(smp, 'aabb_range')):
             return super().batchify_forward(data, is_test)
-        from ..ngp import NgpRenderer
+        from ..ngp import NgpRenderer, disparity
         smp.check_device(data)
         r = getattr(self, '_renderer', None)
         if r is None:
@@ -191,13 +193,16 @@ class HashNerfNetwork(NerfNetwork):
                                              rgb_act=int(smp.rgb_activation), dens_act=int(smp.density_activation), bg=tuple(float(c) for c in self.render.bg_color))
         import xrnerf_b200.raymarch_cuda as rm
         r.calls = rm.rng_calls['ray_sampler']               # the same jitter stream the unfused path would use next (hidden static pcg32 of the reference, Q9)
-        rgb, alpha, _ = r.render_fused(data['rays_o'].contiguous().float(), data['rays_d'].contiguous().float(), smp.density_grid_bitfield)
+        rays_o = data['rays_o'].contiguous().float()
+        depth = torch.empty((rays_o.shape[0], 1), dtype=torch.float32, device=rays_o.device)
+        rgb, alpha, _ = r.render_fused(rays_o, data['rays_d'].contiguous().float(), smp.density_grid_bitfield, depth=depth)
         rm.rng_calls['ray_sampler'] += 1
-        return {'rgb': rgb.clone(), 'alpha': alpha.clone()}
+        return {'rgb': rgb.clone(), 'alpha': alpha.clone(), 'depth': depth, 'disp': disparity(depth, alpha)}
 
     def val_step(self, data, optimizer=None, **kwargs):
         """hashnerf.py:54-93 (rank-0 loop over validation poses) with the image rendered by one launch and the PSNR taken on the device; every rank renders the
-        poses it is given (SURVEY Q17). Returns the reference's keys plus 'psnr'."""
+        poses it is given (SURVEY Q17). Returns the reference's keys plus 'psnr'; 'disps' holds one [H,W,1] disparity map per pose (the reference
+        declares the list and leaves it empty, as the reference-shaped path `fused_inference = False` still does)."""
         if self.phase == 'test':
             return self.test_step(data, **kwargs)
         # validation may run right after mmcv's EMAHook swapped the parameters through `.data` (Parameter._version unchanged): rebuild the fp16 shadows, the cell
@@ -205,7 +210,7 @@ class HashNerfNetwork(NerfNetwork):
         self.mlp.mark_dirty()
         data = {k: unfold_batching(v) for k, v in data.items()}
         poses, images = data['poses'], data.get('images')
-        rgbs, gt_imgs, psnrs, elapsed = [], [], [], []
+        rgbs, disps, gt_imgs, psnrs, elapsed = [], [], [], [], []
         with torch.no_grad():
             for i in range(poses.shape[0]):
                 t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -213,6 +218,8 @@ class HashNerfNetwork(NerfNetwork):
                 d = self.val_pipeline({'pose': poses[i], 'idx': i})
                 ret = self.batchify_forward(d, is_test=True)
                 rgb = recover_shape(ret['rgb'], d['src_shape'])
+                if 'disp' in ret:
+                    disps.append(recover_shape(ret['disp'], d['src_shape']))
                 if images is not None:
                     alpha = images[i][..., 3:].to(rgb.device)
                     gt = images[i][..., :3].to(rgb.device) * alpha
@@ -222,7 +229,7 @@ class HashNerfNetwork(NerfNetwork):
                 t1.record()
                 rgbs.append(rgb); elapsed.append((t0, t1))
         torch.cuda.synchronize()
-        return {'rgbs': rgbs, 'disps': [], 'gt_imgs': gt_imgs, 'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+        return {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
 
     def test_step(self, data, **kwargs):
         """hashnerf.py:95-111: one spiral pose per call; `data` already holds the pose's rays (rays_o, rays_d, src_shape, idx) from the test pipeline.
@@ -236,10 +243,13 @@ class HashNerfNetwork(NerfNetwork):
         with torch.no_grad():
             d = data if 'rays_o' in data else self.val_pipeline({'pose': data['poses'], 'idx': idx})
             ret = self.batchify_forward(d, is_test=True)
-        rgb, alpha = ret['rgb'], ret['alpha']
+        out = {'spiral_rgb': ret['rgb'], 'spiral_alpha': ret['alpha']}
+        if 'disp' in ret:
+            out['spiral_disp'] = ret['disp']
         if 'src_shape' in d:
-            rgb, alpha = recover_shape(rgb, d['src_shape']), recover_shape(alpha, d['src_shape'])
-        return {'spiral_rgb': rgb, 'spiral_alpha': alpha, 'idx': idx}
+            out = {k: recover_shape(v, d['src_shape']) for k, v in out.items()}
+        out['idx'] = idx
+        return out
 
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
