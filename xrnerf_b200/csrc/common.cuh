@@ -53,6 +53,11 @@ inline int persistent_grid(const void *kernel, int block, size_t smem, int64_t w
     if (per_sm < min_per_sm) per_sm = min_per_sm;  // the calculator has been seen to under-report; extra CTAs simply queue
     return persistent_grid(per_sm, work_ctas);
 }
+// grid of a grid-stride launch: the blocks the work needs, at most per_sm blocks on each of NUM_SMS SMs, never fewer than one
+inline int stride_grid(int64_t blocks, int per_sm) {
+    const int64_t cap = (int64_t)NUM_SMS * per_sm;
+    return (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
+}
 
 // ---------------------------------------------------------------- pcg32 (include/op_include/pcg32/pcg32.h:41-165)
 struct Pcg32 {
@@ -215,11 +220,62 @@ __device__ __forceinline__ float unwarp_dt(float dt) {  // ray_sampler_header.h:
     const float max_stepsize = MIN_CONE_STEPSIZE() * (1 << (NERF_CASCADES - 1));
     return add_(mul_(dt, max_stepsize - MIN_CONE_STEPSIZE()), MIN_CONE_STEPSIZE());
 }
+
+// ---------------------------------------------------------------- sample row coords[S, ROW_FLOATS] (ray_sampler.cu:99-115)
+// warped position (0..2), warped dt (ROW_DT), warped direction (ROW_DIR..ROW_DIR+2) of the sample at t on ray (o, d); diag = hi - lo
+constexpr int ROW_FLOATS = 7, ROW_DT = 3, ROW_DIR = 4;
+__device__ __forceinline__ void sample_warped_pos(const float o[3], const float d[3], float t, float lo, float diag, float x[3]) {  // warp_position
+#pragma unroll
+    for (int k = 0; k < 3; ++k) x[k] = div_(sub_(add_(o[k], mul_(t, d[k])), lo), diag);
+}
+__device__ __forceinline__ void sample_warped_dir(const float d[3], float w[3]) {  // warp_direction
+#pragma unroll
+    for (int k = 0; k < 3; ++k) w[k] = mul_(add_(d[k], 1.0f), 0.5f);
+}
+// one float at a time, in row order
+__device__ __forceinline__ void write_sample_row(float *c, const float o[3], const float d[3], float t, float cone, float lo, float diag) {
+    float x[3], w[3];
+    sample_warped_pos(o, d, t, lo, diag, x);
+    sample_warped_dir(d, w);
+    c[0] = x[0]; c[1] = x[1]; c[2] = x[2];
+    c[ROW_DT] = warp_dt(calc_dt(t, cone));
+    c[ROW_DIR] = w[0]; c[ROW_DIR + 1] = w[1]; c[ROW_DIR + 2] = w[2];
+}
+// the dt the composite reads back from a row, and the same value for the sample at t without a row in memory
+__device__ __forceinline__ float row_dt(const float *c) { return unwarp_dt(__ldg(c + ROW_DT)); }
+__device__ __forceinline__ float sample_row_dt(float t, float cone) { return unwarp_dt(warp_dt(calc_dt(t, cone))); }
+// t of a row rebuilt from its warped position: the projection of (position - o) onto d, inv_dd = 1 / |d|^2
+__device__ __forceinline__ float row_t(const float *c, const float o[3], const float d[3], float inv_dd, float lo, float diag) {
+    const float p0 = lo + __ldg(c) * diag - o[0], p1 = lo + __ldg(c + 1) * diag - o[1], p2 = lo + __ldg(c + 2) * diag - o[2];
+    return (p0 * d[0] + p1 * d[1] + p2 * d[2]) * inv_dd;
+}
+
 // start of the march for ray i (ray_sampler.cu:31,:43-51)
 __device__ __forceinline__ float ray_start_t(Pcg32 rng, uint32_t i, float lo, float hi, const float o[3], const float d[3], float near_distance, float cone) {
     rng.advance((uint64_t)(i * 8u));
     float tmin = fmaxf(aabb_ray_tmin(lo, hi, o, d), near_distance);
     return add_(tmin, mul_(calc_dt(tmin, cone), rng.next_float()));
+}
+// The march of ray (o, d) through the cascaded occupancy grid (ray_sampler.cu:58-72), from t with n samples taken so far. Every occupied
+// sample calls on_sample(n, t, dt) and is counted; the march stops when the ray leaves the box, when n reaches limit (both: returns true,
+// the ray has ended) or when on_sample returns false (returns false, a pause: marching on from the returned t and n continues the same sequence).
+template <typename OnSample>
+__device__ __forceinline__ bool march(float &t, uint32_t &n, uint32_t limit, const float o[3], const float d[3], float lo, float hi, float cone, const uint8_t *__restrict__ bitfield,
+                                      const uint32_t *lut, OnSample &&on_sample) {
+    const float idir[3] = {div_(1.0f, d[0]), div_(1.0f, d[1]), div_(1.0f, d[2])};
+    while (true) {
+        float p[3] = {add_(o[0], mul_(t, d[0])), add_(o[1], mul_(t, d[1])), add_(o[2], mul_(t, d[2]))};
+        if (!(aabb_contains(lo, hi, p[0], p[1], p[2]) && n < limit)) return true;
+        float dt = calc_dt(t, cone);
+        uint32_t mip = (uint32_t)mip_from_dt(dt, p[0], p[1], p[2]);
+        if (occupied_at(p[0], p[1], p[2], bitfield, mip, lut)) {
+            const bool go_on = on_sample(n, t, dt);
+            ++n; t = add_(t, dt);
+            if (!go_on) return false;
+        } else {
+            t = advance_to_next_voxel(t, cone, p, d, idir, NERF_GRIDSIZE >> mip);
+        }
+    }
 }
 
 // activations (ray_sampler_header.h:440-456, :534-574; raymarch_shared.h:615-642). __expf as in the reference.
@@ -240,12 +296,54 @@ __device__ __forceinline__ float net_to_density_deriv(float v, int act) {
     switch (act) { case 0: return 1.f; case 1: return v > 0.f ? 1.f : 0.f; case 2: { float s = logistic(v); return s * (1 - s); } case 3: return __expf(clampf(v, -15.f, 15.f)); }
     return 0.f;
 }
+// what one sample adds to the composite (calc_rgb.cu:31-39): its alpha over dt and its activated colour
+struct CompositeTerm { float alpha, r, g, b; };
+__device__ __forceinline__ CompositeTerm composite_term(float4 raw, float dt, int rgb_act, int dens_act) {
+    return {1.f - __expf(-net_to_density(raw.w, dens_act) * dt), net_to_rgb(raw.x, rgb_act), net_to_rgb(raw.y, rgb_act), net_to_rgb(raw.z, rgb_act)};
+}
 
-// warp scans
+// ---------------------------------------------------------------- warp and block scans
 __device__ __forceinline__ uint32_t warp_incl_scan_u32(uint32_t v, int lane) {
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { uint32_t n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += n; }
     return v;
+}
+__device__ __forceinline__ float warp_incl_sum(float v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += n; }
+    return v;
+}
+__device__ __forceinline__ float warp_incl_prod(float v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v *= n; }
+    return v;
+}
+// exclusive product (1 on lane 0); *incl_out = the inclusive one
+__device__ __forceinline__ float warp_excl_prod(float v, int lane, float *incl_out) {
+    const float incl = warp_incl_prod(v, lane), ex = __shfl_up_sync(0xffffffffu, incl, 1);
+    *incl_out = incl;
+    return lane == 0 ? 1.f : ex;
+}
+// sum over the warp, on every lane (butterfly)
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// exclusive scan of one uint32 per thread over a THREADS-thread block; *total = the block's sum. A kernel that calls it twice
+// needs a __syncthreads() between the calls (both use the same shared words).
+template <int THREADS>
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *total) {
+    __shared__ uint32_t warp_tot[THREADS / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t incl = warp_incl_scan_u32(v, lane);
+    if (lane == 31) warp_tot[w] = incl;
+    __syncthreads();
+    uint32_t off = 0, tot = 0;
+#pragma unroll
+    for (int k = 0; k < THREADS / 32; ++k) { const uint32_t s = warp_tot[k]; if (k < w) off += s; tot += s; }
+    *total = tot;
+    return off + incl - v;
 }
 #endif  // __CUDACC__
 

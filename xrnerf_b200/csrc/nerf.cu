@@ -5,21 +5,6 @@
 
 namespace xrb {
 
-__device__ __forceinline__ float wincl_sum(float v, int lane) {
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += n; }
-    return v;
-}
-__device__ __forceinline__ float wincl_prod(float v, int lane) {
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v *= n; }
-    return v;
-}
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 __device__ __forceinline__ float softplusf_(float x) { return x > 20.f ? x : log1pf(expf(x)); }  // F.softplus(beta=1, threshold=20)
 
@@ -35,6 +20,13 @@ __device__ __forceinline__ void sample_terms(const CompositeParams &p, const flo
     float dens = p.density_act == XRB_ACT_SOFTPLUS ? softplusf_(a) : fmaxf(a, 0.f);
     sd = dens * dist;
     alpha = 1.f - expf(-sd);
+}
+// transmittance before each lane's sample; carry = the running sum of sigma*delta (mip) or product of (1-alpha+1e-10) (nerf) of the earlier chunks
+__device__ __forceinline__ float transmittance(bool mip, bool valid, float sd, float alpha, int lane, float &carry) {
+    float T;
+    if (mip) { const float inc = warp_incl_sum(sd, lane); T = expf(-(carry + inc - sd)); carry += __shfl_sync(0xffffffffu, inc, 31); }
+    else { float incl, ex = warp_excl_prod(valid ? (1.f - alpha + 1e-10f) : 1.f, lane, &incl); T = carry * ex; carry *= __shfl_sync(0xffffffffu, incl, 31); }
+    return T;
 }
 
 // BACKWARD == false: rgb/disp/acc/weights.  BACKWARD == true: d_raw given grad_rgb (loss on rgb only, nerf.py:79-84 / mipnerf.py:49-57)
@@ -59,9 +51,7 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
         int k = k0 + lane; bool valid = k < S;
         float4 r = make_float4(0, 0, 0, 0); float sd = 0, alpha = 0;
         if (valid) sample_terms(p, rw, z, dnorm, k, r, sd, alpha);
-        float T;
-        if (p.mip) { float inc = wincl_sum(sd, lane); T = expf(-(carry + inc - sd)); carry += __shfl_sync(0xffffffffu, inc, 31); }
-        else { float f = valid ? (1.f - alpha + 1e-10f) : 1.f; float inc = wincl_prod(f, lane); float ex = __shfl_up_sync(0xffffffffu, inc, 1); T = carry * (lane == 0 ? 1.f : ex); carry *= __shfl_sync(0xffffffffu, inc, 31); }
+        const float T = transmittance(p.mip, valid, sd, alpha, lane, carry);
         float w = valid ? alpha * T : 0.f;
         float cx = sigmoidf_(r.x) * pad_mul - p.rgb_padding, cy = sigmoidf_(r.y) * pad_mul - p.rgb_padding, cz = sigmoidf_(r.z) * pad_mul - p.rgb_padding;
         if (!BACKWARD) {
@@ -73,7 +63,7 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
         }
     }
     if (!BACKWARD) {
-        ax = wsum(ax); ay = wsum(ay); az = wsum(az); acc = wsum(acc); depth = wsum(depth);
+        ax = warp_sum(ax); ay = warp_sum(ay); az = warp_sum(az); acc = warp_sum(acc); depth = warp_sum(depth);
         if (lane == 0) {
             if (p.white_bkgd) { ax += 1.f - acc; ay += 1.f - acc; az += 1.f - acc; }
             rgb_out[3 * (size_t)ray] = ax; rgb_out[3 * (size_t)ray + 1] = ay; rgb_out[3 * (size_t)ray + 2] = az;
@@ -87,22 +77,20 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
         return;
     }
     // ---- pass 2 (backward): dL/d(sigma*delta_i) needs the suffix sum of w_k*G_k over k > i
-    total_wg = wsum(total_wg);
+    total_wg = warp_sum(total_wg);
     carry = p.mip ? 0.f : 1.f;
     float prefix_wg = 0.f;
     for (int k0 = 0; k0 < S; k0 += 32) {
         int k = k0 + lane; bool valid = k < S;
         float4 r = make_float4(0, 0, 0, 0); float sd = 0, alpha = 0;
         if (valid) sample_terms(p, rw, z, dnorm, k, r, sd, alpha);
-        float T;
-        if (p.mip) { float inc = wincl_sum(sd, lane); T = expf(-(carry + inc - sd)); carry += __shfl_sync(0xffffffffu, inc, 31); }
-        else { float f = valid ? (1.f - alpha + 1e-10f) : 1.f; float inc = wincl_prod(f, lane); float ex = __shfl_up_sync(0xffffffffu, inc, 1); T = carry * (lane == 0 ? 1.f : ex); carry *= __shfl_sync(0xffffffffu, inc, 31); }
+        const float T = transmittance(p.mip, valid, sd, alpha, lane, carry);
         float w = valid ? alpha * T : 0.f;
         float sx = sigmoidf_(r.x), sy = sigmoidf_(r.y), sz = sigmoidf_(r.z);
         float cx = sx * pad_mul - p.rgb_padding, cy = sy * pad_mul - p.rgb_padding, cz = sz * pad_mul - p.rgb_padding;
         float wb = p.white_bkgd ? 1.f : 0.f;
         float G = gx * (cx - wb) + gy * (cy - wb) + gz * (cz - wb);
-        float inc_wg = wincl_sum(w * G, lane);
+        float inc_wg = warp_incl_sum(w * G, lane);
         float suffix = total_wg - (prefix_wg + inc_wg);
         prefix_wg += __shfl_sync(0xffffffffu, inc_wg, 31);
         if (valid) {
@@ -138,7 +126,7 @@ __global__ void __launch_bounds__(PDF_WARPS * 32) sample_pdf_kernel(int n_rays, 
     const int nb = S - 1;   // bins (mid-points): S-1 ; pdf entries: S-2 ; cdf entries: S-1
     float part = 0.f;
     for (int k = lane; k < S - 2; k += 32) part += w[k + 1] + 1e-5f;
-    const float wsum_all = wsum(part);
+    const float wsum_all = warp_sum(part);
     for (int k = lane; k < nb; k += 32) bins[k] = 0.5f * (z[k + 1] + z[k]);
     __syncwarp();
     if (lane == 0) {  // sequential cumsum like torch.cumsum on the reference's CPU path
@@ -448,7 +436,7 @@ __global__ void __launch_bounds__(PDF_WARPS * 32) mip_resample_kernel(int n_rays
         float v = 0.5f * (fmaxf(wm1, w0) + fmaxf(w0, wp1)) + resample_padding;
         w[k] = v; part += v;
     }
-    float wsum_all = wsum(part);
+    float wsum_all = warp_sum(part);
     const float eps = 1e-5f;
     float padding = fmaxf(0.f, eps - wsum_all);
     const float add = padding / (float)S;
@@ -612,8 +600,8 @@ int xrb_nerf_posenc(const float *pts, const float *viewdirs, int64_t n_pts, int 
     if (n_pts == 0) return XRB_OK;
     XRB_REQUIRE(pts && viewdirs && embedded, "posenc: null pointer");
     int64_t total = n_pts * (6 + 6 * (int64_t)(multires + multires_dirs));
-    int64_t blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    posenc_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(n_pts, samples_per_ray, multires, multires_dirs, pts, viewdirs, embedded);
+    const int blocks = stride_grid((total + 255) / 256, 16);
+    posenc_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_pts, samples_per_ray, multires, multires_dirs, pts, viewdirs, embedded);
     return check_launch("posenc");
 }
 
@@ -623,8 +611,8 @@ int xrb_mip_embed(const float *z_vals, const float *rays_o, const float *rays_d,
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(z_vals && rays_o && rays_d && radii && viewdirs && embedded && ((means_out == nullptr) == (covs_out == nullptr)), "mip_embed: null pointer");
     int64_t total = (int64_t)n_rays * n_samples * (6 * (max_deg_point - min_deg_point) + 3 + 6 * (max_deg_view - min_deg_view));
-    int64_t blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    mip_embed_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view, max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, embedded,
+    const int blocks = stride_grid((total + 255) / 256, 16);
+    mip_embed_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view, max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, embedded,
                                                                    means_out, covs_out);
     return check_launch("mip_embed");
 }
@@ -636,22 +624,25 @@ int xrb_mip_ipe_tiles_rays(const float *z_vals, const float *rays_o, const float
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(z_vals && rays_o && rays_d && radii && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "mip_ipe_tiles_rays: null/misaligned pointer");
     const int aux = (6 * (max_deg_point - min_deg_point) + 63) / 64;
-    int64_t total = ((n_rays * n_samples + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
+    int64_t total = ((n_rays * n_samples + 127) / 128) * 128 * (aux + 1) * 8;
+    const int blocks = stride_grid((total + 255) / 256, 16);
     if (max_deg_point - min_deg_point == 16 && max_deg_view - min_deg_view == 4 && min_deg_point >= -100 && max_deg_point <= 100 && min_deg_view >= -100 && max_deg_view <= 100) {
         // the reference configuration (configs/mipnerf/*.py): specialised kernel
-        int64_t items = ((n_rays * n_samples + 127) / 128) * 256, fb = (items + 255) / 256; if (fb > NUM_SMS * 16) fb = NUM_SMS * 16;
-        mip_ipe_tiles_fast_kernel<16, 4><<<(int)fb, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, min_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
+        int64_t items = ((n_rays * n_samples + 127) / 128) * 256;
+        const int fb = stride_grid((items + 255) / 256, 16);
+        mip_ipe_tiles_fast_kernel<16, 4><<<fb, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, min_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
         return check_launch("mip_ipe_tiles_rays");
     }
-    mip_ipe_tiles_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view, max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs,
+    mip_ipe_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view, max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs,
                                                                        (uint8_t *)enc_image);
     return check_launch("mip_ipe_tiles_rays");
 }
 
 // called by xrb_nerf_posenc_tiles / xrb_nerf_posenc_tiles_rays (nerf_mlp_tc.cu) for the reference configuration multires=10, multires_dirs=4
 int xrb_internal_posenc_tiles_fast(const float *pts, const float *viewdirs, int64_t n_rows, int samples_per_ray, void *enc_image, const float *rays_o, const float *rays_d, void *stream) {
-    int64_t items = ((n_rows + 127) / 128) * 256, fb = (items + 255) / 256; if (fb > NUM_SMS * 16) fb = NUM_SMS * 16;
-    posenc_tiles_fast_kernel<10, 4><<<(int)fb, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_rows, samples_per_ray, (uint8_t *)enc_image, rays_o, rays_d);
+    int64_t items = ((n_rows + 127) / 128) * 256;
+    const int fb = stride_grid((items + 255) / 256, 16);
+    posenc_tiles_fast_kernel<10, 4><<<fb, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_rows, samples_per_ray, (uint8_t *)enc_image, rays_o, rays_d);
     return check_launch("posenc_tiles");
 }
 
@@ -670,8 +661,8 @@ int xrb_ngp_batch_sample(const float *poses, const float *images_rgba, int n_ima
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(poses && images_rgba && row_idx && rays_o && rays_d && target_s && alpha && img_ids && bg_color, "ngp_batch_sample: null pointer");
     XRB_REQUIRE(((uintptr_t)images_rgba & 15) == 0, "ngp_batch_sample: images must be 16-byte aligned");
-    int64_t blocks = (n + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    ngp_batch_sample_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(poses, images_rgba, n_images, H, W, fx, fy, cx, cy, row_idx, n, u_bg, host_rng(seed, n_prior_calls), rays_o, rays_d,
+    const int blocks = stride_grid((n + 255) / 256, 16);
+    ngp_batch_sample_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(poses, images_rgba, n_images, H, W, fx, fy, cx, cy, row_idx, n, u_bg, host_rng(seed, n_prior_calls), rays_o, rays_d,
                                                                           target_s, alpha, img_ids, bg_color);
     return check_launch("ngp_batch_sample");
 }
@@ -684,8 +675,8 @@ int xrb_nerf_get_rays(const float *c2w_host, int H, int W, float fx, float fy, f
     XRB_REQUIRE(c2w_host && rays_o && rays_d, "get_rays: null pointer");
     RayGenParams p; for (int k = 0; k < 12; ++k) p.c2w[k] = c2w_host[k];
     p.fx = fx; p.fy = fy; p.cx = cx; p.cy = cy; p.H = H; p.W = W; p.convention = convention;
-    int64_t blocks = (n + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    get_rays_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(p, pixel_idx, n, rays_o, rays_d, viewdirs, radii);
+    const int blocks = stride_grid((n + 255) / 256, 16);
+    get_rays_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, pixel_idx, n, rays_o, rays_d, viewdirs, radii);
     return check_launch("get_rays");
 }
 
@@ -693,8 +684,8 @@ int xrb_nerf_zvals(int64_t n_rays, int n_samples, float near_, float far_, int l
     XRB_REQUIRE(n_rays >= 0 && n_samples >= 2, "zvals: bad size");
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(z_vals, "zvals: null pointer");
-    int64_t blocks = (n_rays * n_samples + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    zvals_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, near_, far_, lindisp, u, z_vals);
+    const int blocks = stride_grid((n_rays * n_samples + 255) / 256, 16);
+    zvals_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, near_, far_, lindisp, u, z_vals);
     return check_launch("zvals");
 }
 

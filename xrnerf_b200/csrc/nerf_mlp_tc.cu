@@ -322,8 +322,9 @@ int xrb_nerf_pack_embedded(const float *embedded, int64_t n_rows, int input_ch, 
     if (n_rows == 0) return XRB_OK;
     XRB_REQUIRE(embedded && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_pack_embedded: null/misaligned pointer");
     const int aux = (input_ch + 63) / 64;
-    int64_t total = ((n_rows + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    pack_embedded_tiles_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(embedded, n_rows, input_ch, input_ch_dirs, aux, (uint8_t *)enc_image);
+    int64_t total = ((n_rows + 127) / 128) * 128 * (aux + 1) * 8;
+    const int blocks = stride_grid((total + 255) / 256, 16);
+    pack_embedded_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(embedded, n_rows, input_ch, input_ch_dirs, aux, (uint8_t *)enc_image);
     return check_launch("nerf_pack_embedded");
 }
 
@@ -333,8 +334,9 @@ int xrb_nerf_posenc_tiles(const float *pts, const float *viewdirs, int64_t n_pts
     XRB_REQUIRE(pts && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles: null/misaligned pointer");
     if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(pts, viewdirs, n_pts, samples_per_ray, enc_image, nullptr, nullptr, stream);
     const int aux = (3 + 6 * multires + 63) / 64;
-    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    posenc_tiles_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, nullptr, nullptr);
+    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8;
+    const int blocks = stride_grid((total + 255) / 256, 16);
+    posenc_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, nullptr, nullptr);
     return check_launch("nerf_posenc_tiles");
 }
 
@@ -346,8 +348,9 @@ int xrb_nerf_posenc_tiles_rays(const float *rays_o, const float *rays_d, const f
     if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, enc_image, rays_o, rays_d, stream);
     const int aux = (3 + 6 * multires + 63) / 64;
     const int64_t n_pts = n_rays * samples_per_ray;
-    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8, blocks = (total + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
-    posenc_tiles_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(z_vals, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, rays_o, rays_d);
+    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8;
+    const int blocks = stride_grid((total + 255) / 256, 16);
+    posenc_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z_vals, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, rays_o, rays_d);
     return check_launch("nerf_posenc_tiles_rays");
 }
 

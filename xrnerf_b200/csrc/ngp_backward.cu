@@ -337,8 +337,8 @@ int xrb_ngp_huber5_grad(const float *rgb, const float *target, int64_t n_element
     XRB_REQUIRE(n_elements >= 0 && delta > 0.f, "huber5_grad: bad arguments");
     if (n_elements == 0) return XRB_OK;
     XRB_REQUIRE(rgb && target && grad_out && loss_accum, "huber5_grad: null pointer");
-    int64_t blocks = (n_elements + 255) / 256; if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-    huber5_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(rgb, target, n_elements, delta, grad_out, loss_accum);
+    const int blocks = stride_grid((n_elements + 255) / 256, 8);
+    huber5_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rgb, target, n_elements, delta, grad_out, loss_accum);
     return check_launch("huber5_grad");
 }
 
@@ -347,8 +347,8 @@ int xrb_pack_bf16(const float *src, void *dst_bf16, int64_t n, void *stream) {
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(src && dst_bf16, "pack_bf16: null pointer");
     XRB_REQUIRE(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst_bf16 & 7) == 0, "pack_bf16: misaligned");
-    int64_t blocks = (n / 4 + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16; if (blocks < 1) blocks = 1;
-    pack_bf16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16 *)dst_bf16, n);
+    const int blocks = stride_grid((n / 4 + 255) / 256, 16);
+    pack_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16 *)dst_bf16, n);
     return check_launch("pack_bf16");
 }
 
@@ -406,12 +406,12 @@ static int adam_launch(float *param, void *param_fp16, const void *grad, bool gr
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(param && grad && exp_avg && exp_avg_sq, "adam_step: null pointer");
     double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
-    int64_t blocks = (n + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
+    const int blocks = stride_grid((n + 255) / 256, 16);
     if (grad_bf16)
-        adam_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const __nv_bfloat16 *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay,
+        adam_kernel<__nv_bfloat16><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const __nv_bfloat16 *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay,
                                                                                  (float)bc1, (float)(1.0 / sqrt(bc2)), 1.f / grad_div, ema, ema_momentum);
     else
-        adam_kernel<float><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const float *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, (float)bc1,
+        adam_kernel<float><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const float *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, (float)bc1,
                                                                          (float)(1.0 / sqrt(bc2)), 1.f / grad_div, ema, ema_momentum);
     return check_launch("adam_step");
 }

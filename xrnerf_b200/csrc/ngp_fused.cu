@@ -9,7 +9,7 @@
 //                with wgmma (weights resident in shared memory, accumulators in registers) and posts (rgb, sigma) of every row to the
 //                mailbox of the producer warp that submitted it. Tiles alternate between the two warpgroups.
 //   warps 8..23  "producer" warps, each autonomous over groups of 32 rays taken from a global counter:
-//                  march   : lane i marches ray i (same arithmetic as xrb_rm_rays_sampler, bit-identical sample positions), in
+//                  march   : lane i marches ray i (the march() of xrb_rm_rays_sampler, so bit-identical sample positions), in
 //                            rounds of <= 64 samples per ray; the sample parameters t go to a per-warp scratch (L1/L2 resident)
 //                  encode  : the round's samples are laid out in ray order (warp prefix sum); 32 at a time, lane = sample: a quarter
 //                            of a tile slot is claimed (ticket from a shared counter) and the 16 hash levels are gathered (8 loads in
@@ -235,20 +235,11 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                 if (alive) {
                     const float o[3] = {__ldg(P.rays_o + 3 * (size_t)ray), __ldg(P.rays_o + 3 * (size_t)ray + 1), __ldg(P.rays_o + 3 * (size_t)ray + 2)};
                     const float d[3] = {__ldg(P.rays_d + 3 * (size_t)ray), __ldg(P.rays_d + 3 * (size_t)ray + 1), __ldg(P.rays_d + 3 * (size_t)ray + 2)};
-                    const float idir[3] = {div_(1.0f, d[0]), div_(1.0f, d[1]), div_(1.0f, d[2])};
                     float *tl = tb + (size_t)lane * FR_TCAP;
-                    while (true) {
-                        float p[3] = {add_(o[0], mul_(t, d[0])), add_(o[1], mul_(t, d[1])), add_(o[2], mul_(t, d[2]))};
-                        if (!(aabb_contains(P.lo, P.hi, p[0], p[1], p[2]) && nsteps < NERF_STEPS)) { alive = false; break; }
-                        float dt = calc_dt(t, P.cone);
-                        uint32_t mip = (uint32_t)mip_from_dt(dt, p[0], p[1], p[2]);
-                        if (occupied_at(p[0], p[1], p[2], P.bitfield, mip, ctl->morton)) {
-                            tl[m] = t; ++m; ++nsteps; t = add_(t, dt);
-                            if (m == FR_TCAP) break;
-                        } else {
-                            t = advance_to_next_voxel(t, P.cone, p, d, idir, NERF_GRIDSIZE >> mip);
-                        }
-                    }
+                    alive = !march(t, nsteps, NERF_STEPS, o, d, P.lo, P.hi, P.cone, P.bitfield, ctl->morton, [&](uint32_t, float t, float) {
+                        tl[m] = t;
+                        return ++m != FR_TCAP;
+                    });
                 }
                 __syncwarp();
                 PTICK(0);
@@ -273,23 +264,23 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                             if (cand < 32 && b <= q) j = cand;
                         }
                         const uint32_t bj = __shfl_sync(0xffffffffu, rbase, j);
-                        float x = 0.5f, y = 0.5f, z = 0.5f, wd0 = 0.5f, wd1 = 0.5f, wd2 = 0.5f;
+                        float x[3] = {0.5f, 0.5f, 0.5f}, wd[3] = {0.5f, 0.5f, 0.5f};
                         if (valid) {
                             const float tt = *(volatile float *)(tb + (size_t)j * FR_TCAP + (q - bj));
                             const size_t rj = (size_t)grp * 32 + j;
-                            const float oj0 = __ldg(P.rays_o + 3 * rj), oj1 = __ldg(P.rays_o + 3 * rj + 1), oj2 = __ldg(P.rays_o + 3 * rj + 2);
-                            const float dj0 = __ldg(P.rays_d + 3 * rj), dj1 = __ldg(P.rays_d + 3 * rj + 1), dj2 = __ldg(P.rays_d + 3 * rj + 2);
-                            x = div_(sub_(add_(oj0, mul_(tt, dj0)), P.lo), diag); y = div_(sub_(add_(oj1, mul_(tt, dj1)), P.lo), diag); z = div_(sub_(add_(oj2, mul_(tt, dj2)), P.lo), diag);
-                            wd0 = mul_(add_(dj0, 1.0f), 0.5f); wd1 = mul_(add_(dj1, 1.0f), 0.5f); wd2 = mul_(add_(dj2, 1.0f), 0.5f);
-                            dtc = unwarp_dt(warp_dt(calc_dt(tt, P.cone)));   // the value the unfused composite reads back from coords[:,3]
+                            const float oj[3] = {__ldg(P.rays_o + 3 * rj), __ldg(P.rays_o + 3 * rj + 1), __ldg(P.rays_o + 3 * rj + 2)};
+                            const float dj[3] = {__ldg(P.rays_d + 3 * rj), __ldg(P.rays_d + 3 * rj + 1), __ldg(P.rays_d + 3 * rj + 2)};
+                            sample_warped_pos(oj, dj, tt, P.lo, diag, x);
+                            sample_warped_dir(dj, wd);
+                            dtc = sample_row_dt(tt, P.cone);   // the value the unfused composite reads back from the row
                             if (DEPTH) tc = tt;
                             key = j;
                         }
 #ifdef XRB_FUSED_TIMERS
-                        if (P.dbg & 8) { if (__float_as_uint(x + y + z + dtc) == 0x7fc12345u) pc[6] += 1; }   // force the loads to have landed
+                        if (P.dbg & 8) { if (__float_as_uint(x[0] + x[1] + x[2] + dtc) == 0x7fc12345u) pc[6] += 1; }   // force the loads to have landed
 #endif
                         PTICK(1);
-                        submit_chunk(x, y, z, wd0, wd1, wd2);
+                        submit_chunk(x[0], x[1], x[2], wd[0], wd[1], wd[2]);
                         PTICK(2);
                     }
                     // ---- results of the previous chunk (its tile ran on the tensor core during this gather): composite
@@ -301,9 +292,8 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
                         const float4 raw = *reinterpret_cast<const float4 *>(mailbox + (size_t)((pw << 1) | (kprev & 1)) * 512 + lane * 16);
                         float alpha = 0.f, sx = 0.f, sy = 0.f, sz = 0.f, sd = 0.f;
                         if (pend_key < 32) {
-                            const float density = net_to_density(raw.w, P.dens_act);
-                            alpha = 1.f - __expf(-density * pend_dt);
-                            sx = alpha * net_to_rgb(raw.x, P.rgb_act); sy = alpha * net_to_rgb(raw.y, P.rgb_act); sz = alpha * net_to_rgb(raw.z, P.rgb_act);
+                            const CompositeTerm s = composite_term(raw, pend_dt, P.rgb_act, P.dens_act);
+                            alpha = s.alpha; sx = alpha * s.r; sy = alpha * s.g; sz = alpha * s.b;
                             if (DEPTH) sd = alpha * pend_t;
                         }
                         float pr = 1.f - alpha;

@@ -260,8 +260,8 @@ int xrb_tcnn_cast_params(const float *src, void *dst_fp16, int64_t n, void *stre
     if (n == 0) return XRB_OK;
     XRB_REQUIRE(src && dst_fp16, "cast_params: null pointer");
     XRB_REQUIRE(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst_fp16 & 7) == 0, "cast_params: misaligned");
-    int64_t blocks = (n / 4 + 255) / 256; if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16; if (blocks < 1) blocks = 1;
-    cast_f32_to_f16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src, (__half *)dst_fp16, n);
+    const int blocks = stride_grid((n / 4 + 255) / 256, 16);
+    cast_f32_to_f16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, (__half *)dst_fp16, n);
     return check_launch("cast_params");
 }
 
@@ -290,8 +290,7 @@ int xrb_ngp_build_cell_image(const xrb_ngp_config *cfg, const void *table_fp16, 
     XRB_REQUIRE(((uintptr_t)cell_image & 31) == 0 && ((uintptr_t)table_fp16 & 15) == 0, "build_cell_image: cell image must be 32-byte, table 16-byte aligned");
     HashGridDev g; hashgrid_build(cfg, &g);
     const uint64_t n_words = cell_image_layout(&g, n_packed_levels) / 4;
-    uint64_t blocks = (n_words + 255) / 256; if (blocks > (uint64_t)NUM_SMS * 32) blocks = (uint64_t)NUM_SMS * 32;
-    cell_image_build_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(g, (const __half2 *)table_fp16, (uint32_t *)cell_image, n_packed_levels, n_words);
+    cell_image_build_kernel<<<stride_grid((int64_t)(n_words + 255) / 256, 32), 256, 0, (cudaStream_t)stream>>>(g, (const __half2 *)table_fp16, (uint32_t *)cell_image, n_packed_levels, n_words);
     return check_launch("build_cell_image");
 }
 

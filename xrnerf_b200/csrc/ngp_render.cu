@@ -38,33 +38,18 @@ __global__ void __launch_bounds__(ORDER_THREADS) order_key_kernel(const float *_
     const uint32_t n = order_rows(max_samples, n_dev), lane = threadIdx.x & 31;
     for (uint32_t j0 = (blockIdx.x * ORDER_THREADS + threadIdx.x) & ~31u; j0 < n; j0 += gridDim.x * ORDER_THREADS) {   // warp-uniform trip count
         const uint32_t j = j0 + lane;
-        const uint32_t k = j < n ? order_key(coords + 7 * (size_t)j) : NO_KEY;
+        const uint32_t k = j < n ? order_key(coords + ROW_FLOATS * (size_t)j) : NO_KEY;
         if (j < n) key[j] = k;
         const uint32_t peers = __match_any_sync(0xffffffffu, k);
         if (k != NO_KEY && lane == (uint32_t)__ffs(peers) - 1) atomicAdd(count + k, (uint32_t)__popc(peers));
     }
 }
 
-// exclusive scan of one value per thread over the block; *total = the block's sum
-__device__ __forceinline__ uint32_t order_block_excl_scan(uint32_t v, uint32_t *total) {
-    __shared__ uint32_t warp_tot[ORDER_THREADS / 32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const uint32_t incl = warp_incl_scan_u32(v, lane);
-    if (lane == 31) warp_tot[w] = incl;
-    __syncthreads();
-    uint32_t off = 0, tot = 0;
-#pragma unroll
-    for (int k = 0; k < ORDER_THREADS / 32; ++k) { const uint32_t s = warp_tot[k]; if (k < w) off += s; tot += s; }
-    __syncthreads();   // warp_tot may be reused by the next call
-    *total = tot;
-    return off + incl - v;
-}
-
 // total of each chunk of ORDER_CHUNK buckets
 __global__ void __launch_bounds__(ORDER_THREADS) order_chunk_sum_kernel(const uint4 *__restrict__ count, uint32_t *__restrict__ chunk_sum) {
     const uint4 v = count[blockIdx.x * ORDER_THREADS + threadIdx.x];
     uint32_t tot;
-    order_block_excl_scan(v.x + v.y + v.z + v.w, &tot);
+    block_excl_scan<ORDER_THREADS>(v.x + v.y + v.z + v.w, &tot);
     if (threadIdx.x == 0) chunk_sum[blockIdx.x] = tot;
 }
 
@@ -72,9 +57,10 @@ __global__ void __launch_bounds__(ORDER_THREADS) order_chunk_sum_kernel(const ui
 __global__ void __launch_bounds__(ORDER_THREADS) order_scan_kernel(uint4 *__restrict__ count, const uint32_t *__restrict__ chunk_sum) {
     uint32_t base = 0, tot;
     for (uint32_t t = threadIdx.x; t < blockIdx.x; t += ORDER_THREADS) base += chunk_sum[t];
-    order_block_excl_scan(base, &base);
+    block_excl_scan<ORDER_THREADS>(base, &base);
+    __syncthreads();   // the second scan reuses the first one's shared words
     uint4 v = count[blockIdx.x * ORDER_THREADS + threadIdx.x];
-    uint32_t o = base + order_block_excl_scan(v.x + v.y + v.z + v.w, &tot);
+    uint32_t o = base + block_excl_scan<ORDER_THREADS>(v.x + v.y + v.z + v.w, &tot);
     uint4 r;
     r.x = o; o += v.x; r.y = o; o += v.y; r.z = o; o += v.z; r.w = o;
     count[blockIdx.x * ORDER_THREADS + threadIdx.x] = r;
@@ -105,9 +91,9 @@ static RenderWs render_ws(void *ws, int n_rays, int max_samples, size_t *bytes) 
     size_t a = align256(xrb_rm_rays_sampler_workspace(n_rays));
     w.march = p;
     w.coords = (float *)(p + a);
-    w.raw = w.coords + (size_t)max_samples * 7;
+    w.raw = w.coords + (size_t)max_samples * ROW_FLOATS;
     w.order = (uint32_t *)(w.raw + (size_t)max_samples * 4);
-    a += align256((size_t)max_samples * (7 + 4 + 1) * sizeof(float));
+    a += align256((size_t)max_samples * (ROW_FLOATS + 4 + 1) * sizeof(float));
     w.count = (uint32_t *)(p + a); a += ORDER_BUCKETS * sizeof(uint32_t);
     w.chunk_sum = (uint32_t *)(p + a); a += ORDER_SCAN_BLOCKS * sizeof(uint32_t);
     w.rays_index = (int32_t *)(p + a); a += (size_t)n_rays * sizeof(int32_t);
@@ -118,8 +104,7 @@ static RenderWs render_ws(void *ws, int n_rays, int max_samples, size_t *bytes) 
 // order[0, n) = a permutation of the rows [0, n), n = min(*n_dev, max_samples), bucketed by position (nothing is written when n > SAMPLE_ORDER_MAX_ROWS).
 // `key` (max_samples words) is scratch.
 static void launch_sample_order(const float *coords, int max_samples, const int32_t *n_dev, uint32_t *key, uint32_t *count, uint32_t *chunk_sum, uint32_t *order, cudaStream_t s) {
-    size_t b = ((size_t)max_samples + ORDER_THREADS - 1) / ORDER_THREADS, cap = (size_t)NUM_SMS * 8;
-    const int grid = (int)(b < cap ? b : cap);
+    const int grid = stride_grid(((int64_t)max_samples + ORDER_THREADS - 1) / ORDER_THREADS, 8);
     cudaMemsetAsync(count, 0, ORDER_BUCKETS * sizeof(uint32_t), s);
     order_key_kernel<<<grid, ORDER_THREADS, 0, s>>>(coords, (uint32_t)max_samples, n_dev, key, count);
     order_chunk_sum_kernel<<<ORDER_SCAN_BLOCKS, ORDER_THREADS, 0, s>>>((const uint4 *)count, chunk_sum);
@@ -148,7 +133,7 @@ static int render_chain(const xrb_ngp_config *cfg, const xrb_ngp_table *table, c
     if (ev_before_field) cudaEventRecord((cudaEvent_t)ev_before_field, s);
     // the keys live in `raw` until the field kernel overwrites it with its outputs
     launch_sample_order(w.coords, max_samples, counters + 1, (uint32_t *)w.raw, w.count, w.chunk_sum, w.order, s);
-    e = launch_field(cfg, table, nullptr, nullptr, weight_image, w.coords, 7, w.coords + 4, 7, max_samples, counters + 1, w.order, w.raw, 1, false, s);
+    e = launch_field(cfg, table, nullptr, nullptr, weight_image, w.coords, ROW_FLOATS, w.coords + ROW_DIR, ROW_FLOATS, max_samples, counters + 1, w.order, w.raw, 1, false, s);
     if (ev_after_field) cudaEventRecord((cudaEvent_t)ev_after_field, s);
     if (e) return e;
     if (depth) return launch_composite_depth(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rays_o, rays_d, aabb0, aabb1, rgb_out, alpha_out, depth_out, s);

@@ -202,8 +202,8 @@ int xrb_peer_free(void *ptr) { if (!ptr) return XRB_OK; cudaError_t e = cudaFree
 int xrb_peer_publish_grads(const xrb_peer_layout *L, const float *grad_table, const float *grad_mlp, uint32_t step, void *stream) {
     PeerDev P; int e = peer_dev(L, &P); if (e) return e;
     XRB_REQUIRE(grad_table && (grad_mlp || L->n_mlp == 0) && step > 0, "peer_publish_grads: null pointer / step must start at 1");
-    int64_t blocks = (P.per * P.world / 4 + 255) / 256; if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-    peer_publish_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(P, grad_table, grad_mlp, step);
+    const int blocks = stride_grid((P.per * P.world / 4 + 255) / 256, 8);
+    peer_publish_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(P, grad_table, grad_mlp, step);
     return check_launch("peer_publish_grads");
 }
 
@@ -220,8 +220,8 @@ int xrb_peer_adam_step(const xrb_peer_layout *L, float *master_slice, float *exp
     AdamHyper h{lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)(1.0 / sqrt(bc2)), 1.f / (float)P.world, ema_momentum};
     MlpGroup g0{mlp0->param, (__half *)mlp0->param_fp16, mlp0->exp_avg, mlp0->exp_avg_sq, mlp0->ema, mlp0->n, mlp0->g_off};
     MlpGroup g1{mlp1->param, (__half *)mlp1->param_fp16, mlp1->exp_avg, mlp1->exp_avg_sq, mlp1->ema, mlp1->n, mlp1->g_off};
-    int64_t blocks = ((cnt + 7) / 8 + 255) / 256; if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8; if (blocks < 1) blocks = 1;
-    peer_adam_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(P, master_slice, exp_avg_slice, exp_avg_sq_slice, ema_slice, cnt, h, g0, g1, step);
+    const int blocks = stride_grid(((cnt + 7) / 8 + 255) / 256, 8);
+    peer_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(P, master_slice, exp_avg_slice, exp_avg_sq_slice, ema_slice, cnt, h, g0, g1, step);
     peer_wait_done_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(P, step);
     return check_launch("peer_adam_step");
 }

@@ -23,55 +23,15 @@ int check_launch(const char *what) {
 }
 
 // ============================================================================ ray march
-// One thread per ray. emit==false: count steps (ray_sampler.cu:58-72). emit==true: write rows (:99-115).
+// Count pass: one thread per ray marches it (common.cuh march(), ray_sampler.cu:58-72). Emit pass: one warp per ray writes its rows (:99-115).
 constexpr uint32_t TCAP = 64;                      // per-ray sample-t slots cached inline by the count pass
 constexpr uint32_t OVF_CAP = NERF_STEPS - TCAP;    // a ray with more samples gets ONE overflow chunk of this many slots (bump-allocated), so the emit
                                                    // pass can rebuild all of its rows in parallel; only when the chunk pool is exhausted is it re-marched
 struct OvfPool { uint32_t *counter; float *area; uint32_t n_chunks; int32_t *chunk_of; };
 
-template <bool EMIT>
-__device__ __forceinline__ uint32_t march_ray(const float o[3], const float d[3], float lo, float hi, float startt, float cone,
-                                              const uint8_t *__restrict__ bitfield, uint32_t limit, float *__restrict__ coords, float *__restrict__ tbuf = nullptr,
-                                              const uint32_t *lut = nullptr, const OvfPool *pool = nullptr, uint32_t ray = 0) {
-    const float idir[3] = {div_(1.0f, d[0]), div_(1.0f, d[1]), div_(1.0f, d[2])};
-    float wdir[3], diag = sub_(hi, lo);
-    if (EMIT) { wdir[0] = mul_(add_(d[0], 1.0f), 0.5f); wdir[1] = mul_(add_(d[1], 1.0f), 0.5f); wdir[2] = mul_(add_(d[2], 1.0f), 0.5f); }
-    uint32_t j = 0; float t = startt;
-    float *ovf = nullptr;
-    while (true) {
-        float p[3] = {add_(o[0], mul_(t, d[0])), add_(o[1], mul_(t, d[1])), add_(o[2], mul_(t, d[2]))};
-        if (!(aabb_contains(lo, hi, p[0], p[1], p[2]) && j < limit)) break;
-        float dt = calc_dt(t, cone);
-        uint32_t mip = (uint32_t)mip_from_dt(dt, p[0], p[1], p[2]);
-        if (occupied_at(p[0], p[1], p[2], bitfield, mip, lut)) {
-            if (EMIT) {
-                float *c = coords + 7 * (size_t)j;
-                c[0] = div_(sub_(p[0], lo), diag); c[1] = div_(sub_(p[1], lo), diag); c[2] = div_(sub_(p[2], lo), diag);  // warp_position
-                c[3] = warp_dt(dt);
-                c[4] = wdir[0]; c[5] = wdir[1]; c[6] = wdir[2];
-            } else if (tbuf) {
-                if (j < TCAP) tbuf[j] = t;
-                else if (pool) {
-                    if (j == TCAP) {
-                        const uint32_t c = atomicAdd(pool->counter, 1u);
-                        const bool got = c < pool->n_chunks;
-                        pool->chunk_of[ray] = got ? (int32_t)c : -1;
-                        ovf = got ? pool->area + (size_t)c * OVF_CAP : nullptr;
-                    }
-                    if (ovf) ovf[j - TCAP] = t;
-                }
-            }
-            ++j; t = add_(t, dt);
-        } else {
-            t = advance_to_next_voxel(t, cone, p, d, idir, NERF_GRIDSIZE >> mip);
-        }
-    }
-    return j;
-}
-
 constexpr int MARCH_BLOCK = 128;
 // grid for warp-per-ray kernels with persistent (ray-strided) warps
-static inline int warp_grid(int n_rays) { size_t b = ((size_t)n_rays * 32 + 255) / 256, cap = (size_t)NUM_SMS * 8; return (int)(b < cap ? (b ? b : 1) : cap); }
+static inline int warp_grid(int n_rays) { return stride_grid(((int64_t)n_rays * 32 + 255) / 256, 8); }
 
 struct MarchWs {  // device workspace layout for N rays
     uint32_t *local_excl;  // [N]
@@ -94,20 +54,6 @@ inline MarchWs march_ws(void *ws, int n) {
     return w;
 }
 
-// block-wide exclusive scan of one uint32 per thread (MARCH_BLOCK threads); returns exclusive prefix, total in *total
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *total) {
-    __shared__ uint32_t warp_tot[MARCH_BLOCK / 32];
-    int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    uint32_t incl = warp_incl_scan_u32(v, lane);
-    if (lane == 31) warp_tot[w] = incl;
-    __syncthreads();
-    uint32_t off = 0, tot = 0;
-#pragma unroll
-    for (int k = 0; k < MARCH_BLOCK / 32; ++k) { uint32_t s = warp_tot[k]; if (k < w) off += s; tot += s; }
-    *total = tot;
-    return off + incl - v;
-}
-
 // Count pass: thread i marches ray i, caching its sample t values, and the block scans the per-ray sample counts.
 __global__ void __launch_bounds__(MARCH_BLOCK) march_count_kernel(int n_rays, const float *__restrict__ rays_o, const float *__restrict__ rays_d,
                                                                   const uint8_t *__restrict__ bitfield, float lo, float hi, float near_distance, float cone,
@@ -121,34 +67,41 @@ __global__ void __launch_bounds__(MARCH_BLOCK) march_count_kernel(int n_rays, co
     if (i < (uint32_t)n_rays) {
         float o[3] = {rays_o[3 * (size_t)i], rays_o[3 * (size_t)i + 1], rays_o[3 * (size_t)i + 2]};
         float d[3] = {rays_d[3 * (size_t)i], rays_d[3 * (size_t)i + 1], rays_d[3 * (size_t)i + 2]};
-        float st = ray_start_t(rng, i, lo, hi, o, d, near_distance, cone);
-        startt_out[i] = st;
-        n = march_ray<false>(o, d, lo, hi, st, cone, bitfield, NERF_STEPS, nullptr, tbuf ? tbuf + (size_t)i * TCAP : nullptr, lut, tbuf ? &pool : nullptr, i);
+        float t = ray_start_t(rng, i, lo, hi, o, d, near_distance, cone);
+        startt_out[i] = t;
+        float *tl = tbuf ? tbuf + (size_t)i * TCAP : nullptr, *ovf = nullptr;   // tbuf == nullptr: count only
+        const OvfPool *pp = tbuf ? &pool : nullptr;   // through a pointer, as ever: the by-value form made the training step 0.4 % slower (H100 80GB HBM3, 700 W)
+        march(t, n, NERF_STEPS, o, d, lo, hi, cone, bitfield, lut, [&](uint32_t j, float t, float) {
+            if (!tl) return true;
+            if (j < TCAP) { tl[j] = t; return true; }
+            if (!pp) return true;
+            if (j == TCAP) {   // claim the overflow chunk
+                const uint32_t c = atomicAdd(pp->counter, 1u);
+                const bool got = c < pp->n_chunks;
+                pp->chunk_of[i] = got ? (int32_t)c : -1;
+                ovf = got ? pp->area + (size_t)c * OVF_CAP : nullptr;
+            }
+            if (ovf) ovf[j - TCAP] = t;
+            return true;
+        });
         numsteps[2 * (size_t)i] = (int32_t)n;
     }
     uint32_t tot;
-    uint32_t ex = block_excl_scan(n, &tot);
+    uint32_t ex = block_excl_scan<MARCH_BLOCK>(n, &tot);
     if (i < (uint32_t)n_rays) local_excl[i] = ex;
     if (threadIdx.x == 0) block_sum[blockIdx.x] = tot;
 }
 
 // single block: exclusive scan of block sums, base/ray counters bookkeeping (counters[] accumulate like the reference's atomics)
 __global__ void __launch_bounds__(1024) march_scan_kernel(int n_blocks, uint32_t *__restrict__ block_sum, uint32_t *__restrict__ misc, int32_t *__restrict__ counters) {
-    __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry_s;
-    int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     if (threadIdx.x == 0) carry_s = 0;
     __syncthreads();
     for (int b0 = 0; b0 < n_blocks; b0 += 1024) {
         int b = b0 + threadIdx.x;
-        uint32_t v = b < n_blocks ? block_sum[b] : 0u;
-        uint32_t incl = warp_incl_scan_u32(v, lane);
-        if (lane == 31) warp_tot[w] = incl;
-        __syncthreads();
-        uint32_t off = 0, tot = 0;
-        for (int k = 0; k < 32; ++k) { uint32_t s = warp_tot[k]; if (k < w) off += s; tot += s; }
+        uint32_t tot, ex = block_excl_scan<1024>(b < n_blocks ? block_sum[b] : 0u, &tot);
         uint32_t carry = carry_s;
-        if (b < n_blocks) block_sum[b] = carry + off + incl - v;
+        if (b < n_blocks) block_sum[b] = carry + ex;
         __syncthreads();
         if (threadIdx.x == 0) carry_s = carry + tot;
         __syncthreads();
@@ -188,20 +141,20 @@ __global__ void __launch_bounds__(256) march_emit_kernel(int n_rays, const float
                 const float o[3] = {rays_o[3 * (size_t)i], rays_o[3 * (size_t)i + 1], rays_o[3 * (size_t)i + 2]};
                 const float d[3] = {rays_d[3 * (size_t)i], rays_d[3 * (size_t)i + 1], rays_d[3 * (size_t)i + 2]};
                 const float diag = sub_(hi, lo);
-                const float w0 = mul_(add_(d[0], 1.0f), 0.5f), w1 = mul_(add_(d[1], 1.0f), 0.5f), w2 = mul_(add_(d[2], 1.0f), 0.5f);
                 // rows whose t is cached (inline slots, then the ray's overflow chunk) are rebuilt by all lanes
                 const int32_t chunk = n > TCAP ? chunk_of[i] : -1;
                 const float *tl = tbuf + (size_t)i * TCAP, *to = chunk >= 0 ? ovf + (size_t)chunk * OVF_CAP : nullptr;
                 const uint32_t n_par = n <= TCAP ? n : (to ? n : TCAP - 1);
-                for (uint32_t j = lane; j < n_par; j += 32) {
-                    float t = j < TCAP ? tl[j] : to[j - TCAP];
-                    float *c = coords_out + 7 * (size_t)(base + j);
-                    c[0] = div_(sub_(add_(o[0], mul_(t, d[0])), lo), diag); c[1] = div_(sub_(add_(o[1], mul_(t, d[1])), lo), diag); c[2] = div_(sub_(add_(o[2], mul_(t, d[2])), lo), diag);
-                    c[3] = warp_dt(calc_dt(t, cone));
-                    c[4] = w0; c[5] = w1; c[6] = w2;
-                }
+                for (uint32_t j = lane; j < n_par; j += 32) write_sample_row(coords_out + ROW_FLOATS * (size_t)(base + j), o, d, j < TCAP ? tl[j] : to[j - TCAP], cone, lo, diag);
                 // chunk pool exhausted: lane 0 resumes the march AT cached sample TCAP-1 (the march state is just t) and emits the remaining rows (ray_sampler.cu:99-115)
-                if (n_par < n && lane == 0) march_ray<true>(o, d, lo, hi, tl[TCAP - 1], cone, bitfield, n - (TCAP - 1), coords_out + 7 * (size_t)(base + TCAP - 1));
+                if (n_par < n && lane == 0) {
+                    float *rows = coords_out + ROW_FLOATS * (size_t)(base + TCAP - 1);
+                    float t = tl[TCAP - 1]; uint32_t j = 0;
+                    march(t, j, n - (TCAP - 1), o, d, lo, hi, cone, bitfield, nullptr, [&](uint32_t j, float t, float) {
+                        write_sample_row(rows + ROW_FLOATS * (size_t)j, o, d, t, cone, lo, diag);
+                        return true;
+                    });
+                }
             }
         }
     }
@@ -213,7 +166,7 @@ __global__ void __launch_bounds__(MARCH_BLOCK) compact_count_kernel(int n_rays, 
                                                                     uint32_t *__restrict__ block_sum) {
     uint32_t i = blockIdx.x * MARCH_BLOCK + threadIdx.x;
     uint32_t n = i < (uint32_t)n_rays ? (uint32_t)numsteps[2 * (size_t)i] : 0u;
-    uint32_t tot, ex = block_excl_scan(n, &tot);
+    uint32_t tot, ex = block_excl_scan<MARCH_BLOCK>(n, &tot);
     if (i < (uint32_t)n_rays) local_excl[i] = ex;
     if (threadIdx.x == 0) block_sum[blockIdx.x] = tot;
 }
@@ -228,8 +181,8 @@ __global__ void __launch_bounds__(256) compact_copy_kernel(int n_rays, uint32_t 
     uint32_t cbase = misc[0] + block_off[ray / MARCH_BLOCK] + local_excl[ray];
     uint32_t nc = min(max_compacted - min(max_compacted, cbase), n);  // :64
     if (lane == 0) { numsteps_c[2 * (size_t)ray] = (int32_t)nc; numsteps_c[2 * (size_t)ray + 1] = (int32_t)cbase; if (nc) atomicAdd((unsigned int *)ray_counter, 1u); }
-    const float *src = coords_in + 7 * (size_t)base; float *dst = coords_out + 7 * (size_t)cbase;
-    for (uint32_t k = lane; k < nc * 7; k += 32) dst[k] = src[k];
+    const float *src = coords_in + ROW_FLOATS * (size_t)base; float *dst = coords_out + ROW_FLOATS * (size_t)cbase;
+    for (uint32_t k = lane; k < nc * ROW_FLOATS; k += 32) dst[k] = src[k];
 }
 
 // rays of a compacted batch whose every marched sample survived the compaction (numsteps_c.count == numsteps.count): the rays a training step really trains
@@ -242,25 +195,6 @@ __global__ void __launch_bounds__(256) count_trained_kernel(int n_rays, const in
 }
 
 // ============================================================================ compositing (calc_rgb.cu)
-__device__ __forceinline__ float warp_excl_prod(float v, int lane, float *incl_out) {
-    float incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl *= n; }
-    float ex = __shfl_up_sync(0xffffffffu, incl, 1);
-    *incl_out = incl;
-    return lane == 0 ? 1.f : ex;
-}
-__device__ __forceinline__ float warp_incl_sum(float v, int lane) {
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { float n = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += n; }
-    return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // what the depth composite (MODE 2) needs to rebuild each sample's t from its warped position
 struct CompositeDepth {
     const float *rays_o, *rays_d; float lo, diag; float *depth_out;
@@ -287,31 +221,23 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const fl
         }
         continue;
     }
-    float o0 = 0.f, o1 = 0.f, o2 = 0.f, d0 = 0.f, d1 = 0.f, d2 = 0.f, inv_dd = 1.f;   // one division per ray, not per sample
+    float o[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f}, inv_dd = 1.f;   // one division per ray, not per sample
     if (MODE == 2) {
-        o0 = __ldg(dp.rays_o + 3 * (size_t)ray); o1 = __ldg(dp.rays_o + 3 * (size_t)ray + 1); o2 = __ldg(dp.rays_o + 3 * (size_t)ray + 2);
-        d0 = __ldg(dp.rays_d + 3 * (size_t)ray); d1 = __ldg(dp.rays_d + 3 * (size_t)ray + 1); d2 = __ldg(dp.rays_d + 3 * (size_t)ray + 2);
-        inv_dd = 1.f / (d0 * d0 + d1 * d1 + d2 * d2);
+        o[0] = __ldg(dp.rays_o + 3 * (size_t)ray); o[1] = __ldg(dp.rays_o + 3 * (size_t)ray + 1); o[2] = __ldg(dp.rays_o + 3 * (size_t)ray + 2);
+        d[0] = __ldg(dp.rays_d + 3 * (size_t)ray); d[1] = __ldg(dp.rays_d + 3 * (size_t)ray + 1); d[2] = __ldg(dp.rays_d + 3 * (size_t)ray + 2);
+        inv_dd = 1.f / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
     }
     float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f, ad = 0.f;
     for (uint32_t k0 = 0; k0 < n; k0 += 32) {
         uint32_t k = k0 + lane; bool valid = k < n;
-        float alpha = 0.f, cx = 0.f, cy = 0.f, cz = 0.f, t = 0.f;
+        CompositeTerm s{0.f, 0.f, 0.f, 0.f}; float t = 0.f;
         if (valid) {
-            float4 r = __ldg(raw + base + k);
-            float dt = unwarp_dt(__ldg(coords + 7 * (size_t)(base + k) + 3));
-            float density = net_to_density(r.w, dens_act);
-            alpha = 1.f - __expf(-density * dt);
-            cx = net_to_rgb(r.x, rgb_act); cy = net_to_rgb(r.y, rgb_act); cz = net_to_rgb(r.z, rgb_act);
-            if (MODE == 2) {
-                const float *c = coords + 7 * (size_t)(base + k);
-                const float p0 = dp.lo + __ldg(c) * dp.diag - o0, p1 = dp.lo + __ldg(c + 1) * dp.diag - o1, p2 = dp.lo + __ldg(c + 2) * dp.diag - o2;
-                t = (p0 * d0 + p1 * d1 + p2 * d2) * inv_dd;
-            }
+            s = composite_term(__ldg(raw + base + k), row_dt(coords + ROW_FLOATS * (size_t)(base + k)), rgb_act, dens_act);
+            if (MODE == 2) t = row_t(coords + ROW_FLOATS * (size_t)(base + k), o, d, inv_dd, dp.lo, dp.diag);
         }
-        float incl, ex = warp_excl_prod(1.f - alpha, lane, &incl);
-        float w = alpha * (T * ex);
-        ax += w * cx; ay += w * cy; az += w * cz;
+        float incl, ex = warp_excl_prod(1.f - s.alpha, lane, &incl);
+        float w = s.alpha * (T * ex);
+        ax += w * s.r; ay += w * s.g; az += w * s.b;
         if (MODE == 2) ad += w * t;
         T *= __shfl_sync(0xffffffffu, incl, 31);
     }
@@ -353,22 +279,21 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(int n_rays, const fl
     float T = 1.f, px = 0.f, py = 0.f, pz = 0.f;  // running transmittance / prefix colour carried across 32-sample chunks
     for (uint32_t k0 = 0; k0 < n; k0 += 32) {
         uint32_t k = k0 + lane; bool valid = k < n;
-        float4 r = make_float4(0, 0, 0, 0); float dt = 0.f, alpha = 0.f, cx = 0.f, cy = 0.f, cz = 0.f;
+        float4 r = make_float4(0, 0, 0, 0); float dt = 0.f; CompositeTerm s{0.f, 0.f, 0.f, 0.f};
         if (valid) {
             r = __ldg(raw + base + k);
-            dt = unwarp_dt(__ldg(coords + 7 * (size_t)(base + k) + 3));
-            alpha = 1.f - __expf(-net_to_density(r.w, dens_act) * dt);
-            cx = net_to_rgb(r.x, rgb_act); cy = net_to_rgb(r.y, rgb_act); cz = net_to_rgb(r.z, rgb_act);
+            dt = row_dt(coords + ROW_FLOATS * (size_t)(base + k));
+            s = composite_term(r, dt, rgb_act, dens_act);
         }
-        float incl, ex = warp_excl_prod(1.f - alpha, lane, &incl);
-        float Tb = T * ex, w = alpha * Tb, Ta = Tb * (1.f - alpha);
-        float sx = px + warp_incl_sum(w * cx, lane), sy = py + warp_incl_sum(w * cy, lane), sz = pz + warp_incl_sum(w * cz, lane);  // rgb_ray2 after this sample
+        float incl, ex = warp_excl_prod(1.f - s.alpha, lane, &incl);
+        float Tb = T * ex, w = s.alpha * Tb, Ta = Tb * (1.f - s.alpha);
+        float sx = px + warp_incl_sum(w * s.r, lane), sy = py + warp_incl_sum(w * s.g, lane), sz = pz + warp_incl_sum(w * s.b, lane);  // rgb_ray2 after this sample
         if (valid) {
             float4 o;
             o.x = loss_scale * (w * gx * net_to_rgb_deriv(r.x, rgb_act) + fmaxf(0.0f, l2 * r.x));
             o.y = loss_scale * (w * gy * net_to_rgb_deriv(r.y, rgb_act) + fmaxf(0.0f, l2 * r.y));
             o.z = loss_scale * (w * gz * net_to_rgb_deriv(r.z, rgb_act) + fmaxf(0.0f, l2 * r.z));
-            float dot = gx * (Ta * cx - (fx - sx)) + (gy * (Ta * cy - (fy - sy)) + gz * (Ta * cz - (fz - sz)));
+            float dot = gx * (Ta * s.r - (fx - sx)) + (gy * (Ta * s.g - (fy - sy)) + gz * (Ta * s.b - (fz - sz)));
             o.w = loss_scale * (net_to_density_deriv(r.w, dens_act) * (dt * dot)) + (r.w < 0.f ? -l1 : 0.0f);
             dl_draw[base + k] = o;
         }
@@ -380,11 +305,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(int n_rays, const fl
 
 // ============================================================================ occupancy grid kernels
 constexpr int GRID_THREADS = 256;
-static inline int stream_grid(size_t work_items) {
-    size_t blocks = (work_items + GRID_THREADS - 1) / GRID_THREADS;
-    size_t cap = (size_t)NUM_SMS * 8;
-    return (int)(blocks < cap ? (blocks ? blocks : 1) : cap);
-}
+static inline int stream_grid(size_t work_items) { return stride_grid((int64_t)((work_items + GRID_THREADS - 1) / GRID_THREADS), 8); }
 
 // mark_untrained_density_grid.cu:5-51; always writes (Q1)
 __global__ void __launch_bounds__(GRID_THREADS) mark_untrained_kernel(uint32_t n_elements, float *__restrict__ grid, uint32_t n_images, const float2 *__restrict__ focal,
@@ -585,8 +506,7 @@ int xrb_ngp_count_trained_rays(const int32_t *numsteps, const int32_t *numsteps_
     XRB_REQUIRE(n_rays >= 0, "count_trained_rays: negative size");
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(numsteps && numsteps_compacted && accum && ((uintptr_t)accum & 7) == 0, "count_trained_rays: null / misaligned pointer");
-    int blocks = (n_rays + 255) / 256; if (blocks > NUM_SMS * 4) blocks = NUM_SMS * 4;
-    count_trained_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, numsteps, numsteps_compacted, (unsigned long long *)accum);
+    count_trained_kernel<<<stride_grid((n_rays + 255) / 256, 4), 256, 0, (cudaStream_t)stream>>>(n_rays, numsteps, numsteps_compacted, (unsigned long long *)accum);
     return check_launch("count_trained_rays");
 }
 
