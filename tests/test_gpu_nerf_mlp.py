@@ -181,6 +181,31 @@ def test_posenc_tile_images_match_fp32_posenc():
             assert (diff > 0).float().mean().item() <= (0.0 if generic else 1e-3), (generic, ray_mode)
 
 
+@pytest.mark.parametrize('ic,icd', [(63, 27), (96, 27)])
+def test_pack_embedded_image_decodes_with_the_slab_layout(ic, icd):
+    """xrb_nerf_pack_embedded's image read back with the layout nerf_mlp._slab documents, not with the kernels' own helpers: the point columns,
+    then the direction columns from the last block on, hold embedded.half(); padding columns and the rows past the last one are +0.
+    300 rows: two full tiles and a ragged one."""
+    from xrnerf_b200 import _C
+    n = 300
+    g = torch.Generator(device='cuda').manual_seed(11)
+    emb = torch.randn((n, ic + icd), device='cuda', generator=g)
+    n_tiles, n_blk = (n + 127) // 128, (ic + 63) // 64 + 1
+    nbytes = _C.lib.xrb_nerf_enc_image_bytes(n, ic)
+    assert nbytes == n_tiles * n_blk * 16384
+    img = torch.full((nbytes,), 0xA5, dtype=torch.uint8, device='cuda')
+    _C.check(_C.lib.xrb_nerf_pack_embedded(_C.ptr(emb), n, ic, icd, _C.ptr(img), _C.stream()))
+    r, k = np.meshgrid(np.arange(128), np.arange(64), indexing='ij')
+    off = (r >> 3) * 1024 + (r & 7) * 128 + (((k >> 3) ^ (r & 7)) << 4) + (k & 7) * 2          # byte of element (r, k) of a block
+    blocks = img.cpu().numpy().view(np.float16).reshape(n_tiles, n_blk, 8192)[:, :, off // 2]  # [tile, block, row, col]
+    got = blocks.transpose(0, 2, 1, 3).reshape(n_tiles * 128, n_blk * 64)
+    want = np.zeros_like(got)
+    e = emb.half().cpu().numpy()
+    want[:n, :ic] = e[:, :ic]
+    want[:n, (n_blk - 1) * 64:(n_blk - 1) * 64 + icd] = e[:, ic:]
+    assert np.array_equal(got.view(np.uint16), want.view(np.uint16))
+
+
 def test_fused_mip_renderer_matches_registry_network():
     """MipNerfRenderer (IPE tile images -> wgmma MLP -> composite, 2 levels) vs MipNerfNetwork.forward(is_test=True) with the fp32 library-GEMM MLP.
     Tolerance: fp16-operand MLP over 12 layers, then two composites and a resampling that moves with the coarse weights: rgb 1e-2."""

@@ -1,7 +1,9 @@
-// xrnerf_b200 — NeRF / Mip-NeRF per-ray kernels that are pure PyTorch in the reference (≈25 tiny ATen kernels per
-// render call, a full sort + expanded gathers per sample_pdf call; SURVEY §3a): one launch each, one WARP per ray,
-// lanes over samples with shuffle scans. References relative to /root/reference/xrnerf/models/.
+// xrnerf_b200 — NeRF / Mip-NeRF kernels for what is pure PyTorch in the reference (≈25 tiny ATen kernels per render call, a full
+// sort + expanded gathers per sample_pdf call; SURVEY §3a). Compositing, sample_pdf and Mip-NeRF resampling: one launch each, one WARP per
+// ray, lanes over samples with shuffle scans. Every encoder: positional encoding and Mip-NeRF IPE, into fp32 `embedded` rows or straight
+// into the fp16 tile images the NerfMLP kernels read. Ray generation and z values. References relative to /root/reference/xrnerf/models/.
 #include "common.cuh"
+#include "tc.cuh"
 
 namespace xrb {
 
@@ -172,26 +174,40 @@ __global__ void __launch_bounds__(PDF_WARPS * 32) sample_pdf_kernel(int n_rays, 
     }
 }
 
-// BaseEmbedder.forward (embedders/base.py:57-74): one thread per output element (coalesced row writes)
-__global__ void __launch_bounds__(256) posenc_kernel(int64_t n_pts, int samples_per_ray, int multires, int multires_dirs, const float *__restrict__ pts,
-                                                     const float *__restrict__ viewdirs, float *__restrict__ out) {
-    const int c_pts = 3 + 6 * multires, c_dir = 3 + 6 * multires_dirs, C = c_pts + c_dir;
-    const int64_t total = n_pts * C;
-    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        int64_t i = idx / C; int c = (int)(idx - i * C);
-        const float *src; int cc;
-        if (c < c_pts) { src = pts + 3 * i; cc = c; } else { src = viewdirs + 3 * (i / samples_per_ray); cc = c - c_pts; }
-        float v;
-        if (cc < 3) v = src[cc];
-        else { int q = cc - 3, band = q / 6, r = q % 6; float x = src[r % 3] * exp2f((float)band); v = r < 3 ? sinf(x) : cosf(x); }
-        out[idx] = v;
-    }
+// ---- NeRF / Mip-NeRF encodings. Each encoding column is written once below and used both by the fp32 kernels (one thread per output element of
+// `embedded`) and by the generic tile-image kernels, so a tile image holds the fp16 roundings of exactly the fp32 kernels' values. The tile images
+// (tc.cuh layout) are what the NerfMLP kernels TMA-load: per 128-row tile the point-encoding block(s), zero padded to 64 columns each, then the
+// direction block.
+constexpr float HALF_PI = 1.5707963267948966f;
+__device__ __forceinline__ float sel3(const float *a, int i) { return i == 0 ? a[0] : i == 1 ? a[1] : a[2]; }   // keeps a register array out of local memory
+
+// BaseEmbedder (embedders/base.py:26-52), column c of the encoding of x: x_c for c < 3, then per band b: sin(2^b x_a), cos(2^b x_a) for a = 0, 1, 2
+__device__ __forceinline__ float posenc_col(const float *x, int c) {
+    if (c < 3) return x[c];
+    const int q = c - 3, band = q / 6, r = q % 6;
+    const float y = x[r % 3] * exp2f((float)band);
+    return r < 3 ? sinf(y) : cosf(y);
+}
+// MipNerfEmbedder (mipnerf_embedder.py:35-41, :55-60), IPE column c < c_ipe = 6 n_deg of a sample's Gaussian: exp(-0.5 cov_a 4^deg) sin(mean_a 2^deg),
+// in the second half of the columns sin(mean_a 2^deg + pi/2)
+__device__ __forceinline__ float ipe_col(const float *mean, const float *cov, int c, int c_ipe, int min_deg) {
+    const int q = c < c_ipe / 2 ? c : c - c_ipe / 2, ax = q % 3;
+    const float sc = exp2f((float)(q / 3 + min_deg));
+    float y = sel3(mean, ax) * sc;
+    const float yv = sel3(cov, ax) * sc * sc;
+    if (c >= c_ipe / 2) y += HALF_PI;
+    return expf(-0.5f * yv) * sinf(y);
+}
+// MipNerfEmbedder view-direction column c < 3 + 6 n_deg_v: vd_c for c < 3, then sin(2^deg vd_a), then sin(2^deg vd_a + pi/2)
+__device__ __forceinline__ float mip_dir_col(const float *vd, int c, int n_deg_v, int min_deg_view) {
+    if (c < 3) return vd[c];
+    const int q = c - 3, halfn = 3 * n_deg_v, qq = q < halfn ? q : q - halfn;
+    float x = vd[qq % 3] * exp2f((float)(qq / 3 + min_deg_view));
+    if (q >= halfn) x += HALF_PI;
+    return sinf(x);
 }
 
-
-// Mip-NeRF: cast_rays (networks/utils/mip.py:117-129, conical frustum -> Gaussian :91-114, lift_gaussian :66-88, diag) fused with
-// MipNerfEmbedder.forward (embedders/mipnerf_embedder.py:43-99): one thread per output element of embedded[N*S, 6*n_deg + C_dir].
-// The Gaussians (means/covs) are recomputed per element in registers and optionally also written out (API parity: data['samples']).
+// cast_rays (networks/utils/mip.py:117-129): the conical frustum -> Gaussian (:91-114), lift_gaussian (:66-88), diagonal covariance
 __device__ __forceinline__ void frustum_gaussian(float t0, float t1, float radius, const float d[3], const float o[3], float dmag_sq, float mean[3], float cov[3]) {
     float mu = (t0 + t1) / 2.f, hw = (t1 - t0) / 2.f;
     float mu2 = mu * mu, hw2 = hw * hw, hw4 = hw2 * hw2, den = 3.f * mu2 + hw2;
@@ -205,6 +221,35 @@ __device__ __forceinline__ void frustum_gaussian(float t0, float t1, float radiu
         cov[c] = t_var * dd + r_var * (1.f - dd / dmag_sq);
     }
 }
+// the Gaussian of sample k (interval z[k], z[k+1]) of ray `ray`
+__device__ __forceinline__ void sample_gaussian(const float *z_vals, const float *rays_o, const float *rays_d, const float *radii, int S, int64_t ray, int k, float mean[3],
+                                                float cov[3]) {
+    const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
+    const float o[3] = {rays_o[3 * ray], rays_o[3 * ray + 1], rays_o[3 * ray + 2]};
+    const float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    frustum_gaussian(z_vals[ray * (S + 1) + k], z_vals[ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
+}
+// GetPts (create.py:588-597): o + d * z as a rounded product then a rounded sum (torch), never an FMA — the 2^9-scaled sin arguments amplify the difference
+__device__ __forceinline__ void get_pts(const float *rays_o, const float *rays_d, int64_t ray, float z, float p[3]) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(rays_o[3 * ray + a], __fmul_rn(rays_d[3 * ray + a], z));
+}
+
+// BaseEmbedder.forward (embedders/base.py:57-74): one thread per output element (coalesced row writes)
+__global__ void __launch_bounds__(256) posenc_kernel(int64_t n_pts, int samples_per_ray, int multires, int multires_dirs, const float *__restrict__ pts,
+                                                     const float *__restrict__ viewdirs, float *__restrict__ out) {
+    const int c_pts = 3 + 6 * multires, c_dir = 3 + 6 * multires_dirs, C = c_pts + c_dir;
+    const int64_t total = n_pts * C;
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        int64_t i = idx / C; int c = (int)(idx - i * C);
+        const float *src; int cc;
+        if (c < c_pts) { src = pts + 3 * i; cc = c; } else { src = viewdirs + 3 * (i / samples_per_ray); cc = c - c_pts; }
+        out[idx] = posenc_col(src, cc);
+    }
+}
+
+// Mip-NeRF: cast_rays fused with MipNerfEmbedder.forward (embedders/mipnerf_embedder.py:43-99): one thread per output element of
+// embedded[N*S, 6*n_deg + C_dir]. The Gaussians (means/covs) are recomputed per element in registers and optionally also written out (API parity: data['samples']).
 __global__ void __launch_bounds__(256) mip_embed_kernel(int n_rays, int S, int min_deg, int max_deg, int min_deg_view, int max_deg_view, const float *__restrict__ z_vals,
                                                         const float *__restrict__ rays_o, const float *__restrict__ rays_d, const float *__restrict__ radii,
                                                         const float *__restrict__ viewdirs, float *__restrict__ embedded, float *__restrict__ means_out, float *__restrict__ covs_out) {
@@ -216,99 +261,82 @@ __global__ void __launch_bounds__(256) mip_embed_kernel(int n_rays, int S, int m
         int ray = (int)(row / S), k = (int)(row - (int64_t)ray * S);
         float v;
         if (c < c_ipe) {
-            const float d[3] = {rays_d[3 * (size_t)ray], rays_d[3 * (size_t)ray + 1], rays_d[3 * (size_t)ray + 2]};
-            const float o[3] = {rays_o[3 * (size_t)ray], rays_o[3 * (size_t)ray + 1], rays_o[3 * (size_t)ray + 2]};
-            float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
             float mean[3], cov[3];
-            frustum_gaussian(z_vals[(size_t)ray * (S + 1) + k], z_vals[(size_t)ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
-            int q = c < c_ipe / 2 ? c : c - c_ipe / 2;   // [y | y + pi/2]
-            int deg = q / 3 + min_deg, ax = q % 3;
-            float sc = exp2f((float)deg);
-            float y = mean[ax] * sc, yv = cov[ax] * sc * sc;
-            if (c >= c_ipe / 2) y += 1.5707963267948966f;
-            v = expf(-0.5f * yv) * sinf(y);
-            if (means_out && c < 3) { means_out[row * 3 + c] = mean[c]; covs_out[row * 3 + c] = cov[c]; }
-        } else {
-            int cc = c - c_ipe;
-            const float *vd = viewdirs + 3 * (size_t)ray;
-            if (cc < 3) v = vd[cc];
-            else { int q = cc - 3; int halfn = 3 * n_deg_v; int qq = q < halfn ? q : q - halfn; float x = vd[qq % 3] * exp2f((float)(qq / 3 + min_deg_view)); if (q >= halfn) x += 1.5707963267948966f; v = sinf(x); }
-        }
+            sample_gaussian(z_vals, rays_o, rays_d, radii, S, ray, k, mean, cov);
+            v = ipe_col(mean, cov, c, c_ipe, min_deg);
+            if (means_out && c < 3) { means_out[row * 3 + c] = sel3(mean, c); covs_out[row * 3 + c] = sel3(cov, c); }
+        } else v = mip_dir_col(viewdirs + 3 * (size_t)ray, c - c_ipe, n_deg_v, min_deg_view);
         embedded[idx] = v;
     }
 }
 
-// The same cast_rays + IPE + view-direction encoding written straight into the fp16 tile images (wgmma operand layout) the NerfMLP kernel TMA-loads
-// (csrc/nerf_mlp_tc.cu: per 128-row tile, point blocks [128 x 64] x 2 (96 -> 128 columns, zero padded), then the direction block; K-major,
-// 128-byte swizzle): no fp32 `embedded` [N*S,123] round trip (63 GB per 800x800 image in the reference). One thread per (row, 16-byte chunk);
-// the frustum Gaussian is formed once per thread in registers. Values are the fp16 roundings of exactly what mip_embed_kernel produces.
-__device__ __forceinline__ uint32_t ipe_sw128(uint32_t row, uint32_t chunk16) { return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk16 ^ (row & 7u)) << 4); }
-__device__ __forceinline__ uint32_t ipe_pack_h2(float a, float b) { __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<uint32_t *>(&h); }
-__global__ void __launch_bounds__(256) mip_ipe_tiles_kernel(int64_t n_rays, int S, int min_deg, int max_deg, int min_deg_view, int max_deg_view, const float *__restrict__ z_vals,
-                                                            const float *__restrict__ rays_o, const float *__restrict__ rays_d, const float *__restrict__ radii,
-                                                            const float *__restrict__ viewdirs, uint8_t *__restrict__ image) {
-    const int n_deg = max_deg - min_deg, n_deg_v = max_deg_view - min_deg_view;
-    const int c_ipe = 6 * n_deg, c_dir = 3 + 6 * n_deg_v, aux = (c_ipe + 63) / 64, chunks_per_row = (aux + 1) * 8;
-    const int64_t n_rows = n_rays * S, n_tiles = (n_rows + 127) / 128, total = n_tiles * 128 * chunks_per_row;
+// ---- generic tile-image encoders: one thread per (row, 16-byte chunk) of every tile, fully coalesced 16-byte stores. Blocks 0..n_blk-2 hold the
+// c_pts point columns, block n_blk-1 the c_dir direction columns. For a row < n_rows and a chunk holding n > 0 of its section's columns,
+// enc(row, is_dir, k0, n, v) sets v[q] = column k0 + q of the section for q < n; every other value is zero.
+template <class Enc>
+__device__ __forceinline__ void write_tiles(int64_t n_rows, int n_blk, int c_pts, int c_dir, uint8_t *image, Enc enc) {
+    const int chunks_per_row = n_blk * 8;
+    const int64_t total = (n_rows + 127) / 128 * 128 * chunks_per_row;
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
         const int64_t row = idx / chunks_per_row; const int cc = (int)(idx - row * chunks_per_row);
         const int blk = cc >> 3, ch = cc & 7;
-        const bool is_dir = blk == aux, live = row < n_rows;
-        const int width = is_dir ? c_dir : c_ipe, k0 = (is_dir ? 0 : blk * 64) + ch * 8;
+        const bool is_dir = blk == n_blk - 1;
+        const int k0 = (is_dir ? 0 : blk * 64) + ch * 8, n = (is_dir ? c_dir : c_pts) - k0;
         float v[8];
 #pragma unroll
         for (int q = 0; q < 8; ++q) v[q] = 0.f;
-        if (live && k0 < width) {
-            const int64_t ray = row / S; const int k = (int)(row - ray * S);
-            if (!is_dir) {
-                const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
-                const float o[3] = {rays_o[3 * ray], rays_o[3 * ray + 1], rays_o[3 * ray + 2]};
-                const float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-                float mean[3], cov[3];
-                frustum_gaussian(z_vals[ray * (S + 1) + k], z_vals[ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const int c = k0 + q;
-                    if (c < c_ipe) {
-                        const int qq = c < c_ipe / 2 ? c : c - c_ipe / 2;
-                        const int deg = qq / 3 + min_deg, ax = qq % 3;
-                        const float sc = exp2f((float)deg);
-                        float y = (ax == 0 ? mean[0] : ax == 1 ? mean[1] : mean[2]) * sc;
-                        const float yv = (ax == 0 ? cov[0] : ax == 1 ? cov[1] : cov[2]) * sc * sc;
-                        if (c >= c_ipe / 2) y += 1.5707963267948966f;
-                        v[q] = expf(-0.5f * yv) * sinf(y);
-                    }
-                }
-            } else {
-                const float vd[3] = {viewdirs[3 * ray], viewdirs[3 * ray + 1], viewdirs[3 * ray + 2]};
-                const int halfn = 3 * n_deg_v;
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const int c = k0 + q;
-                    if (c < 3) v[q] = c == 0 ? vd[0] : c == 1 ? vd[1] : vd[2];
-                    else if (c < c_dir) {
-                        const int qd = c - 3, qq = qd < halfn ? qd : qd - halfn, ax = qq % 3;
-                        float x = (ax == 0 ? vd[0] : ax == 1 ? vd[1] : vd[2]) * exp2f((float)(qq / 3 + min_deg_view));
-                        if (qd >= halfn) x += 1.5707963267948966f;
-                        v[q] = sinf(x);
-                    }
-                }
-            }
-        }
-        const int64_t tile = row >> 7; const uint32_t r = (uint32_t)(row & 127);
-        *reinterpret_cast<uint4 *>(image + ((size_t)tile * (aux + 1) + blk) * 16384 + ipe_sw128(r, ch)) =
-            make_uint4(ipe_pack_h2(v[0], v[1]), ipe_pack_h2(v[2], v[3]), ipe_pack_h2(v[4], v[5]), ipe_pack_h2(v[6], v[7]));
+        if (row < n_rows && n > 0) enc(row, is_dir, k0, n, v);
+        st_chunk(tile_block(image, row >> 7, n_blk, blk) + sw128_offset((uint32_t)(row & 127), ch), pack_h8(v));
     }
+}
+// an fp32 embedded[n_rows, ic + icd] (any encoder's output) -> tile image
+__global__ void __launch_bounds__(256) pack_embedded_tiles_kernel(const float *__restrict__ embedded, int64_t n_rows, int ic, int icd, int aux, uint8_t *__restrict__ image) {
+    write_tiles(n_rows, aux + 1, ic, icd, image, [&](int64_t row, bool is_dir, int k0, int n, float *v) {
+        const float *src = embedded + (size_t)row * (ic + icd) + (is_dir ? ic : 0) + k0;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) if (q < n) v[q] = __ldg(src + q);
+    });
+}
+// BaseEmbedder: pts f32[n,3], viewdirs f32[n/S,3]. Ray mode (rays_o != NULL): `pts` is z_vals f32[n_rays, S] and the sample position o + d*z is formed
+// in registers (never materialised: 491 MB per 800x800 image in the reference)
+__global__ void __launch_bounds__(256) posenc_tiles_kernel(const float *__restrict__ pts, const float *__restrict__ viewdirs, int64_t n_rows, int samples_per_ray, int multires,
+                                                           int multires_dirs, uint8_t *__restrict__ image, const float *__restrict__ rays_o, const float *__restrict__ rays_d) {
+    const int ic = 3 + 6 * multires;
+    write_tiles(n_rows, (ic + 63) / 64 + 1, ic, 3 + 6 * multires_dirs, image, [&](int64_t row, bool is_dir, int k0, int n, float *v) {
+        const int64_t ray = row / samples_per_ray;
+        float p[3];
+        const float *x = pts + 3 * row;
+        if (is_dir) x = viewdirs + 3 * ray;
+        else if (rays_o) { get_pts(rays_o, rays_d, ray, pts[row], p); x = p; }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) if (q < n) v[q] = posenc_col(x, k0 + q);
+    });
+}
+// Mip-NeRF cast_rays + IPE + view-direction encoding: no fp32 `embedded` [N*S,123] round trip (63 GB per 800x800 image in the reference); the frustum
+// Gaussian is formed once per thread in registers
+__global__ void __launch_bounds__(256) mip_ipe_tiles_kernel(int64_t n_rays, int S, int min_deg, int max_deg, int min_deg_view, int max_deg_view, const float *__restrict__ z_vals,
+                                                            const float *__restrict__ rays_o, const float *__restrict__ rays_d, const float *__restrict__ radii,
+                                                            const float *__restrict__ viewdirs, uint8_t *__restrict__ image) {
+    const int n_deg = max_deg - min_deg, n_deg_v = max_deg_view - min_deg_view, c_ipe = 6 * n_deg;
+    write_tiles(n_rays * S, (c_ipe + 63) / 64 + 1, c_ipe, 3 + 6 * n_deg_v, image, [&](int64_t row, bool is_dir, int k0, int n, float *v) {
+        const int64_t ray = row / S; const int k = (int)(row - ray * S);
+        if (is_dir) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) if (q < n) v[q] = mip_dir_col(viewdirs + 3 * ray, k0 + q, n_deg_v, min_deg_view);
+        } else {
+            float mean[3], cov[3];
+            sample_gaussian(z_vals, rays_o, rays_d, radii, S, ray, k, mean, cov);
+#pragma unroll
+            for (int q = 0; q < 8; ++q) if (q < n) v[q] = ipe_col(mean, cov, k0 + q, c_ipe, min_deg);
+        }
+    });
 }
 
 // ---- fast tile-image encoders for the reference configurations (thread == (tile, encoding block, row): a warp works on 32 rows of ONE block
 // kind, so there is no intra-warp divergence; every trig evaluation is shared by the columns that use it and all column indices are compile-time).
-// The generic kernels above / in nerf_mlp_tc.cu stay as the fallback for other degrees. Launch list before this change (gpurun_out, 32768 rays):
+// The generic kernels above serve every other degree. Before these kernels existed (32768 rays on an H100):
 // mip_ipe_tiles_kernel 4.29 ms per 4.2 M rows and posenc_tiles_kernel 1.92 ms per 6.3 M rows next to 8.46 ms of MLP.
 __device__ __forceinline__ float pow2i(int e) { return __int_as_float((127 + e) << 23); }   // 2^e, exact, -126 <= e <= 127
-__device__ __forceinline__ void store_chunk(uint8_t *blk_row, uint32_t chunk, uint32_t r7, const float *v) {
-    *reinterpret_cast<uint4 *>(blk_row + ((chunk ^ r7) << 4)) = make_uint4(ipe_pack_h2(v[0], v[1]), ipe_pack_h2(v[2], v[3]), ipe_pack_h2(v[4], v[5]), ipe_pack_h2(v[6], v[7]));
-}
 // Mip-NeRF, 6*NDEG <= 128 point columns (two blocks) + direction block. item 0 = both point blocks of the row, item 1 = direction block.
 // IPE column q (< 3*NDEG): exp(-0.5 * cov_ax * 4^deg) * sin(mean_ax * 2^deg), column 3*NDEG + q: the same with sin(y + pi/2) — the reference's
 // expression, NOT cos(y): fl(y + pi/2) differs from y + pi/2 by up to ulp(y)/2 and the reference's value includes that (mipnerf_embedder.py:35-41,:55-60).
@@ -324,16 +352,11 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_fast_kernel(int64_t n_rays,
         const int64_t row = tile * 128 + r;
         const bool live = row < n_rows;
         const uint32_t r7 = r & 7u;
-        uint8_t *trow = image + (size_t)tile * 3 * 16384 + (r >> 3) * 1024u + r7 * 128u;     // my row inside block 0 of the tile
+        uint8_t *trow = sw128_row_ptr(tile_block(image, tile, 3, 0), r);   // my row inside block 0 of the tile
         const int64_t ray = live ? row / S : 0; const int k = (int)(row - ray * S);
         if (item == 0) {
             float mean[3] = {0.f, 0.f, 0.f}, cov[3] = {0.f, 0.f, 0.f};
-            if (live) {
-                const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
-                const float o[3] = {rays_o[3 * ray], rays_o[3 * ray + 1], rays_o[3 * ray + 2]};
-                const float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-                frustum_gaussian(z_vals[ray * (S + 1) + k], z_vals[ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
-            }
+            if (live) sample_gaussian(z_vals, rays_o, rays_d, radii, S, ray, k, mean, cov);
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
                 float sv[8], cv[8];
@@ -343,16 +366,16 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_fast_kernel(int64_t n_rays,
                     const float sc = pow2i(deg + min_deg);
                     const float y = mean[ax] * sc, hv = 0.5f * (cov[ax] * sc * sc);
                     float s = 0.f, c = 0.f;
-                    if (live && hv <= 20.f) { const float ex = expf(-hv); s = ex * sinf(y); c = ex * sinf(y + 1.5707963267948966f); }
+                    if (live && hv <= 20.f) { const float ex = expf(-hv); s = ex * sinf(y); c = ex * sinf(y + HALF_PI); }
                     sv[e] = s; cv[e] = c;
                 }
-                store_chunk(trow, j, r7, sv);                                                   // columns 8j .. 8j+7 of block 0
-                const int cc = HALF + 8 * j;                                                    // first "cos" column of this group
-                store_chunk(trow + (cc >> 6) * 16384, (uint32_t)(cc & 63) >> 3, r7, cv);
+                st_row_chunk(trow, r7, j, sv);                                          // columns 8j .. 8j+7 of block 0
+                const int cs = HALF + 8 * j;                                                                     // first "cos" column of this group
+                st_row_chunk(trow + (cs >> 6) * TILE_BLOCK_BYTES, r7, (uint32_t)(cs & 63) >> 3, cv);
             }
             const float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-            for (int ch = (6 * NDEG - 64) / 8; ch < 8; ++ch) store_chunk(trow + 16384, ch, r7, z8);   // zero padding of block 1
+            for (int ch = (6 * NDEG - 64) / 8; ch < 8; ++ch) st_row_chunk(trow + TILE_BLOCK_BYTES, r7, ch, z8);   // zero padding of block 1
         } else {
             float v[64];
 #pragma unroll
@@ -364,11 +387,11 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_fast_kernel(int64_t n_rays,
 #pragma unroll
                 for (int q = 0; q < 3 * NDEGV; ++q) {
                     const float x = vd[q % 3] * pow2i(q / 3 + min_deg_view);
-                    v[3 + q] = sinf(x); v[3 + 3 * NDEGV + q] = sinf(x + 1.5707963267948966f);
+                    v[3 + q] = sinf(x); v[3 + 3 * NDEGV + q] = sinf(x + HALF_PI);
                 }
             }
 #pragma unroll
-            for (int ch = 0; ch < 8; ++ch) store_chunk(trow + 2 * 16384, ch, r7, v + 8 * ch);
+            for (int ch = 0; ch < 8; ++ch) st_row_chunk(trow + 2 * TILE_BLOCK_BYTES, r7, ch, v + 8 * ch);
         }
     }
 }
@@ -384,8 +407,7 @@ __global__ void __launch_bounds__(256) posenc_tiles_fast_kernel(const float *__r
         const uint32_t r = (uint32_t)(idx & 127); const int item = (int)((idx >> 7) & 1); const int64_t tile = idx >> 8;
         const int64_t row = tile * 128 + r;
         const bool live = row < n_rows;
-        const uint32_t r7 = r & 7u;
-        uint8_t *trow = image + ((size_t)tile * 2 + item) * 16384 + (r >> 3) * 1024u + r7 * 128u;
+        uint8_t *trow = tile_block(image, tile, 2, item) + sw128_row(r);
         float v[64];
 #pragma unroll
         for (int e = 0; e < 64; ++e) v[e] = 0.f;
@@ -393,11 +415,8 @@ __global__ void __launch_bounds__(256) posenc_tiles_fast_kernel(const float *__r
             float x[3];
             const int64_t ray = row / samples_per_ray;
             if (item == 1) { x[0] = viewdirs[3 * ray]; x[1] = viewdirs[3 * ray + 1]; x[2] = viewdirs[3 * ray + 2]; }
-            else if (rays_o) {
-                const float z = pts[row];
-                // GetPts (create.py:588-597): o + d * z as a rounded product then a rounded sum (torch), never an FMA — the 2^9-scaled sin arguments amplify the difference
-                x[0] = __fadd_rn(rays_o[3 * ray], __fmul_rn(rays_d[3 * ray], z)); x[1] = __fadd_rn(rays_o[3 * ray + 1], __fmul_rn(rays_d[3 * ray + 1], z)); x[2] = __fadd_rn(rays_o[3 * ray + 2], __fmul_rn(rays_d[3 * ray + 2], z));
-            } else { x[0] = pts[3 * row]; x[1] = pts[3 * row + 1]; x[2] = pts[3 * row + 2]; }
+            else if (rays_o) get_pts(rays_o, rays_d, ray, pts[row], x);
+            else { x[0] = pts[3 * row]; x[1] = pts[3 * row + 1]; x[2] = pts[3 * row + 2]; }
 #pragma unroll
             for (int a = 0; a < 3; ++a) v[a] = x[a];
             if (item == 0) {
@@ -413,7 +432,7 @@ __global__ void __launch_bounds__(256) posenc_tiles_fast_kernel(const float *__r
             }
         }
 #pragma unroll
-        for (int ch = 0; ch < 8; ++ch) store_chunk(trow, ch, r7, v + 8 * ch);
+        for (int ch = 0; ch < 8; ++ch) st_chunk(trow + sw128_chunk(r, ch), pack_h8(v + 8 * ch));
     }
 }
 
@@ -617,33 +636,63 @@ int xrb_mip_embed(const float *z_vals, const float *rays_o, const float *rays_d,
     return check_launch("mip_embed");
 }
 
+// grid of a tile-image encoder launch with `per_tile` threads per 128-row tile (generic kernels: 128 x 8 per block, fast kernels: 256)
+static int tile_grid(int64_t n_rows, int64_t per_tile) { return stride_grid(((n_rows + 127) / 128 * per_tile + 255) / 256, 16); }
+
 int xrb_mip_ipe_tiles_rays(const float *z_vals, const float *rays_o, const float *rays_d, const float *radii, const float *viewdirs, int64_t n_rays, int n_samples, int min_deg_point,
                            int max_deg_point, int min_deg_view, int max_deg_view, void *enc_image, void *stream) {
     XRB_REQUIRE(n_rays >= 0 && n_samples >= 1 && max_deg_point > min_deg_point && max_deg_view >= min_deg_view, "mip_ipe_tiles_rays: bad size");
     XRB_REQUIRE(6 * (max_deg_point - min_deg_point) <= 128 && 3 + 6 * (max_deg_view - min_deg_view) <= 64, "mip_ipe_tiles_rays: encoding wider than the tile image (128 + 64 columns)");
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(z_vals && rays_o && rays_d && radii && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "mip_ipe_tiles_rays: null/misaligned pointer");
-    const int aux = (6 * (max_deg_point - min_deg_point) + 63) / 64;
-    int64_t total = ((n_rays * n_samples + 127) / 128) * 128 * (aux + 1) * 8;
-    const int blocks = stride_grid((total + 255) / 256, 16);
-    if (max_deg_point - min_deg_point == 16 && max_deg_view - min_deg_view == 4 && min_deg_point >= -100 && max_deg_point <= 100 && min_deg_view >= -100 && max_deg_view <= 100) {
+    const int64_t n_rows = n_rays * n_samples;
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (max_deg_point - min_deg_point == 16 && max_deg_view - min_deg_view == 4 && min_deg_point >= -100 && max_deg_point <= 100 && min_deg_view >= -100 && max_deg_view <= 100)
         // the reference configuration (configs/mipnerf/*.py): specialised kernel
-        int64_t items = ((n_rays * n_samples + 127) / 128) * 256;
-        const int fb = stride_grid((items + 255) / 256, 16);
-        mip_ipe_tiles_fast_kernel<16, 4><<<fb, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, min_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
-        return check_launch("mip_ipe_tiles_rays");
-    }
-    mip_ipe_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view, max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs,
-                                                                       (uint8_t *)enc_image);
+        mip_ipe_tiles_fast_kernel<16, 4><<<tile_grid(n_rows, 256), 256, 0, s>>>(n_rays, n_samples, min_deg_point, min_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
+    else
+        mip_ipe_tiles_kernel<<<tile_grid(n_rows, 128 * 8 * ((6 * (max_deg_point - min_deg_point) + 63) / 64 + 1)), 256, 0, s>>>(n_rays, n_samples, min_deg_point, max_deg_point, min_deg_view,
+                                                                                                                          max_deg_view, z_vals, rays_o, rays_d, radii, viewdirs, (uint8_t *)enc_image);
     return check_launch("mip_ipe_tiles_rays");
 }
 
-// called by xrb_nerf_posenc_tiles / xrb_nerf_posenc_tiles_rays (nerf_mlp_tc.cu) for the reference configuration multires=10, multires_dirs=4
-int xrb_internal_posenc_tiles_fast(const float *pts, const float *viewdirs, int64_t n_rows, int samples_per_ray, void *enc_image, const float *rays_o, const float *rays_d, void *stream) {
-    int64_t items = ((n_rows + 127) / 128) * 256;
-    const int fb = stride_grid((items + 255) / 256, 16);
-    posenc_tiles_fast_kernel<10, 4><<<fb, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_rows, samples_per_ray, (uint8_t *)enc_image, rays_o, rays_d);
-    return check_launch("posenc_tiles");
+size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch) { return tile_image_bytes(n_rows, (input_ch + 63) / 64 + 1); }
+
+int xrb_nerf_pack_embedded(const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, void *enc_image, void *stream) {
+    XRB_REQUIRE(n_rows >= 0 && input_ch >= 1 && input_ch <= 128 && input_ch_dirs >= 0 && input_ch_dirs <= 64, "nerf_pack_embedded: bad size");
+    if (n_rows == 0) return XRB_OK;
+    XRB_REQUIRE(embedded && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_pack_embedded: null/misaligned pointer");
+    const int aux = (input_ch + 63) / 64;
+    pack_embedded_tiles_kernel<<<tile_grid(n_rows, 128 * 8 * (aux + 1)), 256, 0, (cudaStream_t)stream>>>(embedded, n_rows, input_ch, input_ch_dirs, aux, (uint8_t *)enc_image);
+    return check_launch("nerf_pack_embedded");
+}
+
+// positional encoding into a tile image; ray mode when rays_o != NULL (`pts` is then z_vals). The reference configuration multires = 10,
+// multires_dirs = 4 takes the specialised kernel.
+static int posenc_tiles(const float *pts, const float *viewdirs, int64_t n_rows, int samples_per_ray, int multires, int multires_dirs, void *enc_image, const float *rays_o,
+                        const float *rays_d, void *stream, const char *what) {
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (multires == 10 && multires_dirs == 4)
+        posenc_tiles_fast_kernel<10, 4><<<tile_grid(n_rows, 256), 256, 0, s>>>(pts, viewdirs, n_rows, samples_per_ray, (uint8_t *)enc_image, rays_o, rays_d);
+    else
+        posenc_tiles_kernel<<<tile_grid(n_rows, 128 * 8 * ((3 + 6 * multires + 63) / 64 + 1)), 256, 0, s>>>(pts, viewdirs, n_rows, samples_per_ray, multires, multires_dirs,
+                                                                                                          (uint8_t *)enc_image, rays_o, rays_d);
+    return check_launch(what);
+}
+
+int xrb_nerf_posenc_tiles(const float *pts, const float *viewdirs, int64_t n_pts, int samples_per_ray, int multires, int multires_dirs, void *enc_image, void *stream) {
+    XRB_REQUIRE(n_pts >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles: bad size");
+    if (n_pts == 0) return XRB_OK;
+    XRB_REQUIRE(pts && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles: null/misaligned pointer");
+    return posenc_tiles(pts, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, enc_image, nullptr, nullptr, stream, "nerf_posenc_tiles");
+}
+
+int xrb_nerf_posenc_tiles_rays(const float *rays_o, const float *rays_d, const float *z_vals, const float *viewdirs, int64_t n_rays, int samples_per_ray, int multires, int multires_dirs,
+                               void *enc_image, void *stream) {
+    XRB_REQUIRE(n_rays >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles_rays: bad size");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(rays_o && rays_d && z_vals && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles_rays: null/misaligned pointer");
+    return posenc_tiles(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, multires, multires_dirs, enc_image, rays_o, rays_d, stream, "nerf_posenc_tiles_rays");
 }
 
 int xrb_mip_resample(const float *z_vals, const float *weights, const float *u, int n_rays, int n_samples, float resample_padding, float *z_out, void *stream) {

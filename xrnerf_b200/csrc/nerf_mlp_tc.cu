@@ -12,7 +12,7 @@
 //              the tile's fp16 encoding blocks, re-armed once both warpgroups are past their last reader (views_linears.0).
 // A operand: [128 x 64]-blocks, K-major, 128-byte swizzle: blocks 0-3 hidden state h (256 wide), 4..4+AUX-1 the point encoding
 // (63 -> 64 for NeRF, 96 -> 128 for Mip-NeRF), last block the view-direction encoding (27 -> 64). The encoding blocks come from the fp16
-// encoding tile image (xrb_nerf_pack_embedded / posenc / IPE kernels).
+// encoding tile image (tc.cuh layout), written by the encoders in nerf.cu (xrb_nerf_pack_embedded / posenc / IPE).
 // Weights (packed by xrnerf_b200/nerf_mlp.py pack_nerf_mlp): [256 x 32] K-half slabs (64-byte swizzle) for the 256-wide layers, [N x 64] slabs
 // (128-byte swizzle) otherwise.
 // Numeric contract: fp16 operands (weights and activations), fp32 accumulate; each layer's accumulator is rounded to fp16, then the bias is added in
@@ -20,17 +20,12 @@
 // Parity tolerance vs the fp32 reference in tests/test_gpu_nerf_mlp.py.
 #include "tc.cuh"
 #include "common.cuh"
-#include <cuda_fp16.h>
 
 namespace xrb {
 
 constexpr int NM_THREADS = 384;
 constexpr int NM_LAYERS = 11;
 constexpr int NM_MAX_SLABS = 12;
-constexpr uint32_t NM_BLOCK = 16384;
-
-__device__ __forceinline__ uint32_t nm_pack_h2(float a, float b) { __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<uint32_t *>(&h); }
-__device__ __forceinline__ uint32_t nm_sw128(uint32_t row, uint32_t chunk16) { return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk16 ^ (row & 7u)) << 4); }
 
 // ---- compile-time layer schedule (the consumer's loops over layers and slabs are fully unrolled: accumulator offsets must be constants)
 struct NmSlab {
@@ -91,7 +86,7 @@ __device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc) {
         constexpr NmSlab sl = Ly.s[S];
         const uint32_t slot = x.it % x.n_slots, ph = (x.it / x.n_slots) & 1u;
         tc::mbar_wait(x.full + slot, ph);
-        const uint32_t a0 = tc::smem_u32(x.A + (size_t)sl.a_blk * NM_BLOCK) + x.wg * 8192u + (sl.kh > 0 ? 64u : 0u);
+        const uint32_t a0 = tc::smem_u32(x.A + (size_t)sl.a_blk * TILE_BLOCK_BYTES) + x.wg * 8192u + (sl.kh > 0 ? 64u : 0u);
         const uint32_t b0 = tc::smem_u32(x.ring + (size_t)slot * x.slot_bytes);
         tc::wg_fence();
 #pragma unroll
@@ -137,14 +132,14 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
 #pragma unroll
             for (int j = 0; j < Ly.N / 8; ++j) {
                 const uint32_t col = tc::frag_col(x.t, j);
-                uint8_t *blk = x.A + (size_t)(col >> 6) * NM_BLOCK;
+                uint8_t *blk = x.A + (size_t)(col >> 6) * TILE_BLOCK_BYTES;
                 const float b0 = __ldg(b + col), b1 = __ldg(b + col + 1);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     __half2 h = __hadd2(__floats2half2_rn(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), __floats2half2_rn(b0, b1));
                     if (Ly.relu) h = __hmax2(h, __float2half2_rn(0.f));
                     if (Ly.alpha_dot) { const float2 f = __half22float2(h); adot[e] = fmaf(f.x, __ldg(wa + col), adot[e]); adot[e] = fmaf(f.y, __ldg(wa + col + 1), adot[e]); }
-                    *reinterpret_cast<__half2 *>(blk + nm_sw128(x.r0 + 8u * (uint32_t)e, (col & 63u) >> 3) + (col & 7u) * 2u) = h;
+                    *reinterpret_cast<__half2 *>(sw128_elem(blk, x.r0 + 8u * (uint32_t)e, col & 63u)) = h;
                 }
             }
             if constexpr (Ly.alpha_dot) {   // the four lanes of a quad hold all 256 columns of its two rows
@@ -165,7 +160,7 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     extern __shared__ uint8_t dyn_smem[];
     constexpr int AUX = MIP ? 2 : 1;
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *A = base, *ring = A + (size_t)(5 + AUX) * NM_BLOCK;
+    uint8_t *A = base, *ring = A + (size_t)(5 + AUX) * TILE_BLOCK_BYTES;
     uint64_t *bars = (uint64_t *)(ring + (size_t)P.n_slots * P.slot_bytes);
     uint64_t *full = bars, *empty = bars + P.n_slots, *enc_full = bars + 2 * P.n_slots, *enc_free = enc_full + 1;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -176,7 +171,7 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     }
     __syncthreads();
     const int64_t n_tiles = (P.n_rows + 127) / 128;
-    const uint32_t enc_bytes = (uint32_t)(AUX + 1) * NM_BLOCK;
+    const uint32_t enc_bytes = (uint32_t)(AUX + 1) * TILE_BLOCK_BYTES;
 
     if (warp >= 8) {
         // ===================================================== TMA producer (one lane)
@@ -187,7 +182,7 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
                 // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block)
                 if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
                 tc::mbar_expect_tx(enc_full, enc_bytes);
-                tc::tma_bulk_g2s(A + 4 * NM_BLOCK, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
+                tc::tma_bulk_g2s(A + 4 * TILE_BLOCK_BYTES, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
                 size_t off = 0;
                 for (int l = 0; l < NM_LAYERS; ++l)
                     for (uint32_t s = 0; s < P.n_slabs[l]; ++s, ++it) {
@@ -217,7 +212,7 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     }
 }
 
-static int nm_launch(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
+static void nm_launch(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
     NmParams P{};
     P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.enc_image = (const uint8_t *)enc_image;
     P.n_rows = n_rows; P.input_ch = input_ch; P.input_ch_dirs = input_ch_dirs; P.raw = raw;
@@ -230,74 +225,16 @@ static int nm_launch(const void *weight_image, const float *bias, const void *en
     }
     P.slot_bytes = (max_bytes + 1023) & ~1023u;
     P.n_slots = 4;
-    const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * NM_BLOCK + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
+    const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * TILE_BLOCK_BYTES + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
     const int grid = persistent_grid(1, (n_rows + 127) / 128);
     auto k = mip ? nerf_mlp_wg_kernel<true> : nerf_mlp_wg_kernel<false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);
-    return XRB_OK;
-}
-
-// ---- encoding tile images: per 128-row tile, (aux+1) blocks of [128 x 64] fp16 in the wgmma layout (K-major, 128-byte swizzle),
-// point-encoding block(s) first, direction block last, zero padded; written by fully coalesced 16-byte stores.
-__global__ void __launch_bounds__(256) pack_embedded_tiles_kernel(const float *__restrict__ embedded, int64_t n_rows, int ic, int icd, int aux, uint8_t *__restrict__ image) {
-    const int chunks_per_row = (aux + 1) * 8;
-    const int64_t n_tiles = (n_rows + 127) / 128, total = n_tiles * 128 * chunks_per_row;
-    const int C = ic + icd;
-    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row = idx / chunks_per_row; const int cc = (int)(idx - row * chunks_per_row);
-        const int blk = cc >> 3, ch = cc & 7;
-        const bool is_dir = blk == aux;
-        const int width = is_dir ? icd : ic, c0 = is_dir ? ic : 0, k0 = (is_dir ? 0 : blk * 64) + ch * 8;
-        float v[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) v[q] = (row < n_rows && k0 + q < width) ? __ldg(embedded + (size_t)row * C + c0 + k0 + q) : 0.f;
-        const int64_t tile = row >> 7; const uint32_t r = (uint32_t)(row & 127);
-        *reinterpret_cast<uint4 *>(image + ((size_t)tile * (aux + 1) + blk) * 16384 + nm_sw128(r, ch)) =
-            make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
-    }
-}
-// BaseEmbedder positional encoding (embedders/base.py:26-52) computed straight into the tile image: pts f32[n,3], viewdirs f32[n/S,3]
-// ray mode (rays_o != NULL): `pts` is z_vals f32[n_rays, S] and the sample position o + d*z is formed in registers (GetPts, create.py:588-597,
-// never materialised: 491 MB per 800x800 image in the reference)
-__global__ void __launch_bounds__(256) posenc_tiles_kernel(const float *__restrict__ pts, const float *__restrict__ viewdirs, int64_t n_rows, int samples_per_ray, int multires,
-                                                           int multires_dirs, uint8_t *__restrict__ image, const float *__restrict__ rays_o, const float *__restrict__ rays_d) {
-    const int ic = 3 + 6 * multires, icd = 3 + 6 * multires_dirs, aux = (ic + 63) / 64, chunks_per_row = (aux + 1) * 8;
-    const int64_t n_tiles = (n_rows + 127) / 128, total = n_tiles * 128 * chunks_per_row;
-    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row = idx / chunks_per_row; const int cc = (int)(idx - row * chunks_per_row);
-        const int blk = cc >> 3, ch = cc & 7;
-        const bool is_dir = blk == aux;
-        const int width = is_dir ? icd : ic, k0 = (is_dir ? 0 : blk * 64) + ch * 8;
-        float v[8];
-        const float *src = row < n_rows ? (is_dir ? viewdirs + 3 * (row / samples_per_ray) : pts + 3 * row) : nullptr;
-        float p3[3];
-        if (src && !is_dir && rays_o) {
-            const int64_t ray = row / samples_per_ray; const float z = pts[row];
-            p3[0] = __fadd_rn(rays_o[3 * ray], __fmul_rn(rays_d[3 * ray], z)); p3[1] = __fadd_rn(rays_o[3 * ray + 1], __fmul_rn(rays_d[3 * ray + 1], z)); p3[2] = __fadd_rn(rays_o[3 * ray + 2], __fmul_rn(rays_d[3 * ray + 2], z));   // torch: mul then add, no FMA
-            src = p3;
-        }
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-            const int k = k0 + q;
-            float out = 0.f;
-            if (src && k < width) {
-                if (k < 3) out = src[k];
-                else { int qq = k - 3, band = qq / 6, r6 = qq % 6; float x = src[r6 % 3] * exp2f((float)band); out = r6 < 3 ? sinf(x) : cosf(x); }
-            }
-            v[q] = out;
-        }
-        const int64_t tile = row >> 7; const uint32_t r = (uint32_t)(row & 127);
-        *reinterpret_cast<uint4 *>(image + ((size_t)tile * (aux + 1) + blk) * 16384 + nm_sw128(r, ch)) =
-            make_uint4(nm_pack_h2(v[0], v[1]), nm_pack_h2(v[2], v[3]), nm_pack_h2(v[4], v[5]), nm_pack_h2(v[6], v[7]));
-    }
 }
 
 }  // namespace xrb
 
 using namespace xrb;
-
-extern "C" int xrb_internal_posenc_tiles_fast(const float *pts, const float *viewdirs, int64_t n_rows, int samples_per_ray, void *enc_image, const float *rays_o, const float *rays_d, void *stream);   // nerf.cu
 
 extern "C" {
 
@@ -312,46 +249,8 @@ int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const void
     XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward: null pointer");
     XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0 && ((uintptr_t)bias & 15) == 0,
                 "nerf_mlp_forward: images / bias / raw must be 16-byte aligned");
-    return nm_launch(weight_image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream) ? -100 : check_launch("nerf_mlp_forward");
-}
-
-size_t xrb_nerf_enc_image_bytes(int64_t n_rows, int input_ch) { return (size_t)((n_rows + 127) / 128) * ((input_ch + 63) / 64 + 1) * 16384; }
-
-int xrb_nerf_pack_embedded(const float *embedded, int64_t n_rows, int input_ch, int input_ch_dirs, void *enc_image, void *stream) {
-    XRB_REQUIRE(n_rows >= 0 && input_ch >= 1 && input_ch <= 128 && input_ch_dirs >= 0 && input_ch_dirs <= 64, "nerf_pack_embedded: bad size");
-    if (n_rows == 0) return XRB_OK;
-    XRB_REQUIRE(embedded && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_pack_embedded: null/misaligned pointer");
-    const int aux = (input_ch + 63) / 64;
-    int64_t total = ((n_rows + 127) / 128) * 128 * (aux + 1) * 8;
-    const int blocks = stride_grid((total + 255) / 256, 16);
-    pack_embedded_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(embedded, n_rows, input_ch, input_ch_dirs, aux, (uint8_t *)enc_image);
-    return check_launch("nerf_pack_embedded");
-}
-
-int xrb_nerf_posenc_tiles(const float *pts, const float *viewdirs, int64_t n_pts, int samples_per_ray, int multires, int multires_dirs, void *enc_image, void *stream) {
-    XRB_REQUIRE(n_pts >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles: bad size");
-    if (n_pts == 0) return XRB_OK;
-    XRB_REQUIRE(pts && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles: null/misaligned pointer");
-    if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(pts, viewdirs, n_pts, samples_per_ray, enc_image, nullptr, nullptr, stream);
-    const int aux = (3 + 6 * multires + 63) / 64;
-    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8;
-    const int blocks = stride_grid((total + 255) / 256, 16);
-    posenc_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, nullptr, nullptr);
-    return check_launch("nerf_posenc_tiles");
-}
-
-int xrb_nerf_posenc_tiles_rays(const float *rays_o, const float *rays_d, const float *z_vals, const float *viewdirs, int64_t n_rays, int samples_per_ray, int multires, int multires_dirs,
-                               void *enc_image, void *stream) {
-    XRB_REQUIRE(n_rays >= 0 && samples_per_ray >= 1 && multires >= 0 && multires <= 20 && multires_dirs >= 0 && multires_dirs <= 10, "nerf_posenc_tiles_rays: bad size");
-    if (n_rays == 0) return XRB_OK;
-    XRB_REQUIRE(rays_o && rays_d && z_vals && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles_rays: null/misaligned pointer");
-    if (multires == 10 && multires_dirs == 4) return xrb_internal_posenc_tiles_fast(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, enc_image, rays_o, rays_d, stream);
-    const int aux = (3 + 6 * multires + 63) / 64;
-    const int64_t n_pts = n_rays * samples_per_ray;
-    int64_t total = ((n_pts + 127) / 128) * 128 * (aux + 1) * 8;
-    const int blocks = stride_grid((total + 255) / 256, 16);
-    posenc_tiles_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z_vals, viewdirs, n_pts, samples_per_ray, multires, multires_dirs, (uint8_t *)enc_image, rays_o, rays_d);
-    return check_launch("nerf_posenc_tiles_rays");
+    nm_launch(weight_image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream);
+    return check_launch("nerf_mlp_forward");
 }
 
 }  // extern "C"

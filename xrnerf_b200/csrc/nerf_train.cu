@@ -18,13 +18,11 @@
 // dZ is staged in fp16 with a fixed scale (2^14, applied where dL/draw enters and removed at the dW flush): tcnn-style loss scaling for 1e-6-sized NeRF gradients.
 #include "tc.cuh"
 #include "common.cuh"
-#include "ngp_field.cuh"   // sw128_offset
 #include <cuda_fp16.h>
 #include <stdio.h>
 
 namespace xrb {
 
-constexpr uint32_t TG_BLOCK = 16384;
 constexpr int TG_MAX_A = 6, TG_MAX_SLABS = 10, TG_THREADS = 384, TG_DW_THREADS = 288;   // 6 A blocks: Mip-NeRF's skip layer reads 2 IPE blocks + 4 hidden blocks
 constexpr uint32_t TG_RING_SLOT = 32768;   // one [256 x 64] fp16 slab
 constexpr float TG_SCALE = 16384.f;
@@ -64,8 +62,8 @@ __device__ __forceinline__ void tg_mma(float *acc, int mma_n, int d_col, uint64_
 __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant__ TgP P) {
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *A = base, *RING = A + TG_MAX_A * TG_BLOCK, *Y = RING + 2 * TG_RING_SLOT;
-    uint64_t *bars = (uint64_t *)(Y + 4 * TG_BLOCK);
+    uint8_t *A = base, *RING = A + TG_MAX_A * TILE_BLOCK_BYTES, *Y = RING + 2 * TG_RING_SLOT;
+    uint64_t *bars = (uint64_t *)(Y + 4 * TILE_BLOCK_BYTES);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int k = 0; k < TB_N; ++k) tc::mbar_init(bars + k, 1);
@@ -86,11 +84,11 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
             uint32_t it = 0, g = 0;
             for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
                 if (it > 0) tc::mbar_wait(bars + TB_AEMPTY, (it - 1) & 1);
-                tc::mbar_expect_tx(bars + TB_AFULL, (uint32_t)n_ablk * TG_BLOCK);
+                tc::mbar_expect_tx(bars + TB_AFULL, (uint32_t)n_ablk * TILE_BLOCK_BYTES);
                 int ab = 0;
                 for (int s = 0; s < P.n_a; ++s)
                     for (int k = 0; k < P.a[s].n_blk; ++k, ++ab)
-                        tc::tma_bulk_g2s(A + (size_t)ab * TG_BLOCK, P.a[s].base + (size_t)tile * P.a[s].tile_stride + P.a[s].blk_off + (size_t)k * TG_BLOCK, TG_BLOCK, bars + TB_AFULL);
+                        tc::tma_bulk_g2s(A + (size_t)ab * TILE_BLOCK_BYTES, P.a[s].base + (size_t)tile * P.a[s].tile_stride + P.a[s].blk_off + (size_t)k * TILE_BLOCK_BYTES, TILE_BLOCK_BYTES, bars + TB_AFULL);
                 for (int s = 0; s < P.n_slabs; ++s, ++g) {
                     const uint32_t slot = g & 1u, round = g >> 1;
                     if (round > 0) tc::mbar_wait(bars + TB_SEMPTY + slot, (round - 1) & 1);
@@ -99,9 +97,9 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
                 }
                 if (n_xblk) {
                     if (it > 0) tc::mbar_wait(bars + TB_YEMPTY, (it - 1) & 1);     // the previous tile's output has left the Y region
-                    tc::mbar_expect_tx(bars + TB_XFULL, (uint32_t)n_xblk * TG_BLOCK);
+                    tc::mbar_expect_tx(bars + TB_XFULL, (uint32_t)n_xblk * TILE_BLOCK_BYTES);
                     for (int k = 0; k < n_xblk; ++k)
-                        tc::tma_bulk_g2s(Y + (size_t)k * TG_BLOCK, P.x.base + (size_t)tile * P.x.tile_stride + P.x.blk_off + (size_t)k * TG_BLOCK, TG_BLOCK, bars + TB_XFULL);
+                        tc::tma_bulk_g2s(Y + (size_t)k * TILE_BLOCK_BYTES, P.x.base + (size_t)tile * P.x.tile_stride + P.x.blk_off + (size_t)k * TILE_BLOCK_BYTES, TILE_BLOCK_BYTES, bars + TB_XFULL);
                 }
             }
         }
@@ -121,7 +119,7 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
                 const uint32_t b_base = tc::smem_u32(RING + (size_t)slot * TG_RING_SLOT);
                 tc::wg_fence();
                 for (int j = 0; j < S.n_sub; ++j) {
-                    const uint32_t a0 = tc::smem_u32(A + (size_t)(S.a_blk0 + j) * TG_BLOCK) + (uint32_t)wg * 8192u;
+                    const uint32_t a0 = tc::smem_u32(A + (size_t)(S.a_blk0 + j) * TILE_BLOCK_BYTES) + (uint32_t)wg * 8192u;
                     for (int k = 0; k < S.n_k; ++k) {
                         const uint64_t ad = tc::desc_k128(a0 + k * 32);
                         const uint32_t sc = (S.first && j == 0 && k == 0) ? 0u : 1u;
@@ -160,10 +158,10 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
                         v[0] += b0; v[1] += b1; v[2] += b0; v[3] += b1;
                         if (P.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); v[2] = fmaxf(v[2], 0.f); v[3] = fmaxf(v[3], 0.f); }
                     }
-                    uint8_t *yb = Y + (size_t)(col >> 6) * TG_BLOCK;
+                    uint8_t *yb = Y + (size_t)(col >> 6) * TILE_BLOCK_BYTES;
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        uint32_t *w = reinterpret_cast<uint32_t *>(yb + sw128_offset(r0 + 8u * (uint32_t)e, (col & 63u) >> 3) + (col & 7u) * 2u);
+                        uint32_t *w = reinterpret_cast<uint32_t *>(sw128_elem(yb, r0 + 8u * (uint32_t)e, col & 63u));
                         __half2 h = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
                         if (P.epi == 2) h = __hmul2(h, __hgt2(*reinterpret_cast<const __half2 *>(w), __float2half2_rn(0.f)));   // * [x > 0]
                         *w = *reinterpret_cast<uint32_t *>(&h);
@@ -175,7 +173,7 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tg_kernel(const __grid_constant
                 if (t == 0) {
                     const int n_out_blk = (P.out_cols + 63) / 64;
                     for (int k = 0; k < n_out_blk; ++k)
-                        tc::tma_bulk_s2g(P.y + (size_t)tile * P.y_tile_stride + P.y_blk_off + (size_t)k * TG_BLOCK + (size_t)wg * 8192, Y + (size_t)k * TG_BLOCK + (size_t)wg * 8192, 8192);
+                        tc::tma_bulk_s2g(P.y + (size_t)tile * P.y_tile_stride + P.y_blk_off + (size_t)k * TILE_BLOCK_BYTES + (size_t)wg * 8192, Y + (size_t)k * TILE_BLOCK_BYTES + (size_t)wg * 8192, 8192);
                     tc::tma_bulk_commit_wait_read();
                     if (P.epi == 2) tc::mbar_arrive(bars + TB_YEMPTY);
                 }
@@ -203,7 +201,7 @@ __global__ void __launch_bounds__(TG_DW_THREADS, 1) tg_dw_kernel(const __grid_co
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
     // two stages of (dZ chunk: 2 blocks | X: 4 blocks)
-    constexpr uint32_t STAGE = 6 * TG_BLOCK;
+    constexpr uint32_t STAGE = 6 * TILE_BLOCK_BYTES;
     uint64_t *bars = (uint64_t *)(base + 2 * STAGE);      // full[2], empty[2]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) { tc::mbar_init(bars, 1); tc::mbar_init(bars + 1, 1); tc::mbar_init(bars + 2, 8); tc::mbar_init(bars + 3, 8); tc::fence_mbar_init(); }
@@ -219,12 +217,12 @@ __global__ void __launch_bounds__(TG_DW_THREADS, 1) tg_dw_kernel(const __grid_co
                 const uint32_t st = it & 1u;
                 if (it >= 2) tc::mbar_wait(bars + 2 + st, ((it >> 1) - 1) & 1);
                 uint8_t *S = base + (size_t)st * STAGE;
-                tc::mbar_expect_tx(bars + st, (uint32_t)(z_blk + n_xblk) * TG_BLOCK);
+                tc::mbar_expect_tx(bars + st, (uint32_t)(z_blk + n_xblk) * TILE_BLOCK_BYTES);
                 const uint32_t z_first = P.transposed ? 0u : (uint32_t)chunk * 2u;
                 for (int k = 0; k < z_blk; ++k)
-                    tc::tma_bulk_g2s(S + (size_t)k * TG_BLOCK, P.z.base + (size_t)tile * P.z.tile_stride + P.z.blk_off + (size_t)(z_first + k) * TG_BLOCK, TG_BLOCK, bars + st);
+                    tc::tma_bulk_g2s(S + (size_t)k * TILE_BLOCK_BYTES, P.z.base + (size_t)tile * P.z.tile_stride + P.z.blk_off + (size_t)(z_first + k) * TILE_BLOCK_BYTES, TILE_BLOCK_BYTES, bars + st);
                 for (int k = 0; k < n_xblk; ++k)
-                    tc::tma_bulk_g2s(S + (size_t)(2 + k) * TG_BLOCK, P.x.base + (size_t)tile * P.x.tile_stride + P.x.blk_off + (size_t)k * TG_BLOCK, TG_BLOCK, bars + st);
+                    tc::tma_bulk_g2s(S + (size_t)(2 + k) * TILE_BLOCK_BYTES, P.x.base + (size_t)tile * P.x.tile_stride + P.x.blk_off + (size_t)k * TILE_BLOCK_BYTES, TILE_BLOCK_BYTES, bars + st);
             }
         }
         return;
@@ -247,19 +245,19 @@ __global__ void __launch_bounds__(TG_DW_THREADS, 1) tg_dw_kernel(const __grid_co
             const uint32_t sc = (it | (uint32_t)k) ? 1u : 0u;
             if (!P.transposed) {
                 // D[64 out (dZ block 2 chunk + h) x 64 in per X block] += dZ^T . X
-                const uint64_t ad = tc::desc_mn128(S + (uint32_t)wg * TG_BLOCK + k * 2048, 1024);
+                const uint64_t ad = tc::desc_mn128(S + (uint32_t)wg * TILE_BLOCK_BYTES + k * 2048, 1024);
 #pragma unroll
                 for (int xb = 0; xb < 4; ++xb)
-                    if (xb < n_xblk) tc::wgmma<64, 1, 1>(acc[xb], ad, tc::desc_mn128(S + (2 + xb) * TG_BLOCK + k * 2048, 1024), sc);
+                    if (xb < n_xblk) tc::wgmma<64, 1, 1>(acc[xb], ad, tc::desc_mn128(S + (2 + xb) * TILE_BLOCK_BYTES + k * 2048, 1024), sc);
             } else {
                 // D[64 in (X block 2 chunk + h) x 16 out] += X^T . dZ
-                tc::wgmma<16, 1, 1>(acc[0], tc::desc_mn128(S + (2 + 2 * chunk + wg) * TG_BLOCK + k * 2048, 1024), tc::desc_mn128(S + k * 2048, 1024), sc);
+                tc::wgmma<16, 1, 1>(acc[0], tc::desc_mn128(S + (2 + 2 * chunk + wg) * TILE_BLOCK_BYTES + k * 2048, 1024), tc::desc_mn128(S + k * 2048, 1024), sc);
             }
         }
         tc::wg_commit();
         if (bias_here) {
-            const uint8_t *zb = base + (size_t)st * STAGE + (P.transposed ? 0 : (size_t)wg * TG_BLOCK);
-            for (uint32_t r = b_row0; r < b_row0 + b_rows; ++r) bsum += __half2float(*reinterpret_cast<const __half *>(zb + sw128_offset(r, b_col >> 3) + (b_col & 7u) * 2u));
+            const uint8_t *zb = base + (size_t)st * STAGE + (P.transposed ? 0 : (size_t)wg * TILE_BLOCK_BYTES);
+            for (uint32_t r = b_row0; r < b_row0 + b_rows; ++r) bsum += __half2float(*reinterpret_cast<const __half *>(sw128_elem(zb, r, b_col)));
         }
         tc::wg_wait<0>();
         tc::acc_fence<32>(acc[0]); tc::acc_fence<32>(acc[1]); tc::acc_fence<32>(acc[2]); tc::acc_fence<32>(acc[3]);
@@ -300,31 +298,21 @@ struct TgPackP { const float *W; int N, K_in, n_pad; int n_kb; int col0[TG_MAX_A
 __global__ void tg_pack_weights_kernel(const __grid_constant__ TgPackP P) {
     const int kb = blockIdx.x;
     uint8_t *slab = P.out + (size_t)kb * P.n_pad * 128;
-    for (int t = threadIdx.x; t < P.n_pad * 8; t += blockDim.x) {
-        const int row = t >> 3, chunk = t & 7;
-        __half h[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const int c = chunk * 8 + e;
-            h[e] = (row < P.N && c < P.valid[kb]) ? __float2half_rn(P.W[(size_t)row * P.K_in + P.col0[kb] + c]) : __float2half_rn(0.f);
-        }
-        *reinterpret_cast<uint4 *>(slab + sw128_offset(row, chunk)) = *reinterpret_cast<uint4 *>(h);
-    }
+    for (int t = threadIdx.x; t < P.n_pad * 8; t += blockDim.x) pack_slab_chunk(slab, P.W, P.K_in, P.N, P.col0[kb], P.valid[kb], t >> 3, t & 7);
 }
 // dL/draw fp32 [rows,4] -> two one-block tile images (fp16, scaled): d_rgb in columns 0..2, d_alpha in column 0; rows beyond n_rows are zero
 __global__ void __launch_bounds__(128) tg_pack_draw_kernel(const float4 *__restrict__ d_raw, long long n_rows, uint8_t *__restrict__ z_rgb, uint8_t *__restrict__ z_alpha) {
     const long long tile = blockIdx.x, i = tile * 128 + threadIdx.x;
     const float4 g = i < n_rows ? d_raw[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     const int row = threadIdx.x;
-    uint8_t *br = z_rgb + (size_t)tile * TG_BLOCK, *ba = z_alpha + (size_t)tile * TG_BLOCK;
-    __half2 a = __floats2half2_rn(g.x * TG_SCALE, g.y * TG_SCALE), b = __floats2half2_rn(g.z * TG_SCALE, 0.f), c = __floats2half2_rn(g.w * TG_SCALE, 0.f);
-    uint4 r = make_uint4(*reinterpret_cast<uint32_t *>(&a), *reinterpret_cast<uint32_t *>(&b), 0u, 0u), al = make_uint4(*reinterpret_cast<uint32_t *>(&c), 0u, 0u, 0u), z = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4 *>(br + sw128_offset(row, 0)) = r; *reinterpret_cast<uint4 *>(br + sw128_offset(row, 1)) = z;
-    *reinterpret_cast<uint4 *>(ba + sw128_offset(row, 0)) = al; *reinterpret_cast<uint4 *>(ba + sw128_offset(row, 1)) = z;
+    uint8_t *br = z_rgb + (size_t)tile * TILE_BLOCK_BYTES, *ba = z_alpha + (size_t)tile * TILE_BLOCK_BYTES;
+    const uint4 z = make_uint4(0, 0, 0, 0);
+    st_chunk(br + sw128_offset(row, 0), make_uint4(pack_h2(g.x * TG_SCALE, g.y * TG_SCALE), pack_h2(g.z * TG_SCALE, 0.f), 0u, 0u)); st_chunk(br + sw128_offset(row, 1), z);
+    st_chunk(ba + sw128_offset(row, 0), make_uint4(pack_h2(g.w * TG_SCALE, 0.f), 0u, 0u, 0u)); st_chunk(ba + sw128_offset(row, 1), z);
 }
 
-static size_t tg_smem() { return 1024 + (size_t)TG_MAX_A * TG_BLOCK + 2 * TG_RING_SLOT + 4 * TG_BLOCK + 8 * TB_N + 64; }
-static size_t tg_dw_smem() { return 1024 + 2 * 6 * (size_t)TG_BLOCK + 8 * 4 + 64; }
+static size_t tg_smem() { return 1024 + (size_t)TG_MAX_A * TILE_BLOCK_BYTES + 2 * TG_RING_SLOT + 4 * TILE_BLOCK_BYTES + 8 * TB_N + 64; }
+static size_t tg_dw_smem() { return 1024 + 2 * 6 * (size_t)TILE_BLOCK_BYTES + 8 * 4 + 64; }
 
 }  // namespace xrb
 

@@ -22,17 +22,16 @@
 namespace xrb {
 
 constexpr float BT_SCALE = 4096.f;        // dZ staging scale (fp16): |dL/draw| < 16 stays finite, 1e-8 stays normal
-constexpr uint32_t BT_TILE = 16384;
 
 struct BtWg {
-    uint8_t *tiles;      // this warpgroup's tiles, BT_TILE bytes each
+    uint8_t *tiles;      // this warpgroup's tiles, TILE_BLOCK_BYTES bytes each
     const uint8_t *W;    // forward weight image (shared by both warpgroups)
     uint32_t wg, row, bar;
     bool first;          // first tile of this warpgroup: dW accumulators are overwritten, not accumulated
 };
 
-__device__ __forceinline__ uint8_t *bt_tile(const BtWg &c, int t) { return c.tiles + (size_t)t * BT_TILE; }
-__device__ __forceinline__ void bt_store_chunk(const BtWg &c, int t, uint32_t chunk, uint4 v) { *reinterpret_cast<uint4 *>(bt_tile(c, t) + sw128_offset(c.row, chunk)) = v; }
+__device__ __forceinline__ uint8_t *bt_tile(const BtWg &c, int t) { return c.tiles + (size_t)t * TILE_BLOCK_BYTES; }
+__device__ __forceinline__ void bt_store_chunk(const BtWg &c, int t, uint32_t chunk, uint4 v) { st_chunk(bt_tile(c, t) + sw128_offset(c.row, chunk), v); }
 __device__ __forceinline__ void bt_bar(const BtWg &c) { tc::named_bar_sync(c.bar, 128); }
 // my smem writes -> visible to the tensor core; every row of the warpgroup written
 __device__ __forceinline__ void bt_sync(const BtWg &c) { tc::fence_proxy_async_smem(); bt_bar(c); }
@@ -46,7 +45,7 @@ __device__ __forceinline__ void bt_fwd_issue(const BtWg &c, int x_tile, uint32_t
 }
 // the fp16 pair at (row r, columns col, col+1) of tile t
 __device__ __forceinline__ uint32_t *bt_word(const BtWg &c, int t, uint32_t r, uint32_t col) {
-    return reinterpret_cast<uint32_t *>(bt_tile(c, t) + sw128_offset(r, col >> 3) + (col & 7u) * 2u);
+    return reinterpret_cast<uint32_t *>(bt_tile(c, t) + sw128_offset(r, col >> 3) + (col & 7u) * 2u);   // written out: through sw128_elem this kernel allocates registers differently
 }
 // forward hidden layer: out_tile = ReLU(fp16(X W^T)), 64 wide
 template <int K>
@@ -157,8 +156,8 @@ __device__ __forceinline__ void bt_bwd(const BtWg &c, int dz_tile, int x_tile, u
 }
 // 16 fp32 values -> chunks 0,1 of tile t (fp16)
 __device__ __forceinline__ void bt_store16(const BtWg &c, int t, const float *v) {
-    bt_store_chunk(c, t, 0, make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7])));
-    bt_store_chunk(c, t, 1, make_uint4(pack_h2(v[8], v[9]), pack_h2(v[10], v[11]), pack_h2(v[12], v[13]), pack_h2(v[14], v[15])));
+    bt_store_chunk(c, t, 0, pack_h8(v));
+    bt_store_chunk(c, t, 1, pack_h8(v + 8));
 }
 
 // flush one M=64 dW accumulator (fragment rows m = frag_row (+8), columns n) into the fp32 gradient
@@ -185,7 +184,7 @@ __host__ __device__ constexpr BtLayout bt_layout(int DH, int CH) {
     return L;
 }
 template <int DH, int CH>
-__host__ __device__ constexpr size_t bt_smem_bytes(uint32_t image_bytes) { return 1024 + image_bytes + 2 * (size_t)bt_layout(DH, CH).n_tiles * BT_TILE + 16; }
+__host__ __device__ constexpr size_t bt_smem_bytes(uint32_t image_bytes) { return 1024 + image_bytes + 2 * (size_t)bt_layout(DH, CH).n_tiles * TILE_BLOCK_BYTES + 16; }
 
 template <int DH, int CH, int NP>
 __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
@@ -195,11 +194,11 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     constexpr BtLayout T = bt_layout(DH, CH);
-    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, 2 * (size_t)T.n_tiles * BT_TILE);
+    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, 2 * (size_t)T.n_tiles * TILE_BLOCK_BYTES);
     uint8_t *tiles0 = W + image_bytes;
     BtWg c;
     c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127; c.bar = 1 + c.wg;
-    c.tiles = tiles0 + (size_t)c.wg * T.n_tiles * BT_TILE; c.W = W; c.first = true;
+    c.tiles = tiles0 + (size_t)c.wg * T.n_tiles * TILE_BLOCK_BYTES; c.W = W; c.first = true;
     const WeightImageLayout L = weight_image_layout(DH, CH);
     // weight-gradient accumulators of this warpgroup, in registers for the whole persistent loop (M = 64 fragments)
     float dw_din[16], dw_dhid[DH > 1 ? DH - 1 : 1][32], dw_dout[8], dw_cin[16], dw_chid[CH > 1 ? CH - 1 : 1][32], dw_cout[8];
@@ -236,7 +235,7 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
             color_input_row(dout, dx, dy, dz, cin);                   // fp16 rounding happens in the pack below (round(round(x)) == round(x))
 #pragma unroll
             for (int q = 0; q < 4; ++q)
-                bt_store_chunk(c, T.cin, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
+                bt_store_chunk(c, T.cin, q, pack_h8(cin + 8 * q));
         }
         bt_fwd_hidden<32>(c, T.cin, L.c_in, T.c0);
 #pragma unroll

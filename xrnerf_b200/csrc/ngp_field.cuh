@@ -290,11 +290,8 @@ __device__ __forceinline__ void simt_layer(const __half *__restrict__ W, const f
     }
 }
 
-// ---------------------------------------------------------------------------- wgmma shared-memory image helpers
-// K-major, 128-byte swizzle: row r (one sample / one output neuron) occupies 128 bytes = 64 halfs; 8-row atoms of 1024 B.
-__host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) {  // byte offset of 16-byte chunk `chunk16` (0..7) of `row`
-    return (row >> 3) * 1024u + (row & 7u) * 128u + ((chunk16 ^ (row & 7u)) << 4);
-}
+// ---------------------------------------------------------------------------- wgmma weight image
+// Each matrix is a slab in the tile-image block layout (tc.cuh): row r (one output neuron) occupies 128 bytes = 64 halfs.
 struct WeightImageLayout {  // byte offsets of each matrix inside the packed image
     uint32_t d_in, d_hid[3], d_out, c_in, c_hid[3], c_out, total;
 };

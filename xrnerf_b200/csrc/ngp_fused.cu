@@ -61,7 +61,7 @@ struct FusedCtl {
     uint32_t morton[128];                 // expand_bits7 table for the occupancy test (common.cuh morton_lut_init)
 };
 __host__ __device__ inline size_t fused_smem_bytes(uint32_t image_bytes) {
-    return 1024 + image_bytes + (size_t)FR_N_WG * (16384 + TC_STAGE_BYTES) + (size_t)FR_N_SLOTS * FR_SLOT_BYTES + (size_t)FR_N_PROD * 1024 + sizeof(FusedCtl) + 64;
+    return 1024 + image_bytes + (size_t)FR_N_WG * (TILE_BLOCK_BYTES + TC_STAGE_BYTES) + (size_t)FR_N_SLOTS * FR_SLOT_BYTES + (size_t)FR_N_PROD * 1024 + sizeof(FusedCtl) + 64;
 }
 
 __device__ __forceinline__ void spin_until_ge(volatile uint32_t *p, uint32_t v) {
@@ -73,7 +73,7 @@ template <bool DEPTH>
 __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_fused_kernel(const __grid_constant__ FusedParams P) {
     extern __shared__ uint8_t dyn_smem[];
     uint8_t *base = (uint8_t *)(((uintptr_t)dyn_smem + 1023) & ~(uintptr_t)1023);
-    uint8_t *W = base, *A = W + P.image_bytes, *stage = A + (size_t)FR_N_WG * 16384, *slots = stage + (size_t)FR_N_WG * TC_STAGE_BYTES, *mailbox = slots + (size_t)FR_N_SLOTS * FR_SLOT_BYTES;
+    uint8_t *W = base, *A = W + P.image_bytes, *stage = A + (size_t)FR_N_WG * TILE_BLOCK_BYTES, *slots = stage + (size_t)FR_N_WG * TC_STAGE_BYTES, *mailbox = slots + (size_t)FR_N_SLOTS * FR_SLOT_BYTES;
     FusedCtl *ctl = (FusedCtl *)(mailbox + (size_t)FR_N_PROD * 1024);
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if ((P.dbg & 8) && threadIdx.x == 0) {
@@ -99,7 +99,7 @@ __global__ void __launch_bounds__((4 * FR_N_WG + FR_N_PROD) * 32, 1) ngp_render_
         // ===================================================================== field warpgroups
         TcWarpgroup c;
         c.wg = warp >> 2; c.row = threadIdx.x & 127;
-        c.A = A + (size_t)c.wg * 16384; c.W = W; c.stage = (float *)(stage + (size_t)c.wg * TC_STAGE_BYTES); c.bar = 1 + c.wg;
+        c.A = A + (size_t)c.wg * TILE_BLOCK_BYTES; c.W = W; c.stage = (float *)(stage + (size_t)c.wg * TC_STAGE_BYTES); c.bar = 1 + c.wg;
         const WeightImageLayout L = weight_image_layout(P.density_hidden, P.color_hidden);
         const bool timed = (P.dbg & 8) && c.wg == 0;
         tc::mbar_wait(&ctl->wbar, 0);

@@ -33,13 +33,7 @@ __global__ void pack_weights_kernel(const float *__restrict__ dens, const float 
         for (int q = 0; q < li; ++q) poff += (size_t)64 * (q == 0 ? 32 : 64);
         const float *Wm = params + poff;                                   // W[N][K] row-major (tcnn layout)
         uint32_t ioff = is_color ? (li == 0 ? L.c_in : (li == n_hidden ? L.c_out : L.c_hid[li - 1])) : (li == 0 ? L.d_in : (li == n_hidden ? L.d_out : L.d_hid[li - 1]));
-        for (int t = threadIdx.x; t < N * 8; t += blockDim.x) {
-            int row = t >> 3, chunk = t & 7;
-            __half h[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { int k = chunk * 8 + e; h[e] = k < K ? __float2half_rn(Wm[(size_t)row * K + k]) : __float2half_rn(0.f); }
-            *reinterpret_cast<uint4 *>(image + ioff + sw128_offset(row, chunk)) = *reinterpret_cast<uint4 *>(h);
-        }
+        for (int t = threadIdx.x; t < N * 8; t += blockDim.x) pack_slab_chunk(image + ioff, Wm, K, N, 0, K, t >> 3, t & 7);
     }
 }
 

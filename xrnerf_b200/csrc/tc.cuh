@@ -1,7 +1,9 @@
 // xrnerf_b200 — thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: wgmma (warpgroup MMA, shared-memory operands,
 // register accumulators), mbarrier, 1-D TMA bulk copy, proxy fences. No CUTLASS dependency; descriptor encodings follow the PTX ISA
-// ("Matrix Descriptor Format" of wgmma) and cute/arch/mma_sm90_desc.hpp.
+// ("Matrix Descriptor Format" of wgmma) and cute/arch/mma_sm90_desc.hpp. Also the one definition of the tile-image layout those
+// descriptors read (end of file).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -159,4 +161,43 @@ __device__ __forceinline__ void acc_fence(float *d) {
 __device__ __forceinline__ uint32_t frag_row(uint32_t t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
 __device__ __forceinline__ uint32_t frag_col(uint32_t t, uint32_t j) { return 8u * j + 2u * (t & 3u); }
 
-}}  // namespace xrb::tc
+}  // namespace tc
+
+// ---- tile images: a matrix [rows x C] stored per 128-row tile as C/64 blocks of [128 x 64] fp16, K-major with the 128-byte swizzle desc_k128
+// reads. Row r of a block is 128 bytes (eight 16-byte chunks) in 8-row atoms of 1024 B; chunk c of row r sits at chunk position c ^ (r % 8).
+// The NGP field's A tile and every weight slab [N x 64] use the same block layout.
+constexpr uint32_t TILE_ROWS = 128, TILE_BLOCK_COLS = 64, TILE_BLOCK_BYTES = TILE_ROWS * TILE_BLOCK_COLS * 2;
+
+// byte offset of 16-byte chunk `chunk16` (0..7) of `row` in a block = sw128_row(row) + sw128_chunk(row, chunk16)
+__host__ __device__ __forceinline__ uint32_t sw128_row(uint32_t row) { return (row >> 3) * 1024u + (row & 7u) * 128u; }
+// the address of `row` in the block at blk, its two terms added to the pointer one by one (the schedule of the fast IPE encoder depends on it)
+__device__ __forceinline__ uint8_t *sw128_row_ptr(uint8_t *blk, uint32_t row) { return blk + (row >> 3) * 1024u + (row & 7u) * 128u; }
+__host__ __device__ __forceinline__ uint32_t sw128_chunk(uint32_t row, uint32_t chunk16) { return (chunk16 ^ (row & 7u)) << 4; }
+__host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) { return sw128_row(row) + sw128_chunk(row, chunk16); }
+// address of the fp16 element (row, col) of the block at blk, col < 64
+template <class B> __device__ __forceinline__ B *sw128_elem(B *blk, uint32_t row, uint32_t col) { return blk + sw128_offset(row, col >> 3) + (col & 7u) * 2u; }
+
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t *>(&h);
+}
+// 8 floats -> one chunk of fp16
+__device__ __forceinline__ uint4 pack_h8(const float *v) { return make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7])); }
+__device__ __forceinline__ void st_chunk(uint8_t *p, uint4 v) { *reinterpret_cast<uint4 *>(p) = v; }
+// 8 floats as fp16 into chunk `chunk16` of `row`, given the row's address (kernels that write a whole row compute it once)
+__device__ __forceinline__ void st_row_chunk(uint8_t *row_ptr, uint32_t row, uint32_t chunk16, const float *v) { st_chunk(row_ptr + sw128_chunk(row, chunk16), pack_h8(v)); }
+
+// block b of tile `tile` of an image with n_blk blocks per tile, and the bytes of an image of n_rows rows
+__host__ __device__ __forceinline__ uint8_t *tile_block(uint8_t *image, int64_t tile, int n_blk, int b) { return image + ((size_t)tile * n_blk + b) * TILE_BLOCK_BYTES; }
+__host__ __device__ __forceinline__ size_t tile_image_bytes(int64_t n_rows, int n_blk) { return (size_t)((n_rows + TILE_ROWS - 1) / TILE_ROWS) * n_blk * TILE_BLOCK_BYTES; }
+
+// chunk `chunk` of row `row` of a weight slab <- fp16 of W[row][col0 + 8 chunk ..] (W fp32 row-major with row length ld); zero for rows >= n and
+// for the columns from `valid` on
+__device__ __forceinline__ void pack_slab_chunk(uint8_t *slab, const float *W, int ld, int n, int col0, int valid, int row, int chunk) {
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) { const int c = 8 * chunk + e; v[e] = (row < n && c < valid) ? W[(size_t)row * ld + col0 + c] : 0.f; }
+    st_chunk(slab + sw128_offset(row, chunk), pack_h8(v));
+}
+
+}  // namespace xrb

@@ -29,11 +29,7 @@ struct TcWarpgroup {
 };
 constexpr uint32_t TC_STAGE_BYTES = 128 * 16 * 4;
 
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-__device__ __forceinline__ void a_store_chunk(const TcWarpgroup &c, uint32_t chunk, uint4 v) { *reinterpret_cast<uint4 *>(c.A + sw128_offset(c.row, chunk)) = v; }
+__device__ __forceinline__ void a_store_chunk(const TcWarpgroup &c, uint32_t chunk, uint4 v) { st_chunk(c.A + sw128_offset(c.row, chunk), v); }
 __device__ __forceinline__ void tc_bar(const TcWarpgroup &c) { tc::named_bar_sync(c.bar, 128); }
 
 // accumulator (fp32 pair) -> fp16 -> ReLU. Rounding to fp16 first and clamping the packed pair (one cvt.rn.f16x2 + one max.f16x2 per two values)
@@ -133,8 +129,7 @@ __device__ __forceinline__ void tc_store_color_input(const TcWarpgroup &c, const
     float cin[32];
     color_input_row(dout, dx, dy, dz, cin);
 #pragma unroll
-    for (int q = 0; q < 4; ++q)
-        a_store_chunk(c, q, make_uint4(pack_h2(cin[8 * q], cin[8 * q + 1]), pack_h2(cin[8 * q + 2], cin[8 * q + 3]), pack_h2(cin[8 * q + 4], cin[8 * q + 5]), pack_h2(cin[8 * q + 6], cin[8 * q + 7])));
+    for (int q = 0; q < 4; ++q) a_store_chunk(c, q, pack_h8(cin + 8 * q));
 }
 // Colour half (HashNerfMLP.run_mlp, hashnerf_mlp.py:66-79) given density_net's outputs: raw = (rgb[3], density[1]) for my sample
 __device__ __forceinline__ float4 tc_color_from_density(const TcWarpgroup &c, const WeightImageLayout &L, int color_hidden, const float *dout, float dx, float dy, float dz) {
@@ -154,7 +149,7 @@ __device__ __forceinline__ void tc_gather_levels(const __half2 *__restrict__ tab
 // ---- CTA-level setup shared by the kernels that use the warpgroup evaluator
 // dynamic shared memory layout: [weights image][A tile x WG][staging tile x WG][mbarrier]
 template <int WG>
-__host__ __device__ inline size_t tc_cta_smem_bytes(uint32_t image_bytes) { return 1024 /*align slack*/ + image_bytes + (size_t)WG * (16384 + TC_STAGE_BYTES) + 16; }
+__host__ __device__ inline size_t tc_cta_smem_bytes(uint32_t image_bytes) { return 1024 /*align slack*/ + image_bytes + (size_t)WG * (TILE_BLOCK_BYTES + TC_STAGE_BYTES) + 16; }
 
 // Called by every thread of the CTA: bulk-copies (TMA) the weight image to the first 1024-byte aligned address of the dynamic shared memory, waits for it
 // and returns that address. tiles_bytes: what the kernel keeps between the image (a multiple of 1024 bytes) and the copy's mbarrier.
@@ -174,12 +169,12 @@ __device__ __forceinline__ uint8_t *tc_load_weight_image(uint8_t *dyn_smem, cons
 
 template <int WG>
 __device__ __forceinline__ TcWarpgroup tc_cta_setup(uint8_t *dyn_smem, const void *weight_image, uint32_t image_bytes) {
-    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, (size_t)WG * (16384 + TC_STAGE_BYTES));
+    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, (size_t)WG * (TILE_BLOCK_BYTES + TC_STAGE_BYTES));
     uint8_t *A0 = W + image_bytes;
-    float *stage0 = (float *)(A0 + (size_t)WG * 16384);
+    float *stage0 = (float *)(A0 + (size_t)WG * TILE_BLOCK_BYTES);
     TcWarpgroup c;
     c.wg = threadIdx.x >> 7; c.row = threadIdx.x & 127; c.bar = 1 + c.wg;
-    c.A = A0 + (size_t)c.wg * 16384; c.W = W; c.stage = stage0 + (size_t)c.wg * (TC_STAGE_BYTES / 4);
+    c.A = A0 + (size_t)c.wg * TILE_BLOCK_BYTES; c.W = W; c.stage = stage0 + (size_t)c.wg * (TC_STAGE_BYTES / 4);
     return c;
 }
 

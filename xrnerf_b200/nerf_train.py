@@ -93,13 +93,6 @@ class _Slabs:
                                                      C.c_void_p(self.arena.data_ptr() + L['off']), _C.stream()), 'tg_pack_weights')
 
 
-_C.lib.xrb_nerf_tg_pack_weights.restype = C.c_int
-_C.lib.xrb_nerf_tg_pack_weights.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
-_C.lib.xrb_nerf_tg_pack_draw.restype = C.c_int
-_C.lib.xrb_nerf_tg_pack_draw.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
-_C.lib.xrb_nerf_tg_grad_scale.restype = C.c_float
-
-
 def _layer(n_rows, a_srcs, w_arena, slabs, b_mn, mma_n, out_cols, epi, relu=0, bias=None, x=None, y=None, yf=None, yf_col=0, yf_n=0):
     L = TgLayer()
     for s, a in enumerate(a_srcs):
