@@ -369,7 +369,7 @@ int xrb_nerf_zvals(int64_t n_rays, int n_samples, float near_, float far_, int l
  * K-major 128-byte-swizzle layout: the encoders' output format, xrb_nerf_enc_image_bytes). The host (xrnerf_b200/nerf_train.py) strings the layers together.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
-    /* A operand: up to two sources, concatenated block-wise (e.g. the skip layer: point-encoding block + 4 hidden blocks); <= 5 blocks in total */
+    /* A operand: up to two sources, concatenated block-wise (e.g. the skip layer: point-encoding blocks + 4 hidden blocks); <= 6 blocks in total */
     const void *a_base[2]; uint32_t a_tile_stride[2]; uint32_t a_blk_off[2]; int a_n_blk[2]; int n_a;
     const void *w;                       /* weight slabs (xrb_nerf_tg_pack_weights) */
     /* per weight slab: byte offset in w, bytes (<= 32768), MMA groups using it (A block a_blk0 + j), K-steps of 16 per group (1..4), accumulator column, first-writer flag */
@@ -387,19 +387,23 @@ typedef struct {
 } xrb_tg_layer;
 int xrb_nerf_tg_layer(const xrb_tg_layer *layer, void *stream);
 /* weight gradient of one layer and one input source: dW[N][K] (fp32, ACCUMULATED) [:, k_off : k_off + k_cols] += dZ^T . X over all rows; db[N] += column sums of dZ
- * when db != NULL. z: dZ image (N/64 blocks per tile, 1 block for N <= 16), x: input image source (1..4 blocks). Gradients are unscaled by xrb_nerf_tg_grad_scale(). */
+ * when db != NULL. z: dZ image (N/64 blocks per tile, 1 block for N <= 16; zero in the rows >= n_rows), x: input image source (1..4 blocks, k_cols <= 64 x_n_blk).
+ * Gradients are unscaled by *scale (the staging scale xrb_nerf_tg_pack_draw wrote; NULL: xrb_nerf_tg_grad_scale()). */
 typedef struct {
     const void *z_base; uint32_t z_tile_stride; uint32_t z_blk_off;
     const void *x_base; uint32_t x_tile_stride; uint32_t x_blk_off; int x_n_blk;
     int N, K, k_off, k_cols;
     float *dW; float *db;
     int64_t n_rows;
+    const float *scale;
 } xrb_tg_dw;
 int xrb_nerf_tg_dw(const xrb_tg_dw *layer, void *stream);
 /* nn.Linear weight W[N][K_in] (fp32) -> n_kb slabs [n_pad x 64] fp16 (n_pad = N rounded up to 16): slab kb holds input columns [col0[kb], + valid[kb]) (zero beyond) */
 int xrb_nerf_tg_pack_weights(const float *W, int N, int K_in, int n_pad, int n_kb, const int *col0_host, const int *valid_host, void *slabs, void *stream);
-/* dL/draw f32[n_rows,4] -> the two one-block dZ images of the output heads (d rgb in columns 0..2, d alpha in column 0), scaled by xrb_nerf_tg_grad_scale() */
-int xrb_nerf_tg_pack_draw(const float *d_raw, int64_t n_rows, void *z_rgb_image, void *z_alpha_image, void *stream);
+/* dL/draw f32[n_rows,4] -> the two one-block dZ images of the output heads (d rgb in columns 0..2, d alpha in column 0, every other entry 0), multiplied by
+ * the power of two s chosen on the device with max |dL/draw| s in [2^12, 2^13) (xrb_nerf_tg_grad_scale() when dL/draw is all zero or not finite).
+ * scale: device f32[2], scale[0] workspace, scale[1] <- s (the xrb_tg_dw.scale of the layers' weight gradients). */
+int xrb_nerf_tg_pack_draw(const float *d_raw, int64_t n_rows, void *z_rgb_image, void *z_alpha_image, float *scale, void *stream);
 float xrb_nerf_tg_grad_scale(void);
 
 /* Measurement utility (bench.py's second roofline; no reference counterpart): random reads of 4-, 8- or 32-byte records from a table (L2-resident when

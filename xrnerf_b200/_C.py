@@ -112,7 +112,7 @@ _SIGS = {
     'xrb_nerf_tg_layer': (_i, [P, P]),
     'xrb_nerf_tg_dw': (_i, [P, P]),
     'xrb_nerf_tg_pack_weights': (_i, [P, _i, _i, _i, _i, C.POINTER(C.c_int), C.POINTER(C.c_int), P, P]),
-    'xrb_nerf_tg_pack_draw': (_i, [P, _i64, P, P, P]),
+    'xrb_nerf_tg_pack_draw': (_i, [P, _i64, P, P, P, P]),
     'xrb_nerf_tg_grad_scale': (C.c_float, []),
     'xrb_micro_gather': (_i, [P, _i64, _i, _i, C.POINTER(C.c_int64), P, P]),
     'xrb_nerf_zvals': (_i, [_i64, _i, _f, _f, _i, P, P, P]),

@@ -15,7 +15,9 @@
 //                CUDA cores from the same staged dZ block while the MMAs run. One flush per CTA (fp32 atomics).
 // Warp roles: warps 0-7 two consumer warpgroups (issue the MMAs of their rows, run the epilogue), warp 8 TMA producer (one lane); in tg_kernel the producer's
 // warpgroup (warps 8-11) hands its registers to the consumers (setmaxnreg 40 / 232).
-// dZ is staged in fp16 with a fixed scale (2^14, applied where dL/draw enters and removed at the dW flush): tcnn-style loss scaling for 1e-6-sized NeRF gradients.
+// dZ is staged in fp16 with a per-batch power-of-two scale s, chosen on the device from max |dL/draw| so that the head's largest staged value is in [2^12, 2^13)
+// (tg_draw_max_kernel + tg_pack_draw_kernel), and removed exactly at the dW flush: the NeRF loss gives dL/draw of 1e-8 .. 1e-5, and with a fixed scale most of the
+// trunk's dZ fell below fp16's normal range. No host synchronisation; the head cannot overflow, and dZ shrinks on its way down the trunk.
 #include "tc.cuh"
 #include "common.cuh"
 #include <cuda_fp16.h>
@@ -25,7 +27,8 @@ namespace xrb {
 
 constexpr int TG_MAX_A = 6, TG_MAX_SLABS = 10, TG_THREADS = 384, TG_DW_THREADS = 288;   // 6 A blocks: Mip-NeRF's skip layer reads 2 IPE blocks + 4 hidden blocks
 constexpr uint32_t TG_RING_SLOT = 32768;   // one [256 x 64] fp16 slab
-constexpr float TG_SCALE = 16384.f;
+constexpr float TG_SCALE = 16384.f;      // the scale when dL/draw is all zero or not finite
+constexpr int TG_HEAD_EXP = 12;          // max |dL/draw| s is in [2^TG_HEAD_EXP, 2^(TG_HEAD_EXP + 1))
 
 struct TgOp { const uint8_t *base; uint32_t tile_stride, blk_off; int n_blk; };   // blocks [blk_off/16K, +n_blk) of every tile of an image
 struct TgSlab { uint32_t w_off, bytes; int n_sub, a_blk0, d_col, first, n_k; };    // one weight slab: loaded once per tile, used by n_sub MMA groups (A block a_blk0 + j) of n_k K-steps of 16
@@ -193,6 +196,7 @@ struct TgDwP {
     int k_off, k_cols;      // this source's columns [k_off, k_off + k_cols) of the layer input
     float *dW; float *db;   // fp32 gradients (accumulated); db == NULL: no bias gradient from this launch
     long long n_rows;
+    const float *scale;     // the dZ staging scale (device, written by tg_pack_draw_kernel); NULL: TG_SCALE
 };
 
 // Warps 0-7: two consumer warpgroups, warpgroup h owns accumulator rows 64h..64h+63 of the CTA's 128-row chunk (registers, across the CTA's whole
@@ -265,7 +269,7 @@ __global__ void __launch_bounds__(TG_DW_THREADS, 1) tg_dw_kernel(const __grid_co
         if (lane == 0) tc::mbar_arrive(bars + 2 + st);
     }
     // ---- flush from the fragments: register 4j + i holds row m0 + 8 (i / 2), column 8j + 2 (t % 4) + i % 2
-    const float inv = 1.f / TG_SCALE;
+    const float inv = 1.f / (P.scale ? *P.scale : TG_SCALE);   // a power of two: exact
     const int m0 = 64 * wg + (int)tc::frag_row((uint32_t)t);
     if (!P.transposed) {
 #pragma unroll
@@ -300,15 +304,34 @@ __global__ void tg_pack_weights_kernel(const __grid_constant__ TgPackP P) {
     uint8_t *slab = P.out + (size_t)kb * P.n_pad * 128;
     for (int t = threadIdx.x; t < P.n_pad * 8; t += blockDim.x) pack_slab_chunk(slab, P.W, P.K_in, P.N, P.col0[kb], P.valid[kb], t >> 3, t & 7);
 }
-// dL/draw fp32 [rows,4] -> two one-block tile images (fp16, scaled): d_rgb in columns 0..2, d_alpha in column 0; rows beyond n_rows are zero
-__global__ void __launch_bounds__(128) tg_pack_draw_kernel(const float4 *__restrict__ d_raw, long long n_rows, uint8_t *__restrict__ z_rgb, uint8_t *__restrict__ z_alpha) {
+// max |dL/draw| over the batch -> scale[0] (its fp32 bits: for non-negative floats the unsigned order is the numeric order; NaN sorts above +inf)
+__global__ void __launch_bounds__(256) tg_draw_max_kernel(const float *__restrict__ d_raw, long long n, float *scale) {
+    uint32_t m = 0;
+    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) m = max(m, __float_as_uint(fabsf(d_raw[i])));
+    for (int o = 16; o; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int *>(scale), m);
+}
+// the power of two s with max |dL/draw| s in [2^12, 2^13) (TG_SCALE when the maximum is 0 or not finite), kept within fp32's normal range
+__device__ __forceinline__ float tg_scale_of(uint32_t max_bits) {
+    const float m = __uint_as_float(max_bits);
+    if (!(m > 0.f) || !isfinite(m)) return TG_SCALE;
+    return exp2f((float)min(max(TG_HEAD_EXP - ilogbf(m), -120), 120));
+}
+// dL/draw fp32 [rows,4] -> two one-block tile images (fp16 of dL/draw * s): d_rgb in columns 0..2, d_alpha in column 0, every other entry and the rows beyond
+// n_rows zero; s (from the maximum in scale[0]) -> scale[1] for the dW flushes
+__global__ void __launch_bounds__(128) tg_pack_draw_kernel(const float4 *__restrict__ d_raw, long long n_rows, uint8_t *__restrict__ z_rgb, uint8_t *__restrict__ z_alpha,
+                                                           float *scale) {
     const long long tile = blockIdx.x, i = tile * 128 + threadIdx.x;
+    const float s = tg_scale_of(__float_as_uint(scale[0]));
+    if (tile == 0 && threadIdx.x == 0) scale[1] = s;
     const float4 g = i < n_rows ? d_raw[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     const int row = threadIdx.x;
     uint8_t *br = z_rgb + (size_t)tile * TILE_BLOCK_BYTES, *ba = z_alpha + (size_t)tile * TILE_BLOCK_BYTES;
     const uint4 z = make_uint4(0, 0, 0, 0);
-    st_chunk(br + sw128_offset(row, 0), make_uint4(pack_h2(g.x * TG_SCALE, g.y * TG_SCALE), pack_h2(g.z * TG_SCALE, 0.f), 0u, 0u)); st_chunk(br + sw128_offset(row, 1), z);
-    st_chunk(ba + sw128_offset(row, 0), make_uint4(pack_h2(g.w * TG_SCALE, 0.f), 0u, 0u, 0u)); st_chunk(ba + sw128_offset(row, 1), z);
+    st_chunk(br + sw128_offset(row, 0), make_uint4(pack_h2(g.x * s, g.y * s), pack_h2(g.z * s, 0.f), 0u, 0u));
+    st_chunk(ba + sw128_offset(row, 0), make_uint4(pack_h2(g.w * s, 0.f), 0u, 0u, 0u));
+#pragma unroll
+    for (uint32_t c = 1; c < 8; ++c) { st_chunk(br + sw128_offset(row, c), z); st_chunk(ba + sw128_offset(row, c), z); }
 }
 
 static size_t tg_smem() { return 1024 + (size_t)TG_MAX_A * TILE_BLOCK_BYTES + 2 * TG_RING_SLOT + 4 * TILE_BLOCK_BYTES + 8 * TB_N + 64; }
@@ -342,6 +365,9 @@ int xrb_nerf_tg_layer(const xrb_tg_layer *L, void *stream) {
         XRB_REQUIRE(L->slab_n_k[s] >= 1 && L->slab_n_k[s] <= 4 && L->slab_n_sub[s] >= 1, "tg_layer: slab K-steps");
         XRB_REQUIRE(L->slab_bytes[s] <= TG_RING_SLOT && (L->slab_bytes[s] % 1024) == 0 && (L->slab_w_off[s] % 128) == 0, "tg_layer: slab size/offset");
         XRB_REQUIRE(L->slab_a_blk0[s] + L->slab_n_sub[s] <= n_ablk && L->slab_d_col[s] + L->mma_n <= 256, "tg_layer: slab refers outside the tile");
+        // every MMA reads inside the slab's bytes: K-major, mma_n rows of 128 bytes; MN-major, group j K-step k reads the 2 KB at (4 j + k) * 2048
+        XRB_REQUIRE(L->b_mn ? ((uint32_t)((L->slab_n_sub[s] - 1) * 4 + L->slab_n_k[s]) * 2048u <= L->slab_bytes[s]) : ((uint32_t)L->mma_n * 128u <= L->slab_bytes[s]),
+                    "tg_layer: MMA reads past the slab");
         XRB_REQUIRE(L->mma_n == 64 ? (L->slab_d_col[s] >= 0 && L->slab_d_col[s] % 64 == 0) : L->slab_d_col[s] == 0,
                     "tg_layer: implemented MMA shapes are N = 16 / 128 / 256 at accumulator column 0 and N = 64 at columns 0 / 64 / 128 / 192");
     }
@@ -361,12 +387,13 @@ int xrb_nerf_tg_layer(const xrb_tg_layer *L, void *stream) {
 int xrb_nerf_tg_dw(const xrb_tg_dw *L, void *stream) {
     XRB_REQUIRE(L, "tg_dw: null descriptor");
     XRB_REQUIRE(L->n_rows >= 0 && L->N >= 1 && L->K >= 1 && L->x_n_blk >= 1 && L->x_n_blk <= 4 && L->k_off >= 0 && L->k_cols >= 1 && L->k_off + L->k_cols <= L->K, "tg_dw: bad sizes");
+    XRB_REQUIRE(L->k_cols <= 64 * L->x_n_blk, "tg_dw: k_cols wider than the input blocks");
     if (L->n_rows == 0) return XRB_OK;
     XRB_REQUIRE(L->z_base && L->x_base && L->dW, "tg_dw: null pointer");
     TgDwP P{};
     P.z = TgOp{(const uint8_t *)L->z_base, L->z_tile_stride, L->z_blk_off, 0};
     P.x = TgOp{(const uint8_t *)L->x_base, L->x_tile_stride, L->x_blk_off, L->x_n_blk};
-    P.N = L->N; P.K = L->K; P.k_off = L->k_off; P.k_cols = L->k_cols; P.dW = L->dW; P.db = L->db; P.n_rows = L->n_rows;
+    P.N = L->N; P.K = L->K; P.k_off = L->k_off; P.k_cols = L->k_cols; P.dW = L->dW; P.db = L->db; P.n_rows = L->n_rows; P.scale = L->scale;
     P.transposed = L->N <= 16;
     if (P.transposed) { XRB_REQUIRE((L->x_n_blk % 2) == 0, "tg_dw: 16-output layers take an input image of 128 or 256 columns"); P.n_chunks = L->x_n_blk / 2; }
     else { XRB_REQUIRE(L->N == 128 || L->N == 256, "tg_dw: N must be 128 or 256 (or <= 16)"); P.n_chunks = L->N / 128; }
@@ -387,11 +414,13 @@ int xrb_nerf_tg_pack_weights(const float *W, int N, int K_in, int n_pad, int n_k
     return check_launch("nerf_tg_pack_weights");
 }
 
-int xrb_nerf_tg_pack_draw(const float *d_raw, int64_t n_rows, void *z_rgb_image, void *z_alpha_image, void *stream) {
+int xrb_nerf_tg_pack_draw(const float *d_raw, int64_t n_rows, void *z_rgb_image, void *z_alpha_image, float *scale, void *stream) {
     XRB_REQUIRE(n_rows >= 0, "tg_pack_draw: negative size");
     if (n_rows == 0) return XRB_OK;
-    XRB_REQUIRE(d_raw && z_rgb_image && z_alpha_image && ((uintptr_t)d_raw & 15) == 0, "tg_pack_draw: null / misaligned pointer");
-    tg_pack_draw_kernel<<<(unsigned)((n_rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>((const float4 *)d_raw, n_rows, (uint8_t *)z_rgb_image, (uint8_t *)z_alpha_image);
+    XRB_REQUIRE(d_raw && z_rgb_image && z_alpha_image && scale && ((uintptr_t)d_raw & 15) == 0 && ((uintptr_t)scale & 3) == 0, "tg_pack_draw: null / misaligned pointer");
+    cudaMemsetAsync(scale, 0, sizeof(float), (cudaStream_t)stream);
+    tg_draw_max_kernel<<<stride_grid((4 * n_rows + 255) / 256, 4), 256, 0, (cudaStream_t)stream>>>(d_raw, 4 * n_rows, scale);
+    tg_pack_draw_kernel<<<(unsigned)((n_rows + 127) / 128), 128, 0, (cudaStream_t)stream>>>((const float4 *)d_raw, n_rows, (uint8_t *)z_rgb_image, (uint8_t *)z_alpha_image, scale);
     return check_launch("nerf_tg_pack_draw");
 }
 
