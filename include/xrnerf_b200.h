@@ -215,13 +215,10 @@ int xrb_ngp_mlp_backward_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tabl
                             float *d_density, float *d_color, void *stream);
 
 /* Fused Adam step on an fp32 master vector + refresh of its fp16 working copy (torch.optim.Adam semantics with
- * L2 weight_decay folded into the gradient; configs/instant_ngp/nerf_blender_local01.py:13-18). grad is divided by
- * grad_div first (world size after a sum all-reduce). */
-int xrb_adam_step(float *param, void *param_fp16, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
-                  float beta1, float beta2, float eps, float weight_decay, int step, float grad_div, void *stream);
-/* The same step with the runner's EMAHook (configs/instant_ngp/nerf_blender_local01.py:24: momentum 0.05; mmcv EMAHook.after_train_iter:
- * ema = (1 - m) * ema + m * param, m = min(momentum, (1 + iter) / (warm_up + iter)) computed by the caller) folded into the pass:
- * ema f32[n] (NULL = no EMA), initialised by the caller as a copy of param (EMAHook.before_run). */
+ * L2 weight_decay folded into the gradient; configs/instant_ngp/nerf_blender_local01.py:13-18), with the runner's EMAHook folded into the same
+ * pass (configs/instant_ngp/nerf_blender_local01.py:24: momentum 0.05; mmcv EMAHook.after_train_iter: ema = (1 - m) * ema + m * param,
+ * m = min(momentum, (1 + iter) / (warm_up + iter)) computed by the caller): ema f32[n] (NULL = no EMA), initialised by the caller as a copy of
+ * param (EMAHook.before_run). grad is divided by grad_div first (world size after a sum all-reduce). param_fp16 NULL = no fp16 copy. */
 int xrb_adam_ema_step(float *param, void *param_fp16, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr,
                       float beta1, float beta2, float eps, float weight_decay, int step, float grad_div, float *ema, float ema_momentum, void *stream);
 

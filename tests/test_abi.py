@@ -22,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert len(names) >= 40
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, missing
-    assert lib.xrb_abi_version() == 4 and lib.xrb_built_for_sm() == 90
+    assert lib.xrb_abi_version() == 5 and lib.xrb_built_for_sm() == 90
 
 
 def test_python_binding_covers_header():

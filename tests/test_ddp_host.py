@@ -1,45 +1,9 @@
-"""world_size-2 gloo test (CPU) of the data-parallel host logic: the flat gradient buffer all-reduce and the grad_div it returns."""
+"""world_size-2 gloo test (CPU) of the data-parallel host logic: the sharded gradient exchange (slice bounds, reduce-scatter, all-gather)."""
 import os
 
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
-
-
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    from xrnerf_b200.train import FlatGradBuffer, huber5_grad
-    params = [torch.zeros(1000), torch.zeros(37), torch.zeros(5)]
-    buf = FlatGradBuffer(params)
-    for k, v in enumerate(buf.views):
-        v.fill_(float(rank + 1) * (k + 1))
-    div = buf.allreduce()
-    ok = div == 2.0 and all(torch.allclose(v, torch.full_like(v, 3.0 * (k + 1))) for k, v in enumerate(buf.views)) and buf.flat.numel() == 1042
-    # ray sharding: rank r takes rays r::world of a shuffled table (DistributedSampler semantics, distributed_sampler.py:37)
-    table = torch.arange(64)
-    mine = table[rank::world]
-    gathered = [torch.zeros_like(mine) for _ in range(world)]
-    dist.all_gather(gathered, mine)
-    ok = ok and sorted(torch.cat(gathered).tolist()) == list(range(64))
-    loss, g = huber5_grad(torch.tensor([[0.5, 0.0, 1.0]]), torch.tensor([[0.45, 0.5, 1.0]]))
-    ok = ok and abs(loss.item() - 5 * (0.5 / 0.1 * 0.05 ** 2 + 0.5 - 0.05)) < 1e-6 and torch.allclose(g, torch.tensor([[2.5, -5.0, 0.0]]))
-    q.put((rank, bool(ok)))
-    dist.destroy_process_group()
-
-
-def test_flat_grad_allreduce_gloo_world2():
-    import socket
-    s = socket.socket(); s.bind(('127.0.0.1', 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context('spawn')
-    q = ctx.Queue()
-    ps = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in ps:
-        p.start()
-    res = [q.get(timeout=120) for _ in ps]
-    for p in ps:
-        p.join(timeout=60)
-    assert sorted(res) == [(0, True), (1, True)]
 
 
 def _worker_sharded(rank, world, port, q):

@@ -193,7 +193,8 @@ def test_adam_step_matches_torch():
     for step in range(1, 4):
         ref.grad = g.clone() * step
         opt.step()
-        _C.check(_C.lib.xrb_adam_step(_C.ptr(p), _C.ptr(p16), _C.ptr(g * step * 2.0), _C.ptr(m), _C.ptr(v), n, 1e-2, 0.9, 0.99, 1e-15, 1e-6, step, 2.0, _C.stream()))
+        _C.check(_C.lib.xrb_adam_ema_step(_C.ptr(p), _C.ptr(p16), _C.ptr(g * step * 2.0), _C.ptr(m), _C.ptr(v), n, 1e-2, 0.9, 0.99, 1e-15, 1e-6, step, 2.0, None, 0.0,
+                                          _C.stream()))
     assert torch.allclose(p, ref.detach(), rtol=1e-5, atol=1e-6)
     assert torch.equal(p16, p.half())
 

@@ -1,6 +1,6 @@
 """The NGP training step's small kernels on their own: the 5 x Huber loss and its gradient, the bf16 gradient pack and the Adam + EMA step
-that reads it (the sharded data-parallel path), and the count of fully trained rays. Each is checked bit for bit where its arithmetic is
-one fp32 expression, and against float64 within a stated bound where it is a sum."""
+that reads it (the sharded data-parallel path), the peer-memory Adam + EMA step against the local one, and the count of fully trained rays.
+Each is checked bit for bit where its arithmetic is one fp32 expression, and against float64 within a stated bound where it is a sum."""
 import numpy as np
 import pytest
 import torch
@@ -116,6 +116,68 @@ def test_adam_ema_step_bf16grad():
     assert torch.equal(p16, p16b)
     assert torch.allclose(a['p'].double(), ref.detach(), rtol=1e-5, atol=1e-6)
     assert torch.allclose(a['ema'].double(), ema_ref, rtol=1e-5, atol=1e-6)
+
+
+# ----------------------------------------------------------------------------------------------------------------------------- peer Adam + EMA at world 1
+def test_peer_adam_step_world1_bits_match_local_adam():
+    """xrb_peer_publish_grads + xrb_peer_adam_step on one rank's own exchange block (world 1, no IPC mapping), 4 steps with weight decay and EMA:
+    the table slice (8-wide path and scalar tail: n_table is not a multiple of 8) is bit-identical to xrb_adam_ema_step_bf16grad fed xrb_pack_bf16 of
+    the same fp32 gradient, and both MLP groups to xrb_adam_ema_step on the fp32 gradient (master, moments, EMA, fp16 copies). Parameters have no
+    exact zeros: the peer sum 0 + g turns a -0 gradient into +0, which weight decay would otherwise expose."""
+    from xrnerf_b200 import _C
+    from xrnerf_b200.train import _DevView, shard_range
+    C = _C.C
+    torch.manual_seed(5)
+    n_table, n_mlp = (70003, (4099, 2055))
+    _, _, per, padded = shard_range(n_table, 1, 0)
+    lr, b1, b2, eps, wd = 1e-2, 0.9, 0.99, 1e-15, 1e-6
+    a16 = lambda x: (x + 15) // 16 * 16   # noqa: E731
+    off_g16 = 128
+    off_gmlp = a16(off_g16 + 2 * padded)
+    off_t16 = a16(off_gmlp + 4 * sum(n_mlp))
+    own, handle = C.c_void_p(), (C.c_char * 64)()
+    _C.check(_C.lib.xrb_peer_alloc(a16(off_t16 + 2 * padded), C.byref(own), handle), 'peer_alloc')
+    try:
+        layout = _C.PeerLayout(1, 0, (C.c_void_p * 8)(own.value), off_g16, off_gmlp, off_t16, n_table, per, sum(n_mlp))
+        t16 = torch.as_tensor(_DevView(own.value + off_t16, padded, '<f2'), device='cuda')
+
+        def state(n):
+            p = torch.randn(n, device='cuda')
+            p[p == 0] = 1.0
+            return {'p': p, 'm': torch.zeros_like(p), 'v': torch.zeros_like(p), 'ema': p.clone(), 'p16': torch.empty(n, dtype=torch.float16, device='cuda')}
+        peer = [state(n) for n in (n_table,) + n_mlp]
+        local = [{k: v.clone() for k, v in s.items()} for s in peer]
+        groups = [_C.PeerMlpGroup(_C.ptr(s['p']), _C.ptr(s['p16']), _C.ptr(s['m']), _C.ptr(s['v']), _C.ptr(s['ema']), s['p'].numel(), off)
+                  for s, off in ((peer[1], 0), (peer[2], n_mlp[0]))]
+        g16 = torch.empty(n_table, dtype=torch.bfloat16, device='cuda')
+        for step in range(1, 5):
+            g_table = torch.randn(n_table, device='cuda') * 0.1 * step
+            g_mlp = torch.randn(sum(n_mlp), device='cuda') * 0.1 * step
+            mom = min(0.05, step / (100 + step - 1))
+            tp = peer[0]
+            _C.check(_C.lib.xrb_peer_publish_grads(C.byref(layout), _C.ptr(g_table), _C.ptr(g_mlp), step, _C.stream()), 'peer_publish_grads')
+            _C.check(_C.lib.xrb_peer_adam_step(C.byref(layout), _C.ptr(tp['p']), _C.ptr(tp['m']), _C.ptr(tp['v']), _C.ptr(tp['ema']), C.byref(groups[0]), C.byref(groups[1]),
+                                               lr, b1, b2, eps, wd, step, mom, step, _C.stream()), 'peer_adam_step')
+            _C.check(_C.lib.xrb_pack_bf16(_C.ptr(g_table), _C.ptr(g16), n_table, _C.stream()), 'pack_bf16')
+            tl = local[0]
+            _C.check(_C.lib.xrb_adam_ema_step_bf16grad(_C.ptr(tl['p']), _C.ptr(tl['p16']), _C.ptr(g16), _C.ptr(tl['m']), _C.ptr(tl['v']), n_table, lr, b1, b2, eps, wd, step, 1.0,
+                                                        _C.ptr(tl['ema']), mom, _C.stream()), 'adam bf16')
+            for s, g in zip(local[1:], (g_mlp[:n_mlp[0]], g_mlp[n_mlp[0]:])):
+                _C.check(_C.lib.xrb_adam_ema_step(_C.ptr(s['p']), _C.ptr(s['p16']), _C.ptr(g), _C.ptr(s['m']), _C.ptr(s['v']), s['p'].numel(), lr, b1, b2, eps, wd, step, 1.0,
+                                                  _C.ptr(s['ema']), mom, _C.stream()), 'adam')
+        torch.cuda.synchronize()
+        st = C.c_uint32(1)
+        _C.check(_C.lib.xrb_peer_status(own, C.byref(st), _C.stream()), 'peer_status')
+        assert st.value == 0
+        for name, a, b in zip(('table', 'density', 'color'), peer, local):
+            for k in ('p', 'm', 'v', 'ema'):
+                assert torch.equal(a[k].view(torch.int32), b[k].view(torch.int32)), (name, k)
+        assert torch.equal(t16[:n_table].view(torch.int16), local[0]['p'].half().view(torch.int16))
+        for a, b in zip(peer[1:], local[1:]):
+            assert torch.equal(a['p16'].view(torch.int16), b['p16'].view(torch.int16))
+    finally:
+        torch.cuda.synchronize()
+        _C.check(_C.lib.xrb_peer_free(own), 'peer_free')
 
 
 # ----------------------------------------------------------------------------------------------------------------------------- trained-ray count

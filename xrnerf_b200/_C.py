@@ -80,7 +80,6 @@ _SIGS = {
     'xrb_ngp_density_forward': (_i, [_cfg, _tab, P, P, P, _i, _i, P, _i, P]),
     'xrb_ngp_mlp_backward': (_i, [_cfg, _tab, P, P, P, _i, P, _i, P, _i, P, P, P, P]),
     'xrb_ngp_mlp_backward_tc': (_i, [_cfg, _tab, P, P, _i, P, _i, P, _i, P, P, P, P, P]),
-    'xrb_adam_step': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P]),
     'xrb_adam_ema_step': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P, _f, P]),
     'xrb_adam_ema_step_bf16grad': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P, _f, P]),
     'xrb_pack_bf16': (_i, [P, P, _i64, P]),
@@ -177,7 +176,8 @@ def rows(t):
 
 
 def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    # naming the current device skips torch's device discovery, which costs more host time than the lookup itself (a training step makes ~10 of these)
+    return C.c_void_p(torch.cuda.current_stream(torch.cuda.current_device()).cuda_stream)
 
 
 def float3(v):

@@ -1,4 +1,4 @@
-// xrnerf_b200 — backward of the Instant-NGP field (HashNerfMLP.run_mlp) and the fused Adam step.
+// xrnerf_b200 — backward of the Instant-NGP field (HashNerfMLP.run_mlp) and the training loss.
 //
 // One persistent kernel per training step replaces tcnn's backward (3 network/encoding backward launches + 2 `cat`
 // backward kernels in the reference stack, hashnerf_mlp.py:55-79) :
@@ -13,7 +13,6 @@
 // oracle_ngp_mlp_backward); the dY staging uses fp16 with a fixed 2^12 scale (tcnn uses fp16 + loss scale 128).
 // v1 runs the GEMM-shaped parts on CUDA cores; the tensor-core version is ngp_backward_tc.cu.
 #include "ngp_field.cuh"
-#include <cuda_bf16.h>
 
 namespace xrb {
 
@@ -220,28 +219,6 @@ static int launch_bwd(const HashGridDev &g, const void *table, const void *cells
     return check_launch("ngp_mlp_backward");
 }
 
-// ---------------------------------------------------------------------------- fused Adam (+ fp16 shadow refresh)
-template <typename G> __device__ __forceinline__ float grad_load(const G *g, int64_t i);
-template <> __device__ __forceinline__ float grad_load<float>(const float *g, int64_t i) { return g[i]; }
-template <> __device__ __forceinline__ float grad_load<__nv_bfloat16>(const __nv_bfloat16 *g, int64_t i) { return __bfloat162float(g[i]); }
-
-template <typename G>
-__global__ void __launch_bounds__(256) adam_kernel(float *__restrict__ p, __half *__restrict__ p16, const G *__restrict__ grad, float *__restrict__ m, float *__restrict__ v, int64_t n,
-                                                   float lr, float b1, float b2, float eps, float wd, float bc1, float bc2_sqrt_inv, float grad_mul, float *__restrict__ ema, float ema_m) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float w = p[i];
-        float gval = grad_load<G>(grad, i) * grad_mul + wd * w;       // torch.optim.Adam: weight_decay folded into the gradient
-        float mi = b1 * m[i] + (1.f - b1) * gval;
-        float vi = b2 * v[i] + (1.f - b2) * gval * gval;
-        m[i] = mi; v[i] = vi;
-        float denom = sqrtf(vi) * bc2_sqrt_inv + eps;                // sqrt(v)/sqrt(bias_correction2) + eps
-        w -= (lr / bc1) * (mi / denom);
-        p[i] = w;
-        if (p16) p16[i] = __float2half_rn(w);
-        if (ema) ema[i] = ema[i] * (1.f - ema_m) + ema_m * w;        // EMAHook.after_train_iter: buffer.mul_(1 - momentum).add_(momentum, param)
-    }
-}
-
 // ---------------------------------------------------------------------------- backward of the stand-alone tcnn-shaped modules (xrnerf_b200/tcnn.py autograd)
 // tcnn.Encoding(HashGrid).backward: dL/d enc fp16[n,32] -> fp32 table gradient (+=). thread = (sample, level) like hashgrid_forward_kernel.
 __global__ void __launch_bounds__(256) hashgrid_backward_kernel(HashGridDev g, const float *__restrict__ x, int x_stride, int n, const __half2 *__restrict__ d_enc, float scale,
@@ -298,19 +275,6 @@ static int launch_tcnn_mlp_bwd(const void *params, const void *x, const void *dy
     return check_launch("tcnn_mlp_backward");
 }
 
-// fp32 gradient -> bf16 (the wire format of the sharded data-parallel step: reduce-scatter in bf16, see xrnerf_b200/train.py)
-__global__ void __launch_bounds__(256) pack_bf16_kernel(const float *__restrict__ src, __nv_bfloat16 *__restrict__ dst, int64_t n) {
-    int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
-    for (; i + 3 < n; i += stride) {
-        float4 v = *reinterpret_cast<const float4 *>(src + i);
-        __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-        uint2 o; o.x = *reinterpret_cast<uint32_t *>(&a); o.y = *reinterpret_cast<uint32_t *>(&b);
-        *reinterpret_cast<uint2 *>(dst + i) = o;
-    }
-    if (blockIdx.x == 0 && threadIdx.x < 4) { int64_t t = (n & ~(int64_t)3) + threadIdx.x; if (t < n) dst[t] = __float2bfloat16_rn(src[t]); }
-}
-
 // 5 * HuberLoss(delta, 'sum') of HashNerfNetwork.train_step (networks/utils/metrics.py:8-16, hashnerf.py:39-44): gradient wrt rgb and the loss value in ONE pass
 __global__ void __launch_bounds__(256) huber5_kernel(const float *__restrict__ rgb, const float *__restrict__ target, int64_t n, float delta, float *__restrict__ grad, float *__restrict__ loss_accum) {
     float local = 0.f;
@@ -340,16 +304,6 @@ int xrb_ngp_huber5_grad(const float *rgb, const float *target, int64_t n_element
     const int blocks = stride_grid((n_elements + 255) / 256, 8);
     huber5_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(rgb, target, n_elements, delta, grad_out, loss_accum);
     return check_launch("huber5_grad");
-}
-
-int xrb_pack_bf16(const float *src, void *dst_bf16, int64_t n, void *stream) {
-    XRB_REQUIRE(n >= 0, "pack_bf16: negative size");
-    if (n == 0) return XRB_OK;
-    XRB_REQUIRE(src && dst_bf16, "pack_bf16: null pointer");
-    XRB_REQUIRE(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst_bf16 & 7) == 0, "pack_bf16: misaligned");
-    const int blocks = stride_grid((n / 4 + 255) / 256, 16);
-    pack_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16 *)dst_bf16, n);
-    return check_launch("pack_bf16");
 }
 
 int xrb_tcnn_hashgrid_backward(const xrb_ngp_config *cfg, const float *x, int x_stride, int n, const void *d_enc_fp16, float grad_scale, float *d_table, void *stream) {
@@ -393,37 +347,6 @@ int xrb_ngp_mlp_backward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
 #undef XRB_BW
     set_error("ngp_mlp_backward: (density_hidden, color_hidden) must be one of (1,1) (1,2) (2,2) (1,3) (2,3)");
     return XRB_E_UNSUPPORTED;
-}
-
-int xrb_adam_step(float *param, void *param_fp16, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                  int step, float grad_div, void *stream) {
-    return xrb_adam_ema_step(param, param_fp16, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_div, nullptr, 0.f, stream);
-}
-
-static int adam_launch(float *param, void *param_fp16, const void *grad, bool grad_bf16, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps,
-                       float weight_decay, int step, float grad_div, float *ema, float ema_momentum, void *stream) {
-    XRB_REQUIRE(n >= 0 && step >= 1 && grad_div != 0.f && ema_momentum >= 0.f && ema_momentum <= 1.f, "adam_step: bad arguments");
-    if (n == 0) return XRB_OK;
-    XRB_REQUIRE(param && grad && exp_avg && exp_avg_sq, "adam_step: null pointer");
-    double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
-    const int blocks = stride_grid((n + 255) / 256, 16);
-    if (grad_bf16)
-        adam_kernel<__nv_bfloat16><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const __nv_bfloat16 *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay,
-                                                                                 (float)bc1, (float)(1.0 / sqrt(bc2)), 1.f / grad_div, ema, ema_momentum);
-    else
-        adam_kernel<float><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const float *)grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, (float)bc1,
-                                                                         (float)(1.0 / sqrt(bc2)), 1.f / grad_div, ema, ema_momentum);
-    return check_launch("adam_step");
-}
-
-int xrb_adam_ema_step(float *param, void *param_fp16, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                      int step, float grad_div, float *ema, float ema_momentum, void *stream) {
-    return adam_launch(param, param_fp16, grad, false, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_div, ema, ema_momentum, stream);
-}
-
-int xrb_adam_ema_step_bf16grad(float *param, void *param_fp16, const void *grad_bf16, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps,
-                               float weight_decay, int step, float grad_div, float *ema, float ema_momentum, void *stream) {
-    return adam_launch(param, param_fp16, grad_bf16, true, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_div, ema, ema_momentum, stream);
 }
 
 }  // extern "C"

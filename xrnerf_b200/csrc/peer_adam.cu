@@ -1,5 +1,7 @@
-// xrnerf_b200 — data-parallel optimiser step of the Instant-NGP trainer as ONE exchange over NVLink peer memory.
+// xrnerf_b200 — the optimiser step of the Instant-NGP trainer in every gradient-exchange mode. One Adam + EMA element update (adam_update) and one host
+// computation of its hyper-parameters (adam_hyper) serve both the local step (xrb_adam_ema_step*: one rank, or after a collective) and the peer step below.
 //
+// The peer step: the data-parallel optimiser step as ONE exchange over NVLink peer memory.
 // The reference trains under MMDistributedDataParallel: torch DDP all-reduces the dense fp32 gradient (49 MB for the hash table) and every rank runs the same
 // torch.optim.Adam over all 12.2 M parameters (core/apis/train.py:28-36, hashnerf.py:32-52). Round 2's first answer was reduce-scatter (bf16) -> Adam on this
 // rank's 1/N -> all-gather (fp16) through NCCL: three collectives + five kernels per step, ~113 us of which ~90 are launch / rendezvous latency of the collectives.
@@ -22,6 +24,54 @@
 
 namespace xrb {
 
+// ---------------------------------------------------------------------------- the Adam + EMA element update
+struct AdamHyper { float lr, b1, b2, eps, wd, bc1, bc2_sqrt_inv, grad_mul, ema_m; };
+
+static AdamHyper adam_hyper(float lr, float beta1, float beta2, float eps, float weight_decay, int step, float grad_div, float ema_momentum) {
+    const double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
+    return AdamHyper{lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)(1.0 / sqrt(bc2)), 1.f / grad_div, ema_momentum};
+}
+
+// torch.optim.Adam on element i (weight_decay folded into the gradient), then mmcv's EMAHook.after_train_iter on it: ema[i] = (1 - m) ema[i] + m w
+// (ema == NULL: no EMA). m, v: the element's moments, updated in place. Returns the new weight.
+__device__ __forceinline__ float adam_update(float w, float g, float &m, float &v, float *ema, int64_t i, const AdamHyper &h) {
+    const float gval = g * h.grad_mul + h.wd * w;
+    m = h.b1 * m + (1.f - h.b1) * gval;
+    v = h.b2 * v + (1.f - h.b2) * gval * gval;
+    w -= (h.lr / h.bc1) * (m / (sqrtf(v) * h.bc2_sqrt_inv + h.eps));   // sqrt(v)/sqrt(bias_correction2) + eps
+    if (ema) ema[i] = ema[i] * (1.f - h.ema_m) + h.ema_m * w;
+    return w;
+}
+
+// ---------------------------------------------------------------------------- local step: Adam (+ fp16 shadow refresh) over one vector
+template <typename G> __device__ __forceinline__ float grad_load(const G *g, int64_t i);
+template <> __device__ __forceinline__ float grad_load<float>(const float *g, int64_t i) { return g[i]; }
+template <> __device__ __forceinline__ float grad_load<__nv_bfloat16>(const __nv_bfloat16 *g, int64_t i) { return __bfloat162float(g[i]); }
+
+template <typename G>
+__global__ void __launch_bounds__(256) adam_kernel(float *__restrict__ p, __half *__restrict__ p16, const G *__restrict__ grad, float *__restrict__ m, float *__restrict__ v,
+                                                   float *__restrict__ ema, int64_t n, AdamHyper h) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float w = adam_update(p[i], grad_load<G>(grad, i), m[i], v[i], ema, i, h);
+        p[i] = w;
+        if (p16) p16[i] = __float2half_rn(w);
+    }
+}
+
+// fp32 gradient -> bf16 (the wire format of the sharded data-parallel step: reduce-scatter in bf16, see xrnerf_b200/train.py)
+__global__ void __launch_bounds__(256) pack_bf16_kernel(const float *__restrict__ src, __nv_bfloat16 *__restrict__ dst, int64_t n) {
+    int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
+    for (; i + 3 < n; i += stride) {
+        float4 v = *reinterpret_cast<const float4 *>(src + i);
+        __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+        uint2 o; o.x = *reinterpret_cast<uint32_t *>(&a); o.y = *reinterpret_cast<uint32_t *>(&b);
+        *reinterpret_cast<uint2 *>(dst + i) = o;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < 4) { int64_t t = (n & ~(int64_t)3) + threadIdx.x; if (t < n) dst[t] = __float2bfloat16_rn(src[t]); }
+}
+
+// ---------------------------------------------------------------------------- peer step
 constexpr int PEER_MAX = 8;
 constexpr long long PEER_SPIN_LIMIT = 20000000000ll;   // cycles (~10 s)
 // flags (uint32) at the start of a block: ready[8], done[8], ticket[2], status
@@ -86,15 +136,7 @@ __global__ void __launch_bounds__(256) peer_publish_kernel(PeerDev P, const floa
     peer_signal_when_all_ctas_done(P, F_READY, step, 0);
 }
 
-struct AdamHyper { float lr, b1, b2, eps, wd, bc1, bc2_sqrt_inv, grad_mul, ema_m; };
 struct MlpGroup { float *p; __half *p16; float *m, *v, *ema; int64_t n, g_off; };
-
-__device__ __forceinline__ float adam_one(float w, float g, float &m, float &v, const AdamHyper &h) {
-    const float gval = g * h.grad_mul + h.wd * w;
-    m = h.b1 * m + (1.f - h.b1) * gval;
-    v = h.b2 * v + (1.f - h.b2) * gval * gval;
-    return w - (h.lr / h.bc1) * (m / (sqrtf(v) * h.bc2_sqrt_inv + h.eps));
-}
 
 __global__ void __launch_bounds__(256) peer_adam_kernel(PeerDev P, float *__restrict__ master /*my slice*/, float *__restrict__ m, float *__restrict__ v, float *__restrict__ ema, int64_t cnt /*live elements of my slice*/,
                                                         AdamHyper h, MlpGroup g0, MlpGroup g1, uint32_t step) {
@@ -117,23 +159,19 @@ __global__ void __launch_bounds__(256) peer_adam_kernel(PeerDev P, float *__rest
             float4 m0 = *reinterpret_cast<float4 *>(m + i), m1 = *reinterpret_cast<float4 *>(m + i + 4), v0 = *reinterpret_cast<float4 *>(v + i), v1 = *reinterpret_cast<float4 *>(v + i + 4);
             float *wp = &w0.x, *wq = &w1.x, *mp = &m0.x, *mq = &m1.x, *vp = &v0.x, *vq = &v1.x;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) { wp[k] = adam_one(wp[k], g[k], mp[k], vp[k], h); wq[k] = adam_one(wq[k], g[4 + k], mq[k], vq[k], h); }
+            for (int k = 0; k < 4; ++k) wp[k] = adam_update(wp[k], g[k], mp[k], vp[k], ema, i + k, h);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wq[k] = adam_update(wq[k], g[4 + k], mq[k], vq[k], ema, i + 4 + k, h);
             *reinterpret_cast<float4 *>(master + i) = w0; *reinterpret_cast<float4 *>(master + i + 4) = w1;
             *reinterpret_cast<float4 *>(m + i) = m0; *reinterpret_cast<float4 *>(m + i + 4) = m1; *reinterpret_cast<float4 *>(v + i) = v0; *reinterpret_cast<float4 *>(v + i + 4) = v1;
 #pragma unroll
             for (int k = 0; k < 4; ++k) { out[k] = __float2half_rn(wp[k]); out[4 + k] = __float2half_rn(wq[k]); }
-            if (ema) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) { ema[i + k] = ema[i + k] * (1.f - h.ema_m) + h.ema_m * wp[k]; ema[i + 4 + k] = ema[i + 4 + k] * (1.f - h.ema_m) + h.ema_m * wq[k]; }
-            }
         } else {
             for (int k = 0; k < 8; ++k) {
                 float w = 0.f;
                 if (i + k < cnt) {
-                    float mm = m[i + k], vv = v[i + k];
-                    w = adam_one(master[i + k], g[k], mm, vv, h);
-                    master[i + k] = w; m[i + k] = mm; v[i + k] = vv;
-                    if (ema) ema[i + k] = ema[i + k] * (1.f - h.ema_m) + h.ema_m * w;
+                    w = adam_update(master[i + k], g[k], m[i + k], v[i + k], ema, i + k, h);
+                    master[i + k] = w;
                 }
                 out[k] = __float2half_rn(w);
             }
@@ -147,11 +185,9 @@ __global__ void __launch_bounds__(256) peer_adam_kernel(PeerDev P, float *__rest
         for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < G.n; i += (int64_t)gridDim.x * blockDim.x) {
             float g = 0.f;
             for (int p = 0; p < P.world; ++p) g += __ldcv(reinterpret_cast<const float *>(P.base[p] + P.off_gmlp) + G.g_off + i);
-            float mm = G.m[i], vv = G.v[i];
-            const float w = adam_one(G.p[i], g, mm, vv, h);
-            G.p[i] = w; G.m[i] = mm; G.v[i] = vv;
+            const float w = adam_update(G.p[i], g, G.m[i], G.v[i], G.ema, i, h);
+            G.p[i] = w;
             if (G.p16) G.p16[i] = __float2half_rn(w);
-            if (G.ema) G.ema[i] = G.ema[i] * (1.f - h.ema_m) + h.ema_m * w;
         }
     }
     peer_signal_when_all_ctas_done(P, F_DONE, step, 1);
@@ -173,6 +209,40 @@ static int peer_dev(const xrb_peer_layout *L, PeerDev *P) {
 using namespace xrb;
 
 extern "C" {
+
+static int adam_launch(float *param, void *param_fp16, const void *grad, bool grad_bf16, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps,
+                       float weight_decay, int step, float grad_div, float *ema, float ema_momentum, void *stream) {
+    XRB_REQUIRE(n >= 0 && step >= 1 && grad_div != 0.f && ema_momentum >= 0.f && ema_momentum <= 1.f, "adam_step: bad arguments");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(param && grad && exp_avg && exp_avg_sq, "adam_step: null pointer");
+    const AdamHyper h = adam_hyper(lr, beta1, beta2, eps, weight_decay, step, grad_div, ema_momentum);
+    const int blocks = stride_grid((n + 255) / 256, 16);
+    if (grad_bf16)
+        adam_kernel<__nv_bfloat16><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const __nv_bfloat16 *)grad, exp_avg, exp_avg_sq, ema, n, h);
+    else
+        adam_kernel<float><<<blocks, 256, 0, (cudaStream_t)stream>>>(param, (__half *)param_fp16, (const float *)grad, exp_avg, exp_avg_sq, ema, n, h);
+    return check_launch("adam_step");
+}
+
+int xrb_adam_ema_step(float *param, void *param_fp16, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                      int step, float grad_div, float *ema, float ema_momentum, void *stream) {
+    return adam_launch(param, param_fp16, grad, false, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_div, ema, ema_momentum, stream);
+}
+
+int xrb_adam_ema_step_bf16grad(float *param, void *param_fp16, const void *grad_bf16, float *exp_avg, float *exp_avg_sq, int64_t n, float lr, float beta1, float beta2, float eps,
+                               float weight_decay, int step, float grad_div, float *ema, float ema_momentum, void *stream) {
+    return adam_launch(param, param_fp16, grad_bf16, true, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_div, ema, ema_momentum, stream);
+}
+
+int xrb_pack_bf16(const float *src, void *dst_bf16, int64_t n, void *stream) {
+    XRB_REQUIRE(n >= 0, "pack_bf16: negative size");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(src && dst_bf16, "pack_bf16: null pointer");
+    XRB_REQUIRE(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst_bf16 & 7) == 0, "pack_bf16: misaligned");
+    const int blocks = stride_grid((n / 4 + 255) / 256, 16);
+    pack_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, (__nv_bfloat16 *)dst_bf16, n);
+    return check_launch("pack_bf16");
+}
 
 int xrb_peer_alloc(size_t bytes, void **ptr, void *ipc_handle64) {
     XRB_REQUIRE(ptr && ipc_handle64 && bytes >= 128, "peer_alloc: null pointer / block smaller than its flags");
@@ -216,8 +286,7 @@ int xrb_peer_adam_step(const xrb_peer_layout *L, float *master_slice, float *exp
     XRB_REQUIRE((((uintptr_t)master_slice | (uintptr_t)exp_avg_slice | (uintptr_t)exp_avg_sq_slice) & 15) == 0, "peer_adam_step: slices must be 16-byte aligned");
     XRB_REQUIRE(!(ema_slice && !(ema_momentum > 0.f && ema_momentum < 1.f)), "peer_adam_step: EMA momentum must be in (0,1)");
     XRB_REQUIRE(mlp0->g_off >= 0 && mlp1->g_off >= 0 && mlp0->g_off + mlp0->n <= P.n_mlp && mlp1->g_off + mlp1->n <= P.n_mlp, "peer_adam_step: MLP group outside the gradient block");
-    const double bc1 = 1.0 - pow((double)beta1, opt_step), bc2 = 1.0 - pow((double)beta2, opt_step);
-    AdamHyper h{lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)(1.0 / sqrt(bc2)), 1.f / (float)P.world, ema_momentum};
+    const AdamHyper h = adam_hyper(lr, beta1, beta2, eps, weight_decay, opt_step, (float)P.world, ema_momentum);
     MlpGroup g0{mlp0->param, (__half *)mlp0->param_fp16, mlp0->exp_avg, mlp0->exp_avg_sq, mlp0->ema, mlp0->n, mlp0->g_off};
     MlpGroup g1{mlp1->param, (__half *)mlp1->param_fp16, mlp1->exp_avg, mlp1->exp_avg_sq, mlp1->ema, mlp1->n, mlp1->g_off};
     const int blocks = stride_grid(((cnt + 7) / 8 + 255) / 256, 8);

@@ -450,7 +450,7 @@ extern "C" {
 // 2: xrb_ngp_table (cell image), explicit profile events in xrb_ngp_render
 // 3: xrb_nerf_mlp_forward takes the fp16 encoding tile image where it took fp32 `embedded` rows, and the K-half weight packing; the other NerfMLP
 //    entry points are gone. The symbol name is unchanged but its arguments mean something else, so an old caller must not load this library silently.
-int xrb_abi_version(void) { return 4; }
+int xrb_abi_version(void) { return 5; }
 int xrb_built_for_sm(void) { return 90; }
 const char *xrb_last_error(void) { return g_err; }
 

@@ -61,7 +61,29 @@ class NgpField(nn.Module):
         self._image = torch.empty(_C.lib.xrb_ngp_weight_image_bytes(self.cfg), dtype=torch.uint8, device=dev)
         nb = _C.lib.xrb_ngp_cell_image_bytes(self.cfg, self.n_packed) if self.n_packed > 0 else 0
         self._cells = torch.empty(nb, dtype=torch.uint8, device=dev) if nb else None
-        self.tab = _C.NgpTable(self._table16.data_ptr(), self._cells.data_ptr() if nb else None, self.n_packed if nb else 0)
+        self._bind_table()
+
+    def _bind_table(self):
+        """self.tab <- the xrb_ngp_table of the current fp16 table and cell image"""
+        cells = self._cells is not None
+        self.tab = _C.NgpTable(self._table16.data_ptr(), self._cells.data_ptr() if cells else None, self.n_packed if cells else 0)
+
+    def use_table(self, table16=None):
+        """Read the fp16 hash table from `table16`, a caller-owned fp16 tensor of hash_params.numel() elements (e.g. the working table inside a
+        peer-exchange block, which other processes write), after copying the current table into it. None: from a private copy of the current table again."""
+        if table16 is None:
+            table16 = self._table16.clone()
+        elif table16.data_ptr() == self._table16.data_ptr():
+            return
+        else:
+            table16.copy_(self._table16)
+        self._table16 = table16
+        self._bind_table()
+
+    def params_and_shadows(self):
+        """(fp32 master, fp16 working copy) of the hash table, the density net and the colour net: what an optimiser updates in place before calling
+        shadows_updated()"""
+        return [(self.hash_params, self._table16), (self.density_params, self._dens16), (self.color_params, self._color16)]
 
     def set_packed_levels(self, n):
         """change how many levels the cell image holds (re-allocates and rebuilds it on the next refresh)"""
@@ -75,9 +97,11 @@ class NgpField(nn.Module):
         if self._cells is not None:
             _C.check(_C.lib.xrb_ngp_build_cell_image(self.cfg, _C.ptr(self._table16), self.n_packed, _C.ptr(self._cells), _C.stream()), 'build cell image')
 
+    def _version_key(self):
+        return (self.hash_params._version, self.density_params._version, self.color_params._version, self.hash_params.device)
+
     def refresh(self, force=False):
-        ver = (self.hash_params._version, self.density_params._version, self.color_params._version, self.hash_params.device)
-        if not force and ver == self._ver:
+        if not force and self._version_key() == self._ver:
             return
         dev = self.hash_params.device
         if self._table16 is None or self._table16.device != dev:
@@ -86,21 +110,30 @@ class NgpField(nn.Module):
         _C.check(_C.lib.xrb_tcnn_cast_params(_C.ptr(self.hash_params.detach()), _C.ptr(self._table16), self.hash_params.numel(), s), 'cast hash')
         _C.check(_C.lib.xrb_tcnn_cast_params(_C.ptr(self.density_params.detach()), _C.ptr(self._dens16), self.density_params.numel(), s), 'cast density')
         _C.check(_C.lib.xrb_tcnn_cast_params(_C.ptr(self.color_params.detach()), _C.ptr(self._color16), self.color_params.numel(), s), 'cast color')
-        _C.check(_C.lib.xrb_ngp_pack_weights(self.cfg, _C.ptr(self.density_params.detach()), _C.ptr(self.color_params.detach()), _C.ptr(self._image), s), 'pack')
+        self.shadows_updated()
+
+    def shadows_updated(self):
+        """The fp16 working copies hold the current parameters (an optimiser updated masters and copies in place, params_and_shadows()): re-pack the
+        weight image, rebuild the cell image and record the parameters' versions as current, so that refresh() does not cast the masters again (a
+        data-parallel trainer keeps only its own slice of the fp32 hash table up to date)."""
+        _C.check(_C.lib.xrb_ngp_pack_weights(self.cfg, _C.ptr(self.density_params.detach()), _C.ptr(self.color_params.detach()), _C.ptr(self._image), _C.stream()), 'pack')
         self.rebuild_cells()
-        self._ver = ver
+        self._ver = self._version_key()
 
     def run_mlp(self, pts, dirs, impl=None):
         """pts, dirs: [S,3] float32 views (row stride in floats may be > 3, e.g. coords[:, :3] / coords[:, 4:]). -> raw [S,4] f32."""
         _C.require_cuda(pts, dirs)
         self.refresh()
+        return self.mlp_rows(pts, dirs, torch.empty((pts.shape[0], 4), dtype=torch.float32, device=pts.device), impl=impl)
+
+    def mlp_rows(self, pts, dirs, out, n_rows_dev=None, impl=None):
+        """run_mlp into `out` [S,4] from the working copies as they are, without refresh(): a training step between optimiser updates, where the fp32
+        masters may be stale, calls this. n_rows_dev (int32 device tensor, optional): only the first min(S, n_rows_dev[0]) rows are evaluated."""
         (pp, ps), (dp, ds) = _C.rows(pts), _C.rows(dirs)
-        n = pts.shape[0]
-        raw = torch.empty((n, 4), dtype=torch.float32, device=pts.device)
         impl = self.impl if impl is None else impl
-        _C.check(_C.lib.xrb_ngp_mlp_forward(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._color16), _C.ptr(self._image), pp, ps, dp, ds, n, None, _C.ptr(raw), impl, _C.stream()),
-                 'ngp_mlp_forward')
-        return raw
+        _C.check(_C.lib.xrb_ngp_mlp_forward(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._color16), _C.ptr(self._image), pp, ps, dp, ds, pts.shape[0], _C.i32(n_rows_dev),
+                                            _C.f32(out), impl, _C.stream()), 'ngp_mlp_forward')
+        return out
 
     def forward(self, pts, dirs):
         """differentiable (w.r.t. the parameters) HashNerfMLP.run_mlp"""
@@ -118,13 +151,20 @@ class NgpField(nn.Module):
         self.refresh()
         if out is None:
             out = (torch.zeros_like(self.hash_params), torch.zeros_like(self.density_params), torch.zeros_like(self.color_params))
+        return self.backward_rows(pts, dirs, grad_raw, out, impl=impl)
+
+    def backward_rows(self, pts, dirs, grad_raw, out, n_rows_dev=None, impl=None):
+        """backward_params into `out` from the working copies as they are, without refresh() (see mlp_rows). n_rows_dev as in mlp_rows; the CUDA-core
+        kernel (impl 0) takes its row count from the host, so with n_rows_dev it waits for the device once."""
         n = pts.shape[0]
         (pp, ps), (dp, ds) = _C.rows(pts), _C.rows(dirs)
         impl = (self.impl if self.tc_backward_ok() else 0) if impl is None else impl
         if impl == 1:
-            _C.check(_C.lib.xrb_ngp_mlp_backward_tc(self.cfg, self.tab, _C.ptr(self._image), pp, ps, dp, ds, _C.f32(grad_raw), n, None, _C.f32(out[0]), _C.f32(out[1]), _C.f32(out[2]),
-                                                    _C.stream()), 'ngp_mlp_backward_tc')
+            _C.check(_C.lib.xrb_ngp_mlp_backward_tc(self.cfg, self.tab, _C.ptr(self._image), pp, ps, dp, ds, _C.f32(grad_raw), n, _C.i32(n_rows_dev), _C.f32(out[0]), _C.f32(out[1]),
+                                                    _C.f32(out[2]), _C.stream()), 'ngp_mlp_backward_tc')
             return out
+        if n_rows_dev is not None:
+            n = min(n, int(n_rows_dev[0].item()))
         _C.check(_C.lib.xrb_ngp_mlp_backward(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._color16), pp, ps, dp, ds, _C.f32(grad_raw), n, _C.f32(out[0]), _C.f32(out[1]),
                                              _C.f32(out[2]), _C.stream()), 'ngp_mlp_backward')
         return out

@@ -29,29 +29,6 @@ import torch
 from . import _C
 
 
-class FlatGradBuffer:
-    """One contiguous fp32 buffer viewed as the per-parameter gradients (host logic; works on CPU tensors for the gloo test)."""
-
-    def __init__(self, params):
-        self.sizes = [int(p.numel()) for p in params]
-        self.flat = torch.zeros(sum(self.sizes), dtype=torch.float32, device=params[0].device)
-        self.views, o = [], 0
-        for n in self.sizes:
-            self.views.append(self.flat[o:o + n])
-            o += n
-
-    def zero_(self):
-        self.flat.zero_()
-
-    def allreduce(self, group=None):
-        """SUM over ranks (the division by world size happens in the optimiser kernel). Returns the divisor to apply."""
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
-            dist.all_reduce(self.flat, op=dist.ReduceOp.SUM, group=group)
-            return float(dist.get_world_size(group))
-        return 1.0
-
-
 def shard_range(n, world, rank, align=8):
     """[begin, end) of rank's slice of an n-element vector cut into `world` equal slices of ceil(n / world) rounded up to `align` elements
     (the last slices may be short or empty); `padded` = world * slice length is the size collectives operate on."""
@@ -265,7 +242,7 @@ class NgpTrainer:
         self.g_color = self.g_mlp[field.density_params.numel():]
         self.grads = [self.g_hash, self.g_dens, self.g_color]
         if self.px is not None:
-            self._alias_table()
+            field.use_table(self.px.t16[:self.px.n_table])     # the field's working table lives inside this rank's exchange block (the other ranks write their slices into it)
         if self.ex:
             if self.px is None:
                 self.g16 = torch.zeros(pad, dtype=torch.bfloat16, device=dev)                 # wire format of the hash gradient
@@ -340,9 +317,8 @@ class NgpTrainer:
         main = torch.cuda.current_stream()
         main.wait_event(s.ready)
         st = _C.stream()
-        n_rows_dev = _C.ptr(s.cnt_c[1:2])
-        pp, dp = _C.rows(s.coords_c[:, :3])[0], _C.rows(s.coords_c[:, 4:])[0]
-        _C.check(_C.lib.xrb_ngp_mlp_forward(f.cfg, f.tab, _C.ptr(f._dens16), _C.ptr(f._color16), _C.ptr(f._image), pp, 7, dp, 7, self.T, n_rows_dev, _C.ptr(self.raw), self.fwd_impl, st), 'field fwd')
+        pts, dirs, n_rows_dev = s.coords_c[:, :3], s.coords_c[:, 4:], s.cnt_c[1:2]
+        f.mlp_rows(pts, dirs, self.raw, n_rows_dev, self.fwd_impl)       # never refresh() here: the fp32 master outside this rank's slice is stale
         _C.check(_C.lib.xrb_rm_calc_rgb_forward(_C.ptr(self.raw), _C.ptr(s.coords_c), _C.ptr(s.numsteps), _C.ptr(s.numsteps_c), _C.f32(bg), self.n_rays, self.rgb_act, self.dens_act,
                                                 _C.ptr(self.rgb), st), 'calc_rgb_forward')
         self.loss_accum.zero_()
@@ -351,21 +327,13 @@ class NgpTrainer:
         _C.check(_C.lib.xrb_rm_calc_rgb_backward(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean), self.n_rays,
                                                  self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward')
         self.gflat.zero_()
-        if self.bwd_impl == 1:
-            _C.check(_C.lib.xrb_ngp_mlp_backward_tc(f.cfg, f.tab, _C.ptr(f._image), pp, 7, dp, 7, _C.ptr(self.draw), self.T, n_rows_dev, _C.ptr(self.g_hash), _C.ptr(self.g_dens),
-                                                    _C.ptr(self.g_color), st), 'field bwd (wgmma)')
-        else:
-            n_rows = int(s.cnt_c[1].item())           # the CUDA-core kernel has no device-side count: one sync (comparator path only)
-            _C.check(_C.lib.xrb_ngp_mlp_backward(f.cfg, f.tab, _C.ptr(f._dens16), _C.ptr(f._color16), pp, 7, dp, 7, _C.ptr(self.draw), n_rows, _C.ptr(self.g_hash), _C.ptr(self.g_dens),
-                                                 _C.ptr(self.g_color), st), 'field bwd')
+        f.backward_rows(pts, dirs, self.draw, self.grads, n_rows_dev, self.bwd_impl)
         s.free = torch.cuda.Event(); s.free.record(main)
         self.step_n += 1
         it = self.step_n - 1                                                            # runner.iter inside after_train_iter
         mom = 0.0 if self.ema_momentum is None else min(self.ema_momentum, (1 + it) / (self.ema_warm_up + it))
         self._exchange_and_update(mom)
-        _C.check(_C.lib.xrb_ngp_pack_weights(f.cfg, _C.ptr(f.density_params.data), _C.ptr(f.color_params.data), _C.ptr(f._image), _C.stream()), 'pack')
-        f.rebuild_cells()                                                               # the fp16 table changed: refresh its cell image
-        f._ver = (f.hash_params._version, f.density_params._version, f.color_params._version, f.hash_params.device)  # shadows are current
+        f.shadows_updated()
         self.cur ^= 1
         return self.loss_accum[0]
 
@@ -383,39 +351,26 @@ class NgpTrainer:
         if self.world > 1:
             import torch.distributed as dist
             dist.barrier(group=self.group)
-        f = self.f
-        if f._table16 is not None and f._table16.data_ptr() == self.px.own + self.px.off_t16:
-            f._table16 = f._table16.clone()
-            f.tab = _C.NgpTable(f._table16.data_ptr(), f._cells.data_ptr() if f._cells is not None else None, f.n_packed if f._cells is not None else 0)
+        self.f.use_table(None)
         self.px.close()
         self.px = None
         self.grad_comm = 'closed'
 
-    def _alias_table(self):
-        """peer mode: the field's fp16 working table lives inside this rank's exchange block (the other ranks write their slices into it)"""
-        f, px = self.f, self.px
-        want = px.own + px.off_t16
-        if f._table16 is None or f._table16.data_ptr() != want:
-            if f._table16 is not None:
-                px.t16[:px.n_table].copy_(f._table16)
-            f._table16 = px.t16[:px.n_table]
-            f.tab = _C.NgpTable(want, f._cells.data_ptr() if f._cells is not None else None, f.n_packed if f._cells is not None else 0)
-
     def _exchange_and_update(self, mom):
         import torch.distributed as dist
         f = self.f
+        pairs = f.params_and_shadows()           # the MLPs' copies; the table's is the exchange block's in peer mode
         if self.grad_comm == 'peer':
             px, ex, C = self.px, self.ex, _C.C
-            self._alias_table()
+            f.use_table(px.t16[:px.n_table])
             if px.step == 0:                 # first exchange: line the ranks up on the host once (lazy module loading / allocator warm-up differ by rank; the kernels give up after ~10 s)
                 torch.cuda.synchronize()
                 dist.barrier(group=self.group)
             px.step += 1
             st = _C.stream()
             _C.check(_C.lib.xrb_peer_publish_grads(C.byref(px.layout), _C.ptr(self.g_hash), _C.ptr(self.g_mlp), px.step, st), 'peer_publish_grads')
-            nd = f.density_params.numel()
-            groups = [_C.PeerMlpGroup(_C.ptr(p.data), _C.ptr(p16), _C.ptr(m), _C.ptr(v), _C.ptr(e) if e is not None else None, p.numel(), off)
-                      for p, p16, m, v, e, off in ((f.density_params, f._dens16, self.m[1], self.v[1], self.ema[1], 0), (f.color_params, f._color16, self.m[2], self.v[2], self.ema[2], nd))]
+            groups = [_C.PeerMlpGroup(_C.ptr(p.data), _C.ptr(p16), _C.ptr(m), _C.ptr(v), _C.ptr(e), p.numel(), off)
+                      for (p, p16), m, v, e, off in zip(pairs[1:], self.m[1:], self.v[1:], self.ema[1:], (0, f.density_params.numel()))]
             b, e_ = ex.begin, ex.end
             sl = f.hash_params.data[b:e_]
             _C.check(_C.lib.xrb_peer_adam_step(C.byref(px.layout), _C.ptr(sl) if e_ > b else None, _C.ptr(self.m[0]) if e_ > b else None, _C.ptr(self.v[0]) if e_ > b else None,
@@ -432,17 +387,16 @@ class NgpTrainer:
             if e > b:
                 self._adam(f.hash_params.data[b:e], self.t16_pad[b:e], self.g16_mine[:e - b], self.m[0], self.v[0], self.ema[0], mom, float(self.world), bf16=True)
             ex.all_gather(self.t16_pad, self.t16_pad[self.rank * ex.per:(self.rank + 1) * ex.per])
-            f._table16.copy_(self.t16_pad[:ex.n])
+            pairs[0][1].copy_(self.t16_pad[:ex.n])
             self.master_stale = True
-            self._adam(f.density_params.data, f._dens16, self.g_dens, self.m[1], self.v[1], self.ema[1], mom, float(self.world))
-            self._adam(f.color_params.data, f._color16, self.g_color, self.m[2], self.v[2], self.ema[2], mom, float(self.world))
+            for (p, p16), g_, m, v, e in zip(pairs[1:], self.grads[1:], self.m[1:], self.v[1:], self.ema[1:]):
+                self._adam(p.data, p16, g_, m, v, e, mom, float(self.world))
             return
         div = 1.0
         if self.grad_comm == 'allreduce':
             dist.all_reduce(self.gflat, op=dist.ReduceOp.SUM, group=self.group)
             div = float(self.world)
-        shadows = [f._table16, f._dens16, f._color16]
-        for p, p16, g_, m, v, e in zip(self.params, shadows, self.grads, self.m, self.v, self.ema):
+        for (p, p16), g_, m, v, e in zip(pairs, self.grads, self.m, self.v, self.ema):
             self._adam(p.data, p16, g_, m, v, e, mom, div)
 
     # ------------------------------------------------------------------ bookkeeping
