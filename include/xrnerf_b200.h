@@ -403,6 +403,40 @@ int xrb_nerf_tg_pack_weights(const float *W, int N, int K_in, int n_pad, int n_k
 int xrb_nerf_tg_pack_draw(const float *d_raw, int64_t n_rows, void *z_rgb_image, void *z_alpha_image, float *scale, void *stream);
 float xrb_nerf_tg_grad_scale(void);
 
+/* ---- NGP mesh export (csrc/mesh.cu; no reference counterpart): the field's density on a lattice, then a triangle mesh of one of its level sets.
+ *
+ * Lattice of nx x ny x nz points (each size 2..1024) spanning the box [box_min, box_max] (host float[3] each), volumes f32[nz][ny][nx] (x fastest).
+ * Point (i, j, k) sits at (X(i), Y(j), Z(k)), per axis with n points from lo to hi:
+ *   X(i) = min(lo + i * ((hi - lo) / (n - 1)), hi)      (fp32, each operation rounded once, in this order; the min keeps the last point in the box)
+ * A lattice with a size of 0 is empty: every call on it is a no-op that touches no pointer.
+ *
+ * xrb_ngp_density_lattice: out[k][j][i] <- the raw (pre-activation) density the field returns at lattice point (i, j, k), the very value
+ * xrb_ngp_density_forward gives for that position with the same impl. The box must lie in the field's warped domain, 0 <= box_min < box_max <= 1
+ * (outside it the dense levels would be addressed past their end); it is checked, with the sizes, before any CUDA call. The positions are
+ * staged through `workspace` (xrb_ngp_density_lattice_workspace() bytes, 16-byte aligned, independent of the lattice size) in chunks of
+ * consecutive points, each evaluated by the density-only field kernel into its slice of `out`. */
+size_t xrb_ngp_density_lattice_workspace(void);
+int xrb_ngp_density_lattice(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const void *weight_image, int nx, int ny, int nz,
+                            const float *box_min_host, const float *box_max_host, float *out, int impl, void *workspace, void *stream);
+/* Marching cubes of `volume` at `threshold` (not NaN), in two calls on one workspace (xrb_mc_workspace(nx, ny, nz) bytes, 8-byte aligned: 4 bytes per
+ * lattice point plus 8 per 256 points plus 16; 0 for bad sizes):
+ *   xrb_mc_count  counts <- (V, F), device int32[2] (both -1 when either exceeds INT32_MAX; xrb_mc_emit then writes nothing);
+ *   xrb_mc_emit   verts f32[V,3] (box coordinates) and faces int32[F,3] (vertex indices), from the workspace xrb_mc_count filled with the same
+ *                 volume, sizes and threshold. box: finite, box_min < box_max.
+ * A lattice value v is inside iff v > threshold; a lattice edge is crossing iff exactly one endpoint is inside. Each crossing edge has ONE vertex,
+ * shared by every triangle that uses it: the edge from point p along +x, +y or +z belongs to p, and its vertex is
+ *   p_out + t * (p_in - p_out),   t = (threshold - v_out) / (v_in - v_out) in [0, 1]
+ * on the edge's axis (the other two coordinates are p's), in fp32 with each operation rounded once.
+ * Order, independent of the launch: vertices by lattice point (z, then y, then x), then axis x, y, z; triangles by cell (z, y, x; a cell is named
+ * by its lowest corner), then in the order of the triangulation table (csrc/mc_table.cuh, generated by scripts/gen_mc_table.py). The table
+ * draws the same segments on a face from both cells that share it (a face with two diagonal inside corners cuts each off on its own), so a
+ * volume whose boundary points are all outside gives a closed mesh: every edge in exactly two triangles, once in each direction. Triangles wind
+ * counter-clockwise seen from outside: their right-hand normals point out of the inside region. No crossing edge gives V = F = 0. */
+size_t xrb_mc_workspace(int nx, int ny, int nz);
+int xrb_mc_count(const float *volume, int nx, int ny, int nz, float threshold, void *workspace, int32_t *counts, void *stream);
+int xrb_mc_emit(const float *volume, int nx, int ny, int nz, float threshold, const float *box_min_host, const float *box_max_host, const void *workspace,
+                float *verts, int32_t *faces, void *stream);
+
 /* Measurement utility (bench.py's second roofline; no reference counterpart): random reads of 4-, 8- or 32-byte records from a table (L2-resident when
  * it is the size of the fp16 hash table) by SMs x 8 CTAs x 256 threads, `rounds` rounds of 8 independent loads per thread. *loads_issued (host) receives the
  * number of loads of the launch; every 4/8-byte load costs one 32-byte sector, which is what bounds the hash gather. */

@@ -1,0 +1,81 @@
+"""Triangle meshes of a density volume: marching cubes on the GPU (xrb_mc_count / xrb_mc_emit, include/xrnerf_b200.h), a binary PLY writer, and
+the map from the Instant-NGP field's frame back to the dataset's (Blender / NeRF) world frame.
+
+    verts, faces = network.extract_mesh(resolution=256)          # HashNerfNetwork: vertices in the frame the rays are given in
+    write_ply('mesh.ply', ngp_to_nerf(verts), faces)
+"""
+import numpy as np
+import torch
+
+from . import _C
+
+
+def marching_cubes(volume, threshold, box=((0.0, 0.0, 0.0), (1.0, 1.0, 1.0))):
+    """volume: CUDA f32[nz,ny,nx] (x fastest), each size 2..1024. -> (verts f32[V,3], faces i32[F,3]) CUDA tensors, vertices in the coordinates of
+    box = (box_min, box_max), which the lattice spans. A value is inside iff it is > threshold; triangles wind counter-clockwise seen from outside.
+    Order and rounding: xrb_mc_emit. Waits for the device once, to size the outputs."""
+    _C.require_cuda(volume)
+    if volume.dim() != 3:
+        raise _C.XrbError(f'XRB_E_BADARG: volume must be [nz,ny,nx], got {tuple(volume.shape)}')
+    nz, ny, nx = volume.shape
+    dev = volume.device
+    ws = torch.empty(_C.lib.xrb_mc_workspace(nx, ny, nz), dtype=torch.uint8, device=dev)
+    counts = torch.zeros(2, dtype=torch.int32, device=dev)
+    _C.check(_C.lib.xrb_mc_count(_C.f32(volume), nx, ny, nz, float(threshold), _C.ptr(ws), _C.i32(counts), _C.stream()), 'mc_count')
+    n_verts, n_faces = (int(v) for v in counts.tolist())
+    if n_verts < 0:
+        raise _C.XrbError('marching cubes: more than 2^31 - 1 vertices or triangles')
+    verts = torch.empty((n_verts, 3), dtype=torch.float32, device=dev)
+    faces = torch.empty((n_faces, 3), dtype=torch.int32, device=dev)
+    if n_verts:
+        _C.check(_C.lib.xrb_mc_emit(_C.f32(volume), nx, ny, nz, float(threshold), _C.float3(box[0]), _C.float3(box[1]), _C.ptr(ws), _C.f32(verts), _C.i32(faces),
+                                    _C.stream()), 'mc_emit')
+    return verts, faces
+
+
+def write_ply(path, verts, faces):
+    """Binary little-endian PLY: `element vertex` with float x, y, z; `element face` with list uchar int vertex_indices."""
+    v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype='<f4').reshape(-1, 3)
+    f = np.ascontiguousarray(torch.as_tensor(faces).detach().cpu().numpy(), dtype='<i4').reshape(-1, 3)
+    rec = np.empty(len(f), dtype=[('n', 'u1'), ('idx', '<i4', (3,))])
+    rec['n'] = 3
+    rec['idx'] = f
+    header = ('ply\nformat binary_little_endian 1.0\n'
+              f'element vertex {len(v)}\nproperty float x\nproperty float y\nproperty float z\n'
+              f'element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n')
+    with open(path, 'wb') as fh:
+        fh.write(header.encode('ascii'))
+        fh.write(v.tobytes())
+        fh.write(rec.tobytes())
+
+
+def ngp_to_nerf(verts, scale=0.33, offset=(0.5, 0.5, 0.5)):
+    """Inverse of the position map of synth.poses_nerf2ngp (and the reference's NGP loader): there a NeRF point p becomes
+    (p * scale + offset)[[1, 2, 0]]; here a point q of the field's frame becomes p with p[[1, 2, 0]] = q, then (p - offset) / scale."""
+    q = torch.as_tensor(verts)
+    p = q[:, [2, 0, 1]]
+    return (p - torch.as_tensor(offset, dtype=p.dtype, device=p.device)) / scale
+
+
+def raw_density_threshold(sigma, activation):
+    """The raw network output whose activated density is sigma (the sampler's density_activation: 0 None, 1 ReLU, 2 Logistic, 3 Exponential):
+    v > raw  <=>  act(v) > sigma. ValueError when sigma is outside the activation's range (or the activation is unknown)."""
+    s = float(sigma)
+    act = int(activation)
+    if not np.isfinite(s):
+        raise ValueError(f'density threshold must be finite, got {sigma}')
+    if act == 0:
+        return s
+    if act == 1:
+        if s < 0:
+            raise ValueError(f'a ReLU density is never negative: threshold {s}')
+        return s
+    if act == 2:
+        if not 0.0 < s < 1.0:
+            raise ValueError(f'a logistic density lies in (0, 1): threshold {s}')
+        return float(np.log(s) - np.log1p(-s))
+    if act == 3:
+        if s <= 0:
+            raise ValueError(f'an exponential density is positive: threshold {s}')
+        return float(np.log(s))
+    raise ValueError(f'unknown density activation {activation}')

@@ -179,6 +179,21 @@ class NgpField(nn.Module):
         _C.check(_C.lib.xrb_ngp_density_forward(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._image), pp, ps, n, _C.ptr(out), impl, _C.stream()), 'ngp_density_forward')
         return out
 
+    def density_lattice(self, shape, box=((0.0, 0.0, 0.0), (1.0, 1.0, 1.0)), impl=None):
+        """Raw density on the lattice of shape (nz, ny, nx) over box = (box_min, box_max) in the warped [0,1]^3 domain -> f32[nz,ny,nx] on the field's
+        device (x fastest). Lattice positions and limits: xrb_ngp_density_lattice (include/xrnerf_b200.h); each value equals run_density at that position."""
+        if not self.hash_params.is_cuda:
+            raise _C.XrbError('xrnerf_b200 kernels need CUDA tensors; there is no CPU fallback')
+        self.refresh()
+        nz, ny, nx = (int(n) for n in shape)
+        dev = self.hash_params.device
+        out = torch.empty((nz, ny, nx), dtype=torch.float32, device=dev)
+        ws = torch.empty(_C.lib.xrb_ngp_density_lattice_workspace(), dtype=torch.uint8, device=dev)
+        impl = self.impl if impl is None else impl
+        _C.check(_C.lib.xrb_ngp_density_lattice(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._image), nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]), _C.f32(out), impl,
+                                                _C.ptr(ws), _C.stream()), 'ngp_density_lattice')
+        return out
+
 
 class _FieldFn(torch.autograd.Function):
     """autograd bridge for NgpField.run_mlp: forward = xrb_ngp_mlp_forward, backward = xrb_ngp_mlp_backward (one kernel

@@ -251,6 +251,24 @@ class HashNerfNetwork(NerfNetwork):
         out['idx'] = idx
         return out
 
+    def extract_mesh(self, resolution=256, threshold=2.5):
+        """Triangle mesh of the field's density level set sigma = threshold -> (verts f32[V,3], faces i32[F,3]) CUDA tensors, vertices in the frame the
+        rays are given in (the warped [0,1]^3 mapped through sampler.aabb_range; the unit cube before set_data), triangles wound counter-clockwise
+        seen from outside. The density is sampled on a resolution^3 lattice over the whole warped domain (NgpField.density_lattice) and meshed by
+        xrnerf_b200.mesh.marching_cubes.
+
+        threshold is a density sigma, mapped to the network's raw output through the inverse of sampler.density_activation (ValueError outside
+        its range). The default 2.5 is Instant-NGP's usual mesh threshold; it has not been checked here on a trained scene. For a Blender-frame
+        mesh of a scene loaded the NGP way, pass the vertices through xrnerf_b200.mesh.ngp_to_nerf."""
+        from ..mesh import marching_cubes, raw_density_threshold
+        raw = raw_density_threshold(threshold, self.sampler.density_activation)
+        self.mlp.mark_dirty()                  # weights may have been swapped through `.data` (EMAHook) since the last pack
+        with torch.no_grad():
+            vol = self.mlp.field.density_lattice((resolution,) * 3)
+            verts, faces = marching_cubes(vol, raw)
+            lo, hi = (float(a) for a in getattr(self.sampler, 'aabb_range', (0.0, 1.0)))
+            return verts * (hi - lo) + lo, faces
+
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
         ret = self.forward(data, is_test=False)
