@@ -198,6 +198,17 @@ int xrb_ngp_mlp_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, c
 /* HashNerfMLP.run_density (hashnerf_mlp.py:107-111): -> density f32[n] (raw, pre-activation) */
 int xrb_ngp_density_forward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const void *weight_image,
                             const float *pts, int pts_stride, int n, float *density, int impl, void *stream);
+/* The raw density and its gradient with respect to the warped position (mesh vertex normals), on CUDA cores, one thread per point:
+ *   density[i] (f32[n], may be NULL) is bit-identical to xrb_ngp_density_forward with impl = 0 at the same position;
+ *   grad[i] (f32[n,3]) is d(raw density)/d(warped position) of that same function, evaluated in fp32 on the fp16 parameters. The fp16 rounding of the
+ *   encoding and of the hidden activations is taken as the identity (straight-through); the ReLU masks are the forward's (a unit is live iff its fp16
+ *   activation is > 0, as in the CUDA-core backward). Level l contributes scale_l * sum over its 8 corners of dw_c/df * v_c, with v_c the corner's fp16
+ *   feature pair and f the in-cell position of the level's grid cell; at a cell face the derivative is the one inside the cell the forward gathered from
+ *   (the cell whose lower face it is).
+ * Positions must lie in [0,1]^3, as for every field entry point. n == 0 is a no-op that touches no pointer. Returns XRB_E_BADARG for a null cfg, table,
+ * density_fp16, pts or grad, n < 0 or pts_stride < 3, and XRB_E_UNSUPPORTED for a config the field does not support, all before any CUDA call. */
+int xrb_ngp_density_grad(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const float *pts, int pts_stride, int n,
+                         float *density /* f32[n], may be NULL */, float *grad /* f32[n,3] */, void *stream);
 
 /* Backward of run_mlp: dL/draw f32[n,4] -> fp32 gradients of the three parameter vectors (ACCUMULATED into the
  * outputs with atomics; caller zeroes them). */

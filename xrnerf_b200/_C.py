@@ -78,6 +78,7 @@ _SIGS = {
     'xrb_tcnn_mlp_backward': (_i, [P, P, P, _i, _i, _i, _i, P, P, P]),
     'xrb_ngp_mlp_forward': (_i, [_cfg, _tab, P, P, P, P, _i, P, _i, _i, P, P, _i, P]),
     'xrb_ngp_density_forward': (_i, [_cfg, _tab, P, P, P, _i, _i, P, _i, P]),
+    'xrb_ngp_density_grad': (_i, [_cfg, _tab, P, P, _i, _i, P, P, P]),
     'xrb_ngp_mlp_backward': (_i, [_cfg, _tab, P, P, P, _i, P, _i, P, _i, P, P, P, P]),
     'xrb_ngp_mlp_backward_tc': (_i, [_cfg, _tab, P, P, _i, P, _i, P, _i, P, P, P, P, P]),
     'xrb_adam_ema_step': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P, _f, P]),

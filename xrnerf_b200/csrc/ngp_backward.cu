@@ -27,12 +27,12 @@ __device__ __forceinline__ void load_row_h(const __half *row, float *v, int n) {
 __device__ __forceinline__ void store_row_h(__half *row, const float *v, int n) {
     for (int k = 0; k < n; k += 2) reinterpret_cast<__half2 *>(row)[k >> 1] = __floats2half2_rn(v[k], v[k + 1]);
 }
-// gx[k] = sum_o W[o][k] * gy[o]
-template <int IN, int OUT>
+// gx[k] = sum_o W[o][k] * gy[o]. UNROLL: how many outputs are unrolled (the training kernels take 2; OUT keeps gy in registers)
+template <int IN, int OUT, int UNROLL = 2>
 __device__ __forceinline__ void bwd_layer_dx(const __half *__restrict__ W, const float *gy, float *gx) {
 #pragma unroll
     for (int k = 0; k < IN; ++k) gx[k] = 0.f;
-#pragma unroll 2
+#pragma unroll UNROLL
     for (int o = 0; o < OUT; ++o) {
         const float g = gy[o];
         const __half2 *w2 = reinterpret_cast<const __half2 *>(W + (size_t)o * IN);
@@ -275,6 +275,67 @@ static int launch_tcnn_mlp_bwd(const void *params, const void *x, const void *dy
     return check_launch("tcnn_mlp_backward");
 }
 
+// ---------------------------------------------------------------------------- density and its position gradient (xrb_ngp_density_grad: mesh normals)
+// thread = point. The forward is the CUDA-core density of ngp_field_simt_kernel<true> (same gather, rounding and FMA order, so the density is bit-identical),
+// keeping each hidden layer's ReLU mask (relu_mask's convention: the fp16 activation is > 0). The backward differentiates output 0 only: its weight row,
+// masked, then the W^T chain down to dL/d(encoding), fp32 throughout (fp16 roundings are taken as the identity), then position_grad_level per level.
+// The hidden layers are a run-time loop (density_hidden 1..4, as simt_net); each thread parks its layers' 64-bit masks in its own shared-memory slots, so
+// nothing is indexed dynamically in registers. The density net's fp16 weights follow the masks in shared memory, read as broadcasts.
+constexpr int DG_THREADS = 128;
+__host__ __device__ constexpr size_t density_grad_smem(int dh) { return sizeof(uint64_t) * dh * DG_THREADS + sizeof(__half) * (size_t)net_params(dh); }
+__global__ void __launch_bounds__(DG_THREADS) ngp_density_grad_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const __half *__restrict__ dens_p,
+                                                                      int dh, const float *__restrict__ pts, int pts_stride, int n, float *__restrict__ density, float *__restrict__ grad) {
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    uint64_t *s_mask = reinterpret_cast<uint64_t *>(smem_raw);              // [dh][DG_THREADS]
+    __half *s_w = reinterpret_cast<__half *>(s_mask + dh * DG_THREADS);
+    const int nd = net_params(dh);
+    for (int k = threadIdx.x; k < nd; k += DG_THREADS) s_w[k] = dens_p[k];
+    __syncthreads();
+    const __half *w_out = s_w + NET_IN + (dh - 1) * NET_HID;
+    for (int base = blockIdx.x * DG_THREADS; base < n; base += gridDim.x * DG_THREADS) {   // (a block-uniform base keeps the point index out of the register file)
+        const int i = base + threadIdx.x;
+        if (i >= n) break;
+        const float *p = pts + (size_t)i * pts_stride;
+        const float x = p[0], y = p[1], z = p[2];
+        float a[64], b[64];
+        {
+            float enc[32];
+#pragma unroll
+            for (int l = 0; l < 16; ++l) { float2 f = hash_level(table, cells, g, l, x, y, z); enc[2 * l] = round_h(f.x); enc[2 * l + 1] = round_h(f.y); }
+            simt_layer<32, 64, true>(s_w, enc, a);
+        }
+        for (int k = 0;; ++k) {   // a = output of hidden layer k
+            uint64_t m = 0;
+#pragma unroll
+            for (int q = 0; q < 64; ++q) m |= (uint64_t)(a[q] > 0.f) << q;
+            s_mask[k * DG_THREADS + threadIdx.x] = m;
+            if (k == dh - 1) break;
+            simt_layer<64, 64, true>(s_w + NET_IN + k * NET_HID, a, b);
+#pragma unroll
+            for (int q = 0; q < 64; ++q) a[q] = b[q];
+        }
+        float d;
+        simt_layer<64, 1, false>(w_out, a, &d);
+        if (density) density[i] = d;
+        // a <- d(out 0)/d(output of the last hidden layer), masked; then one masked W^T step per hidden matrix
+        uint64_t m = s_mask[(dh - 1) * DG_THREADS + threadIdx.x];
+#pragma unroll
+        for (int q = 0; q < 64; ++q) a[q] = (m >> q) & 1u ? __half2float(w_out[q]) : 0.f;
+        for (int k = dh - 1; k >= 1; --k) {
+            bwd_layer_dx<64, 64, 64>(s_w + NET_IN + (k - 1) * NET_HID, a, b);
+            m = s_mask[(k - 1) * DG_THREADS + threadIdx.x];
+#pragma unroll
+            for (int q = 0; q < 64; ++q) a[q] = (m >> q) & 1u ? b[q] : 0.f;
+        }
+        bwd_layer_dx<32, 64, 64>(s_w, a, b);   // b[0..31] = d(out 0)/d(encoding)
+        float3 dp = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+        for (int l = 0; l < 16; ++l) position_grad_level(table, g, l, x, y, z, b[2 * l], b[2 * l + 1], dp);
+        float *o = grad + 3 * (size_t)i;
+        o[0] = dp.x; o[1] = dp.y; o[2] = dp.z;
+    }
+}
+
 // 5 * HuberLoss(delta, 'sum') of HashNerfNetwork.train_step (networks/utils/metrics.py:8-16, hashnerf.py:39-44): gradient wrt rgb and the loss value in ONE pass
 __global__ void __launch_bounds__(256) huber5_kernel(const float *__restrict__ rgb, const float *__restrict__ target, int64_t n, float delta, float *__restrict__ grad, float *__restrict__ loss_accum) {
     float local = 0.f;
@@ -347,6 +408,20 @@ int xrb_ngp_mlp_backward(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
 #undef XRB_BW
     set_error("ngp_mlp_backward: (density_hidden, color_hidden) must be one of (1,1) (1,2) (2,2) (1,3) (2,3)");
     return XRB_E_UNSUPPORTED;
+}
+
+int xrb_ngp_density_grad(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *density_fp16, const float *pts, int pts_stride, int n, float *density, float *grad,
+                         void *stream) {
+    int e = check_cfg(cfg); if (e) return e;
+    XRB_REQUIRE(n >= 0 && pts_stride >= 3, "ngp_density_grad: bad size");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(table && density_fp16 && pts && grad, "ngp_density_grad: null pointer");
+    HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
+    const size_t smem = density_grad_smem(cfg->density_hidden);   // <= 34 KB (density_hidden 4): no opt-in needed
+    const int grid = persistent_grid((const void *)ngp_density_grad_kernel, DG_THREADS, smem, (n + DG_THREADS - 1) / DG_THREADS);
+    ngp_density_grad_kernel<<<grid, DG_THREADS, smem, (cudaStream_t)stream>>>(g, (const __half2 *)table->table_fp16, (const uint8_t *)table->cell_image, (const __half *)density_fp16,
+                                                                              cfg->density_hidden, pts, pts_stride, n, density, grad);
+    return check_launch("ngp_density_grad");
 }
 
 }  // extern "C"

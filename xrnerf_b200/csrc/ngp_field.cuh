@@ -242,6 +242,27 @@ __device__ __forceinline__ void scatter_level(float *__restrict__ d_table, const
         atomicAdd(tl + idx, make_float2(w * g0, w * g1));
     }
 }
+// Backward of hash_level with respect to the position: adds scale_l * sum_c (dw_c/df) * (v_c . (g0, g1)) to d, where v_c are the 8 corner feature pairs
+// (re-read from the fp16 table at grid_index), w_c the trilinear weights and f the in-cell position grid_cell computes; (g0, g1) = dL/d(the level's two
+// features). df/dx = scale_l. At a cell face the derivative is the one inside the cell grid_cell selects, the cell the gather read.
+__device__ __forceinline__ void position_grad_level(const __half2 *__restrict__ table, const HashGridDev &g, int l, float x, float y, float z, float g0, float g1, float3 &d) {
+    const GridCell c = grid_cell(g, l, x, y, z);
+    const float ux = 1.f - c.fx, uy = 1.f - c.fy, uz = 1.f - c.fz;
+    float dx = 0.f, dy = 0.f, dz = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint32_t idx = grid_index(c.gx + (k & 1), c.gy + ((k >> 1) & 1), c.gz + ((k >> 2) & 1), c.hs, c.res);
+        const float2 v = __half22float2(__ldg(table + c.off + idx));
+        const float s = fmaf(v.y, g1, v.x * g0);   // dL/dw_c
+        const float wx = (k & 1) ? c.fx : ux, wy = (k & 2) ? c.fy : uy, wz = (k & 4) ? c.fz : uz;
+        const float ayz = wy * wz, axz = wx * wz, axy = wx * wy;
+        dx = fmaf((k & 1) ? ayz : -ayz, s, dx);
+        dy = fmaf((k & 2) ? axz : -axz, s, dy);
+        dz = fmaf((k & 4) ? axy : -axy, s, dz);
+    }
+    const float sc = g.scale[l];
+    d.x = fmaf(sc, dx, d.x); d.y = fmaf(sc, dy, d.y); d.z = fmaf(sc, dz, d.z);
+}
 // The paired form of the tensor-core backward (d_table 16-byte aligned). Its scatter is bound by the LSU's reduction issue rate (~1.3 cycles per lane
 // and RED, measured: 450 of 880 us per 700 K samples with 128 two-float REDs per sample), so x-adjacent corners that are also adjacent in memory go out
 // as ONE 16-byte red.global.add.v4.f32:

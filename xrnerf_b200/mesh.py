@@ -3,6 +3,8 @@ the map from the Instant-NGP field's frame back to the dataset's (Blender / NeRF
 
     verts, faces = network.extract_mesh(resolution=256)          # HashNerfNetwork: vertices in the frame the rays are given in
     write_ply('mesh.ply', ngp_to_nerf(verts), faces)
+    verts, faces, normals, colors = network.extract_colored_mesh(resolution=256)
+    write_ply('mesh.ply', ngp_to_nerf(verts), faces, ngp_to_nerf_normals(normals), colors)
 """
 import numpy as np
 import torch
@@ -33,19 +35,35 @@ def marching_cubes(volume, threshold, box=((0.0, 0.0, 0.0), (1.0, 1.0, 1.0))):
     return verts, faces
 
 
-def write_ply(path, verts, faces):
-    """Binary little-endian PLY: `element vertex` with float x, y, z; `element face` with list uchar int vertex_indices."""
+def write_ply(path, verts, faces, normals=None, colors=None):
+    """Binary little-endian PLY: `element vertex` with float x, y, z, then float nx, ny, nz when `normals` [V,3] is given, then uchar red, green, blue when
+    `colors` [V,3] in [0,1] is given (each channel floor(clamp(c, 0, 1) * 255 + 0.5)), interleaved per vertex; `element face` with list uchar int
+    vertex_indices."""
     v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype='<f4').reshape(-1, 3)
     f = np.ascontiguousarray(torch.as_tensor(faces).detach().cpu().numpy(), dtype='<i4').reshape(-1, 3)
+    fields, props = [('xyz', '<f4', (3,))], 'property float x\nproperty float y\nproperty float z\n'
+    if normals is not None:
+        fields.append(('n', '<f4', (3,)))
+        props += 'property float nx\nproperty float ny\nproperty float nz\n'
+    if colors is not None:
+        fields.append(('rgb', 'u1', (3,)))
+        props += 'property uchar red\nproperty uchar green\nproperty uchar blue\n'
+    vrec = np.empty(len(v), dtype=fields)
+    vrec['xyz'] = v
+    if normals is not None:
+        vrec['n'] = np.asarray(torch.as_tensor(normals).detach().cpu().numpy(), dtype='<f4').reshape(-1, 3)
+    if colors is not None:
+        c = np.asarray(torch.as_tensor(colors).detach().cpu().numpy(), dtype=np.float64).reshape(-1, 3)
+        vrec['rgb'] = np.floor(np.clip(c, 0.0, 1.0) * 255.0 + 0.5).astype(np.uint8)
     rec = np.empty(len(f), dtype=[('n', 'u1'), ('idx', '<i4', (3,))])
     rec['n'] = 3
     rec['idx'] = f
     header = ('ply\nformat binary_little_endian 1.0\n'
-              f'element vertex {len(v)}\nproperty float x\nproperty float y\nproperty float z\n'
+              f'element vertex {len(v)}\n{props}'
               f'element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n')
     with open(path, 'wb') as fh:
         fh.write(header.encode('ascii'))
-        fh.write(v.tobytes())
+        fh.write(vrec.tobytes())
         fh.write(rec.tobytes())
 
 
@@ -55,6 +73,12 @@ def ngp_to_nerf(verts, scale=0.33, offset=(0.5, 0.5, 0.5)):
     q = torch.as_tensor(verts)
     p = q[:, [2, 0, 1]]
     return (p - torch.as_tensor(offset, dtype=p.dtype, device=p.device)) / scale
+
+
+def ngp_to_nerf_normals(normals):
+    """Normals (directions) of the field's frame in the NeRF world frame: the axis permutation of ngp_to_nerf. Its scale is positive and uniform, so it
+    drops out of a unit normal; zero normals stay zero."""
+    return torch.as_tensor(normals)[:, [2, 0, 1]]
 
 
 def raw_density_threshold(sigma, activation):
@@ -79,3 +103,17 @@ def raw_density_threshold(sigma, activation):
             raise ValueError(f'an exponential density is positive: threshold {s}')
         return float(np.log(s))
     raise ValueError(f'unknown density activation {activation}')
+
+
+def activate_rgb(raw, activation):
+    """The sampler's rgb_activation (0 None, 1 ReLU, 2 Logistic, 3 Exponential of the value clamped to [-10, 10], as the composite applies it) on a tensor"""
+    act = int(activation)
+    if act == 0:
+        return raw
+    if act == 1:
+        return torch.relu(raw)
+    if act == 2:
+        return torch.sigmoid(raw)
+    if act == 3:
+        return torch.exp(torch.clamp(raw, -10.0, 10.0))
+    raise ValueError(f'unknown rgb activation {activation}')

@@ -179,6 +179,18 @@ class NgpField(nn.Module):
         _C.check(_C.lib.xrb_ngp_density_forward(self.cfg, self.tab, _C.ptr(self._dens16), _C.ptr(self._image), pp, ps, n, _C.ptr(out), impl, _C.stream()), 'ngp_density_forward')
         return out
 
+    def density_grad(self, pts):
+        """pts: [n,3] float32 view in the warped [0,1]^3 domain (row stride may be > 3). -> (density f32[n,1], grad f32[n,3]): the raw density, bit-identical
+        to run_density(pts, impl=0), and its gradient with respect to the position, on CUDA cores (xrb_ngp_density_grad, include/xrnerf_b200.h)."""
+        _C.require_cuda(pts)
+        self.refresh()
+        pp, ps = _C.rows(pts)
+        n = pts.shape[0]
+        density = torch.empty((n, 1), dtype=torch.float32, device=pts.device)
+        grad = torch.empty((n, 3), dtype=torch.float32, device=pts.device)
+        _C.check(_C.lib.xrb_ngp_density_grad(self.cfg, self.tab, _C.ptr(self._dens16), pp, ps, n, _C.f32(density), _C.f32(grad), _C.stream()), 'ngp_density_grad')
+        return density, grad
+
     def density_lattice(self, shape, box=((0.0, 0.0, 0.0), (1.0, 1.0, 1.0)), impl=None):
         """Raw density on the lattice of shape (nz, ny, nx) over box = (box_min, box_max) in the warped [0,1]^3 domain -> f32[nz,ny,nx] on the field's
         device (x fastest). Lattice positions and limits: xrb_ngp_density_lattice (include/xrnerf_b200.h); each value equals run_density at that position."""

@@ -260,14 +260,43 @@ class HashNerfNetwork(NerfNetwork):
         threshold is a density sigma, mapped to the network's raw output through the inverse of sampler.density_activation (ValueError outside
         its range). The default 2.5 is Instant-NGP's usual mesh threshold; it has not been checked here on a trained scene. For a Blender-frame
         mesh of a scene loaded the NGP way, pass the vertices through xrnerf_b200.mesh.ngp_to_nerf."""
+        verts, faces = self._warped_mesh(resolution, threshold)
+        return self._from_warped(verts), faces
+
+    def _warped_mesh(self, resolution, threshold):
+        """extract_mesh's triangles with the vertices still in the field's warped [0,1]^3 domain"""
         from ..mesh import marching_cubes, raw_density_threshold
         raw = raw_density_threshold(threshold, self.sampler.density_activation)
         self.mlp.mark_dirty()                  # weights may have been swapped through `.data` (EMAHook) since the last pack
         with torch.no_grad():
             vol = self.mlp.field.density_lattice((resolution,) * 3)
-            verts, faces = marching_cubes(vol, raw)
-            lo, hi = (float(a) for a in getattr(self.sampler, 'aabb_range', (0.0, 1.0)))
-            return verts * (hi - lo) + lo, faces
+            return marching_cubes(vol, raw)
+
+    def _from_warped(self, verts):
+        lo, hi = (float(a) for a in getattr(self.sampler, 'aabb_range', (0.0, 1.0)))
+        return verts * (hi - lo) + lo
+
+    def extract_colored_mesh(self, resolution=256, threshold=2.5):
+        """extract_mesh with a unit normal and a colour per vertex -> (verts f32[V,3], faces i32[F,3], normals f32[V,3], colors f32[V,3]) CUDA tensors, in
+        the frame extract_mesh uses; verts and faces are bit-identical to extract_mesh(resolution, threshold).
+
+        normal = -g / |g| (0 where g = 0), with g the gradient of the raw density at the vertex's warped position (NgpField.density_grad). Inside is
+        "raw > threshold", so the normal points outward. sampler.aabb_range is a positive uniform scale, so the normals need no map. The gradient is that of
+        the CUDA-core density (impl 0), while the lattice the vertices come from uses the field's impl: the two densities agree to the field's fp16
+        tolerance, not bit for bit.
+
+        color = sampler.rgb_activation(run_mlp(warped vertex, dir)[:, :3]) with dir = (1 - normal) / 2: the field seen from outside, looking along
+        -normal, in the warped [0,1]^3 direction convention of the ray march (dir = (d + 1) / 2 for a unit ray direction d). A zero normal gives the
+        direction (0.5, 0.5, 0.5). For the Blender frame, map verts with xrnerf_b200.mesh.ngp_to_nerf and normals with ngp_to_nerf_normals."""
+        from ..mesh import activate_rgb
+        verts_w, faces = self._warped_mesh(resolution, threshold)
+        field = self.mlp.field
+        with torch.no_grad():
+            _, g = field.density_grad(verts_w)
+            norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
+            normals = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+            colors = activate_rgb(field.run_mlp(verts_w, (1.0 - normals) * 0.5)[:, :3], self.sampler.rgb_activation)
+            return self._from_warped(verts_w), faces, normals, colors
 
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
