@@ -448,6 +448,25 @@ int xrb_mc_count(const float *volume, int nx, int ny, int nz, float threshold, v
 int xrb_mc_emit(const float *volume, int nx, int ny, int nz, float threshold, const float *box_min_host, const float *box_max_host, const void *workspace,
                 float *verts, int32_t *faces, void *stream);
 
+/* ---- NeRF mesh export (csrc/nerf_mlp_tc.cu, csrc/nerf.cu; no reference counterpart): the NerfMLP's density on the lattice above, and the gradient of
+ * its raw density with respect to the position (vertex normals).
+ *
+ * xrb_nerf_density_lattice: out[k][j][i] <- raw[:, 3] of xrb_nerf_mlp_forward (same weight_image and bias, from pack_nerf_mlp) on the
+ * xrb_nerf_posenc_tiles encoding of lattice point (i, j, k), bit for bit; the view direction does not enter alpha. The lattice positions are the ones
+ * above; the box is any finite box with box_min < box_max (the NeRF world frame). The same wgmma kernel with its layer schedule cut after
+ * pts_linears.7: it writes each point's encoding into shared memory from the lattice index and stores alpha from the layer-7 epilogue, so it needs
+ * no position tensor, encoding image or workspace. Only input_ch = 63, multires = 10 (the reference NeRF configs) is implemented: anything else returns
+ * XRB_E_UNSUPPORTED. Sizes, input_ch and box are checked before any CUDA call; weight_image and bias must be 16-byte aligned.
+ *
+ * xrb_nerf_posenc_grad: grad f32[n,3] <- the gradient with respect to the position through BaseEmbedder's encoding (multires 0..10) of pts f32[n,3].
+ * d_enc_image is a tile image of n_terms (1..4) one-block terms per 128-row tile; the gradient with respect to the 3 + 6 multires encoding columns is
+ * e = (sum of the terms, fp32) / *scale (device float: the staging scale xrb_nerf_tg_pack_draw wrote, scale[1]), and
+ *   grad[i][a] = e[a] + sum_b 2^b (cos(2^b x_a) e[3 + 6b + a] - sin(2^b x_a) e[6 + 6b + a])
+ * with the column order of xrb_nerf_posenc. n == 0 is a no-op that touches no pointer. */
+int xrb_nerf_density_lattice(const void *weight_image, const float *bias, int input_ch, int multires, int nx, int ny, int nz, const float *box_min_host,
+                             const float *box_max_host, float *out, void *stream);
+int xrb_nerf_posenc_grad(const float *pts, int64_t n_pts, int multires, const void *d_enc_image, int n_terms, const float *scale, float *grad, void *stream);
+
 /* Measurement utility (bench.py's second roofline; no reference counterpart): random reads of 4-, 8- or 32-byte records from a table (L2-resident when
  * it is the size of the fp16 hash table) by SMs x 8 CTAs x 256 threads, `rounds` rounds of 8 independent loads per thread. *loads_issued (host) receives the
  * number of loads of the launch; every 4/8-byte load costs one 32-byte sector, which is what bounds the hash gather. */

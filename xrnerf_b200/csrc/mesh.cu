@@ -12,15 +12,10 @@
 #include <cmath>
 
 #include "ngp_field.cuh"
+#include "lattice.cuh"
 #include "mc_table.cuh"
 
 namespace xrb {
-
-// coordinate of lattice index i on an axis of n points from lo to hi: min(lo + i * ((hi - lo) / (n - 1)), hi), each operation rounded once.
-// The min keeps the last point inside the box when the rounded step overshoots.
-__device__ __forceinline__ float lattice_coord(float lo, float hi, int n, int i) { return fminf(add_(lo, mul_((float)i, div_(sub_(hi, lo), (float)(n - 1)))), hi); }
-
-struct Box { float lo[3], hi[3]; };
 
 // ---------------------------------------------------------------------------------------------------------------- density on a lattice
 // positions of `n` consecutive lattice points from `first` (x fastest) as the field's [n,3] rows
@@ -174,23 +169,6 @@ __global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restri
 }
 
 // ---------------------------------------------------------------------------------------------------------------- argument checks
-// 0: an empty lattice (some size 0); 1: every size in [2, 1024]; -1: otherwise (the error is set)
-static int lattice_sizes(int nx, int ny, int nz, const char *who) {
-    const int n[3] = {nx, ny, nz};
-    bool empty = false, ok = true;
-    for (int a = 0; a < 3; ++a) { empty |= n[a] == 0; ok &= n[a] == 0 || (n[a] >= 2 && n[a] <= 1024); }
-    if (!ok) { set_error(who); return -1; }
-    return empty ? 0 : 1;
-}
-static int read_box(const float *lo, const float *hi, bool unit, Box *b, const char *who) {
-    XRB_REQUIRE(lo && hi, who);
-    for (int a = 0; a < 3; ++a) {
-        XRB_REQUIRE(lo[a] < hi[a] && std::isfinite(lo[a]) && std::isfinite(hi[a]), who);
-        XRB_REQUIRE(!unit || (lo[a] >= 0.f && hi[a] <= 1.f), who);
-        b->lo[a] = lo[a]; b->hi[a] = hi[a];
-    }
-    return XRB_OK;
-}
 static Lattice lattice(int nx, int ny, int nz) { Lattice L; L.nx = nx; L.ny = ny; L.nz = nz; L.nxy = (int64_t)nx * ny; L.points = L.nxy * nz; return L; }
 
 }  // namespace xrb

@@ -3,6 +3,7 @@
 // ray, lanes over samples with shuffle scans. Every encoder: positional encoding and Mip-NeRF IPE, into fp32 `embedded` rows or straight
 // into the fp16 tile images the NerfMLP kernels read. Ray generation and z values. References relative to /root/reference/xrnerf/models/.
 #include "common.cuh"
+#include "posenc.cuh"
 #include "tc.cuh"
 
 namespace xrb {
@@ -336,7 +337,6 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_kernel(int64_t n_rays, int 
 // kind, so there is no intra-warp divergence; every trig evaluation is shared by the columns that use it and all column indices are compile-time).
 // The generic kernels above serve every other degree. Before these kernels existed (32768 rays on an H100):
 // mip_ipe_tiles_kernel 4.29 ms per 4.2 M rows and posenc_tiles_kernel 1.92 ms per 6.3 M rows next to 8.46 ms of MLP.
-__device__ __forceinline__ float pow2i(int e) { return __int_as_float((127 + e) << 23); }   // 2^e, exact, -126 <= e <= 127
 // Mip-NeRF, 6*NDEG <= 128 point columns (two blocks) + direction block. item 0 = both point blocks of the row, item 1 = direction block.
 // IPE column q (< 3*NDEG): exp(-0.5 * cov_ax * 4^deg) * sin(mean_ax * 2^deg), column 3*NDEG + q: the same with sin(y + pi/2) — the reference's
 // expression, NOT cos(y): fl(y + pi/2) differs from y + pi/2 by up to ulp(y)/2 and the reference's value includes that (mipnerf_embedder.py:35-41,:55-60).
@@ -419,20 +419,54 @@ __global__ void __launch_bounds__(256) posenc_tiles_fast_kernel(const float *__r
             else { x[0] = pts[3 * row]; x[1] = pts[3 * row + 1]; x[2] = pts[3 * row + 2]; }
 #pragma unroll
             for (int a = 0; a < 3; ++a) v[a] = x[a];
-            if (item == 0) {
-#pragma unroll
-                for (int bnd = 0; bnd < LP; ++bnd)
-#pragma unroll
-                    for (int a = 0; a < 3; ++a) { float sn, cs; sincosf(x[a] * pow2i(bnd), &sn, &cs); v[3 + 6 * bnd + a] = sn; v[6 + 6 * bnd + a] = cs; }
-            } else {
-#pragma unroll
-                for (int bnd = 0; bnd < LD; ++bnd)
-#pragma unroll
-                    for (int a = 0; a < 3; ++a) { float sn, cs; sincosf(x[a] * pow2i(bnd), &sn, &cs); v[3 + 6 * bnd + a] = sn; v[6 + 6 * bnd + a] = cs; }
-            }
+            if (item == 0) posenc_bands<LP>(x, v);
+            else posenc_bands<LD>(x, v);
         }
 #pragma unroll
         for (int ch = 0; ch < 8; ++ch) st_chunk(trow + sw128_chunk(r, ch), pack_h8(v + 8 * ch));
+    }
+}
+
+// The gradient with respect to the position through BaseEmbedder's encoding (mesh normals of a NerfMLP), one thread per point. The gradient with
+// respect to the encoding, e, is the sum of the n_terms one-block fp16 tile images of d_enc (block k of every tile = term k: the input gradients of the
+// layers that read the point encoding) divided by the staging scale s; with the column order above,
+//   dL/dx_a = e[a] + sum_b 2^b (cos(2^b x_a) e[3 + 6b + a] - sin(2^b x_a) e[6 + 6b + a])
+__global__ void __launch_bounds__(256) posenc_grad_kernel(const float *__restrict__ pts, int64_t n_pts, int multires, const uint8_t *__restrict__ d_enc, int n_terms,
+                                                          const float *__restrict__ scale, float *__restrict__ grad) {
+    const float inv = 1.f / *scale;   // a power of two: exact
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)(i & 127);
+        float e[64];
+#pragma unroll
+        for (int c = 0; c < 64; ++c) e[c] = 0.f;
+        for (int k = 0; k < n_terms; ++k) {
+            const uint8_t *row = tile_block(const_cast<uint8_t *>(d_enc), i >> 7, n_terms, k) + sw128_row(r);
+#pragma unroll
+            for (int ch = 0; ch < 8; ++ch) {
+                const uint4 q = __ldg(reinterpret_cast<const uint4 *>(row + sw128_chunk(r, ch)));
+                const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[j]));
+                    e[8 * ch + 2 * j] += f.x; e[8 * ch + 2 * j + 1] += f.y;
+                }
+            }
+        }
+        const float x[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
+        float g[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) g[a] = e[a] * inv;
+#pragma unroll
+        for (int bnd = 0; bnd < 10; ++bnd) {
+            if (bnd >= multires) break;
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                float sn, cs; sincosf(x[a] * pow2i(bnd), &sn, &cs);
+                g[a] += pow2i(bnd) * (cs * (e[3 + 6 * bnd + a] * inv) - sn * (e[6 + 6 * bnd + a] * inv));
+            }
+        }
+#pragma unroll
+        for (int a = 0; a < 3; ++a) grad[3 * i + a] = g[a];
     }
 }
 
@@ -693,6 +727,14 @@ int xrb_nerf_posenc_tiles_rays(const float *rays_o, const float *rays_d, const f
     if (n_rays == 0) return XRB_OK;
     XRB_REQUIRE(rays_o && rays_d && z_vals && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "nerf_posenc_tiles_rays: null/misaligned pointer");
     return posenc_tiles(z_vals, viewdirs, n_rays * samples_per_ray, samples_per_ray, multires, multires_dirs, enc_image, rays_o, rays_d, stream, "nerf_posenc_tiles_rays");
+}
+
+int xrb_nerf_posenc_grad(const float *pts, int64_t n_pts, int multires, const void *d_enc_image, int n_terms, const float *scale, float *grad, void *stream) {
+    XRB_REQUIRE(n_pts >= 0 && multires >= 0 && multires <= 10 && n_terms >= 1 && n_terms <= 4, "nerf_posenc_grad: bad size (multires 0..10, n_terms 1..4)");
+    if (n_pts == 0) return XRB_OK;
+    XRB_REQUIRE(pts && d_enc_image && scale && grad && ((uintptr_t)d_enc_image & 15) == 0, "nerf_posenc_grad: null/misaligned pointer");
+    posenc_grad_kernel<<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, multires, (const uint8_t *)d_enc_image, n_terms, scale, grad);
+    return check_launch("nerf_posenc_grad");
 }
 
 int xrb_mip_resample(const float *z_vals, const float *weights, const float *u, int n_rays, int n_samples, float resample_padding, float *z_out, void *stream) {

@@ -18,8 +18,14 @@
 // Numeric contract: fp16 operands (weights and activations), fp32 accumulate; each layer's accumulator is rounded to fp16, then the bias is added in
 // fp16; alpha is an fp32 register dot product of the fp16 pts_linears.7 output with alpha_linear, formed in that layer's epilogue.
 // Parity tolerance vs the fp32 reference in tests/test_gpu_nerf_mlp.py.
+//
+// The density lattice (xrb_nerf_density_lattice, mesh export) is the same kernel with LAT = true: the layer schedule stops after pts_linears.7, the
+// producer streams only those layers' slabs (a prefix of the weight image) and no encoding blocks, each consumer warpgroup writes the point-encoding
+// rows of its 64 lattice points into A block 4 before layer 0 (from the lattice index, in registers), and the pts_linears.7 epilogue stores alpha.
 #include "tc.cuh"
 #include "common.cuh"
+#include "lattice.cuh"
+#include "posenc.cuh"
 
 namespace xrb {
 
@@ -68,6 +74,7 @@ struct NmParams {
     float *raw;
     uint32_t slot_bytes; int n_slots;
     uint32_t n_slabs[NM_LAYERS]; uint32_t slab_bytes[NM_LAYERS][NM_MAX_SLABS];   // the producer's stream (from nm_layer on the host)
+    int lat_n[3]; Box lat_box;                                                     // LAT: lattice sizes and box; raw is then out f32[n_rows]
 };
 
 struct NmCtx {
@@ -104,12 +111,13 @@ __device__ __forceinline__ void nm_slabs(NmCtx &x, float *acc) {
     }
 }
 
-// layers [L, 11) of one tile for my 64 rows
-template <bool MIP, int L>
+// layers [L, 11) of one tile for my 64 rows (LAT: [L, 8))
+template <bool MIP, bool LAT, int L>
 __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t tile, float *alpha) {
-    if constexpr (L < NM_LAYERS) {
+    if constexpr (L < (LAT ? 8 : NM_LAYERS)) {
         constexpr NmLayer Ly = nm_layer<MIP>(L);
         float acc[Ly.N / 2];
+        if constexpr (LAT) asm volatile("" : "+l"(x.A), "+r"(x.t), "+r"(x.r0));   // the layer's addresses are formed here, not hoisted out of the tile loop
         tc::fence_proxy_async_smem();        // my epilogue writes -> visible to the tensor core
         tc::named_bar_sync(1 + x.wg, 128);   // ... and every row of my warpgroup written
         nm_slabs<MIP, L, 0>(x, acc);
@@ -139,7 +147,7 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
                     __half2 h = __hadd2(__floats2half2_rn(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]), __floats2half2_rn(b0, b1));
                     if (Ly.relu) h = __hmax2(h, __float2half2_rn(0.f));
                     if (Ly.alpha_dot) { const float2 f = __half22float2(h); adot[e] = fmaf(f.x, __ldg(wa + col), adot[e]); adot[e] = fmaf(f.y, __ldg(wa + col + 1), adot[e]); }
-                    *reinterpret_cast<__half2 *>(sw128_elem(blk, x.r0 + 8u * (uint32_t)e, col & 63u)) = h;
+                    if (!(LAT && Ly.alpha_dot)) *reinterpret_cast<__half2 *>(sw128_elem(blk, x.r0 + 8u * (uint32_t)e, col & 63u)) = h;   // LAT: h7 has no reader
                 }
             }
             if constexpr (Ly.alpha_dot) {   // the four lanes of a quad hold all 256 columns of its two rows
@@ -149,13 +157,40 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
                     adot[e] += __shfl_xor_sync(0xffffffffu, adot[e], 2);
                     alpha[e] = adot[e] + __ldg(wa + 256);
                 }
+                if constexpr (LAT) {
+                    if ((x.t & 3u) == 0) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int64_t i = tile * 128 + x.r0 + 8 * e;
+                            if (i < P.n_rows) P.raw[i] = alpha[e];
+                        }
+                    }
+                }
             }
         }
-        nm_layers<MIP, L + 1>(x, P, tile, alpha);
+        nm_layers<MIP, LAT, L + 1>(x, P, tile, alpha);
     }
 }
 
-template <bool MIP>
+// LAT: the positional encoding (multires 10) of lattice point p, zero past the last point, as row `row` of the point-encoding A block `blk`. Each
+// column goes to shared memory as soon as it is formed (fp16, the rounding of pack_h8), so no 64-float row is live beside the sincosf reductions.
+__device__ __forceinline__ void nm_lattice_row(const NmParams &P, uint8_t *blk, uint32_t row, int64_t p) {
+    auto put = [&](int c, float y) { *reinterpret_cast<__half *>(sw128_elem(blk, row, (uint32_t)c)) = __float2half_rn(y); };
+    if (p < P.n_rows) {
+        const int idx[3] = {(int)(p % P.lat_n[0]), (int)((p / P.lat_n[0]) % P.lat_n[1]), (int)(p / ((int64_t)P.lat_n[0] * P.lat_n[1]))};
+        float x[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) { x[a] = lattice_coord(P.lat_box.lo[a], P.lat_box.hi[a], P.lat_n[a], idx[a]); put(a, x[a]); }
+        posenc_bands<10>(x, put);
+        put(63, 0.f);
+    } else {
+        uint8_t *r = blk + sw128_row(row);
+#pragma unroll
+        for (int ch = 0; ch < 8; ++ch) st_chunk(r + sw128_chunk(row, ch), make_uint4(0u, 0u, 0u, 0u));
+    }
+}
+
+template <bool MIP, bool LAT>
 __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid_constant__ NmParams P) {
     extern __shared__ uint8_t dyn_smem[];
     constexpr int AUX = MIP ? 2 : 1;
@@ -179,10 +214,12 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
         if (warp == 8 && lane == 0) {
             uint32_t it = 0, n = 0;
             for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
-                // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block)
-                if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
-                tc::mbar_expect_tx(enc_full, enc_bytes);
-                tc::tma_bulk_g2s(A + 4 * TILE_BLOCK_BYTES, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
+                // the tile's encoding blocks land in A blocks 4.. (point blocks, then the direction block); LAT: the consumers write them
+                if constexpr (!LAT) {
+                    if (n > 0) tc::mbar_wait(enc_free, (n - 1) & 1);
+                    tc::mbar_expect_tx(enc_full, enc_bytes);
+                    tc::tma_bulk_g2s(A + 4 * TILE_BLOCK_BYTES, P.enc_image + (size_t)tile * enc_bytes, enc_bytes, enc_full);
+                }
                 size_t off = 0;
                 for (int l = 0; l < NM_LAYERS; ++l)
                     for (uint32_t s = 0; s < P.n_slabs[l]; ++s, ++it) {
@@ -203,31 +240,36 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     x.wg = threadIdx.x >> 7; x.t = threadIdx.x & 127; x.lane = lane; x.r0 = 64u * x.wg + tc::frag_row(x.t);
     uint32_t n = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
-        tc::mbar_wait(enc_full, n & 1);
+        if constexpr (LAT) {   // my rows' MMAs of the previous tile are complete; layer 0's fence and barrier publish these writes
+            if (x.t < 64) nm_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
+        } else {
+            tc::mbar_wait(enc_full, n & 1);
+        }
         float alpha[2] = {0.f, 0.f};
-        nm_layers<MIP, 0>(x, P, tile, alpha);
-        // views_linears.0 was the last reader of the encoding blocks: the producer may load the next tile's
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(enc_free);
+        nm_layers<MIP, LAT, 0>(x, P, tile, alpha);
+        if constexpr (!LAT) {
+            // views_linears.0 was the last reader of the encoding blocks: the producer may load the next tile's
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(enc_free);
+        }
     }
 }
 
-static void nm_launch(const void *weight_image, const float *bias, const void *enc_image, int64_t n_rows, int input_ch, int input_ch_dirs, float *raw, cudaStream_t s) {
-    NmParams P{};
-    P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.enc_image = (const uint8_t *)enc_image;
-    P.n_rows = n_rows; P.input_ch = input_ch; P.input_ch_dirs = input_ch_dirs; P.raw = raw;
-    const bool mip = input_ch > 64;
+// P holds the pointers, n_rows and channels (and the lattice when `lattice`); the schedule and the launch shape are filled in here
+static void nm_launch(NmParams &P, bool lattice, cudaStream_t s) {
+    const int64_t n_rows = P.n_rows;
+    const bool mip = P.input_ch > 64;
     uint32_t max_bytes = 0;
     for (int l = 0; l < NM_LAYERS; ++l) {
         const NmLayer L = mip ? nm_layer<true>(l) : nm_layer<false>(l);
-        P.n_slabs[l] = (uint32_t)L.n_slabs;
+        P.n_slabs[l] = lattice && l > 7 ? 0u : (uint32_t)L.n_slabs;   // the lattice stops after pts_linears.7: its stream is a prefix of the image
         for (int k = 0; k < L.n_slabs; ++k) { P.slab_bytes[l][k] = nm_slab_bytes(L.s[k]); if (P.slab_bytes[l][k] > max_bytes) max_bytes = P.slab_bytes[l][k]; }
     }
     P.slot_bytes = (max_bytes + 1023) & ~1023u;
     P.n_slots = 4;
     const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * TILE_BLOCK_BYTES + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
     const int grid = persistent_grid(1, (n_rows + 127) / 128);
-    auto k = mip ? nerf_mlp_wg_kernel<true> : nerf_mlp_wg_kernel<false>;
+    auto k = lattice ? nerf_mlp_wg_kernel<false, true> : mip ? nerf_mlp_wg_kernel<true, false> : nerf_mlp_wg_kernel<false, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);
 }
@@ -249,8 +291,35 @@ int xrb_nerf_mlp_forward(const void *weight_image, const float *bias, const void
     XRB_REQUIRE(weight_image && bias && enc_image && raw, "nerf_mlp_forward: null pointer");
     XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)raw & 15) == 0 && ((uintptr_t)enc_image & 15) == 0 && ((uintptr_t)bias & 15) == 0,
                 "nerf_mlp_forward: images / bias / raw must be 16-byte aligned");
-    nm_launch(weight_image, bias, enc_image, n_rows, input_ch, input_ch_dirs, raw, (cudaStream_t)stream);
+    NmParams P{};
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias; P.enc_image = (const uint8_t *)enc_image;
+    P.n_rows = n_rows; P.input_ch = input_ch; P.input_ch_dirs = input_ch_dirs; P.raw = raw;
+    nm_launch(P, false, (cudaStream_t)stream);
     return check_launch("nerf_mlp_forward");
+}
+
+// the raw alpha of xrb_nerf_mlp_forward at every point of a lattice, the point encoding formed inside the kernel. See include/xrnerf_b200.h.
+int xrb_nerf_density_lattice(const void *weight_image, const float *bias, int input_ch, int multires, int nx, int ny, int nz, const float *box_min_host,
+                             const float *box_max_host, float *out, void *stream) {
+    const int sz = lattice_sizes(nx, ny, nz, "nerf_density_lattice: bad size: every lattice size must be 2..1024");
+    if (sz < 0) return XRB_E_BADARG;
+    if (!(input_ch == 63 && multires == 10)) {
+        set_error("nerf_density_lattice: implemented for the NerfMLP point encoding of the reference configs, input_ch 63 (multires 10)");
+        return XRB_E_UNSUPPORTED;
+    }
+    Box b;
+    const int e = read_box(box_min_host, box_max_host, false, &b, "nerf_density_lattice: the box must be finite with box_min < box_max on every axis");
+    if (e) return e;
+    if (sz == 0) return XRB_OK;
+    XRB_REQUIRE(weight_image && bias && out, "nerf_density_lattice: null pointer");
+    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)bias & 15) == 0 && ((uintptr_t)out & 3) == 0,
+                "nerf_density_lattice: weight image / bias must be 16-byte aligned, out 4-byte aligned");
+    NmParams P{};
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias;
+    P.n_rows = (int64_t)nx * ny * nz; P.input_ch = 63; P.input_ch_dirs = 27; P.raw = out;
+    P.lat_n[0] = nx; P.lat_n[1] = ny; P.lat_n[2] = nz; P.lat_box = b;
+    nm_launch(P, true, (cudaStream_t)stream);
+    return check_launch("nerf_density_lattice");
 }
 
 }  // extern "C"

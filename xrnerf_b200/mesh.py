@@ -5,6 +5,10 @@ the map from the Instant-NGP field's frame back to the dataset's (Blender / NeRF
     write_ply('mesh.ply', ngp_to_nerf(verts), faces)
     verts, faces, normals, colors = network.extract_colored_mesh(resolution=256)
     write_ply('mesh.ply', ngp_to_nerf(verts), faces, ngp_to_nerf_normals(normals), colors)
+
+    verts, faces = nerf_network.extract_mesh(resolution=256)     # NerfNetwork: vertices and normals already in the NeRF world frame
+    verts, faces, normals, colors = nerf_network.extract_colored_mesh(resolution=256)
+    write_ply('mesh.ply', verts, faces, normals, colors)
 """
 import numpy as np
 import torch
@@ -81,19 +85,31 @@ def ngp_to_nerf_normals(normals):
     return torch.as_tensor(normals)[:, [2, 0, 1]]
 
 
-def raw_density_threshold(sigma, activation):
-    """The raw network output whose activated density is sigma (the sampler's density_activation: 0 None, 1 ReLU, 2 Logistic, 3 Exponential):
-    v > raw  <=>  act(v) > sigma. ValueError when sigma is outside the activation's range (or the activation is unknown)."""
+def raw_density_threshold(sigma, activation, density_bias=0.0):
+    """The raw network output whose activated density is sigma (the NGP sampler's density_activation code: 0 None, 1 ReLU, 2 Logistic, 3 Exponential;
+    or NerfRender's density_activation name: 'relu', or 'softplus' with threshold 20 as in the NeRF composite, the library's code 4), the activation
+    applied to raw + density_bias: v > raw  <=>  act(v + density_bias) > sigma. ValueError when sigma is outside the activation's range (or the
+    activation is unknown)."""
     s = float(sigma)
-    act = int(activation)
+    act = {'relu': 1, 'softplus': 4}.get(activation, -1) if isinstance(activation, str) else int(activation)
+    if act == 4 and not isinstance(activation, str):
+        act = -1                                   # the sampler codes stop at 3
     if not np.isfinite(s):
         raise ValueError(f'density threshold must be finite, got {sigma}')
+    return _inverse_density_act(s, act) - float(density_bias)
+
+
+def _inverse_density_act(s, act):
     if act == 0:
         return s
     if act == 1:
         if s < 0:
             raise ValueError(f'a ReLU density is never negative: threshold {s}')
         return s
+    if act == 4:
+        if s <= 0:
+            raise ValueError(f'a softplus density is positive: threshold {s}')
+        return s if s > 20.0 else float(np.log(np.expm1(s)))   # softplus(v) = v above 20
     if act == 2:
         if not 0.0 < s < 1.0:
             raise ValueError(f'a logistic density lies in (0, 1): threshold {s}')
@@ -102,7 +118,7 @@ def raw_density_threshold(sigma, activation):
         if s <= 0:
             raise ValueError(f'an exponential density is positive: threshold {s}')
         return float(np.log(s))
-    raise ValueError(f'unknown density activation {activation}')
+    raise ValueError('unknown density activation')
 
 
 def activate_rgb(raw, activation):

@@ -4,6 +4,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+from .. import _C
 from . import builder
 from .builder import MLPS
 from ..ngp import NgpField, PER_LEVEL_SCALE
@@ -61,6 +62,35 @@ class NerfMLP(BaseMLP):
     def _fused_ok(self, x):
         return (self.fused and not torch.is_grad_enabled() and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4]
                 and self.pts_linears[0].out_features == 256 and (self.input_ch, self.input_ch_dirs) in ((63, 27), (96, 27)))
+
+    def _mesh_check(self, x):
+        """mesh export runs the fused kernels only, for the reference NeRF shape with the positional encoding of multires 10: anything else is an error"""
+        if not (self.fused and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4] and self.pts_linears[0].out_features == 256
+                and (self.input_ch, self.input_ch_dirs) == (63, 27) and getattr(self.embedder, 'multires', None) == 10):
+            raise NotImplementedError('NerfMLP mesh export is implemented for the fused CUDA NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs=True) '
+                                      'with BaseEmbedder(multires=10, multires_dirs=4) on a CUDA device (input channels (63, 27))')
+
+    def density_lattice(self, shape, box):
+        """Raw alpha on the lattice of shape (nz, ny, nx) over box = (box_min, box_max) -> CUDA f32[nz,ny,nx] (x fastest); lattice positions:
+        xrb_nerf_density_lattice (include/xrnerf_b200.h). Each value is bit-identical to the inference raw[:, 3] (nerf_mlp_forward on the
+        xrb_nerf_posenc_tiles encoding of the point)."""
+        w = self.pts_linears[0].weight
+        self._mesh_check(w)
+        nz, ny, nx = (int(n) for n in shape)
+        image, bias = self._packed()
+        out = torch.empty((nz, ny, nx), dtype=torch.float32, device=w.device)
+        _C.check(_C.lib.xrb_nerf_density_lattice(_C.ptr(image), _C.f32(bias), self.input_ch, self.embedder.multires, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
+                                                 _C.f32(out), _C.stream()), 'nerf_density_lattice')
+        return out
+
+    def density_grad(self, pts):
+        """pts f32[n,3] in the frame the rays are given in -> (raw density f32[n], grad f32[n,3] = d(raw alpha)/d(position)). Computed with the training
+        kernels (xrnerf_b200.nerf_train.density_grad: forward with saved activations, then the input gradients from alpha_linear down to the point
+        encoding); that forward's density agrees with the inference kernel's, which density_lattice uses, to the fp16 tolerance, not bit for bit."""
+        self._mesh_check(pts)
+        from .. import nerf_train
+        with torch.no_grad():
+            return nerf_train.density_grad(self, pts.detach().reshape(-1, 3).contiguous().float())
 
     def _packed(self):
         ver = tuple(p._version for p in self.parameters()) + (self.pts_linears[0].weight.device,)

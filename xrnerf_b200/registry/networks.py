@@ -132,6 +132,63 @@ class NerfNetwork(nn.Module):
     def set_val_pipeline(self, func):
         self.val_pipeline = func
 
+    def _mesh_mlp(self):
+        """the network whose output the renderer returns"""
+        return self.mlp_fine if self.N_importance > 0 else self.mlp
+
+    def extract_mesh(self, resolution=256, threshold=50.0, box=((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))):
+        """Triangle mesh of the density level set sigma = threshold -> (verts f32[V,3], faces i32[F,3]) CUDA tensors, in the world frame of the rays,
+        triangles wound counter-clockwise seen from outside. The raw alpha of mlp_fine (mlp when N_importance == 0) is sampled on a resolution^3 lattice
+        spanning `box` (NerfMLP.density_lattice) and meshed by xrnerf_b200.mesh.marching_cubes.
+
+        threshold is a density sigma = act(raw + density_bias) with the renderer's activation (relu or softplus), mapped to raw alpha by
+        mesh.raw_density_threshold (ValueError outside the activation's range). The default of 50 has not been checked here on a trained scene.
+        The default box is the cube the Instant-NGP path's unit cube covers (synth.poses_nerf2ngp: scale 0.33, offset 0.5), so meshes of one scene
+        from both networks cover the same region."""
+        return self._lattice_mesh(resolution, threshold, box)
+
+    def _lattice_mesh(self, resolution, threshold, box):
+        from ..mesh import marching_cubes, raw_density_threshold
+        r = self.render
+        raw = raw_density_threshold(threshold, r.density_activation, r.density_bias)
+        mlp = self._mesh_mlp()
+        mlp.mark_dirty()                       # weights may have been swapped through `.data` (EMAHook) since the last pack
+        with torch.no_grad():
+            vol = mlp.density_lattice((resolution,) * 3, box)
+            return marching_cubes(vol, raw, box)
+
+    def extract_colored_mesh(self, resolution=256, threshold=50.0, box=((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))):
+        """extract_mesh with a unit normal and a colour per vertex -> (verts f32[V,3], faces i32[F,3], normals f32[V,3], colors f32[V,3]) CUDA tensors;
+        verts and faces are bit-identical to extract_mesh(resolution, threshold, box).
+
+        normal = -g / |g| (0 where g = 0), with g the gradient of the raw alpha at the vertex (NerfMLP.density_grad). Inside is "sigma > threshold", so the
+        normal points outward. The gradient comes from the training kernels' forward, the lattice from the inference kernel: the two densities agree to
+        the fp16 tolerance, not bit for bit.
+        color = NerfRender's rgb activation sigmoid(raw[:3]) (1 + 2 rgb_padding) - rgb_padding of the inference kernel at the vertex, with view
+        direction -normal: the surface seen from outside."""
+        verts, faces = self._lattice_mesh(resolution, threshold, box)
+        mlp = self._mesh_mlp()
+        with torch.no_grad():
+            _, g = mlp.density_grad(verts)
+            norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
+            normals = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+            colors = nerf_vertex_colors(mlp, verts, -normals, self.render.rgb_padding)
+            return verts, faces, normals, colors
+
+
+def nerf_vertex_colors(mlp, pts, dirs, rgb_padding):
+    """NerfRender's rgb activation of the fused inference NerfMLP at pts f32[n,3] seen along dirs f32[n,3] (one encoding row per point,
+    xrb_nerf_posenc_tiles with samples_per_ray = 1)"""
+    from ..nerf_mlp import nerf_mlp_forward_tiles
+    n = int(pts.shape[0])
+    emb = mlp.embedder
+    image, bias = mlp._packed()
+    enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(n, mlp.input_ch), dtype=torch.uint8, device=pts.device)
+    p, d = pts.contiguous().float(), dirs.contiguous().float()
+    _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(d), n, 1, emb.multires, emb.multires_dirs, _C.ptr(enc), _C.stream()), 'nerf_posenc_tiles')
+    raw = nerf_mlp_forward_tiles(image, bias, enc, n, mlp.input_ch, mlp.input_ch_dirs)
+    return torch.sigmoid(raw[:, :3]) * (1 + 2 * rgb_padding) - rgb_padding
+
 
 @NETWORKS.register_module()
 class MipNerfNetwork(NerfNetwork):
@@ -139,6 +196,12 @@ class MipNerfNetwork(NerfNetwork):
         super().__init__(cfg, mlp=mlp, render=render)
         self.num_levels, self.resample_padding, self.ray_shape = cfg.num_levels if hasattr(cfg, 'num_levels') else cfg['num_levels'], cfg['resample_padding'], cfg['ray_shape']
         self.use_multiscale, self.coarse_loss_mult = cfg['use_multiscale'], cfg['coarse_loss_mult']
+
+    def extract_mesh(self, *args, **kwargs):
+        raise NotImplementedError('MipNerfNetwork: mesh export is not implemented: the field is defined on conical frusta, and a point query needs a chosen footprint')
+
+    def extract_colored_mesh(self, *args, **kwargs):
+        raise NotImplementedError('MipNerfNetwork: mesh export is not implemented: the field is defined on conical frusta, and a point query needs a chosen footprint')
 
     def forward(self, data, is_test):
         randomized = not is_test
