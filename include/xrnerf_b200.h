@@ -467,6 +467,35 @@ int xrb_nerf_density_lattice(const void *weight_image, const float *bias, int in
                              const float *box_max_host, float *out, void *stream);
 int xrb_nerf_posenc_grad(const float *pts, int64_t n_pts, int multires, const void *d_enc_image, int n_terms, const float *scale, float *grad, void *stream);
 
+/* ---- Mip-NeRF mesh export (csrc/nerf.cu, csrc/nerf_mlp_tc.cu; no reference counterpart). Mip-NeRF's field is defined on Gaussians; a POINT QUERY AT
+ * FOOTPRINT sigma >= 0 is MipNerfEmbedder.integrated_pos_enc with mean p and covariance sigma^2 I (an isotropic Gaussian of standard deviation sigma in
+ * the rays' world frame): for band k = 0 .. max_deg_point - min_deg_point - 1, deg = min_deg_point + k, axis a, with y = p_a 2^deg and
+ * a_k = exp(-0.5 sigma^2 4^deg) (formed once per call, rounded once to fp32), column 3k + a = a_k sin(y) and column 3 n_deg + 3k + a = a_k sin(y + pi/2)
+ * (fp32 y + pi/2, as in the reference). A band whose fp32 0.5 ((sigma^2 2^deg) 2^deg) exceeds 20 is zero, the rule of xrb_mip_ipe_tiles_rays.
+ * Point degrees: 1 <= max - min, 6 (max - min) <= 128, both in [-100, 100]; sigma finite and >= 0. All three entries check sizes, degrees and sigma
+ * before any CUDA call (XRB_E_BADARG), and n == 0 / an empty lattice is a no-op that touches no pointer.
+ *
+ * xrb_mip_ipe_tiles_points: the point query's encoding of pts f32[n_pts,3] at footprint sigma into point blocks 0 and 1 of the tile image, and
+ * MipNerfEmbedder.pos_enc of viewdirs f32[n_pts / samples_per_ray, 3] (identity, then the bands; view degrees 3 + 6 (max - min) <= 64) into block 2, the
+ * values xrb_mip_ipe_tiles_rays writes for a direction: the encoding image xrb_nerf_mlp_forward reads (input_ch 96 when 16 point bands). enc_image
+ * 16-byte aligned, xrb_nerf_enc_image_bytes(n_pts, 96) bytes.
+ *
+ * xrb_mip_density_lattice: out[k][j][i] <- raw[:, 3] of xrb_nerf_mlp_forward (input_ch 96, input_ch_dirs 27; weight_image and bias from
+ * pack_nerf_mlp) on the xrb_mip_ipe_tiles_points encoding at footprint sigma of lattice point (i, j, k), bit for bit; lattice positions and box as for
+ * xrb_nerf_density_lattice. The Mip-NeRF instantiation of the same lattice kernel: it forms each point's IPE in shared memory, so it needs no position
+ * tensor, encoding image or workspace. The box is checked before any CUDA call; weight_image and bias must be 16-byte aligned, out 4-byte aligned.
+ *
+ * xrb_mip_ipe_grad: grad f32[n,3] <- the gradient with respect to the position through the point query's encoding at footprint sigma of pts f32[n,3].
+ * d_enc_image is a tile image of n_terms (1..4) two-block terms per 128-row tile (blocks 2t, 2t + 1 = term t); the gradient with respect to the 6 n_deg
+ * encoding columns is e = (sum of the terms, fp32) / *scale (device float: the staging scale xrb_nerf_tg_pack_draw wrote, scale[1]), and
+ *   grad[i][a] = sum_{live k} a_k 2^deg (cos(y) e[3k + a] + cos(y + pi/2) e[3 n_deg + 3k + a]). d_enc_image must be 16-byte aligned. */
+int xrb_mip_ipe_tiles_points(const float *pts, const float *viewdirs, int64_t n_pts, int samples_per_ray, float sigma, int min_deg_point, int max_deg_point, int min_deg_view,
+                             int max_deg_view, void *enc_image, void *stream);
+int xrb_mip_density_lattice(const void *weight_image, const float *bias, int min_deg_point, int max_deg_point, float sigma, int nx, int ny, int nz,
+                            const float *box_min_host, const float *box_max_host, float *out, void *stream);
+int xrb_mip_ipe_grad(const float *pts, int64_t n_pts, float sigma, int min_deg_point, int max_deg_point, const void *d_enc_image, int n_terms, const float *scale, float *grad,
+                     void *stream);
+
 /* Measurement utility (bench.py's second roofline; no reference counterpart): random reads of 4-, 8- or 32-byte records from a table (L2-resident when
  * it is the size of the fp16 hash table) by SMs x 8 CTAs x 256 threads, `rounds` rounds of 8 independent loads per thread. *loads_issued (host) receives the
  * number of loads of the launch; every 4/8-byte load costs one 32-byte sector, which is what bounds the hash gather. */

@@ -126,6 +126,9 @@ _SIGS = {
     'xrb_mc_emit': (_i, [P, _i, _i, _i, _f, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P, P, P]),
     'xrb_nerf_density_lattice': (_i, [P, P, _i, _i, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P]),
     'xrb_nerf_posenc_grad': (_i, [P, _i64, _i, P, _i, P, P, P]),
+    'xrb_mip_ipe_tiles_points': (_i, [P, P, _i64, _i, _f, _i, _i, _i, _i, P, P]),
+    'xrb_mip_density_lattice': (_i, [P, P, _i, _i, _f, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P]),
+    'xrb_mip_ipe_grad': (_i, [P, _i64, _f, _i, _i, P, _i, P, P, P]),
 }
 
 EXPORTS = sorted(_SIGS)  # every symbol the header declares and the library currently implements

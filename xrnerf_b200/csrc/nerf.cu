@@ -179,7 +179,6 @@ __global__ void __launch_bounds__(PDF_WARPS * 32) sample_pdf_kernel(int n_rays, 
 // `embedded`) and by the generic tile-image kernels, so a tile image holds the fp16 roundings of exactly the fp32 kernels' values. The tile images
 // (tc.cuh layout) are what the NerfMLP kernels TMA-load: per 128-row tile the point-encoding block(s), zero padded to 64 columns each, then the
 // direction block.
-constexpr float HALF_PI = 1.5707963267948966f;
 __device__ __forceinline__ float sel3(const float *a, int i) { return i == 0 ? a[0] : i == 1 ? a[1] : a[2]; }   // keeps a register array out of local memory
 
 // BaseEmbedder (embedders/base.py:26-52), column c of the encoding of x: x_c for c < 3, then per band b: sin(2^b x_a), cos(2^b x_a) for a = 0, 1, 2
@@ -470,6 +469,69 @@ __global__ void __launch_bounds__(256) posenc_grad_kernel(const float *__restric
     }
 }
 
+// Mip-NeRF point query at a footprint (mesh export): ipe_point_bands of pts into point blocks 0 and 1, and MipNerfEmbedder.pos_enc of the view
+// direction into block 2 with the expressions of mip_ipe_tiles_fast_kernel's direction block. thread == (tile, item, row) as in the fast encoders:
+// item 0 = both point blocks of the row, item 1 = the direction block. The degrees are run-time values, so the row is zeroed with 16-byte stores and
+// each column is then stored as fp16 (the rounding of pack_h8).
+__global__ void __launch_bounds__(256) mip_ipe_tiles_points_kernel(const float *__restrict__ pts, const float *__restrict__ viewdirs, int64_t n_rows, int samples_per_ray,
+                                                                   const __grid_constant__ IpeBands B, int min_deg_view, int n_deg_view, uint8_t *__restrict__ image) {
+    const int64_t n_tiles = (n_rows + 127) / 128, total = n_tiles * 256;
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)(idx & 127); const int item = (int)((idx >> 7) & 1); const int64_t tile = idx >> 8;
+        const int64_t row = tile * 128 + r;
+        uint8_t *blk = tile_block(image, tile, 3, item == 0 ? 0 : 2);
+        for (int b = 0; b < (item == 0 ? 2 : 1); ++b)
+#pragma unroll
+            for (int ch = 0; ch < 8; ++ch) st_chunk(blk + b * TILE_BLOCK_BYTES + sw128_offset(r, ch), make_uint4(0u, 0u, 0u, 0u));
+        if (row >= n_rows) continue;
+        auto put = [&](int c, float y) { *reinterpret_cast<__half *>(sw128_elem(blk + (c >> 6) * TILE_BLOCK_BYTES, r, (uint32_t)(c & 63))) = __float2half_rn(y); };
+        if (item == 0) {
+            const float x[3] = {pts[3 * row], pts[3 * row + 1], pts[3 * row + 2]};
+            ipe_point_bands(x, B, put);
+        } else {
+            const int64_t ray = row / samples_per_ray;
+            const float vd[3] = {viewdirs[3 * ray], viewdirs[3 * ray + 1], viewdirs[3 * ray + 2]};
+#pragma unroll
+            for (int a = 0; a < 3; ++a) put(a, vd[a]);
+            for (int q = 0; q < 3 * n_deg_view; ++q) {
+                const float x = sel3(vd, q % 3) * pow2i(q / 3 + min_deg_view);
+                put(3 + q, sinf(x)); put(3 + 3 * n_deg_view + q, sinf(x + HALF_PI));
+            }
+        }
+    }
+}
+
+// The gradient with respect to the position through the point query's IPE (mesh normals of a Mip-NeRF NerfMLP), one thread per point. e is the sum of
+// the n_terms two-block fp16 terms of d_enc (blocks 2t, 2t + 1 of every tile = term t) divided by the staging scale, as in posenc_grad_kernel; with the
+// columns of ipe_point_bands (dead bands are constant zero),
+//   dL/dx_a = sum_{k < n_live} a_k 2^deg (cos(y) e[3k + a] + cos(y + pi/2) e[3 n_deg + 3k + a]),  y = x_a 2^deg, deg = min_deg + k
+// The entries of e are read where they are needed (the columns are run-time values).
+__global__ void __launch_bounds__(256) mip_ipe_grad_kernel(const float *__restrict__ pts, int64_t n_pts, const __grid_constant__ IpeBands B, const uint8_t *__restrict__ d_enc, int n_terms,
+                                                           const float *__restrict__ scale, float *__restrict__ grad) {
+    const float inv = 1.f / *scale;   // a power of two: exact
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)(i & 127);
+        auto e = [&](int c) {
+            float s = 0.f;
+            for (int t = 0; t < n_terms; ++t)
+                s += __half2float(__ldg(reinterpret_cast<const __half *>(sw128_elem(tile_block(const_cast<uint8_t *>(d_enc), i >> 7, 2 * n_terms, 2 * t + (c >> 6)), r, (uint32_t)(c & 63)))));
+            return s * inv;
+        };
+        const float x[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
+        float g[3] = {0.f, 0.f, 0.f};
+        for (int k = 0; k < B.n_live; ++k) {
+            const float sc = pow2i(B.min_deg + k), f = B.fac[k];
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                const float y = x[a] * sc;
+                g[a] += f * sc * (cosf(y) * e(3 * k + a) + cosf(y + HALF_PI) * e(3 * B.n_deg + 3 * k + a));
+            }
+        }
+#pragma unroll
+        for (int a = 0; a < 3; ++a) grad[3 * i + a] = g[a];
+    }
+}
+
 // Mip-NeRF resample_along_rays + sorted_piecewise_constant_pdf (networks/utils/mip.py:146-176, :7-63), randomized=False or
 // caller-supplied jitter: one warp per ray, O(S log S) interval search instead of the reference's [N,S+2,S+1] mask.
 constexpr int MIP_MAX_S = 256;
@@ -735,6 +797,31 @@ int xrb_nerf_posenc_grad(const float *pts, int64_t n_pts, int multires, const vo
     XRB_REQUIRE(pts && d_enc_image && scale && grad && ((uintptr_t)d_enc_image & 15) == 0, "nerf_posenc_grad: null/misaligned pointer");
     posenc_grad_kernel<<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, multires, (const uint8_t *)d_enc_image, n_terms, scale, grad);
     return check_launch("nerf_posenc_grad");
+}
+
+int xrb_mip_ipe_tiles_points(const float *pts, const float *viewdirs, int64_t n_pts, int samples_per_ray, float sigma, int min_deg_point, int max_deg_point, int min_deg_view,
+                             int max_deg_view, void *enc_image, void *stream) {
+    XRB_REQUIRE(n_pts >= 0 && samples_per_ray >= 1 && ipe_point_degrees_ok(min_deg_point, max_deg_point) && max_deg_view >= min_deg_view && min_deg_view >= -100
+                && max_deg_view <= 100 && 3 + 6 * (max_deg_view - min_deg_view) <= 64,
+                "mip_ipe_tiles_points: bad size (point degrees: 6 (max - min) <= 128, view degrees: 3 + 6 (max - min) <= 64, degrees in [-100, 100])");
+    XRB_REQUIRE(std::isfinite(sigma) && sigma >= 0.f, "mip_ipe_tiles_points: the footprint sigma must be finite and >= 0");
+    if (n_pts == 0) return XRB_OK;
+    XRB_REQUIRE(pts && viewdirs && enc_image && ((uintptr_t)enc_image & 15) == 0, "mip_ipe_tiles_points: null/misaligned pointer");
+    mip_ipe_tiles_points_kernel<<<tile_grid(n_pts, 256), 256, 0, (cudaStream_t)stream>>>(pts, viewdirs, n_pts, samples_per_ray, ipe_bands(sigma, min_deg_point, max_deg_point),
+                                                                                          min_deg_view, max_deg_view - min_deg_view, (uint8_t *)enc_image);
+    return check_launch("mip_ipe_tiles_points");
+}
+
+int xrb_mip_ipe_grad(const float *pts, int64_t n_pts, float sigma, int min_deg_point, int max_deg_point, const void *d_enc_image, int n_terms, const float *scale, float *grad,
+                     void *stream) {
+    XRB_REQUIRE(n_pts >= 0 && ipe_point_degrees_ok(min_deg_point, max_deg_point) && n_terms >= 1 && n_terms <= 4,
+                "mip_ipe_grad: bad size (point degrees: 6 (max - min) <= 128 in [-100, 100], n_terms 1..4)");
+    XRB_REQUIRE(std::isfinite(sigma) && sigma >= 0.f, "mip_ipe_grad: the footprint sigma must be finite and >= 0");
+    if (n_pts == 0) return XRB_OK;
+    XRB_REQUIRE(pts && d_enc_image && scale && grad && ((uintptr_t)d_enc_image & 15) == 0, "mip_ipe_grad: null/misaligned pointer");
+    mip_ipe_grad_kernel<<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, ipe_bands(sigma, min_deg_point, max_deg_point),
+                                                                                                (const uint8_t *)d_enc_image, n_terms, scale, grad);
+    return check_launch("mip_ipe_grad");
 }
 
 int xrb_mip_resample(const float *z_vals, const float *weights, const float *u, int n_rays, int n_samples, float resample_padding, float *z_out, void *stream) {

@@ -75,6 +75,7 @@ struct NmParams {
     uint32_t slot_bytes; int n_slots;
     uint32_t n_slabs[NM_LAYERS]; uint32_t slab_bytes[NM_LAYERS][NM_MAX_SLABS];   // the producer's stream (from nm_layer on the host)
     int lat_n[3]; Box lat_box;                                                     // LAT: lattice sizes and box; raw is then out f32[n_rows]
+    IpeBands lat_ipe;                                                              // LAT && MIP: the point query's IPE bands
 };
 
 struct NmCtx {
@@ -190,6 +191,26 @@ __device__ __forceinline__ void nm_lattice_row(const NmParams &P, uint8_t *blk, 
     }
 }
 
+// LAT && MIP: the IPE of lattice point p at the launch's footprint (ipe_point_bands, as xrb_mip_ipe_tiles_points), zero past the last point, as row
+// `row` of the two point-encoding A blocks from `blk` (columns 6 n_deg .. 127 zero). The row is zeroed first, then each column is stored as fp16.
+__device__ __forceinline__ void nm_mip_lattice_row(const NmParams &P, uint8_t *blk, uint32_t row, int64_t p) {
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+        uint8_t *r = blk + b * TILE_BLOCK_BYTES + sw128_row(row);
+#pragma unroll
+        for (int ch = 0; ch < 8; ++ch) st_chunk(r + sw128_chunk(row, ch), make_uint4(0u, 0u, 0u, 0u));
+    }
+    if (p < P.n_rows) {
+        const int idx[3] = {(int)(p % P.lat_n[0]), (int)((p / P.lat_n[0]) % P.lat_n[1]), (int)(p / ((int64_t)P.lat_n[0] * P.lat_n[1]))};
+        float x[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) x[a] = lattice_coord(P.lat_box.lo[a], P.lat_box.hi[a], P.lat_n[a], idx[a]);
+        ipe_point_bands(x, P.lat_ipe, [&](int c, float y) {
+            *reinterpret_cast<__half *>(sw128_elem(blk + (c >> 6) * TILE_BLOCK_BYTES, row, (uint32_t)(c & 63))) = __float2half_rn(y);
+        });
+    }
+}
+
 template <bool MIP, bool LAT>
 __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid_constant__ NmParams P) {
     extern __shared__ uint8_t dyn_smem[];
@@ -241,7 +262,11 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     uint32_t n = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
         if constexpr (LAT) {   // my rows' MMAs of the previous tile are complete; layer 0's fence and barrier publish these writes
-            if (x.t < 64) nm_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
+            if constexpr (MIP) {
+                if (x.t < 64) nm_mip_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
+            } else {
+                if (x.t < 64) nm_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
+            }
         } else {
             tc::mbar_wait(enc_full, n & 1);
         }
@@ -269,7 +294,7 @@ static void nm_launch(NmParams &P, bool lattice, cudaStream_t s) {
     P.n_slots = 4;
     const size_t smem = 1024 + (size_t)(5 + (mip ? 2 : 1)) * TILE_BLOCK_BYTES + (size_t)P.n_slots * P.slot_bytes + 8 * (2 * P.n_slots + 2);
     const int grid = persistent_grid(1, (n_rows + 127) / 128);
-    auto k = lattice ? nerf_mlp_wg_kernel<false, true> : mip ? nerf_mlp_wg_kernel<true, false> : nerf_mlp_wg_kernel<false, false>;
+    auto k = lattice ? (mip ? nerf_mlp_wg_kernel<true, true> : nerf_mlp_wg_kernel<false, true>) : mip ? nerf_mlp_wg_kernel<true, false> : nerf_mlp_wg_kernel<false, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);
 }
@@ -320,6 +345,30 @@ int xrb_nerf_density_lattice(const void *weight_image, const float *bias, int in
     P.lat_n[0] = nx; P.lat_n[1] = ny; P.lat_n[2] = nz; P.lat_box = b;
     nm_launch(P, true, (cudaStream_t)stream);
     return check_launch("nerf_density_lattice");
+}
+
+// the raw alpha of xrb_nerf_mlp_forward (Mip-NeRF layout) at every point of a lattice, on the xrb_mip_ipe_tiles_points encoding at footprint sigma
+// formed inside the kernel. See include/xrnerf_b200.h.
+int xrb_mip_density_lattice(const void *weight_image, const float *bias, int min_deg_point, int max_deg_point, float sigma, int nx, int ny, int nz,
+                            const float *box_min_host, const float *box_max_host, float *out, void *stream) {
+    const int sz = lattice_sizes(nx, ny, nz, "mip_density_lattice: bad size: every lattice size must be 2..1024");
+    if (sz < 0) return XRB_E_BADARG;
+    XRB_REQUIRE(ipe_point_degrees_ok(min_deg_point, max_deg_point), "mip_density_lattice: bad degrees (6 (max - min) <= 128, both in [-100, 100])");
+    XRB_REQUIRE(std::isfinite(sigma) && sigma >= 0.f, "mip_density_lattice: the footprint sigma must be finite and >= 0");
+    Box b;
+    const int e = read_box(box_min_host, box_max_host, false, &b, "mip_density_lattice: the box must be finite with box_min < box_max on every axis");
+    if (e) return e;
+    if (sz == 0) return XRB_OK;
+    XRB_REQUIRE(weight_image && bias && out, "mip_density_lattice: null pointer");
+    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)bias & 15) == 0 && ((uintptr_t)out & 3) == 0,
+                "mip_density_lattice: weight image / bias must be 16-byte aligned, out 4-byte aligned");
+    NmParams P{};
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias;
+    P.n_rows = (int64_t)nx * ny * nz; P.input_ch = 96; P.input_ch_dirs = 27; P.raw = out;
+    P.lat_n[0] = nx; P.lat_n[1] = ny; P.lat_n[2] = nz; P.lat_box = b;
+    P.lat_ipe = ipe_bands(sigma, min_deg_point, max_deg_point);
+    nm_launch(P, true, (cudaStream_t)stream);
+    return check_launch("mip_density_lattice");
 }
 
 }  // extern "C"

@@ -9,6 +9,8 @@ the map from the Instant-NGP field's frame back to the dataset's (Blender / NeRF
     verts, faces = nerf_network.extract_mesh(resolution=256)     # NerfNetwork: vertices and normals already in the NeRF world frame
     verts, faces, normals, colors = nerf_network.extract_colored_mesh(resolution=256)
     write_ply('mesh.ply', verts, faces, normals, colors)
+
+    verts, faces, normals, colors = mip_network.extract_colored_mesh(resolution=256, footprint='cell')   # MipNerfNetwork: a footprint is required
 """
 import numpy as np
 import torch
@@ -83,6 +85,26 @@ def ngp_to_nerf_normals(normals):
     """Normals (directions) of the field's frame in the NeRF world frame: the axis permutation of ngp_to_nerf. Its scale is positive and uniform, so it
     drops out of a unit normal; zero normals stay zero."""
     return torch.as_tensor(normals)[:, [2, 0, 1]]
+
+
+def footprint_sigma(footprint, shape=None, box=None):
+    """The standard deviation sigma of a Mip-NeRF point query (include/xrnerf_b200.h, Mip-NeRF mesh export) -> float. `footprint` is sigma itself,
+    finite and >= 0, in the world frame of the rays; or 'cell': sigma = h / sqrt(12) with h = max over axes of (hi - lo) / (n - 1), the standard
+    deviation of a uniform distribution over one cell of the lattice of shape (nz, ny, nx) over box = (box_min, box_max), so that a mesh sampled at
+    resolution n sees the field filtered at its own spacing. ValueError for a negative or non-finite sigma or an unknown string."""
+    if isinstance(footprint, str):
+        if footprint != 'cell':
+            raise ValueError(f"footprint must be a number sigma >= 0 or 'cell', got {footprint!r}")
+        if shape is None or box is None:
+            raise ValueError("footprint 'cell' needs a lattice: pass the point query's sigma")
+        nz, ny, nx = (int(n) for n in shape)
+        h = max([(float(box[1][a]) - float(box[0][a])) / (n - 1) for a, n in enumerate((nx, ny, nz)) if n >= 2] or [0.0])
+        s = h / np.sqrt(12.0)
+    else:
+        s = float(footprint)
+    if not (0.0 <= s <= float(np.finfo(np.float32).max)):                     # finite as the fp32 the kernels take (NaN fails too)
+        raise ValueError(f'footprint sigma must be finite and >= 0, got {footprint}')
+    return s
 
 
 def raw_density_threshold(sigma, activation, density_bias=0.0):

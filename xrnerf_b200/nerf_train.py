@@ -242,28 +242,38 @@ class NerfMlpTrainFn(torch.autograd.Function):
 GRAD_CHUNK = 1 << 18   # rows per pass of density_grad: about 1.5 GB of tile images
 
 
-def density_grad(mlp, pts, chunk=GRAD_CHUNK):
-    """pts f32[n,3] -> (raw density f32[n], d(raw density)/d(position) f32[n,3]) of a NerfMLP with the positional encoding of input_ch 63, from the
-    training kernels: the forward of pts_linears.0..7 and alpha_linear with saved activations, then d_raw = (0, 0, 0, 1) through alpha_linear and the
-    trunk's input gradients down to the point encoding (the pts_linears.0 term and the point-block term of the skip layer pts_linears.5, ReLU masks of the
-    forward), contracted with the encoding's derivative by xrb_nerf_posenc_grad. feature_linear and the view branch are not run. In chunks of `chunk` rows."""
+def density_grad(mlp, pts, chunk=GRAD_CHUNK, sigma=None):
+    """pts f32[n,3] -> (raw density f32[n], d(raw density)/d(position) f32[n,3]) of a NerfMLP, from the training kernels: the forward of
+    pts_linears.0..7 and alpha_linear with saved activations, then d_raw = (0, 0, 0, 1) through alpha_linear and the trunk's input gradients down to
+    the point encoding (the pts_linears.0 term and the point-block term of the skip layer pts_linears.5, ReLU masks of the forward), contracted with the
+    encoding's derivative. feature_linear and the view branch are not run. In chunks of `chunk` rows.
+
+    BaseEmbedder (input_ch 63, one point block; sigma None): the positional encoding, xrb_nerf_posenc_tiles and xrb_nerf_posenc_grad.
+    MipNerfEmbedder (two point blocks): the point query at footprint `sigma` (include/xrnerf_b200.h), xrb_mip_ipe_tiles_points and xrb_mip_ipe_grad.
+    The staged activation gradients are fp16 at a scale of 2^12: an encoding-gradient entry above about 16 would overflow."""
     dev = pts.device
     n_all = int(pts.shape[0])
     dens = torch.empty(n_all, dtype=torch.float32, device=dev)
     grad = torch.empty((n_all, 3), dtype=torch.float32, device=dev)
+    P = (mlp.input_ch + 63) // 64                                     # point blocks of the encoding
     S = getattr(mlp, '_tg_slabs', None)
     if S is None or S.arena.device != dev:
-        S = mlp._tg_slabs = _Slabs(mlp, 1)
+        S = mlp._tg_slabs = _Slabs(mlp, P)
     S.pack()
     emb = mlp.embedder
+    mip = sigma is not None
     vd = torch.zeros((1, 3), dtype=torch.float32, device=dev)         # any direction: the view branch is not evaluated
     for i0 in range(0, n_all, chunk):
         p = pts[i0:i0 + chunk]
         n = int(p.shape[0])
         nt = (n + 127) // 128
-        enc = Img.new(nt, 2, dev)
-        _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(vd), n, n, emb.multires, emb.multires_dirs, _C.ptr(enc.buf), _C.stream()), 'nerf_posenc_tiles')
-        pts_img = enc.sub(0, 1)
+        enc = Img.new(nt, P + 1, dev)
+        if mip:
+            _C.check(_C.lib.xrb_mip_ipe_tiles_points(_C.f32(p), _C.f32(vd), n, n, float(sigma), emb.min_deg, emb.max_deg, emb.min_deg_view, emb.max_deg_view,
+                                                     _C.ptr(enc.buf), _C.stream()), 'mip_ipe_tiles_points')
+        else:
+            _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(vd), n, n, emb.multires, emb.multires_dirs, _C.ptr(enc.buf), _C.stream()), 'nerf_posenc_tiles')
+        pts_img = enc.sub(0, P)
         H = [Img.new(nt, 4, dev) for _ in range(8)]
         _fwd(n, S, 'pts0', [pts_img], H[0])
         for l in range(1, 8):
@@ -276,18 +286,22 @@ def density_grad(mlp, pts, chunk=GRAD_CHUNK):
         sc = torch.empty(2, dtype=torch.float32, device=dev)
         _C.check(_C.lib.xrb_nerf_tg_pack_draw(_C.ptr(d_raw), n, _C.ptr(z_rgb.buf), _C.ptr(z_alpha.buf), _C.ptr(sc), _C.stream()), 'tg_pack_draw')
         Za, Zb = Img.new(nt, 4, dev), Img.new(nt, 4, dev)
-        d_enc = Img.new(nt, 2, dev)                                   # block 0: through pts_linears.0, block 1: through the skip layer's point block
+        d_enc = Img.new(nt, 2 * P, dev)                               # blocks 0..P-1: through pts_linears.0, P..2P-1: through the skip layer's point blocks
         _dx(n, S, [('alpha', z_alpha)], [0, 1, 2, 3], Za, mask=H[7])
         for l in range(7, 0, -1):
             if (l - 1) in mlp.skips:
-                _dx(n, S, [(f'pts{l}', Za)], [0], d_enc.sub(1, 1))
-                _dx(n, S, [(f'pts{l}', Za)], [1 + k for k in range(4)], Zb, mask=H[l - 1])
+                _dx(n, S, [(f'pts{l}', Za)], list(range(P)), d_enc.sub(P, P))
+                _dx(n, S, [(f'pts{l}', Za)], [P + k for k in range(4)], Zb, mask=H[l - 1])
             else:
                 _dx(n, S, [(f'pts{l}', Za)], [0, 1, 2, 3], Zb, mask=H[l - 1])
             Za, Zb = Zb, Za
-        _dx(n, S, [('pts0', Za)], [0], d_enc.sub(0, 1))
-        _C.check(_C.lib.xrb_nerf_posenc_grad(_C.f32(p), n, emb.multires, _C.ptr(d_enc.buf), 2, C.c_void_p(sc.data_ptr() + 4), _C.f32(grad[i0:i0 + n]), _C.stream()),
-                 'nerf_posenc_grad')
+        _dx(n, S, [('pts0', Za)], list(range(P)), d_enc.sub(0, P))
+        scale = C.c_void_p(sc.data_ptr() + 4)
+        if mip:
+            _C.check(_C.lib.xrb_mip_ipe_grad(_C.f32(p), n, float(sigma), emb.min_deg, emb.max_deg, _C.ptr(d_enc.buf), 2, scale, _C.f32(grad[i0:i0 + n]), _C.stream()),
+                     'mip_ipe_grad')
+        else:
+            _C.check(_C.lib.xrb_nerf_posenc_grad(_C.f32(p), n, emb.multires, _C.ptr(d_enc.buf), 2, scale, _C.f32(grad[i0:i0 + n]), _C.stream()), 'nerf_posenc_grad')
     return dens, grad
 
 

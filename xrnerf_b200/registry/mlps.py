@@ -63,34 +63,67 @@ class NerfMLP(BaseMLP):
         return (self.fused and not torch.is_grad_enabled() and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4]
                 and self.pts_linears[0].out_features == 256 and (self.input_ch, self.input_ch_dirs) in ((63, 27), (96, 27)))
 
-    def _mesh_check(self, x):
-        """mesh export runs the fused kernels only, for the reference NeRF shape with the positional encoding of multires 10: anything else is an error"""
-        if not (self.fused and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4] and self.pts_linears[0].out_features == 256
-                and (self.input_ch, self.input_ch_dirs) == (63, 27) and getattr(self.embedder, 'multires', None) == 10):
-            raise NotImplementedError('NerfMLP mesh export is implemented for the fused CUDA NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs=True) '
-                                      'with BaseEmbedder(multires=10, multires_dirs=4) on a CUDA device (input channels (63, 27))')
+    def _is_mip(self):
+        return hasattr(self.embedder, 'min_deg')
 
-    def density_lattice(self, shape, box):
+    def _mesh_check(self, x):
+        """mesh export runs the fused kernels only, for the reference NeRF shape with the positional encoding of multires 10 (input channels (63, 27)) or
+        the reference Mip-NeRF IPE (point degrees 0..16, view degrees 0..4: (96, 27)): anything else is an error"""
+        e = self.embedder
+        enc_ok = ((self.input_ch, self.input_ch_dirs) == (96, 27) and (e.min_deg, e.max_deg, e.min_deg_view, e.max_deg_view) == (0, 16, 0, 4)) if self._is_mip() else \
+            ((self.input_ch, self.input_ch_dirs) == (63, 27) and getattr(e, 'multires', None) == 10)
+        if not (self.fused and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4] and self.pts_linears[0].out_features == 256
+                and enc_ok):
+            raise NotImplementedError('NerfMLP mesh export is implemented for the fused CUDA NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs=True) '
+                                      'with BaseEmbedder(multires=10, multires_dirs=4) (input channels (63, 27)) or MipNerfEmbedder(min_deg_point=0, '
+                                      'max_deg_point=16, min_deg_view=0, max_deg_view=4) (input channels (96, 27)) on a CUDA device')
+
+    def _footprint(self, footprint, shape=None, box=None):
+        """the point query's sigma (Mip-NeRF), or None (NeRF): a MipNerfEmbedder needs a footprint, a BaseEmbedder takes none"""
+        from ..mesh import footprint_sigma
+        if not self._is_mip():
+            if footprint is not None:
+                raise ValueError('a BaseEmbedder NerfMLP is defined at points: footprint must be None')
+            return None
+        if footprint is None:
+            raise NotImplementedError('a Mip-NeRF field is defined on conical frusta, and a point query needs a chosen footprint: pass footprint=sigma or \'cell\'')
+        return footprint_sigma(footprint, shape, box)
+
+    def density_lattice(self, shape, box, footprint=None):
         """Raw alpha on the lattice of shape (nz, ny, nx) over box = (box_min, box_max) -> CUDA f32[nz,ny,nx] (x fastest); lattice positions:
         xrb_nerf_density_lattice (include/xrnerf_b200.h). Each value is bit-identical to the inference raw[:, 3] (nerf_mlp_forward on the
-        xrb_nerf_posenc_tiles encoding of the point)."""
+        xrb_nerf_posenc_tiles encoding of the point).
+
+        With a MipNerfEmbedder the field is a point query at footprint sigma (xrb_mip_density_lattice: the IPE of the isotropic Gaussian of standard
+        deviation sigma at the point, bit-identical to nerf_mlp_forward on the xrb_mip_ipe_tiles_points encoding): `footprint` is sigma >= 0 in the
+        rays' world frame, or 'cell' (mesh.footprint_sigma: the standard deviation of a uniform distribution over one lattice cell). A BaseEmbedder takes
+        footprint=None."""
         w = self.pts_linears[0].weight
         self._mesh_check(w)
         nz, ny, nx = (int(n) for n in shape)
+        sigma = self._footprint(footprint, (nz, ny, nx), box)
         image, bias = self._packed()
         out = torch.empty((nz, ny, nx), dtype=torch.float32, device=w.device)
-        _C.check(_C.lib.xrb_nerf_density_lattice(_C.ptr(image), _C.f32(bias), self.input_ch, self.embedder.multires, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
-                                                 _C.f32(out), _C.stream()), 'nerf_density_lattice')
+        if sigma is None:
+            _C.check(_C.lib.xrb_nerf_density_lattice(_C.ptr(image), _C.f32(bias), self.input_ch, self.embedder.multires, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
+                                                     _C.f32(out), _C.stream()), 'nerf_density_lattice')
+        else:
+            e = self.embedder
+            _C.check(_C.lib.xrb_mip_density_lattice(_C.ptr(image), _C.f32(bias), e.min_deg, e.max_deg, sigma, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
+                                                    _C.f32(out), _C.stream()), 'mip_density_lattice')
         return out
 
-    def density_grad(self, pts):
+    def density_grad(self, pts, footprint=None):
         """pts f32[n,3] in the frame the rays are given in -> (raw density f32[n], grad f32[n,3] = d(raw alpha)/d(position)). Computed with the training
         kernels (xrnerf_b200.nerf_train.density_grad: forward with saved activations, then the input gradients from alpha_linear down to the point
-        encoding); that forward's density agrees with the inference kernel's, which density_lattice uses, to the fp16 tolerance, not bit for bit."""
+        encoding); that forward's density agrees with the inference kernel's, which density_lattice uses, to the fp16 tolerance, not bit for bit.
+        With a MipNerfEmbedder, `footprint` is the point query's sigma >= 0 (required; 'cell' needs a lattice, so it is not accepted here); a
+        BaseEmbedder takes footprint=None."""
         self._mesh_check(pts)
+        sigma = self._footprint(footprint)
         from .. import nerf_train
         with torch.no_grad():
-            return nerf_train.density_grad(self, pts.detach().reshape(-1, 3).contiguous().float())
+            return nerf_train.density_grad(self, pts.detach().reshape(-1, 3).contiguous().float(), sigma=sigma)
 
     def _packed(self):
         ver = tuple(p._version for p in self.parameters()) + (self.pts_linears[0].weight.device,)

@@ -147,14 +147,15 @@ class NerfNetwork(nn.Module):
         from both networks cover the same region."""
         return self._lattice_mesh(resolution, threshold, box)
 
-    def _lattice_mesh(self, resolution, threshold, box):
+    def _lattice_mesh(self, resolution, threshold, box, sigma=None):
+        """sigma: the Mip-NeRF point query's footprint (None for NeRF)"""
         from ..mesh import marching_cubes, raw_density_threshold
         r = self.render
         raw = raw_density_threshold(threshold, r.density_activation, r.density_bias)
         mlp = self._mesh_mlp()
         mlp.mark_dirty()                       # weights may have been swapped through `.data` (EMAHook) since the last pack
         with torch.no_grad():
-            vol = mlp.density_lattice((resolution,) * 3, box)
+            vol = mlp.density_lattice((resolution,) * 3, box, sigma)
             return marching_cubes(vol, raw, box)
 
     def extract_colored_mesh(self, resolution=256, threshold=50.0, box=((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))):
@@ -166,26 +167,33 @@ class NerfNetwork(nn.Module):
         the fp16 tolerance, not bit for bit.
         color = NerfRender's rgb activation sigmoid(raw[:3]) (1 + 2 rgb_padding) - rgb_padding of the inference kernel at the vertex, with view
         direction -normal: the surface seen from outside."""
-        verts, faces = self._lattice_mesh(resolution, threshold, box)
+        return self._colored_lattice_mesh(resolution, threshold, box)
+
+    def _colored_lattice_mesh(self, resolution, threshold, box, sigma=None):
+        verts, faces = self._lattice_mesh(resolution, threshold, box, sigma)
         mlp = self._mesh_mlp()
         with torch.no_grad():
-            _, g = mlp.density_grad(verts)
+            _, g = mlp.density_grad(verts, sigma)
             norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
             normals = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
-            colors = nerf_vertex_colors(mlp, verts, -normals, self.render.rgb_padding)
+            colors = nerf_vertex_colors(mlp, verts, -normals, self.render.rgb_padding, sigma)
             return verts, faces, normals, colors
 
 
-def nerf_vertex_colors(mlp, pts, dirs, rgb_padding):
-    """NerfRender's rgb activation of the fused inference NerfMLP at pts f32[n,3] seen along dirs f32[n,3] (one encoding row per point,
-    xrb_nerf_posenc_tiles with samples_per_ray = 1)"""
+def nerf_vertex_colors(mlp, pts, dirs, rgb_padding, sigma=None):
+    """NerfRender's rgb activation of the fused inference NerfMLP at pts f32[n,3] seen along dirs f32[n,3] (one encoding row per point: BaseEmbedder
+    xrb_nerf_posenc_tiles, MipNerfEmbedder the point query at footprint sigma, xrb_mip_ipe_tiles_points, with samples_per_ray = 1)"""
     from ..nerf_mlp import nerf_mlp_forward_tiles
     n = int(pts.shape[0])
     emb = mlp.embedder
     image, bias = mlp._packed()
     enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(n, mlp.input_ch), dtype=torch.uint8, device=pts.device)
     p, d = pts.contiguous().float(), dirs.contiguous().float()
-    _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(d), n, 1, emb.multires, emb.multires_dirs, _C.ptr(enc), _C.stream()), 'nerf_posenc_tiles')
+    if sigma is None:
+        _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(d), n, 1, emb.multires, emb.multires_dirs, _C.ptr(enc), _C.stream()), 'nerf_posenc_tiles')
+    else:
+        _C.check(_C.lib.xrb_mip_ipe_tiles_points(_C.f32(p), _C.f32(d), n, 1, float(sigma), emb.min_deg, emb.max_deg, emb.min_deg_view, emb.max_deg_view, _C.ptr(enc),
+                                                 _C.stream()), 'mip_ipe_tiles_points')
     raw = nerf_mlp_forward_tiles(image, bias, enc, n, mlp.input_ch, mlp.input_ch_dirs)
     return torch.sigmoid(raw[:, :3]) * (1 + 2 * rgb_padding) - rgb_padding
 
@@ -197,11 +205,41 @@ class MipNerfNetwork(NerfNetwork):
         self.num_levels, self.resample_padding, self.ray_shape = cfg.num_levels if hasattr(cfg, 'num_levels') else cfg['num_levels'], cfg['resample_padding'], cfg['ray_shape']
         self.use_multiscale, self.coarse_loss_mult = cfg['use_multiscale'], cfg['coarse_loss_mult']
 
-    def extract_mesh(self, *args, **kwargs):
-        raise NotImplementedError('MipNerfNetwork: mesh export is not implemented: the field is defined on conical frusta, and a point query needs a chosen footprint')
+    _NO_FOOTPRINT = "MipNerfNetwork: the field is defined on conical frusta, and a point query needs a chosen footprint: pass footprint=sigma or 'cell'"
 
-    def extract_colored_mesh(self, *args, **kwargs):
-        raise NotImplementedError('MipNerfNetwork: mesh export is not implemented: the field is defined on conical frusta, and a point query needs a chosen footprint')
+    def _mesh_mlp(self):
+        """one MLP serves every level"""
+        return self.mlp
+
+    def extract_mesh(self, resolution=256, threshold=50.0, box=((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5)), footprint=None):
+        """Triangle mesh of the density level set sigma_density = threshold of the point query at `footprint` -> (verts f32[V,3], faces i32[F,3]) CUDA
+        tensors, in the world frame of the rays, triangles wound counter-clockwise seen from outside: NerfMLP.density_lattice (xrb_mip_density_lattice)
+        on a resolution^3 lattice spanning `box`, meshed by xrnerf_b200.mesh.marching_cubes.
+
+        Mip-NeRF's field is defined on conical frusta, so a point query needs a footprint: the isotropic Gaussian of standard deviation sigma around the
+        point, encoded by the IPE (include/xrnerf_b200.h). footprint = sigma >= 0 in the rays' world frame, or 'cell': sigma = h / sqrt(12) for the
+        lattice spacing h = max over axes (hi - lo) / (resolution - 1), the standard deviation of a uniform distribution over one cell, so the mesh sees
+        the field filtered at its own spacing. footprint=None raises NotImplementedError; a negative or non-finite sigma or an unknown string raises
+        ValueError. Neither the 'cell' default nor the threshold of 50 has been checked here on a trained scene.
+
+        threshold is a density act(raw + density_bias) with the renderer's activation (the reference config: softplus, density_bias = -1), mapped to raw
+        alpha by mesh.raw_density_threshold (ValueError outside the activation's range)."""
+        if footprint is None:
+            raise NotImplementedError(self._NO_FOOTPRINT)
+        from ..mesh import footprint_sigma
+        return self._lattice_mesh(resolution, threshold, box, footprint_sigma(footprint, (resolution,) * 3, box))
+
+    def extract_colored_mesh(self, resolution=256, threshold=50.0, box=((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5)), footprint=None):
+        """extract_mesh with a unit normal and a colour per vertex -> (verts, faces, normals, colors) CUDA tensors; verts and faces are bit-identical to
+        extract_mesh(resolution, threshold, box, footprint). One sigma serves the lattice, the gradient and the colours.
+
+        normal = -g / |g| (0 where g = 0), g the gradient of the point query's raw alpha at the vertex (NerfMLP.density_grad at the same sigma); it
+        points outward. color = the renderer's sigmoid(raw[:3]) (1 + 2 rgb_padding) - rgb_padding of the inference kernel on the point query at the
+        vertex, with view direction -normal."""
+        if footprint is None:
+            raise NotImplementedError(self._NO_FOOTPRINT)
+        from ..mesh import footprint_sigma
+        return self._colored_lattice_mesh(resolution, threshold, box, footprint_sigma(footprint, (resolution,) * 3, box))
 
     def forward(self, data, is_test):
         randomized = not is_test
