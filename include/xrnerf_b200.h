@@ -308,6 +308,12 @@ int xrb_ngp_render_fused_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *t
 int xrb_nerf_composite_forward(const float *raw, const float *z_vals, const float *rays_d, int n_rays, int n_samples, int mip,
                                int white_bkgd, float rgb_padding, float density_bias, int density_act, float *rgb, float *disp,
                                float *acc, float *weights, void *stream);
+/* The same forward, also writing depth f32[N] = sum_k w_k z_k (the interval mid-points (z_k + z_{k+1})/2 when mip), not divided by acc (the
+ * convention of xrb_ngp_render_depth): the value disp is formed from. rgb, disp, acc and weights are bit-identical to xrb_nerf_composite_forward's.
+ * Arguments are checked as there; a NULL depth is XRB_E_BADARG. */
+int xrb_nerf_composite_forward_depth(const float *raw, const float *z_vals, const float *rays_d, int n_rays, int n_samples, int mip,
+                                     int white_bkgd, float rgb_padding, float density_bias, int density_act, float *rgb, float *disp,
+                                     float *acc, float *weights, float *depth, void *stream);
 /* backward wrt raw of rgb (grad_rgb f32[N,3]); disp/acc/weights are treated as non-differentiated outputs
  * exactly as the reference's losses use them (nerf.py:79-84: loss on rgb only). */
 int xrb_nerf_composite_backward(const float *raw, const float *z_vals, const float *rays_d, const float *grad_rgb, int n_rays,

@@ -96,7 +96,8 @@ _SIGS = {
     'xrb_ngp_render_fused_workspace': (_sz, []),
     'xrb_ngp_render_fused': (_i, [_cfg, _tab, P, P, P, P, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P]),
     'xrb_nerf_composite_forward': (_i, [P, P, P, _i, _i, _i, _i, _f, _f, _i, P, P, P, P, P]),
-    'xrb_nerf_composite_backward': (_i, [P, P, P, P, _i, _i, _i, _i, _f, _f, _i, P, P]),
+    'xrb_nerf_composite_forward_depth': (_i, [P, P, P, _i, _i, _i, _i, _f, _f, _i, P, P, P, P, P, P]),
+    'xrb_nerf_composite_backward':(_i, [P, P, P, P, _i, _i, _i, _i, _f, _f, _i, P, P]),
     'xrb_nerf_sample_pdf': (_i, [P, P, P, P, P, _i, _i, _i, P, P, P]),
     'xrb_nerf_posenc': (_i, [P, P, _i64, _i, _i, _i, P, P]),
     'xrb_nerf_mlp_forward': (_i, [P, P, P, _i64, _i, _i, P, P]),

@@ -32,11 +32,13 @@ __device__ __forceinline__ float transmittance(bool mip, bool valid, float sd, f
     return T;
 }
 
-// BACKWARD == false: rgb/disp/acc/weights.  BACKWARD == true: d_raw given grad_rgb (loss on rgb only, nerf.py:79-84 / mipnerf.py:49-57)
-template <bool BACKWARD>
+// BACKWARD == false: rgb/disp/acc/weights, plus depth_out = sum of w * z (interval mid-points when mip) when DEPTH.
+// BACKWARD == true: d_raw given grad_rgb (loss on rgb only, nerf.py:79-84 / mipnerf.py:49-57)
+template <bool BACKWARD, bool DEPTH = false>
 __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, const float *__restrict__ raw, const float *__restrict__ z_vals, const float *__restrict__ rays_d,
                                                              const float *__restrict__ grad_rgb, float *__restrict__ rgb_out, float *__restrict__ disp_out, float *__restrict__ acc_out,
-                                                             float *__restrict__ weights_out, float *__restrict__ d_raw) {
+                                                             float *__restrict__ weights_out, float *__restrict__ d_raw, float *__restrict__ depth_out) {
+    static_assert(!(BACKWARD && DEPTH), "depth is a forward output");
     const int lane = threadIdx.x & 31;
     const int ray = (blockIdx.x * 256 + threadIdx.x) >> 5;
     if (ray >= p.n_rays) return;
@@ -71,6 +73,7 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
             if (p.white_bkgd) { ax += 1.f - acc; ay += 1.f - acc; az += 1.f - acc; }
             rgb_out[3 * (size_t)ray] = ax; rgb_out[3 * (size_t)ray + 1] = ay; rgb_out[3 * (size_t)ray + 2] = az;
             acc_out[ray] = acc;
+            if (DEPTH) depth_out[ray] = depth;
             float q = depth / acc, disp;
             if (p.mip) { if (isnan(q)) q = INFINITY; disp = fmaxf(fminf(q, z[S]), z[0]); }          // mipnerf_render.py:18-24
             else disp = 1.f / fmaxf(1e-10f, q);                                                       // nerf_render.py:32-36 (torch.max propagates NaN)
@@ -685,8 +688,19 @@ int xrb_nerf_composite_forward(const float *raw, const float *z_vals, const floa
     XRB_REQUIRE(rgb && disp && acc && weights, "nerf_composite_forward: null output");
     CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
     int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
-    nerf_composite_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr);
+    nerf_composite_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, nullptr);
     return check_launch("nerf_composite_forward");
+}
+
+int xrb_nerf_composite_forward_depth(const float *raw, const float *z_vals, const float *rays_d, int n_rays, int n_samples, int mip, int white_bkgd, float rgb_padding,
+                                     float density_bias, int density_act, float *rgb, float *disp, float *acc, float *weights, float *depth, void *stream) {
+    int e = composite_args_ok(raw, z_vals, rays_d, n_rays, n_samples, density_act); if (e) return e;
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(rgb && disp && acc && weights && depth, "nerf_composite_forward_depth: null output");
+    CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
+    int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
+    nerf_composite_kernel<false, true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, depth);
+    return check_launch("nerf_composite_forward_depth");
 }
 
 int xrb_nerf_composite_backward(const float *raw, const float *z_vals, const float *rays_d, const float *grad_rgb, int n_rays, int n_samples, int mip, int white_bkgd, float rgb_padding,
@@ -696,7 +710,7 @@ int xrb_nerf_composite_backward(const float *raw, const float *z_vals, const flo
     XRB_REQUIRE(grad_rgb && d_raw && ((uintptr_t)d_raw & 15) == 0, "nerf_composite_backward: null/misaligned pointer");
     CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
     int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
-    nerf_composite_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, grad_rgb, nullptr, nullptr, nullptr, nullptr, d_raw);
+    nerf_composite_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, grad_rgb, nullptr, nullptr, nullptr, nullptr, d_raw, nullptr);
     return check_launch("nerf_composite_backward");
 }
 

@@ -96,6 +96,32 @@ class NerfNetwork(nn.Module):
         return ret
 
     def batchify_forward(self, data, is_test=False):
+        """Inference over a whole ray set. With is_test, `fused_inference` (default True), rays on CUDA and the fused NerfMLP shape (NerfMLP._fused_ok),
+        the rays go through the fused renderer (xrnerf_b200.nerf.NerfRenderer; MipNerfRenderer for Mip-NeRF) in ray batches of bounded size, on the
+        pipeline's data['z_vals'] (the reference Blender configs' linspace(2, 6) when absent) and, for Mip-NeRF, data['radii']. That path also returns
+        each ray's `depth` [n,1] (sum of w * z, not divided by acc; `coarse_depth` for the coarse level); `fused_ray_batch` sets its rays per batch
+        (None: xrnerf_b200.nerf.ray_batch_size). Training, `fused_inference = False` and other shapes run the reference's chunk loop over forward()
+        (nerf.py:50-69), which returns the reference's keys only."""
+        if is_test and getattr(self, 'fused_inference', True) and self._fused_ok(data['rays_o']):
+            return self._fused_forward(data)
+        return self._chunked_forward(data, is_test)
+
+    def _fused_mlps(self):
+        return [self.mlp] + ([self.mlp_fine] if getattr(self, 'N_importance', 0) > 0 else [])
+
+    def _fused_ok(self, x):
+        """the fused renderer serves this network: CUDA rays, NerfMLPs of the fused shape with the encoding the renderer forms (BaseEmbedder (63, 27) for
+        NeRF, MipNerfEmbedder (96, 27) for Mip-NeRF), and the matching composite"""
+        mip, mlps = isinstance(self, MipNerfNetwork), self._fused_mlps()
+        return (x.is_cuda and bool(mlps) and getattr(self.render, 'mip', None) == mip
+                and all(hasattr(m, '_fused_ok') and m._fused_ok(x) and m._is_mip() == mip for m in mlps))
+
+    def _fused_forward(self, data):
+        from ..nerf import NerfRenderer
+        r = NerfRenderer(self, ray_batch=getattr(self, 'fused_ray_batch', None))
+        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], z_vals=data.get('z_vals'), depth=True)
+
+    def _chunked_forward(self, data, is_test):
         N = data[self.bs_data].shape[0]
         all_ret = {}
         for i in range(0, N, self.chunk):
@@ -115,19 +141,55 @@ class NerfNetwork(nn.Module):
             loss = loss + img2mse(ret['coarse_rgb'], data['target_s'])
         return {'loss': loss, 'log_vars': {'loss': loss.item(), 'psnr': psnr.item()}, 'num_samples': ret['rgb'].shape[0]}
 
-    def val_step(self, data, optimizer=None, **kwargs):
-        """Renders data['poses'] through the installed val pipeline (rank 0 only in the reference; here every rank renders what it is given)."""
-        data = {k: unfold_batching(v) for k, v in data.items()}
+    def _mark_dirty(self):
         for m in (getattr(self, 'mlp', None), getattr(self, 'mlp_fine', None)):
             if m is not None and hasattr(m, 'mark_dirty'):
                 m.mark_dirty()                      # weights may have been swapped through `.data` (EMAHook) since the last pack
-        rgbs = []
+
+    def val_step(self, data, optimizer=None, **kwargs):
+        """nerf.py:94-142: phase 'test' dispatches to test_step. Otherwise renders data['poses'] and, when given, data['spiral_poses'] through the
+        installed val pipeline (rank 0 only in the reference; here every rank renders what it is given). Returns the reference's keys as device tensors:
+        rgbs [H,W,3] and disps [H,W,1] per pose, gt_imgs (data['images'] per pose, when given), spiral_rgbs / spiral_disps, elapsed_time per pose in
+        seconds (pipeline + render, CUDA events); plus psnr per pose, taken on the device against images[..., :3]."""
+        if self.phase == 'test':
+            return self.test_step(data, **kwargs)
+        self._mark_dirty()
+        data = {k: unfold_batching(v) for k, v in data.items()}
+        poses, images, spiral = data['poses'], data.get('images'), data.get('spiral_poses')
+        rgbs, disps, gt_imgs, psnrs, elapsed, spiral_rgbs, spiral_disps = [], [], [], [], [], [], []
         with torch.no_grad():
-            for i in range(data['poses'].shape[0]):
-                d = self.val_pipeline({'pose': data['poses'][i], 'idx': i})
+            for i in range(poses.shape[0]):
+                t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                t0.record()
+                d = self.val_pipeline({'pose': poses[i], 'idx': i})
                 ret = self.batchify_forward(d, is_test=True)
-                rgbs.append(recover_shape(ret['rgb'], d['src_shape']))
-        return {'rgbs': rgbs}
+                rgb = recover_shape(ret['rgb'], d['src_shape'])
+                t1.record()
+                rgbs.append(rgb); disps.append(recover_shape(ret['disp'], d['src_shape'])); elapsed.append((t0, t1))
+                if images is not None:
+                    gt = images[i].to(rgb.device)
+                    gt_imgs.append(gt)
+                    psnrs.append(mse2psnr(img2mse(rgb, gt[..., :3])))
+            for i in range(0 if spiral is None else spiral.shape[0]):
+                d = self.val_pipeline({'pose': spiral[i], 'idx': i})
+                ret = self.batchify_forward(d, is_test=True)
+                spiral_rgbs.append(recover_shape(ret['rgb'], d['src_shape'])); spiral_disps.append(recover_shape(ret['disp'], d['src_shape']))
+        torch.cuda.synchronize()
+        return {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'spiral_rgbs': spiral_rgbs, 'spiral_disps': spiral_disps,
+                'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+
+    def test_step(self, data, **kwargs):
+        """nerf.py:144-169: one test pose (data['pose'], data['image'], data['idx']) through the installed val pipeline -> rgb [H,W,3], disp [H,W,1],
+        gt_img (data['image'] on the render's device) and idx (an int)."""
+        self._mark_dirty()
+        data = {k: unfold_batching(v) for k, v in data.items()}
+        idx = data['idx']
+        idx = int(idx.item()) if torch.is_tensor(idx) else int(idx)
+        with torch.no_grad():
+            d = self.val_pipeline({'pose': data['pose'], 'idx': idx})
+            ret = self.batchify_forward(d, is_test=True)
+        rgb = recover_shape(ret['rgb'], d['src_shape'])
+        return {'rgb': rgb, 'disp': recover_shape(ret['disp'], d['src_shape']), 'gt_img': data['image'].to(rgb.device), 'idx': idx}
 
     def set_val_pipeline(self, func):
         self.val_pipeline = func
@@ -241,6 +303,37 @@ class MipNerfNetwork(NerfNetwork):
         from ..mesh import footprint_sigma
         return self._colored_lattice_mesh(resolution, threshold, box, footprint_sigma(footprint, (resolution,) * 3, box))
 
+    def _fused_mlps(self):
+        return [self.mlp] if self.ray_shape == 'cone' else []      # resample_along_rays implements the cone
+
+    def _fused_forward(self, data):
+        from ..nerf import MipNerfRenderer
+        r = MipNerfRenderer(self, ray_batch=getattr(self, 'fused_ray_batch', None))
+        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], data['radii'], z_vals=data.get('z_vals'), depth=True)
+
+    def val_step(self, data, optimizer=None, **kwargs):
+        """mipnerf.py:76-98: without use_multiscale NerfNetwork.val_step. With it, one pixel-shaped view through evaluate_once: phase 'test' returns
+        rgb [H,W,3], gt_img, disp [H,W,1] and idx; validation returns rgbs, gt_imgs and disps as one-element lists. Device tensors throughout."""
+        if not self.use_multiscale:
+            return super().val_step(data, optimizer, **kwargs)
+        rgb, image, disp, idx = self.evaluate_once(data, **kwargs)
+        if self.phase == 'test':
+            return {'rgb': rgb, 'gt_img': image, 'disp': disp, 'idx': idx}
+        return {'rgbs': [rgb], 'gt_imgs': [image], 'disps': [disp]}
+
+    def evaluate_once(self, data, **kwargs):
+        """mipnerf.py:100-117: data holds one view's per-pixel rays [1,H,W,...] (rays_o, rays_d, viewdirs, radii, z_vals, ..., image) and idx; every
+        tensor is flattened to [H*W, -1] float32 rows and rendered by batchify_forward(is_test=True) -> (rgb [H,W,3], image [H,W,C], disp [H,W,1], idx)"""
+        self._mark_dirty()
+        H, W = data['image'].shape[1:3]
+        idx = data['idx']
+        idx = int(idx.item()) if torch.is_tensor(idx) else int(idx)
+        rays = {k: v.squeeze(0).reshape(H * W, -1).to(torch.float32) for k, v in data.items() if k != 'idx' and torch.is_tensor(v)}
+        with torch.no_grad():
+            ret = self.batchify_forward(rays, is_test=True)
+        rgb = ret['rgb'].reshape((H, W, -1))
+        return rgb, rays['image'].reshape((H, W, -1)).to(rgb.device), ret['disp'].reshape((H, W, -1)), idx
+
     def forward(self, data, is_test):
         randomized = not is_test
         ret = {}
@@ -285,7 +378,7 @@ class HashNerfNetwork(NerfNetwork):
         alpha == 0); the reference-shaped path returns the reference's keys only."""
         smp = self.sampler
         if not (is_test and getattr(self, 'fused_inference', True) and data['rays_o'].is_cuda and hasattr(smp, 'aabb_range')):
-            return super().batchify_forward(data, is_test)
+            return self._chunked_forward(data, is_test)
         from ..ngp import NgpRenderer, disparity
         smp.check_device(data)
         r = getattr(self, '_renderer', None)
