@@ -1,5 +1,6 @@
-// xrnerf_b200 — the density lattice shared by the mesh-export entry points (xrb_ngp_density_lattice, xrb_nerf_density_lattice, xrb_mc_emit):
-// the position of a lattice point and the checks of the lattice sizes and box. The contract is in include/xrnerf_b200.h (mesh section).
+// xrnerf_b200 — the density lattice shared by the mesh-export entry points (xrb_ngp_density_lattice, xrb_nerf_density_lattice,
+// xrb_mip_density_lattice, xrb_mc_count, xrb_mc_emit): a lattice point's coordinates and position, and the checks of the lattice sizes and box.
+// The contract is in include/xrnerf_b200.h (mesh section).
 #pragma once
 #include <cmath>
 
@@ -12,6 +13,25 @@ namespace xrb {
 __device__ __forceinline__ float lattice_coord(float lo, float hi, int n, int i) { return fminf(add_(lo, mul_((float)i, div_(sub_(hi, lo), (float)(n - 1)))), hi); }
 
 struct Box { float lo[3], hi[3]; };
+
+// n[0] x n[1] x n[2] points over `box`, point index p = x + n[0] (y + n[1] z)
+struct Lattice {
+    int n[3];
+    int64_t nxy, points;
+    Box box;
+    __device__ void coords(int64_t p, int idx[3]) const { idx[0] = (int)(p % n[0]); idx[1] = (int)((p / n[0]) % n[1]); idx[2] = (int)(p / nxy); }
+    __device__ float coord(int a, int i) const { return lattice_coord(box.lo[a], box.hi[a], n[a], i); }
+    __device__ void position(int64_t p, float x[3]) const {
+        int idx[3]; coords(p, idx);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) x[a] = coord(a, idx[a]);
+    }
+    __device__ int64_t stride(int axis) const { return axis == 0 ? 1 : axis == 1 ? (int64_t)n[0] : nxy; }
+};
+static inline Lattice make_lattice(int nx, int ny, int nz, const Box &b = Box{}) {
+    Lattice L{{nx, ny, nz}, (int64_t)nx * ny, (int64_t)nx * ny * nz, b};
+    return L;
+}
 
 // 0: an empty lattice (some size 0); 1: every size in [2, 1024]; -1: otherwise (the error is set)
 static inline int lattice_sizes(int nx, int ny, int nz, const char *who) {

@@ -20,14 +20,10 @@ namespace xrb {
 // ---------------------------------------------------------------------------------------------------------------- density on a lattice
 // positions of `n` consecutive lattice points from `first` (x fastest) as the field's [n,3] rows
 constexpr int LATTICE_CHUNK = 1 << 20;
-__global__ void __launch_bounds__(256) lattice_points_kernel(int64_t first, int n, int nx, int ny, int nz, Box b, float *__restrict__ pts) {
+__global__ void __launch_bounds__(256) lattice_points_kernel(int64_t first, int n, Lattice L, float *__restrict__ pts) {
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
-    const int64_t p = first + i;
-    const int x = (int)(p % nx), y = (int)((p / nx) % ny), z = (int)(p / ((int64_t)nx * ny));
-    pts[3 * (size_t)i] = lattice_coord(b.lo[0], b.hi[0], nx, x);
-    pts[3 * (size_t)i + 1] = lattice_coord(b.lo[1], b.hi[1], ny, y);
-    pts[3 * (size_t)i + 2] = lattice_coord(b.lo[2], b.hi[2], nz, z);
+    L.position(first + i, pts + 3 * (size_t)i);
 }
 
 // ---------------------------------------------------------------------------------------------------------------- marching cubes
@@ -47,18 +43,11 @@ inline McWs mc_ws(void *ws, int64_t points) {
     return w;
 }
 
-struct Lattice {
-    int nx, ny, nz;
-    int64_t nxy, points;
-    __device__ void coords(int64_t p, int &x, int &y, int &z) const { x = (int)(p % nx); y = (int)((p / nx) % ny); z = (int)(p / nxy); }
-    __device__ int64_t stride(int axis) const { return axis == 0 ? 1 : axis == 1 ? (int64_t)nx : nxy; }
-};
-
 // case index of the cell whose lowest corner is p (corner c at p + (c & 1, c >> 1 & 1, c >> 2 & 1))
 __device__ __forceinline__ uint32_t cell_case(const float *__restrict__ vol, const Lattice &L, int64_t p, float thr) {
     uint32_t c = 0;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) c |= (uint32_t)(__ldg(vol + p + (k & 1) + ((k >> 1) & 1) * (int64_t)L.nx + ((k >> 2) & 1) * L.nxy) > thr) << k;
+    for (int k = 0; k < 8; ++k) c |= (uint32_t)(__ldg(vol + p + (k & 1) + ((k >> 1) & 1) * (int64_t)L.n[0] + ((k >> 2) & 1) * L.nxy) > thr) << k;
     return c;
 }
 
@@ -67,12 +56,12 @@ __global__ void __launch_bounds__(MC_BLOCK) mc_count_kernel(const float *__restr
     const int64_t p = (int64_t)blockIdx.x * MC_BLOCK + threadIdx.x;
     uint32_t mask = 0, nt = 0;
     if (p < L.points) {
-        int x, y, z; L.coords(p, x, y, z);
+        int idx[3]; L.coords(p, idx);
         const bool in0 = __ldg(vol + p) > thr;
-        if (x + 1 < L.nx) mask |= (uint32_t)(in0 != (__ldg(vol + p + 1) > thr));
-        if (y + 1 < L.ny) mask |= (uint32_t)(in0 != (__ldg(vol + p + L.nx) > thr)) << 1;
-        if (z + 1 < L.nz) mask |= (uint32_t)(in0 != (__ldg(vol + p + L.nxy) > thr)) << 2;
-        if (x + 1 < L.nx && y + 1 < L.ny && z + 1 < L.nz) nt = MC_TRI_COUNT[cell_case(vol, L, p, thr)];
+        if (idx[0] + 1 < L.n[0]) mask |= (uint32_t)(in0 != (__ldg(vol + p + 1) > thr));
+        if (idx[1] + 1 < L.n[1]) mask |= (uint32_t)(in0 != (__ldg(vol + p + L.n[0]) > thr)) << 1;
+        if (idx[2] + 1 < L.n[2]) mask |= (uint32_t)(in0 != (__ldg(vol + p + L.nxy) > thr)) << 2;
+        if (idx[0] + 1 < L.n[0] && idx[1] + 1 < L.n[1] && idx[2] + 1 < L.n[2]) nt = MC_TRI_COUNT[cell_case(vol, L, p, thr)];
     }
     uint32_t vtot, ftot;
     const uint32_t vex = block_excl_scan<MC_BLOCK>(__popc(mask), &vtot);
@@ -122,20 +111,19 @@ __device__ __forceinline__ int32_t owned_vertex(const uint32_t *__restrict__ wor
     return (int32_t)(__ldg(vblock + q / MC_BLOCK) + (w & MC_OFF_MASK) + __popc((w >> MC_CROSS_SHIFT) & ((1u << axis) - 1u)));
 }
 
-__global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restrict__ vol, Lattice L, float thr, Box b, const uint32_t *__restrict__ word,
+__global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restrict__ vol, Lattice L, float thr, const uint32_t *__restrict__ word,
                                                            const uint32_t *__restrict__ vblock, const uint32_t *__restrict__ fblock, const uint32_t *__restrict__ misc,
                                                            float *__restrict__ verts, int32_t *__restrict__ faces) {
     if (misc[2]) return;
     const int64_t p = (int64_t)blockIdx.x * MC_BLOCK + threadIdx.x;
     uint32_t nt = 0, cs = 0;
     if (p < L.points) {
-        int x, y, z; L.coords(p, x, y, z);
-        const int idx[3] = {x, y, z}, n[3] = {L.nx, L.ny, L.nz};
+        int idx[3]; L.coords(p, idx);
         const uint32_t w = word[p], mask = w >> MC_CROSS_SHIFT;
         if (mask) {
             float pos[3];
 #pragma unroll
-            for (int a = 0; a < 3; ++a) pos[a] = lattice_coord(b.lo[a], b.hi[a], n[a], idx[a]);
+            for (int a = 0; a < 3; ++a) pos[a] = L.coord(a, idx[a]);
             const float vp = __ldg(vol + p);
             float *out = verts + 3 * (size_t)(vblock[blockIdx.x] + (w & MC_OFF_MASK));
 #pragma unroll
@@ -146,7 +134,7 @@ __global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restri
                 const bool p_in = vp > thr;
                 const float v_in = p_in ? vp : vq, v_out = p_in ? vq : vp;
                 const float t = div_(sub_(thr, v_out), sub_(v_in, v_out));
-                const float P = pos[a], Q = lattice_coord(b.lo[a], b.hi[a], n[a], idx[a] + 1);
+                const float P = pos[a], Q = L.coord(a, idx[a] + 1);
                 const float P_in = p_in ? P : Q, P_out = p_in ? Q : P;
                 float v[3] = {pos[0], pos[1], pos[2]};
                 v[a] = add_(P_out, mul_(t, sub_(P_in, P_out)));
@@ -154,7 +142,7 @@ __global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restri
                 out += 3;
             }
         }
-        if (x + 1 < L.nx && y + 1 < L.ny && z + 1 < L.nz) { cs = cell_case(vol, L, p, thr); nt = MC_TRI_COUNT[cs]; }
+        if (idx[0] + 1 < L.n[0] && idx[1] + 1 < L.n[1] && idx[2] + 1 < L.n[2]) { cs = cell_case(vol, L, p, thr); nt = MC_TRI_COUNT[cs]; }
     }
     uint32_t ftot;
     const uint32_t fex = block_excl_scan<MC_BLOCK>(nt, &ftot);
@@ -164,12 +152,9 @@ __global__ void __launch_bounds__(MC_BLOCK) mc_emit_kernel(const float *__restri
         // edge e runs along axis e / 4 from the corner with that axis' bit 0; the other two axes, in increasing order, take the bits of e % 4
         const int e = MC_TRI_EDGES[cs][k], a = e >> 2, lo = e & 1, hi = (e >> 1) & 1;
         const int dx = a == 0 ? 0 : lo, dy = a == 0 ? lo : (a == 1 ? 0 : hi), dz = a == 2 ? 0 : hi;
-        f[k] = owned_vertex(word, vblock, p + dx + dy * (int64_t)L.nx + dz * L.nxy, a);
+        f[k] = owned_vertex(word, vblock, p + dx + dy * (int64_t)L.n[0] + dz * L.nxy, a);
     }
 }
-
-// ---------------------------------------------------------------------------------------------------------------- argument checks
-static Lattice lattice(int nx, int ny, int nz) { Lattice L; L.nx = nx; L.ny = ny; L.nz = nz; L.nxy = (int64_t)nx * ny; L.points = L.nxy * nz; return L; }
 
 }  // namespace xrb
 
@@ -197,7 +182,7 @@ int xrb_ngp_density_lattice(const xrb_ngp_config *cfg, const xrb_ngp_table *tabl
     float *pts = (float *)workspace;
     for (int64_t first = 0; first < points; first += LATTICE_CHUNK) {
         const int n = (int)(points - first < LATTICE_CHUNK ? points - first : LATTICE_CHUNK);
-        lattice_points_kernel<<<(n + 255) / 256, 256, 0, s>>>(first, n, nx, ny, nz, b, pts);
+        lattice_points_kernel<<<(n + 255) / 256, 256, 0, s>>>(first, n, make_lattice(nx, ny, nz, b), pts);
         e = launch_field(cfg, table, density_fp16, nullptr, weight_image, pts, 3, nullptr, 3, n, nullptr, nullptr, out + first, impl, true, s);
         if (e) return e;
     }
@@ -216,7 +201,7 @@ int xrb_mc_count(const float *volume, int nx, int ny, int nz, float threshold, v
     if (sz == 0) return XRB_OK;
     XRB_REQUIRE(volume && workspace && counts, "mc_count: null pointer");
     XRB_REQUIRE(((uintptr_t)volume & 3) == 0 && ((uintptr_t)workspace & 7) == 0 && ((uintptr_t)counts & 7) == 0, "mc_count: misaligned pointer");
-    const Lattice L = lattice(nx, ny, nz);
+    const Lattice L = make_lattice(nx, ny, nz);
     const McWs w = mc_ws(workspace, L.points);
     const int64_t nb = mc_blocks(L.points);
     cudaStream_t s = (cudaStream_t)stream;
@@ -236,9 +221,9 @@ int xrb_mc_emit(const float *volume, int nx, int ny, int nz, float threshold, co
     if (sz == 0) return XRB_OK;
     XRB_REQUIRE(volume && workspace && verts && faces, "mc_emit: null pointer");
     XRB_REQUIRE(((uintptr_t)volume & 3) == 0 && ((uintptr_t)workspace & 7) == 0 && ((uintptr_t)verts & 3) == 0 && ((uintptr_t)faces & 3) == 0, "mc_emit: misaligned pointer");
-    const Lattice L = lattice(nx, ny, nz);
+    const Lattice L = make_lattice(nx, ny, nz, b);
     const McWs w = mc_ws(const_cast<void *>(workspace), L.points);
-    mc_emit_kernel<<<(unsigned)mc_blocks(L.points), MC_BLOCK, 0, (cudaStream_t)stream>>>(volume, L, threshold, b, w.word, w.vblock, w.fblock, w.misc, verts, faces);
+    mc_emit_kernel<<<(unsigned)mc_blocks(L.points), MC_BLOCK, 0, (cudaStream_t)stream>>>(volume, L, threshold, w.word, w.vblock, w.fblock, w.misc, verts, faces);
     return check_launch("mc_emit");
 }
 

@@ -182,8 +182,6 @@ __global__ void __launch_bounds__(PDF_WARPS * 32) sample_pdf_kernel(int n_rays, 
 // `embedded`) and by the generic tile-image kernels, so a tile image holds the fp16 roundings of exactly the fp32 kernels' values. The tile images
 // (tc.cuh layout) are what the NerfMLP kernels TMA-load: per 128-row tile the point-encoding block(s), zero padded to 64 columns each, then the
 // direction block.
-__device__ __forceinline__ float sel3(const float *a, int i) { return i == 0 ? a[0] : i == 1 ? a[1] : a[2]; }   // keeps a register array out of local memory
-
 // BaseEmbedder (embedders/base.py:26-52), column c of the encoding of x: x_c for c < 3, then per band b: sin(2^b x_a), cos(2^b x_a) for a = 0, 1, 2
 __device__ __forceinline__ float posenc_col(const float *x, int c) {
     if (c < 3) return x[c];
@@ -384,13 +382,7 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_fast_kernel(int64_t n_rays,
             for (int e = 0; e < 64; ++e) v[e] = 0.f;
             if (live) {
                 const float vd[3] = {viewdirs[3 * ray], viewdirs[3 * ray + 1], viewdirs[3 * ray + 2]};
-#pragma unroll
-                for (int a = 0; a < 3; ++a) v[a] = vd[a];
-#pragma unroll
-                for (int q = 0; q < 3 * NDEGV; ++q) {
-                    const float x = vd[q % 3] * pow2i(q / 3 + min_deg_view);
-                    v[3 + q] = sinf(x); v[3 + 3 * NDEGV + q] = sinf(x + HALF_PI);
-                }
+                mip_dir_bands(vd, min_deg_view, NDEGV, [&](int c, float y) { v[c] = y; });
             }
 #pragma unroll
             for (int ch = 0; ch < 8; ++ch) st_row_chunk(trow + 2 * TILE_BLOCK_BYTES, r7, ch, v + 8 * ch);
@@ -429,49 +421,6 @@ __global__ void __launch_bounds__(256) posenc_tiles_fast_kernel(const float *__r
     }
 }
 
-// The gradient with respect to the position through BaseEmbedder's encoding (mesh normals of a NerfMLP), one thread per point. The gradient with
-// respect to the encoding, e, is the sum of the n_terms one-block fp16 tile images of d_enc (block k of every tile = term k: the input gradients of the
-// layers that read the point encoding) divided by the staging scale s; with the column order above,
-//   dL/dx_a = e[a] + sum_b 2^b (cos(2^b x_a) e[3 + 6b + a] - sin(2^b x_a) e[6 + 6b + a])
-__global__ void __launch_bounds__(256) posenc_grad_kernel(const float *__restrict__ pts, int64_t n_pts, int multires, const uint8_t *__restrict__ d_enc, int n_terms,
-                                                          const float *__restrict__ scale, float *__restrict__ grad) {
-    const float inv = 1.f / *scale;   // a power of two: exact
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += (int64_t)gridDim.x * blockDim.x) {
-        const uint32_t r = (uint32_t)(i & 127);
-        float e[64];
-#pragma unroll
-        for (int c = 0; c < 64; ++c) e[c] = 0.f;
-        for (int k = 0; k < n_terms; ++k) {
-            const uint8_t *row = tile_block(const_cast<uint8_t *>(d_enc), i >> 7, n_terms, k) + sw128_row(r);
-#pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {
-                const uint4 q = __ldg(reinterpret_cast<const uint4 *>(row + sw128_chunk(r, ch)));
-                const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[j]));
-                    e[8 * ch + 2 * j] += f.x; e[8 * ch + 2 * j + 1] += f.y;
-                }
-            }
-        }
-        const float x[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
-        float g[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) g[a] = e[a] * inv;
-#pragma unroll
-        for (int bnd = 0; bnd < 10; ++bnd) {
-            if (bnd >= multires) break;
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                float sn, cs; sincosf(x[a] * pow2i(bnd), &sn, &cs);
-                g[a] += pow2i(bnd) * (cs * (e[3 + 6 * bnd + a] * inv) - sn * (e[6 + 6 * bnd + a] * inv));
-            }
-        }
-#pragma unroll
-        for (int a = 0; a < 3; ++a) grad[3 * i + a] = g[a];
-    }
-}
-
 // Mip-NeRF point query at a footprint (mesh export): ipe_point_bands of pts into point blocks 0 and 1, and MipNerfEmbedder.pos_enc of the view
 // direction into block 2 with the expressions of mip_ipe_tiles_fast_kernel's direction block. thread == (tile, item, row) as in the fast encoders:
 // item 0 = both point blocks of the row, item 1 = the direction block. The degrees are run-time values, so the row is zeroed with 16-byte stores and
@@ -494,41 +443,54 @@ __global__ void __launch_bounds__(256) mip_ipe_tiles_points_kernel(const float *
         } else {
             const int64_t ray = row / samples_per_ray;
             const float vd[3] = {viewdirs[3 * ray], viewdirs[3 * ray + 1], viewdirs[3 * ray + 2]};
-#pragma unroll
-            for (int a = 0; a < 3; ++a) put(a, vd[a]);
-            for (int q = 0; q < 3 * n_deg_view; ++q) {
-                const float x = sel3(vd, q % 3) * pow2i(q / 3 + min_deg_view);
-                put(3 + q, sinf(x)); put(3 + 3 * n_deg_view + q, sinf(x + HALF_PI));
-            }
+            mip_dir_bands(vd, min_deg_view, n_deg_view, put);
         }
     }
 }
 
-// The gradient with respect to the position through the point query's IPE (mesh normals of a Mip-NeRF NerfMLP), one thread per point. e is the sum of
-// the n_terms two-block fp16 terms of d_enc (blocks 2t, 2t + 1 of every tile = term t) divided by the staging scale, as in posenc_grad_kernel; with the
-// columns of ipe_point_bands (dead bands are constant zero),
-//   dL/dx_a = sum_{k < n_live} a_k 2^deg (cos(y) e[3k + a] + cos(y + pi/2) e[3 n_deg + 3k + a]),  y = x_a 2^deg, deg = min_deg + k
-// The entries of e are read where they are needed (the columns are run-time values).
-__global__ void __launch_bounds__(256) mip_ipe_grad_kernel(const float *__restrict__ pts, int64_t n_pts, const __grid_constant__ IpeBands B, const uint8_t *__restrict__ d_enc, int n_terms,
-                                                           const float *__restrict__ scale, float *__restrict__ grad) {
+// The gradient with respect to the position through a point encoding (mesh normals of a NerfMLP), one thread per point: BaseEmbedder's
+// (posenc_bands_grad, multires <= 10, one point block) or, when MIP, the point query's IPE (ipe_point_bands_grad, two point blocks). The gradient with
+// respect to the encoding, e, is the sum of the n_terms fp16 terms of d_enc (term t = point blocks P t .. P t + P - 1 of every tile: the input
+// gradients of the layers that read the point encoding) divided by the staging scale. enc_grad_read forms entries of e; NeRF reads its whole row with
+// 16-byte loads, Mip-NeRF reads each entry where it is needed (its columns are run-time values).
+template <int P, int W>
+__device__ __forceinline__ void enc_grad_read(const uint8_t *d_enc, int n_terms, int64_t i, int c0, float inv, float *e) {
+    static_assert(W == 1 || W == 64, "one entry or a whole block row");
+    const uint32_t r = (uint32_t)(i & 127);
+#pragma unroll
+    for (int c = 0; c < W; ++c) e[c] = 0.f;
+    for (int t = 0; t < n_terms; ++t) {
+        const uint8_t *blk = tile_block(const_cast<uint8_t *>(d_enc), i >> 7, P * n_terms, P * t + (c0 >> 6));
+        if constexpr (W == 1) e[0] += __half2float(__ldg(reinterpret_cast<const __half *>(sw128_elem(blk, r, (uint32_t)(c0 & 63)))));
+        else {
+#pragma unroll
+            for (int ch = 0; ch < 8; ++ch) {
+                const uint4 q = __ldg(reinterpret_cast<const uint4 *>(blk + sw128_offset(r, ch)));
+                const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[j]));
+                    e[8 * ch + 2 * j] += f.x; e[8 * ch + 2 * j + 1] += f.y;
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < W; ++c) e[c] *= inv;
+}
+template <bool MIP>
+__global__ void __launch_bounds__(256) point_enc_grad_kernel(const float *__restrict__ pts, int64_t n_pts, int multires, const __grid_constant__ IpeBands B,
+                                                             const uint8_t *__restrict__ d_enc, int n_terms, const float *__restrict__ scale, float *__restrict__ grad) {
     const float inv = 1.f / *scale;   // a power of two: exact
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += (int64_t)gridDim.x * blockDim.x) {
-        const uint32_t r = (uint32_t)(i & 127);
-        auto e = [&](int c) {
-            float s = 0.f;
-            for (int t = 0; t < n_terms; ++t)
-                s += __half2float(__ldg(reinterpret_cast<const __half *>(sw128_elem(tile_block(const_cast<uint8_t *>(d_enc), i >> 7, 2 * n_terms, 2 * t + (c >> 6)), r, (uint32_t)(c & 63)))));
-            return s * inv;
-        };
         const float x[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
-        float g[3] = {0.f, 0.f, 0.f};
-        for (int k = 0; k < B.n_live; ++k) {
-            const float sc = pow2i(B.min_deg + k), f = B.fac[k];
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                const float y = x[a] * sc;
-                g[a] += f * sc * (cosf(y) * e(3 * k + a) + cosf(y + HALF_PI) * e(3 * B.n_deg + 3 * k + a));
-            }
+        float g[3];
+        if constexpr (MIP) {
+            ipe_point_bands_grad(x, B, [&](int c) { float v; enc_grad_read<2, 1>(d_enc, n_terms, i, c, inv, &v); return v; }, g);
+        } else {
+            float e[64];
+            enc_grad_read<1, 64>(d_enc, n_terms, i, 0, inv, e);
+            posenc_bands_grad<10>(x, multires, [&](int c) { return e[c]; }, g);
         }
 #pragma unroll
         for (int a = 0; a < 3; ++a) grad[3 * i + a] = g[a];
@@ -809,7 +771,8 @@ int xrb_nerf_posenc_grad(const float *pts, int64_t n_pts, int multires, const vo
     XRB_REQUIRE(n_pts >= 0 && multires >= 0 && multires <= 10 && n_terms >= 1 && n_terms <= 4, "nerf_posenc_grad: bad size (multires 0..10, n_terms 1..4)");
     if (n_pts == 0) return XRB_OK;
     XRB_REQUIRE(pts && d_enc_image && scale && grad && ((uintptr_t)d_enc_image & 15) == 0, "nerf_posenc_grad: null/misaligned pointer");
-    posenc_grad_kernel<<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, multires, (const uint8_t *)d_enc_image, n_terms, scale, grad);
+    point_enc_grad_kernel<false><<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, multires, IpeBands{}, (const uint8_t *)d_enc_image, n_terms,
+                                                                                                       scale, grad);
     return check_launch("nerf_posenc_grad");
 }
 
@@ -833,8 +796,8 @@ int xrb_mip_ipe_grad(const float *pts, int64_t n_pts, float sigma, int min_deg_p
     XRB_REQUIRE(std::isfinite(sigma) && sigma >= 0.f, "mip_ipe_grad: the footprint sigma must be finite and >= 0");
     if (n_pts == 0) return XRB_OK;
     XRB_REQUIRE(pts && d_enc_image && scale && grad && ((uintptr_t)d_enc_image & 15) == 0, "mip_ipe_grad: null/misaligned pointer");
-    mip_ipe_grad_kernel<<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, ipe_bands(sigma, min_deg_point, max_deg_point),
-                                                                                                (const uint8_t *)d_enc_image, n_terms, scale, grad);
+    point_enc_grad_kernel<true><<<stride_grid((n_pts + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(pts, n_pts, 0, ipe_bands(sigma, min_deg_point, max_deg_point),
+                                                                                                      (const uint8_t *)d_enc_image, n_terms, scale, grad);
     return check_launch("mip_ipe_grad");
 }
 

@@ -22,6 +22,8 @@
 // The density lattice (xrb_nerf_density_lattice, mesh export) is the same kernel with LAT = true: the layer schedule stops after pts_linears.7, the
 // producer streams only those layers' slabs (a prefix of the weight image) and no encoding blocks, each consumer warpgroup writes the point-encoding
 // rows of its 64 lattice points into A block 4 before layer 0 (from the lattice index, in registers), and the pts_linears.7 epilogue stores alpha.
+#include <string>
+
 #include "tc.cuh"
 #include "common.cuh"
 #include "lattice.cuh"
@@ -74,7 +76,7 @@ struct NmParams {
     float *raw;
     uint32_t slot_bytes; int n_slots;
     uint32_t n_slabs[NM_LAYERS]; uint32_t slab_bytes[NM_LAYERS][NM_MAX_SLABS];   // the producer's stream (from nm_layer on the host)
-    int lat_n[3]; Box lat_box;                                                     // LAT: lattice sizes and box; raw is then out f32[n_rows]
+    Lattice lat;                                                                   // LAT: the lattice; raw is then out f32[n_rows]
     IpeBands lat_ipe;                                                              // LAT && MIP: the point query's IPE bands
 };
 
@@ -173,41 +175,31 @@ __device__ __forceinline__ void nm_layers(NmCtx &x, const NmParams &P, int64_t t
     }
 }
 
-// LAT: the positional encoding (multires 10) of lattice point p, zero past the last point, as row `row` of the point-encoding A block `blk`. Each
-// column goes to shared memory as soon as it is formed (fp16, the rounding of pack_h8), so no 64-float row is live beside the sincosf reductions.
+// LAT: the point encoding of lattice point p, zero past the last point, as row `row` of the point-encoding A blocks from `blk`: the positional encoding
+// (multires 10, column 63 zero) or, when MIP, the IPE at the launch's footprint (ipe_point_bands, as xrb_mip_ipe_tiles_points; columns 6 n_deg .. 127
+// zero, so the row is zeroed first). Each column goes to shared memory as soon as it is formed (fp16, the rounding of pack_h8), so no row of floats
+// is live beside the trig reductions.
+template <bool MIP>
 __device__ __forceinline__ void nm_lattice_row(const NmParams &P, uint8_t *blk, uint32_t row, int64_t p) {
-    auto put = [&](int c, float y) { *reinterpret_cast<__half *>(sw128_elem(blk, row, (uint32_t)c)) = __float2half_rn(y); };
-    if (p < P.n_rows) {
-        const int idx[3] = {(int)(p % P.lat_n[0]), (int)((p / P.lat_n[0]) % P.lat_n[1]), (int)(p / ((int64_t)P.lat_n[0] * P.lat_n[1]))};
-        float x[3];
+    auto put = [&](int c, float y) { *reinterpret_cast<__half *>(sw128_elem(blk + (c >> 6) * TILE_BLOCK_BYTES, row, (uint32_t)(c & 63))) = __float2half_rn(y); };
+    if (MIP || p >= P.n_rows) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) { x[a] = lattice_coord(P.lat_box.lo[a], P.lat_box.hi[a], P.lat_n[a], idx[a]); put(a, x[a]); }
-        posenc_bands<10>(x, put);
-        put(63, 0.f);
-    } else {
-        uint8_t *r = blk + sw128_row(row);
+        for (int b = 0; b < (MIP ? 2 : 1); ++b) {
+            uint8_t *r = blk + b * TILE_BLOCK_BYTES + sw128_row(row);
 #pragma unroll
-        for (int ch = 0; ch < 8; ++ch) st_chunk(r + sw128_chunk(row, ch), make_uint4(0u, 0u, 0u, 0u));
-    }
-}
-
-// LAT && MIP: the IPE of lattice point p at the launch's footprint (ipe_point_bands, as xrb_mip_ipe_tiles_points), zero past the last point, as row
-// `row` of the two point-encoding A blocks from `blk` (columns 6 n_deg .. 127 zero). The row is zeroed first, then each column is stored as fp16.
-__device__ __forceinline__ void nm_mip_lattice_row(const NmParams &P, uint8_t *blk, uint32_t row, int64_t p) {
-#pragma unroll
-    for (int b = 0; b < 2; ++b) {
-        uint8_t *r = blk + b * TILE_BLOCK_BYTES + sw128_row(row);
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) st_chunk(r + sw128_chunk(row, ch), make_uint4(0u, 0u, 0u, 0u));
+            for (int ch = 0; ch < 8; ++ch) st_chunk(r + sw128_chunk(row, ch), make_uint4(0u, 0u, 0u, 0u));
+        }
     }
     if (p < P.n_rows) {
-        const int idx[3] = {(int)(p % P.lat_n[0]), (int)((p / P.lat_n[0]) % P.lat_n[1]), (int)(p / ((int64_t)P.lat_n[0] * P.lat_n[1]))};
         float x[3];
+        P.lat.position(p, x);
+        if constexpr (MIP) ipe_point_bands(x, P.lat_ipe, put);
+        else {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) x[a] = lattice_coord(P.lat_box.lo[a], P.lat_box.hi[a], P.lat_n[a], idx[a]);
-        ipe_point_bands(x, P.lat_ipe, [&](int c, float y) {
-            *reinterpret_cast<__half *>(sw128_elem(blk + (c >> 6) * TILE_BLOCK_BYTES, row, (uint32_t)(c & 63))) = __float2half_rn(y);
-        });
+            for (int a = 0; a < 3; ++a) put(a, x[a]);
+            posenc_bands<10>(x, put);
+            put(63, 0.f);
+        }
     }
 }
 
@@ -262,11 +254,7 @@ __global__ void __launch_bounds__(NM_THREADS, 1) nerf_mlp_wg_kernel(const __grid
     uint32_t n = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
         if constexpr (LAT) {   // my rows' MMAs of the previous tile are complete; layer 0's fence and barrier publish these writes
-            if constexpr (MIP) {
-                if (x.t < 64) nm_mip_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
-            } else {
-                if (x.t < 64) nm_lattice_row(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
-            }
+            if (x.t < 64) nm_lattice_row<MIP>(P, A + 4 * TILE_BLOCK_BYTES, 64u * x.wg + x.t, tile * 128 + 64 * x.wg + x.t);
         } else {
             tc::mbar_wait(enc_full, n & 1);
         }
@@ -297,6 +285,25 @@ static void nm_launch(NmParams &P, bool lattice, cudaStream_t s) {
     auto k = lattice ? (mip ? nerf_mlp_wg_kernel<true, true> : nerf_mlp_wg_kernel<false, true>) : mip ? nerf_mlp_wg_kernel<true, false> : nerf_mlp_wg_kernel<false, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k<<<grid, NM_THREADS, smem, s>>>(P);
+}
+
+// the rest of a density-lattice entry after its size check (sz: lattice_sizes' result) and its encoding checks: the box, the pointers, the launch
+static int nm_density_lattice(const char *who, int sz, int input_ch, const IpeBands &ipe, const void *weight_image, const float *bias, int nx, int ny, int nz,
+                              const float *box_min_host, const float *box_max_host, float *out, void *stream) {
+    const std::string w = who;
+    Box b;
+    const int e = read_box(box_min_host, box_max_host, false, &b, (w + ": the box must be finite with box_min < box_max on every axis").c_str());
+    if (e) return e;
+    if (sz == 0) return XRB_OK;
+    XRB_REQUIRE(weight_image && bias && out, (w + ": null pointer").c_str());
+    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)bias & 15) == 0 && ((uintptr_t)out & 3) == 0,
+                (w + ": weight image / bias must be 16-byte aligned, out 4-byte aligned").c_str());
+    NmParams P{};
+    P.weight_image = (const uint8_t *)weight_image; P.bias = bias;
+    P.n_rows = (int64_t)nx * ny * nz; P.input_ch = input_ch; P.input_ch_dirs = 27; P.raw = out;
+    P.lat = make_lattice(nx, ny, nz, b); P.lat_ipe = ipe;
+    nm_launch(P, true, (cudaStream_t)stream);
+    return check_launch(who);
 }
 
 }  // namespace xrb
@@ -332,19 +339,7 @@ int xrb_nerf_density_lattice(const void *weight_image, const float *bias, int in
         set_error("nerf_density_lattice: implemented for the NerfMLP point encoding of the reference configs, input_ch 63 (multires 10)");
         return XRB_E_UNSUPPORTED;
     }
-    Box b;
-    const int e = read_box(box_min_host, box_max_host, false, &b, "nerf_density_lattice: the box must be finite with box_min < box_max on every axis");
-    if (e) return e;
-    if (sz == 0) return XRB_OK;
-    XRB_REQUIRE(weight_image && bias && out, "nerf_density_lattice: null pointer");
-    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)bias & 15) == 0 && ((uintptr_t)out & 3) == 0,
-                "nerf_density_lattice: weight image / bias must be 16-byte aligned, out 4-byte aligned");
-    NmParams P{};
-    P.weight_image = (const uint8_t *)weight_image; P.bias = bias;
-    P.n_rows = (int64_t)nx * ny * nz; P.input_ch = 63; P.input_ch_dirs = 27; P.raw = out;
-    P.lat_n[0] = nx; P.lat_n[1] = ny; P.lat_n[2] = nz; P.lat_box = b;
-    nm_launch(P, true, (cudaStream_t)stream);
-    return check_launch("nerf_density_lattice");
+    return nm_density_lattice("nerf_density_lattice", sz, 63, IpeBands{}, weight_image, bias, nx, ny, nz, box_min_host, box_max_host, out, stream);
 }
 
 // the raw alpha of xrb_nerf_mlp_forward (Mip-NeRF layout) at every point of a lattice, on the xrb_mip_ipe_tiles_points encoding at footprint sigma
@@ -355,20 +350,8 @@ int xrb_mip_density_lattice(const void *weight_image, const float *bias, int min
     if (sz < 0) return XRB_E_BADARG;
     XRB_REQUIRE(ipe_point_degrees_ok(min_deg_point, max_deg_point), "mip_density_lattice: bad degrees (6 (max - min) <= 128, both in [-100, 100])");
     XRB_REQUIRE(std::isfinite(sigma) && sigma >= 0.f, "mip_density_lattice: the footprint sigma must be finite and >= 0");
-    Box b;
-    const int e = read_box(box_min_host, box_max_host, false, &b, "mip_density_lattice: the box must be finite with box_min < box_max on every axis");
-    if (e) return e;
-    if (sz == 0) return XRB_OK;
-    XRB_REQUIRE(weight_image && bias && out, "mip_density_lattice: null pointer");
-    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0 && ((uintptr_t)bias & 15) == 0 && ((uintptr_t)out & 3) == 0,
-                "mip_density_lattice: weight image / bias must be 16-byte aligned, out 4-byte aligned");
-    NmParams P{};
-    P.weight_image = (const uint8_t *)weight_image; P.bias = bias;
-    P.n_rows = (int64_t)nx * ny * nz; P.input_ch = 96; P.input_ch_dirs = 27; P.raw = out;
-    P.lat_n[0] = nx; P.lat_n[1] = ny; P.lat_n[2] = nz; P.lat_box = b;
-    P.lat_ipe = ipe_bands(sigma, min_deg_point, max_deg_point);
-    nm_launch(P, true, (cudaStream_t)stream);
-    return check_launch("mip_density_lattice");
+    return nm_density_lattice("mip_density_lattice", sz, 96, ipe_bands(sigma, min_deg_point, max_deg_point), weight_image, bias, nx, ny, nz, box_min_host,
+                              box_max_host, out, stream);
 }
 
 }  // extern "C"

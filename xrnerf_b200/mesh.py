@@ -87,6 +87,12 @@ def ngp_to_nerf_normals(normals):
     return torch.as_tensor(normals)[:, [2, 0, 1]]
 
 
+def outward_normals(g):
+    """-g / |g| per row of g f32[n,3] (0 where g = 0): the outward unit normal of a level set whose inside is where the field exceeds the level"""
+    norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
+    return torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+
+
 def footprint_sigma(footprint, shape=None, box=None):
     """The standard deviation sigma of a Mip-NeRF point query (include/xrnerf_b200.h, Mip-NeRF mesh export) -> float. `footprint` is sigma itself,
     finite and >= 0, in the world frame of the rays; or 'cell': sigma = h / sqrt(12) with h = max over axes of (hi - lo) / (n - 1), the standard

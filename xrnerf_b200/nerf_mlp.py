@@ -1,10 +1,55 @@
 """Host side of the fused wgmma NerfMLP (csrc/nerf_mlp_tc.cu): packs the nn.Linear weights of the reference-shaped NerfMLP
 (/root/reference/xrnerf/models/mlps/nerf_mlp.py:29-49) into the kernel's weight image — fp16 slabs, K-major, in the exact order the kernel's
-TMA producer streams them — and its bias vector, and runs the kernel on the fp16 encoding tile image of the rows."""
+TMA producer streams them — and its bias vector, and runs the kernel on the fp16 encoding tile image of the rows. Also the NerfMLP's point queries
+(mesh export): the one map from its embedder, and a Mip-NeRF footprint sigma, to the point-encoder, density-lattice and encoding-gradient kernels."""
+import ctypes as C
+
 import numpy as np
 import torch
 
 from . import _C
+
+
+def fused_shape(mlp):
+    """the NerfMLP shape the fused kernels implement: netdepth 8, netwidth 256, skips [4], use_viewdirs, input channels (63, 27) (BaseEmbedder,
+    multires 10 / 4) or (96, 27) (MipNerfEmbedder, 16 point and 4 view bands)"""
+    return (mlp.use_viewdirs and len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.pts_linears[0].out_features == 256
+            and (mlp.input_ch, mlp.input_ch_dirs) in ((63, 27), (96, 27)))
+
+
+# ---- point queries: BaseEmbedder when sigma is None, otherwise the Mip-NeRF point query at footprint sigma (include/xrnerf_b200.h, mesh export)
+def encode_points(mlp, sigma, pts, dirs, samples_per_ray, enc):
+    """the encoding tile image enc (u8, xrb_nerf_enc_image_bytes) of pts f32[n,3] with view directions dirs f32[n / samples_per_ray, 3]:
+    xrb_nerf_posenc_tiles or xrb_mip_ipe_tiles_points"""
+    e, n = mlp.embedder, int(pts.shape[0])
+    if sigma is None:
+        _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(pts), _C.f32(dirs), n, samples_per_ray, e.multires, e.multires_dirs, _C.ptr(enc), _C.stream()), 'nerf_posenc_tiles')
+    else:
+        _C.check(_C.lib.xrb_mip_ipe_tiles_points(_C.f32(pts), _C.f32(dirs), n, samples_per_ray, float(sigma), e.min_deg, e.max_deg, e.min_deg_view, e.max_deg_view,
+                                                 _C.ptr(enc), _C.stream()), 'mip_ipe_tiles_points')
+
+
+def density_lattice(mlp, sigma, image, bias, shape, box, out):
+    """out f32[nz,ny,nx] <- the raw alpha on the lattice of shape (nz, ny, nx) over box: xrb_nerf_density_lattice or xrb_mip_density_lattice"""
+    e = mlp.embedder
+    nz, ny, nx = shape
+    lo, hi = _C.float3(box[0]), _C.float3(box[1])
+    if sigma is None:
+        _C.check(_C.lib.xrb_nerf_density_lattice(_C.ptr(image), _C.f32(bias), mlp.input_ch, e.multires, nx, ny, nz, lo, hi, _C.f32(out), _C.stream()),
+                 'nerf_density_lattice')
+    else:
+        _C.check(_C.lib.xrb_mip_density_lattice(_C.ptr(image), _C.f32(bias), e.min_deg, e.max_deg, float(sigma), nx, ny, nz, lo, hi, _C.f32(out), _C.stream()),
+                 'mip_density_lattice')
+
+
+def encoding_grad(mlp, sigma, pts, d_enc, n_terms, scale, grad):
+    """grad f32[n,3] <- the gradient with respect to pts f32[n,3] through the point encoding, from the n_terms encoding-gradient terms in the tile image
+    d_enc and the staging scale at device address `scale`: xrb_nerf_posenc_grad or xrb_mip_ipe_grad"""
+    e, n, scale = mlp.embedder, int(pts.shape[0]), C.c_void_p(scale)
+    if sigma is None:
+        _C.check(_C.lib.xrb_nerf_posenc_grad(_C.f32(pts), n, e.multires, _C.ptr(d_enc), n_terms, scale, _C.f32(grad), _C.stream()), 'nerf_posenc_grad')
+    else:
+        _C.check(_C.lib.xrb_mip_ipe_grad(_C.f32(pts), n, float(sigma), e.min_deg, e.max_deg, _C.ptr(d_enc), n_terms, scale, _C.f32(grad), _C.stream()), 'mip_ipe_grad')
 
 
 def _slab(w_rows_by_64):
@@ -43,14 +88,12 @@ def _slab64(w_rows_by_32):
 
 
 def pack_nerf_mlp(mlp):
-    """mlp: registry NerfMLP (netdepth 8, netwidth 256, skips [4], use_viewdirs). Returns (image u8, bias f32) on the module's device.
+    """mlp: registry NerfMLP of the fused shape (fused_shape). Returns (image u8, bias f32) on the module's device.
     Image: 16 KB slabs in the kernel's stream order — per layer, per K-block (the point / direction block first where a layer reads it):
     the 256-wide layers as two K-halves [256 x 32] (SWIZZLE_64B), views_linears.0 / rgb_linear as one [N x 64] slab (SWIZZLE_128B). Bias vector: fp32 per-layer biases, Wa[256], ba, padded to 8 floats, then an fp16 copy of the per-layer biases."""
-    assert len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.use_viewdirs and mlp.pts_linears[0].out_features == 256, \
-        'fused NerfMLP kernel: netdepth=8, netwidth=256, skips=[4], use_viewdirs=True'
+    assert fused_shape(mlp), 'fused NerfMLP kernel: netdepth=8, netwidth=256, skips=[4], use_viewdirs=True, input channels (63, 27) or (96, 27)'
     ic, icd = mlp.input_ch, mlp.input_ch_dirs
     aux = (ic + 63) // 64
-    assert aux in (1, 2)
     g = lambda lin: (lin.weight.detach().float().cpu().numpy(), lin.bias.detach().float().cpu().numpy())
     H = lambda W, j, off=0: _pad_cols(W, off + 64 * j, off + 64 * (j + 1))
     layers = []   # (column blocks in K order, N, n_halves, bias)

@@ -17,6 +17,7 @@ import ctypes as C
 import torch
 
 from . import _C
+from . import nerf_mlp as nm
 
 BLOCK = 16384
 
@@ -156,8 +157,7 @@ def _dw(n_rows, z, x, lin, gW, gb, k_off, k_cols, with_bias, scale=None):
 
 
 def supported(mlp):
-    return (mlp.use_viewdirs and len(mlp.pts_linears) == 8 and list(mlp.skips) == [4] and mlp.pts_linears[0].out_features == 256
-            and (mlp.input_ch, mlp.input_ch_dirs) in ((63, 27), (96, 27)))
+    return nm.fused_shape(mlp)
 
 
 def param_list(mlp):
@@ -248,8 +248,8 @@ def density_grad(mlp, pts, chunk=GRAD_CHUNK, sigma=None):
     the point encoding (the pts_linears.0 term and the point-block term of the skip layer pts_linears.5, ReLU masks of the forward), contracted with the
     encoding's derivative. feature_linear and the view branch are not run. In chunks of `chunk` rows.
 
-    BaseEmbedder (input_ch 63, one point block; sigma None): the positional encoding, xrb_nerf_posenc_tiles and xrb_nerf_posenc_grad.
-    MipNerfEmbedder (two point blocks): the point query at footprint `sigma` (include/xrnerf_b200.h), xrb_mip_ipe_tiles_points and xrb_mip_ipe_grad.
+    BaseEmbedder (input_ch 63, one point block; sigma None): the positional encoding. MipNerfEmbedder (two point blocks): the point query at
+    footprint `sigma` (include/xrnerf_b200.h). The kernels are nerf_mlp.encode_points and nerf_mlp.encoding_grad.
     The staged activation gradients are fp16 at a scale of 2^12: an encoding-gradient entry above about 16 would overflow."""
     dev = pts.device
     n_all = int(pts.shape[0])
@@ -260,19 +260,13 @@ def density_grad(mlp, pts, chunk=GRAD_CHUNK, sigma=None):
     if S is None or S.arena.device != dev:
         S = mlp._tg_slabs = _Slabs(mlp, P)
     S.pack()
-    emb = mlp.embedder
-    mip = sigma is not None
     vd = torch.zeros((1, 3), dtype=torch.float32, device=dev)         # any direction: the view branch is not evaluated
     for i0 in range(0, n_all, chunk):
         p = pts[i0:i0 + chunk]
         n = int(p.shape[0])
         nt = (n + 127) // 128
         enc = Img.new(nt, P + 1, dev)
-        if mip:
-            _C.check(_C.lib.xrb_mip_ipe_tiles_points(_C.f32(p), _C.f32(vd), n, n, float(sigma), emb.min_deg, emb.max_deg, emb.min_deg_view, emb.max_deg_view,
-                                                     _C.ptr(enc.buf), _C.stream()), 'mip_ipe_tiles_points')
-        else:
-            _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(vd), n, n, emb.multires, emb.multires_dirs, _C.ptr(enc.buf), _C.stream()), 'nerf_posenc_tiles')
+        nm.encode_points(mlp, sigma, p, vd, n, enc.buf)
         pts_img = enc.sub(0, P)
         H = [Img.new(nt, 4, dev) for _ in range(8)]
         _fwd(n, S, 'pts0', [pts_img], H[0])
@@ -296,12 +290,7 @@ def density_grad(mlp, pts, chunk=GRAD_CHUNK, sigma=None):
                 _dx(n, S, [(f'pts{l}', Za)], [0, 1, 2, 3], Zb, mask=H[l - 1])
             Za, Zb = Zb, Za
         _dx(n, S, [('pts0', Za)], list(range(P)), d_enc.sub(0, P))
-        scale = C.c_void_p(sc.data_ptr() + 4)
-        if mip:
-            _C.check(_C.lib.xrb_mip_ipe_grad(_C.f32(p), n, float(sigma), emb.min_deg, emb.max_deg, _C.ptr(d_enc.buf), 2, scale, _C.f32(grad[i0:i0 + n]), _C.stream()),
-                     'mip_ipe_grad')
-        else:
-            _C.check(_C.lib.xrb_nerf_posenc_grad(_C.f32(p), n, emb.multires, _C.ptr(d_enc.buf), 2, scale, _C.f32(grad[i0:i0 + n]), _C.stream()), 'nerf_posenc_grad')
+        nm.encoding_grad(mlp, sigma, p, d_enc.buf, 2, sc.data_ptr() + 4, grad[i0:i0 + n])
     return dens, grad
 
 

@@ -4,7 +4,6 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .. import _C
 from . import builder
 from .builder import MLPS
 from ..ngp import NgpField, PER_LEVEL_SCALE
@@ -60,8 +59,8 @@ class NerfMLP(BaseMLP):
         return super()._load_from_state_dict(*a, **kw)
 
     def _fused_ok(self, x):
-        return (self.fused and not torch.is_grad_enabled() and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4]
-                and self.pts_linears[0].out_features == 256 and (self.input_ch, self.input_ch_dirs) in ((63, 27), (96, 27)))
+        from ..nerf_mlp import fused_shape
+        return self.fused and not torch.is_grad_enabled() and x.is_cuda and fused_shape(self)
 
     def _is_mip(self):
         return hasattr(self.embedder, 'min_deg')
@@ -69,11 +68,10 @@ class NerfMLP(BaseMLP):
     def _mesh_check(self, x):
         """mesh export runs the fused kernels only, for the reference NeRF shape with the positional encoding of multires 10 (input channels (63, 27)) or
         the reference Mip-NeRF IPE (point degrees 0..16, view degrees 0..4: (96, 27)): anything else is an error"""
+        from ..nerf_mlp import fused_shape
         e = self.embedder
-        enc_ok = ((self.input_ch, self.input_ch_dirs) == (96, 27) and (e.min_deg, e.max_deg, e.min_deg_view, e.max_deg_view) == (0, 16, 0, 4)) if self._is_mip() else \
-            ((self.input_ch, self.input_ch_dirs) == (63, 27) and getattr(e, 'multires', None) == 10)
-        if not (self.fused and x.is_cuda and self.use_viewdirs and len(self.pts_linears) == 8 and list(self.skips) == [4] and self.pts_linears[0].out_features == 256
-                and enc_ok):
+        enc_ok = ((e.min_deg, e.max_deg, e.min_deg_view, e.max_deg_view) == (0, 16, 0, 4)) if self._is_mip() else (getattr(e, 'multires', None) == 10)
+        if not (self.fused and x.is_cuda and fused_shape(self) and enc_ok):
             raise NotImplementedError('NerfMLP mesh export is implemented for the fused CUDA NerfMLP(netdepth=8, netwidth=256, skips=[4], use_viewdirs=True) '
                                       'with BaseEmbedder(multires=10, multires_dirs=4) (input channels (63, 27)) or MipNerfEmbedder(min_deg_point=0, '
                                       'max_deg_point=16, min_deg_view=0, max_deg_view=4) (input channels (96, 27)) on a CUDA device')
@@ -98,19 +96,14 @@ class NerfMLP(BaseMLP):
         deviation sigma at the point, bit-identical to nerf_mlp_forward on the xrb_mip_ipe_tiles_points encoding): `footprint` is sigma >= 0 in the
         rays' world frame, or 'cell' (mesh.footprint_sigma: the standard deviation of a uniform distribution over one lattice cell). A BaseEmbedder takes
         footprint=None."""
+        from ..nerf_mlp import density_lattice
         w = self.pts_linears[0].weight
         self._mesh_check(w)
-        nz, ny, nx = (int(n) for n in shape)
-        sigma = self._footprint(footprint, (nz, ny, nx), box)
+        shape = tuple(int(n) for n in shape)
+        sigma = self._footprint(footprint, shape, box)
         image, bias = self._packed()
-        out = torch.empty((nz, ny, nx), dtype=torch.float32, device=w.device)
-        if sigma is None:
-            _C.check(_C.lib.xrb_nerf_density_lattice(_C.ptr(image), _C.f32(bias), self.input_ch, self.embedder.multires, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
-                                                     _C.f32(out), _C.stream()), 'nerf_density_lattice')
-        else:
-            e = self.embedder
-            _C.check(_C.lib.xrb_mip_density_lattice(_C.ptr(image), _C.f32(bias), e.min_deg, e.max_deg, sigma, nx, ny, nz, _C.float3(box[0]), _C.float3(box[1]),
-                                                    _C.f32(out), _C.stream()), 'mip_density_lattice')
+        out = torch.empty(shape, dtype=torch.float32, device=w.device)
+        density_lattice(self, sigma, image, bias, shape, box, out)
         return out
 
     def density_grad(self, pts, footprint=None):

@@ -232,30 +232,23 @@ class NerfNetwork(nn.Module):
         return self._colored_lattice_mesh(resolution, threshold, box)
 
     def _colored_lattice_mesh(self, resolution, threshold, box, sigma=None):
+        from ..mesh import outward_normals
         verts, faces = self._lattice_mesh(resolution, threshold, box, sigma)
         mlp = self._mesh_mlp()
         with torch.no_grad():
-            _, g = mlp.density_grad(verts, sigma)
-            norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
-            normals = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+            normals = outward_normals(mlp.density_grad(verts, sigma)[1])
             colors = nerf_vertex_colors(mlp, verts, -normals, self.render.rgb_padding, sigma)
             return verts, faces, normals, colors
 
 
 def nerf_vertex_colors(mlp, pts, dirs, rgb_padding, sigma=None):
-    """NerfRender's rgb activation of the fused inference NerfMLP at pts f32[n,3] seen along dirs f32[n,3] (one encoding row per point: BaseEmbedder
-    xrb_nerf_posenc_tiles, MipNerfEmbedder the point query at footprint sigma, xrb_mip_ipe_tiles_points, with samples_per_ray = 1)"""
-    from ..nerf_mlp import nerf_mlp_forward_tiles
+    """NerfRender's rgb activation of the fused inference NerfMLP at pts f32[n,3] seen along dirs f32[n,3] (one encoding row per point,
+    nerf_mlp.encode_points: BaseEmbedder, or with a MipNerfEmbedder the point query at footprint sigma)"""
+    from ..nerf_mlp import encode_points, nerf_mlp_forward_tiles
     n = int(pts.shape[0])
-    emb = mlp.embedder
     image, bias = mlp._packed()
     enc = torch.empty(_C.lib.xrb_nerf_enc_image_bytes(n, mlp.input_ch), dtype=torch.uint8, device=pts.device)
-    p, d = pts.contiguous().float(), dirs.contiguous().float()
-    if sigma is None:
-        _C.check(_C.lib.xrb_nerf_posenc_tiles(_C.f32(p), _C.f32(d), n, 1, emb.multires, emb.multires_dirs, _C.ptr(enc), _C.stream()), 'nerf_posenc_tiles')
-    else:
-        _C.check(_C.lib.xrb_mip_ipe_tiles_points(_C.f32(p), _C.f32(d), n, 1, float(sigma), emb.min_deg, emb.max_deg, emb.min_deg_view, emb.max_deg_view, _C.ptr(enc),
-                                                 _C.stream()), 'mip_ipe_tiles_points')
+    encode_points(mlp, sigma, pts.contiguous().float(), dirs.contiguous().float(), 1, enc)
     raw = nerf_mlp_forward_tiles(image, bias, enc, n, mlp.input_ch, mlp.input_ch_dirs)
     return torch.sigmoid(raw[:, :3]) * (1 + 2 * rgb_padding) - rgb_padding
 
@@ -482,13 +475,11 @@ class HashNerfNetwork(NerfNetwork):
         color = sampler.rgb_activation(run_mlp(warped vertex, dir)[:, :3]) with dir = (1 - normal) / 2: the field seen from outside, looking along
         -normal, in the warped [0,1]^3 direction convention of the ray march (dir = (d + 1) / 2 for a unit ray direction d). A zero normal gives the
         direction (0.5, 0.5, 0.5). For the Blender frame, map verts with xrnerf_b200.mesh.ngp_to_nerf and normals with ngp_to_nerf_normals."""
-        from ..mesh import activate_rgb
+        from ..mesh import activate_rgb, outward_normals
         verts_w, faces = self._warped_mesh(resolution, threshold)
         field = self.mlp.field
         with torch.no_grad():
-            _, g = field.density_grad(verts_w)
-            norm = torch.linalg.vector_norm(g, dim=1, keepdim=True)
-            normals = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+            normals = outward_normals(field.density_grad(verts_w)[1])
             colors = activate_rgb(field.run_mlp(verts_w, (1.0 - normals) * 0.5)[:, :3], self.sampler.rgb_activation)
             return self._from_warped(verts_w), faces, normals, colors
 
