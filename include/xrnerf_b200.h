@@ -502,6 +502,28 @@ int xrb_mip_density_lattice(const void *weight_image, const float *bias, int min
 int xrb_mip_ipe_grad(const float *pts, int64_t n_pts, float sigma, int min_deg_point, int max_deg_point, const void *d_enc_image, int n_terms, const float *scale, float *grad,
                      void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Image metrics (csrc/metrics.cu)
+ * ---------------------------------------------------------------------------------------------- */
+
+/* SSIM of n image pairs: what the reference's ValidateHook / TestHook ask scikit-image for (hooks/utils.py:20-28, calculate_ssim:
+ * structural_similarity(im1, im2, multichannel=True, full=True), 7 x 7 uniform window, K1 = 0.01, K2 = 0.03, sample covariance).
+ * x, y f32[n, H, W, C] (contiguous, HWC, 4-byte aligned), H >= 7, W >= 7, 1 <= C <= 4. Each channel is its own 2-D image. Per entry, in double
+ * (each fp32 input converted exactly), with ux, uy, uxx, uyy, uxy the 7 x 7 window means (window sum x 1/49) of x, y, x^2, y^2, x y, borders
+ * reflected as scipy.ndimage's mode 'reflect' (d c b a | a b c d | d c b a):
+ *   vx = cn (uxx - ux^2), vy = cn (uyy - uy^2), vxy = cn (uxy - ux uy), cn = 49/48;  C1 = (0.01 R)^2, C2 = (0.03 R)^2, R = data_range (finite, > 0)
+ *   S = ((2 ux uy + C1)(2 vxy + C2)) / ((ux^2 + uy^2 + C1)(vx + vy + C2))
+ * every operation rounded once, in this order (no FMA contraction): S(x, x) = 1 and S(x, y) = S(y, x) hold bit for bit.
+ * Outputs: mean_full f64[n] <- the mean of S over all H W C entries (calculate_ssim's value), mean_crop f64[n] <- the mean over the entries of the
+ * crop [3, H-3) x [3, W-3) (scikit-image's mssim); s_map f32[n, H, W, C] <- S rounded once to fp32, or NULL to skip it.
+ * Window sums: horizontal 7-sums left to right, then vertical 7-sums top to bottom; the means sum per-tile partials in a fixed order. An image's
+ * results are bit-identical alone, in any batch and from run to run. workspace: xrb_ssim_workspace(n, H, W) bytes (0 for bad sizes), 8-byte
+ * aligned, passed with its size. Sizes, channels, data_range, pointers and the workspace size are checked before any CUDA call (XRB_E_BADARG);
+ * n == 0 is a no-op that touches no pointer. No allocation inside: capturable in a CUDA graph. */
+size_t xrb_ssim_workspace(int n, int height, int width);
+int xrb_ssim(const float *x, const float *y, int n, int height, int width, int channels, double data_range, double *mean_full, double *mean_crop, float *s_map,
+             void *workspace, size_t workspace_bytes, void *stream);
+
 /* Measurement utility (bench.py's second roofline; no reference counterpart): random reads of 4-, 8- or 32-byte records from a table (L2-resident when
  * it is the size of the fp16 hash table) by SMs x 8 CTAs x 256 threads, `rounds` rounds of 8 independent loads per thread. *loads_issued (host) receives the
  * number of loads of the launch; every 4/8-byte load costs one 32-byte sector, which is what bounds the hash gather. */

@@ -130,6 +130,8 @@ _SIGS = {
     'xrb_mip_ipe_tiles_points': (_i, [P, P, _i64, _i, _f, _i, _i, _i, _i, P, P]),
     'xrb_mip_density_lattice': (_i, [P, P, _i, _i, _f, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), P, P]),
     'xrb_mip_ipe_grad': (_i, [P, _i64, _f, _i, _i, P, _i, P, P, P]),
+    'xrb_ssim_workspace': (_sz, [_i, _i, _i]),
+    'xrb_ssim': (_i, [P, P, _i, _i, _i, _i, C.c_double, P, P, P, P, _sz, P]),
 }
 
 EXPORTS = sorted(_SIGS)  # every symbol the header declares and the library currently implements
