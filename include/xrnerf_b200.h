@@ -296,6 +296,40 @@ int xrb_ngp_render_fused_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *t
                                float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act, int dens_act,
                                float *rgb_out, float *alpha_out, float *depth_out, int32_t *n_samples_out, void *workspace, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Normal maps (chain render path only)
+ *   per-sample gradient  g_k = d(raw density, density-net output 0) / d(warped position) of sample k;
+ *   per-sample normal    n_k = -g_k / |g_k| in fp32, 0 where g_k = 0. Inside is the larger density, so n_k points out of the surface
+ *                        (the rule of xrnerf_b200.mesh.outward_normals). The warp to [0,1]^3 is a positive uniform scale, so n_k is also the
+ *                        direction in the rays' frame (xrnerf_b200.mesh.ngp_to_nerf_normals maps it to the Blender frame);
+ *   per-ray normal       normal = sum_k w_k n_k in fp32, w_k = T_k alpha_k the weights of the ray's rgb and depth. No background term, 0 for a ray
+ *                        without samples, and NOT normalised (as depth is not divided by alpha).
+ * ---------------------------------------------------------------------------------------------- */
+/* The raw density and its position gradient on wgmma tensor-core tiles (one warpgroup per 128-row tile):
+ *   density[i] (f32[n], may be NULL) is bit-identical to xrb_ngp_density_forward with impl = 1 at the same position;
+ *   grad[i] (f32[n,3]) is g of that function: the density net's ReLU masks are the forward's (a unit is live iff its fp16 activation is > 0), the
+ *   backward through the net runs on fp16 operands with fp32 accumulation, d(density)/d(hidden) staged in fp16 with a fixed 2^10 scale (finite
+ *   while every |d density / d hidden unit| < 64), d(density)/d(encoding) in fp32; the levels' position derivative as xrb_ngp_density_grad.
+ *   Rows outside [-0.5, 1.5]^3, or not finite, get grad 0 (no march writes such a row).
+ * pts f32 rows of pts_stride floats (7 for the chain's sample rows); n_rows_dev (optional, device): the effective row count is min(n, *n_rows_dev);
+ * order (optional, device u32): tile slot j evaluates row order[j], a permutation of the effective rows, used when there are at most 2^21 of them
+ * (the range in which the chain orders its samples) and ignored above. Every output row is independent of the order and of the row count.
+ * n == 0 is a no-op that touches no pointer. Returns XRB_E_BADARG for a null cfg, table, weight_image, pts or grad, n < 0, pts_stride < 3, or a
+ * weight image that is not 16-byte aligned, and XRB_E_UNSUPPORTED for a config the field does not support, all before any CUDA call. */
+int xrb_ngp_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, int n,
+                            const int32_t *n_rows_dev, const uint32_t *order, float *density /* f32[n], may be NULL */, float *grad /* f32[n,3] */,
+                            void *stream);
+/* xrb_ngp_render_depth plus normal_out f32[n_rays,3] (non-NULL), right after depth_out: march -> sample order -> field -> xrb_ngp_density_grad_tc
+ * on the same rows in the same order -> composite. rgb, alpha, depth and the sample counts are bit-identical to xrb_ngp_render_depth's.
+ * workspace: xrb_ngp_render_normals_workspace(N, max_samples) bytes, 256-byte aligned: the chain's workspace followed, at 256-byte alignment, by the
+ * per-row gradient f32[max_samples,3]. Every argument is checked before any CUDA call. */
+size_t xrb_ngp_render_normals_workspace(int n_rays, int max_samples);
+int xrb_ngp_render_normals(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield,
+                           const float *rays_o, const float *rays_d, int n_rays, int max_samples, float aabb0, float aabb1,
+                           float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                           int dens_act, float *rgb_out, float *alpha_out, float *depth_out, float *normal_out, int32_t *numsteps, int32_t *counters,
+                           void *workspace, void *ev_before_field, void *ev_after_field, void *stream);
+
 
 /* ------------------------------------------------------------------------------------------------
  * NeRF / Mip-NeRF composite + sampling kernels (pure-PyTorch in the reference)

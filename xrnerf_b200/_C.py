@@ -120,6 +120,9 @@ _SIGS = {
     'xrb_ngp_render': (_i, [_cfg, _tab, P, P, P, P, _i, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P, P, P]),
     'xrb_ngp_render_depth': (_i, [_cfg, _tab, P, P, P, P, _i, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P, P, P, P]),
     'xrb_ngp_render_fused_depth': (_i, [_cfg, _tab, P, P, P, P, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P]),
+    'xrb_ngp_density_grad_tc': (_i, [_cfg, _tab, P, P, _i, _i, P, P, P, P, P]),
+    'xrb_ngp_render_normals_workspace': (_sz, [_i, _i]),
+    'xrb_ngp_render_normals': (_i, [_cfg, _tab, P, P, P, P, _i, _i, _f, _f, _f, _f, _u64, _i64, C.POINTER(C.c_float), _i, _i, P, P, P, P, P, P, P, P, P, P]),
     'xrb_ngp_density_lattice_workspace': (_sz, []),
     'xrb_ngp_density_lattice': (_i, [_cfg, _tab, P, P, _i, _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), P, _i, P, P]),
     'xrb_mc_workspace': (_sz, [_i, _i, _i]),

@@ -107,36 +107,21 @@ __device__ __forceinline__ void bt_fwd_out(const BtWg &c, int x_tile, uint32_t w
     bt_stage_rows<16>(c, st, acc[0], acc[1], out);
 }
 
-// backward round of one layer with OUT outputs and IN inputs:
-//   dX[128 x IN] = dZ[128 x OUT] . W[OUT x IN]          (two M=64 halves)
-//   dW accumulators (registers, M = 64):
-//     OUT == 64:  D[m = out][n = in]  += dZ^T X   (A = dZ tile, B = X tile, N = IN)            IN/2 registers
-//     OUT == 16:  D[m = in][n = out]  += X^T dZ   (A = X tile (IN == 64), B = dZ tile, N = 16)   8 registers, stored transposed at the flush
-// EPI 0: dZ tile := fp16(dX) * [act > 0] (act_tile);  EPI 1: thread r receives dX row r in `out` (fp32, staged through tile `st`)
-template <int IN, int OUT, int EPI>
-__device__ __forceinline__ void bt_bwd(const BtWg &c, int dz_tile, int x_tile, uint32_t w_off, float *dw, int act_tile, int st, float *out) {
-    constexpr int DWN = OUT == 64 ? IN : 16;
-    bt_sync(c);
-    const uint32_t z0 = tc::smem_u32(bt_tile(c, dz_tile)), x0 = tc::smem_u32(bt_tile(c, x_tile)), w0 = tc::smem_u32(c.W + w_off);
-    float acc[2][IN / 2];
-    tc::wg_fence();
-    // weight gradient: contraction over the 128 sample rows, 16 rows (2 x 1024 bytes) per instruction
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const uint32_t sc = (k > 0 || !c.first) ? 1u : 0u;
-        if (OUT == 64) tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(z0 + k * 2048, 1024), tc::desc_mn128(x0 + k * 2048, 1024), sc);
-        else tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(x0 + k * 2048, 1024), tc::desc_mn128(z0 + k * 2048, 1024), sc);
-    }
-    // input gradient: contraction over OUT; B = forward weight image W[OUT rows][IN cols] read MN-major (N = IN contiguous, K = OUT rows)
+// input gradient of one layer with OUT outputs and IN inputs, issued (not committed): dX[128 x IN] = dZ[128 x OUT] . W[OUT x IN] as two M=64 halves,
+// contraction over OUT; A = the dZ tile at z0 (K-major), B = the forward weight image W[OUT rows][IN cols] at w0 read MN-major (N = IN contiguous, K = OUT rows)
+template <int IN, int OUT>
+__device__ __forceinline__ void bt_dx_issue(uint32_t z0, uint32_t w0, float (*acc)[IN / 2]) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int k = 0; k < OUT / 16; ++k) tc::wgmma<IN, 0, 1>(acc[h], tc::desc_k128(z0 + h * 8192 + k * 32), tc::desc_mn128(w0 + k * 2048, 1024), k > 0 ? 1u : 0u);
-    tc::wg_commit();
-    tc::wg_wait<0>();
-    tc::acc_fence<DWN / 2>(dw); tc::acc_fence<IN / 2>(acc[0]); tc::acc_fence<IN / 2>(acc[1]);
+}
+// what happens to a completed dX (accumulators fenced):
+// EPI 0: dZ tile := fp16(dX) * [act > 0] (act_tile);  EPI 1: thread r receives dX row r in `out` (fp32, staged through tile `st`)
+template <int IN, int EPI>
+__device__ __forceinline__ void bt_dx_epilogue(const BtWg &c, float (*acc)[IN / 2], int dz_tile, int act_tile, int st, float *out) {
     if (EPI == 1) { bt_stage_rows<IN>(c, st, acc[0], acc[1], out); return; }
-    bt_bar(c);   // every warp's share of the dW MMA (which reads all dZ rows) has completed before dZ is overwritten
+    bt_bar(c);   // every warp's share of the MMAs that read the dZ rows has completed before dZ is overwritten
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const uint32_t r = 64u * (uint32_t)h + tc::frag_row(c.row);
@@ -153,6 +138,43 @@ __device__ __forceinline__ void bt_bwd(const BtWg &c, int dz_tile, int x_tile, u
             }
         }
     }
+}
+// backward round of one layer with OUT outputs and IN inputs:
+//   dX[128 x IN] = dZ[128 x OUT] . W[OUT x IN]          (bt_dx_issue, then bt_dx_epilogue<IN, EPI>)
+//   dW accumulators (registers, M = 64):
+//     OUT == 64:  D[m = out][n = in]  += dZ^T X   (A = dZ tile, B = X tile, N = IN)            IN/2 registers
+//     OUT == 16:  D[m = in][n = out]  += X^T dZ   (A = X tile (IN == 64), B = dZ tile, N = 16)   8 registers, stored transposed at the flush
+template <int IN, int OUT, int EPI>
+__device__ __forceinline__ void bt_bwd(const BtWg &c, int dz_tile, int x_tile, uint32_t w_off, float *dw, int act_tile, int st, float *out) {
+    constexpr int DWN = OUT == 64 ? IN : 16;
+    bt_sync(c);
+    const uint32_t z0 = tc::smem_u32(bt_tile(c, dz_tile)), x0 = tc::smem_u32(bt_tile(c, x_tile)), w0 = tc::smem_u32(c.W + w_off);
+    float acc[2][IN / 2];
+    tc::wg_fence();
+    // weight gradient: contraction over the 128 sample rows, 16 rows (2 x 1024 bytes) per instruction
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint32_t sc = (k > 0 || !c.first) ? 1u : 0u;
+        if (OUT == 64) tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(z0 + k * 2048, 1024), tc::desc_mn128(x0 + k * 2048, 1024), sc);
+        else tc::wgmma<DWN, 1, 1>(dw, tc::desc_mn128(x0 + k * 2048, 1024), tc::desc_mn128(z0 + k * 2048, 1024), sc);
+    }
+    bt_dx_issue<IN, OUT>(z0, w0, acc);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::acc_fence<DWN / 2>(dw); tc::acc_fence<IN / 2>(acc[0]); tc::acc_fence<IN / 2>(acc[1]);
+    bt_dx_epilogue<IN, EPI>(c, acc, dz_tile, act_tile, st, out);
+}
+// the input-gradient half of bt_bwd alone (no weight gradient): a chain that differentiates with respect to the inputs only
+template <int IN, int OUT, int EPI>
+__device__ __forceinline__ void bt_bwd_dx(const BtWg &c, int dz_tile, uint32_t w_off, int act_tile, int st, float *out) {
+    bt_sync(c);
+    float acc[2][IN / 2];
+    tc::wg_fence();
+    bt_dx_issue<IN, OUT>(tc::smem_u32(bt_tile(c, dz_tile)), tc::smem_u32(c.W + w_off), acc);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::acc_fence<IN / 2>(acc[0]); tc::acc_fence<IN / 2>(acc[1]);
+    bt_dx_epilogue<IN, EPI>(c, acc, dz_tile, act_tile, st, out);
 }
 // 16 fp32 values -> chunks 0,1 of tile t (fp16)
 __device__ __forceinline__ void bt_store16(const BtWg &c, int t, const float *v) {
@@ -305,6 +327,97 @@ static int launch_bwd_tc(const HashGridDev &g, const xrb_ngp_table *tab, const v
     return check_launch("ngp_mlp_backward_tc");
 }
 
+// ---------------------------------------------------------------------------- density and its position gradient on tensor cores (xrb_ngp_density_grad_tc)
+// The gradient stage of the chain render's normal maps. One warpgroup per CTA and 128-row tile, persistent:
+//   forward   hash gather -> ENC tile; density hidden layers through bt_fwd_hidden, each activation parked as a tile (its ReLU mask is "fp16 value > 0");
+//             the N=16 output layer through bt_fwd_out. Same fp16 operands, K order and roundings as the production field (tc_net), so the density is
+//             bit-identical to ngp_field_tc_kernel<true, *>'s.
+//   backward  only output 0 is differentiated: dZ of the last hidden layer = fp16(DG_TC_SCALE * W_out[0,:]) * [H > 0], written row by row from the resident
+//             weight image; then the masked W^T rounds of bt_bwd_dx (the weight-gradient half of the training backward is not issued) down to
+//             dL/d(encoding) in fp32 (EPI 1), and position_grad_level per level.
+// Tiles per warpgroup: ENC, H0..H(dh-1), dZ. Only the density part of the weight image is loaded. dh is a run-time loop: tile indices and weight offsets
+// are computed, nothing is indexed in registers.
+__device__ __forceinline__ uint32_t h2_as_u32(__half2 h) { return *reinterpret_cast<uint32_t *>(&h); }
+constexpr float DG_TC_SCALE = 1024.f;    // dZ staging scale (fp16): |d density / d hidden unit| < 64 stays finite, entries down to 2^-24 / 1024 stay exact
+__global__ void __launch_bounds__(128) ngp_density_grad_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells,
+                                                                   const void *__restrict__ weight_image, uint32_t image_bytes, int dh, const float *__restrict__ pts,
+                                                                   int pts_stride, int n, const int32_t *__restrict__ n_dev, const uint32_t *__restrict__ order,
+                                                                   float *__restrict__ density, float *__restrict__ grad) {
+    extern __shared__ uint8_t dyn_smem[];
+    if (n_dev) n = min(n, max(*n_dev, 0));
+    if (n > (int)SAMPLE_ORDER_MAX_ROWS) order = nullptr;   // as the field: beyond this the chain evaluates rows in ray order
+    const int T_ENC = 0, T_H0 = 1, T_DZ = 1 + dh;
+    uint8_t *W = tc_load_weight_image(dyn_smem, weight_image, image_bytes, (size_t)(dh + 2) * TILE_BLOCK_BYTES);
+    BtWg c;
+    c.wg = 0; c.row = threadIdx.x; c.bar = 1;
+    c.tiles = W + image_bytes; c.W = W; c.first = true;
+    const WeightImageLayout L = weight_image_layout(dh, 1);
+    const int n_tiles = (n + 127) / 128;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int j = tile * 128 + (int)c.row;
+        const bool valid = j < n;
+        const int i = valid && order ? (int)__ldg(order + j) : j;   // the row this tile slot evaluates: the rows of a tile are independent
+        float x = 0.5f, y = 0.5f, z = 0.5f;
+        if (valid) { const float *p = pts + (size_t)i * pts_stride; x = p[0]; y = p[1]; z = p[2]; }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            uint32_t e[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { const float2 f = hash_level(table, cells, g, 4 * q + k, x, y, z); e[k] = pack_h2(f.x, f.y); }
+            bt_store_chunk(c, T_ENC, q, make_uint4(e[0], e[1], e[2], e[3]));
+        }
+        bt_fwd_hidden<32>(c, T_ENC, L.d_in, T_H0);
+        for (int h = 1; h < dh; ++h) bt_fwd_hidden<64>(c, T_H0 + h - 1, L.d_in + 8192u * (uint32_t)h, T_H0 + h);
+        const int t_last = T_H0 + dh - 1;
+        {
+            float dout[16];
+            bt_fwd_out(c, t_last, L.d_out, T_DZ, dout);   // dZ is free until it is written below (bt_stage_rows ends with a barrier)
+            if (valid && density) density[i] = round_h(dout[0]);
+        }
+        // dZ row r = fp16(scale * W_out[0, :]) masked by the last hidden layer's activation of row r
+        const __half2 s2 = __float2half2_rn(DG_TC_SCALE), zero2 = __float2half2_rn(0.f);
+#pragma unroll
+        for (int ch = 0; ch < 8; ++ch) {
+            const uint4 w = *reinterpret_cast<const uint4 *>(W + L.d_out + sw128_offset(0, (uint32_t)ch));
+            const uint4 a = *reinterpret_cast<const uint4 *>(bt_tile(c, t_last) + sw128_offset(c.row, (uint32_t)ch));
+            auto masked = [&](uint32_t wk, uint32_t ak) { return h2_as_u32(__hmul2(__hmul2(as_h2(wk), s2), __hgt2(as_h2(ak), zero2))); };
+            bt_store_chunk(c, T_DZ, (uint32_t)ch, make_uint4(masked(w.x, a.x), masked(w.y, a.y), masked(w.z, a.z), masked(w.w, a.w)));
+        }
+        for (int k = dh - 1; k >= 1; --k) bt_bwd_dx<64, 64, 0>(c, T_DZ, L.d_in + 8192u * (uint32_t)k, T_H0 + k - 1, 0, nullptr);
+        float genc[32];
+        bt_bwd_dx<32, 64, 1>(c, T_DZ, L.d_in, 0, T_ENC, genc);   // d density / d encoding (scaled); ENC is dead after this round
+        if (valid) {
+            float3 d = make_float3(0.f, 0.f, 0.f);
+            // a row no march writes (outside [-0.5, 1.5]^3, or not finite: stale rows past an overflowed ray) gets 0 without touching the table
+            if (fabsf(x - 0.5f) <= 1.f && fabsf(y - 0.5f) <= 1.f && fabsf(z - 0.5f) <= 1.f) {
+#pragma unroll 1
+                for (int l = 0; l < 16; ++l) {
+                    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+                    for (int q = 0; q < 16; ++q) if (q == l) { g0 = genc[2 * q]; g1 = genc[2 * q + 1]; }   // select, as the training backward's scatter: never indexed in registers
+                    position_grad_level(table, g, l, x, y, z, g0 * (1.f / DG_TC_SCALE), g1 * (1.f / DG_TC_SCALE), d);
+                }
+            }
+            float *o = grad + 3 * (size_t)i;
+            o[0] = d.x; o[1] = d.y; o[2] = d.z;
+        }
+    }
+}
+
+// launched by xrb_ngp_density_grad_tc and by the normal-map render (ngp_render.cu); arguments validated by the caller
+int launch_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *weight_image, const float *pts, int pts_stride, int n, const int32_t *n_dev,
+                           const uint32_t *order, float *density, float *grad, cudaStream_t s) {
+    HashGridDev g; int e = table_setup(cfg, tab, &g); if (e) return e;
+    const int dh = cfg->density_hidden;
+    const uint32_t image_bytes = weight_image_layout(dh, 1).c_in;   // the density net's matrices lead the image
+    const size_t smem = 1024 + image_bytes + (size_t)(dh + 2) * TILE_BLOCK_BYTES + 16;
+    cudaFuncSetAttribute(ngp_density_grad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int grid = persistent_grid((const void *)ngp_density_grad_tc_kernel, 128, smem, (n + 127) / 128);
+    ngp_density_grad_tc_kernel<<<grid, 128, smem, s>>>(g, (const __half2 *)tab->table_fp16, (const uint8_t *)tab->cell_image, weight_image, image_bytes, dh, pts, pts_stride, n, n_dev,
+                                                       order, density, grad);
+    return check_launch("ngp_density_grad_tc");
+}
+
 }  // namespace xrb
 
 using namespace xrb;
@@ -333,6 +446,16 @@ int xrb_ngp_mlp_backward_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tabl
     XRB_BWT(1, 1) XRB_BWT(1, 2)
 #undef XRB_BWT
     return XRB_E_UNSUPPORTED;
+}
+
+int xrb_ngp_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, int n, const int32_t *n_rows_dev,
+                            const uint32_t *order, float *density, float *grad, void *stream) {
+    int e = check_cfg(cfg); if (e) return e;
+    XRB_REQUIRE(n >= 0 && pts_stride >= 3, "ngp_density_grad_tc: bad size");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(table && weight_image && pts && grad, "ngp_density_grad_tc: null pointer");
+    XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0, "ngp_density_grad_tc: the weight image must be 16-byte aligned");
+    return launch_density_grad_tc(cfg, table, weight_image, pts, pts_stride, n, n_rows_dev, order, density, grad, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -79,9 +79,14 @@ constexpr uint32_t SAMPLE_ORDER_MAX_ROWS = 1u << 21;
 int table_setup(const xrb_ngp_config *cfg, const xrb_ngp_table *t, HashGridDev *g);
 int launch_field(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *dens, const void *color, const void *image, const float *pts, int pts_stride, const float *dirs,
                  int dirs_stride, int n, const int32_t *n_dev, const uint32_t *order, float *out, int impl, bool density_only, cudaStream_t s);
-// defined in raymarch.cu: xrb_rm_calc_rgb_inference that also writes depth f32[n_rays] (t of each sample rebuilt from its coords row and the ray)
+// defined in raymarch.cu: xrb_rm_calc_rgb_inference that also writes depth f32[n_rays] (t of each sample rebuilt from its coords row and the ray);
+// with normal_out (and grad f32[rows,3], the per-row density gradient), also normal f32[n_rays,3] = sum of w * (-g / |g|)
 int launch_composite_depth(const float *raw, const float *coords, const int32_t *numsteps, const float *bg3_host, int n_rays, int rgb_act, int dens_act, const float *rays_o,
-                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s);
+                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s,
+                           const float *grad = nullptr, float *normal_out = nullptr);
+// defined in ngp_backward_tc.cu: xrb_ngp_density_grad_tc after its argument checks (n_dev, order as in launch_field)
+int launch_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, const void *weight_image, const float *pts, int pts_stride, int n, const int32_t *n_dev,
+                           const uint32_t *order, float *density, float *grad, cudaStream_t s);
 
 #ifdef __CUDACC__
 __device__ __forceinline__ float round_h(float x) { return __half2float(__float2half_rn(x)); }

@@ -112,18 +112,24 @@ static void launch_sample_order(const float *coords, int max_samples, const int3
     order_scatter_kernel<<<grid, ORDER_THREADS, 0, s>>>(key, (uint32_t)max_samples, n_dev, count, order);
 }
 
-// xrb_ngp_render (depth == false, depth_out unused) and xrb_ngp_render_depth
+// xrb_ngp_render (depth == false, depth_out unused), xrb_ngp_render_depth and, with normal_out, xrb_ngp_render_normals (depth == true); the
+// normals' per-row gradient f32[max_samples,3] follows the chain's workspace at align256(render_ws bytes)
 static int render_chain(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
                         int max_samples, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
                         int dens_act, float *rgb_out, float *alpha_out, bool depth, float *depth_out, int32_t *numsteps, int32_t *counters, void *workspace, void *ev_before_field,
-                        void *ev_after_field, void *stream) {
+                        void *ev_after_field, void *stream, bool normals = false, float *normal_out = nullptr) {
     int e = check_cfg(cfg); if (e) return e;
     XRB_REQUIRE(n_rays >= 0 && max_samples > 0, "ngp_render: bad size");
     if (n_rays == 0) return XRB_OK;
-    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && (depth_out || !depth) && numsteps && counters && workspace,
-                "ngp_render: null pointer");
+    XRB_REQUIRE(table && weight_image && bitfield && rays_o && rays_d && bg3_host && rgb_out && alpha_out && (depth_out || !depth) && (normal_out || !normals) && numsteps && counters &&
+                workspace, "ngp_render: null pointer");
+    if (normals) {   // the gradient kernel's checks, before any CUDA call
+        XRB_REQUIRE(((uintptr_t)weight_image & 15) == 0, "ngp_render_normals: the weight image must be 16-byte aligned");
+        HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
+    }
     cudaStream_t s = (cudaStream_t)stream;
-    const RenderWs w = render_ws(workspace, n_rays, max_samples, nullptr);
+    size_t ws_bytes = 0;
+    const RenderWs w = render_ws(workspace, n_rays, max_samples, &ws_bytes);
     cudaMemsetAsync(counters, 0, 2 * sizeof(int32_t), s);
     e = xrb_rm_rays_sampler(rays_o, rays_d, bitfield, nullptr, nullptr, nullptr, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, w.coords, w.rays_index,
                             numsteps, counters, w.march, stream);
@@ -136,6 +142,12 @@ static int render_chain(const xrb_ngp_config *cfg, const xrb_ngp_table *table, c
     e = launch_field(cfg, table, nullptr, nullptr, weight_image, w.coords, ROW_FLOATS, w.coords + ROW_DIR, ROW_FLOATS, max_samples, counters + 1, w.order, w.raw, 1, false, s);
     if (ev_after_field) cudaEventRecord((cudaEvent_t)ev_after_field, s);
     if (e) return e;
+    if (normals) {   // the density gradient of the same rows, in the same order, then the composite with normals
+        float *grad = (float *)((uint8_t *)workspace + align256(ws_bytes));
+        e = launch_density_grad_tc(cfg, table, weight_image, w.coords, ROW_FLOATS, max_samples, counters + 1, w.order, nullptr, grad, s);
+        if (e) return e;
+        return launch_composite_depth(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rays_o, rays_d, aabb0, aabb1, rgb_out, alpha_out, depth_out, s, grad, normal_out);
+    }
     if (depth) return launch_composite_depth(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rays_o, rays_d, aabb0, aabb1, rgb_out, alpha_out, depth_out, s);
     return xrb_rm_calc_rgb_inference(w.raw, w.coords, numsteps, bg3_host, n_rays, rgb_act, dens_act, rgb_out, alpha_out, stream);
 }
@@ -163,6 +175,18 @@ int xrb_ngp_render_depth(const xrb_ngp_config *cfg, const xrb_ngp_table *table, 
                          void *ev_after_field, void *stream) {
     return xrb::render_chain(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act,
                              dens_act, rgb_out, alpha_out, true, depth_out, numsteps, counters, workspace, ev_before_field, ev_after_field, stream);
+}
+
+size_t xrb_ngp_render_normals_workspace(int n_rays, int max_samples) {
+    return xrb_ngp_render_workspace(n_rays, max_samples) + xrb::align256((size_t)max_samples * 3 * sizeof(float));
+}
+
+int xrb_ngp_render_normals(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const uint8_t *bitfield, const float *rays_o, const float *rays_d, int n_rays,
+                           int max_samples, float aabb0, float aabb1, float near_distance, float cone_angle, uint64_t seed, int64_t n_prior_calls, const float *bg3_host, int rgb_act,
+                           int dens_act, float *rgb_out, float *alpha_out, float *depth_out, float *normal_out, int32_t *numsteps, int32_t *counters, void *workspace,
+                           void *ev_before_field, void *ev_after_field, void *stream) {
+    return xrb::render_chain(cfg, table, weight_image, bitfield, rays_o, rays_d, n_rays, max_samples, aabb0, aabb1, near_distance, cone_angle, seed, n_prior_calls, bg3_host, rgb_act,
+                             dens_act, rgb_out, alpha_out, true, depth_out, numsteps, counters, workspace, ev_before_field, ev_after_field, stream, true, normal_out);
 }
 
 }  // extern "C"

@@ -195,14 +195,17 @@ __global__ void __launch_bounds__(256) count_trained_kernel(int n_rays, const in
 }
 
 // ============================================================================ compositing (calc_rgb.cu)
-// what the depth composite (MODE 2) needs to rebuild each sample's t from its warped position
+// what the depth composite (MODE 2) needs to rebuild each sample's t from its warped position; MODE 3 also reads each row's density gradient
+// (grad f32[rows,3]) and writes normal_out f32[n_rays,3]
 struct CompositeDepth {
     const float *rays_o, *rays_d; float lo, diag; float *depth_out;
+    const float *grad; float *normal_out;
 };
 
 // MODE 0: training forward (per-ray bg, background only if not truncated; calc_rgb.cu:5-67)
 // MODE 1: inference (global bg, alpha out; calc_rgb.cu:143-206)
 // MODE 2: inference as MODE 1, plus depth = sum of w * t (include/xrnerf_b200.h, xrb_ngp_render_depth)
+// MODE 3: MODE 2, plus normal = sum of w * n, n = -g / |g| (0 where g = 0) of the row's gradient g (xrb_ngp_render_normals)
 template <int MODE>
 __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const float4 *__restrict__ raw, const float *__restrict__ coords, const int32_t *__restrict__ numsteps,
                                                             const int32_t *__restrict__ numsteps_c, const float *__restrict__ bg, float3 bg_global, int rgb_act, int dens_act,
@@ -217,48 +220,62 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const fl
         if (lane == 0) {
             rgb_out[3 * (size_t)ray] = b.x; rgb_out[3 * (size_t)ray + 1] = b.y; rgb_out[3 * (size_t)ray + 2] = b.z;
             if (MODE >= 1) alpha_out[ray] = 0.f;
-            if (MODE == 2) dp.depth_out[ray] = 0.f;
+            if (MODE >= 2) dp.depth_out[ray] = 0.f;
+            if (MODE == 3) { dp.normal_out[3 * (size_t)ray] = 0.f; dp.normal_out[3 * (size_t)ray + 1] = 0.f; dp.normal_out[3 * (size_t)ray + 2] = 0.f; }
         }
         continue;
     }
     float o[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f}, inv_dd = 1.f;   // one division per ray, not per sample
-    if (MODE == 2) {
+    if (MODE >= 2) {
         o[0] = __ldg(dp.rays_o + 3 * (size_t)ray); o[1] = __ldg(dp.rays_o + 3 * (size_t)ray + 1); o[2] = __ldg(dp.rays_o + 3 * (size_t)ray + 2);
         d[0] = __ldg(dp.rays_d + 3 * (size_t)ray); d[1] = __ldg(dp.rays_d + 3 * (size_t)ray + 1); d[2] = __ldg(dp.rays_d + 3 * (size_t)ray + 2);
         inv_dd = 1.f / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
     }
-    float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f, ad = 0.f;
+    float T = 1.f, ax = 0.f, ay = 0.f, az = 0.f, ad = 0.f, nx = 0.f, ny = 0.f, nz = 0.f;
     for (uint32_t k0 = 0; k0 < n; k0 += 32) {
         uint32_t k = k0 + lane; bool valid = k < n;
-        CompositeTerm s{0.f, 0.f, 0.f, 0.f}; float t = 0.f;
+        CompositeTerm s{0.f, 0.f, 0.f, 0.f}; float t = 0.f, n3[3] = {0.f, 0.f, 0.f};
         if (valid) {
             s = composite_term(__ldg(raw + base + k), row_dt(coords + ROW_FLOATS * (size_t)(base + k)), rgb_act, dens_act);
-            if (MODE == 2) t = row_t(coords + ROW_FLOATS * (size_t)(base + k), o, d, inv_dd, dp.lo, dp.diag);
+            if (MODE >= 2) t = row_t(coords + ROW_FLOATS * (size_t)(base + k), o, d, inv_dd, dp.lo, dp.diag);
+            if (MODE == 3) {   // the sample's outward unit normal: inside is the larger density
+                const float *gp = dp.grad + 3 * (size_t)(base + k);
+                const float g0 = __ldg(gp), g1 = __ldg(gp + 1), g2 = __ldg(gp + 2), len = norm3df(g0, g1, g2);
+                if (len > 0.f) { n3[0] = -g0 / len; n3[1] = -g1 / len; n3[2] = -g2 / len; }
+            }
         }
         float incl, ex = warp_excl_prod(1.f - s.alpha, lane, &incl);
         float w = s.alpha * (T * ex);
         ax += w * s.r; ay += w * s.g; az += w * s.b;
-        if (MODE == 2) ad += w * t;
+        if (MODE >= 2) ad += w * t;
+        if (MODE == 3) { nx += w * n3[0]; ny += w * n3[1]; nz += w * n3[2]; }
         T *= __shfl_sync(0xffffffffu, incl, 31);
     }
     ax = warp_sum(ax); ay = warp_sum(ay); az = warp_sum(az);
-    if (MODE == 2) ad = warp_sum(ad);
+    if (MODE >= 2) ad = warp_sum(ad);
+    if (MODE == 3) { nx = warp_sum(nx); ny = warp_sum(ny); nz = warp_sum(nz); }
     if (lane == 0) {
         bool add_bg = MODE >= 1 ? true : (n == (uint32_t)numsteps[2 * (size_t)ray]);  // :61-64 / :199-202
         if (add_bg) { ax += T * b.x; ay += T * b.y; az += T * b.z; }
         rgb_out[3 * (size_t)ray] = ax; rgb_out[3 * (size_t)ray + 1] = ay; rgb_out[3 * (size_t)ray + 2] = az;
         if (MODE >= 1) alpha_out[ray] = 1.f - T;
-        if (MODE == 2) dp.depth_out[ray] = ad;
+        if (MODE >= 2) dp.depth_out[ray] = ad;
+        if (MODE == 3) { dp.normal_out[3 * (size_t)ray] = nx; dp.normal_out[3 * (size_t)ray + 1] = ny; dp.normal_out[3 * (size_t)ray + 2] = nz; }
     }
     }
 }
 
 // the chain render's composite with depth (xrb_ngp_render_depth; arguments validated there)
 int launch_composite_depth(const float *raw, const float *coords, const int32_t *numsteps, const float *bg3_host, int n_rays, int rgb_act, int dens_act, const float *rays_o,
-                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s) {
-    const CompositeDepth dp{rays_o, rays_d, aabb0, aabb1 - aabb0, depth_out};
-    composite_fwd_kernel<2><<<warp_grid(n_rays), 256, 0, s>>>(n_rays, (const float4 *)raw, coords, numsteps, nullptr, nullptr, make_float3(bg3_host[0], bg3_host[1], bg3_host[2]),
-                                                              rgb_act, dens_act, rgb_out, alpha_out, dp);
+                           const float *rays_d, float aabb0, float aabb1, float *rgb_out, float *alpha_out, float *depth_out, cudaStream_t s, const float *grad,
+                           float *normal_out) {
+    const CompositeDepth dp{rays_o, rays_d, aabb0, aabb1 - aabb0, depth_out, grad, normal_out};
+    const float3 bg = make_float3(bg3_host[0], bg3_host[1], bg3_host[2]);
+    if (normal_out) {
+        composite_fwd_kernel<3><<<warp_grid(n_rays), 256, 0, s>>>(n_rays, (const float4 *)raw, coords, numsteps, nullptr, nullptr, bg, rgb_act, dens_act, rgb_out, alpha_out, dp);
+        return check_launch("ngp_render_normals composite");
+    }
+    composite_fwd_kernel<2><<<warp_grid(n_rays), 256, 0, s>>>(n_rays, (const float4 *)raw, coords, numsteps, nullptr, nullptr, bg, rgb_act, dens_act, rgb_out, alpha_out, dp);
     return check_launch("ngp_render_depth composite");
 }
 

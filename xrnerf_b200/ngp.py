@@ -191,6 +191,21 @@ class NgpField(nn.Module):
         _C.check(_C.lib.xrb_ngp_density_grad(self.cfg, self.tab, _C.ptr(self._dens16), pp, ps, n, _C.f32(density), _C.f32(grad), _C.stream()), 'ngp_density_grad')
         return density, grad
 
+    def density_grad_tc(self, pts, density=True, order=None, n_rows_dev=None):
+        """pts: [n,3] float32 view in the warped [0,1]^3 domain (row stride may be > 3, e.g. the chain's sample rows). -> (density f32[n,1] or None,
+        grad f32[n,3]): the raw density, bit-identical to run_density(pts, impl=1), and its position gradient on tensor cores (xrb_ngp_density_grad_tc,
+        include/xrnerf_b200.h: the gradient that the normal maps use). order (int32 device tensor, optional): slot j evaluates row order[j], a permutation
+        of the effective rows; n_rows_dev (int32 device tensor, optional): only the first min(n, n_rows_dev[0]) rows are written."""
+        _C.require_cuda(pts, order, n_rows_dev)
+        self.refresh()
+        pp, ps = _C.rows(pts)
+        n = pts.shape[0]
+        dens = torch.empty((n, 1), dtype=torch.float32, device=pts.device) if density else None
+        grad = torch.empty((n, 3), dtype=torch.float32, device=pts.device)
+        _C.check(_C.lib.xrb_ngp_density_grad_tc(self.cfg, self.tab, _C.ptr(self._image), pp, ps, n, _C.i32(n_rows_dev), _C.i32(order), _C.f32(dens), _C.f32(grad), _C.stream()),
+                 'ngp_density_grad_tc')
+        return dens, grad
+
     def density_lattice(self, shape, box=((0.0, 0.0, 0.0), (1.0, 1.0, 1.0)), impl=None):
         """Raw density on the lattice of shape (nz, ny, nx) over box = (box_min, box_max) in the warped [0,1]^3 domain -> f32[nz,ny,nx] on the field's
         device (x fastest). Lattice positions and limits: xrb_ngp_density_lattice (include/xrnerf_b200.h); each value equals run_density at that position."""
@@ -237,11 +252,12 @@ def _rays(t):
     return t.contiguous()
 
 
-def _depth_ptr(depth, n, device):
-    """pointer of a caller-owned depth output: a dense float32 tensor of n elements on the rays' device"""
-    if not torch.is_tensor(depth) or depth.dtype != torch.float32 or depth.numel() != n or depth.device != device:
+def _depth_ptr(depth, n, device, name='depth', width=1):
+    """pointer of a caller-owned depth (width 1) or normal (width 3) output: a dense float32 tensor of n * width elements on the rays' device"""
+    if not torch.is_tensor(depth) or depth.dtype != torch.float32 or depth.numel() != n * width or depth.device != device or (width > 1 and depth.shape[-1] != width):
         what = f'{depth.dtype} {tuple(depth.shape)} on {depth.device}' if torch.is_tensor(depth) else type(depth).__name__
-        raise _C.XrbError(f'XRB_E_BADARG: depth must be a float32 tensor of {n} elements on {device}, got {what}')
+        shape = f'of {n} elements' if width == 1 else f'of shape [{n},{width}]'
+        raise _C.XrbError(f'XRB_E_BADARG: {name} must be a float32 tensor {shape} on {device}, got {what}')
     return _C.f32(depth)
 
 
@@ -276,19 +292,25 @@ class NgpRenderer:
         """0-dim bool tensor (device): did the last chain render drop rays because the batch marched more samples than the budget holds?"""
         return counters[1] > self._max_samples
 
-    def render(self, rays_o, rays_d, bitfield, out=None, profile_events=None, depth=None):
+    def render(self, rays_o, rays_d, bitfield, out=None, profile_events=None, depth=None, normals=None, max_samples=None):
         """profile_events: optional (torch.cuda.Event, torch.cuda.Event) recorded right before / after the field kernel (bench roofline).
         depth: optional caller-owned float32 tensor of n elements on the rays' device, filled with each ray's depth (xrb_ngp_render_depth,
-        include/xrnerf_b200.h); the returned tuple is the same either way."""
+        include/xrnerf_b200.h); the returned tuple is the same either way.
+        normals: optional caller-owned float32 [n,3] tensor on the rays' device, filled with each ray's normal (xrb_ngp_render_normals: sum of w * the
+        samples' outward unit normals, not normalised); it needs `depth` as well. max_samples: rows of the sample buffer (default n * the budget)."""
+        if normals is not None and depth is None:
+            raise _C.XrbError('XRB_E_BADARG: normals need a depth output as well (xrb_ngp_render_normals writes both)')
         _C.require_cuda(rays_o, rays_d, bitfield)
         rays_o, rays_d = _rays(rays_o), _rays(rays_d)
         n = rays_o.shape[0]
         depth_p = None if depth is None else _depth_ptr(depth, n, rays_o.device)
+        normal_p = None if normals is None else _depth_ptr(normals, n, rays_o.device, 'normals', 3)
         f = self.field
         f.refresh()
-        max_samples = n * self.budget
+        max_samples = n * self.budget if max_samples is None else int(max_samples)
         self._max_samples = max_samples
-        need = _C.lib.xrb_ngp_render_workspace(n, max_samples)
+        ws_bytes = _C.lib.xrb_ngp_render_workspace if normal_p is None else _C.lib.xrb_ngp_render_normals_workspace
+        need = ws_bytes(n, max_samples)
         if self._ws is None or self._ws.numel() < need or self._ws.device != rays_o.device:
             self._ws = torch.empty(need, dtype=torch.uint8, device=rays_o.device)
         if out is None:
@@ -306,8 +328,10 @@ class NgpRenderer:
         tail = (_C.i32(numsteps), _C.i32(counters), _C.ptr(self._ws), ev0, ev1, _C.stream())
         if depth_p is None:
             _C.check(_C.lib.xrb_ngp_render(*head, *tail), 'ngp_render')
-        else:
+        elif normal_p is None:
             _C.check(_C.lib.xrb_ngp_render_depth(*head, depth_p, *tail), 'ngp_render_depth')
+        else:
+            _C.check(_C.lib.xrb_ngp_render_normals(*head, depth_p, normal_p, *tail), 'ngp_render_normals')
         self.calls += 1
         return rgb, alpha, numsteps, counters
 

@@ -351,6 +351,8 @@ class MipNerfNetwork(NerfNetwork):
 
 @NETWORKS.register_module()
 class HashNerfNetwork(NerfNetwork):
+    render_normals = False   # True: the test path also returns per-pixel normal maps (batchify_forward)
+
     def __init__(self, cfg, sampler=None, mlp=None, render=None):
         super().__init__(cfg)
         self.sampler = builder.build_sampler(sampler)
@@ -368,8 +370,14 @@ class HashNerfNetwork(NerfNetwork):
         Here the test path is ONE fused launch per call for any number of rays (xrb_ngp_render_fused; no chunk loop, no host sync, no [S,7]/[S,4] buffers);
         `fused_inference = False` or training falls back to the reference-shaped chunk loop over forward().
         The fused path also returns each ray's `depth` [n,1] (sum of w * t, not divided by alpha) and `disp` [n,1] (xrnerf_b200.ngp.disparity: 0 where
-        alpha == 0); the reference-shaped path returns the reference's keys only."""
+        alpha == 0); the reference-shaped path returns the reference's keys only.
+        `render_normals` (default False) selects the normal-map output: the test path then renders through the chain (xrb_ngp_render_normals) and also
+        returns each ray's `normal` [n,3] (sum of w * the samples' outward unit normals, not normalised; include/xrnerf_b200.h "Normal maps"); rgb,
+        depth and disp come from the same chain render. It needs the fused path: with `fused_inference = False` it raises NotImplementedError."""
         smp = self.sampler
+        normals = is_test and getattr(self, 'render_normals', False)
+        if normals and not getattr(self, 'fused_inference', True):
+            raise NotImplementedError('render_normals: normal maps come from the fused NGP renderer; set fused_inference = True')
         if not (is_test and getattr(self, 'fused_inference', True) and data['rays_o'].is_cuda and hasattr(smp, 'aabb_range')):
             return self._chunked_forward(data, is_test)
         from ..ngp import NgpRenderer, disparity
@@ -382,9 +390,28 @@ class HashNerfNetwork(NerfNetwork):
         r.calls = rm.rng_calls['ray_sampler']               # the same jitter stream the unfused path would use next (hidden static pcg32 of the reference, Q9)
         rays_o = data['rays_o'].contiguous().float()
         depth = torch.empty((rays_o.shape[0], 1), dtype=torch.float32, device=rays_o.device)
+        if normals:
+            return self._render_normals(r, rays_o, data['rays_d'].contiguous().float(), depth)
         rgb, alpha, _ = r.render_fused(rays_o, data['rays_d'].contiguous().float(), smp.density_grid_bitfield, depth=depth)
         rm.rng_calls['ray_sampler'] += 1
         return {'rgb': rgb.clone(), 'alpha': alpha.clone(), 'depth': depth, 'disp': disparity(depth, alpha)}
+
+    def _render_normals(self, r, rays_o, rays_d, depth):
+        """the `render_normals` view through the chain render. The sample buffer holds the renderer's budget per ray; a view that marched more rows is
+        rendered again with a buffer of exactly its row count and the same call index (the same jitter), so no ray is dropped. One host read per view."""
+        import xrnerf_b200.raymarch_cuda as rm
+        from ..ngp import disparity
+        n = rays_o.shape[0]
+        normal = torch.empty((n, 3), dtype=torch.float32, device=rays_o.device)
+        calls, bitfield = rm.rng_calls['ray_sampler'], self.sampler.density_grid_bitfield
+        r.calls = calls
+        rgb, alpha, _, counters = r.render(rays_o, rays_d, bitfield, depth=depth, normals=normal)
+        marched = int(counters[1].item())
+        if marched > n * r.budget:
+            r.calls = calls
+            rgb, alpha, _, counters = r.render(rays_o, rays_d, bitfield, depth=depth, normals=normal, max_samples=marched)
+        rm.rng_calls['ray_sampler'] += 1
+        return {'rgb': rgb.clone(), 'alpha': alpha.clone(), 'depth': depth, 'disp': disparity(depth, alpha), 'normal': normal}
 
     def val_step(self, data, optimizer=None, **kwargs):
         """hashnerf.py:54-93 (rank-0 loop over validation poses) with the image rendered by one launch and the PSNR taken on the device; every rank renders the
@@ -397,7 +424,7 @@ class HashNerfNetwork(NerfNetwork):
         self.mlp.mark_dirty()
         data = {k: unfold_batching(v) for k, v in data.items()}
         poses, images = data['poses'], data.get('images')
-        rgbs, disps, gt_imgs, psnrs, elapsed = [], [], [], [], []
+        rgbs, disps, normals, gt_imgs, psnrs, elapsed = [], [], [], [], [], []
         with torch.no_grad():
             for i in range(poses.shape[0]):
                 t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -407,6 +434,8 @@ class HashNerfNetwork(NerfNetwork):
                 rgb = recover_shape(ret['rgb'], d['src_shape'])
                 if 'disp' in ret:
                     disps.append(recover_shape(ret['disp'], d['src_shape']))
+                if 'normal' in ret:
+                    normals.append(recover_shape(ret['normal'], d['src_shape']))
                 if images is not None:
                     alpha = images[i][..., 3:].to(rgb.device)
                     gt = images[i][..., :3].to(rgb.device) * alpha
@@ -416,7 +445,10 @@ class HashNerfNetwork(NerfNetwork):
                 t1.record()
                 rgbs.append(rgb); elapsed.append((t0, t1))
         torch.cuda.synchronize()
-        return {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+        out = {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+        if getattr(self, 'render_normals', False):
+            out['normals'] = normals      # one [H,W,3] normal map per pose (batchify_forward)
+        return out
 
     def test_step(self, data, **kwargs):
         """hashnerf.py:95-111: one spiral pose per call; `data` already holds the pose's rays (rays_o, rays_d, src_shape, idx) from the test pipeline.
@@ -433,6 +465,8 @@ class HashNerfNetwork(NerfNetwork):
         out = {'spiral_rgb': ret['rgb'], 'spiral_alpha': ret['alpha']}
         if 'disp' in ret:
             out['spiral_disp'] = ret['disp']
+        if 'normal' in ret:
+            out['spiral_normal'] = ret['normal']
         if 'src_shape' in d:
             out = {k: recover_shape(v, d['src_shape']) for k, v in out.items()}
         out['idx'] = idx
