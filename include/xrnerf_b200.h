@@ -332,6 +332,38 @@ int xrb_ngp_render_normals(const xrb_ngp_config *cfg, const xrb_ngp_table *table
 
 
 /* ------------------------------------------------------------------------------------------------
+ * NeRF / Mip-NeRF normal maps (csrc/nerf_grad_tc.cu; the fused renderers xrnerf_b200.nerf.NerfRenderer / MipNerfRenderer with normals=True)
+ *   per-sample gradient  g_k = d(raw density, NerfMLP output 3 = alpha_linear, before the render's activation) / d(position) of sample k, where the
+ *                        position is, for NeRF, p = o + d z formed as the ray encoder forms it (a rounded product, then a rounded sum), and for
+ *                        Mip-NeRF the mean mu of the sample's conical-frustum Gaussian (cast_rays), its covariance held fixed;
+ *   per-sample normal    n_k = -g_k / |g_k| in fp32, 0 where g_k = 0 (the rule of xrnerf_b200.mesh.outward_normals);
+ *   per-ray normal       normal = sum_k w_k n_k over the LAST level only (the fine level of NeRF with N_importance > 0, the last level of Mip-NeRF),
+ *                        w_k the weights that level's composite returns (the bits rgb is formed from). No background term, NOT normalised, 0 for a
+ *                        ray whose weights are all 0. Positions are in the rays' frame, so the normal needs no frame map.
+ * ---------------------------------------------------------------------------------------------- */
+/* The raw density and g for every row of a ray batch's encoding image, one wgmma kernel per call (no activation leaves the SM):
+ *   the trunk (pts_linears.0..7 and the alpha dot) runs as in xrb_nerf_mlp_forward, so density_out[i] (f32[n_rays*S], may be NULL) is bit-identical
+ *   to raw[i, 3] of xrb_nerf_mlp_forward on the same weight_image, bias and enc_image. Each ReLU mask is the forward's (a unit is live iff
+ *   fp16(acc) + fp16(b) > 0). The backward runs on fp16 operands with fp32 accumulation; each row's d(density)/d(hidden) is scaled by a power of two
+ *   before its fp16 rounding, so the result is finite whenever fp32 allows. d(density)/d(encoding) is the sum, in fp32 and in this order, of the skip
+ *   layer's point columns' term and pts_linears.0's term, contracted with the encoding's derivative at the fp32 position.
+ * weight_image, bias: pack_nerf_mlp; grad_image: pack_nerf_mlp_grad of the same weights (W^T of pts_linears.7 .. .1 and the point columns of .5 and .0);
+ * enc_image: the ray encoder's tile image of these rows (xrb_nerf_posenc_tiles_rays with multires 10 / 4, or xrb_mip_ipe_tiles_rays with 16 point and
+ * 4 view bands); rays_o, rays_d f32[n_rays,3]; z_vals f32[n_rays,S] (NeRF) or f32[n_rays,S+1] (Mip-NeRF interval ends); radii f32[n_rays];
+ * grad_out f32[n_rays*S,3]. Only the fused NerfMLP shape is implemented: input channels (63, 27) for NeRF, (96, 27) with max_deg_point - min_deg_point
+ * = 16 for Mip-NeRF; anything else returns XRB_E_UNSUPPORTED. n_rays < 0 or S < 1 returns XRB_E_BADARG; n_rays == 0 is a no-op that touches no
+ * pointer; a null pointer (other than density_out), or an image or bias that is not 16-byte aligned, returns XRB_E_BADARG. All before any CUDA call. */
+int xrb_nerf_density_grad_rays(const void *weight_image, const void *grad_image, const float *bias, const void *enc_image, const float *rays_o,
+                               const float *rays_d, const float *z_vals, int n_rays, int S, int input_ch, int input_ch_dirs, float *density_out,
+                               float *grad_out, void *stream);
+int xrb_mip_density_grad_rays(const void *weight_image, const void *grad_image, const float *bias, const void *enc_image, const float *rays_o,
+                              const float *rays_d, const float *z_vals, const float *radii, int n_rays, int S, int input_ch, int input_ch_dirs,
+                              int min_deg_point, int max_deg_point, float *density_out, float *grad_out, void *stream);
+/* normal_out f32[n_rays,3] <- sum over k = 0, 1, .. S-1 in that order of w_k n_k, n_k = -g_k / norm3df(g_k) (0 where g_k = 0); weights f32[n_rays,S],
+ * grad f32[n_rays*S,3]. n_rays < 0 or S < 1 returns XRB_E_BADARG; n_rays == 0 is a no-op; null pointers return XRB_E_BADARG before any CUDA call. */
+int xrb_nerf_composite_normals(const float *weights, const float *grad, int n_rays, int S, float *normal_out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * NeRF / Mip-NeRF composite + sampling kernels (pure-PyTorch in the reference)
  * ---------------------------------------------------------------------------------------------- */
 

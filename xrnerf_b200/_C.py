@@ -101,6 +101,9 @@ _SIGS = {
     'xrb_nerf_sample_pdf': (_i, [P, P, P, P, P, _i, _i, _i, P, P, P]),
     'xrb_nerf_posenc': (_i, [P, P, _i64, _i, _i, _i, P, P]),
     'xrb_nerf_mlp_forward': (_i, [P, P, P, _i64, _i, _i, P, P]),
+    'xrb_nerf_density_grad_rays': (_i, [P, P, P, P, P, P, P, _i, _i, _i, _i, P, P, P]),
+    'xrb_mip_density_grad_rays': (_i, [P, P, P, P, P, P, P, P, _i, _i, _i, _i, _i, _i, P, P, P]),
+    'xrb_nerf_composite_normals': (_i, [P, P, _i, _i, P, P]),
     'xrb_nerf_enc_image_bytes': (_sz, [_i64, _i]),
     'xrb_nerf_pack_embedded': (_i, [P, _i64, _i, _i, P, P]),
     'xrb_nerf_posenc_tiles': (_i, [P, P, _i64, _i, _i, _i, P, P]),

@@ -208,34 +208,6 @@ __device__ __forceinline__ float mip_dir_col(const float *vd, int c, int n_deg_v
     return sinf(x);
 }
 
-// cast_rays (networks/utils/mip.py:117-129): the conical frustum -> Gaussian (:91-114), lift_gaussian (:66-88), diagonal covariance
-__device__ __forceinline__ void frustum_gaussian(float t0, float t1, float radius, const float d[3], const float o[3], float dmag_sq, float mean[3], float cov[3]) {
-    float mu = (t0 + t1) / 2.f, hw = (t1 - t0) / 2.f;
-    float mu2 = mu * mu, hw2 = hw * hw, hw4 = hw2 * hw2, den = 3.f * mu2 + hw2;
-    float t_mean = mu + (2.f * mu * hw2) / den;
-    float t_var = hw2 / 3.f - (4.f / 15.f) * ((hw4 * (12.f * mu2 - hw2)) / (den * den));
-    float r_var = radius * radius * (mu2 / 4.f + (5.f / 12.f) * hw2 - 4.f / 15.f * hw4 / den);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        float dd = d[c] * d[c];
-        mean[c] = d[c] * t_mean + o[c];
-        cov[c] = t_var * dd + r_var * (1.f - dd / dmag_sq);
-    }
-}
-// the Gaussian of sample k (interval z[k], z[k+1]) of ray `ray`
-__device__ __forceinline__ void sample_gaussian(const float *z_vals, const float *rays_o, const float *rays_d, const float *radii, int S, int64_t ray, int k, float mean[3],
-                                                float cov[3]) {
-    const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
-    const float o[3] = {rays_o[3 * ray], rays_o[3 * ray + 1], rays_o[3 * ray + 2]};
-    const float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    frustum_gaussian(z_vals[ray * (S + 1) + k], z_vals[ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
-}
-// GetPts (create.py:588-597): o + d * z as a rounded product then a rounded sum (torch), never an FMA — the 2^9-scaled sin arguments amplify the difference
-__device__ __forceinline__ void get_pts(const float *rays_o, const float *rays_d, int64_t ray, float z, float p[3]) {
-#pragma unroll
-    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(rays_o[3 * ray + a], __fmul_rn(rays_d[3 * ray + a], z));
-}
-
 // BaseEmbedder.forward (embedders/base.py:57-74): one thread per output element (coalesced row writes)
 __global__ void __launch_bounds__(256) posenc_kernel(int64_t n_pts, int samples_per_ray, int multires, int multires_dirs, const float *__restrict__ pts,
                                                      const float *__restrict__ viewdirs, float *__restrict__ out) {

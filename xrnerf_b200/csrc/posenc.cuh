@@ -2,7 +2,9 @@
 // the same fp16 tile-image values: the fast tile-image encoder (csrc/nerf.cu) and the NerfMLP density lattice (csrc/nerf_mlp_tc.cu). Likewise the
 // integrated positional encoding of a Mip-NeRF point query (ipe_point_bands): the point encoder (csrc/nerf.cu) and the Mip-NeRF density lattice
 // (csrc/nerf_mlp_tc.cu); and Mip-NeRF's view-direction bands (mip_dir_bands): the ray and point encoders (csrc/nerf.cu). Each point encoding's
-// derivative (posenc_bands_grad, ipe_point_bands_grad) sits beside it, for the gradient kernel of csrc/nerf.cu.
+// derivative (posenc_bands_grad, ipe_point_bands_grad) sits beside it, for the gradient kernel of csrc/nerf.cu; the ray IPE's (ipe_ray_grad) serves the
+// normal-map gradient kernel of csrc/nerf_grad_tc.cu. A ray sample's position (get_pts, sample_gaussian) is defined here once, for the ray encoders of
+// csrc/nerf.cu and that gradient kernel.
 #pragma once
 #include <stdint.h>
 #include <cmath>
@@ -96,6 +98,54 @@ __device__ __forceinline__ void ipe_point_bands_grad(const float *x, const IpeBa
         for (int a = 0; a < 3; ++a) {
             const float y = x[a] * sc;
             g[a] += f * sc * (cosf(y) * e(3 * k + a) + cosf(y + HALF_PI) * e(3 * B.n_deg + 3 * k + a));
+        }
+    }
+}
+
+// ---- a ray sample's position. NeRF: the point o + d z; Mip-NeRF: the Gaussian of the sample's conical frustum (its mean is the position)
+// cast_rays (networks/utils/mip.py:117-129): the conical frustum -> Gaussian (:91-114), lift_gaussian (:66-88), diagonal covariance
+__device__ __forceinline__ void frustum_gaussian(float t0, float t1, float radius, const float d[3], const float o[3], float dmag_sq, float mean[3], float cov[3]) {
+    float mu = (t0 + t1) / 2.f, hw = (t1 - t0) / 2.f;
+    float mu2 = mu * mu, hw2 = hw * hw, hw4 = hw2 * hw2, den = 3.f * mu2 + hw2;
+    float t_mean = mu + (2.f * mu * hw2) / den;
+    float t_var = hw2 / 3.f - (4.f / 15.f) * ((hw4 * (12.f * mu2 - hw2)) / (den * den));
+    float r_var = radius * radius * (mu2 / 4.f + (5.f / 12.f) * hw2 - 4.f / 15.f * hw4 / den);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        float dd = d[c] * d[c];
+        mean[c] = d[c] * t_mean + o[c];
+        cov[c] = t_var * dd + r_var * (1.f - dd / dmag_sq);
+    }
+}
+// the Gaussian of sample k (interval z[k], z[k+1]) of ray `ray`
+__device__ __forceinline__ void sample_gaussian(const float *z_vals, const float *rays_o, const float *rays_d, const float *radii, int S, int64_t ray, int k, float mean[3],
+                                                float cov[3]) {
+    const float d[3] = {rays_d[3 * ray], rays_d[3 * ray + 1], rays_d[3 * ray + 2]};
+    const float o[3] = {rays_o[3 * ray], rays_o[3 * ray + 1], rays_o[3 * ray + 2]};
+    const float dmag = fmaxf(1e-10f, d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    frustum_gaussian(z_vals[ray * (S + 1) + k], z_vals[ray * (S + 1) + k + 1], radii[ray], d, o, dmag, mean, cov);
+}
+// GetPts (create.py:588-597): o + d * z as a rounded product then a rounded sum (torch), never an FMA — the 2^9-scaled sin arguments amplify the difference
+__device__ __forceinline__ void get_pts(const float *rays_o, const float *rays_d, int64_t ray, float z, float p[3]) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(rays_o[3 * ray + a], __fmul_rn(rays_d[3 * ray + a], z));
+}
+
+// the gradient with respect to the mean of the ray IPE columns mip_ipe_tiles_fast_kernel writes (NDEG bands from min_deg, covariance cov held fixed),
+// given e(c) = dL/d(column c):
+//   g_a = sum_k exp(-0.5 cov_a 4^deg) 2^deg (cos(y) e(3k + a) + cos(y + pi/2) e(3 NDEG + 3k + a)),  y = mean_a 2^deg, deg = min_deg + k,
+// with the encoder's dead-band rule: a band whose 0.5 cov_a 4^deg exceeds 20 is constant zero
+template <int NDEG, class E>
+__device__ __forceinline__ void ipe_ray_grad(const float *mean, const float *cov, int min_deg, E e, float *g) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) g[a] = 0.f;
+#pragma unroll
+    for (int k = 0; k < NDEG; ++k) {
+        const float sc = pow2i(min_deg + k);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const float y = mean[a] * sc, hv = 0.5f * (cov[a] * sc * sc);
+            if (hv <= 20.f) g[a] += expf(-hv) * sc * (cosf(y) * e(3 * k + a) + cosf(y + HALF_PI) * e(3 * NDEG + 3 * k + a));
         }
     }
 }

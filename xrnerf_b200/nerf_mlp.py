@@ -135,6 +135,33 @@ def pack_nerf_mlp(mlp):
     return torch.from_numpy(np.concatenate(slabs)).to(dev), torch.from_numpy(np.concatenate([f32, h16.view(np.float32)])).to(dev)
 
 
+def pack_nerf_mlp_grad(mlp):
+    """The gradient image of the density-gradient kernel (xrb_nerf_density_grad_rays): W^T of the trunk as B operands, in the order its producer
+    streams them — pts_linears.7, .6, the point columns of .5, the hidden columns of .5, then .4 .. .1, the point columns of .0. A 256-wide step is
+    four K-blocks of W^T (K = the layer's outputs), each as two K-halves [256 x 32] (SWIZZLE_64B, as pack_nerf_mlp's); a point step is [NP x 64]
+    slabs (SWIZZLE_128B) of W[:, :input_ch]^T zero padded to NP = 64 (NeRF) or 128 (Mip-NeRF) rows."""
+    assert fused_shape(mlp), 'fused NerfMLP kernel: netdepth=8, netwidth=256, skips=[4], use_viewdirs=True, input channels (63, 27) or (96, 27)'
+    ic = mlp.input_ch
+    n_pts = 64 if ic <= 64 else 128
+    W = [lin.weight.detach().float().cpu().numpy() for lin in mlp.pts_linears]
+    slabs = []
+
+    def wide(wt):
+        for j in range(4):
+            blk = wt[:, 64 * j:64 * (j + 1)]
+            slabs.extend(_slab64(np.ascontiguousarray(blk[:, 32 * kh:32 * (kh + 1)])) for kh in range(2))
+
+    def points(wp):
+        wt = np.zeros((n_pts, 256), np.float32)
+        wt[:ic] = wp.T
+        slabs.extend(_slab(np.ascontiguousarray(wt[:, 64 * j:64 * (j + 1)])) for j in range(4))
+    wide(W[7].T); wide(W[6].T); points(W[5][:, :ic]); wide(W[5][:, ic:].T)
+    for l in (4, 3, 2, 1):
+        wide(W[l].T)
+    points(W[0])
+    return torch.from_numpy(np.concatenate(slabs)).to(mlp.pts_linears[0].weight.device)
+
+
 def nerf_mlp_forward(image, bias, embedded, input_ch, input_ch_dirs):
     """fp32 embedded rows [n, input_ch + input_ch_dirs] -> raw [n, 4]: packs the fp16 encoding tile image (one streaming kernel), then runs the MLP kernel,
     which TMA-loads it. image/bias come from pack_nerf_mlp."""

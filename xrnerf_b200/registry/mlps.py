@@ -118,13 +118,38 @@ class NerfMLP(BaseMLP):
         with torch.no_grad():
             return nerf_train.density_grad(self, pts.detach().reshape(-1, 3).contiguous().float(), sigma=sigma)
 
-    def _packed(self):
+    def density_grad_rays(self, rays_o, rays_d, z_vals, radii=None, enc=None):
+        """The raw density and its gradient at every sample of a set of rays -> (density f32[n*S], grad f32[n*S,3]), from one tensor-core kernel
+        (xrb_nerf_density_grad_rays / xrb_mip_density_grad_rays, include/xrnerf_b200.h "NeRF / Mip-NeRF normal maps"): rays_o, rays_d f32[n,3];
+        z_vals f32[n,S] (BaseEmbedder: positions o + d z) or, with a MipNerfEmbedder, f32[n,S+1] interval ends and radii f32[n] (positions: the
+        frustum Gaussians' means). enc: the rows' encoding tile image (None: formed here by the renderer's encoder, xrnerf_b200.nerf.encode_rays).
+        density is bit-identical to the inference kernel's raw[:, 3] on that image."""
+        from ..nerf import density_grad_rays, encode_rays
+        self._mesh_check(rays_o)
+        o, d, z = (t.contiguous().float() for t in (rays_o, rays_d, z_vals))
+        rad = None if radii is None else radii.reshape(-1).contiguous().float()
+        n, s = z.shape[0], z.shape[1] - (1 if self._is_mip() else 0)
+        if enc is None:
+            enc = encode_rays(self, o, d, d, z, rad)
+        density = torch.empty(n * s, dtype=torch.float32, device=o.device)
+        grad = density_grad_rays(self, enc, o, d, z, rad, density)
+        return density, grad
+
+    def _packed(self, grad=False):
+        """(weight image, bias) of pack_nerf_mlp, and with grad=True also pack_nerf_mlp_grad's image of the same weights; each is packed once per weight
+        version (mark_dirty forgets both)"""
         ver = tuple(p._version for p in self.parameters()) + (self.pts_linears[0].weight.device,)
         if getattr(self, '_pack_ver', None) != ver:
             from ..nerf_mlp import pack_nerf_mlp
             self._pack = pack_nerf_mlp(self)
+            self._pack_grad = None
             self._pack_ver = ver
-        return self._pack
+        if not grad:
+            return self._pack
+        if self._pack_grad is None:
+            from ..nerf_mlp import pack_nerf_mlp_grad
+            self._pack_grad = pack_nerf_mlp_grad(self)
+        return self._pack + (self._pack_grad,)
 
     def batchify_run_mlp(self, x):
         if self._fused_ok(x):   # inference: the whole 12-GEMM chain in one wgmma kernel, no chunking needed (activations never leave the SM)

@@ -73,6 +73,8 @@ def resample_along_rays(data, randomized, ray_shape, resample_padding, rand=None
 
 @NETWORKS.register_module()
 class NerfNetwork(nn.Module):
+    render_normals = False   # True: the fused test path also returns per-pixel normal maps of the last level (batchify_forward)
+
     def __init__(self, cfg, mlp=None, mlp_fine=None, render=None):
         super().__init__()
         self.phase = cfg.get('phase', 'train')
@@ -104,6 +106,9 @@ class NerfNetwork(nn.Module):
         (nerf.py:50-69), which returns the reference's keys only."""
         if is_test and getattr(self, 'fused_inference', True) and self._fused_ok(data['rays_o']):
             return self._fused_forward(data)
+        if is_test and self.render_normals:
+            raise NotImplementedError('render_normals: normal maps come from the fused NeRF / Mip-NeRF renderer (CUDA rays, the fused NerfMLP shape); '
+                                      'set fused_inference = True')
         return self._chunked_forward(data, is_test)
 
     def _fused_mlps(self):
@@ -119,7 +124,7 @@ class NerfNetwork(nn.Module):
     def _fused_forward(self, data):
         from ..nerf import NerfRenderer
         r = NerfRenderer(self, ray_batch=getattr(self, 'fused_ray_batch', None))
-        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], z_vals=data.get('z_vals'), depth=True)
+        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], z_vals=data.get('z_vals'), depth=True, normals=self.render_normals)
 
     def _chunked_forward(self, data, is_test):
         N = data[self.bs_data].shape[0]
@@ -150,13 +155,14 @@ class NerfNetwork(nn.Module):
         """nerf.py:94-142: phase 'test' dispatches to test_step. Otherwise renders data['poses'] and, when given, data['spiral_poses'] through the
         installed val pipeline (rank 0 only in the reference; here every rank renders what it is given). Returns the reference's keys as device tensors:
         rgbs [H,W,3] and disps [H,W,1] per pose, gt_imgs (data['images'] per pose, when given), spiral_rgbs / spiral_disps, elapsed_time per pose in
-        seconds (pipeline + render, CUDA events); plus psnr per pose, taken on the device against images[..., :3]."""
+        seconds (pipeline + render, CUDA events); plus psnr per pose, taken on the device against images[..., :3]. With `render_normals` also normals
+        and spiral_normals: one [H,W,3] normal map per pose (batchify_forward's `normal`)."""
         if self.phase == 'test':
             return self.test_step(data, **kwargs)
         self._mark_dirty()
         data = {k: unfold_batching(v) for k, v in data.items()}
         poses, images, spiral = data['poses'], data.get('images'), data.get('spiral_poses')
-        rgbs, disps, gt_imgs, psnrs, elapsed, spiral_rgbs, spiral_disps = [], [], [], [], [], [], []
+        rgbs, disps, gt_imgs, psnrs, elapsed, spiral_rgbs, spiral_disps, normals, spiral_normals = [], [], [], [], [], [], [], [], []
         with torch.no_grad():
             for i in range(poses.shape[0]):
                 t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -166,6 +172,8 @@ class NerfNetwork(nn.Module):
                 rgb = recover_shape(ret['rgb'], d['src_shape'])
                 t1.record()
                 rgbs.append(rgb); disps.append(recover_shape(ret['disp'], d['src_shape'])); elapsed.append((t0, t1))
+                if 'normal' in ret:
+                    normals.append(recover_shape(ret['normal'], d['src_shape']))
                 if images is not None:
                     gt = images[i].to(rgb.device)
                     gt_imgs.append(gt)
@@ -174,13 +182,18 @@ class NerfNetwork(nn.Module):
                 d = self.val_pipeline({'pose': spiral[i], 'idx': i})
                 ret = self.batchify_forward(d, is_test=True)
                 spiral_rgbs.append(recover_shape(ret['rgb'], d['src_shape'])); spiral_disps.append(recover_shape(ret['disp'], d['src_shape']))
+                if 'normal' in ret:
+                    spiral_normals.append(recover_shape(ret['normal'], d['src_shape']))
         torch.cuda.synchronize()
-        return {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'spiral_rgbs': spiral_rgbs, 'spiral_disps': spiral_disps,
-                'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+        out = {'rgbs': rgbs, 'disps': disps, 'gt_imgs': gt_imgs, 'spiral_rgbs': spiral_rgbs, 'spiral_disps': spiral_disps,
+               'elapsed_time': [a.elapsed_time(b) * 1e-3 for a, b in elapsed], 'psnr': [float(p.item()) for p in psnrs]}
+        if self.render_normals:
+            out['normals'], out['spiral_normals'] = normals, spiral_normals
+        return out
 
     def test_step(self, data, **kwargs):
         """nerf.py:144-169: one test pose (data['pose'], data['image'], data['idx']) through the installed val pipeline -> rgb [H,W,3], disp [H,W,1],
-        gt_img (data['image'] on the render's device) and idx (an int)."""
+        gt_img (data['image'] on the render's device) and idx (an int); with `render_normals` also normal [H,W,3]."""
         self._mark_dirty()
         data = {k: unfold_batching(v) for k, v in data.items()}
         idx = data['idx']
@@ -189,7 +202,10 @@ class NerfNetwork(nn.Module):
             d = self.val_pipeline({'pose': data['pose'], 'idx': idx})
             ret = self.batchify_forward(d, is_test=True)
         rgb = recover_shape(ret['rgb'], d['src_shape'])
-        return {'rgb': rgb, 'disp': recover_shape(ret['disp'], d['src_shape']), 'gt_img': data['image'].to(rgb.device), 'idx': idx}
+        out = {'rgb': rgb, 'disp': recover_shape(ret['disp'], d['src_shape']), 'gt_img': data['image'].to(rgb.device), 'idx': idx}
+        if 'normal' in ret:
+            out['normal'] = recover_shape(ret['normal'], d['src_shape'])
+        return out
 
     def set_val_pipeline(self, func):
         self.val_pipeline = func
@@ -302,21 +318,22 @@ class MipNerfNetwork(NerfNetwork):
     def _fused_forward(self, data):
         from ..nerf import MipNerfRenderer
         r = MipNerfRenderer(self, ray_batch=getattr(self, 'fused_ray_batch', None))
-        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], data['radii'], z_vals=data.get('z_vals'), depth=True)
+        return r.render(data['rays_o'], data['rays_d'], data['viewdirs'], data['radii'], z_vals=data.get('z_vals'), depth=True, normals=self.render_normals)
 
     def val_step(self, data, optimizer=None, **kwargs):
         """mipnerf.py:76-98: without use_multiscale NerfNetwork.val_step. With it, one pixel-shaped view through evaluate_once: phase 'test' returns
         rgb [H,W,3], gt_img, disp [H,W,1] and idx; validation returns rgbs, gt_imgs and disps as one-element lists. Device tensors throughout."""
         if not self.use_multiscale:
             return super().val_step(data, optimizer, **kwargs)
-        rgb, image, disp, idx = self.evaluate_once(data, **kwargs)
+        rgb, image, disp, idx, *normal = self.evaluate_once(data, **kwargs)
         if self.phase == 'test':
-            return {'rgb': rgb, 'gt_img': image, 'disp': disp, 'idx': idx}
-        return {'rgbs': [rgb], 'gt_imgs': [image], 'disps': [disp]}
+            return dict({'rgb': rgb, 'gt_img': image, 'disp': disp, 'idx': idx}, **({'normal': normal[0]} if normal else {}))
+        return dict({'rgbs': [rgb], 'gt_imgs': [image], 'disps': [disp]}, **({'normals': normal} if normal else {}))
 
     def evaluate_once(self, data, **kwargs):
         """mipnerf.py:100-117: data holds one view's per-pixel rays [1,H,W,...] (rays_o, rays_d, viewdirs, radii, z_vals, ..., image) and idx; every
-        tensor is flattened to [H*W, -1] float32 rows and rendered by batchify_forward(is_test=True) -> (rgb [H,W,3], image [H,W,C], disp [H,W,1], idx)"""
+        tensor is flattened to [H*W, -1] float32 rows and rendered by batchify_forward(is_test=True) -> (rgb [H,W,3], image [H,W,C], disp [H,W,1], idx),
+        and with `render_normals` a fifth element, the normal map [H,W,3]"""
         self._mark_dirty()
         H, W = data['image'].shape[1:3]
         idx = data['idx']
@@ -325,7 +342,8 @@ class MipNerfNetwork(NerfNetwork):
         with torch.no_grad():
             ret = self.batchify_forward(rays, is_test=True)
         rgb = ret['rgb'].reshape((H, W, -1))
-        return rgb, rays['image'].reshape((H, W, -1)).to(rgb.device), ret['disp'].reshape((H, W, -1)), idx
+        out = (rgb, rays['image'].reshape((H, W, -1)).to(rgb.device), ret['disp'].reshape((H, W, -1)), idx)
+        return out + ((ret['normal'].reshape((H, W, 3)),) if 'normal' in ret else ())
 
     def forward(self, data, is_test):
         randomized = not is_test
