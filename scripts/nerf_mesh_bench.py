@@ -44,7 +44,8 @@ def timed(fn, reps):
 
 def nerf_meshes():
     """[(name, network, threshold)] of the plain mode"""
-    from test_gpu_nerf_mesh import NERF_MLP, _octahedron_network
+    from cases import NERF_MLP
+    from test_gpu_nerf_mesh import _octahedron_network
     from xrnerf_b200.registry.networks import NerfNetwork
     octahedron = _octahedron_network()
     default = NerfNetwork(dict(N_importance=0, chunk=1024, bs_data='rays_o', is_perturb=False), mlp=NERF_MLP,
@@ -54,7 +55,8 @@ def nerf_meshes():
 
 def mip_meshes():
     """[(name, network, threshold)] of --mip"""
-    from test_gpu_mip_mesh import MIP_MLP, RGB_PADDING, _sine_network
+    from cases import MIP_MLP
+    from test_gpu_mip_mesh import RGB_PADDING, _sine_network
     from xrnerf_b200.registry.networks import MipNerfNetwork
     default = MipNerfNetwork(dict(phase='test', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800,
                                   bs_data='rays_o'),
@@ -71,6 +73,8 @@ def main():
     assert torch.cuda.is_available(), 'needs a GPU'
     import test_gpu_mip_mesh as tm
     import test_gpu_nerf_mesh as tn
+    from cases import MIP_MLP, NERF_MLP
+    from restate64 import lattice_points, mip_bands
     from xrnerf_b200 import registry as R
     from xrnerf_b200.mesh import footprint_sigma
     mip = args.mip
@@ -78,19 +82,19 @@ def main():
     fp = dict(footprint='cell') if mip else {}
     out = {'card_before': card()}
     torch.manual_seed(0)
-    mlp = R.build_mlp(tm.MIP_MLP if mip else tn.NERF_MLP).cuda()
+    mlp = R.build_mlp(MIP_MLP if mip else NERF_MLP).cuda()
     with torch.no_grad():
         for n in (256, 512):
             shape = (n, n, n)
             sigma = footprint_sigma('cell', shape, box)
-            pts = tn._lattice_points(shape, box)
+            pts = lattice_points(shape, box)
             dirs = torch.nn.functional.normalize(torch.randn_like(pts), dim=-1)
             t_lat = timed(lambda: mlp.density_lattice(shape, box, **fp), args.reps)
             infer = (lambda p, d: tm._infer(mlp, p, d, sigma)) if mip else (lambda p, d: tn._infer(mlp, p, d))
             ch = 1 << 21
             t_cmp = timed(lambda: [infer(pts[i:i + ch], dirs[i:i + ch]) for i in range(0, pts.shape[0], ch)], args.reps)
             npt = n ** 3
-            r = dict(sigma=sigma, live_bands=int((tm._bands(sigma) > 0).sum())) if mip else {}
+            r = dict(sigma=sigma, live_bands=int((mip_bands(sigma) > 0).sum())) if mip else {}
             r.update({'density_lattice_ms': t_lat, 'encoder_plus_mlp_ms' if mip else 'posenc_plus_mlp_ms': t_cmp,
                       'lattice_tflops': 2 * MAC_DENSITY[mip] * npt / t_lat * 1e-9, 'comparison_tflops': 2 * MAC_FULL[mip] * npt / t_cmp * 1e-9})
             out[f'lattice_{n}'] = r

@@ -4,11 +4,13 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
 import test_gpu_nerf_train as T
+from cases import NERF_MLP
+from restate64 import emulated_fp16_forward
 from xrnerf_b200 import registry as R
 
 for n in [int(a) for a in sys.argv[1:]] or [128, 129, 256, 300, 384]:
     torch.manual_seed(n)
-    mlp = R.build_mlp(dict(T.NERF)).cuda()
+    mlp = R.build_mlp(dict(NERF_MLP)).cuda()
     x = torch.rand((n, 90), device='cuda') * 2 - 1
     g = torch.randn((n, 4), device='cuda') * 1e-3
     if os.environ.get('ONLY_RGB'):
@@ -16,7 +18,7 @@ for n in [int(a) for a in sys.argv[1:]] or [128, 129, 256, 300, 384]:
     if os.environ.get('ONLY_ALPHA'):
         g[:, :3] = 0
     mlp.fused_train = False
-    ref = T._grads(mlp, T._emulated_fp16_forward(mlp, x), g)
+    ref = T._grads(mlp, emulated_fp16_forward(mlp, x), g)
     mlp.fused_train = True
     ours = T._grads(mlp, mlp.batchify_run_mlp(x), g)
     out = []

@@ -6,14 +6,10 @@ import os
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
 G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'nerf_golden_r2.npz'))
-
-
-def dev(a, dt=None):
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return (t if dt is None else t.to(dt)).cuda()
 
 
 def test_ngp_ray_source_matches_reference_table_batching_and_bg():

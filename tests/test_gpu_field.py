@@ -4,12 +4,9 @@ table entries), MLP outputs 2e-3 abs / 1e-2 rel (fp16 activations; accumulation 
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 @pytest.fixture(scope='module')

@@ -32,46 +32,24 @@ gives each entry's contribution mass M. Every entry of the table, density and co
   * E = |dZ|^T e_x: the kernel's activations may differ from ours by e_x where the fp16 rounding of an activation is ambiguous.
 Nothing in tau, D or the floor is fitted to a run.
 """
-import ctypes as C
 import time
 
 import numpy as np
 import pytest
 import torch
+from cases import dev, load_ngp_weights
+from restate64 import GAMMA_TC, U16, Grid, f16, hashgrid_enc16, ngp_mats, ulp16
 
 pytestmark = pytest.mark.gpu
 
-U16 = 2.0 ** -11            # fp16 unit roundoff
 SCALE = 4096.0              # staging scale of dZ / dY in both backward kernels
 FLOOR = 2.0 ** -26          # (2^-25 / SCALE) / U16: the subnormal half-step at the staging scale, as a floor on the staged magnitude
 REJECT_CEILING = 2.0 / 3.0  # a batch with more rejected samples than this does not test enough
-GAMMA_TC = 2.0 ** -22       # per-term accumulation bound of a K-term dot product on the tensor cores (gamma = K GAMMA_TC)
-GAMMA_FMA = 2.0 ** -24 * (1 + 2.0 ** -16)   # ... as a chain of K fp32 fma (the CUDA-core kernels): K u / (1 - K u), K <= 64
-P1, P2 = 2654435761, 805459861
+GAMMA_FMA = 2.0 ** -24 * (1 + 2.0 ** -16)   # per-term accumulation bound of a K-term dot product as a chain of K fp32 fma (the CUDA-core kernels): K u / (1 - K u), K <= 64
 REPORT = []
 
 
-def _f16(a):
-    return np.asarray(a, np.float64).astype(np.float16).astype(np.float64)
-
-
-def _ulp16(v):
-    """fp16 spacing at |v| (the subnormal step 2^-24 below 2^-14)"""
-    _, e = np.frexp(np.maximum(np.abs(v), 2.0 ** -14))
-    return np.ldexp(1.0, e - 11)
-
-
-def _mats(params, n_hidden):
-    w = _f16(params)
-    out, o = [], 0
-    for (r, c) in [(64, 32)] + [(64, 64)] * (n_hidden - 1) + [(16, 64)]:
-        out.append(w[o:o + r * c].reshape(r, c))
-        o += r * c
-    assert o == w.size
-    return out
-
-
-def _layer(W, x, ex, relu, gamma_unit, rnd=_f16):
+def _layer(W, x, ex, relu, gamma_unit, rnd=f16):
     aW = np.abs(W)
     z = x @ W.T
     b = ex @ aW.T + W.shape[1] * gamma_unit * ((np.abs(x) + ex) @ aW.T)
@@ -86,7 +64,7 @@ def _layer(W, x, ex, relu, gamma_unit, rnd=_f16):
 class Forward:
     """float64 forward of the field with per-unit bounds: layer inputs (value, bound) and masks of both nets, raw64 and its bound, stable rows"""
 
-    def __init__(self, dm, cm, enc, sh, gamma_unit=GAMMA_TC, rnd=_f16):
+    def __init__(self, dm, cm, enc, sh, gamma_unit=GAMMA_TC, rnd=f16):
         n = enc.shape[0]
         self.flip = np.zeros(n, bool)
         self.g = gamma_unit
@@ -113,7 +91,7 @@ class Forward:
         """|raw_kernel - raw64| <= b + ulp16(|raw64| + b) on every row (the interval bound holds across a ReLU kink, so rows with an unstable
         decision are checked too, only more loosely); returns the largest err / bound"""
         r, b = self.raw[:, cols], self.braw[:, cols]
-        bound = b + _ulp16(np.abs(r) + b)
+        bound = b + ulp16(np.abs(r) + b)
         err = np.abs(np.asarray(raw, np.float64).reshape(r.shape) - r)
         assert np.isfinite(raw).all()
         ratio = float((err / bound).max()) if err.size else 0.0
@@ -151,47 +129,6 @@ def field_chain(F, dm, cm, draw, rows, absolute):
     return dd, dc, genc, ed, ec
 
 
-class Grid:
-    """tcnn's multiresolution grid (layout from the library), restated in numpy: per level the 8 corner entries and trilinear weights"""
-
-    def __init__(self, cfg):
-        from xrnerf_b200 import _C
-        off = (C.c_uint32 * 17)(); sc = (C.c_float * 16)(); res = (C.c_uint32 * 16)()
-        _C.check(_C.lib.xrb_tcnn_hashgrid_layout(cfg, off, sc, res))
-        self.off = np.array(list(off), np.int64); self.sc = np.array(list(sc), np.float32); self.res = np.array(list(res), np.int64)
-        self.hashed = self.res ** 3 > np.diff(self.off)
-        self.n_entries = int(self.off[-1])
-
-    def corners(self, pts, l):
-        """(entry index [n,8] into the whole table, weight [n,8] float64, ix [n]) of level l. q = fp32 fma(scale, p, 0.5): the float64 product is
-        exact and the sum is exact for every input not below ~2^-29, so rounding it once to fp32 gives the fma's bits."""
-        q = (np.float64(self.sc[l]) * pts.astype(np.float64) + 0.5).astype(np.float32).astype(np.float64)
-        i = np.floor(q); f = q - i; i = i.astype(np.int64)
-        hs, r = int(self.off[l + 1] - self.off[l]), int(self.res[l])
-        idx = np.empty((pts.shape[0], 8), np.int64); w = np.empty((pts.shape[0], 8))
-        for c in range(8):
-            cx, cy, cz = i[:, 0] + (c & 1), i[:, 1] + ((c >> 1) & 1), i[:, 2] + ((c >> 2) & 1)
-            if self.hashed[l]:
-                h = (cx ^ ((cy * P1) & 0xffffffff) ^ ((cz * P2) & 0xffffffff)) % hs
-            else:
-                h = (cx + cy * r + cz * r * r) % hs
-            idx[:, c] = self.off[l] + h
-            w[:, c] = (f[:, 0] if c & 1 else 1 - f[:, 0]) * (f[:, 1] if c & 2 else 1 - f[:, 1]) * (f[:, 2] if c & 4 else 1 - f[:, 2])
-        return idx, w, i[:, 0]
-
-    def scatter(self, pts, genc, rows):
-        """(table gradient of dL/denc [n,32], contribution count per scalar); only `rows` contribute"""
-        acc = np.zeros(2 * self.n_entries); cnt = np.zeros(2 * self.n_entries)
-        p, g = pts[rows], genc[rows]
-        for l in range(16):
-            idx, w, _ = self.corners(p, l)
-            for f in range(2):
-                k = (2 * idx + f).ravel()
-                acc += np.bincount(k, (w * g[:, 2 * l + f:2 * l + f + 1]).ravel(), minlength=acc.size)
-                cnt += np.bincount(k, minlength=acc.size)
-        return acc, cnt
-
-
 def within(name, got, ref, M, E, tau, depth, pre=None):
     """the per-entry assertion; returns (passes, largest err / bound, worst index)"""
     got = np.asarray(got, np.float64)
@@ -224,11 +161,7 @@ def field(dh, ch, npk):
     from xrnerf_b200.ngp import NgpField
     if (dh, ch) not in _FIELDS:
         _FIELDS.clear()
-        table, dens, color = _weights(dh, ch)
-        f = NgpField(density_hidden=dh, color_hidden=ch, n_packed_levels=npk).cuda()
-        with torch.no_grad():
-            f.hash_params.copy_(torch.from_numpy(table)); f.density_params.copy_(torch.from_numpy(dens)); f.color_params.copy_(torch.from_numpy(color))
-        _FIELDS[(dh, ch)] = f
+        _FIELDS[(dh, ch)] = load_ngp_weights(NgpField(density_hidden=dh, color_hidden=ch, n_packed_levels=npk).cuda(), _weights(dh, ch))
     f = _FIELDS[(dh, ch)]
     f.set_packed_levels(npk)
     f.refresh()
@@ -247,19 +180,14 @@ def _report():
     _CASES.clear()
 
 
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def kernel_inputs(f, pts_d, dirs_d):
     """the bits the field kernels feed their networks: fp16 encodings (xrb_tcnn_hashgrid_forward on the field's table) and fp16 SH"""
     from xrnerf_b200 import _C
     n = pts_d.shape[0]
-    enc = torch.empty((n, 32), dtype=torch.float16, device='cuda'); sh = torch.empty((n, 16), dtype=torch.float16, device='cuda')
-    (pp, ps), (dp, ds) = _C.rows(pts_d), _C.rows(dirs_d)
-    _C.check(_C.lib.xrb_tcnn_hashgrid_forward(f.cfg, f.tab, pp, ps, n, _C.ptr(enc), _C.stream()))
+    sh = torch.empty((n, 16), dtype=torch.float16, device='cuda')
+    dp, ds = _C.rows(dirs_d)
     _C.check(_C.lib.xrb_tcnn_sh4_forward(dp, ds, n, _C.ptr(sh), _C.stream()))
-    return enc.cpu().numpy().astype(np.float64), sh.cpu().numpy().astype(np.float64)
+    return hashgrid_enc16(f, pts_d), sh.cpu().numpy().astype(np.float64)
 
 
 def random_batch(n, seed):
@@ -273,10 +201,10 @@ def random_batch(n, seed):
 def contention_batch(grid, n=5000, seed=5):
     """n samples strictly inside ONE finest-level cell: every sample's atomics hit the same 8 entries per level"""
     rng = np.random.default_rng(seed)
-    sc = np.float64(grid.sc[15])
+    sc = np.float64(grid.scale[15])
     cell = np.array([1000, 1377, 642])
     pts = ((cell - 0.5 + rng.uniform(0.05, 0.95, (n, 3))) / sc).astype(np.float32)
-    assert len(np.unique(grid.corners(pts, 15)[0][:, 0])) == 1
+    assert len(np.unique(grid.corners(15, pts)[0][:, 0])) == 1
     dirs = rng.random((n, 3)).astype(np.float32)
     draw = (rng.normal(0, 1, (n, 4)) * 1e-3).astype(np.float32)
     return pts, dirs, draw
@@ -289,7 +217,7 @@ def boundary_batch(grid, seed=6):
     rows = [[a, b, c] for a in (0.0, 1.0) for b in (0.0, 1.0) for c in (0.0, 1.0)]
     parity = set()
     for l in range(16):
-        sc = np.float64(grid.sc[l])
+        sc = np.float64(grid.scale[l])
         for k in rng.choice(np.arange(1, int(grid.res[l]) - 1), min(24, int(grid.res[l]) - 2), replace=False):
             # the fp32 value nearest (k - 0.5) / scale, or one of its neighbours, for which fma(scale, p, 0.5) is exactly k
             up = dn = np.float32((k - 0.5) / sc)
@@ -323,7 +251,7 @@ class Case:
         pts_d = dev(pts) if pts_d is None else pts_d[:n_eff]
         dirs_d = dev(dirs) if dirs_d is None else dirs_d[:n_eff]
         self.grid = Grid(f.cfg)
-        self.dm, self.cm = _mats(dens, dh), _mats(color, ch)
+        self.dm, self.cm = ngp_mats(dens, dh), ngp_mats(color, ch)
         enc, sh = kernel_inputs(f, pts_d, dirs_d) if n_eff else (np.zeros((0, 32)), np.zeros((0, 16)))
         self.F = F = Forward(self.dm, self.cm, enc, sh, GAMMA_TC if impl == 1 else GAMMA_FMA)
         self.n = n_eff
@@ -404,7 +332,7 @@ def test_forward_within_derived_bound(dh, ch):
         enc, sh = kernel_inputs(f, pts_d, dirs_d)
         if F is None:
             enc0 = enc
-            F = Forward(_mats(dens, dh), _mats(color, ch), enc, sh)
+            F = Forward(ngp_mats(dens, dh), ngp_mats(color, ch), enc, sh)
         assert np.array_equal(enc, enc0), npk
         for impl in (0, 1):
             worst = max(worst, F.check_raw(f.run_mlp(pts_d, dirs_d, impl=impl).cpu().numpy()))
@@ -473,7 +401,7 @@ def _altered_references_are_rejected(case, got, tau):
     s = int(np.argmax(np.abs(case.genc[:, 30:32]).sum(1) * case.rows))
     assert case.rows[s]
     p = case.pts[s:s + 1]
-    idx, w, _ = grid.corners(p, 15)
+    idx, w = grid.corners(15, p)
     ref, M = case.dt.copy(), case.Mt.copy()
     for c in range(8):
         for ft in range(2):
@@ -483,7 +411,7 @@ def _altered_references_are_rejected(case, got, tau):
     # (b): the hashed level and sample with the largest |w1 - w0| |g|
     best = None
     for l in np.nonzero(grid.hashed)[0]:
-        idx, w, _ = grid.corners(case.pts, l)
+        idx, w = grid.corners(l, case.pts)
         gl = np.abs(case.genc[:, 2 * l]) * case.rows
         score = (np.abs(w[:, 1] - w[:, 0]) * gl)
         k = int(np.argmax(score))
@@ -592,7 +520,7 @@ def test_tcnn_mlp_backward_entrywise(n_hidden):
     from xrnerf_b200 import _C, synth
     n = 20001
     _, dens, _ = synth.ngp_weights(seed=50 + n_hidden, n_hash_params=8, dens_hidden=n_hidden)
-    mats = _mats(dens, n_hidden)
+    mats = ngp_mats(dens, n_hidden)
     rng = np.random.default_rng(51)
     x16 = rng.uniform(-1, 1, (n, 32)).astype(np.float16)
     x16[:, 31] = 1
@@ -613,7 +541,7 @@ def test_tcnn_mlp_backward_entrywise(n_hidden):
     dw, _, dx = _back(mats, xs, masks, dy16.astype(np.float64), live, False)
     Mw, Ew, Mx = _back(mats, xs, masks, dy16.astype(np.float64), live, True)
     pre = (rng.normal(0, 1, dw.size) * np.abs(dw).max()).astype(np.float32)
-    p16, x_d, dy_d, d = dev(_f16(dens).astype(np.float16)), dev(x16), dev(dy16), dev(pre)
+    p16, x_d, dy_d, d = dev(f16(dens).astype(np.float16)), dev(x16), dev(dy16), dev(pre)
     dx_k = torch.empty((n, 32), dtype=torch.float16, device='cuda')
     _C.check(_C.lib.xrb_tcnn_mlp_backward(_C.ptr(p16), _C.ptr(x_d), _C.ptr(dy_d), n, 32, 64, n_hidden, _C.ptr(dx_k), _C.f32(d), _C.stream()))
     tau = 2 * U16

@@ -5,114 +5,15 @@ The marching-cubes kernels are compared bit for bit, in order, with `mc_oracle`,
 over the triangulation table that scripts/gen_mc_table.py generates. That the table is right is not taken from the table itself: the oracle's
 meshes (CPU tests) and the kernels' meshes (GPU tests) must be closed and consistently oriented, with outward normals, the right Euler
 characteristic and, at 128^3, the analytic enclosed volume and area."""
-import ctypes as C
-import importlib.util
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
+from cases import NGP_MODEL, cpu_args, dev
+from restate64 import GEN, area, check_closed_oriented, euler, lattice_coords, mc_oracle
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
-
-
-def _gen():
-    spec = importlib.util.spec_from_file_location('gen_mc_table', os.path.join(ROOT, 'scripts', 'gen_mc_table.py'))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
-
-
-GEN = _gen()
-COUNTS, TRIS = GEN.build_table()
-
-
-# ---------------------------------------------------------------------------------------------------------------- numpy restatement
-def lattice_coords(lo, hi, n):
-    """float32 coordinates of lattice indices 0..n-1 on one axis: min(lo + i * ((hi - lo) / (n - 1)), hi), each operation rounded once"""
-    lo, hi = f32(lo), f32(hi)
-    step = f32(hi - lo) / f32(n - 1)
-    return np.minimum(lo + np.arange(n, dtype=f32) * f32(step), hi).astype(f32)
-
-
-def mc_oracle(vol, threshold, box=((0, 0, 0), (1, 1, 1))):
-    """(verts f32[V,3], faces i32[F,3]) of vol f32[nz,ny,nx] (x fastest), by the contract of xrb_mc_emit"""
-    vol = np.ascontiguousarray(vol, f32)
-    thr = f32(threshold)
-    nz, ny, nx = vol.shape
-    cx, cy, cz = (lattice_coords(box[0][a], box[1][a], n) for a, n in enumerate((nx, ny, nz)))
-    inside = vol > thr
-    cross = np.zeros((nz, ny, nx, 3), bool)                   # the edge from each point in +x, +y, +z crosses
-    cross[:, :, :-1, 0] = inside[:, :, :-1] != inside[:, :, 1:]
-    cross[:, :-1, :, 1] = inside[:, :-1, :] != inside[:, 1:, :]
-    cross[:-1, :, :, 2] = inside[:-1, :, :] != inside[1:, :, :]
-    vid = np.cumsum(cross.reshape(-1)).reshape(cross.shape).astype(np.int64) - 1
-    pz, py, px, ax = np.nonzero(cross)                         # lattice-point order, then axis: the vertex order
-    step = np.stack([ax == 0, ax == 1, ax == 2], 1).astype(np.int64)
-    qx, qy, qz = px + step[:, 0], py + step[:, 1], pz + step[:, 2]
-    vp, vq = vol[pz, py, px], vol[qz, qy, qx]
-    p_in = vp > thr
-    v_in, v_out = np.where(p_in, vp, vq), np.where(p_in, vq, vp)
-    t = (f32(thr) - v_out).astype(f32) / (v_in - v_out).astype(f32)
-    verts = np.stack([cx[px], cy[py], cz[pz]], 1).astype(f32)
-    for a, (c, ip, iq) in enumerate(((cx, px, qx), (cy, py, qy), (cz, pz, qz))):
-        sel = ax == a
-        P, Q = c[ip[sel]], c[iq[sel]]
-        pin = p_in[sel]
-        Pin, Pout = np.where(pin, P, Q), np.where(pin, Q, P)
-        verts[sel, a] = Pout + (t[sel] * (Pin - Pout).astype(f32)).astype(f32)
-    # cells
-    case = np.zeros((nz - 1, ny - 1, nx - 1), np.int64)
-    for c in range(8):
-        ox, oy, oz = c & 1, (c >> 1) & 1, (c >> 2) & 1
-        case |= inside[oz:nz - 1 + oz, oy:ny - 1 + oy, ox:nx - 1 + ox].astype(np.int64) << c
-    case = case.reshape(-1)
-    n_t = COUNTS[case].astype(np.int64)
-    cell = np.repeat(np.arange(case.size), n_t)
-    slot = np.arange(cell.size) - np.repeat(np.cumsum(n_t) - n_t, n_t)
-    edges = TRIS[case[cell], slot].astype(np.int64)                         # [F,3]
-    gz, gy, gx = np.unravel_index(cell, (nz - 1, ny - 1, nx - 1))
-    start = np.array([GEN.edge_corners(e)[0] for e in range(12)])
-    eo = np.stack([start & 1, (start >> 1) & 1, (start >> 2) & 1], 1)    # owner offset of each edge
-    ea = np.arange(12) // 4
-    faces = vid[gz[:, None] + eo[edges, 2], gy[:, None] + eo[edges, 1], gx[:, None] + eo[edges, 0], ea[edges]]
-    return verts, faces.astype(np.int32).reshape(-1, 3)
-
-
-# ---------------------------------------------------------------------------------------------------------------- geometric checks
-def check_closed_oriented(verts, faces):
-    """every undirected edge in exactly two triangles, every directed edge once, every vertex used, signed volume > 0; returns the volume"""
-    faces = np.asarray(faces, np.int64)
-    assert faces.shape[0] > 0
-    d = np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-    key = d[:, 0] * (1 << 32) + d[:, 1]
-    assert np.unique(key).size == key.size, 'a directed edge appears twice'
-    und = np.minimum(d[:, 0], d[:, 1]) * (1 << 32) + np.maximum(d[:, 0], d[:, 1])
-    _, cnt = np.unique(und, return_counts=True)
-    assert (cnt == 2).all(), 'an edge does not lie in exactly two triangles'
-    assert np.unique(faces).size == len(verts), 'an unused vertex'
-    vol = signed_volume(verts, faces)
-    assert vol > 0
-    return vol
-
-
-def signed_volume(verts, faces):
-    v = np.asarray(verts, np.float64)[np.asarray(faces, np.int64)]
-    return float(np.einsum('ij,ij->i', v[:, 0], np.cross(v[:, 1], v[:, 2])).sum() / 6)
-
-
-def area(verts, faces):
-    v = np.asarray(verts, np.float64)[np.asarray(faces, np.int64)]
-    return float(np.linalg.norm(np.cross(v[:, 1] - v[:, 0], v[:, 2] - v[:, 0]), axis=1).sum() / 2)
-
-
-def euler(verts, faces):
-    faces = np.asarray(faces, np.int64)
-    d = np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]])
-    n_edges = np.unique(np.minimum(d[:, 0], d[:, 1]) * (1 << 32) + np.maximum(d[:, 0], d[:, 1])).size
-    return len(verts) - n_edges + len(faces)
 
 
 # ---------------------------------------------------------------------------------------------------------------- volumes
@@ -202,17 +103,8 @@ def test_oracle_topology_and_geometry():
     check_closed_oriented(*mc_oracle(smooth_noise((40, 33, 47)), 0.0))
 
 
-def _cpu_args():
-    from xrnerf_b200 import _C
-    buf = (C.c_char * 4096)()
-    p = C.c_void_p((C.addressof(buf) + 255) & ~255)                     # 256-byte aligned host memory: never dereferenced by a rejected call
-    cfg = _C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 1, 2)
-    tab = _C.NgpTable(p.value, None, 0)
-    return _C, buf, p, cfg, tab
-
-
 def test_mesh_entry_points_validate_arguments_without_gpu():
-    _C, _buf, p, cfg, tab = _cpu_args()
+    _C, _buf, p, cfg, tab = cpu_args()
     lib = _C.lib
     unit = (_C.float3((0, 0, 0)), _C.float3((1, 1, 1)))
     lattice = lambda n, box=unit, out=p: lib.xrb_ngp_density_lattice(cfg, tab, p, p, n[0], n[1], n[2], box[0], box[1], out, 1, p, None)
@@ -285,10 +177,6 @@ def test_density_threshold_mapping():
 
 
 # ================================================================================================================ GPU tests
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def gpu_mc(vol, thr, box=((0, 0, 0), (1, 1, 1))):
     from xrnerf_b200.mesh import marching_cubes
     v, f = marching_cubes(dev(vol), thr, box)
@@ -398,18 +286,6 @@ def test_density_lattice_matches_run_density(field, impl):
     big = (130, 100, 90)                                                 # more points than one staging chunk (2^20)
     got = field.density_lattice(big, impl=impl)
     assert torch.equal(got.view(torch.int32), field.run_density(dev(lattice_positions(big, ((0, 0, 0), (1, 1, 1)))), impl=impl).reshape(big).view(torch.int32))
-
-
-NGP_MODEL = dict(   # configs/instant_ngp/nerf_blender_local01.py's model
-    type='HashNerfNetwork', cfg=dict(phase='train', chunk=4096, bs_data='rays_o'),
-    mlp=dict(type='HashNerfMLP', bound=1,
-             embedder_pos=dict(n_input_dims=3, encoding_config=dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=16, interpolation='Linear')),
-             embedder_dir=dict(n_input_dims=3, encoding_config=dict(otype='SphericalHarmonics', degree=4)),
-             density_net=dict(n_input_dims=32, n_output_dims=16, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=1)),
-             color_net=dict(n_output_dims=3, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=2))),
-    sampler=dict(type='NGPGridSampler', update_grid_freq=16, update_block_size=5000000, n_rays_per_batch=4096, cone_angle_constant=0.00390625, near_distance=0.2,
-                 target_batch_size=1 << 18, rgb_activation=2, density_activation=3),
-    render=dict(type='HashNerfRender', bg_color=[0, 0, 0]))
 
 
 def _network():

@@ -4,8 +4,9 @@ and the PLY attributes (xrnerf_b200.mesh.write_ply, ngp_to_nerf_normals).
 Restatement (numpy; include/xrnerf_b200.h states the contract). The kernel's encodings come from xrb_tcnn_hashgrid_forward (the same hash_level and fp16
 rounding as the density kernels); the density net then runs as the CUDA-core kernel does it, one sequential fp32 fma chain per unit, restated exactly
 (each fp16 x fp16 product is exact, and the sum is formed in extended precision and rounded once to fp32). That gives the forward activations and masks;
-the density it produces must equal the kernel's bit for bit, which is what shows the masks are the kernel's. The grid cell is restated with the same
-fp32 arithmetic (px = fp32(scale * x + 0.5), exact in extended precision before the one rounding), so the in-cell positions are the kernel's too.
+the density it produces must equal the kernel's bit for bit, which is what shows the masks are the kernel's. The grid cell is restated exactly
+(restate64.Grid: px = fp32(fma(scale, x, 0.5)) for every fp32 x), so the in-cell positions are the kernel's too. The restatement is
+restate64.cuda_core_density_grad.
 
 Gradient bound. With those masks and in-cell positions, the kernel's gradient is a sum of products, each of the form
     scale_l * (+-w_y w_z) * v_c * (a path of weights through the net),
@@ -13,35 +14,21 @@ computed in fp32 with at most n roundings along any product: 64 per W^T step of 
 product, 8 for the sum over corners and 16 for the sum over levels. So |kernel - exact| <= gamma_n * M, gamma_n = n u / (1 - n u), u = 2^-24, where M is
 the same sum on absolute values; the float64 restatement adds its own gamma_n with u = 2^-53. Nothing in the bound is fitted to a run.
 """
-import ctypes as C
 import math
 
 import numpy as np
 import pytest
 import torch
+from cases import SPHERE_C, SPHERE_THR, cpu_args, face_points, ngp_density_grad, ngp_field, ngp_network, random_points, sphere_network
+from restate64 import U32, U64, Grid, cuda_core_density, cuda_core_density_grad, enc_grad, field_mats, gamma, hashgrid_enc16
 
 f32 = np.float32
-U32, U64 = 2.0 ** -24, 2.0 ** -53
-P1, P2 = 2654435761, 805459861
 REPORT = []
 
 
-def gamma(n, u):
-    return n * u / (1 - n * u)
-
-
 # ================================================================================================================ CPU-only tests
-def _cpu_args():
-    from xrnerf_b200 import _C
-    buf = (C.c_char * 4096)()
-    p = C.c_void_p((C.addressof(buf) + 255) & ~255)                     # 256-byte aligned host memory: never dereferenced by a rejected call
-    cfg = _C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 1, 2)
-    tab = _C.NgpTable(p.value, None, 0)
-    return _C, buf, p, cfg, tab
-
-
 def test_density_grad_validates_arguments_without_gpu():
-    _C, _buf, p, cfg, tab = _cpu_args()
+    _C, _buf, p, cfg, tab = cpu_args()
     lib = _C.lib
     call = lambda cfg=cfg, tab=tab, w=p, pts=p, stride=3, n=4, dens=p, grad=p: lib.xrb_ngp_density_grad(cfg, tab, w, pts, stride, n, dens, grad, None)
     assert call(cfg=None) == -1 and b'null' in lib.xrb_last_error()
@@ -135,171 +122,6 @@ def test_ngp_to_nerf_normals_matches_the_position_map():
     assert torch.equal(ngp_to_nerf_normals(torch.zeros((2, 3))), torch.zeros((2, 3))) and ngp_to_nerf_normals(torch.zeros((0, 3))).shape == (0, 3)
 
 
-# ================================================================================================================ restatement
-class Grid:
-    """the field's grid (xrb_tcnn_hashgrid_layout) and fp16 table, with grid_cell / grid_index restated"""
-
-    def __init__(self, field):
-        from xrnerf_b200 import _C
-        off = (C.c_uint32 * 17)(); sc = (C.c_float * 16)(); res = (C.c_uint32 * 16)()
-        _C.check(_C.lib.xrb_tcnn_hashgrid_layout(field.cfg, off, sc, res))
-        self.off = np.array(off[:], np.int64)
-        self.scale = np.array(sc[:], f32)
-        self.res = np.array(res[:], np.int64)
-        field.refresh()
-        self.table = field._table16.cpu().numpy().astype(np.float64).reshape(-1, 2)
-
-    def cell(self, l, x):
-        """x f32[n,3] -> (integer cell i64[n,3], in-cell position f32 as float64 [n,3]) exactly as grid_cell computes them"""
-        px = (np.longdouble(self.scale[l]) * x.astype(np.longdouble) + np.longdouble(0.5)).astype(f32)
-        fl = np.floor(px)
-        return fl.astype(np.int64), (px - fl).astype(np.float64)
-
-    def corner_values(self, l, gi):
-        """fp16 feature pairs of the 8 corners [n,8,2] (corner c = bit0 x, bit1 y, bit2 z)"""
-        hs, r = int(self.off[l + 1] - self.off[l]), int(self.res[l])
-        out = []
-        for c in range(8):
-            x, y, z = (gi[:, a] + ((c >> a) & 1) for a in range(3))
-            if r ** 3 > hs:
-                idx = (x ^ ((y * P1) & 0xffffffff) ^ ((z * P2) & 0xffffffff)) & (hs - 1)
-            else:
-                idx = x + y * r + z * r * r
-                idx = np.where(idx >= hs, idx - hs, idx)
-            out.append(self.table[self.off[l] + idx])
-        return np.stack(out, 1)
-
-
-def trilinear_grad_terms(f):
-    """d w_c / d f for the 8 corners: [n,8,3] (float64 of the fp32 in-cell positions) and the weights themselves [n,8]"""
-    u = 1.0 - f
-    dw, w = np.zeros(f.shape[:1] + (8, 3)), np.zeros(f.shape[:1] + (8,))
-    for c in range(8):
-        pick = [f[:, a] if (c >> a) & 1 else u[:, a] for a in range(3)]
-        w[:, c] = pick[0] * pick[1] * pick[2]
-        for a in range(3):
-            o = [pick[b] for b in range(3) if b != a]
-            dw[:, c, a] = (1.0 if (c >> a) & 1 else -1.0) * o[0] * o[1]
-    return dw, w
-
-
-def net_mats(field):
-    field.refresh()
-    w = field._dens16.cpu().numpy().astype(np.float64)
-    dh = field.cfg.density_hidden
-    mats, o = [], 0
-    for (r, c) in [(64, 32)] + [(64, 64)] * (dh - 1) + [(16, 64)]:
-        mats.append(w[o:o + r * c].reshape(r, c))
-        o += r * c
-    return mats
-
-
-def fma_layer(W, x):
-    """the CUDA-core layer's pre-activations: per unit a sequential fp32 fma chain over the inputs, each step rounded once"""
-    s = np.zeros((x.shape[0], W.shape[0]), f32)
-    for k in range(W.shape[1]):
-        s = (np.longdouble(1) * W[:, k][None, :] * x[:, k][:, None] + s.astype(np.longdouble)).astype(f32)
-    return s.astype(np.float64)
-
-
-def kernel_forward(mats, enc16):
-    """density and hidden-layer masks as the CUDA-core density computes them (enc16: the fp16 encodings as float64)"""
-    a, masks = enc16, []
-    for W in mats[:-1]:
-        a = np.maximum(fma_layer(W, a), 0).astype(np.float16).astype(np.float64)
-        masks.append(a > 0)
-    return fma_layer(mats[-1][:1], a)[:, 0].astype(np.float16).astype(np.float64), masks
-
-
-def enc_grad(mats, masks):
-    """d(out 0)/d(encoding) [n,32] in float64 and the same chain on absolute values"""
-    g = masks[-1] * mats[-1][0][None, :]
-    ga = np.abs(g)
-    for k in range(len(mats) - 2, 0, -1):
-        g, ga = masks[k - 1] * (g @ mats[k]), masks[k - 1] * (ga @ np.abs(mats[k]))
-    return g @ mats[0], ga @ np.abs(mats[0])
-
-
-def position_grad(grid, x, ge, gea):
-    """sum over levels of scale_l sum_c dw_c/df (v_c . ge_l) [n,3], and the same sum on absolute values (the mass M of the bound)"""
-    g, m = np.zeros((x.shape[0], 3)), np.zeros((x.shape[0], 3))
-    for l in range(16):
-        gi, f = grid.cell(l, x)
-        v = grid.corner_values(l, gi)
-        dw, _ = trilinear_grad_terms(f)
-        s = v[:, :, 0] * ge[:, None, 2 * l] + v[:, :, 1] * ge[:, None, 2 * l + 1]
-        sa = np.abs(v[:, :, 0]) * gea[:, None, 2 * l] + np.abs(v[:, :, 1]) * gea[:, None, 2 * l + 1]
-        g += float(grid.scale[l]) * (dw * s[:, :, None]).sum(1)
-        m += float(grid.scale[l]) * (np.abs(dw) * sa[:, :, None]).sum(1)
-    return g, m
-
-
-def restated(field, grid, x):
-    """(density as the kernel computes it, float64 gradient, its bound) at x f32[n,3]"""
-    from xrnerf_b200 import _C
-    xt = torch.from_numpy(x).cuda()
-    enc = torch.empty((len(x), 32), dtype=torch.float16, device='cuda')
-    _C.check(_C.lib.xrb_tcnn_hashgrid_forward(field.cfg, field.tab, _C.ptr(xt), 3, len(x), _C.ptr(enc), _C.stream()), 'hashgrid_forward')
-    mats = net_mats(field)
-    dens, masks = kernel_forward(mats, enc.cpu().numpy().astype(np.float64))
-    ge, gea = enc_grad(mats, masks)
-    g, m = position_grad(grid, x, ge, gea)
-    n = 64 * field.cfg.density_hidden + 2 + 1 + 8 + 16
-    return dens, g, (gamma(n, U32) + gamma(n, U64)) * m
-
-
-def make_field(dh, n_packed, seed=3):
-    from xrnerf_b200 import synth
-    from xrnerf_b200.ngp import NgpField
-    f = NgpField(density_hidden=dh, color_hidden=2, n_packed_levels=n_packed).cuda()
-    table, dens, color = synth.ngp_weights(seed=seed, dens_hidden=dh, hash_range=0.5, mlp_gain=2.0)
-    with torch.no_grad():
-        f.hash_params.copy_(torch.from_numpy(table)); f.density_params.copy_(torch.from_numpy(dens)); f.color_params.copy_(torch.from_numpy(color))
-    return f
-
-
-def random_points(n, seed):
-    return np.random.default_rng(seed).uniform(1 / 64, 1 - 1 / 64, (n, 3)).astype(f32)
-
-
-def face_points(grid, n_per, seed):
-    """points with one coordinate exactly on a cell face of some level: fp32(scale_l * x + 0.5) is an integer"""
-    rng = np.random.default_rng(seed)
-    pts = []
-    for l in (0, 2, 4, 5, 7, 9, 12, 15):
-        sc = np.longdouble(grid.scale[l])
-        for _ in range(n_per):
-            k = int(rng.integers(2, int(grid.res[l]) - 1))
-            x = f32((k - 0.5) / float(sc))
-            for _ in range(64):
-                px = f32(sc * np.longdouble(x) + np.longdouble(0.5))
-                if px == k:
-                    break
-                x = np.nextafter(x, f32(np.inf) if px < k else f32(-np.inf))
-            if px != k:
-                continue
-            p = rng.uniform(1 / 64, 1 - 1 / 64, 3).astype(f32)
-            p[rng.integers(0, 3)] = x
-            if rng.uniform() < 0.3:                                          # on faces of two axes at once
-                p[(np.argmax(p == x) + 1) % 3] = x
-            pts.append(p)
-    return np.stack(pts).astype(f32)
-
-
-def kernel_density_grad(field, x, with_density=True):
-    """xrb_ngp_density_grad on x f32[n,3] through the C ABI (density=NULL when with_density is False)"""
-    from xrnerf_b200 import _C
-    field.refresh()
-    n = len(x)
-    xt = torch.from_numpy(np.ascontiguousarray(x)).cuda() if n else torch.empty((0, 3), device='cuda')
-    dens = torch.full((n,), float('nan'), device='cuda')
-    grad = torch.full((n, 3), float('nan'), device='cuda')
-    _C.check(_C.lib.xrb_ngp_density_grad(field.cfg, field.tab, _C.ptr(field._dens16), _C.ptr(xt), 3, n, _C.f32(dens) if with_density else None, _C.f32(grad), _C.stream()),
-             'density_grad')
-    torch.cuda.synchronize()
-    return dens.cpu().numpy().astype(np.float64), grad.cpu().numpy().astype(np.float64)
-
-
 # ================================================================================================================ GPU tests
 CASES = [(dh, npk) for dh in (1, 2) for npk in (0, 6, 7)]
 
@@ -307,8 +129,8 @@ CASES = [(dh, npk) for dh in (1, 2) for npk in (0, 6, 7)]
 @pytest.fixture(scope='module', params=CASES, ids=[f'dh{dh}-packed{npk}' for dh, npk in CASES])
 def case(request):
     dh, npk = request.param
-    f = make_field(dh, npk)
-    return f, Grid(f)
+    f = ngp_field(dh, npk)
+    return f, Grid.of(f)
 
 
 @pytest.mark.gpu
@@ -327,10 +149,10 @@ def test_density_is_bit_identical_to_run_density(case):
 
 
 def _check_against_restatement(field, grid, x, what, with_density=True):
-    dens, g = kernel_density_grad(field, x, with_density)
+    dens, g = ngp_density_grad(field, x, with_density)
     if not len(x):
         return 0
-    want_d, g64, bound = restated(field, grid, x)
+    want_d, g64, bound = cuda_core_density_grad(field, grid, x)
     if with_density:
         assert np.array_equal(dens.astype(f32).view(np.uint32), want_d.astype(f32).view(np.uint32)), f'{what}: density differs from the restated CUDA-core forward'
     else:
@@ -361,7 +183,7 @@ def f64_density(grid, mats, x):
     for l in range(16):
         px = float(grid.scale[l]) * x + 0.5
         gi = np.floor(px).astype(np.int64)
-        _, w = trilinear_grad_terms(px - gi)
+        _, w = grid.trilinear(px - gi)
         v = grid.corner_values(l, gi)
         enc[:, 2 * l:2 * l + 2] = (w[:, :, None] * v).sum(1)
     a, pre = enc, []
@@ -379,9 +201,9 @@ def test_gradient_matches_finite_differences(dh):
     decision fixed, that function is linear along each axis, so the difference quotient is its derivative up to float64 rounding. The kernel differs
     from it by its fp32 rounding (the restatement's bound), by its in-cell positions being fp32 (|df| <= 2^-24 (scale_l + 1) per axis, moving the
     weight products by at most the sum over the other two axes) and by the difference quotient's float64 rounding."""
-    field = make_field(dh, 6, seed=5)
-    grid = Grid(field)
-    mats = net_mats(field)
+    field = ngp_field(dh, 6, seed=5)
+    grid = Grid.of(field)
+    mats = field_mats(field)
     h = 2.0 ** -20
     x = random_points(6000, 21).astype(np.float64)
     keep = np.ones(len(x), bool)
@@ -399,13 +221,13 @@ def test_gradient_matches_finite_differences(dh):
             for z0, z in zip(pre0, pre):
                 keep &= ((z0 > 0) == (z > 0)).all(1)
     xk = x.astype(f32)
-    _, masks_k = kernel_forward(mats, _enc16(field, xk))
+    _, masks_k = cuda_core_density(mats, hashgrid_enc16(field, xk))
     for z0, mk in zip(pre0, masks_k):                                     # the kernel's masks (fp16 activation > 0) are the float64 function's
         keep &= ((z0 > 0) == mk).all(1)
     assert keep.sum() >= 1000, keep.sum()
     fd = np.stack([(sides[2 * a + 1] - sides[2 * a]) / (2 * h) for a in range(3)], 1)[keep]
-    _, g = kernel_density_grad(field, xk[keep])
-    _, _, bound = restated(field, grid, xk[keep])
+    _, g = ngp_density_grad(field, xk[keep])
+    _, _, bound = cuda_core_density_grad(field, grid, xk[keep])
     # the in-cell positions: the kernel's are fp32 (|df| <= 2^-24 (scale_l + 1) per axis), which moves dw_c/df_a by at most the sum of |df| over the
     # other two axes; the float64 function's are rounded too (2^-53 (scale_l + 1)), which moves each side's value by the level's |dF/df| times that
     ge, gea = enc_grad(mats, [m[keep] for m in masks_k])
@@ -414,7 +236,7 @@ def test_gradient_matches_finite_differences(dh):
     for l in range(16):
         gi, fk = grid.cell(l, xk[keep])
         v = grid.corner_values(l, gi)
-        dw, w = trilinear_grad_terms(fk)
+        dw, w = grid.trilinear(fk)
         sa = np.abs(v[:, :, 0]) * gea[:, None, 2 * l] + np.abs(v[:, :, 1]) * gea[:, None, 2 * l + 1]
         sc = float(grid.scale[l])
         cellpos += sc * 2 * U32 * (sc + 1) * sa.sum(1)[:, None] * 1.0001
@@ -433,65 +255,10 @@ def test_gradient_matches_finite_differences(dh):
     print(REPORT[-1])
 
 
-def _enc16(field, x):
-    from xrnerf_b200 import _C
-    xt = torch.from_numpy(np.ascontiguousarray(x, f32)).cuda()
-    enc = torch.empty((len(x), 32), dtype=torch.float16, device='cuda')
-    _C.check(_C.lib.xrb_tcnn_hashgrid_forward(field.cfg, field.tab, _C.ptr(xt), 3, len(x), _C.ptr(enc), _C.stream()), 'hashgrid_forward')
-    return enc.cpu().numpy().astype(np.float64)
-
-
-NGP_MODEL = dict(   # configs/instant_ngp/nerf_blender_local01.py's model
-    type='HashNerfNetwork', cfg=dict(phase='train', chunk=4096, bs_data='rays_o'),
-    mlp=dict(type='HashNerfMLP', bound=1,
-             embedder_pos=dict(n_input_dims=3, encoding_config=dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=16, interpolation='Linear')),
-             embedder_dir=dict(n_input_dims=3, encoding_config=dict(otype='SphericalHarmonics', degree=4)),
-             density_net=dict(n_input_dims=32, n_output_dims=16, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=1)),
-             color_net=dict(n_output_dims=3, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=2))),
-    sampler=dict(type='NGPGridSampler', update_grid_freq=16, update_block_size=5000000, n_rays_per_batch=4096, cone_angle_constant=0.00390625, near_distance=0.2,
-                 target_batch_size=1 << 18, rgb_activation=2, density_activation=3),
-    render=dict(type='HashNerfRender', bg_color=[0, 0, 0]))
-
-
-def _network():
-    from xrnerf_b200 import registry as R, synth
-    net = R.build_network(NGP_MODEL).cuda()
-    table, dens, color = synth.ngp_weights(seed=3, hash_range=0.5, mlp_gain=2.0)
-    with torch.no_grad():
-        f = net.mlp.field
-        f.hash_params.copy_(torch.from_numpy(table)); f.density_params.copy_(torch.from_numpy(dens)); f.color_params.copy_(torch.from_numpy(color))
-    return net
-
-
-SPHERE_C, SPHERE_R, SPHERE_THR = 0.5, 0.3, 0.05   # raw density = fp16(r - |x - c|) at the level-4 grid points, level set raw = 0.05
-
-
-def _sphere_network():
-    """level 4 (dense, resolution 59) holds fp16 samples of r - |x - c| in feature 0 and every other entry is 0; the density net has two hidden units,
-    +enc[8] and -enc[8], and output row (+1, -1): the raw density is the trilinear interpolant of those samples"""
-    net = _network()
-    f = net.mlp.field
-    grid = Grid(f)
-    l, r = 4, int(grid.res[4])
-    assert r == 59 and r ** 3 <= grid.off[5] - grid.off[4]
-    i = np.arange(r)
-    z, y, x = np.meshgrid(i, i, i, indexing='ij')                         # grid point (x, y, z) at index x + y r + z r^2
-    pos = (np.stack([x, y, z], -1).astype(np.float64) - 0.5) / float(grid.scale[l])
-    sdf = (SPHERE_R - np.linalg.norm(pos - SPHERE_C, axis=-1)).astype(np.float16).astype(f32)
-    table = np.zeros(f.hash_params.numel(), f32)
-    table[2 * grid.off[l]:2 * (grid.off[l] + r ** 3):2] = sdf.reshape(-1)
-    dens = np.zeros(f.density_params.numel(), f32)
-    dens[0 * 32 + 8], dens[1 * 32 + 8] = 1.0, -1.0                       # W_in [64][32]
-    dens[64 * 32 + 0], dens[64 * 32 + 1] = 1.0, -1.0                     # W_out row 0
-    with torch.no_grad():
-        f.hash_params.copy_(torch.from_numpy(table)); f.density_params.copy_(torch.from_numpy(dens))
-    return net, Grid(f)
-
-
 @pytest.mark.gpu
 def test_sphere_normals():
     from xrnerf_b200.mesh import marching_cubes, raw_density_threshold
-    net, grid = _sphere_network()
+    net, grid = sphere_network()
     field = net.mlp.field
     sigma = math.exp(SPHERE_THR)                                         # the sampler's density activation is exponential
     verts, faces, normals, colors = net.extract_colored_mesh(resolution=128, threshold=sigma)
@@ -499,8 +266,8 @@ def test_sphere_normals():
     vw = marching_cubes(field.density_lattice((128,) * 3), raw_density_threshold(sigma, 3))[0]
     x = vw.cpu().numpy()
     # the kernel's gradient is the interpolant's: the restatement with d(out 0)/d(encoding) = e_8
-    _, g = kernel_density_grad(field, x)
-    dens, g64, bound = restated(field, grid, x)
+    _, g = ngp_density_grad(field, x)
+    dens, g64, bound = cuda_core_density_grad(field, grid, x)
     assert (dens > 0).all() and (np.abs(g - g64) <= bound).all()
     n = normals.cpu().numpy().astype(np.float64)
     v, fc = verts.cpu().numpy().astype(np.float64), faces.cpu().numpy()
@@ -526,7 +293,7 @@ def test_sphere_normals():
 @pytest.mark.gpu
 def test_extract_colored_mesh_equals_its_parts():
     from xrnerf_b200.mesh import marching_cubes, activate_rgb, raw_density_threshold
-    net = _network()
+    net = ngp_network()
     field = net.mlp.field
     vol = field.density_lattice((48, 48, 48))
     sigma = math.exp(float(torch.quantile(vol.reshape(-1)[::7], 0.7)))

@@ -8,54 +8,26 @@ weights, activations and ReLU masks. The mesh path is checked on a NerfMLP whose
 band-0 sine columns, so the footprint moves the surface."""
 import ctypes as C
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
+from cases import MIP_CFG, MIP_MLP, MIP_RENDER, NERF_MLP, host_buffer, nerf_mlp
+from restate64 import U16, U32, area, check_closed_oriented, columns, euler, lattice_coords, lattice_points, mc_oracle, mip_bands, trunk_grad, w16
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_mesh import check_closed_oriented, area, euler, lattice_coords, mc_oracle  # noqa: E402
-from test_gpu_nerf_mesh import U16, U32, _decode, _lattice_points, _w16  # noqa: E402
-
-MIP_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-               embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
 BOX = ((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))
 CELL_256 = 3.0 / 255 / math.sqrt(12.0)                                  # footprint 'cell' at 256^3 over BOX: 3.4e-3
 SIGMAS = [0.0, 1e-3, CELL_256, 0.05, 1.0]
 HALF_PI32 = np.float32(0.5 * np.pi)
 
 
-def _bands(sigma, min_deg=0, max_deg=16):
-    """the per-band factors a_k of a launch as the library forms them: hv = 0.5 ((sigma^2 2^deg) 2^deg) in fp32, a_k = fp32(exp(-hv)), and the band is
-    live iff hv <= 20 -> float64 [n_deg] (0 for a dead band)"""
-    s = np.float32(sigma)
-    cov = s * s
-    out = np.zeros(max_deg - min_deg)
-    for k in range(max_deg - min_deg):
-        sc = np.float32(2.0 ** (min_deg + k))
-        hv = np.float32(0.5) * (cov * sc * sc)
-        if not hv <= 20:
-            break
-        out[k] = float(np.float32(np.exp(-np.float64(hv))))
-    return out
-
-
 # ---------------------------------------------------------------------------------------------------------------- CPU: argument checks
-def _cpu_buf():
-    buf = (C.c_char * 64)()
-    a = (C.addressof(buf) + 15) & ~15
-    return buf, a, C.c_void_p(a)
-
-
 def test_mip_density_lattice_validates_arguments_without_gpu():
     from xrnerf_b200 import _C
     lib = _C.lib
     lo, hi = _C.float3(BOX[0]), _C.float3(BOX[1])
-    buf, a, p = _cpu_buf()
+    buf, a = host_buffer()
+    p = C.c_void_p(a)
     for n in ((1, 4, 4), (4, 1025, 4), (4, 4, -1)):
         assert lib.xrb_mip_density_lattice(p, p, 0, 16, 0.01, *n, lo, hi, p, None) == -1 and b'bad size' in lib.xrb_last_error()
     for d0, d1 in ((0, 22), (4, 4), (5, 2), (-101, -90)):
@@ -78,7 +50,8 @@ def test_mip_density_lattice_validates_arguments_without_gpu():
 def test_mip_ipe_tiles_points_validates_arguments_without_gpu():
     from xrnerf_b200 import _C
     lib = _C.lib
-    buf, a, p = _cpu_buf()
+    buf, a = host_buffer()
+    p = C.c_void_p(a)
     f = lib.xrb_mip_ipe_tiles_points
     assert f(p, p, -1, 1, 0.01, 0, 16, 0, 4, p, None) == -1 and b'bad size' in lib.xrb_last_error()
     assert f(p, p, 4, 0, 0.01, 0, 16, 0, 4, p, None) == -1
@@ -95,7 +68,8 @@ def test_mip_ipe_tiles_points_validates_arguments_without_gpu():
 def test_mip_ipe_grad_validates_arguments_without_gpu():
     from xrnerf_b200 import _C
     lib = _C.lib
-    buf, a, p = _cpu_buf()
+    buf, a = host_buffer()
+    p = C.c_void_p(a)
     f = lib.xrb_mip_ipe_grad
     assert f(p, -1, 0.01, 0, 16, p, 2, p, p, None) == -1 and b'bad size' in lib.xrb_last_error()
     assert f(p, 4, 0.01, 0, 22, p, 2, p, p, None) == -1 and f(p, 4, 0.01, 2, 2, p, 2, p, p, None) == -1
@@ -156,17 +130,6 @@ def test_mip_network_footprint_errors_without_gpu():
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU helpers
-def _mlp(seed, scaled=False):
-    from xrnerf_b200 import registry as R
-    torch.manual_seed(seed)
-    mlp = R.build_mlp(MIP_MLP).cuda()
-    if scaled:   # larger weights and biases of both signs: units switch on and off across the box
-        with torch.no_grad():
-            for p in mlp.parameters():
-                p.mul_(2.0) if p.dim() == 2 else p.uniform_(-0.5, 0.5)
-    return mlp
-
-
 def _encode(pts, dirs, sigma, spr=1):
     """the point encoder's tile image (3 blocks per tile) of (pts, dirs) at footprint sigma"""
     from xrnerf_b200 import _C
@@ -182,11 +145,6 @@ def _infer(mlp, pts, dirs, sigma):
     from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles
     image, bias = mlp._packed()
     return nerf_mlp_forward_tiles(image, bias, _encode(pts, dirs, sigma), pts.shape[0], 96, 27)
-
-
-class _Img:
-    def __init__(self, buf):
-        self.buf = buf
 
 
 def _threshold_sigma():
@@ -221,23 +179,23 @@ def test_point_encoder_matches_reference_ipe():
     sig_thr = _threshold_sigma()
     for sigma in SIGMAS + [sig_thr]:
         enc = _encode(pts, dirs, sigma)
-        got = _decode(_Img(enc), n, 3, 0, 96).cpu().numpy()
+        got = columns(enc, n, 3, 0, 96).cpu().numpy()
         s32 = np.float32(sigma)
         want = O.integrated_pos_enc(p64, np.full_like(p64, s32 * s32), 0, 16).astype(np.float64)
         tol = (U16 + 2 * U32) * np.abs(want) + 2.0 ** -25 + 8 * U32
         assert (np.abs(got - want) <= tol).all(), (sigma, float((np.abs(got - want) / tol).max()))
-        fac = _bands(sigma)
+        fac = mip_bands(sigma)
         dead = np.concatenate([np.repeat(fac == 0, 3)] * 2)
         assert (got[:, dead] == 0).all()
         if sigma == 1.0:
             assert dead.sum() == 6 * 13                                   # hv = 0.5, 2, 8 live; 32 and above dead
         if sigma == sig_thr:
             assert not dead[9] and dead[12] and fac[3] > 0               # band 3 exactly at the threshold: evaluated (and below fp16's range)
-        d_got = _decode(_Img(enc), n, 3, 2, 27).cpu().numpy()
+        d_got = columns(enc, n, 3, 2, 27).cpu().numpy()
         d_want = O.mip_pos_enc(dirs.cpu().numpy(), 0, 4).astype(np.float64)
         assert (np.abs(d_got - d_want) <= U16 * np.abs(d_want) + 8 * U32).all()
         # padding columns 96..127 and the rows past n are +0
-        pad = _decode(_Img(enc), (n + 127) // 128 * 128, 3, 0, 128).cpu().numpy()
+        pad = columns(enc, (n + 127) // 128 * 128, 3, 0, 128).cpu().numpy()
         assert (pad[:, 96:] == 0).all() and (pad[n:] == 0).all()
     # the direction block, byte for byte, against the ray encoder's (one sample per ray)
     rays = _C.lib.xrb_nerf_enc_image_bytes(n, 96)
@@ -258,9 +216,9 @@ def test_mip_density_lattice_equals_encoder_and_inference_kernel_bit_for_bit(sha
     """(nz, ny, nx); totals 8, 105, 5049 and 2^21: three are not a multiple of the 128-row tile. A centred box and one with negative coordinates;
     every footprint of SIGMAS and 'cell' of the lattice itself."""
     from xrnerf_b200.mesh import footprint_sigma
-    mlp = _mlp(11, scaled)
+    mlp = nerf_mlp(MIP_MLP, 11, scaled)
     for box in (BOX, ((-2.0, -0.25, -3.5), (-0.5, 1.75, -1.0))):
-        pts = _lattice_points(shape, box)
+        pts = lattice_points(shape, box)
         dirs = torch.nn.functional.normalize(torch.randn_like(pts), dim=-1)
         for fp in SIGMAS + ['cell']:
             sigma = footprint_sigma(fp, shape, box)
@@ -285,27 +243,14 @@ def _kernel_forward(mlp, pts, sigma):
     T._fwd(n, S, 'pts0', [img.sub(0, 2)], H[0])
     for l in range(1, 8):
         T._fwd(n, S, f'pts{l}', ([img.sub(0, 2), H[l - 1]] if l == 5 else [H[l - 1]]), H[l])
-    return _decode(img, n, 3, 0, 96), [_decode(h, n, 4, 0, 256) for h in H]
+    return columns(enc, n, 3, 0, 96), [columns(h.buf, n, 4, 0, 256) for h in H]
 
 
 def _restated_grad(mlp, pts, sigma, H):
     """float64 d(raw alpha)/d(position) over the fp16 weights, with the kernels' ReLU masks (fp16 activation > 0) and the library's a_k; also the same
     chain on absolute values, which bounds the rounding error, and the absolute error bound of the final contraction's cosines"""
-    g, ga = _w16(mlp.alpha_linear)[0].expand(pts.shape[0], 256), _w16(mlp.alpha_linear)[0].abs().expand(pts.shape[0], 256)
-    e = torch.zeros((pts.shape[0], 96), dtype=torch.float64, device='cuda')
-    ea = torch.zeros_like(e)
-    for l in range(7, -1, -1):
-        m = (H[l] > 0).double()
-        g, ga = g * m, ga * m                                 # dZ of layer l
-        W = _w16(mlp.pts_linears[l])
-        if l == 0:
-            e, ea = e + g @ W, ea + ga @ W.abs()
-        elif l == 5:
-            e, ea = e + g @ W[:, :96], ea + ga @ W[:, :96].abs()
-            g, ga = g @ W[:, 96:], ga @ W[:, 96:].abs()
-        else:
-            g, ga = g @ W, ga @ W.abs()
-    fac = _bands(sigma)
+    e, ea = trunk_grad(mlp, H, 96)
+    fac = mip_bands(sigma)
     out, outa, trig = (torch.zeros_like(pts, dtype=torch.float64) for _ in range(3))
     for k in range(16):
         if fac[k] == 0:
@@ -341,7 +286,7 @@ def _check_grad(mlp, pts, sigma):
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [0, 1, 127, 129])
 def test_mip_density_grad_matches_float64_restatement(n):
-    mlp = _mlp(21, scaled=True)
+    mlp = nerf_mlp(MIP_MLP, 21, scaled=True)
     torch.manual_seed(n)
     pts = (torch.rand((n, 3), device='cuda') * 3 - 1.5).contiguous()
     for sigma in SIGMAS:
@@ -360,7 +305,7 @@ def test_mip_density_grad_matches_float64_restatement(n):
 def test_mip_density_grad_chunks_are_row_independent():
     """one chunk + 1 rows: the last rows equal the same rows run alone, bit for bit, and match the float64 restatement"""
     from xrnerf_b200 import nerf_train as T
-    mlp = _mlp(22, scaled=True)
+    mlp = nerf_mlp(MIP_MLP, 22, scaled=True)
     n = T.GRAD_CHUNK + 1
     torch.manual_seed(5)
     pts = (torch.rand((n, 3), device='cuda') * 3 - 1.5).contiguous()
@@ -374,18 +319,18 @@ def _f64_alpha(mlp, pts, sigma, phase):
     """the unrounded float64 raw alpha of the point query over the fp16 weights (no activation rounding) -> [n], and its pre-activations. The cos
     columns are a_k sin(y + phase), phase = the kernel's fp32 (y + pi/2) - y at the base point (the reference's expression), held over the stencil."""
     x = pts.double()
-    fac = _bands(sigma)
+    fac = mip_bands(sigma)
     sins = [fac[k] * torch.sin(x * 2.0 ** k) for k in range(16)]
     coss = [fac[k] * torch.sin(x * 2.0 ** k + phase[k]) for k in range(16)]
     enc = torch.cat([torch.cat(sins, -1), torch.cat(coss, -1)], -1)
     h, pre = enc, []
     for l, lin in enumerate(mlp.pts_linears):
-        z = h @ _w16(lin).T + lin.bias.detach().double()
+        z = h @ w16(lin).T + lin.bias.detach().double()
         pre.append(z)
         h = torch.relu(z)
         if l == 4:
             h = torch.cat([enc, h], -1)
-    return (h @ _w16(mlp.alpha_linear).T)[:, 0] + mlp.alpha_linear.bias.detach().double()[0], pre
+    return (h @ w16(mlp.alpha_linear).T)[:, 0] + mlp.alpha_linear.bias.detach().double()[0], pre
 
 
 @pytest.mark.gpu
@@ -393,11 +338,11 @@ def _f64_alpha(mlp, pts, sigma, phase):
 def test_mip_density_grad_matches_central_differences(sigma):
     """central differences of the unrounded float64 function, at points where its ReLU masks equal the kernels' and do not change over the stencil.
     The step is 1e-6 scaled to the highest live band, 2^top h <= 2^9 1e-6 (NeRF's stencil at its 2^9-scaled sines), so the masks can hold over it."""
-    mlp = _mlp(23, scaled=True)
+    mlp = nerf_mlp(MIP_MLP, 23, scaled=True)
     torch.manual_seed(9)
     pts = (torch.rand((4096, 3), device='cuda') * 3 - 1.5).contiguous()
     phase = lambda p: [((p * 2.0 ** k) + float(HALF_PI32)).double() - (p * 2.0 ** k).double() for k in range(16)]
-    top = int(np.nonzero(_bands(sigma))[0].max())
+    top = int(np.nonzero(mip_bands(sigma))[0].max())
     h = 1e-6 * min(1.0, 2.0 ** (9 - top))
     eye = torch.eye(3, device='cuda', dtype=torch.float64)
     mlp.density_grad(pts[:1], footprint=sigma)
@@ -433,9 +378,7 @@ def _sine_network():
     view direction: pts_linears.0 takes relu(+-a_0 sin x_a) from the band-0 sine columns 0..2, layers 1-7 pass the six units through, alpha_linear
     sums them; views_linears.0 takes relu(+-d_a) from the direction's identity columns, rgb_linear forms d_a."""
     from xrnerf_b200.registry.networks import MipNerfNetwork
-    net = MipNerfNetwork(dict(phase='test', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800, bs_data='rays_o'),
-                         mlp=MIP_MLP, render=dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=RGB_PADDING, density_bias=-1,
-                                                  density_activation='softplus')).cuda()
+    net = MipNerfNetwork(dict(MIP_CFG, phase='test'), mlp=MIP_MLP, render=dict(MIP_RENDER, rgb_padding=RGB_PADDING)).cuda()
     m = net.mlp
     with torch.no_grad():
         for p in m.parameters():
@@ -458,7 +401,7 @@ def _sine_network():
 def test_sine_field_mesh_geometry_normals_and_colours(sigma):
     from xrnerf_b200.mesh import raw_density_threshold
     net = _sine_network()
-    a0 = _bands(sigma)[0]
+    a0 = mip_bands(sigma)[0]
     assert a0 == (1.0 if sigma == 0 else float(np.float32(math.exp(-0.125))))
     dens = math.log1p(math.exp(-1.0))                                    # softplus(raw - 1) at raw = 0: the level set raw = 0
     thr = raw_density_threshold(dens, 'softplus', -1.0)
@@ -503,9 +446,7 @@ def test_mip_colored_mesh_equals_its_parts():
     from xrnerf_b200.mesh import footprint_sigma, marching_cubes, raw_density_threshold
     from xrnerf_b200.registry.networks import MipNerfNetwork
     torch.manual_seed(31)
-    net = MipNerfNetwork(dict(phase='test', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800, bs_data='rays_o'),
-                         mlp=MIP_MLP, render=dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=RGB_PADDING, density_bias=-1,
-                                                  density_activation='softplus')).cuda()
+    net = MipNerfNetwork(dict(MIP_CFG, phase='test'), mlp=MIP_MLP, render=dict(MIP_RENDER, rgb_padding=RGB_PADDING)).cuda()
     res = 48
     sigma = footprint_sigma('cell', (res,) * 3, BOX)
     with torch.no_grad():

@@ -6,13 +6,10 @@ import os
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
 G = {**np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden.npz')), **np.load(os.path.join(os.path.dirname(__file__), 'golden', 'nerf_golden_embedded.npz'))}
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def close(a, b, tol=2e-5):

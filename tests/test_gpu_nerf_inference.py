@@ -7,66 +7,25 @@ import ctypes as C
 import numpy as np
 import pytest
 import torch
+from cases import FAR, MIP_CFG, MIP_MODEL, NEAR, NERF_MODEL, bits, nerf_net, view_rays, zvals
 
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-NERF_MODEL = dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF_MLP, mlp_fine=NERF_MLP,
-                  render=dict(type='NerfRender', white_bkgd=True, raw_noise_std=0))
-MIP_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-               embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
-MIP_CFG = dict(phase='train', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800, bs_data='rays_o')
-MIP_RENDER = dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=0.001, density_bias=-1, density_activation='softplus')
-NEAR, FAR = 0.5, 3.0        # not the linspace(2, 6) the renderers default to
 LEVEL_KEYS = ('rgb', 'disp', 'acc')
-
-
-def _net(mip, seed=0, **cfg):
-    from xrnerf_b200 import registry as R
-    torch.manual_seed(seed)
-    model = dict(type='MipNerfNetwork', cfg=dict(MIP_CFG, **cfg), mlp=MIP_MLP, render=MIP_RENDER) if mip else \
-        dict(NERF_MODEL, cfg=dict(NERF_MODEL['cfg'], **cfg))
-    return R.build_network(model).cuda()
-
-
-def _view_rays(H, W, seed, radii=True):
-    """every pixel of an H x W view of a Blender spiral pose, Blender intrinsics scaled to the view (xrb_nerf_get_rays, GetRays + GetViewdirs)"""
-    from xrnerf_b200 import _C, synth
-    rng = np.random.default_rng(seed)
-    pose = synth.pose_spherical(float(rng.uniform(-180, 180)), -30.0, 4.0)
-    c2w = (C.c_float * 12)(*[float(v) for v in pose[:3, :4].reshape(-1)])
-    n = H * W
-    f = float(synth.FOCAL) * W / 800.0
-    o, d, v = (torch.empty((n, 3), device='cuda') for _ in range(3))
-    r = torch.empty((n, 1), device='cuda') if radii else None
-    _C.check(_C.lib.xrb_nerf_get_rays(c2w, H, W, f, f, W / 2.0, H / 2.0, 0, None, n, _C.ptr(o), _C.ptr(d), _C.ptr(v), _C.ptr(r), _C.stream()), 'get_rays')
-    return o, d, v, r
-
-
-def _zvals(n, s, near=NEAR, far=FAR, lindisp=True):
-    from xrnerf_b200 import _C
-    z = torch.empty((n, s), device='cuda')
-    _C.check(_C.lib.xrb_nerf_zvals(n, s, float(near), float(far), int(lindisp), None, _C.ptr(z), _C.stream()), 'zvals')
-    return z
 
 
 def _nerf_data(n, seed):
     """rays through an 800 x 800 Blender camera (the first n pixels of a view 800 wide), GetZvals(lindisp, NEAR, FAR, 64) and GetPts"""
-    o, d, v, _ = _view_rays(n // 800 + 1, 800, seed, radii=False)
+    o, d, v, _ = view_rays(n // 800 + 1, 800, seed, radii=False)
     o, d, v = o[:n].contiguous(), d[:n].contiguous(), v[:n].contiguous()
-    z = _zvals(n, 64)
+    z = zvals(n, 64)
     return {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': z, 'pts': o[:, None] + d[:, None] * z[..., None]}
 
 
 def _mip_data(n, seed):
     """as _nerf_data with GetZvals(129) and per-ray radii spread over 0.5x..2x the camera's"""
-    o, d, v, r = _view_rays(n // 800 + 3, 800, seed)                             # the radii take a pixel's neighbours: H >= 3
+    o, d, v, r = view_rays(n // 800 + 3, 800, seed)                             # the radii take a pixel's neighbours: H >= 3
     g = torch.Generator(device='cuda').manual_seed(seed)
     r = r[:n] * (0.5 + 1.5 * torch.rand((n, 1), device='cuda', generator=g))
-    return {'rays_o': o[:n].contiguous(), 'rays_d': d[:n].contiguous(), 'viewdirs': v[:n].contiguous(), 'radii': r.contiguous(), 'z_vals': _zvals(n, 129)}
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
+    return {'rays_o': o[:n].contiguous(), 'rays_d': d[:n].contiguous(), 'viewdirs': v[:n].contiguous(), 'radii': r.contiguous(), 'z_vals': zvals(n, 129)}
 
 
 # ------------------------------------------------------------------------------------------------ fused == chunked
@@ -76,7 +35,7 @@ def _bits(t):
 def test_nerf_fused_batchify_matches_chunked(ray_batch):
     """NeRF 64 + 128 on lindisp z values over [0.5, 3]: the fused path equals the reference-shaped chunk loop within the renderer tolerances
     (coarse 2e-3, fine 5e-3). 1000 rays: not a multiple of either batch size. Rendering on linspace(2, 6) instead fails the tolerance."""
-    net = _net(False)
+    net = nerf_net(False)
     net.fused_ray_batch = ray_batch
     data = _nerf_data(1000, 1)
     with torch.no_grad():
@@ -98,7 +57,7 @@ def test_nerf_fused_batchify_matches_chunked(ray_batch):
 @pytest.mark.parametrize('ray_batch', [None, 384])
 def test_mip_fused_batchify_matches_chunked(ray_batch):
     """Mip-NeRF 2 x 128 with per-ray radii on lindisp z values over [0.5, 3]: fused == chunk loop within 1e-2 on rgb and acc of both levels."""
-    net = _net(True, seed=5)
+    net = nerf_net(True, seed=5)
     net.fused_ray_batch = ray_batch
     data = _mip_data(1000, 2)
     with torch.no_grad():
@@ -120,7 +79,7 @@ def test_mip_fused_batchify_matches_chunked(ray_batch):
 def test_batch_split_is_invisible(mip):
     """one batch and batches of 200 and 333 rays (1000 rays) give bit-identical rgb, disp, acc and depth on every level"""
     from xrnerf_b200.nerf import NerfRenderer, MipNerfRenderer
-    net = _net(mip, seed=7)
+    net = nerf_net(mip, seed=7)
     data = _mip_data(1000, 3) if mip else _nerf_data(1000, 3)
     outs = []
     for batch in (None, 200, 333):
@@ -131,7 +90,7 @@ def test_batch_split_is_invisible(mip):
     assert set(outs[0]) == {p + k for p in ('', 'coarse_') for k in LEVEL_KEYS + ('depth',)}
     for other in outs[1:]:
         for k, v in outs[0].items():
-            assert torch.equal(_bits(v), _bits(other[k])), k
+            assert torch.equal(bits(v), bits(other[k])), k
 
 
 # ------------------------------------------------------------------------------------------------ depth
@@ -162,7 +121,7 @@ def _mip_disp(depth, acc, z0, zl):
 
 def _same_bits_or_nan(a, b):
     na, nb = torch.isnan(a), torch.isnan(b)
-    return torch.equal(na, nb) and torch.equal(_bits(torch.where(na, 0.0, a)), _bits(torch.where(nb, 0.0, b)))
+    return torch.equal(na, nb) and torch.equal(bits(torch.where(na, 0.0, a)), bits(torch.where(nb, 0.0, b)))
 
 
 @pytest.mark.gpu
@@ -201,7 +160,7 @@ def test_renderer_disp_is_the_reference_formula_on_depth(mip):
     """the fused renderers' disp equals, bit for bit, the reference formula in fp32 on the returned depth and acc: both NeRF levels, and Mip-NeRF's first
     level (whose z_0 / z_last are the given z values); depth=False leaves the other outputs bit-identical"""
     from xrnerf_b200.nerf import NerfRenderer, MipNerfRenderer
-    net = _net(mip, seed=9)
+    net = nerf_net(mip, seed=9)
     data = _mip_data(700, 4) if mip else _nerf_data(700, 4)
     if mip:
         run = lambda dep: MipNerfRenderer(net).render(data['rays_o'], data['rays_d'], data['viewdirs'], data['radii'], z_vals=data['z_vals'], depth=dep)
@@ -230,9 +189,9 @@ def test_nerf_val_and_test_steps():
     """val_step: the reference's keys plus psnr, [H,W,3] / [H,W,1] device tensors for the validation and spiral poses; phase 'test' -> test_step
     (rgb, gt_img, disp, idx). fused_inference = False keeps the reference's keys in batchify_forward."""
     H, W = 24, 40
-    net = _net(False, seed=11)
-    o, d, v, _ = _view_rays(H, W, 5, radii=False)
-    z = _zvals(H * W, 64)
+    net = nerf_net(False, seed=11)
+    o, d, v, _ = view_rays(H, W, 5, radii=False)
+    z = zvals(H * W, 64)
     d_view = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': z, 'pts': o[:, None] + d[:, None] * z[..., None], 'src_shape': torch.tensor([H, W, 3])}
     seen = []
     net.set_val_pipeline(lambda item: (seen.append(item['pose'].shape), dict(d_view))[1])
@@ -264,9 +223,9 @@ def test_mip_multiscale_evaluate_once():
     """use_multiscale: a pixel-shaped view (per-pixel radii) is flattened and rendered through the fused path; validation returns one-element lists,
     phase 'test' the evaluate_once keys. Without use_multiscale val_step is NerfNetwork's."""
     H, W = 20, 36
-    net = _net(True, seed=13, use_multiscale=True)
-    o, d, v, r = _view_rays(H, W, 6)
-    z = _zvals(H * W, 129)
+    net = nerf_net(True, seed=13, use_multiscale=True)
+    o, d, v, r = view_rays(H, W, 6)
+    z = zvals(H * W, 129)
     image = torch.rand((1, H, W, 3), device='cuda')
     px = lambda t: t.reshape(1, H, W, -1)
     data = {'rays_o': px(o), 'rays_d': px(d), 'viewdirs': px(v), 'radii': px(r), 'z_vals': px(z), 'lossmult': torch.ones((1, H, W, 1), device='cuda'),
@@ -295,9 +254,9 @@ def test_whole_view_renders_in_bounded_memory():
     from xrnerf_b200.nerf import bytes_per_ray, ray_batch_size
     H = W = 800
     n = H * W
-    net = _net(False, seed=17)
-    o, d, v, _ = _view_rays(H, W, 8, radii=False)
-    view = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': _zvals(n, 64, 2.0, 6.0, False), 'src_shape': torch.tensor([H, W, 3])}
+    net = nerf_net(False, seed=17)
+    o, d, v, _ = view_rays(H, W, 8, radii=False)
+    view = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': zvals(n, 64, 2.0, 6.0, False), 'src_shape': torch.tensor([H, W, 3])}
     net.set_val_pipeline(lambda item: dict(view))
     image = torch.rand((1, 1, H, W, 3), device='cuda')
     net.val_step({'poses': torch.zeros((1, 1, 4, 4)), 'images': image})        # packs the weights once
@@ -367,7 +326,7 @@ def test_test_phase_dispatch_without_gpu():
     assert set(out) == {'rgb', 'gt_img', 'disp', 'idx'} and out['idx'] == 7 and torch.equal(out['gt_img'], image[0])
     assert out['rgb'].shape == (H, W, 3) and out['disp'].shape == (H, W, 1) and stub.calls[0][1] is True
     assert torch.equal(seen[0]['pose'], torch.eye(4)) and seen[0]['idx'] == 7
-    mip = R.build_network(dict(type='MipNerfNetwork', cfg=dict(MIP_CFG, use_multiscale=True), mlp=MIP_MLP, render=MIP_RENDER))
+    mip = R.build_network(dict(MIP_MODEL, cfg=dict(MIP_CFG, use_multiscale=True)))
     mip.batchify_forward = stub = _Stub()
     px = lambda c: torch.rand((1, H, W, c))
     data = {'rays_o': px(3), 'rays_d': px(3), 'viewdirs': px(3), 'radii': px(1), 'z_vals': px(129), 'image': image, 'idx': torch.tensor([[2]])}

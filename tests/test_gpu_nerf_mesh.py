@@ -6,20 +6,12 @@ with a float64 restatement over the kernels' own fp16 weights, activations and R
 r - (|x| + |y| + |z|): an octahedron with known volume, area and normals."""
 import ctypes as C
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_mesh import check_closed_oriented, area, euler, lattice_coords, mc_oracle  # noqa: E402
-
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-U16 = 2.0 ** -11   # unit roundoff of fp16
-U32 = 2.0 ** -24
+from cases import NERF_MLP, host_buffer, nerf_mlp
+from restate64 import U16, U32, area, check_closed_oriented, columns, euler, lattice_coords, lattice_points, mc_oracle, trunk_grad, w16
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU: argument checks
@@ -27,8 +19,7 @@ def test_density_lattice_validates_arguments_without_gpu():
     from xrnerf_b200 import _C
     lib = _C.lib
     lo, hi = _C.float3((-1.5, -1.5, -1.5)), _C.float3((1.5, 1.5, 1.5))
-    buf = (C.c_char * 64)()
-    a = (C.addressof(buf) + 15) & ~15
+    buf, a = host_buffer()
     p = C.c_void_p(a)
     for n in ((1, 4, 4), (4, 1025, 4), (4, 4, -1)):
         assert lib.xrb_nerf_density_lattice(p, p, 63, 10, *n, lo, hi, p, None) == -1 and b'bad size' in lib.xrb_last_error()
@@ -47,8 +38,7 @@ def test_density_lattice_validates_arguments_without_gpu():
 def test_posenc_grad_validates_arguments_without_gpu():
     from xrnerf_b200 import _C
     lib = _C.lib
-    buf = (C.c_char * 64)()
-    a = (C.addressof(buf) + 15) & ~15
+    buf, a = host_buffer()
     p = C.c_void_p(a)
     assert lib.xrb_nerf_posenc_grad(p, -1, 10, p, 2, p, p, None) == -1 and b'bad size' in lib.xrb_last_error()
     assert lib.xrb_nerf_posenc_grad(p, 4, 11, p, 2, p, p, None) == -1
@@ -91,24 +81,6 @@ def test_mip_network_and_cpu_mlp_refuse_mesh_export():
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU helpers
-def _mlp(seed, scaled=False):
-    from xrnerf_b200 import registry as R
-    torch.manual_seed(seed)
-    mlp = R.build_mlp(NERF_MLP).cuda()
-    if scaled:   # larger weights and biases of both signs: units switch on and off across the box
-        with torch.no_grad():
-            for p in mlp.parameters():
-                p.mul_(2.0) if p.dim() == 2 else p.uniform_(-0.5, 0.5)
-    return mlp
-
-
-def _lattice_points(shape, box):
-    nz, ny, nx = shape
-    cx, cy, cz = (lattice_coords(box[0][a], box[1][a], n) for a, n in enumerate((nx, ny, nz)))
-    Z, Y, X = np.meshgrid(cz, cy, cx, indexing='ij')
-    return torch.from_numpy(np.stack([X, Y, Z], -1).reshape(-1, 3).copy()).cuda()
-
-
 def _infer(mlp, pts, dirs):
     """raw f32[n,4] of the inference kernel on the posenc_tiles encoding of (pts, dirs)"""
     from xrnerf_b200 import _C
@@ -126,11 +98,11 @@ def _infer(mlp, pts, dirs):
 @pytest.mark.parametrize('scaled', [False, True])
 def test_density_lattice_equals_inference_kernel_bit_for_bit(shape, scaled):
     """(nz, ny, nx); totals 8, 105, 5049 and 2^21: three are not a multiple of the 128-row tile. Boxes with negative coordinates."""
-    mlp = _mlp(11, scaled)
+    mlp = nerf_mlp(NERF_MLP, 11, scaled)
     for box in (((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5)), ((-2.0, -0.25, -3.5), (-0.5, 1.75, -1.0))):
         with torch.no_grad():
             vol = mlp.density_lattice(shape, box)
-            pts = _lattice_points(shape, box)
+            pts = lattice_points(shape, box)
             dirs = torch.nn.functional.normalize(torch.randn_like(pts), dim=-1)
             raw = _infer(mlp, pts, dirs)
         torch.cuda.synchronize()
@@ -139,18 +111,6 @@ def test_density_lattice_equals_inference_kernel_bit_for_bit(shape, scaled):
 
 
 # ---------------------------------------------------------------------------------------------------------------- gradient: float64 restatement
-def _decode(img, n, n_blk, blk0, cols):
-    """fp16 entries (row, col) of the `cols` columns starting at block blk0 of a tile image with n_blk blocks per tile -> float64 [n, cols]"""
-    r = torch.arange(n, device='cuda')[:, None]
-    c = torch.arange(cols, device='cuda')[None, :]
-    b = blk0 + c // 64
-    cc = c % 64
-    rr = r % 128
-    off = ((r // 128) * n_blk + b) * 16384 + (rr >> 3) * 1024 + (rr & 7) * 128 + (((cc >> 3) ^ (rr & 7)) << 4) + (cc & 7) * 2
-    h = img.buf.view(torch.float16)
-    return h[(off // 2).reshape(-1)].reshape(n, cols).double()
-
-
 def _kernel_forward(mlp, pts):
     """the training kernels' forward as density_grad runs it: encoding (fp16) and the 8 hidden activations (fp16) as float64"""
     from xrnerf_b200 import _C
@@ -165,30 +125,13 @@ def _kernel_forward(mlp, pts):
     T._fwd(n, S, 'pts0', [enc.sub(0, 1)], H[0])
     for l in range(1, 8):
         T._fwd(n, S, f'pts{l}', ([enc.sub(0, 1), H[l - 1]] if l == 5 else [H[l - 1]]), H[l])
-    return _decode(enc, n, 2, 0, 63), [_decode(h, n, 4, 0, 256) for h in H]
-
-
-def _w16(lin):
-    return lin.weight.detach().half().double()
+    return columns(enc.buf, n, 2, 0, 63), [columns(h.buf, n, 4, 0, 256) for h in H]
 
 
 def _restated_grad(mlp, pts, enc, H):
     """float64 d(raw alpha)/d(position) over the fp16 weights, with the kernels' ReLU masks (fp16 activation > 0); also the same chain on absolute
     values, which bounds the rounding error"""
-    g, ga = _w16(mlp.alpha_linear)[0].expand(pts.shape[0], 256), _w16(mlp.alpha_linear)[0].abs().expand(pts.shape[0], 256)
-    e = torch.zeros((pts.shape[0], 63), dtype=torch.float64, device='cuda')
-    ea = torch.zeros_like(e)
-    for l in range(7, -1, -1):
-        m = (H[l] > 0).double()
-        g, ga = g * m, ga * m                                 # dZ of layer l
-        W = _w16(mlp.pts_linears[l])
-        if l == 0:
-            e, ea = e + g @ W, ea + ga @ W.abs()
-        elif l == 5:
-            e, ea = e + g @ W[:, :63], ea + ga @ W[:, :63].abs()
-            g, ga = g @ W[:, 63:], ga @ W[:, 63:].abs()
-        else:
-            g, ga = g @ W, ga @ W.abs()
+    e, ea = trunk_grad(mlp, H, 63)
     out, outa = e[:, :3].clone(), ea[:, :3].clone()
     for b in range(10):
         y = (pts * 2.0 ** b).double()                         # the kernel's fp32 argument, exact
@@ -217,7 +160,7 @@ def _check_grad(mlp, pts):
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [0, 1, 127, 129])
 def test_density_grad_matches_float64_restatement(n):
-    mlp = _mlp(21, scaled=True)
+    mlp = nerf_mlp(NERF_MLP, 21, scaled=True)
     torch.manual_seed(n)
     pts = (torch.rand((n, 3), device='cuda') * 3 - 1.5).contiguous()
     dens, grad = mlp.density_grad(pts)
@@ -235,7 +178,7 @@ def test_density_grad_matches_float64_restatement(n):
 def test_density_grad_chunks_are_row_independent():
     """one chunk + 1 rows: the last rows equal the same rows run alone, bit for bit, and match the float64 restatement"""
     from xrnerf_b200 import nerf_train as T
-    mlp = _mlp(22, scaled=True)
+    mlp = nerf_mlp(NERF_MLP, 22, scaled=True)
     n = T.GRAD_CHUNK + 1
     torch.manual_seed(5)
     pts = (torch.rand((n, 3), device='cuda') * 3 - 1.5).contiguous()
@@ -251,18 +194,18 @@ def _f64_alpha(mlp, pts):
     enc = torch.cat([x] + [torch.cat([torch.sin(x * 2.0 ** b), torch.cos(x * 2.0 ** b)], -1) for b in range(10)], -1)
     h, pre = enc, []
     for l, lin in enumerate(mlp.pts_linears):
-        z = h @ _w16(lin).T + lin.bias.detach().double()
+        z = h @ w16(lin).T + lin.bias.detach().double()
         pre.append(z)
         h = torch.relu(z)
         if l == 4:
             h = torch.cat([enc, h], -1)
-    return (h @ _w16(mlp.alpha_linear).T)[:, 0] + mlp.alpha_linear.bias.detach().double()[0], pre
+    return (h @ w16(mlp.alpha_linear).T)[:, 0] + mlp.alpha_linear.bias.detach().double()[0], pre
 
 
 @pytest.mark.gpu
 def test_density_grad_matches_central_differences():
     """central differences of the unrounded float64 function, at points where its ReLU masks equal the kernels' and do not change over the stencil"""
-    mlp = _mlp(23, scaled=True)
+    mlp = nerf_mlp(NERF_MLP, 23, scaled=True)
     torch.manual_seed(9)
     pts = (torch.rand((4096, 3), device='cuda') * 3 - 1.5).contiguous()
     h = 1e-6

@@ -4,13 +4,9 @@ reference's arithmetic) and the numpy oracle. Tolerance for the fp16-operand / f
 import numpy as np
 import pytest
 import torch
+from cases import MIP_CFG, MIP_MLP, MIP_MODEL, NERF_MLP
 
 pytestmark = pytest.mark.gpu
-
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-MIP_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-               embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
 
 
 def _ref_fp32(mlp, emb):
@@ -115,8 +111,7 @@ def test_weight_repack_on_update():
     assert torch.allclose(b[..., :3], a[..., :3] + 1.0, atol=1e-5) and torch.equal(a[..., 3], b[..., 3])
 
 
-MIP_MODEL = dict(type='MipNerfNetwork', cfg=dict(phase='test', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800, bs_data='rays_o'),
-                 mlp=MIP_MLP, render=dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=0.001, density_bias=-1, density_activation='softplus'))
+MIP_TEST_MODEL = dict(MIP_MODEL, cfg=dict(MIP_CFG, phase='test'))
 
 
 def _mip_rays(n, seed):
@@ -212,7 +207,7 @@ def test_fused_mip_renderer_matches_registry_network():
     from xrnerf_b200 import registry as R
     from xrnerf_b200.nerf import MipNerfRenderer
     torch.manual_seed(5)
-    net = R.build_network(MIP_MODEL).cuda()
+    net = R.build_network(MIP_TEST_MODEL).cuda()
     n, S = 200, 128
     o, d, vd, radii = _mip_rays(n, 6)
     with torch.no_grad():

@@ -18,34 +18,21 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_nerf_inference import MIP_CFG, MIP_MLP, MIP_RENDER, NERF_MLP, NERF_MODEL, _bits, _view_rays, _zvals
+from cases import MIP_MLP, NERF_MLP, bits, nerf_net, view_rays, zvals
+from restate64 import GAMMA_TC as TC, U16, columns, decode, f16, w16
 
-U16, TC = 2.0 ** -11, 2.0 ** -22
 REPORT = []
-
-
-def _net(mip, seed=0, scale=1.0, **cfg):
-    from xrnerf_b200 import registry as R
-    torch.manual_seed(seed)
-    model = dict(type='MipNerfNetwork', cfg=dict(MIP_CFG, **cfg), mlp=MIP_MLP, render=MIP_RENDER) if mip else dict(NERF_MODEL, cfg=dict(NERF_MODEL['cfg'], **cfg))
-    net = R.build_network(model).cuda()
-    if scale != 1.0:        # layers 1..7 scaled by 2^-6: d(density)/d(hidden) spans 2^42 and more between pts_linears.7 and pts_linears.0
-        with torch.no_grad():
-            for m in net._fused_mlps():
-                for lin in m.pts_linears[1:]:
-                    lin.weight.mul_(scale)
-    return net
 
 
 def _rays(mip, n, s, seed, d_zero=False):
     """n rays of an 800-wide Blender view with s samples each (z [n,s], or [n,s+1] interval ends and radii for Mip-NeRF)"""
-    o, d, v, r = _view_rays(n // 800 + 3, 800, seed)
+    o, d, v, r = view_rays(n // 800 + 3, 800, seed)
     o, d, v, r = o[:n].contiguous(), d[:n].contiguous(), v[:n].contiguous(), r[:n].reshape(-1).contiguous()
     if d_zero:
         d = torch.zeros_like(d)
         r = torch.zeros_like(r)
     w = s + 1 if mip else s
-    z = _zvals(n, w, 2.0, 6.0, False) if w > 1 else torch.full((n, 1), 3.0, device='cuda')
+    z = zvals(n, w, 2.0, 6.0, False) if w > 1 else torch.full((n, 1), 3.0, device='cuda')
     return o, d, v, z, (r if mip else None)
 
 
@@ -58,16 +45,7 @@ def _grad(mlp, o, d, v, z, r):
 
 def _enc_rows(enc, n_rows, ic):
     """the fp16 point-encoding columns of the tile image, float64 [n_rows, ic]"""
-    nb = (ic + 63) // 64 + 1
-    h = enc.cpu().numpy().view(np.float16).reshape(-1, nb, 128, 64)          # [tile][block][8-row atoms x 8 rows][64]
-    r = np.arange(128)
-    out = np.zeros((h.shape[0], 128, (nb - 1) * 64))
-    flat = enc.cpu().numpy().view(np.float16).reshape(-1, nb, 128 * 64)
-    for b in range(nb - 1):
-        for c in range(64):
-            off = ((r >> 3) * 1024 + (r & 7) * 128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7) * 2) // 2
-            out[:, :, 64 * b + c] = flat[:, b, off]
-    return out.reshape(-1, (nb - 1) * 64)[:n_rows, :ic].astype(np.float64)
+    return columns(enc, n_rows, (ic + 63) // 64 + 1, 0, ic).cpu().numpy()
 
 
 def _positions(mip, o, d, z, r, e):
@@ -109,13 +87,12 @@ def _positions(mip, o, d, z, r, e):
 
 def _restated(mlp, enc16, J):
     """float64 gradient, its bound and the rows whose masks are unambiguous"""
-    W = [l.weight.detach().half().double().cpu().numpy() for l in mlp.pts_linears]
-    b = [l.bias.detach().float().cpu().numpy().astype(np.float16).astype(np.float64) for l in mlp.pts_linears]
+    W = [w16(l).cpu().numpy() for l in mlp.pts_linears]
+    b = [f16(l.bias.detach().float().cpu().numpy()) for l in mlp.pts_linears]
     wa = mlp.alpha_linear.weight.detach().float().cpu().numpy()[0].astype(np.float64)
     ic = mlp.input_ch
     masks, ambs, ok = [], [], np.ones(len(enc16), bool)
     h, eh = enc16, np.zeros_like(enc16)                        # layer input and its spread against the kernel's
-    f16 = lambda t: t.astype(np.float16).astype(np.float64)
     for l in range(8):
         x, ex = (np.concatenate([enc16, h], 1), np.concatenate([np.zeros_like(enc16), eh], 1)) if l == 5 else (h, eh)
         z = x @ W[l].T
@@ -165,26 +142,26 @@ def test_density_bit_identical_to_the_inference_kernel(mip, scale):
     """density_out == raw[:, 3] of xrb_nerf_mlp_forward on the same encoding image, for 1, 127, 129 and 5000 rows (ragged S); a row does not depend on
     the batch split (200 / 333 rays against one batch)"""
     from xrnerf_b200.nerf_mlp import nerf_mlp_forward_tiles
-    net = _net(mip, seed=1, scale=scale)
+    net = nerf_net(mip, seed=1, scale=scale)
     mlp = net.mlp
     image, bias = mlp._packed()
     for n, s in ((1, 1), (1, 127), (3, 43), (50, 100)):
         o, d, v, z, r = _rays(mip, n, s, seed=n)
         enc, dens, g = _grad(mlp, o, d, v, z, r)
         raw = nerf_mlp_forward_tiles(image, bias, enc, n * s, mlp.input_ch, mlp.input_ch_dirs)
-        assert torch.equal(_bits(dens), _bits(raw[:, 3].contiguous())), (n, s)
+        assert torch.equal(bits(dens), bits(raw[:, 3].contiguous())), (n, s)
         assert torch.isfinite(g).all()
     o, d, v, z, r = _rays(mip, 533, 37, seed=9)
     _, d_all, g_all = _grad(mlp, o, d, v, z, r)
     for lo, hi in ((0, 200), (200, 533)):
         _, dp, gp = _grad(mlp, o[lo:hi], d[lo:hi], v[lo:hi], z[lo:hi], None if r is None else r[lo:hi])
-        assert torch.equal(_bits(dp), _bits(d_all[lo * 37:hi * 37])) and torch.equal(_bits(gp), _bits(g_all[lo * 37:hi * 37]))
+        assert torch.equal(bits(dp), bits(d_all[lo * 37:hi * 37])) and torch.equal(bits(gp), bits(g_all[lo * 37:hi * 37]))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('mip,scale', CASES, ids=IDS)
 def test_gradient_against_float64(mip, scale):
-    net = _net(mip, seed=2, scale=scale)
+    net = nerf_net(mip, seed=2, scale=scale)
     mlp = net.mlp
     n, s = 40, 64
     o, d, v, z, r = _rays(mip, n, s, seed=3)
@@ -211,7 +188,7 @@ def test_agrees_with_the_training_kernel_gradient(mip):
     fp16 through the same eight layers with tensor-core sums, so each is within this file's float64 bound of the restatement; they must agree within
     twice it (the training path's fixed 2^12 staging scale adds its subnormal term, negligible at these magnitudes)"""
     from xrnerf_b200 import nerf_train
-    net = _net(mip, seed=4)
+    net = nerf_net(mip, seed=4)
     mlp = net.mlp
     n, s = 64, 2
     o, d, v, z, r = _rays(mip, n, s, seed=5, d_zero=True)
@@ -229,7 +206,7 @@ def test_agrees_with_the_training_kernel_gradient(mip):
 @pytest.mark.parametrize('mip', [False, True])
 def test_normals_change_nothing_else(mip):
     from xrnerf_b200.nerf import MipNerfRenderer, NerfRenderer
-    net = _net(mip, seed=6)
+    net = nerf_net(mip, seed=6)
     o, d, v, z, r = _rays(mip, 700, 64, seed=7)
     R = MipNerfRenderer(net, ray_batch=256) if mip else NerfRenderer(net, ray_batch=256)
     args = (o, d, v, r) if mip else (o, d, v)
@@ -237,7 +214,7 @@ def test_normals_change_nothing_else(mip):
     b = R.render(*args, z_vals=z, depth=True, normals=True)
     assert set(b) == set(a) | {'normal'} and b['normal'].shape == (700, 3)
     for k in a:
-        assert torch.equal(_bits(a[k]), _bits(b[k])), k
+        assert torch.equal(bits(a[k]), bits(b[k])), k
     assert torch.isfinite(b['normal']).all()
 
 
@@ -300,7 +277,7 @@ def _octant_rays(n, samples):
 def test_octahedron_normals_nerf():
     """samples near a face of the octahedron |x| + |y| + |z| = 0.5, away from its edges, in all 8 octants (so both relu(x_a) and relu(-x_a) units are
     live somewhere): n = -g / |g| is the face's outward normal (+-1, +-1, +-1)/sqrt(3) to 1e-3 rad, and it faces the camera (n . d < 0)"""
-    net = _net(False, seed=8)
+    net = nerf_net(False, seed=8)
     _octahedron(net, 0.5)
     o, d, sgn, z = _octant_rays(512, 64)
     _, g = net.mlp.density_grad_rays(o, d, z)
@@ -321,7 +298,7 @@ def test_octahedron_normals_mip():
     float64 at the frustum Gaussians' means and covariances and with the signs of the fp16 columns read back from the encoding image; every sample's
     normal is within 1e-3 rad of it, and where |mu_a| < 1 on all axes and the sample is near the level set it faces the camera."""
     from xrnerf_b200.nerf import encode_rays
-    net = _net(True, seed=9)
+    net = nerf_net(True, seed=9)
     _octahedron(net, 0.5)
     mlp = net.mlp
     o, d, sgn, z = _octant_rays(256, 65)
@@ -345,9 +322,9 @@ def test_octahedron_normals_mip():
 def test_network_api_and_whole_view():
     """val_step / test_step keys with render_normals on and off; a whole 800 x 800 NeRF view with normals; NotImplementedError without the fused path"""
     H, W = 24, 40
-    net = _net(False, seed=11)
-    o, d, v, _ = _view_rays(H, W, 5, radii=False)
-    z = _zvals(H * W, 64)
+    net = nerf_net(False, seed=11)
+    o, d, v, _ = view_rays(H, W, 5, radii=False)
+    z = zvals(H * W, 64)
     view = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': z, 'src_shape': torch.tensor([H, W, 3])}
     net.set_val_pipeline(lambda item: dict(view))
     images = torch.rand((1, 2, H, W, 3), device='cuda')
@@ -363,15 +340,15 @@ def test_network_api_and_whole_view():
     net.fused_inference = False
     with pytest.raises(NotImplementedError):
         net.batchify_forward(dict(view), is_test=True)
-    mip = _net(True, seed=12)
+    mip = nerf_net(True, seed=12)
     mip.render_normals = True
-    _, _, _, r = _view_rays(H, W, 6)
-    mview = dict(view, radii=r, z_vals=_zvals(H * W, 129))
+    _, _, _, r = view_rays(H, W, 6)
+    mview = dict(view, radii=r, z_vals=zvals(H * W, 129))
     mip.set_val_pipeline(lambda item: dict(mview))
     mo = mip.val_step({'poses': torch.zeros((1, 1, 4, 4)), 'images': images[:, :1]})
     assert mo['normals'][0].shape == (H, W, 3)
     # Mip-NeRF use_multiscale: evaluate_once returns the normal map as a fifth element, val_step as normals / normal
-    ms = _net(True, seed=13, use_multiscale=True)
+    ms = nerf_net(True, seed=13, use_multiscale=True)
     px = lambda t: t.reshape(1, H, W, -1)
     mdata = {'rays_o': px(o), 'rays_d': px(d), 'viewdirs': px(v), 'radii': px(r), 'z_vals': px(mview['z_vals']), 'image': images[:, 0], 'idx': torch.tensor([[4]])}
     assert len(ms.evaluate_once(dict(mdata))) == 4
@@ -384,11 +361,11 @@ def test_network_api_and_whole_view():
     t = ms.val_step(dict(mdata))
     assert set(t) == {'rgb', 'gt_img', 'disp', 'idx', 'normal'} and torch.equal(t['normal'], normal)
     # a whole 800 x 800 view
-    big = _net(False, seed=17)
+    big = nerf_net(False, seed=17)
     big.render_normals = True
     H = W = 800
-    o, d, v, _ = _view_rays(H, W, 8, radii=False)
-    bview = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': _zvals(H * W, 64, 2.0, 6.0, False), 'src_shape': torch.tensor([H, W, 3])}
+    o, d, v, _ = view_rays(H, W, 8, radii=False)
+    bview = {'rays_o': o, 'rays_d': d, 'viewdirs': v, 'z_vals': zvals(H * W, 64, 2.0, 6.0, False), 'src_shape': torch.tensor([H, W, 3])}
     big.set_val_pipeline(lambda item: dict(bview))
     from xrnerf_b200.nerf import bytes_per_ray, ray_batch_size
     image = torch.rand((1, 1, H, W, 3), device='cuda')
@@ -443,12 +420,9 @@ def _unslab64(buf, n):
 
 
 def _unslab(buf, n):
-    h = np.frombuffer(buf, np.float16).reshape(n // 8, 8, 8, 8)
-    rows = np.arange(n)
-    out = np.zeros((n, 64), np.float16)
-    for c in range(8):
-        out[:, 8 * c:8 * c + 8] = h[rows >> 3, rows & 7, c ^ (rows & 7)]
-    return out
+    """an [n x 64] fp16 slab with the tile images' 128-byte swizzle"""
+    from xrnerf_b200.nerf_train import Img
+    return decode(Img(torch.frombuffer(bytearray(buf), dtype=torch.uint8), n * 128, 0, 1), 1, rows=n).numpy()
 
 
 @pytest.mark.parametrize('mip', [False, True])

@@ -12,35 +12,10 @@ every batch size (measured worst cases 1.4e-2 / 4.4e-2); the two output heads, w
 import numpy as np
 import pytest
 import torch
+from cases import MIP_MLP, NERF_MLP
+from restate64 import emulated_fp16_forward
 
 pytestmark = pytest.mark.gpu
-
-NERF = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True, embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-MIP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-           embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
-
-
-def _ste_half(t):
-    """value rounded to fp16, gradient passed straight through: what storing an activation as fp16 does"""
-    return t + (t.half().float() - t).detach()
-
-
-def _emulated_fp16_forward(mlp, x):
-    """the reference's run_mlp (nerf_mlp.py:70-94) with the tensor-core path's operand precision: fp16 weights and fp16 layer inputs, fp32 accumulation and bias, so that a
-    comparison isolates the kernels (same ReLU pattern) from the precision choice"""
-    import torch.nn.functional as F
-    lin = lambda l, h: F.linear(h, _ste_half(l.weight), l.bias)
-    pts, views = torch.split(_ste_half(x), [mlp.input_ch, mlp.input_ch_dirs], dim=-1)
-    h = pts
-    for i, l in enumerate(mlp.pts_linears):
-        h = _ste_half(F.relu(lin(l, h)))
-        if i in mlp.skips:
-            h = torch.cat([pts, h], -1)
-    alpha = lin(mlp.alpha_linear, h)
-    h = torch.cat([_ste_half(lin(mlp.feature_linear, h)), views], -1)
-    h = _ste_half(F.relu(lin(mlp.views_linears[0], h)))
-    return torch.cat([lin(mlp.rgb_linear, h), alpha], -1)
-
 
 def _grads(mlp, raw, g):
     for p in mlp.parameters():
@@ -60,7 +35,7 @@ def _run(cfg, n, seed, tol_emu=2.5e-2, tol_32=6e-2):
     mlp.fused_train = False
     raw32 = mlp.batchify_run_mlp(x)                            # the reference arithmetic: nn.Linear under autograd, fp32
     ref32 = _grads(mlp, raw32, g)
-    raw16 = _emulated_fp16_forward(mlp, x)
+    raw16 = emulated_fp16_forward(mlp, x)
     ref16 = _grads(mlp, raw16, g)
     mlp.fused_train = True
     raw = mlp.batchify_run_mlp(x)
@@ -89,27 +64,27 @@ def _run(cfg, n, seed, tol_emu=2.5e-2, tol_32=6e-2):
 
 
 def test_nerf_mlp_train_single_tile_is_exact_to_rounding():
-    _run(NERF, 128, seed=128, tol_emu=2e-3)          # no flip at this seed: every tensor within 8e-4 of the emulated path
+    _run(NERF_MLP, 128, seed=128, tol_emu=2e-3)          # no flip at this seed: every tensor within 8e-4 of the emulated path
 
 
 @pytest.mark.parametrize('n', [129, 300])
 def test_nerf_mlp_train_ragged_tiles(n):
-    _run(NERF, n, seed=n)
+    _run(NERF_MLP, n, seed=n)
 
 
 def test_nerf_mlp_train_many_tiles_per_cta():
-    _run(NERF, 40000, seed=40000, tol_emu=2e-2, tol_32=6e-2)      # 313 tiles: several tiles per CTA, the slab ring and the weight-gradient stage ring wrap
+    _run(NERF_MLP, 40000, seed=40000, tol_emu=2e-2, tol_32=6e-2)      # 313 tiles: several tiles per CTA, the slab ring and the weight-gradient stage ring wrap
 
 
 def test_mip_nerf_mlp_train_matches_autograd():
-    _run(MIP, 5000, seed=3)
+    _run(MIP_MLP, 5000, seed=3)
 
 
 def test_nerf_network_train_step_uses_tensor_core_path_and_learns():
     """NerfNetwork.train_step (networks/nerf.py:71-92) end to end: loss finite, gradients on every parameter, a few Adam steps reduce the loss"""
     from xrnerf_b200 import registry as R
     torch.manual_seed(0)
-    net = R.build_network(dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF, mlp_fine=NERF,
+    net = R.build_network(dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF_MLP, mlp_fine=NERF_MLP,
                                render=dict(type='NerfRender', white_bkgd=True, raw_noise_std=0))).cuda()
     opt = torch.optim.Adam(net.parameters(), lr=5e-4)
     n = 512

@@ -1,7 +1,7 @@
 """The NerfMLP training kernels (csrc/nerf_train.cu: xrb_nerf_tg_layer, xrb_nerf_tg_dw, xrb_nerf_tg_pack_weights, xrb_nerf_tg_pack_draw) one launch
 at a time, and NerfMlpTrainFn's whole chain, against float64 restatements of the same operations, entry by entry.
 
-Tile images are read and written by this file's own encoder / decoder, which implements the documented layout (csrc/tc.cuh, nerf_mlp._slab):
+Tile images are read and written by restate64's encoder / decoder, which implements the documented layout (csrc/tc.cuh, nerf_mlp._slab):
 fp16 element (r, k) of a [128 x 64] block sits at byte (r >> 3) 1024 + (r & 7) 128 + (((k >> 3) ^ (r & 7)) << 4) + (k & 7) 2, and a weight slab
 [n_pad x 64] uses the same formula with n_pad rows. Every reference starts from the kernel's own fp16 operands (the images handed to a launch, or
 decoded from what the previous launch wrote), so its inputs are exact and no ReLU decision can differ.
@@ -55,58 +55,12 @@ import time
 import numpy as np
 import pytest
 import torch
+from cases import MIP_MLP, NERF_MLP, host_buffer
+from restate64 import BLOCK, GAMMA_TC, U16, decode, encode, f16, image, swz, ulp16, w16
 
-U16 = 2.0 ** -11            # fp16 unit roundoff
 SCALE = 16384.0             # xrb_nerf_tg_grad_scale(): the staging scale of a tg_dw launch without a device scale
-GAMMA_TC = 2.0 ** -22       # per-product bound of fp32 accumulation on the tensor cores
-BLOCK = 16384
 REPORT = []
-
-NERF = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True, embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-MIP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-           embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
-MODELS = {'nerf': NERF, 'mip': MIP}
-
-
-# ----------------------------------------------------------------------------------------------------------------------------- tile images
-def _swz(rows):
-    """fp16 index of element (r, k) of a [rows x 64] block or slab, from the documented formula"""
-    r, k = np.meshgrid(np.arange(rows), np.arange(64), indexing='ij')
-    return (((r >> 3) * 1024 + (r & 7) * 128 + (((k >> 3) ^ (r & 7)) << 4) + (k & 7) * 2) // 2).reshape(-1)
-
-
-def decode(img, n_tiles, rows=128):
-    """an Img (or a raw slab arena with rows = n_pad) -> fp16 [n_tiles * rows, n_blk * 64] (torch, on the image's device)"""
-    buf, stride, off, nb = img.buf, img.tile_stride // 2, img.blk_off // 2, img.n_blk
-    h = buf.view(torch.float16)[:n_tiles * stride].reshape(n_tiles, stride)[:, off:off + nb * rows * 64].reshape(n_tiles, nb, rows * 64)
-    idx = torch.as_tensor(_swz(rows), device=buf.device)
-    return h[:, :, idx].reshape(n_tiles, nb, rows, 64).permute(0, 2, 1, 3).reshape(n_tiles * rows, nb * 64)
-
-
-def encode(m16):
-    """fp16 [n_tiles * 128, n_blk * 64] -> tile image bytes (the inverse of decode)"""
-    R, Cc = m16.shape
-    nt, nb = R // 128, Cc // 64
-    blocks = m16.reshape(nt, 128, nb, 64).permute(0, 2, 1, 3).reshape(nt, nb, 8192)
-    out = torch.empty_like(blocks)
-    out[:, :, torch.as_tensor(_swz(128), device=m16.device)] = blocks
-    return out.reshape(-1).view(torch.uint8)
-
-
-def image(m16):
-    from xrnerf_b200.nerf_train import Img
-    nb = m16.shape[1] // 64
-    return Img(encode(m16), nb * BLOCK, 0, nb)
-
-
-def _f16(t):
-    """float64 tensor rounded to fp16 once (numpy's conversion is a single RNE rounding) and back"""
-    return torch.from_numpy(t.detach().cpu().numpy().astype(np.float16).astype(np.float64)).to(t.device)
-
-
-def _ulp16(v):
-    _, e = torch.frexp(torch.clamp(v.abs(), min=2.0 ** -14))
-    return torch.ldexp(torch.ones_like(v), (e - 11).to(torch.int32))
+MODELS = {'nerf': NERF_MLP, 'mip': MIP_MLP}
 
 
 def within(got, ref, bound):
@@ -122,12 +76,12 @@ def within(got, ref, bound):
 def interval(y16, z, b, relu, mask=None):
     """(every fp16 output inside [fp16(act(z - b)), fp16(act(z + b))] (x mask), largest |y - act(z)| / (b + half an ulp))"""
     act = (lambda v: v.clamp_min(0.0)) if relu else (lambda v: v)
-    lo, hi, a = _f16(act(z - b)), _f16(act(z + b)), act(z)
+    lo, hi, a = f16(act(z - b)), f16(act(z + b)), act(z)
     if mask is not None:
         lo, hi, a = (torch.where(mask, v, torch.zeros_like(v)) for v in (lo, hi, a))
     y = y16.double()
     ok = bool(torch.isfinite(y).all() and ((y >= lo) & (y <= hi)).all())
-    ratio = float(((y - a).abs() / (b + 0.5 * _ulp16(a.abs() + b))).max()) if y.numel() else 0.0
+    ratio = float(((y - a).abs() / (b + 0.5 * ulp16(a.abs() + b))).max()) if y.numel() else 0.0
     return ok, ratio
 
 
@@ -175,11 +129,6 @@ def mlp_for(kind):
     return _MLPS[kind]
 
 
-def w16(lin):
-    """the fp16 weights the slabs hold (test_pack_weights_bit_exact), as float64"""
-    return torch.from_numpy(lin.weight.detach().cpu().numpy().astype(np.float16).astype(np.float64)).cuda()
-
-
 def b32(lin):
     return lin.bias.detach().double()
 
@@ -225,7 +174,7 @@ def test_pack_weights_bit_exact(kind):
         for kb, (col0, valid) in enumerate(L['blocks']):
             seen.add((N, W.shape[1], n_pad, col0, valid))
             off = L['off'] + kb * L['slab_bytes']
-            slab = S.arena[off:off + n_pad * 128].view(torch.float16).cpu().numpy()[_swz(n_pad)].reshape(n_pad, 64)
+            slab = S.arena[off:off + n_pad * 128].view(torch.float16).cpu().numpy()[swz(n_pad)].reshape(n_pad, 64)
             want = np.zeros((n_pad, 64), np.float16)
             want[:N, :valid] = W[:, col0:col0 + valid].astype(np.float16)
             assert np.array_equal(slab.view(np.uint16), want.view(np.uint16)), (name, kb, col0, valid)
@@ -336,7 +285,7 @@ def run_layer_cases(kind, n, seed=1, bias_shift=None):
         z, b = fwd_ref(x64, lin, K)
         if bias_shift and bias_shift[0] == name:
             c = bias_shift[1]
-            z[:, c] += float(_ulp16(_f16(lin.bias.detach().double()[c:c + 1])))   # one ulp of the fp16 the bias rounds to
+            z[:, c] += float(ulp16(f16(lin.bias.detach().double()[c:c + 1])))   # one ulp of the fp16 the bias rounds to
         ok, r = interval(decode(y, O.nt)[:n, :lin.out_features], z, b, relu)
         out[f'fwd {name}'] = (ok, r)
 
@@ -690,14 +639,14 @@ def _blender_step(kind):
     o, d = _blender_rays(n, 1)
     tgt = torch.rand((1, n, 3), generator=torch.Generator().manual_seed(2)).cuda()
     if kind == 'nerf':
-        net = R.build_network(dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF,
-                                   mlp_fine=NERF, render=dict(type='NerfRender', white_bkgd=True, raw_noise_std=0))).cuda()
+        net = R.build_network(dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF_MLP,
+                                   mlp_fine=NERF_MLP, render=dict(type='NerfRender', white_bkgd=True, raw_noise_std=0))).cuda()
         t = torch.linspace(0., 1., 64, device='cuda')
         z = (2.0 * (1. - t) + 6.0 * t).expand(n, 64).contiguous()
         data = {'rays_o': o[None], 'rays_d': d[None], 'viewdirs': d[None], 'z_vals': z[None], 'pts': (o[:, None, :] + d[:, None, :] * z[:, :, None])[None], 'target_s': tgt}
     else:
         net = R.build_network(dict(type='MipNerfNetwork', cfg=dict(phase='train', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1,
-                                                                   num_levels=2, chunk=1024 * 32, bs_data='rays_o'), mlp=MIP,
+                                                                   num_levels=2, chunk=1024 * 32, bs_data='rays_o'), mlp=MIP_MLP,
                                    render=dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=0.001, density_bias=-1, density_activation='softplus'))).cuda()
         t = torch.linspace(0., 1., 129, device='cuda')
         z = (2.0 * (1. - t) + 6.0 * t).expand(n, 129).contiguous()
@@ -777,11 +726,6 @@ def _lib():
     return _C.lib
 
 
-def _host(nbytes=1 << 16):
-    buf = (C.c_char * (nbytes + 256))()
-    return buf, (C.addressof(buf) + 255) & ~255
-
-
 def _good_layer(a):
     """a descriptor that passes every check (forward pts1: 4 A blocks, 4 slabs of 256 x 64); never launched here"""
     from xrnerf_b200.nerf_train import TgLayer
@@ -799,7 +743,7 @@ def _good_layer(a):
 def test_tg_layer_argument_validation_without_gpu():
     """every XRB_REQUIRE of xrb_nerf_tg_layer, each violated alone on a descriptor that otherwise passes"""
     lib = _lib()
-    _, a = _host()
+    _, a = host_buffer(1 << 16)
     assert lib.xrb_nerf_tg_layer(None, None) == -1 and b'null descriptor' in lib.xrb_last_error()
 
     def bad(msg, **kv):
@@ -850,7 +794,7 @@ def test_tg_dw_argument_validation_without_gpu():
     """every XRB_REQUIRE of xrb_nerf_tg_dw, including k_cols <= 64 x_n_blk (wider columns would never be written)"""
     from xrnerf_b200.nerf_train import TgDw
     lib = _lib()
-    _, a = _host()
+    _, a = host_buffer(1 << 16)
     assert lib.xrb_nerf_tg_dw(None, None) == -1 and b'null descriptor' in lib.xrb_last_error()
 
     def desc(**kv):
@@ -878,7 +822,7 @@ def test_tg_dw_argument_validation_without_gpu():
 def test_tg_pack_argument_validation_without_gpu():
     """every XRB_REQUIRE of xrb_nerf_tg_pack_weights and xrb_nerf_tg_pack_draw"""
     lib = _lib()
-    _, a = _host()
+    _, a = host_buffer(1 << 16)
     I = lambda *v: (C.c_int * len(v))(*v)
     w, s = C.c_void_p(a), C.c_void_p(a)
 

@@ -8,25 +8,12 @@ import ctypes as C
 import numpy as np
 import pytest
 import torch
+from cases import NGP_MODEL, cpu_args, dev
 
 BG = (0.1, 0.5, 0.9)
-NGP_MODEL = dict(   # configs/instant_ngp/nerf_blender_local01.py's model
-    type='HashNerfNetwork', cfg=dict(phase='train', chunk=4096, bs_data='rays_o'),
-    mlp=dict(type='HashNerfMLP', bound=1,
-             embedder_pos=dict(n_input_dims=3, encoding_config=dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=16, interpolation='Linear')),
-             embedder_dir=dict(n_input_dims=3, encoding_config=dict(otype='SphericalHarmonics', degree=4)),
-             density_net=dict(n_input_dims=32, n_output_dims=16, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=1)),
-             color_net=dict(n_output_dims=3, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=2))),
-    sampler=dict(type='NGPGridSampler', update_grid_freq=16, update_block_size=5000000, n_rays_per_batch=4096, cone_angle_constant=0.00390625, near_distance=0.2,
-                 target_batch_size=1 << 18, rgb_activation=2, density_activation=3),
-    render=dict(type='HashNerfRender', bg_color=[0, 0, 0]))
 # unwarp_dt (common.cuh): the fp32 constants of the march, evaluated in float64
 MIN_DT = float(np.float32(np.float32(1.73205080757) / np.float32(1024)))
 MAX_DT = MIN_DT * 128
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 @pytest.fixture(scope='module')
@@ -228,17 +215,9 @@ def test_hashnerf_network_returns_disparity(scene):
 
 # ------------------------------------------------------------------------------------------------ CPU
 
-def _cpu_args():
-    from xrnerf_b200 import _C
-    buf = (C.c_char * 4096)()
-    p = C.c_void_p((C.addressof(buf) + 255) & ~255)                     # 256-byte aligned host memory: never dereferenced by a rejected call
-    cfg = _C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 1, 2)
-    tab = _C.NgpTable(p.value, None, 0)
-    return _C, buf, p, cfg, tab
-
 
 def test_depth_entry_points_validate_arguments_without_gpu():
-    _C, _buf, p, cfg, tab = _cpu_args()
+    _C, _buf, p, cfg, tab = cpu_args()
     lib = _C.lib
     bg = _C.float3(BG)
     f = C.c_float

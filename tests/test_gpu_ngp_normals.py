@@ -17,32 +17,18 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_mesh_attributes import (U32, U64, Grid, face_points, gamma, kernel_density_grad, make_field, net_mats, position_grad, random_points, restated,
-                                      trilinear_grad_terms)
+from cases import NGP_MODEL, SPHERE_C, SPHERE_R, cpu_args, dev, face_points, load_ngp_weights, ngp_density_grad, ngp_field, random_points, sphere_network
+from restate64 import GAMMA_TC, U16, U32, U64, Grid, cuda_core_density_grad, field_mats, gamma, hashgrid_enc16, position_grad
 
 f32 = np.float32
-UH = 2.0 ** -11                      # fp16 unit roundoff
 SUB = 2.0 ** -25 / 1024              # fp16 staging: half the subnormal spacing, over the 2^10 staging scale
-GAMMA_TC = 2.0 ** -22                # per-term bound of a K-term fp32 accumulation on the tensor cores (as test_gpu_field_grad_exact)
 REPORT = []
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def enc16(field, x):
-    from xrnerf_b200 import _C
-    xt = dev(x.astype(f32))
-    enc = torch.empty((len(x), 32), dtype=torch.float16, device='cuda')
-    _C.check(_C.lib.xrb_tcnn_hashgrid_forward(field.cfg, field.tab, _C.ptr(xt), 3, len(x), _C.ptr(enc), _C.stream()), 'hashgrid_forward')
-    return enc.cpu().numpy().astype(np.float64)
 
 
 def tc_restated(field, grid, x):
     """float64 gradient, its bound and the rows whose masks are unambiguous, at x f32[n,3]"""
-    mats = net_mats(field)
-    a, ea = enc16(field, x), np.zeros((len(x), 32))           # layer input and its absolute error against the kernel's
+    mats = field_mats(field)
+    a, ea = hashgrid_enc16(field, x), np.zeros((len(x), 32))           # layer input and its absolute error against the kernel's
     masks, ok = [], np.ones(len(x), bool)
     for W in mats[:-1]:
         z = a @ W.T
@@ -64,7 +50,7 @@ def tc_restated(field, grid, x):
     ge, gea, ges = g @ mats[0], ga @ np.abs(mats[0]), gs @ np.abs(mats[0])
     pg, m = position_grad(grid, x, ge, gea)
     _, ms = position_grad(grid, x, ge, ges)
-    rel = (1 + UH) ** (dh - 1) * (1 + 64 * dh * GAMMA_TC) * (1 + gamma(27, U32)) - 1
+    rel = (1 + U16) ** (dh - 1) * (1 + 64 * dh * GAMMA_TC) * (1 + gamma(27, U32)) - 1
     return pg, (rel + gamma(64 * dh + 27, U64)) * m + (1 + rel) * ms, ok
 
 
@@ -79,8 +65,8 @@ CASES = [(dh, npk) for dh in (1, 2) for npk in (0, 6, 7)]
 @pytest.fixture(scope='module', params=CASES, ids=[f'dh{dh}-packed{npk}' for dh, npk in CASES])
 def case(request):
     dh, npk = request.param
-    f = make_field(dh, npk)
-    return f, Grid(f)
+    f = ngp_field(dh, npk)
+    return f, Grid.of(f)
 
 
 # ================================================================================================================ row stage
@@ -152,8 +138,8 @@ def test_agrees_with_cuda_core_kernel(case):
     field, grid = case
     x = random_points(2000, 61)
     _, g_tc, b_tc = _check(field, grid, x, 'tc')[2:]
-    _, g_cc = kernel_density_grad(field, x)
-    _, _, b_cc = restated(field, grid, x)
+    _, g_cc = ngp_density_grad(field, x)
+    _, _, b_cc = cuda_core_density_grad(field, grid, x)
     _, _, ok = tc_restated(field, grid, x)
     err = np.abs(g_tc - g_cc)[ok]
     assert (err <= (b_tc + b_cc)[ok]).all(), f'max err/bound {float((err / (b_tc + b_cc)[ok]).max()):.3g}'
@@ -163,11 +149,7 @@ def test_agrees_with_cuda_core_kernel(case):
 def _ngp_field():
     from xrnerf_b200 import synth
     from xrnerf_b200.ngp import NgpField
-    f = NgpField().cuda()
-    table, dens, color = synth.ngp_weights(seed=3, hash_range=0.5, mlp_gain=2.0)
-    with torch.no_grad():
-        f.hash_params.copy_(dev(table)); f.density_params.copy_(dev(dens)); f.color_params.copy_(dev(color))
-    return f
+    return load_ngp_weights(NgpField().cuda(), synth.ngp_weights(seed=3, hash_range=0.5, mlp_gain=2.0))
 
 
 def _workspace_rows(r, n, max_samples):
@@ -247,16 +229,15 @@ def test_render_normals_match_float64_composite(scene, n):
 
 @pytest.mark.gpu
 def test_sphere_normals_face_the_camera():
-    """The sphere field of test_gpu_mesh_attributes (raw = K (r - |x - c|) by trilinear interpolation of fp16 samples on level 4, K = 20 so that central
+    """The sphere field of cases.sphere_network (raw = K (r - |x - c|) by trilinear interpolation of fp16 samples on level 4, K = 20 so that central
     rays become opaque). At every pixel with alpha > 0.99: N . d < 0, and the angle between the normal and the float64 composite of the analytic radial
     directions at the same samples with the same weights is within the bound derived from the trilinear error: the interpolant's gradient differs from
     the exact one by at most 3 h / (rho - sqrt(3) h) (each edge difference quotient is the derivative at a point of the edge, within sqrt(3) h of the
     sample, and |Hessian| = 1 / rho) plus 2 sqrt(3) delta / h for the fp16 samples (delta = 2^-11 (|sdf| + sqrt(3) h), the corners' largest
     magnitude), so the unit normals differ by at most twice that;
     2^-8 more covers the kernel's own arithmetic, which the row tests bound far tighter."""
-    from test_gpu_mesh_attributes import SPHERE_C, SPHERE_R, _sphere_network
     from xrnerf_b200.ngp import NgpRenderer
-    net, grid = _sphere_network()
+    net, grid = sphere_network()
     f = net.mlp.field
     K = 20.0
     with torch.no_grad():
@@ -287,7 +268,7 @@ def test_sphere_normals_face_the_camera():
         rad = x - SPHERE_C
         rho = np.linalg.norm(rad, axis=1)
         radial = rad / rho[:, None]
-        delta = UH * (np.abs(SPHERE_R - rho) + math.sqrt(3) * h)
+        delta = U16 * (np.abs(SPHERE_R - rho) + math.sqrt(3) * h)
         E = 3 * h / np.maximum(rho - math.sqrt(3) * h, 1e-30) + 2 * math.sqrt(3) * delta / h
         e = np.where(rho > 2 * math.sqrt(3) * h, np.minimum(2.0, 2 * E + 2.0 ** -8), 2.0)
         want = (w[:, None] * radial).sum(0)
@@ -303,18 +284,6 @@ def test_sphere_normals_face_the_camera():
 
 
 # ================================================================================================================ network
-NGP_MODEL = dict(   # configs/instant_ngp/nerf_blender_local01.py's model
-    type='HashNerfNetwork', cfg=dict(phase='train', chunk=4096, bs_data='rays_o'),
-    mlp=dict(type='HashNerfMLP', bound=1,
-             embedder_pos=dict(n_input_dims=3, encoding_config=dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=16, interpolation='Linear')),
-             embedder_dir=dict(n_input_dims=3, encoding_config=dict(otype='SphericalHarmonics', degree=4)),
-             density_net=dict(n_input_dims=32, n_output_dims=16, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=1)),
-             color_net=dict(n_output_dims=3, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=2))),
-    sampler=dict(type='NGPGridSampler', update_grid_freq=16, update_block_size=5000000, n_rays_per_batch=4096, cone_angle_constant=0.00390625, near_distance=0.2,
-                 target_batch_size=1 << 18, rgb_activation=2, density_activation=3),
-    render=dict(type='HashNerfRender', bg_color=[0, 0, 0]))
-
-
 def _net(scene):
     from xrnerf_b200 import registry as R, synth
     torch.manual_seed(0)
@@ -377,21 +346,12 @@ def test_report():
 
 
 # ================================================================================================================ CPU
-def _cpu_args():
-    from xrnerf_b200 import _C
-    buf = (C.c_char * 4096)()
-    p = C.c_void_p((C.addressof(buf) + 255) & ~255)                     # 256-byte aligned host memory: never dereferenced by a rejected call
-    cfg = _C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 1, 2)
-    tab = _C.NgpTable(p.value, None, 0)
-    return _C, buf, p, cfg, tab
-
-
 BAD_CFGS = lambda _C: (_C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 5, 2), _C.NgpConfig(16, 2, 19, 16, 1.38191288, 64, 0, 2),
                        _C.NgpConfig(16, 2, 19, 16, 1.38191288, 32, 1, 2), _C.NgpConfig(8, 2, 19, 16, 1.38191288, 64, 1, 2))
 
 
 def test_density_grad_tc_validates_arguments_without_gpu():
-    _C, _buf, p, cfg, tab = _cpu_args()
+    _C, _buf, p, cfg, tab = cpu_args()
     lib = _C.lib
     call = lambda cfg=cfg, tab=tab, w=p, pts=p, stride=3, n=4, nd=None, order=None, dens=p, grad=p: lib.xrb_ngp_density_grad_tc(cfg, tab, w, pts, stride, n, nd, order, dens, grad, None)
     assert call(cfg=None) == -1 and b'null' in lib.xrb_last_error()
@@ -410,7 +370,7 @@ def test_density_grad_tc_validates_arguments_without_gpu():
 
 
 def test_render_normals_validates_arguments_without_gpu():
-    _C, _buf, p, cfg, tab = _cpu_args()
+    _C, _buf, p, cfg, tab = cpu_args()
     lib = _C.lib
     bg = (C.c_float * 3)(0, 0, 0)
 

@@ -4,19 +4,13 @@ Index path: bit-exact. Compositing (__expf + warp-scan association): |err| <= 2e
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
 
 
 def _bits(a):
     return np.ascontiguousarray(a).view(np.uint32)
-
-
-def dev(a, dt=None):
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    if dt is not None:
-        t = t.to(dt)
-    return t.cuda()
 
 
 @pytest.fixture(scope='module')

@@ -4,12 +4,9 @@ numsteps: bit-exact. rgb/alpha: 2e-3 abs (fp16 field, see test_gpu_field.py)."""
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 @pytest.fixture(scope='module')

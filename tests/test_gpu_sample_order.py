@@ -3,12 +3,9 @@ marched rows sorted by bucket, and the rendered pixels are bit-identical to the 
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 @pytest.fixture(scope='module')

@@ -4,12 +4,9 @@ Each is checked bit for bit where its arithmetic is one fp32 expression, and aga
 import numpy as np
 import pytest
 import torch
+from cases import dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 # ----------------------------------------------------------------------------------------------------------------------------- 5 x Huber

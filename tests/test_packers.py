@@ -2,14 +2,10 @@
 shared-memory descriptors assume, and the stream image sizes / bias vector layout of csrc/nerf_mlp_tc.cu. No GPU needed."""
 import numpy as np
 import torch
+from cases import MIP_MLP, NERF_MLP
 
 from xrnerf_b200 import nerf_mlp as nm
 from xrnerf_b200 import registry as R
-
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-MIP_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-               embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True))
 
 
 def test_swizzle_128b_slab_layout():

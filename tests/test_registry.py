@@ -4,26 +4,7 @@ forward/train steps."""
 import numpy as np
 import pytest
 import torch
-
-NGP_MODEL = dict(
-    type='HashNerfNetwork', cfg=dict(phase='train', chunk=4096, bs_data='rays_o'),
-    mlp=dict(type='HashNerfMLP', bound=1,
-             embedder_pos=dict(n_input_dims=3, encoding_config=dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=16, interpolation='Linear')),
-             embedder_dir=dict(n_input_dims=3, encoding_config=dict(otype='SphericalHarmonics', degree=4)),
-             density_net=dict(n_input_dims=32, n_output_dims=16, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=1)),
-             color_net=dict(n_output_dims=3, network_config=dict(otype='FullyFusedMLP', activation='ReLU', output_activation='None', n_neurons=64, num_layers=2))),
-    sampler=dict(type='NGPGridSampler', update_grid_freq=16, update_block_size=5000000, n_rays_per_batch=4096, cone_angle_constant=0.00390625, near_distance=0.2,
-                 target_batch_size=1 << 18, rgb_activation=2, density_activation=3),
-    render=dict(type='HashNerfRender', bg_color=[0, 0, 0]))
-
-NERF_MLP = dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, output_ch=5, use_viewdirs=True,
-                embedder=dict(type='BaseEmbedder', i_embed=0, multires=10, multires_dirs=4))
-NERF_MODEL = dict(type='NerfNetwork', cfg=dict(phase='train', N_importance=128, is_perturb=False, chunk=1024 * 32, bs_data='rays_o'), mlp=NERF_MLP, mlp_fine=NERF_MLP,
-                  render=dict(type='NerfRender', white_bkgd=True, raw_noise_std=0))
-MIP_MODEL = dict(type='MipNerfNetwork', cfg=dict(phase='train', ray_shape='cone', resample_padding=0.01, use_multiscale=False, coarse_loss_mult=0.1, num_levels=2, chunk=800, bs_data='rays_o'),
-                 mlp=dict(type='NerfMLP', skips=[4], netdepth=8, netwidth=256, netchunk=1024 * 32, use_viewdirs=True,
-                          embedder=dict(type='MipNerfEmbedder', min_deg_point=0, max_deg_point=16, min_deg_view=0, max_deg_view=4, use_viewdirs=True, append_identity=True)),
-                 render=dict(type='MipNerfRender', white_bkgd=True, raw_noise_std=0, rgb_padding=0.001, density_bias=-1, density_activation='softplus'))
+from cases import MIP_MODEL, NERF_MLP, NERF_MODEL, NGP_MODEL
 
 
 def test_registry_names_and_state_dict_keys():
