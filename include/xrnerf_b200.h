@@ -386,6 +386,50 @@ int xrb_nerf_composite_backward(const float *raw, const float *z_vals, const flo
                                 int n_samples, int mip, int white_bkgd, float rgb_padding, float density_bias, int density_act,
                                 float *d_raw, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Depth and opacity supervision (all three models; opt-in: the colour-only entry points above are unchanged)
+ *   depth   D = sum_k w_k t_k (NGP: t_k the sample's ray parameter, rebuilt from its row as in xrb_ngp_render_depth; NeRF: z_k; Mip-NeRF: the interval
+ *           mid-point (z_k + z_{k+1}) / 2), NOT divided by the opacity;
+ *   opacity A = sum_k w_k = 1 - T_N (NGP: `alpha`; NeRF / Mip-NeRF: `acc`).
+ * The backward entry points take dL/dD and dL/dA per ray (grad_depth, grad_alpha / grad_acc f32[n_rays]; either may be NULL: no such term) and add, in
+ * the density channel of sample k, dL/dD (T_k+ t_k - (D - D_<=k)) + dL/dA (T_k+ - (A - A_<=k)), T_k+ the transmittance behind sample k. The colour
+ * channels are those of the colour-only backward, bit for bit.
+ * NGP: the training composite's dL/draw carries the reference's loss_scale = 128 / n_rays and its l1 / l2 terms (calc_rgb.cu:92-104) on the colour AND
+ * the geometry terms, so the geometry weights of a loss are relative to the colour loss as that kernel scales it.
+ * ---------------------------------------------------------------------------------------------- */
+/* xrb_rm_calc_rgb_forward plus alpha_out f32[n_rays] = 1 - T and depth_out f32[n_rays] = D over the compacted rows of each ray, t_k rebuilt from the row with
+ * (rays_o, rays_d f32[n_rays,3], the march's aabb0 / aabb1). rgb is bit-identical to xrb_rm_calc_rgb_forward's; for a ray the compaction did not truncate
+ * (numsteps_compacted.count == numsteps.count) alpha and depth are bit-identical to xrb_ngp_render_depth's on the same rows. Null pointers or a raw that
+ * is not 16-byte aligned return XRB_E_BADARG before any CUDA call. */
+int xrb_rm_calc_rgb_forward_geom(const float *raw, const float *coords, const int32_t *numsteps, const int32_t *numsteps_compacted, const float *bg,
+                                 const float *rays_o, const float *rays_d, int n_rays, float aabb0, float aabb1, int rgb_act, int dens_act, float *rgb_out,
+                                 float *alpha_out, float *depth_out, void *stream);
+/* xrb_rm_calc_rgb_backward plus the geometry terms: depth / alpha are the forward's outputs (xrb_rm_calc_rgb_forward_geom), grad_depth / grad_alpha
+ * f32[n_rays] may be NULL. Every other pointer is required (XRB_E_BADARG before any CUDA call). */
+int xrb_rm_calc_rgb_backward_geom(const float *raw, const int32_t *numsteps_compacted, const float *coords, const float *grad_rgb, const float *rgb,
+                                  const float *grid_mean, const float *rays_o, const float *rays_d, float aabb0, float aabb1, const float *depth,
+                                  const float *alpha, const float *grad_depth, const float *grad_alpha, int n_rays, int rgb_act, int dens_act,
+                                  float *dl_draw, void *stream);
+/* xrb_nerf_composite_backward plus the geometry terms, for the depth xrb_nerf_composite_forward_depth writes and for acc: per sample the weight's
+ * gradient is G_k = grad_rgb . (c_k - wb) + grad_depth z_k + grad_acc (z_k the mid-point when mip). grad_depth / grad_acc f32[N] may be NULL; with both
+ * NULL, d_raw is bit-identical to xrb_nerf_composite_backward's. Arguments are checked as there. */
+int xrb_nerf_composite_backward_geom(const float *raw, const float *z_vals, const float *rays_d, const float *grad_rgb, const float *grad_depth,
+                                     const float *grad_acc, int n_rays, int n_samples, int mip, int white_bkgd, float rgb_padding, float density_bias,
+                                     int density_act, float *d_raw, void *stream);
+/* Depth / opacity loss and its gradient, one launch:
+ *   loss = depth_weight * sum |D - D*| / c_d + opacity_weight * sum (A - A*)^2 / c_a,   ADDED to *loss_accum (device float);
+ *   grad_depth = depth_weight sign(D - D*) / c_d (0 where D = D*), grad_alpha = 2 opacity_weight (A - A*) / c_a, and 0 on every ray a term drops.
+ * A ray drops out of both terms when numsteps_compacted.count != numsteps.count (NGP: the compaction truncated it; its D and A are partial sums, the
+ * test of xrb_ngp_count_trained_rays); numsteps / numsteps_compacted i32[n,2] may both be NULL (NeRF / Mip-NeRF: no ray drops). It drops out of the
+ * depth term where D* is not finite or D* <= 0 (no depth measured). mean == 0: c = 1 (reduction 'sum', as NGP's 5 x Huber); mean == 1: c = the number
+ * of rays the term keeps (as NeRF's MSE; a term that keeps no ray adds 0). depth, alpha, target_depth, target_alpha, grad_depth, grad_alpha f32[n].
+ * A term whose weight is 0 reads none of its inputs; a grad pointer that is given is always written. Returns XRB_E_BADARG, before any CUDA call, for
+ * n < 0, a weight that is negative or not finite, mean not 0 / 1, only one of numsteps / numsteps_compacted, a null loss_accum (n > 0), or a null
+ * input / output of a term whose weight is > 0. */
+int xrb_geom_loss_grad(const float *depth, const float *alpha, const float *target_depth, const float *target_alpha, const int32_t *numsteps,
+                       const int32_t *numsteps_compacted, int n_rays, float depth_weight, float opacity_weight, int mean, float *grad_depth,
+                       float *grad_alpha, float *loss_accum, void *stream);
+
 /* sample_pdf (hierarchical_sample.py:6-53), deterministic (`det`) or with caller-supplied uniforms u f32[N,n_importance].
  * z_vals f32[N,S], weights f32[N,S] -> z_out f32[N,S+n_importance] sorted, pts f32[N,S+n_importance,3] (may be NULL). */
 int xrb_nerf_sample_pdf(const float *z_vals, const float *weights, const float *rays_o, const float *rays_d, const float *u,
@@ -440,6 +484,12 @@ int xrb_nerf_get_rays(const float *c2w_host, int H, int W, float fx, float fy, f
 int xrb_ngp_batch_sample(const float *poses, const float *images_rgba, int n_images, int H, int W, float fx, float fy, float cx, float cy, const int64_t *row_idx, int64_t n,
                          const float *u_bg, uint64_t seed, int64_t n_prior_calls, float *rays_o, float *rays_d, float *target_s, float *alpha, float *img_ids, float *bg_color,
                          void *stream);
+/* Target depth of an NGP batch: depths f32[I,H,W] z-depth images (distance along the optical axis, the dataset's units), row_idx i64[n] as in
+ * xrb_ngp_batch_sample -> target_depth f32[n] = scale * z * |((i + 0.5 - cx) / fx, (j + 0.5 - cy) / fy, 1)|, the ray parameter of the pixel's unit-direction
+ * ray (scale: poses_nerf2ngp's 0.33). A z that is 0 or not finite stays so (the loss drops such rays). Bad sizes or null pointers return XRB_E_BADARG
+ * before any CUDA call. NeRF / Mip-NeRF need no conversion: GetRays directions have a unit camera-z component, so z-depth already is t. */
+int xrb_ngp_batch_depth(const float *depths, int n_images, int H, int W, float fx, float fy, float cx, float cy, float scale, const int64_t *row_idx, int64_t n,
+                        float *target_depth, void *stream);
 /* GetZvals (create.py:502-531, near/far constants) and, with u f32[n_rays, S] != NULL, PerturbZvals (augment.py:269-283) */
 int xrb_nerf_zvals(int64_t n_rays, int n_samples, float near_, float far_, int lindisp, const float *u, float *z_vals, void *stream);
 

@@ -62,6 +62,11 @@ _SIGS = {
     'xrb_rm_calc_rgb_forward': (_i, [P, P, P, P, P, _i, _i, _i, P, P]),
     'xrb_rm_calc_rgb_backward': (_i, [P, P, P, P, P, P, _i, _i, _i, P, P]),
     'xrb_rm_calc_rgb_inference': (_i, [P, P, P, C.POINTER(C.c_float), _i, _i, _i, P, P, P]),
+    'xrb_rm_calc_rgb_forward_geom': (_i, [P, P, P, P, P, P, P, _i, _f, _f, _i, _i, P, P, P, P]),
+    'xrb_rm_calc_rgb_backward_geom': (_i, [P, P, P, P, P, P, P, P, _f, _f, P, P, P, P, _i, _i, _i, P, P]),
+    'xrb_nerf_composite_backward_geom': (_i, [P, P, P, P, P, P, _i, _i, _i, _i, _f, _f, _i, P, P]),
+    'xrb_geom_loss_grad': (_i, [P, P, P, P, P, P, _i, _f, _f, _i, P, P, P, P]),
+    'xrb_ngp_batch_depth': (_i, [P, _i, _i, _i, _f, _f, _f, _f, _f, P, _i64, P, P]),
     'xrb_tcnn_hashgrid_num_params': (_i64, [_cfg]),
     'xrb_tcnn_density_num_params': (_i64, [_cfg]),
     'xrb_tcnn_color_num_params': (_i64, [_cfg]),

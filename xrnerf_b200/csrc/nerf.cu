@@ -33,12 +33,15 @@ __device__ __forceinline__ float transmittance(bool mip, bool valid, float sd, f
 }
 
 // BACKWARD == false: rgb/disp/acc/weights, plus depth_out = sum of w * z (interval mid-points when mip) when DEPTH.
-// BACKWARD == true: d_raw given grad_rgb (loss on rgb only, nerf.py:79-84 / mipnerf.py:49-57)
-template <bool BACKWARD, bool DEPTH = false>
+// BACKWARD == true: d_raw given grad_rgb (loss on rgb only, nerf.py:79-84 / mipnerf.py:49-57); GEOM: also given grad_depth and grad_acc (either may be
+// NULL), the gradients of the depth DEPTH writes and of acc, so that d L / d w_k = G_k = g . (c_k - wb) + g_d z_k + g_a
+template <bool BACKWARD, bool DEPTH = false, bool GEOM = false>
 __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, const float *__restrict__ raw, const float *__restrict__ z_vals, const float *__restrict__ rays_d,
                                                              const float *__restrict__ grad_rgb, float *__restrict__ rgb_out, float *__restrict__ disp_out, float *__restrict__ acc_out,
-                                                             float *__restrict__ weights_out, float *__restrict__ d_raw, float *__restrict__ depth_out) {
+                                                             float *__restrict__ weights_out, float *__restrict__ d_raw, float *__restrict__ depth_out,
+                                                             const float *__restrict__ grad_depth, const float *__restrict__ grad_acc) {
     static_assert(!(BACKWARD && DEPTH), "depth is a forward output");
+    static_assert(!GEOM || BACKWARD, "the geometry gradients are a backward input");
     const int lane = threadIdx.x & 31;
     const int ray = (blockIdx.x * 256 + threadIdx.x) >> 5;
     if (ray >= p.n_rays) return;
@@ -49,6 +52,9 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
     const float pad_mul = 1.f + 2.f * p.rgb_padding;
     float gx = 0, gy = 0, gz = 0;
     if (BACKWARD) { gx = grad_rgb[3 * (size_t)ray]; gy = grad_rgb[3 * (size_t)ray + 1]; gz = grad_rgb[3 * (size_t)ray + 2]; }
+    float gd = 0.f, ga = 0.f;
+    const bool geo = GEOM && (grad_depth || grad_acc);   // without either gradient, the colour-only arithmetic exactly
+    if (geo) { gd = grad_depth ? grad_depth[ray] : 0.f; ga = grad_acc ? grad_acc[ray] : 0.f; }
     // ---- pass 1: forward accumulation
     float carry = p.mip ? 0.f : 1.f;  // mip: running sum of sigma*delta; nerf: running product of (1-alpha+1e-10)
     float ax = 0, ay = 0, az = 0, acc = 0, depth = 0, total_wg = 0;
@@ -64,7 +70,9 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
             if (valid) { depth += w * (p.mip ? 0.5f * (z[k] + z[k + 1]) : z[k]); weights_out[(size_t)ray * S + k] = w; }
         } else {
             float wb = p.white_bkgd ? 1.f : 0.f;
-            total_wg += w * (gx * (cx - wb) + gy * (cy - wb) + gz * (cz - wb));
+            float G = gx * (cx - wb) + gy * (cy - wb) + gz * (cz - wb);
+            if (geo && valid) G += gd * (p.mip ? 0.5f * (z[k] + z[k + 1]) : z[k]) + ga;
+            total_wg += w * G;
         }
     }
     if (!BACKWARD) {
@@ -96,6 +104,7 @@ __global__ void __launch_bounds__(256) nerf_composite_kernel(CompositeParams p, 
         float cx = sx * pad_mul - p.rgb_padding, cy = sy * pad_mul - p.rgb_padding, cz = sz * pad_mul - p.rgb_padding;
         float wb = p.white_bkgd ? 1.f : 0.f;
         float G = gx * (cx - wb) + gy * (cy - wb) + gz * (cz - wb);
+        if (geo && valid) G += gd * (p.mip ? 0.5f * (z[k] + z[k + 1]) : z[k]) + ga;
         float inc_wg = warp_incl_sum(w * G, lane);
         float suffix = total_wg - (prefix_wg + inc_wg);
         prefix_wg += __shfl_sync(0xffffffffu, inc_wg, 31);
@@ -535,16 +544,24 @@ __device__ __forceinline__ void raygen_dir(const RayGenParams &p, float i, float
 //   the table shuffle (hashnerf_dataset.py:41-44) = the caller's row permutation; HashBatchSample (create.py:153-190) = a slice of it
 //   RandomBGColor (augment.py:290-313): bg = U[0,1)^3, target = rgb * alpha + bg * (1 - alpha) (float64 on the host, rounded to fp32)
 // without the 2.8 GB host table: one thread per ray regenerates its row from (pose, pixel) and blends the background.
+// pixel `row` of the virtual [I*H*W] table of an NGP batch: its image and its pixel in the image
+__device__ __forceinline__ void ngp_pixel(int64_t row, int64_t hw, int &img, int &pix) { img = (int)(row / hw); pix = (int)(row % hw); }
+// the camera-frame direction (x, y, 1) through the centre of pixel `pix` of a W-wide image (get_rays.py:35-69)
+__device__ __forceinline__ void ngp_pixel_dir(int pix, int W, float fx, float fy, float cx, float cy, float &x, float &y) {
+    const int j = pix / W, i = pix % W;
+    x = ((float)i + 0.5f - cx) / fx; y = ((float)j + 0.5f - cy) / fy;
+}
+
 __global__ void __launch_bounds__(256) ngp_batch_sample_kernel(const float *__restrict__ poses, const float *__restrict__ images, int n_img, int H, int W, float fx, float fy, float cx,
                                                                float cy, const int64_t *__restrict__ row_idx, int64_t n, const float *__restrict__ u_bg, Pcg32 rng,
                                                                float *__restrict__ rays_o, float *__restrict__ rays_d, float *__restrict__ target_s, float *__restrict__ alpha_out,
                                                                float *__restrict__ img_ids, float *__restrict__ bg_color) {
     const int64_t hw = (int64_t)H * W;
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row = row_idx[t];
-        const int img = (int)(row / hw), pix = (int)(row % hw), j = pix / W, i = pix % W;
+        int img, pix; float x, y;
+        ngp_pixel(row_idx[t], hw, img, pix);
         const float *P = poses + (size_t)img * 12;                 // [4,3]: rows 0..2 = rotation columns (c2w = P^T), row 3 = camera origin
-        const float x = ((float)i + 0.5f - cx) / fx, y = ((float)j + 0.5f - cy) / fy;
+        ngp_pixel_dir(pix, W, fx, fy, cx, cy, x, y);
         float d[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) d[c] = (x * P[c] + y * P[3 + c]) + P[6 + c];
@@ -563,6 +580,18 @@ __global__ void __launch_bounds__(256) ngp_batch_sample_kernel(const float *__re
         }
         alpha_out[t] = px.w;
         img_ids[t] = (float)img;
+    }
+}
+
+// target depth of an NGP batch: the z-depth of the pixel (along the optical axis) as the ray parameter of the unit-direction NGP ray, t = scale z |(x, y, 1)|
+__global__ void __launch_bounds__(256) ngp_batch_depth_kernel(const float *__restrict__ depths, int H, int W, float fx, float fy, float cx, float cy, float scale,
+                                                              const int64_t *__restrict__ row_idx, int64_t n, float *__restrict__ target_depth) {
+    const int64_t hw = (int64_t)H * W;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+        int img, pix; float x, y;
+        ngp_pixel(row_idx[t], hw, img, pix);
+        ngp_pixel_dir(pix, W, fx, fy, cx, cy, x, y);
+        target_depth[t] = scale * depths[(size_t)img * hw + pix] * sqrtf(x * x + y * y + 1.f);
     }
 }
 
@@ -622,7 +651,7 @@ int xrb_nerf_composite_forward(const float *raw, const float *z_vals, const floa
     XRB_REQUIRE(rgb && disp && acc && weights, "nerf_composite_forward: null output");
     CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
     int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
-    nerf_composite_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, nullptr);
+    nerf_composite_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, nullptr, nullptr, nullptr);
     return check_launch("nerf_composite_forward");
 }
 
@@ -633,7 +662,7 @@ int xrb_nerf_composite_forward_depth(const float *raw, const float *z_vals, cons
     XRB_REQUIRE(rgb && disp && acc && weights && depth, "nerf_composite_forward_depth: null output");
     CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
     int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
-    nerf_composite_kernel<false, true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, depth);
+    nerf_composite_kernel<false, true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, nullptr, rgb, disp, acc, weights, nullptr, depth, nullptr, nullptr);
     return check_launch("nerf_composite_forward_depth");
 }
 
@@ -644,8 +673,20 @@ int xrb_nerf_composite_backward(const float *raw, const float *z_vals, const flo
     XRB_REQUIRE(grad_rgb && d_raw && ((uintptr_t)d_raw & 15) == 0, "nerf_composite_backward: null/misaligned pointer");
     CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
     int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
-    nerf_composite_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, grad_rgb, nullptr, nullptr, nullptr, nullptr, d_raw, nullptr);
+    nerf_composite_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, grad_rgb, nullptr, nullptr, nullptr, nullptr, d_raw, nullptr, nullptr, nullptr);
     return check_launch("nerf_composite_backward");
+}
+
+int xrb_nerf_composite_backward_geom(const float *raw, const float *z_vals, const float *rays_d, const float *grad_rgb, const float *grad_depth, const float *grad_acc,
+                                     int n_rays, int n_samples, int mip, int white_bkgd, float rgb_padding, float density_bias, int density_act, float *d_raw, void *stream) {
+    int e = composite_args_ok(raw, z_vals, rays_d, n_rays, n_samples, density_act); if (e) return e;
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(grad_rgb && d_raw && ((uintptr_t)d_raw & 15) == 0, "nerf_composite_backward_geom: null/misaligned pointer");
+    CompositeParams p{n_rays, n_samples, mip, white_bkgd, density_act, rgb_padding, density_bias};
+    int blocks = (int)(((size_t)n_rays * 32 + 255) / 256);
+    nerf_composite_kernel<true, false, true><<<blocks, 256, 0, (cudaStream_t)stream>>>(p, raw, z_vals, rays_d, grad_rgb, nullptr, nullptr, nullptr, nullptr, d_raw, nullptr,
+                                                                                       grad_depth, grad_acc);
+    return check_launch("nerf_composite_backward_geom");
 }
 
 int xrb_nerf_sample_pdf(const float *z_vals, const float *weights, const float *rays_o, const float *rays_d, const float *u, int n_rays, int n_samples, int n_importance, float *z_out,
@@ -792,6 +833,15 @@ int xrb_ngp_batch_sample(const float *poses, const float *images_rgba, int n_ima
     ngp_batch_sample_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(poses, images_rgba, n_images, H, W, fx, fy, cx, cy, row_idx, n, u_bg, host_rng(seed, n_prior_calls), rays_o, rays_d,
                                                                           target_s, alpha, img_ids, bg_color);
     return check_launch("ngp_batch_sample");
+}
+
+int xrb_ngp_batch_depth(const float *depths, int n_images, int H, int W, float fx, float fy, float cx, float cy, float scale, const int64_t *row_idx, int64_t n,
+                        float *target_depth, void *stream) {
+    XRB_REQUIRE(n_images >= 1 && H >= 1 && W >= 1 && n >= 0, "ngp_batch_depth: bad arguments");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(depths && row_idx && target_depth, "ngp_batch_depth: null pointer");
+    ngp_batch_depth_kernel<<<stride_grid((n + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(depths, H, W, fx, fy, cx, cy, scale, row_idx, n, target_depth);
+    return check_launch("ngp_batch_depth");
 }
 
 int xrb_nerf_get_rays(const float *c2w_host, int H, int W, float fx, float fy, float cx, float cy, int convention, const int32_t *pixel_idx, int64_t n, float *rays_o, float *rays_d,

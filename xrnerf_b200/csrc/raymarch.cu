@@ -206,6 +206,7 @@ struct CompositeDepth {
 // MODE 1: inference (global bg, alpha out; calc_rgb.cu:143-206)
 // MODE 2: inference as MODE 1, plus depth = sum of w * t (include/xrnerf_b200.h, xrb_ngp_render_depth)
 // MODE 3: MODE 2, plus normal = sum of w * n, n = -g / |g| (0 where g = 0) of the row's gradient g (xrb_ngp_render_normals)
+// MODE 4: training forward as MODE 0, plus alpha = 1 - T and depth = sum of w * t as in MODE 2 (xrb_rm_calc_rgb_forward_geom)
 template <int MODE>
 __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const float4 *__restrict__ raw, const float *__restrict__ coords, const int32_t *__restrict__ numsteps,
                                                             const int32_t *__restrict__ numsteps_c, const float *__restrict__ bg, float3 bg_global, int rgb_act, int dens_act,
@@ -213,9 +214,9 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const fl
     int lane = threadIdx.x & 31;
     const uint32_t n_warps = (gridDim.x * 256) >> 5;
     for (uint32_t ray = (blockIdx.x * 256 + threadIdx.x) >> 5; ray < (uint32_t)n_rays; ray += n_warps) {
-    const int32_t *ns = MODE == 0 ? numsteps_c : numsteps;
+    const int32_t *ns = MODE == 0 || MODE == 4 ? numsteps_c : numsteps;
     uint32_t n = (uint32_t)ns[2 * (size_t)ray], base = (uint32_t)ns[2 * (size_t)ray + 1];
-    float3 b = MODE == 0 ? make_float3(bg[3 * (size_t)ray], bg[3 * (size_t)ray + 1], bg[3 * (size_t)ray + 2]) : bg_global;
+    float3 b = MODE == 0 || MODE == 4 ? make_float3(bg[3 * (size_t)ray], bg[3 * (size_t)ray + 1], bg[3 * (size_t)ray + 2]) : bg_global;
     if (n == 0) {
         if (lane == 0) {
             rgb_out[3 * (size_t)ray] = b.x; rgb_out[3 * (size_t)ray + 1] = b.y; rgb_out[3 * (size_t)ray + 2] = b.z;
@@ -255,7 +256,7 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(int n_rays, const fl
     if (MODE >= 2) ad = warp_sum(ad);
     if (MODE == 3) { nx = warp_sum(nx); ny = warp_sum(ny); nz = warp_sum(nz); }
     if (lane == 0) {
-        bool add_bg = MODE >= 1 ? true : (n == (uint32_t)numsteps[2 * (size_t)ray]);  // :61-64 / :199-202
+        bool add_bg = MODE >= 1 && MODE <= 3 ? true : (n == (uint32_t)numsteps[2 * (size_t)ray]);  // :61-64 / :199-202
         if (add_bg) { ax += T * b.x; ay += T * b.y; az += T * b.z; }
         rgb_out[3 * (size_t)ray] = ax; rgb_out[3 * (size_t)ray + 1] = ay; rgb_out[3 * (size_t)ray + 2] = az;
         if (MODE >= 1) alpha_out[ray] = 1.f - T;
@@ -279,10 +280,19 @@ int launch_composite_depth(const float *raw, const float *coords, const int32_t 
     return check_launch("ngp_render_depth composite");
 }
 
-// compute_rgbs_grad (calc_rgb.cu:70-140)
+// what the geometry backward (GEOM) reads beyond the colour gradient: the rays (t of each row, as row_t in MODE 2 / 4), the forward's depth and alpha,
+// and their gradients (either may be NULL: no such term)
+struct CompositeGeom {
+    const float *rays_o, *rays_d; float lo, diag;
+    const float *depth, *alpha, *grad_depth, *grad_alpha;
+};
+
+// compute_rgbs_grad (calc_rgb.cu:70-140). GEOM: the density channel also carries the depth and opacity terms,
+// d depth / d(sigma_k dt_k) = Ta t_k - (D - D_<=k) and d alpha / d(sigma_k dt_k) = Ta - (A - A_<=k), under the same loss_scale
+template <bool GEOM = false>
 __global__ void __launch_bounds__(256) composite_bwd_kernel(int n_rays, const float4 *__restrict__ raw, const float *__restrict__ coords, const int32_t *__restrict__ numsteps_c,
                                                             const float *__restrict__ grad_rgb, const float *__restrict__ rgb_final, const float *__restrict__ grid_mean,
-                                                            int rgb_act, int dens_act, float4 *__restrict__ dl_draw) {
+                                                            int rgb_act, int dens_act, float4 *__restrict__ dl_draw, CompositeGeom gm) {
     int lane = threadIdx.x & 31;
     const uint32_t n_warps = (gridDim.x * 256) >> 5;
     for (uint32_t ray = (blockIdx.x * 256 + threadIdx.x) >> 5; ray < (uint32_t)n_rays; ray += n_warps) {
@@ -293,29 +303,43 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(int n_rays, const fl
     const float l1 = __ldg(grid_mean) < NERF_MIN_OPTICAL_THICKNESS ? 1e-4f : 0.0f;    // :104
     float gx = grad_rgb[3 * (size_t)ray], gy = grad_rgb[3 * (size_t)ray + 1], gz = grad_rgb[3 * (size_t)ray + 2];
     float fx = rgb_final[3 * (size_t)ray], fy = rgb_final[3 * (size_t)ray + 1], fz = rgb_final[3 * (size_t)ray + 2];
-    float T = 1.f, px = 0.f, py = 0.f, pz = 0.f;  // running transmittance / prefix colour carried across 32-sample chunks
+    float gd = 0.f, ga = 0.f, fd = 0.f, fa = 0.f, ro[3] = {0.f, 0.f, 0.f}, d[3] = {0.f, 0.f, 0.f}, inv_dd = 1.f;
+    const bool geo = GEOM && (gm.grad_depth || gm.grad_alpha);   // without either gradient, the colour-only arithmetic exactly
+    if (geo) {
+        gd = gm.grad_depth ? gm.grad_depth[ray] : 0.f; ga = gm.grad_alpha ? gm.grad_alpha[ray] : 0.f;
+        fd = gm.depth[ray]; fa = gm.alpha[ray];
+        ro[0] = __ldg(gm.rays_o + 3 * (size_t)ray); ro[1] = __ldg(gm.rays_o + 3 * (size_t)ray + 1); ro[2] = __ldg(gm.rays_o + 3 * (size_t)ray + 2);
+        d[0] = __ldg(gm.rays_d + 3 * (size_t)ray); d[1] = __ldg(gm.rays_d + 3 * (size_t)ray + 1); d[2] = __ldg(gm.rays_d + 3 * (size_t)ray + 2);
+        inv_dd = 1.f / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    }
+    float T = 1.f, px = 0.f, py = 0.f, pz = 0.f, pd = 0.f, pa = 0.f;  // running transmittance / prefix colour (and depth, alpha) carried across 32-sample chunks
     for (uint32_t k0 = 0; k0 < n; k0 += 32) {
         uint32_t k = k0 + lane; bool valid = k < n;
-        float4 r = make_float4(0, 0, 0, 0); float dt = 0.f; CompositeTerm s{0.f, 0.f, 0.f, 0.f};
+        float4 r = make_float4(0, 0, 0, 0); float dt = 0.f, t = 0.f; CompositeTerm s{0.f, 0.f, 0.f, 0.f};
         if (valid) {
             r = __ldg(raw + base + k);
             dt = row_dt(coords + ROW_FLOATS * (size_t)(base + k));
             s = composite_term(r, dt, rgb_act, dens_act);
+            if (geo) t = row_t(coords + ROW_FLOATS * (size_t)(base + k), ro, d, inv_dd, gm.lo, gm.diag);
         }
         float incl, ex = warp_excl_prod(1.f - s.alpha, lane, &incl);
         float Tb = T * ex, w = s.alpha * Tb, Ta = Tb * (1.f - s.alpha);
         float sx = px + warp_incl_sum(w * s.r, lane), sy = py + warp_incl_sum(w * s.g, lane), sz = pz + warp_incl_sum(w * s.b, lane);  // rgb_ray2 after this sample
+        float sd = 0.f, sa = 0.f;
+        if (geo) { sd = pd + warp_incl_sum(w * t, lane); sa = pa + warp_incl_sum(w, lane); }     // depth and alpha after this sample
         if (valid) {
             float4 o;
             o.x = loss_scale * (w * gx * net_to_rgb_deriv(r.x, rgb_act) + fmaxf(0.0f, l2 * r.x));
             o.y = loss_scale * (w * gy * net_to_rgb_deriv(r.y, rgb_act) + fmaxf(0.0f, l2 * r.y));
             o.z = loss_scale * (w * gz * net_to_rgb_deriv(r.z, rgb_act) + fmaxf(0.0f, l2 * r.z));
             float dot = gx * (Ta * s.r - (fx - sx)) + (gy * (Ta * s.g - (fy - sy)) + gz * (Ta * s.b - (fz - sz)));
+            if (geo) dot += gd * (Ta * t - (fd - sd)) + ga * (Ta - (fa - sa));
             o.w = loss_scale * (net_to_density_deriv(r.w, dens_act) * (dt * dot)) + (r.w < 0.f ? -l1 : 0.0f);
             dl_draw[base + k] = o;
         }
         T *= __shfl_sync(0xffffffffu, incl, 31);
         px = __shfl_sync(0xffffffffu, sx, 31); py = __shfl_sync(0xffffffffu, sy, 31); pz = __shfl_sync(0xffffffffu, sz, 31);
+        if (geo) { pd = __shfl_sync(0xffffffffu, sd, 31); pa = __shfl_sync(0xffffffffu, sa, 31); }
     }
     }
 }
@@ -539,6 +563,32 @@ int xrb_rm_calc_rgb_forward(const float *raw, const float *coords, const int32_t
     return check_launch("calc_rgb_forward");
 }
 
+int xrb_rm_calc_rgb_forward_geom(const float *raw, const float *coords, const int32_t *numsteps, const int32_t *numsteps_compacted, const float *bg, const float *rays_o,
+                                 const float *rays_d, int n_rays, float aabb0, float aabb1, int rgb_act, int dens_act, float *rgb_out, float *alpha_out, float *depth_out,
+                                 void *stream) {
+    XRB_REQUIRE(n_rays >= 0, "calc_rgb_forward_geom: negative size");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(raw && coords && numsteps && numsteps_compacted && bg && rays_o && rays_d && rgb_out && alpha_out && depth_out, "calc_rgb_forward_geom: null pointer");
+    XRB_REQUIRE(((uintptr_t)raw & 15) == 0, "calc_rgb_forward_geom: raw must be 16-byte aligned");
+    const CompositeDepth dp{rays_o, rays_d, aabb0, aabb1 - aabb0, depth_out, nullptr, nullptr};
+    composite_fwd_kernel<4><<<warp_grid(n_rays), 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps, numsteps_compacted, bg, make_float3(0, 0, 0), rgb_act,
+                                                                                 dens_act, rgb_out, alpha_out, dp);
+    return check_launch("calc_rgb_forward_geom");
+}
+
+int xrb_rm_calc_rgb_backward_geom(const float *raw, const int32_t *numsteps_compacted, const float *coords, const float *grad_rgb, const float *rgb, const float *grid_mean,
+                                  const float *rays_o, const float *rays_d, float aabb0, float aabb1, const float *depth, const float *alpha, const float *grad_depth,
+                                  const float *grad_alpha, int n_rays, int rgb_act, int dens_act, float *dl_draw, void *stream) {
+    XRB_REQUIRE(n_rays >= 0, "calc_rgb_backward_geom: negative size");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(raw && coords && numsteps_compacted && grad_rgb && rgb && grid_mean && rays_o && rays_d && depth && alpha && dl_draw, "calc_rgb_backward_geom: null pointer");
+    XRB_REQUIRE(((uintptr_t)raw & 15) == 0 && ((uintptr_t)dl_draw & 15) == 0, "calc_rgb_backward_geom: raw/dl_draw must be 16-byte aligned");
+    const CompositeGeom gm{rays_o, rays_d, aabb0, aabb1 - aabb0, depth, alpha, grad_depth, grad_alpha};
+    composite_bwd_kernel<true><<<warp_grid(n_rays), 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps_compacted, grad_rgb, rgb, grid_mean, rgb_act,
+                                                                                    dens_act, (float4 *)dl_draw, gm);
+    return check_launch("calc_rgb_backward_geom");
+}
+
 int xrb_rm_calc_rgb_backward(const float *raw, const int32_t *numsteps_compacted, const float *coords, const float *grad_rgb, const float *rgb, const float *grid_mean,
                              int n_rays, int rgb_act, int dens_act, float *dl_draw, void *stream) {
     XRB_REQUIRE(n_rays >= 0, "calc_rgb_backward: negative size");
@@ -546,8 +596,8 @@ int xrb_rm_calc_rgb_backward(const float *raw, const int32_t *numsteps_compacted
     XRB_REQUIRE(raw && coords && numsteps_compacted && grad_rgb && rgb && grid_mean && dl_draw, "calc_rgb_backward: null pointer");
     XRB_REQUIRE(((uintptr_t)raw & 15) == 0 && ((uintptr_t)dl_draw & 15) == 0, "calc_rgb_backward: raw/dl_draw must be 16-byte aligned");
     int blocks = warp_grid(n_rays);
-    composite_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps_compacted, grad_rgb, rgb, grid_mean, rgb_act, dens_act,
-                                                                   (float4 *)dl_draw);
+    composite_bwd_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps_compacted, grad_rgb, rgb, grid_mean, rgb_act, dens_act,
+                                                                   (float4 *)dl_draw, CompositeGeom{});
     return check_launch("calc_rgb_backward");
 }
 

@@ -16,11 +16,17 @@ from . import _C
 
 
 class NgpRaySource:
-    def __init__(self, poses43, images_rgba, K, seed=0):
-        """poses43 [I,4,3] NGP xforms (poses_nerf2ngp, datasets/utils/hashnerf.py:4-23); images_rgba [I,H,W,4] float32; K 3x3 intrinsics."""
+    def __init__(self, poses43, images_rgba, K, seed=0, depths=None, depth_scale=0.33):
+        """poses43 [I,4,3] NGP xforms (poses_nerf2ngp, datasets/utils/hashnerf.py:4-23); images_rgba [I,H,W,4] float32; K 3x3 intrinsics.
+        depths [I,H,W] (optional): z-depth images, the distance along each camera's optical axis in the dataset's units (0 or not finite: no depth); batches
+        then also hold target_depth [n,1], the ray parameter of the NGP ray (xrb_ngp_batch_depth) with depth_scale the scale of poses_nerf2ngp."""
         self.poses = torch.as_tensor(poses43, dtype=torch.float32).contiguous()
         self.images = torch.as_tensor(images_rgba, dtype=torch.float32).contiguous()
         self.I, self.H, self.W = self.images.shape[:3]
+        self.depths = None if depths is None else torch.as_tensor(depths, dtype=torch.float32).contiguous()
+        if self.depths is not None and tuple(self.depths.shape) != (self.I, self.H, self.W):
+            raise ValueError(f'depths: expected shape {(self.I, self.H, self.W)}, got {tuple(self.depths.shape)}')
+        self.depth_scale = float(depth_scale)
         self.fx, self.fy, self.cx, self.cy = float(K[0][0]), float(K[1][1]), float(K[0][2]), float(K[1][2])
         self.n_rows = self.I * self.H * self.W
         self.perm = None
@@ -29,6 +35,8 @@ class NgpRaySource:
 
     def cuda(self, device=None):
         self.poses, self.images = self.poses.cuda(device), self.images.cuda(device)
+        if self.depths is not None:
+            self.depths = self.depths.cuda(device)
         if self.perm is not None:
             self.perm = self.perm.cuda(device)
         return self
@@ -63,6 +71,11 @@ class NgpRaySource:
                                              _C.ptr(u_bg), self.seed, self.calls, _C.ptr(out['rays_o']), _C.ptr(out['rays_d']), _C.ptr(out['target_s']), _C.ptr(out['alpha']),
                                              _C.ptr(out['img_ids']), _C.ptr(out['bg_color']), _C.stream()), 'ngp_batch_sample')
         self.calls += 1
+        if self.depths is not None:
+            _C.require_cuda(self.depths)
+            out['target_depth'] = f(1)
+            _C.check(_C.lib.xrb_ngp_batch_depth(_C.f32(self.depths), self.I, self.H, self.W, self.fx, self.fy, self.cx, self.cy, self.depth_scale, _C.ptr(row_idx, torch.int64), n,
+                                                _C.ptr(out['target_depth']), _C.stream()), 'ngp_batch_depth')
         return out
 
 
@@ -89,9 +102,10 @@ class NerfRaySource:
         self.fx, self.fy, self.cx, self.cy = float(K[0][0]), float(K[1][1]), float(K[0][2]), float(K[1][2])
         self.include_radius = include_radius
 
-    def batch(self, c2w, image_rgb, pixel_idx):
+    def batch(self, c2w, image_rgb, pixel_idx, depth=None, alpha=None):
         """c2w [3,4] or [4,4] camera-to-world (host or device), image_rgb [H,W,3] device tensor, pixel_idx int32[n] (select_rays_indices) ->
-        rays_o, rays_d, viewdirs, target_s (+ radii)"""
+        rays_o, rays_d, viewdirs, target_s (+ radii). depth [H,W] (z-depth; GetRays directions have a unit camera-z component, so it is the ray's z
+        already) and alpha [H,W] (optional, device) add target_depth / target_alpha [n,1] at the same pixels."""
         dev = image_rgb.device
         _C.require_cuda(image_rgb)
         pixel_idx = pixel_idx.to(device=dev, dtype=torch.int32).contiguous()
@@ -105,4 +119,8 @@ class NerfRaySource:
         out = dict(rays_o=o, rays_d=d, viewdirs=v, target_s=image_rgb.reshape(-1, image_rgb.shape[-1])[pixel_idx.long()])
         if r is not None:
             out['radii'] = r
+        for key, img in (('target_depth', depth), ('target_alpha', alpha)):
+            if img is not None:
+                _C.require_cuda(img)
+                out[key] = img.reshape(-1, 1).to(torch.float32)[pixel_idx.long()]
         return out

@@ -33,6 +33,47 @@ def merge_ret(ret, fine_ret):
     return out
 
 
+class _GeomLossFn(torch.autograd.Function):
+    """w_d * sum |D - D*| / c_d + w_a * sum (A - A*)^2 / c_a over the rays each term keeps (xrb_geom_loss_grad: depth only where D* is finite and > 0;
+    with numsteps, only the rays the compaction kept whole), c = 1 (mean=False) or the number of rays kept"""
+
+    @staticmethod
+    def forward(ctx, depth, alpha, target_depth, target_alpha, numsteps, numsteps_c, wd, wa, mean):
+        ref = depth if depth is not None else alpha
+        n = ref.numel()
+        vec = lambda t: None if t is None else t.detach().reshape(-1).contiguous().float()   # noqa: E731
+        loss = torch.zeros(1, dtype=torch.float32, device=ref.device)
+        gd = torch.zeros(n, dtype=torch.float32, device=ref.device) if depth is not None else None
+        ga = torch.zeros(n, dtype=torch.float32, device=ref.device) if alpha is not None else None
+        ts = [vec(t) for t in (depth, alpha, target_depth, target_alpha)]
+        _C.require_cuda(*ts)
+        _C.check(_C.lib.xrb_geom_loss_grad(*[_C.ptr(t) for t in ts], _C.ptr(numsteps), _C.ptr(numsteps_c), n, float(wd), float(wa), int(mean), _C.ptr(gd), _C.ptr(ga),
+                                           _C.ptr(loss), _C.stream()), 'geom_loss_grad')
+        ctx.save_for_backward(gd, ga)
+        ctx.shapes = (None if depth is None else depth.shape, None if alpha is None else alpha.shape)
+        return loss[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        gd, ga = ctx.saved_tensors
+        sd, sa = ctx.shapes
+        return (None if gd is None else (g * gd).reshape(sd), None if ga is None else (g * ga).reshape(sa), None, None, None, None, None, None, None)
+
+
+def geom_loss(ret, data, depth_weight, opacity_weight, prefix='', numsteps=None, mean=True, alpha_key='acc', target_alpha_key='target_alpha'):
+    """(depth term, opacity term) of one level (ret keys prefix + 'depth' / prefix + alpha_key), each None when its weight is 0 or its target is absent"""
+    ns, nsc = numsteps if numsteps is not None else (None, None)
+    out = []
+    for w, key, tkey in ((depth_weight, 'depth', 'target_depth'), (opacity_weight, alpha_key, target_alpha_key)):
+        if w > 0 and tkey in data:
+            d, a = (ret[prefix + key], None) if key == 'depth' else (None, ret[prefix + key])
+            out.append(_GeomLossFn.apply(d, a, data[tkey] if key == 'depth' else None, data[tkey] if key != 'depth' else None, ns, nsc,
+                                         w if key == 'depth' else 0.0, w if key != 'depth' else 0.0, mean))
+        else:
+            out.append(None)
+    return out
+
+
 def recover_shape(x, src_shape):
     return x.reshape([int(v) for v in src_shape[:2]] + [-1])
 
@@ -78,6 +119,8 @@ class NerfNetwork(nn.Module):
     def __init__(self, cfg, mlp=None, mlp_fine=None, render=None):
         super().__init__()
         self.phase = cfg.get('phase', 'train')
+        # depth / opacity supervision (opt-in): weights of L1 depth and squared opacity terms added to the colour loss when a batch holds the targets
+        self.depth_loss_weight, self.opacity_loss_weight = float(cfg.get('depth_loss_weight', 0.0)), float(cfg.get('opacity_loss_weight', 0.0))
         for k in ('chunk', 'bs_data', 'is_perturb', 'N_importance'):
             if k in cfg:
                 setattr(self, k, cfg[k])
@@ -136,15 +179,44 @@ class NerfNetwork(nn.Module):
                 all_ret.setdefault(k, []).append(v)
         return {k: torch.cat(v, 0) for k, v in all_ret.items()}
 
+    def _geometry_wanted(self, data, alpha_key='target_alpha'):
+        return (self.depth_loss_weight > 0 and 'target_depth' in data) or (self.opacity_loss_weight > 0 and alpha_key in data)
+
+    def _forward_geometry(self, data, geometry):
+        """forward() with the render's geometry_grad flag set for this call when the depth / opacity terms are wanted"""
+        if not geometry:
+            return self.forward(data, is_test=False)
+        flag = self.render.geometry_grad
+        self.render.geometry_grad = True
+        try:
+            return self.forward(data, is_test=False)
+        finally:
+            self.render.geometry_grad = flag
+
+    def _add_geometry(self, loss, log, ret, data, levels, **kw):
+        """adds the depth / opacity terms of every (prefix, multiplier) level to the loss; log_vars gain loss_depth / loss_opacity"""
+        per_level = [(m, geom_loss(ret, data, self.depth_loss_weight, self.opacity_loss_weight, prefix=p, **kw)) for p, m in levels]
+        for i, name in enumerate(('loss_depth', 'loss_opacity')):
+            terms = [t[i] if m == 1.0 else m * t[i] for m, t in per_level if t[i] is not None]
+            if terms:
+                term = sum(terms[1:], terms[0])
+                loss = loss + term
+                log[name] = term.item()
+        return loss
+
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
-        ret = self.forward(data, is_test=False)
+        geometry = self._geometry_wanted(data)
+        ret = self._forward_geometry(data, geometry)
         img_loss = img2mse(ret['rgb'], data['target_s'])
         psnr = mse2psnr(img_loss)
         loss = img_loss
         if 'coarse_rgb' in ret:
             loss = loss + img2mse(ret['coarse_rgb'], data['target_s'])
-        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'psnr': psnr.item()}, 'num_samples': ret['rgb'].shape[0]}
+        log = {}
+        if geometry:   # both levels, as the colour loss
+            loss = self._add_geometry(loss, log, ret, data, [('', 1.0)] + ([('coarse_', 1.0)] if 'coarse_rgb' in ret else []))
+        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'psnr': psnr.item(), **log}, 'num_samples': ret['rgb'].shape[0]}
 
     def _mark_dirty(self):
         for m in (getattr(self, 'mlp', None), getattr(self, 'mlp_fine', None)):
@@ -358,13 +430,18 @@ class MipNerfNetwork(NerfNetwork):
 
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
-        ret = self.forward(data, is_test=False)
+        geometry = self._geometry_wanted(data)
+        ret = self._forward_geometry(data, geometry)
         mask = torch.broadcast_to(data['lossmult'], ret['rgb'].shape) if 'lossmult' in data else torch.ones_like(ret['rgb'])
         loss_fine = (mask * (ret['rgb'] - data['target_s']) ** 2).sum() / mask.sum()
         loss_coarse = (mask * (ret['coarse_rgb'] - data['target_s']) ** 2).sum() / mask.sum()
         loss = loss_fine + self.coarse_loss_mult * loss_coarse
         psnr = mse2psnr(loss_fine)
-        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'loss_fine': loss_fine.item(), 'loss_coarse': loss_coarse.item(), 'psnr': psnr.item()}, 'num_samples': ret['rgb'].shape[0]}
+        log = {}
+        if geometry:   # the coarse level weighted like its colour loss
+            loss = self._add_geometry(loss, log, ret, data, [('', 1.0), ('coarse_', float(self.coarse_loss_mult))])
+        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'loss_fine': loss_fine.item(), 'loss_coarse': loss_coarse.item(), 'psnr': psnr.item(), **log},
+                'num_samples': ret['rgb'].shape[0]}
 
 
 @NETWORKS.register_module()
@@ -537,10 +614,16 @@ class HashNerfNetwork(NerfNetwork):
 
     def train_step(self, data, optimizer, **kwargs):
         data = {k: unfold_batching(v) for k, v in data.items()}
-        ret = self.forward(data, is_test=False)
+        geometry = self._geometry_wanted(data, alpha_key='alpha')
+        ret = self._forward_geometry(data, geometry)
         bs = ret['rgb'].shape[0]
         alpha = data['alpha'].detach()
         huber = HuberLoss(ret['rgb'], data['target_s'], 0.1, 'sum')
         psnr = mse2psnr(img2mse(ret['rgb'] * alpha, data['target_s'] * alpha))
         loss = huber * 5
-        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'psnr': psnr.item()}, 'num_samples': bs}
+        log = {}
+        if geometry:   # reduction 'sum' like the Huber term; rays the compaction truncated drop out (their depth and alpha are partial sums)
+            smp = self.sampler
+            loss = self._add_geometry(loss, log, ret, data, [('', 1.0)], numsteps=(smp.rays_numsteps, smp.rays_numsteps_compacted), mean=False, alpha_key='alpha',
+                                      target_alpha_key='alpha')
+        return {'loss': loss, 'log_vars': {'loss': loss.item(), 'psnr': psnr.item(), **log}, 'num_samples': bs}

@@ -204,7 +204,7 @@ class _Slot:
 class NgpTrainer:
     def __init__(self, field, bitfield, n_rays, target_batch_size=1 << 18, aabb=(0.0, 1.0), near=0.05, cone=1.0 / 256, rgb_act=2, dens_act=3,
                  lr=1e-2, betas=(0.9, 0.99), eps=1e-15, weight_decay=1e-6, samples_per_ray_budget=64, group=None, ema_momentum=None, ema_warm_up=100,
-                 grad_comm='auto', bwd_impl=None):
+                 grad_comm='auto', bwd_impl=None, depth_weight=0.0, opacity_weight=0.0):
         import torch.distributed as dist
         self.f, self.bitfield, self.n_rays, self.T = field, bitfield, n_rays, int(target_batch_size)
         self.aabb, self.near, self.cone, self.rgb_act, self.dens_act = aabb, near, cone, rgb_act, dens_act
@@ -270,6 +270,13 @@ class NgpTrainer:
         self.rgb = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
         self.grad_rgb = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
         self.loss_accum = torch.zeros(1, dtype=torch.float32, device=dev)
+        # depth / opacity supervision (step's target_depth / target_alpha): lambda_d sum |D - D*| + lambda_a sum (A - A*)^2 over the rays the compaction kept
+        # whole, added to the 5 x Huber colour loss; the gradient reaches the field through the same loss_scale as the colour's (include/xrnerf_b200.h)
+        self.depth_weight, self.opacity_weight = float(depth_weight), float(opacity_weight)
+        if not (self.depth_weight >= 0.0 and self.opacity_weight >= 0.0):
+            raise ValueError(f'depth_weight {depth_weight} / opacity_weight {opacity_weight}: must be >= 0')
+        if self.depth_weight > 0.0 or self.opacity_weight > 0.0:
+            self.alpha, self.depth, self.grad_alpha, self.grad_depth = (torch.zeros(n_rays, dtype=torch.float32, device=dev) for _ in range(4))
         self.grid_mean = torch.ones(1, dtype=torch.float32, device=dev)
         self.aux = torch.cuda.Stream(device=dev) if dev.type == 'cuda' else None
         self.trained_total = torch.zeros(1, dtype=torch.int64, device=dev)    # rays fully trained, summed over every batch prepared so far (device counter, no sync)
@@ -305,9 +312,11 @@ class NgpTrainer:
         s.rays = (rays_o, rays_d)                      # keep the tensors alive until the kernels ran
 
     # ------------------------------------------------------------------ one training step
-    def step(self, rays_o, rays_d, target, bg, next_rays=None):
+    def step(self, rays_o, rays_d, target, bg, next_rays=None, target_depth=None, target_alpha=None):
         """Trains on (rays_o, rays_d, target, bg). next_rays = (rays_o, rays_d) of the FOLLOWING call (optional): their march starts now, on the aux
-        stream, and overlaps this step's field kernels and gradient exchange. Returns the loss as a 0-dim device tensor (no sync)."""
+        stream, and overlaps this step's field kernels and gradient exchange. Returns the loss as a 0-dim device tensor (no sync).
+        target_depth / target_alpha f32[n] or [n,1]: the depth (ray parameter t, e.g. NgpRaySource's target_depth; not finite or <= 0: no depth) and
+        opacity each ray should render; used when depth_weight / opacity_weight > 0, and then the loss also holds their terms."""
         f = self.f
         s = self.slots[self.cur]
         if s.ready is None or s.rays is None or s.rays[0].data_ptr() != _ptr_of(rays_o):
@@ -319,13 +328,18 @@ class NgpTrainer:
         st = _C.stream()
         pts, dirs, n_rows_dev = s.coords_c[:, :3], s.coords_c[:, 4:], s.cnt_c[1:2]
         f.mlp_rows(pts, dirs, self.raw, n_rows_dev, self.fwd_impl)       # never refresh() here: the fp32 master outside this rank's slice is stale
-        _C.check(_C.lib.xrb_rm_calc_rgb_forward(_C.ptr(self.raw), _C.ptr(s.coords_c), _C.ptr(s.numsteps), _C.ptr(s.numsteps_c), _C.f32(bg), self.n_rays, self.rgb_act, self.dens_act,
-                                                _C.ptr(self.rgb), st), 'calc_rgb_forward')
-        self.loss_accum.zero_()
-        _C.check(_C.lib.xrb_ngp_huber5_grad(_C.ptr(self.rgb), _C.f32(target), self.n_rays * 3, 0.1, _C.ptr(self.grad_rgb), _C.ptr(self.loss_accum), st), 'huber5')
-        # rows of dL/draw beyond the compacted count are never read (n_rows_dev); rows owned by rays are all written by the kernel
-        _C.check(_C.lib.xrb_rm_calc_rgb_backward(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean), self.n_rays,
-                                                 self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward')
+        wd = self.depth_weight if target_depth is not None else 0.0
+        wa = self.opacity_weight if target_alpha is not None else 0.0
+        if wd > 0.0 or wa > 0.0:
+            self._composite_geom(s, bg, target, target_depth if wd > 0.0 else None, target_alpha if wa > 0.0 else None, wd, wa, st)
+        else:
+            _C.check(_C.lib.xrb_rm_calc_rgb_forward(_C.ptr(self.raw), _C.ptr(s.coords_c), _C.ptr(s.numsteps), _C.ptr(s.numsteps_c), _C.f32(bg), self.n_rays, self.rgb_act,
+                                                    self.dens_act, _C.ptr(self.rgb), st), 'calc_rgb_forward')
+            self.loss_accum.zero_()
+            _C.check(_C.lib.xrb_ngp_huber5_grad(_C.ptr(self.rgb), _C.f32(target), self.n_rays * 3, 0.1, _C.ptr(self.grad_rgb), _C.ptr(self.loss_accum), st), 'huber5')
+            # rows of dL/draw beyond the compacted count are never read (n_rows_dev); rows owned by rays are all written by the kernel
+            _C.check(_C.lib.xrb_rm_calc_rgb_backward(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean),
+                                                     self.n_rays, self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward')
         self.gflat.zero_()
         f.backward_rows(pts, dirs, self.draw, self.grads, n_rows_dev, self.bwd_impl)
         s.free = torch.cuda.Event(); s.free.record(main)
@@ -336,6 +350,23 @@ class NgpTrainer:
         f.shadows_updated()
         self.cur ^= 1
         return self.loss_accum[0]
+
+    def _composite_geom(self, s, bg, target, target_depth, target_alpha, wd, wa, st):
+        """composite forward with depth and alpha -> 5 x Huber -> depth / opacity loss (same loss_accum) -> composite backward with the geometry terms"""
+        rays_o, rays_d = s.rays
+        lo, hi = float(self.aabb[0]), float(self.aabb[1])
+        _C.check(_C.lib.xrb_rm_calc_rgb_forward_geom(_C.ptr(self.raw), _C.ptr(s.coords_c), _C.ptr(s.numsteps), _C.ptr(s.numsteps_c), _C.f32(bg), _C.ptr(rays_o), _C.ptr(rays_d),
+                                                     self.n_rays, lo, hi, self.rgb_act, self.dens_act, _C.ptr(self.rgb), _C.ptr(self.alpha), _C.ptr(self.depth), st),
+                 'calc_rgb_forward_geom')
+        self.loss_accum.zero_()
+        _C.check(_C.lib.xrb_ngp_huber5_grad(_C.ptr(self.rgb), _C.f32(target), self.n_rays * 3, 0.1, _C.ptr(self.grad_rgb), _C.ptr(self.loss_accum), st), 'huber5')
+        gd = self.grad_depth if wd > 0.0 else None
+        ga = self.grad_alpha if wa > 0.0 else None
+        _C.check(_C.lib.xrb_geom_loss_grad(_C.ptr(self.depth), _C.ptr(self.alpha), _ray_vec(target_depth, self.n_rays), _ray_vec(target_alpha, self.n_rays), _C.ptr(s.numsteps),
+                                           _C.ptr(s.numsteps_c), self.n_rays, wd, wa, 0, _C.ptr(gd), _C.ptr(ga), _C.ptr(self.loss_accum), st), 'geom_loss_grad')
+        _C.check(_C.lib.xrb_rm_calc_rgb_backward_geom(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean),
+                                                      _C.ptr(rays_o), _C.ptr(rays_d), lo, hi, _C.ptr(self.depth), _C.ptr(self.alpha), _C.ptr(gd), _C.ptr(ga), self.n_rays,
+                                                      self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward_geom')
 
     def _adam(self, p, p16, g, m, v, e, mom, div, bf16=False):
         fn = _C.lib.xrb_adam_ema_step_bf16grad if bf16 else _C.lib.xrb_adam_ema_step
@@ -433,6 +464,16 @@ class NgpTrainer:
         mine[:ex.end - ex.begin].copy_(self.ema[0])
         ex.all_gather(full, mine)
         return full[:ex.n]
+
+
+def _ray_vec(t, n):
+    """pointer of a per-ray f32 target ([n] or [n,1]); None -> NULL"""
+    if t is None:
+        return None
+    if t.numel() != n:
+        raise _C.XrbError(f'XRB_E_BADARG ({_C.XRB_E_BADARG}): expected {n} per-ray values, got shape {tuple(t.shape)}')
+    _C.require_cuda(t)
+    return _C.f32(t)
 
 
 def _ptr_of(t):
