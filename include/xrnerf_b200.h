@@ -494,6 +494,37 @@ int xrb_ngp_batch_depth(const float *depths, int n_images, int H, int W, float f
 int xrb_nerf_zvals(int64_t n_rays, int n_samples, float near_, float far_, int lindisp, const float *u, float *z_vals, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * NGP camera pose refinement (csrc/ngp_backward_tc.cu, csrc/raymarch.cu, csrc/nerf.cu; no reference counterpart: the reference trains on fixed poses)
+ * Poses are refined in the NGP frame, the xforms P [I,4,3] xrb_ngp_batch_sample takes (rows 0..2: the rotation's columns, row 3: the centre). Image i
+ * has a correction xi_i = (omega_i, rho_i) in R^6, initially 0; the corrected pose is R'_i = R_i Exp(omega_i) (a camera-frame rotation; Exp the Rodrigues
+ * map) and o'_i = o_i + rho_i, and its rays are xrb_ngp_batch_sample's: d = R' (x, y, 1) / |R' (x, y, 1)|, o = o'. Sample k of a ray is at the warped
+ * position x_k = (o + t_k d - lo) / diag with warped direction w = (d + 1) / 2, and each t_k is held fixed: the march's choice of samples and dt are not
+ * differentiated. The chain is field backward (dL/dx, dL/dw per row) -> per ray (dL/do, dL/dd) -> per image dL/dP'; the rotation's Exp and the update
+ * of xi (xrb_adam_ema_step) are the caller's (xrnerf_b200.data.NgpRaySource.pose_step).
+ * ---------------------------------------------------------------------------------------------- */
+/* xrb_ngp_mlp_backward_tc plus d_rows f32[n,6] <- (dL/dx, dL/dw) of every effective row in the units of dl_draw: dL/dx = sum over the 16 levels of
+ * xrb_ngp_density_grad_tc's position gradient applied to dL/d(encoding) (0 for a row outside [-0.5, 1.5]^3), dL/dw = the derivative of the SH
+ * encoding applied to dL/d(SH) (the colour net's input gradient before its fp16 staging scale is undone). The parameter gradients it accumulates are
+ * xrb_ngp_mlp_backward_tc's: same operands, same order. Same shapes, checks and return codes, and XRB_E_BADARG for a null d_rows (n > 0). */
+int xrb_ngp_mlp_backward_tc_inputs(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride,
+                                   const float *dirs, int dirs_stride, const float *dl_draw, int n, const int32_t *n_rows_dev, float *d_table,
+                                   float *d_density, float *d_color, float *d_rows, void *stream);
+/* Per ray: d_rows f32[rows,6] of the compacted rows coords f32[rows,7] (numsteps_compacted i32[n_rays,2] = (count, first row)), rays_o / rays_d f32[n_rays,3]
+ * as marched over the box [aabb0, aabb1]^3 (diag = aabb1 - aabb0) -> grad_o, grad_d f32[n_rays,3] (WRITTEN, 0 for a ray without compacted rows):
+ *   grad_o = scale sum_k dL/dx_k / diag,   grad_d = scale (sum_k t_k dL/dx_k / diag + 1/2 sum_k dL/dw_k),
+ * t_k rebuilt from the row as xrb_ngp_render_depth does; grad_d is with respect to the unit direction. One warp per ray. XRB_E_BADARG before any CUDA
+ * call for n_rays < 0, aabb1 <= aabb0 or a null pointer (n_rays > 0). */
+int xrb_ngp_ray_grad(const float *d_rows, const float *coords, const int32_t *numsteps_compacted, const float *rays_o, const float *rays_d, int n_rays,
+                     float aabb0, float aabb1, float scale, float *grad_o, float *grad_d, void *stream);
+/* Per image: the batch's rows row_idx i64[n] (as xrb_ngp_batch_sample), the corrected poses f32[I,4,3] the batch was generated from and grad_o / grad_d
+ * f32[n,3] -> dL/dP' ACCUMULATED into d_poses f32[I,4,3] (same layout as poses): the unit direction's gradient through the normalisation,
+ * dL/dd~ = (I - d^ d^T) grad_d / |d~|, then dL/dP'[r][c] += dL/dd~[c] (x, y, 1)[r] for r < 3 and dL/dP'[3][c] += grad_o[c]. Each block sums its rays first,
+ * in shared memory when I x 12 floats fit in 48 KB, otherwise per warp and image before a global atomic; any I works. Sizes and null pointers are checked
+ * before any CUDA call (XRB_E_BADARG); row_idx must address rows of the [I*H*W] table. */
+int xrb_ngp_pose_grad(const int64_t *row_idx, int64_t n, const float *poses, int n_images, int H, int W, float fx, float fy, float cx, float cy,
+                      const float *grad_o, const float *grad_d, float *d_poses, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * NerfMLP training on tensor cores (csrc/nerf_train.cu): what torch.autograd + cuBLAS do for the reference's NerfMLP (xrnerf/models/mlps/nerf_mlp.py:70-94,
  * trained by networks/nerf.py:71-92 / networks/mipnerf.py:45-74) as wgmma kernels over TILE IMAGES (per 128-row tile, C/64 blocks of [128 x 64] fp16 in the
  * K-major 128-byte-swizzle layout: the encoders' output format, xrb_nerf_enc_image_bytes). The host (xrnerf_b200/nerf_train.py) strings the layers together.

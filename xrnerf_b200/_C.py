@@ -86,6 +86,9 @@ _SIGS = {
     'xrb_ngp_density_grad': (_i, [_cfg, _tab, P, P, _i, _i, P, P, P]),
     'xrb_ngp_mlp_backward': (_i, [_cfg, _tab, P, P, P, _i, P, _i, P, _i, P, P, P, P]),
     'xrb_ngp_mlp_backward_tc': (_i, [_cfg, _tab, P, P, _i, P, _i, P, _i, P, P, P, P, P]),
+    'xrb_ngp_mlp_backward_tc_inputs': (_i, [_cfg, _tab, P, P, _i, P, _i, P, _i, P, P, P, P, P, P]),
+    'xrb_ngp_ray_grad': (_i, [P, P, P, P, P, _i, _f, _f, _f, P, P, P]),
+    'xrb_ngp_pose_grad': (_i, [P, _i64, P, _i, _i, _i, _f, _f, _f, _f, P, P, P, P]),
     'xrb_adam_ema_step': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P, _f, P]),
     'xrb_adam_ema_step_bf16grad': (_i, [P, P, P, P, P, _i64, _f, _f, _f, _f, _f, _i, _f, P, _f, P]),
     'xrb_pack_bf16': (_i, [P, P, _i64, P]),

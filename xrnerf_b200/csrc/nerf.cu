@@ -595,6 +595,75 @@ __global__ void __launch_bounds__(256) ngp_batch_depth_kernel(const float *__res
     }
 }
 
+// NGP camera pose refinement (xrb_ngp_pose_grad): dL/d(rays_o, unit rays_d) of each batch ray -> dL/dP' [I,4,3] of the corrected poses it was generated
+// from (ngp_batch_sample_kernel's ray generation, differentiated): d~ = R' (x, y, 1), dL/dd~ = (I - d^ d^T) grad_d / |d~|; row r < 3 of P' gets
+// dL/dd~ (x, y, 1)[r], row 3 gets grad_o. SHARED: each block sums into shared memory [I x 12] and adds its non-zero entries to the output; otherwise each
+// warp adds, per distinct image among its rays, one warp-reduced sum per entry with a global atomic.
+constexpr int POSE_GRAD_SMEM_MAX = 48 * 1024;
+template <bool SHARED>
+__global__ void __launch_bounds__(256) ngp_pose_grad_kernel(const int64_t *__restrict__ row_idx, int64_t n, int n_img, int H, int W, float fx, float fy, float cx, float cy,
+                                                            const float *__restrict__ poses, const float *__restrict__ grad_o, const float *__restrict__ grad_d,
+                                                            float *__restrict__ d_poses) {
+    extern __shared__ float s_acc[];
+    if (SHARED) {
+        for (int k = threadIdx.x; k < n_img * 12; k += blockDim.x) s_acc[k] = 0.f;
+        __syncthreads();
+    }
+    const int64_t hw = (int64_t)H * W;
+    const int lane = threadIdx.x & 31;
+    for (int64_t t0 = (int64_t)blockIdx.x * blockDim.x; t0 < n; t0 += (int64_t)gridDim.x * blockDim.x) {   // uniform per block: every lane takes part in the warp sums
+        const int64_t t = t0 + threadIdx.x;
+        const bool valid = t < n;
+        float v[12];
+        int img = -1;
+        if (valid) {
+            int pix; float x, y;
+            ngp_pixel(row_idx[t], hw, img, pix);
+            ngp_pixel_dir(pix, W, fx, fy, cx, cy, x, y);
+            const float *P = poses + (size_t)img * 12;
+            float d[3], g[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) { d[c] = (x * P[c] + y * P[3 + c]) + P[6 + c]; g[c] = grad_d[3 * t + c]; }
+            const float nrm = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), inv = 1.f / nrm;
+            const float u[3] = {d[0] * inv, d[1] * inv, d[2] * inv}, ug = u[0] * g[0] + u[1] * g[1] + u[2] * g[2];
+            const float in[3] = {x, y, 1.f};
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float gd = (g[c] - u[c] * ug) * inv;   // dL/dd~
+#pragma unroll
+                for (int r = 0; r < 3; ++r) v[3 * r + c] = gd * in[r];
+                v[9 + c] = grad_o[3 * t + c];
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 12; ++k) v[k] = 0.f;
+        }
+        if (SHARED) {
+            if (valid) {
+#pragma unroll
+                for (int k = 0; k < 12; ++k) atomicAdd(s_acc + 12 * img + k, v[k]);
+            }
+        } else {
+            unsigned pending = __ballot_sync(0xffffffffu, valid);
+            while (pending) {   // one round per distinct image among the warp's rays
+                const int leader = __ffs(pending) - 1, mine = __shfl_sync(0xffffffffu, img, leader);
+                const bool in_group = valid && img == mine;
+                pending &= ~__ballot_sync(0xffffffffu, in_group);
+#pragma unroll
+                for (int k = 0; k < 12; ++k) {
+                    const float sum = warp_sum(in_group ? v[k] : 0.f);
+                    if (lane == leader) atomicAdd(d_poses + 12 * (size_t)mine + k, sum);
+                }
+            }
+        }
+    }
+    if (SHARED) {
+        __syncthreads();
+        for (int k = threadIdx.x; k < n_img * 12; k += blockDim.x)
+            if (s_acc[k] != 0.f) atomicAdd(d_poses + k, s_acc[k]);
+    }
+}
+
 __global__ void __launch_bounds__(256) get_rays_kernel(RayGenParams p, const int32_t *__restrict__ pixel_idx, int64_t n, float *__restrict__ rays_o, float *__restrict__ rays_d,
                                                        float *__restrict__ viewdirs, float *__restrict__ radii) {
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
@@ -842,6 +911,20 @@ int xrb_ngp_batch_depth(const float *depths, int n_images, int H, int W, float f
     XRB_REQUIRE(depths && row_idx && target_depth, "ngp_batch_depth: null pointer");
     ngp_batch_depth_kernel<<<stride_grid((n + 255) / 256, 16), 256, 0, (cudaStream_t)stream>>>(depths, H, W, fx, fy, cx, cy, scale, row_idx, n, target_depth);
     return check_launch("ngp_batch_depth");
+}
+
+int xrb_ngp_pose_grad(const int64_t *row_idx, int64_t n, const float *poses, int n_images, int H, int W, float fx, float fy, float cx, float cy, const float *grad_o,
+                      const float *grad_d, float *d_poses, void *stream) {
+    XRB_REQUIRE(n_images >= 1 && H >= 1 && W >= 1 && n >= 0, "ngp_pose_grad: bad arguments");
+    if (n == 0) return XRB_OK;
+    XRB_REQUIRE(row_idx && poses && grad_o && grad_d && d_poses, "ngp_pose_grad: null pointer");
+    const int blocks = stride_grid((n + 255) / 256, 4);
+    const size_t smem = (size_t)n_images * 12 * sizeof(float);
+    if (smem <= (size_t)POSE_GRAD_SMEM_MAX)
+        ngp_pose_grad_kernel<true><<<blocks, 256, smem, (cudaStream_t)stream>>>(row_idx, n, n_images, H, W, fx, fy, cx, cy, poses, grad_o, grad_d, d_poses);
+    else
+        ngp_pose_grad_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(row_idx, n, n_images, H, W, fx, fy, cx, cy, poses, grad_o, grad_d, d_poses);
+    return check_launch("ngp_pose_grad");
 }
 
 int xrb_nerf_get_rays(const float *c2w_host, int H, int W, float fx, float fy, float cx, float cy, int convention, const int32_t *pixel_idx, int64_t n, float *rays_o, float *rays_d,

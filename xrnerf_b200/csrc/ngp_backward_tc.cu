@@ -17,6 +17,8 @@
 // At the end each warpgroup adds its dW accumulators to the fp32 gradient with atomics.
 // Shared memory: weight image + 2 x (ENC, H.., CIN, C.., dZ) tiles. Row-wise reads of accumulators (density outputs, dL/dcin, dL/dencoding) are
 // staged through a tile that is dead at that point (fp32 [128 x 16|32]).
+#include <cstdio>
+
 #include "tc_field.cuh"
 
 namespace xrb {
@@ -208,11 +210,14 @@ __host__ __device__ constexpr BtLayout bt_layout(int DH, int CH) {
 template <int DH, int CH>
 __host__ __device__ constexpr size_t bt_smem_bytes(uint32_t image_bytes) { return 1024 + image_bytes + 2 * (size_t)bt_layout(DH, CH).n_tiles * TILE_BLOCK_BYTES + 16; }
 
-template <int DH, int CH, int NP>
-__global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
-                                                                  uint32_t image_bytes, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride,
-                                                                  const float4 *__restrict__ dl_draw, int n, const int32_t *__restrict__ n_dev, float *__restrict__ d_table,
-                                                                  float *__restrict__ d_dens, float *__restrict__ d_color) {
+// The body of both field backward kernels. INPUTS (ngp_field_bwd_tc_inputs_kernel, xrb_ngp_mlp_backward_tc_inputs): also d_rows f32[n,6] = (dL/dx, dL/dw)
+// of each row: dL/dSH through sh4_grad right after the colour net's input round, dL/d(encoding) through position_grad_level inside the scatter loop. The
+// parameter gradients are those of ngp_field_bwd_tc_kernel: same operands, same order.
+template <int DH, int CH, int NP, bool INPUTS>
+__device__ __forceinline__ void ngp_field_bwd_tc(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
+                                                 uint32_t image_bytes, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride,
+                                                 const float4 *__restrict__ dl_draw, int n, const int32_t *__restrict__ n_dev, float *__restrict__ d_table,
+                                                 float *__restrict__ d_dens, float *__restrict__ d_color, float *__restrict__ d_rows) {
     extern __shared__ uint8_t dyn_smem[];
     if (n_dev) n = min(n, max(*n_dev, 0));
     constexpr BtLayout T = bt_layout(DH, CH);
@@ -278,6 +283,11 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
         {
             float gcin[32], gy[16];
             bt_bwd<32, 64, 1>(c, T.dz, T.cin, L.c_in, dw_cin, 0, T.cin, gcin);   // dL/dcin (scaled); CIN is dead after this round
+            if (INPUTS && valid) {   // dL/dw from dL/dSH = gcin[15..30]; written now, so it holds no registers through the density backward
+                const float3 gw = sh4_grad(dx, dy, dz, gcin + 15);
+                float *o = d_rows + 6 * (size_t)i;
+                o[3] = gw.x * (1.f / BT_SCALE); o[4] = gw.y * (1.f / BT_SCALE); o[5] = gw.z * (1.f / BT_SCALE);
+            }
             gy[0] = gr.w * BT_SCALE;                // dL/d density_out = (draw.w, dcin[0..14])   (hashnerf_mlp.py:69-78: raw[3] = density_out[0], colour input = density_out[1:])
 #pragma unroll
             for (int k = 0; k < 15; ++k) gy[k + 1] = gcin[k];
@@ -292,13 +302,18 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
         c.first = false;
         // ------------------------------------------------ hash-table gradient scatter
         if (valid) {
+            // as xrb_ngp_density_grad_tc: a row outside [-0.5, 1.5]^3 (or not finite) gets a zero position gradient without reading the table again
+            const bool inside = INPUTS && fabsf(px - 0.5f) <= 1.f && fabsf(py - 0.5f) <= 1.f && fabsf(pz - 0.5f) <= 1.f;
+            float3 gx = make_float3(0.f, 0.f, 0.f);
 #pragma unroll 1
             for (int l = 0; l < 16; ++l) {
                 float g0 = 0.f, g1 = 0.f;
 #pragma unroll
                 for (int q = 0; q < 16; ++q) if (q == l) { g0 = genc[2 * q]; g1 = genc[2 * q + 1]; }   // register array indexed by the rolled loop counter: select, never spill
                 scatter_level_paired(d_table, grid_cell(g, l, px, py, pz), (g.hashed_mask >> l) & 1u, g0 * (1.f / BT_SCALE), g1 * (1.f / BT_SCALE));
+                if (inside) position_grad_level(table, g, l, px, py, pz, g0 * (1.f / BT_SCALE), g1 * (1.f / BT_SCALE), gx);
             }
+            if (INPUTS) { float *o = d_rows + 6 * (size_t)i; o[0] = gx.x; o[1] = gx.y; o[2] = gx.z; }
         }
     }
     // ---------------------------------------------------- flush the weight-gradient accumulators (once per warpgroup)
@@ -316,15 +331,38 @@ __global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g,
 }
 
 template <int DH, int CH, int NP>
+__global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells, const void *__restrict__ weight_image,
+                                                                  uint32_t image_bytes, const float *__restrict__ pts, int pts_stride, const float *__restrict__ dirs, int dirs_stride,
+                                                                  const float4 *__restrict__ dl_draw, int n, const int32_t *__restrict__ n_dev, float *__restrict__ d_table,
+                                                                  float *__restrict__ d_dens, float *__restrict__ d_color) {
+    ngp_field_bwd_tc<DH, CH, NP, false>(g, table, cells, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_dev, d_table, d_dens, d_color, nullptr);
+}
+template <int DH, int CH, int NP>
+__global__ void __launch_bounds__(256, 1) ngp_field_bwd_tc_inputs_kernel(HashGridDev g, const __half2 *__restrict__ table, const uint8_t *__restrict__ cells,
+                                                                         const void *__restrict__ weight_image, uint32_t image_bytes, const float *__restrict__ pts, int pts_stride,
+                                                                         const float *__restrict__ dirs, int dirs_stride, const float4 *__restrict__ dl_draw, int n,
+                                                                         const int32_t *__restrict__ n_dev, float *__restrict__ d_table, float *__restrict__ d_dens,
+                                                                         float *__restrict__ d_color, float *__restrict__ d_rows) {
+    ngp_field_bwd_tc<DH, CH, NP, true>(g, table, cells, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_dev, d_table, d_dens, d_color, d_rows);
+}
+
+template <int DH, int CH, int NP, bool INPUTS>
 static int launch_bwd_tc(const HashGridDev &g, const xrb_ngp_table *tab, const void *image, uint32_t image_bytes, const float *pts, int pts_stride, const float *dirs, int dirs_stride,
-                         const float *dl_draw, int n, const int32_t *n_dev, float *d_table, float *d_dens, float *d_color, cudaStream_t s) {
-    auto k = ngp_field_bwd_tc_kernel<DH, CH, NP>;
+                         const float *dl_draw, int n, const int32_t *n_dev, float *d_table, float *d_dens, float *d_color, float *d_rows, cudaStream_t s) {
     const size_t smem = bt_smem_bytes<DH, CH>(image_bytes);
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const int n_tiles = (n + 127) / 128, grid = persistent_grid(1, (n_tiles + 1) / 2);   // one CTA per SM, two tiles (warpgroups) per CTA
-    k<<<grid, 256, smem, s>>>(g, (const __half2 *)tab->table_fp16, (const uint8_t *)tab->cell_image, image, image_bytes, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev,
-                              d_table, d_dens, d_color);
-    return check_launch("ngp_mlp_backward_tc");
+    const __half2 *table = (const __half2 *)tab->table_fp16;
+    const uint8_t *cells = (const uint8_t *)tab->cell_image;
+    if (INPUTS) {
+        auto k = ngp_field_bwd_tc_inputs_kernel<DH, CH, NP>;
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        k<<<grid, 256, smem, s>>>(g, table, cells, image, image_bytes, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev, d_table, d_dens, d_color, d_rows);
+    } else {
+        auto k = ngp_field_bwd_tc_kernel<DH, CH, NP>;
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        k<<<grid, 256, smem, s>>>(g, table, cells, image, image_bytes, pts, pts_stride, dirs, dirs_stride, (const float4 *)dl_draw, n, n_dev, d_table, d_dens, d_color);
+    }
+    return check_launch(INPUTS ? "ngp_mlp_backward_tc_inputs" : "ngp_mlp_backward_tc");
 }
 
 // ---------------------------------------------------------------------------- density and its position gradient on tensor cores (xrb_ngp_density_grad_tc)
@@ -422,30 +460,51 @@ int launch_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *tab, 
 
 using namespace xrb;
 
-extern "C" {
-
-int xrb_ngp_mlp_backward_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, const float *dirs, int dirs_stride,
-                            const float *dl_draw, int n, const int32_t *n_rows_dev, float *d_table, float *d_density, float *d_color, void *stream) {
+// both entry points of the field backward: d_rows == NULL launches the parameter-gradient kernel, otherwise its INPUTS variant (what names the errors)
+static int ngp_mlp_backward_tc(const char *what, const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride,
+                               const float *dirs, int dirs_stride, const float *dl_draw, int n, const int32_t *n_rows_dev, float *d_table, float *d_density, float *d_color,
+                               float *d_rows, void *stream) {
+    static char msg[256];
+    auto fail = [&](const char *m) { snprintf(msg, sizeof msg, "%s: %s", what, m); set_error(msg); return XRB_E_BADARG; };
     int e = check_cfg(cfg); if (e) return e;
-    XRB_REQUIRE(n >= 0 && pts_stride >= 3 && dirs_stride >= 3, "ngp_mlp_backward_tc: bad size");
+    if (!(n >= 0 && pts_stride >= 3 && dirs_stride >= 3)) return fail("bad size");
     if (n == 0) return XRB_OK;
-    XRB_REQUIRE(table && weight_image && pts && dirs && dl_draw && d_table && d_density && d_color, "ngp_mlp_backward_tc: null pointer");
-    XRB_REQUIRE(((uintptr_t)dl_draw & 15) == 0 && ((uintptr_t)d_table & 15) == 0 && ((uintptr_t)weight_image & 15) == 0, "ngp_mlp_backward_tc: dl_draw, d_table and the weight image must be 16-byte aligned");
+    if (!(table && weight_image && pts && dirs && dl_draw && d_table && d_density && d_color)) return fail("null pointer");
+    if (!(((uintptr_t)dl_draw & 15) == 0 && ((uintptr_t)d_table & 15) == 0 && ((uintptr_t)weight_image & 15) == 0))
+        return fail("dl_draw, d_table and the weight image must be 16-byte aligned");
     if (!((cfg->density_hidden == 1 && cfg->color_hidden == 1) || (cfg->density_hidden == 1 && cfg->color_hidden == 2))) {
-        set_error("ngp_mlp_backward_tc: tensor-core backward is built for (density_hidden, color_hidden) = (1,1) or (1,2); use xrb_ngp_mlp_backward");
+        snprintf(msg, sizeof msg, "%s: tensor-core backward is built for (density_hidden, color_hidden) = (1,1) or (1,2); use xrb_ngp_mlp_backward", what);
+        set_error(msg);
         return XRB_E_UNSUPPORTED;
     }
     HashGridDev g; e = table_setup(cfg, table, &g); if (e) return e;
     const uint32_t image_bytes = weight_image_layout(cfg->density_hidden, cfg->color_hidden).total;
     cudaStream_t s = (cudaStream_t)stream;
     const bool plan6 = plan_valid(g, table->n_packed_levels) && table->n_packed_levels == 6;
-#define XRB_BWT(DH, CH)                                                                                                                                          \
+#define XRB_BWT(DH, CH, IN)                                                                                                                                      \
     if (cfg->density_hidden == DH && cfg->color_hidden == CH)                                                                                                    \
-        return plan6 ? launch_bwd_tc<DH, CH, 6>(g, table, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color, s) \
-                     : launch_bwd_tc<DH, CH, 0>(g, table, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color, s);
-    XRB_BWT(1, 1) XRB_BWT(1, 2)
+        return plan6 ? launch_bwd_tc<DH, CH, 6, IN>(g, table, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color, d_rows, s) \
+                     : launch_bwd_tc<DH, CH, 0, IN>(g, table, weight_image, image_bytes, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color, d_rows, s);
+    if (d_rows) { XRB_BWT(1, 1, true) XRB_BWT(1, 2, true) }
+    else { XRB_BWT(1, 1, false) XRB_BWT(1, 2, false) }
 #undef XRB_BWT
     return XRB_E_UNSUPPORTED;
+}
+
+extern "C" {
+
+int xrb_ngp_mlp_backward_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, const float *dirs, int dirs_stride,
+                            const float *dl_draw, int n, const int32_t *n_rows_dev, float *d_table, float *d_density, float *d_color, void *stream) {
+    return ngp_mlp_backward_tc("ngp_mlp_backward_tc", cfg, table, weight_image, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color, nullptr,
+                               stream);
+}
+
+int xrb_ngp_mlp_backward_tc_inputs(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, const float *dirs,
+                                   int dirs_stride, const float *dl_draw, int n, const int32_t *n_rows_dev, float *d_table, float *d_density, float *d_color, float *d_rows,
+                                   void *stream) {
+    if (n > 0 && !d_rows) { set_error("ngp_mlp_backward_tc_inputs: null pointer (d_rows)"); return XRB_E_BADARG; }
+    return ngp_mlp_backward_tc("ngp_mlp_backward_tc_inputs", cfg, table, weight_image, pts, pts_stride, dirs, dirs_stride, dl_draw, n, n_rows_dev, d_table, d_density, d_color,
+                               d_rows, stream);
 }
 
 int xrb_ngp_density_grad_tc(const xrb_ngp_config *cfg, const xrb_ngp_table *table, const void *weight_image, const float *pts, int pts_stride, int n, const int32_t *n_rows_dev,

@@ -235,6 +235,20 @@ __device__ __forceinline__ void sh4(float dx01, float dy01, float dz01, float *o
     out[14] = 1.4453057213202769f * z * (x2 - y2);
     out[15] = 0.59004358992664352f * x * (-x2 + 3.0f * y2);
 }
+// Backward of sh4 with respect to its input: g[16] = dL/d(the 16 SH values) -> dL/d(dx01, dy01, dz01) = 2 sum_k g_k dSH_k/d(x, y, z), fp32
+__device__ __forceinline__ float3 sh4_grad(float dx01, float dy01, float dz01, const float *g) {
+    const float x = dx01 * 2.f - 1.f, y = dy01 * 2.f - 1.f, z = dz01 * 2.f - 1.f;
+    const float xy = x * y, xz = x * z, yz = y * z, x2 = x * x, y2 = y * y, z2 = z * z;
+    const float C1 = 0.48860251190291987f, C4 = 1.0925484305920792f, C6 = 0.94617469575755997f, C8 = 0.54627421529603959f, C9 = 0.59004358992664352f,
+                C10 = 2.8906114426405538f, C11 = 0.45704579946446572f, C12 = 0.3731763325901154f, C14 = 1.4453057213202769f;
+    float gx = -C1 * g[3] + C4 * y * g[4] - C4 * z * g[7] + 2.f * C8 * x * g[8] - 6.f * C9 * xy * g[9] + C10 * yz * g[10] + C11 * (1.f - 5.f * z2) * g[13]
+               + 2.f * C14 * xz * g[14] + 3.f * C9 * (y2 - x2) * g[15];
+    float gy = -C1 * g[1] + C4 * x * g[4] - C4 * z * g[5] - 2.f * C8 * y * g[8] + 3.f * C9 * (y2 - x2) * g[9] + C10 * xz * g[10] + C11 * (1.f - 5.f * z2) * g[11]
+               - 2.f * C14 * yz * g[14] + 6.f * C9 * xy * g[15];
+    float gz = C1 * g[2] - C4 * y * g[5] + 2.f * C6 * z * g[6] - C4 * x * g[7] + C10 * xy * g[10] - 10.f * C11 * yz * g[11] + C12 * (15.f * z2 - 3.f) * g[12]
+               - 10.f * C11 * xz * g[13] + C14 * (x2 - y2) * g[14];
+    return make_float3(2.f * gx, 2.f * gy, 2.f * gz);
+}
 
 // Backward of hash_level: adds the trilinear shares of (g0, g1) = dL/d(the level's two features) to the 8 corner entries of the fp32 table gradient.
 // The plain form: one red.global.add.v2.f32 per corner. The CUDA-core backward kernels use it; they are what the tests compare the paired form against.

@@ -344,6 +344,41 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(int n_rays, const fl
     }
 }
 
+// NGP camera pose refinement (xrb_ngp_ray_grad): per-row (dL/dx, dL/dw) of the field's INPUTS backward -> dL/do and dL/dd of each ray, t_k held fixed:
+//   dL/do = sum_k dL/dx_k / diag,  dL/dd = sum_k t_k dL/dx_k / diag + 1/2 sum_k dL/dw_k,  times `scale`; one warp per ray over its compacted rows
+__global__ void __launch_bounds__(256) ray_grad_kernel(int n_rays, const float *__restrict__ d_rows, const float *__restrict__ coords, const int32_t *__restrict__ numsteps_c,
+                                                       const float *__restrict__ rays_o, const float *__restrict__ rays_d, float lo, float diag, float scale,
+                                                       float *__restrict__ grad_o, float *__restrict__ grad_d) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t n_warps = (gridDim.x * 256) >> 5;
+    for (uint32_t ray = (blockIdx.x * 256 + threadIdx.x) >> 5; ray < (uint32_t)n_rays; ray += n_warps) {
+        const uint32_t n = (uint32_t)numsteps_c[2 * (size_t)ray], base = (uint32_t)numsteps_c[2 * (size_t)ray + 1];
+        float o[3], d[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { o[c] = __ldg(rays_o + 3 * (size_t)ray + c); d[c] = __ldg(rays_d + 3 * (size_t)ray + c); }
+        const float inv_dd = 1.f / (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+        float sx[3] = {0.f, 0.f, 0.f}, stx[3] = {0.f, 0.f, 0.f}, sw[3] = {0.f, 0.f, 0.f};
+        for (uint32_t k = lane; k < n; k += 32) {
+            const float *r = d_rows + 6 * (size_t)(base + k);
+            const float t = row_t(coords + ROW_FLOATS * (size_t)(base + k), o, d, inv_dd, lo, diag);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float gx = __ldg(r + c);
+                sx[c] += gx; stx[c] = fmaf(t, gx, stx[c]); sw[c] += __ldg(r + 3 + c);
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { sx[c] = warp_sum(sx[c]); stx[c] = warp_sum(stx[c]); sw[c] = warp_sum(sw[c]); }
+        if (lane == 0) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                grad_o[3 * (size_t)ray + c] = scale * (sx[c] / diag);
+                grad_d[3 * (size_t)ray + c] = scale * (stx[c] / diag + 0.5f * sw[c]);
+            }
+        }
+    }
+}
+
 // ============================================================================ occupancy grid kernels
 constexpr int GRID_THREADS = 256;
 static inline int stream_grid(size_t work_items) { return stride_grid((int64_t)((work_items + GRID_THREADS - 1) / GRID_THREADS), 8); }
@@ -599,6 +634,16 @@ int xrb_rm_calc_rgb_backward(const float *raw, const int32_t *numsteps_compacted
     composite_bwd_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(n_rays, (const float4 *)raw, coords, numsteps_compacted, grad_rgb, rgb, grid_mean, rgb_act, dens_act,
                                                                    (float4 *)dl_draw, CompositeGeom{});
     return check_launch("calc_rgb_backward");
+}
+
+int xrb_ngp_ray_grad(const float *d_rows, const float *coords, const int32_t *numsteps_compacted, const float *rays_o, const float *rays_d, int n_rays, float aabb0, float aabb1,
+                     float scale, float *grad_o, float *grad_d, void *stream) {
+    XRB_REQUIRE(n_rays >= 0, "ngp_ray_grad: negative size");
+    XRB_REQUIRE(aabb1 > aabb0, "ngp_ray_grad: need aabb0 < aabb1");
+    if (n_rays == 0) return XRB_OK;
+    XRB_REQUIRE(d_rows && coords && numsteps_compacted && rays_o && rays_d && grad_o && grad_d, "ngp_ray_grad: null pointer");
+    ray_grad_kernel<<<warp_grid(n_rays), 256, 0, (cudaStream_t)stream>>>(n_rays, d_rows, coords, numsteps_compacted, rays_o, rays_d, aabb0, aabb1 - aabb0, scale, grad_o, grad_d);
+    return check_launch("ngp_ray_grad");
 }
 
 int xrb_rm_calc_rgb_inference(const float *raw, const float *coords, const int32_t *numsteps, const float *bg3_host, int n_rays, int rgb_act, int dens_act, float *rgb_out,

@@ -15,11 +15,47 @@ import torch
 from . import _C
 
 
+POSE_LR = 3e-3           # default Adam learning rate of the pose corrections (NgpRaySource.pose_step), chosen with the convergence test of tests/test_gpu_pose_refine.py (DESIGN §4.10)
+
+
+def so3_exp(omega):
+    """Exp of the rotation vectors omega [..., 3] -> [..., 3, 3]: I + A [w]x + B [w]x^2 with A = sin(t) / t, B = (1 - cos(t)) / t^2 = 2 sin^2(t/2) / t^2 (no
+    cancellation), and their Taylor series through t^4 below t = 0.05 (truncation < 1e-11), so that the value and its autograd derivative are finite and accurate at 0"""
+    t2 = (omega * omega).sum(-1, keepdim=True)[..., None]
+    small = t2 < 0.0025
+    t = torch.sqrt(torch.where(small, torch.ones_like(t2), t2))
+    h = 0.5 * t
+    a = torch.where(small, 1.0 - t2 / 6.0 + t2 * t2 / 120.0, torch.sin(t) / t)
+    b = torch.where(small, 0.5 - t2 / 24.0 + t2 * t2 / 720.0, 0.5 * (torch.sin(h) / h) ** 2)
+    x, y, z = omega.unbind(-1)
+    zero = torch.zeros_like(x)
+    K = torch.stack([zero, -z, y, z, zero, -x, -y, x, zero], -1).reshape(omega.shape[:-1] + (3, 3))
+    eye = torch.eye(3, dtype=omega.dtype, device=omega.device)
+    return eye + a * K + b * (K @ K)
+
+
+def corrected_poses(poses43, xi):
+    """NGP xforms [I,4,3] (rows 0..2: the rotation's columns, row 3: the centre) corrected by xi = (omega, rho) [I,6]: R' = R Exp(omega), o' = o + rho
+    (include/xrnerf_b200.h, "NGP camera pose refinement"). Rows 0..2 of an xform are R^T, so they become Exp(omega)^T R^T."""
+    rot = so3_exp(xi[:, :3]).transpose(-1, -2) @ poses43[:, :3]
+    return torch.cat([rot, (poses43[:, 3] + xi[:, 3:])[:, None]], 1)
+
+
+def pose_xi_grad(poses43, xi, d_poses):
+    """dL/dxi [I,6] from dL/dP' [I,4,3] at the corrected poses corrected_poses(poses43, xi): autograd of the Exp map (float32)"""
+    with torch.enable_grad():
+        x = xi.detach().clone().requires_grad_(True)
+        (g,) = torch.autograd.grad(corrected_poses(poses43, x), x, d_poses)
+    return g
+
+
 class NgpRaySource:
-    def __init__(self, poses43, images_rgba, K, seed=0, depths=None, depth_scale=0.33):
+    def __init__(self, poses43, images_rgba, K, seed=0, depths=None, depth_scale=0.33, refine_poses=False):
         """poses43 [I,4,3] NGP xforms (poses_nerf2ngp, datasets/utils/hashnerf.py:4-23); images_rgba [I,H,W,4] float32; K 3x3 intrinsics.
         depths [I,H,W] (optional): z-depth images, the distance along each camera's optical axis in the dataset's units (0 or not finite: no depth); batches
-        then also hold target_depth [n,1], the ray parameter of the NGP ray (xrb_ngp_batch_depth) with depth_scale the scale of poses_nerf2ngp."""
+        then also hold target_depth [n,1], the ray parameter of the NGP ray (xrb_ngp_batch_depth) with depth_scale the scale of poses_nerf2ngp.
+        refine_poses: hold a correction xi [I,6] per image (include/xrnerf_b200.h, "NGP camera pose refinement"), initially 0, and generate every batch from
+        the corrected poses; batches then also hold row_idx [n] (int64) and pose_xi [I,6], the corrections they were drawn with, and pose_step() updates xi."""
         self.poses = torch.as_tensor(poses43, dtype=torch.float32).contiguous()
         self.images = torch.as_tensor(images_rgba, dtype=torch.float32).contiguous()
         self.I, self.H, self.W = self.images.shape[:3]
@@ -32,9 +68,15 @@ class NgpRaySource:
         self.perm = None
         self.cur_i = 0
         self.seed, self.calls = int(seed), 0
+        self.refine_poses = bool(refine_poses)
+        if self.refine_poses:
+            self.xi, self.xi_m, self.xi_v = (torch.zeros((self.I, 6), dtype=torch.float32) for _ in range(3))
+            self.pose_steps = 0
 
     def cuda(self, device=None):
         self.poses, self.images = self.poses.cuda(device), self.images.cuda(device)
+        if self.refine_poses:
+            self.xi, self.xi_m, self.xi_v = self.xi.cuda(device), self.xi_m.cuda(device), self.xi_v.cuda(device)
         if self.depths is not None:
             self.depths = self.depths.cuda(device)
         if self.perm is not None:
@@ -67,7 +109,12 @@ class NgpRaySource:
         out = dict(rays_o=f(3), rays_d=f(3), target_s=f(3), alpha=f(1), img_ids=f(1), bg_color=f(3))
         if u_bg is not None:
             u_bg = torch.as_tensor(u_bg, dtype=torch.float32).to(dev).contiguous()
-        _C.check(_C.lib.xrb_ngp_batch_sample(_C.f32(self.poses), _C.f32(self.images), self.I, self.H, self.W, self.fx, self.fy, self.cx, self.cy, _C.ptr(row_idx, torch.int64), n,
+        poses = self.poses
+        if self.refine_poses:
+            xi = self.xi.clone()
+            poses = corrected_poses(self.poses, xi).contiguous()
+            out.update(row_idx=row_idx, pose_xi=xi)
+        _C.check(_C.lib.xrb_ngp_batch_sample(_C.f32(poses), _C.f32(self.images), self.I, self.H, self.W, self.fx, self.fy, self.cx, self.cy, _C.ptr(row_idx, torch.int64), n,
                                              _C.ptr(u_bg), self.seed, self.calls, _C.ptr(out['rays_o']), _C.ptr(out['rays_d']), _C.ptr(out['target_s']), _C.ptr(out['alpha']),
                                              _C.ptr(out['img_ids']), _C.ptr(out['bg_color']), _C.stream()), 'ngp_batch_sample')
         self.calls += 1
@@ -77,6 +124,40 @@ class NgpRaySource:
             _C.check(_C.lib.xrb_ngp_batch_depth(_C.f32(self.depths), self.I, self.H, self.W, self.fx, self.fy, self.cx, self.cy, self.depth_scale, _C.ptr(row_idx, torch.int64), n,
                                                 _C.ptr(out['target_depth']), _C.stream()), 'ngp_batch_depth')
         return out
+
+    def refined_poses(self):
+        """the corrected NGP xforms [I,4,3] (the given poses without refine_poses), for rendering and export"""
+        if not self.refine_poses:
+            return self.poses.clone()
+        return corrected_poses(self.poses, self.xi)
+
+    def pose_step(self, batch, grad_o, grad_d, lr=POSE_LR, betas=(0.9, 0.999), eps=1e-8):
+        """One Adam step on the pose corrections from the gradient of a loss with respect to the rays of `batch` (a dict this source returned): grad_o /
+        grad_d [n,3], e.g. NgpTrainer(ray_grad=True)'s grad_rays_o / grad_rays_d after step(batch['rays_o'], batch['rays_d'], ...). xrb_ngp_pose_grad chains them
+        to the corrected poses, autograd of the Exp map to xi, then xrb_adam_ema_step updates xi. No host synchronisation.
+        The gradient is taken at the corrections the batch was drawn with (batch['pose_xi']): a batch generated before the previous pose_step (e.g. one
+        prefetched for NgpTrainer.step's next_rays) yields a gradient one step stale, which Adam tolerates at these step sizes."""
+        if not self.refine_poses:
+            raise _C.XrbError('XRB_E_BADARG: pose_step needs NgpRaySource(..., refine_poses=True)')
+        if 'pose_xi' not in batch or 'row_idx' not in batch:
+            raise _C.XrbError('XRB_E_BADARG: pose_step needs a batch drawn from this source with refine_poses=True (row_idx, pose_xi)')
+        row_idx, xi = batch['row_idx'], batch['pose_xi']
+        n = int(row_idx.numel())
+        for name, g in (('grad_o', grad_o), ('grad_d', grad_d)):
+            if not torch.is_tensor(g) or g.dtype != torch.float32 or tuple(g.shape) != (n, 3):
+                what = f'{g.dtype} {tuple(g.shape)}' if torch.is_tensor(g) else type(g).__name__
+                raise _C.XrbError(f'XRB_E_BADARG: {name} must be float32 [{n},3], got {what}')
+        _C.require_cuda(self.poses, row_idx, grad_o, grad_d)
+        poses = corrected_poses(self.poses, xi).contiguous()
+        grad_o, grad_d = grad_o.contiguous(), grad_d.contiguous()      # held by name until the launch: the kernel reads them
+        d_poses = torch.zeros((self.I, 4, 3), dtype=torch.float32, device=self.poses.device)
+        _C.check(_C.lib.xrb_ngp_pose_grad(_C.ptr(row_idx, torch.int64), n, _C.f32(poses), self.I, self.H, self.W, self.fx, self.fy, self.cx, self.cy, _C.f32(grad_o),
+                                          _C.f32(grad_d), _C.f32(d_poses), _C.stream()), 'ngp_pose_grad')
+        g = pose_xi_grad(self.poses, xi, d_poses).contiguous()
+        self.pose_steps += 1
+        _C.check(_C.lib.xrb_adam_ema_step(_C.f32(self.xi), None, _C.f32(g), _C.f32(self.xi_m), _C.f32(self.xi_v), self.xi.numel(), float(lr), float(betas[0]), float(betas[1]),
+                                          float(eps), 0.0, self.pose_steps, 1.0, None, 0.0, _C.stream()), 'pose adam')
+        return g
 
 
 def select_rays_indices(H, W, sel_n, iter_n=0, precrop_iters=0, precrop_frac=0.5, select_inds=None, generator=None, device='cpu'):

@@ -153,12 +153,22 @@ class NgpField(nn.Module):
             out = (torch.zeros_like(self.hash_params), torch.zeros_like(self.density_params), torch.zeros_like(self.color_params))
         return self.backward_rows(pts, dirs, grad_raw, out, impl=impl)
 
-    def backward_rows(self, pts, dirs, grad_raw, out, n_rows_dev=None, impl=None):
+    def backward_rows(self, pts, dirs, grad_raw, out, n_rows_dev=None, impl=None, d_rows=None):
         """backward_params into `out` from the working copies as they are, without refresh() (see mlp_rows). n_rows_dev as in mlp_rows; the CUDA-core
-        kernel (impl 0) takes its row count from the host, so with n_rows_dev it waits for the device once."""
+        kernel (impl 0) takes its row count from the host, so with n_rows_dev it waits for the device once.
+        d_rows (optional): a dense float32 [S,6] tensor that receives each effective row's (dL/dx, dL/dw), the gradient with respect to the warped
+        position and direction (xrb_ngp_mlp_backward_tc_inputs, include/xrnerf_b200.h "NGP camera pose refinement"); tensor-core backward only."""
         n = pts.shape[0]
         (pp, ps), (dp, ds) = _C.rows(pts), _C.rows(dirs)
         impl = (self.impl if self.tc_backward_ok() else 0) if impl is None else impl
+        if d_rows is not None:
+            if impl != 1:
+                raise _C.XrbError('XRB_E_BADARG: d_rows needs the tensor-core backward (impl 1)')
+            if d_rows.dim() != 2 or d_rows.shape[1] != 6 or d_rows.shape[0] < n:
+                raise _C.XrbError(f'XRB_E_BADARG: d_rows must be float32 [>= {n}, 6], got {tuple(d_rows.shape)}')
+            _C.check(_C.lib.xrb_ngp_mlp_backward_tc_inputs(self.cfg, self.tab, _C.ptr(self._image), pp, ps, dp, ds, _C.f32(grad_raw), n, _C.i32(n_rows_dev), _C.f32(out[0]),
+                                                           _C.f32(out[1]), _C.f32(out[2]), _C.f32(d_rows), _C.stream()), 'ngp_mlp_backward_tc_inputs')
+            return out
         if impl == 1:
             _C.check(_C.lib.xrb_ngp_mlp_backward_tc(self.cfg, self.tab, _C.ptr(self._image), pp, ps, dp, ds, _C.f32(grad_raw), n, _C.i32(n_rows_dev), _C.f32(out[0]), _C.f32(out[1]),
                                                     _C.f32(out[2]), _C.stream()), 'ngp_mlp_backward_tc')

@@ -204,7 +204,7 @@ class _Slot:
 class NgpTrainer:
     def __init__(self, field, bitfield, n_rays, target_batch_size=1 << 18, aabb=(0.0, 1.0), near=0.05, cone=1.0 / 256, rgb_act=2, dens_act=3,
                  lr=1e-2, betas=(0.9, 0.99), eps=1e-15, weight_decay=1e-6, samples_per_ray_budget=64, group=None, ema_momentum=None, ema_warm_up=100,
-                 grad_comm='auto', bwd_impl=None, depth_weight=0.0, opacity_weight=0.0):
+                 grad_comm='auto', bwd_impl=None, depth_weight=0.0, opacity_weight=0.0, ray_grad=False):
         import torch.distributed as dist
         self.f, self.bitfield, self.n_rays, self.T = field, bitfield, n_rays, int(target_batch_size)
         self.aabb, self.near, self.cone, self.rgb_act, self.dens_act = aabb, near, cone, rgb_act, dens_act
@@ -216,6 +216,13 @@ class NgpTrainer:
         self.grad_comm = grad_comm if self.world > 1 else 'none'
         self.bwd_impl = (1 if field.tc_backward_ok() else 0) if bwd_impl is None else bwd_impl
         self.fwd_impl = 1
+        self.ray_grad = bool(ray_grad)
+        if self.ray_grad:
+            if self.world > 1:
+                raise ValueError('ray_grad: only for a single process (world size 1)')
+            if self.bwd_impl != 1 or not field.tc_backward_ok():
+                raise ValueError(f'ray_grad: needs the tensor-core field backward, built for (density_hidden, color_hidden) = (1,1) or (1,2); this field is '
+                                 f'({field.cfg.density_hidden},{field.cfg.color_hidden}) with bwd_impl {self.bwd_impl}')
         self.params = [field.hash_params, field.density_params, field.color_params]
         if field.n_packed > 6:
             field.set_packed_levels(6)     # the cell image is rebuilt after every optimiser step: 35 us for 6 levels (27.6 MB) vs 88 us for 7
@@ -277,6 +284,13 @@ class NgpTrainer:
             raise ValueError(f'depth_weight {depth_weight} / opacity_weight {opacity_weight}: must be >= 0')
         if self.depth_weight > 0.0 or self.opacity_weight > 0.0:
             self.alpha, self.depth, self.grad_alpha, self.grad_depth = (torch.zeros(n_rays, dtype=torch.float32, device=dev) for _ in range(4))
+        # camera pose refinement (NgpRaySource.pose_step): step() also fills grad_rays_o / grad_rays_d [n_rays,3], the gradient of the loss it returns with
+        # respect to the rays it was given (sample t held fixed; include/xrnerf_b200.h "NGP camera pose refinement")
+        if self.ray_grad:
+            self.d_rows = torch.zeros((self.T, 6), dtype=torch.float32, device=dev)
+            self.grad_rays_o = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
+            self.grad_rays_d = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
+            self.inv_loss_scale = 1.0 / float(torch.tensor(128.0, dtype=torch.float32) / n_rays)   # the composite's fp32 128.f / n_rays, inverted
         self.grid_mean = torch.ones(1, dtype=torch.float32, device=dev)
         self.aux = torch.cuda.Stream(device=dev) if dev.type == 'cuda' else None
         self.trained_total = torch.zeros(1, dtype=torch.int64, device=dev)    # rays fully trained, summed over every batch prepared so far (device counter, no sync)
@@ -341,7 +355,11 @@ class NgpTrainer:
             _C.check(_C.lib.xrb_rm_calc_rgb_backward(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean),
                                                      self.n_rays, self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward')
         self.gflat.zero_()
-        f.backward_rows(pts, dirs, self.draw, self.grads, n_rows_dev, self.bwd_impl)
+        if self.ray_grad:
+            f.backward_rows(pts, dirs, self.draw, self.grads, n_rows_dev, self.bwd_impl, d_rows=self.d_rows)
+            self._ray_grad(s, st)
+        else:
+            f.backward_rows(pts, dirs, self.draw, self.grads, n_rows_dev, self.bwd_impl)
         s.free = torch.cuda.Event(); s.free.record(main)
         self.step_n += 1
         it = self.step_n - 1                                                            # runner.iter inside after_train_iter
@@ -367,6 +385,13 @@ class NgpTrainer:
         _C.check(_C.lib.xrb_rm_calc_rgb_backward_geom(_C.ptr(self.raw), _C.ptr(s.numsteps_c), _C.ptr(s.coords_c), _C.ptr(self.grad_rgb), _C.ptr(self.rgb), _C.ptr(self.grid_mean),
                                                       _C.ptr(rays_o), _C.ptr(rays_d), lo, hi, _C.ptr(self.depth), _C.ptr(self.alpha), _C.ptr(gd), _C.ptr(ga), self.n_rays,
                                                       self.rgb_act, self.dens_act, _C.ptr(self.draw), st), 'calc_rgb_backward_geom')
+
+    def _ray_grad(self, s, st):
+        """d_rows -> grad_rays_o / grad_rays_d. dL/draw carries the composite's loss_scale = 128 / n_rays (calc_rgb.cu:92-93); its inverse restores the
+        gradient of the loss step() returns (plus the composite's l1 / l2 regularisers, 0 unless rgb_act is exponential or the grid mean is below 0.01)"""
+        rays_o, rays_d = s.rays
+        _C.check(_C.lib.xrb_ngp_ray_grad(_C.ptr(self.d_rows), _C.ptr(s.coords_c), _C.ptr(s.numsteps_c), _C.ptr(rays_o), _C.ptr(rays_d), self.n_rays, float(self.aabb[0]),
+                                         float(self.aabb[1]), self.inv_loss_scale, _C.ptr(self.grad_rays_o), _C.ptr(self.grad_rays_d), st), 'ngp_ray_grad')
 
     def _adam(self, p, p16, g, m, v, e, mom, div, bf16=False):
         fn = _C.lib.xrb_adam_ema_step_bf16grad if bf16 else _C.lib.xrb_adam_ema_step
